@@ -1,6 +1,6 @@
 """Python-side mirror of the C ABI in include/lmot.h (ctypes; used by tests/, bench.py and __graft_entry__).
 
-The product is liblmot.so (CUDA kernels for sm_100a behind `extern "C"`).  This module only loads it and
+The product is liblmot.so (CUDA kernels for sm_90a behind `extern "C"`).  This module only loads it and
 marshals numpy arrays / raw device pointers; it contains NO implementation of any pipeline stage and there is
 no CPU fallback: if the library is missing or no CUDA device is usable, construction raises.
 
@@ -336,7 +336,7 @@ class Lmot:
     # ---- batched ticks: F sensor streams, one frame each, one shared track table (BASELINE.json configs[3]) --------
     def batch_prepare(self, dev_frames):
         """Marshal a tick's (device pointer, n) list ONCE: the returned handle can be passed to batch_dev / batch_detect_dev /
-        batch_ground_ccl_dev in place of the list (a timing loop must not spend 20 us per call building ctypes arrays)."""
+        batch_ground_ccl_dev in place of the list (a timing loop must not build ctypes arrays on every call)."""
         return ("prepared",) + tuple(self._batch_args(dev_frames, True))
 
     def _batch_args(self, frames, device: bool):

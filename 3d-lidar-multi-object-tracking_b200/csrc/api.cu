@@ -131,7 +131,7 @@ int submit_tracker(Ctx* c, Slot* s, Result* r, const float* d_boxes, const int* 
   if (gated) {
     // Nothing but kernels on the tracker stream (an event record between spawn_output_kernel and the next frame's gate
     // kernel would serialise the two launches): publish_kernel polls the device-side step count, and "the slot is free"
-    // is recorded behind it on the publish stream -- ~10 us later than strictly necessary, detection has >100 us of slack
+    // is recorded behind it on the publish stream -- a little later than strictly necessary, detection has the slack
     if ((rc = tracker_publish(c, r, c->pub_stream))) return rc;
     LMOT_CUDA(c, cudaEventRecord(r->ev_done, c->pub_stream));
     LMOT_CUDA(c, cudaEventRecord(s->ev_trk_done, c->pub_stream));
@@ -419,7 +419,7 @@ int lmot_default_params(lmot_params* p) {
   p->global_frame = 0;
   p->node_prefilter = 0; p->filter_z_min = -3.0f; p->filter_z_max = 1.0f;
   p->filter_x_min = -15.f; p->filter_x_max = 5.f; p->filter_y_min = -50.f; p->filter_y_max = 50.f;
-  p->pipeline_depth = 8;   // detection takes ~150 us per frame: 8 frames in flight keep it ahead of the ~40 us tracker chain
+  p->pipeline_depth = 8;   // detection takes 2-3x as long per frame as the tracker chain (H100: ~110 vs ~46 us): 8 frames in flight keep it ahead
   p->result_ring = 32;
   return LMOT_OK;
 }
@@ -436,7 +436,7 @@ const char* lmot_strerror(int s) {
   }
 }
 
-const char* lmot_build_info(void) { return "liblmot sm_100a, nvcc " __DATE__ " -fmad=false"; }
+const char* lmot_build_info(void) { return "liblmot sm_90a, nvcc " __DATE__ " -fmad=false"; }
 
 int lmot_get_params(const lmot_ctx* ctx, lmot_params* out) {
   if (!ctx || !out) return LMOT_ERR_INVALID;
@@ -468,6 +468,11 @@ int lmot_create(lmot_ctx** out, const lmot_params* params, int device) {
   Ctx* c = &h->c;
   c->prm = p;
   c->device = device;
+  // grid-stride kernels are sized to the device: box fitting 2 CTAs per SM, the two wide tracker kernels 4 per SM
+  int sms = 0;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0) { delete h; return LMOT_ERR_CUDA; }
+  c->fit_ctas = 2 * sms;
+  c->trk_ctas = 4 * sms;
   c->max_points = p.max_points;
   c->n_slots = p.pipeline_depth;
   c->n_results = p.result_ring;
@@ -764,15 +769,14 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, false);
   if (!r) return LMOT_ERR_STATE;
-  // (Measured: end-to-end frames/s is bound by these copies -- one 1.9 MB copy per frame sustains ~39 GB/s, 49 us per frame,
-  // against 41 us for the tracker chain.  A copy stream of its own changed nothing, two alternating ones made cudaMemcpyAsync
+  // (End-to-end frames/s is bound by these copies -- one 1.9 MB copy per frame -- not by the tracker chain.  A copy stream of its
+  // own changed nothing, two alternating ones made cudaMemcpyAsync
   // block the host.)
   // ZERO COPY (opt-in, LMOT_ZERO_COPY=1): a frame in page-locked host memory (lmot_pinned_alloc, cudaHostAlloc, cudaHostRegister) is
   // not copied; under unified addressing the ground kernel's bulk copies read it over PCIe straight into shared memory, so every
   // input byte crosses the link once and never touches HBM (possible whenever the launch keeps each CTA's chunk resident,
-  // ground_reads_input_once).  Bit-identical results (tests/test_pipeline_gpu.py) -- but MEASURED SLOWER than the copy engine on
-  // B200: SM-issued reads reach ~26 GB/s of the link (74 us per 1.9 MB frame, 13.4 k frames/s end to end) where cudaMemcpyAsync
-  // sustains ~39 GB/s at this copy size (49 us, 20.4 k frames/s).  Hence off by default.  The buffer must stay untouched until
+  // ground_reads_input_once).  Bit-identical results (tests/test_pipeline_gpu.py) -- but SM-issued reads over the link were
+  // slower than the copy engine at this copy size.  Hence off by default.  The buffer must stay untouched until
   // the frame has been collected (the same contract as the asynchronous copy).
   if (c->zero_copy && stride == 4 && n > 0 && n <= c->max_points && (reinterpret_cast<uintptr_t>(points) & 15u) == 0 && ground_reads_input_once(c, n)) {
     cudaPointerAttributes pa;

@@ -1,4 +1,4 @@
-// boxfit.cu -- per-cluster L-shape / minimum-area-rectangle box fitting on sm_100a.
+// boxfit.cu -- per-cluster L-shape / minimum-area-rectangle box fitting on sm_90a.
 //
 // Replaces boxFitting (/root/reference/object_tracking/src/cluster/box_fitting.cpp:422-431):
 //   getClusteredPoints (:46-72)   gather the elevated points of every cluster IN CLOUD ORDER
@@ -29,8 +29,8 @@ namespace lmot {
 namespace {
 
 constexpr int kTile = 1024;
-constexpr int kFitThreadsFrame = 512;   // one CTA per cluster: the largest cluster IS the kernel of a single frame (16 us of point pass at 256 threads)
-constexpr int kFitThreadsBatch = 256;   // batched ticks hold ~8x the clusters: more, smaller CTAs per SM finish the union sooner (51 us at 512, 45 at 256)
+constexpr int kFitThreadsFrame = 512;   // one CTA per cluster: the largest cluster IS the kernel of a single frame
+constexpr int kFitThreadsBatch = 256;   // batched ticks hold ~8x the clusters: more, smaller CTAs per SM finish the union sooner
 constexpr int kCols = 1800;        // pixel columns a cluster can span: offsetX-450 = picX-initPicX in [-899,899]
 constexpr int kColShift = 899 - 450;
 constexpr int kHullCap = 2048;
@@ -39,7 +39,7 @@ constexpr int kHullCap = 2048;
 // CTAs become resident once EVERY CTA of the kernel before it has started (they all trigger at their first instruction) and wait there
 // for it to finish -- its launch latency leaves the frame's critical path.  Deadlock-free next to the ground kernel's own barrier: a
 // waiting CTA only ever waits for a grid that is completely resident and waits for nobody.  (Not used in front of tile_hist: its CTAs
-// would hold SM slots for the ~12 us of the ground kernel, slots the tracker chain needs.)
+// would hold SM slots for the duration of the ground kernel, slots the tracker chain needs.)
 __device__ __forceinline__ void fit_pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void fit_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
@@ -212,7 +212,7 @@ scatter_kernel(const __grid_constant__ FitBatch B, int max_clusters) {
   const int rank = __popc(grp & ((1u << lane) - 1u));
   // Ranks follow the cloud order: the warps' groups must take their segment ranges in warp order.  Every warp lists its groups
   // (cluster id, size); warp 0 then walks the 32 lists in order, one group per lane -- a warp's groups have distinct ids, so only
-  // consecutive lists depend on each other.  (The warps taking turns behind 32 CTA barriers was ~5 of this kernel's ~8 us.)
+  // consecutive lists depend on each other.  (The warps taking turns behind 32 CTA barriers was most of this kernel's time.)
   __shared__ unsigned short s_gcid[kTile / 32][32];
   __shared__ unsigned char s_gcnt[kTile / 32][32], s_gn[kTile / 32];
   __shared__ int s_gbase[kTile / 32][32];
@@ -361,7 +361,7 @@ box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxPa
     float maxZ = -99.f;
     double sx = 0, sy = 0, sz = 0;
     float mnx = FLT_MAX, mny = FLT_MAX, mnz = FLT_MAX, mxx = -FLT_MAX, mxy = -FLT_MAX, mxz = -FLT_MAX;
-    // four points per thread in flight: as a plain loop this was one L2 round trip per iteration (18 us for a 5000-point cluster)
+    // four points per thread in flight: as a plain loop this was one L2 round trip per iteration
     for (int j0 = tid; j0 < n; j0 += 4 * kFitThreads) {
       float4 qq[4];
 #pragma unroll
@@ -544,7 +544,7 @@ box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxPa
       __syncthreads();
       // hull sequence = lower-chain vertices left to right, then upper-chain vertices right to left: positions from two block-wide
       // counts (thread t owns the compacted columns [8t, 8t+8)); as a loop on thread 0 this was 2 W dependent shared-memory
-      // round trips -- 12 us for a 400-column cluster, the longest phase of the slowest CTA
+      // round trips, the longest phase of the slowest CTA
       if (W == 1) {
         if (tid == 0) {
           int m = 1;
@@ -738,7 +738,7 @@ concat_boxes_kernel(const __grid_constant__ FitBatch B, int n_frames, int max_bo
   __shared__ int s_off[kMaxBatch + 1];
   __shared__ int s_fc[kMaxBatch][5];
   // thread f fetches frame f's five counters (independent loads: one L2 round trip for the whole tick; a single thread walking the
-  // frames was 40 dependent round trips, 20 us)
+  // frames was 40 dependent round trips)
   if (threadIdx.x < n_frames) {
     const int f = threadIdx.x;
     int* fc = B.f[f].counters;
@@ -766,7 +766,7 @@ concat_boxes_kernel(const __grid_constant__ FitBatch B, int n_frames, int max_bo
   __syncthreads();
   {
     // warp w copies frame w's list (96-byte boxes: six 16-byte words each, source and destination 16-byte aligned), four words per
-    // lane in flight.  (One flat loop over all floats with a per-element frame search was 40 dependent L2 round trips: 18 us.)
+    // lane in flight.  (One flat loop over all floats with a per-element frame search was 40 dependent L2 round trips.)
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (w < n_frames) {
       const int off = s_off[w], cnt = min(s_off[w + 1], max_boxes) - off;

@@ -89,7 +89,7 @@ __device__ __forceinline__ void ccl_mark(unsigned long long* clk, int row, int s
 // ---------------------------------------------------------------------------------------------------------------
 // Node ids are DENSE.  (Round 1 / the first version of round 2 numbered a piece word * 16 + k: the 32 lanes of a warp then hit the
 // same shared-memory bank on every parent access, each thread walked its own ragged list of pieces, and every flatten / union was a
-// data-dependent loop of dependent loads: 18-26 us per frame.)  A block-wide scan of the pieces per word gives every piece its
+// data-dependent loop of dependent loads.)  A block-wide scan of the pieces per word gives every piece its
 // raster-order rank as id (still monotone: the smallest id of a component is its first piece in raster order), so that
 //   * flattening is pointer jumping with thread t on ids t, t + 1024, ...: conflict-free, ~log2(depth) steps per node;
 //   * the adjacencies step C cannot express as a parent link go to a pair list and are united one pair per thread.
@@ -99,7 +99,7 @@ constexpr int kDenseSmem = kNodes * 4 + 3 * kBitWords * 4 + (kBitWords + 8) * 4 
 // flatten: every node re-points itself at its grandparent until its parent is a root (uf_compress), thread t on ids t, t + 1024,
 // ...; only the owner stores to L[id], every store moves id to an ancestor, roots do not change while this runs -- so the walks
 // need no barrier between them and shorten each other: ~log2(depth) steps per node.  (Barrier-synchronised rounds with
-// __syncthreads_or were measured at 0.64 us PER ROUND, 4.5 us for the 7 rounds of a depth-54 forest.)
+// __syncthreads_or pay a CTA barrier PER ROUND.)
 __device__ __forceinline__ void ccl_flatten(volatile int* L, int P) {
   for (int id = threadIdx.x; id < P; id += kCclThreads) uf_compress(L, id);
   __syncthreads();

@@ -1,4 +1,4 @@
-// cluster.cu -- 2-D occupancy-grid connected-component clustering on sm_100a.
+// cluster.cu -- 2-D occupancy-grid connected-component clustering on sm_90a.
 //
 // Replaces componentClustering (/root/reference/object_tracking/src/cluster/component_clustering.cpp:260-268):
 //   mapCartesianGrid (:28-225)  count points per 0.2 m cell of the 250x250 grid over +-25 m; every cell holding
@@ -6,7 +6,7 @@
 //   findComponent/search (:228-257)  raster scan (x outer, y inner); each unlabelled occupied cell starts
 //                               id = ++numCluster and a recursive 8-connected flood fill
 //
-// B200 design: the grid is 250 rows of 250 BITS (8 words per row, 8 KB in all), not 62,500 counters.
+// Design: the grid is 250 rows of 250 BITS (8 words per row, 8 KB in all), not 62,500 counters.
 //   * "count > 1" needs no counter: two bit planes, `once` and `twice`.  A point sets its cell's bit in `once`; if it
 //     was set already (or two points of one warp share the cell) it sets the bit in `twice`.  seed == twice.
 //     (cart_mark(), called by ground_fused_kernel for every elevated point while it is still in registers, or by

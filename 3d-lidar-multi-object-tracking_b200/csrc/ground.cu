@@ -1,4 +1,4 @@
-// ground.cu -- slope-based polar-grid ground removal on sm_100a.
+// ground.cu -- slope-based polar-grid ground removal on sm_90a.
 //
 // Replaces groundRemove (/root/reference/object_tracking/src/groundremove/ground_removal.cpp:177-249) and
 // gaussSmoothen (src/groundremove/gaus_blur.cpp:52-68) with ONE cooperative kernel per frame, ground_fused_kernel:
@@ -35,7 +35,7 @@ namespace {
 std::mutex g_ground_mutex;                 // one ground kernel in flight per device (see ground_launch_batch)
 // the chain of ground kernels of a device: every launch waits for the previous one.  On the same stream that is stream order; on
 // another stream it is `done`, recorded right behind the launch -- or, for the stand-alone entry points (`chain`), only when a
-// launch on another stream needs it: kernel / event record / kernel costs ~2 us more per launch than kernel / kernel.
+// launch on another stream needs it: kernel / event record / kernel costs a launch latency more per launch than kernel / kernel.
 struct GroundChain {
   cudaEvent_t done = nullptr;
   cudaStream_t last = nullptr;
@@ -310,17 +310,17 @@ __device__ __forceinline__ void grid_barrier(unsigned* bar, unsigned target, uns
 
 constexpr int kTilePts = kFusedThreads;             // 1024 points = 16 KB per TMA tile
 
-constexpr int kMaxResTiles = 7;                     // tiles of a CTA's chunk that stay in shared memory (112 KB)
+constexpr int kMaxResTiles = 8;                     // tiles of a CTA's chunk that stay in shared memory (128 KB): 132 CTAs hold 1.08 M points
 constexpr int kDescStride = 16;                     // u64 words between two CTAs' count descriptors (128 bytes)
-constexpr int kLookBatch = 5;                       // 5 x 32 >= 148 CTAs: all predecessors in one batch of loads
+constexpr int kLookBatch = 5;                       // 5 x 32 >= 132 CTAs: all predecessors in one batch of loads
 constexpr int kMaxTiles = 16;                       // tiles per chunk (labels of a thread's points: 2 bits each in one register)
 constexpr int kPendCap = 2048;                      // points of a chunk whose cell needs the exact evaluation, queued for a compact pass
 constexpr unsigned kPending = 0xFFFDu;              // cell id of a queued point until that pass has run
 constexpr int kKeysPerThread = (kPolarCells + kFusedThreads - 1) / kFusedThreads;   // 10: cells of the CTA's key grid per thread
 // dynamic shared memory layout (bytes): fixed part (incl. the CTA's private min-z key grid), then the resident tiles, then the cell
 // ids of every tile of the chunk.
-constexpr int kOffBar = 0;                                                  // [7] mbarriers of the tiles + [1] of the label limits
-constexpr int kOffMeta = 64;                                                // [3] pending points
+constexpr int kOffBar = 0;                                                  // [kMaxResTiles] mbarriers of the tiles + [1] of the label limits
+constexpr int kOffMeta = 80;                                                // [3] pending points
 constexpr int kOffCnt = 128;                                                // [16][32] u32 elevated | ground << 16 per warp
 constexpr int kOffWex = kOffCnt + kMaxTiles * 32 * 4;                       // [16][32] u32 exclusive inside the tile
 constexpr int kOffTtot = kOffWex + kMaxTiles * 32 * 4;                      // [16] u32 tile totals
@@ -333,6 +333,7 @@ constexpr int kOffPts = (kOffKeys + kPolarCells * 4 + 127) & ~127;          // [
 __host__ __device__ constexpr int fused_smem_bytes(int res_tiles, int tiles) { return kOffPts + res_tiles * kTilePts * 16 + tiles * kTilePts * 2; }
 constexpr int kFusedSmem = fused_smem_bytes(kMaxResTiles, kMaxTiles);
 static_assert(kFusedSmem <= 227 * 1024, "ground_fused_kernel: shared memory budget");
+static_assert(kOffBar + (kMaxResTiles + 1) * 8 <= kOffMeta && kOffMeta + 3 * 4 <= kOffCnt, "ground_fused_kernel: fixed layout");
 static_assert(kDenseSmem <= kFusedSmem, "the fused CCL reuses the ground kernel's shared memory");
 
 struct FusedOut {
@@ -481,9 +482,9 @@ __device__ __forceinline__ void bin_pair(int t0, int T, int cnt, int res_tiles, 
 }
 
 // ONE launch per frame -- or per batch of frames (one per sensor stream), CTA groups own frames and synchronise among themselves.
-// (Round 2 also tried "no second barrier": every CTA evaluating the polar grid for the channels its own points fall into, in shared
-// memory.  With ring-major clouds a chunk spans most of the 80 channels, so 148 CTAs each redid ~90 % of the grid: 7 M of the
-// kernel's 17 M warp instructions at 1 M points, 9 us -- profiles/README.md.  The grid is evaluated ONCE, spread over the CTAs.)
+// ("No second barrier" was tried: every CTA evaluating the polar grid for the channels its own points fall into, in shared
+// memory.  With ring-major clouds a chunk spans most of the 80 channels, so every CTA redid most of the grid and the kernel
+// issued far more instructions.  The grid is evaluated ONCE, spread over the CTAs.)
 __global__ void __launch_bounds__(kFusedThreads, 1)
 ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant__ GroundParams p, float roi,
                     unsigned long long* __restrict__ phase_clock) {
@@ -592,8 +593,8 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
   // ---- phase 3: labels (ground_removal.cpp:221-247), per-warp counts
   unsigned labs = 0;                                // 2 bits per tile: 0 dropped, 1 ground, 2 elevated
   // Long chunks: the 38 KB of label limits come into shared memory with ONE bulk copy (over the key grid, which was flushed before
-  // barrier 1) -- a gather of scattered cells from L2 moves a 32-byte sector per point, 6,800 points per CTA of a 1 M point frame
-  // made that 2.3 us.  Short chunks (an HDL-64 frame over 74-148 CTAs) touch fewer sectors than the grid has: they gather.
+  // barrier 1) -- a gather of scattered cells from L2 moves a 32-byte sector per point.  Short chunks (an HDL-64 frame over half
+  // or all of the SMs) touch fewer sectors than the grid has: they gather.
   const bool stage_lim = chunk > 2 * kTilePts;      // (frame-uniform)
   if (stage_lim) {
     if (tid == 0) {
@@ -670,8 +671,8 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { te += __shfl_xor_sync(0xFFFFFFFFu, te, o); tg += __shfl_xor_sync(0xFFFFFFFFu, tg, o); }
     // one word per CTA: launch tag (32) | elevated (16) | ground (16); a chunk holds at most 16384 points.  The words sit
-    // kDescStride apart (one 128-byte line each): with all of them in ten adjacent lines, 148 CTAs polling the same
-    // L2 slices serialised the whole exchange (measured: 4-6 us instead of one L2 round trip)
+    // kDescStride apart (one 128-byte line each): with all of them in a few adjacent lines, every CTA polling the same
+    // L2 slices serialised the whole exchange
     const unsigned epoch = F.epoch;
     volatile unsigned long long* d = F.desc;
     if (lane == 0) d[cta * kDescStride] = ((unsigned long long)epoch << 32) | ((unsigned long long)te << 16) | tg;
@@ -861,9 +862,9 @@ int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* 
   if (G < kMinCtas) G = kMinCtas;
   int cap = c->fused_max_ctas / F;
   // Inside the frame pipeline the kernel keeps to HALF of the SMs (as long as its chunks still fit in shared memory): a
-  // 1024-thread CTA holds 47 K of an SM's 64 K registers, and with the box-fitting CTAs of another frame next to it the SM has no
-  // room for a CTA of the tracker chain -- measured: the last imm_predict_gate CTA started 10-15 us after the first one, the
-  // sequential chain (the bound of frames/s) was 84 us per frame instead of 55.  Detection has >100 us of slack per frame.
+  // 1024-thread CTA holds 48 K of an SM's 64 K registers, and with the box-fitting CTAs of another frame next to it the SM has no
+  // room for a CTA of the tracker chain -- the last imm_predict_gate CTA then starts well after the first one and stretches the
+  // sequential chain (the bound of frames/s).  Detection has slack per frame.
   if (F == 1 && fuse_count && c->ground_half_sms) {
     const int half = cap / 2 > kMinCtas ? cap / 2 : kMinCtas;
     if ((long long)half * kMaxResTiles * kTilePts >= (long long)n_max) cap = half;

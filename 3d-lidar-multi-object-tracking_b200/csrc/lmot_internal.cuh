@@ -178,7 +178,7 @@ struct Ctx {
   GroundParams gp;
 
   // ---- capacities
-  int max_points = 0, max_sort_tiles = 0, fit_ctas = 296, n_mt_raw = 0;
+  int max_points = 0, max_sort_tiles = 0, fit_ctas = 0, n_mt_raw = 0;   // fit_ctas / trk_ctas: from the SM count (lmot_create)
   bool coop_launch = false;            // LMOT_COOP=1: cudaLaunchCooperativeKernel for the ground kernel (A/B diagnostics)
   int fused_max_ctas = 0;              // co-residency limit of the cooperative ground kernel on this device
   unsigned long long* d_trk_trace = nullptr;     // diagnostic: [kTraceRows][8] per-frame kernel spans of the tracker chain + 32 phase stamps (same switch)
@@ -224,7 +224,7 @@ struct Ctx {
   void* d_summary = nullptr;           // [max_tracks] ActSummary (tracker.cu): what TC needs of each active track, written by TB
   Result* last_trk_res = nullptr;      // result block of the previous tracker step (its device copy seeds the next one)
   bool act_valid = false;              // false after the table was written from the host: rebuilt before the next step
-  int trk_ctas = 592, gate_words = 0;
+  int trk_ctas = 0, gate_words = 0;
   int last_n_act = 0;          // active tracks (live or visible) in the last result the host has read: picks spawn_output_kernel's variant
   bool tc_wide = false;
   int tc_force = -1;           // LMOT_TC_WIDE: -1 by count, 0 / 1 pinned

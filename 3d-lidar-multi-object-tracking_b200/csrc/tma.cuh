@@ -1,6 +1,5 @@
-// tma.cuh -- minimal inline-PTX wrappers for the Blackwell bulk async copy engine (TMA, non-tensor form) and the
-// shared-memory mbarrier it signals.  `cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes` shows up in
-// SASS as UBLKCP, `mbarrier.arrive.expect_tx` as SYNCS.ARRIVE.TRANS64 (B300_MICROARCH.md, "cp.async/LDGSTS").
+// tma.cuh -- minimal inline-PTX wrappers for the Hopper bulk async copy engine (TMA, non-tensor form, sm_90) and the
+// shared-memory mbarrier it signals.
 #pragma once
 #include <cstdint>
 

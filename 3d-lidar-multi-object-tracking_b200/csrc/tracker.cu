@@ -1,4 +1,4 @@
-// tracker.cu -- batched IMM-UKF-PDA tracker on sm_100a.
+// tracker.cu -- batched IMM-UKF-PDA tracker on sm_90a.
 //
 // Replaces immUkfJpdaf (/root/reference/object_tracking/tracking/imm_ukf_jpda.cpp:704-1112) and class UKF
 // (tracking/ukf.cpp).  The reference walks its tracks sequentially; the only cross-track couplings are
@@ -167,7 +167,7 @@ __device__ void ukf_initialize(TrackState& t, double zx, double zy) {   // UKF::
 // ------------------------------------------------------------------------------------------------ gate
 // The tracker of frame f+1 needs (a) the tracker of frame f (same stream) and (b) the detection stages of frame f+1 (another
 // stream).  (b) as a stream-level event wait in front of TA costs a full launch latency on the sequential chain AFTER the
-// previous spawn_output_kernel has drained (measured 6.5-9.4 us of 44 per frame), because an event wait cannot sit between two
+// previous spawn_output_kernel has drained, because an event wait cannot sit between two
 // programmatically dependent launches.  Instead: box_fit_kernel's last CTA posts a per-slot semaphore, and this one-warp
 // kernel -- launched as a programmatic dependent of the previous frame's spawn_output_kernel, so it is resident early --
 // polls it, THEN lets TA's CTAs come (they hold SM resources, so they must not be resident while anything they wait for is
@@ -188,7 +188,7 @@ tracker_gate_kernel(const int* __restrict__ det_sem, unsigned long long* __restr
   pdl_launch_dependents();
   // (no griddepcontrol.wait: this kernel may finish before the previous frame's spawn_output_kernel does.  TA's CTAs, resident from
   // here on, wait for that step through its completion counter -- one L2 poll after spawn_output_kernel's last store instead of two
-  // grid-completion hops (TC -> this kernel -> TA), which were most of the 5.2 us between TC's end and the next TA's start.)
+  // grid-completion hops (TC -> this kernel -> TA).)
   if (phase && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); phase[27] = t; }
 }
 
@@ -1081,7 +1081,7 @@ __device__ __forceinline__ int emit_track(TrackState& t, int i, double ego_yaw, 
 
 // dst[0..n) = src[0..n) by the whole CTA, U loads in flight per thread before the first store.  (A plain
 // `for (...) dst[e] = src[e]` over pointers the compiler cannot prove distinct is a chain of load -> store -> load round
-// trips; on the one CTA of the tracker's sequential chain every one of them is ~1 us.)
+// trips; on the one CTA of the tracker's sequential chain every one of them is on the critical path.)
 template <int NT, typename T, int U>
 __device__ __forceinline__ void cta_copy(T* dst, const T* src, int n) {
   for (int base = 0; base < n; base += NT * U) {
@@ -1181,7 +1181,7 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
   const bool cp = prev.targets != o.targets;
   // everything else this kernel reads that does not depend on the summaries: the frame's box list (it travels with the
   // results), the previous result block (dead tracks: unchanged), the packed yaw of every track, the spawn inputs.  ALL loads
-  // are issued before the first store -- each load -> store pair behind another one was one more L2 round trip (~0.45 us)
+  // are issued before the first store -- each load -> store pair behind another one was one more L2 round trip
   constexpr int UB = 4, UT = 4, UM = 2, UY = 4;
   const int nbx = M * 6, ntg = cp ? (T0 * 12 + 15) / 16 : 0, ntm = cp ? (T0 * 4 + 15) / 16 : 0, nsv = cp ? (T0 + 15) / 16 : 0;
   uint4 vbx[UB], vtg[UT], vtm[UM], vst[1], vvi[1];
@@ -1271,7 +1271,7 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
   // ---- mergeOverSegmentation, pass A: imax = largest visible box index containing this (live) track
   // (track x box) pairs spread over the whole CTA: a warp takes every 8th box (broadcast loads); its lanes hold the tracks
   // jt = lane, lane + 32, ... in REGISTERS for the whole loop, so an iteration is two independent shared-memory loads and
-  // compares (the previous form, one dependent load chain per pair, took 2.9 us for ~90 boxes x ~100 tracks)
+  // compares (the previous form was one dependent load chain per pair)
   {
     const int warp = tid >> 5;
     constexpr int kPerLane = NT / 32;

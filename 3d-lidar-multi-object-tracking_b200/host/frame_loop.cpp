@@ -4,8 +4,8 @@
 // PointCloud2 message (src/groundremove/main.cpp:91-136, src/cluster/main.cpp:63-234, tracking/main.cpp:65-390).  This is
 // the same loop over lmot_frame_submit / lmot_frame_collect with HOST buffers: every frame is copied host -> device from
 // pinned memory inside lmot_frame_submit, and every frame's boxes and track outputs are read back by lmot_frame_collect.
-// bench.py times its `e2e` figure with this binary (a Python loop around the same two calls adds ~15 us of interpreter and
-// ctypes time per frame, which is more than a third of the frame time).
+// bench.py times its `e2e` figure with this binary (a Python loop around the same two calls adds interpreter and ctypes time
+// to every frame).
 //
 // usage: frame_loop <frames.bin> <n_frames> <n_points> <warmup> <steps> [dt_us=100000] [windows=1] [in_flight=0]
 //   frames.bin: n_frames x n_points x 4 float32 (XYZI).  n_frames >= warmup + windows * steps.

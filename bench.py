@@ -1,14 +1,14 @@
 #!/usr/bin/env python
 """bench.py -- HDL-64 frames/s of the LiDAR->tracks hot path (ground_removal -> component_clustering -> box_fitting ->
-imm_ukf_jpda) on B200, next to the reference's own CPU implementation timed on the same host.
+imm_ukf_jpda) on H100, next to the reference's own CPU implementation timed on the same host.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]           # our CUDA path
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # our CUDA path
     python bench.py --impl reference [--steps K] [--warmup W]     # the reference's sources (oracle/_ref) on the host CPU
     torchrun ... bench.py --gpus N ...                            # one rank per GPU, independent sensor streams (weak scaling)
 
 One "step" = one 120,000-point synthetic HDL-64 frame (64 rings x 1875 azimuths, ~64 live tracks) through all four
 stages, tracker state carried from frame to frame.  Frames are consecutive frames of ONE moving scene; every step reads
-a different frame (the ring of W+K frames is larger than the 126 MB L2, so inputs never sit in L2 from the previous step).
+a different frame (the ring of W+K frames is larger than the 50 MB L2, so inputs never sit in L2 from the previous step).
 
 Printed JSON (rank 0, one line):
   value     whole-job frames/s with the frames already resident in HBM (CUDA events around K steps, max over ranks)
@@ -16,15 +16,19 @@ Printed JSON (rank 0, one line):
             every step copies its frame H2D, runs the four stages and reads boxes + track outputs back; timed by the C++ loop
             host/frame_loop.cpp (the reference's host language), the same loop from Python/ctypes is reported next to it
   roofline  ground_fused_kernel (the whole ground-removal stage in one cooperative launch, the only stage that streams
-            the whole frame): algorithmic bytes per frame / its CUDA-event duration, vs the measured HBM peak
+            the whole frame): algorithmic bytes per frame / its CUDA-event duration, vs the HBM peak
   cpu_baseline  the reference's own four entry points on a bounded sample of the same frames, one host thread
   parity_check  the CUDA path against the reference ON THE BENCH SCENE, frame by frame over the cpu_baseline sample: counts, boxes
             (bit-exact), trackManage (identical), UKF states of well-conditioned tracks (<= 1e-4); a failing check withholds `value`
-  windows   the K-step timed region is repeated `windows` times on consecutive frames (barrier + synchronize on both sides of
-            each); `value`, `ms_per_step` and `e2e` are the MEDIAN window, `window_values` lists all of them
+  windows   the K timed steps are split into `windows` equal windows of consecutive frames (barrier + synchronize on both sides
+            of each); `value`, `ms_per_step` and `e2e` are the MEDIAN window, `window_values` lists all of them
   latency_us    p50 / p99 per stage and per frame, one frame in flight (CUDA events) and at the pipeline's depth (host clock)
   batched_8x120k  BASELINE.json configs[3]: 8 sensor streams, one frame each per tick, one shared track table: ticks through
             lmot_batch_dev, and the ground_removal + CCL roofline of the two batched launches
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned to its caller (boxes, track outputs of the
+last frame with the states of its live tracks, and its counts) as DIR/<name>.npy in float32 / float64.  The frames are seeded: the
+same arguments give the same inputs.
 """
 from __future__ import annotations
 
@@ -50,12 +54,6 @@ SCENE = dict(n_objects=150, lattice_pitch=3.8, ped_fraction=0.65, seed=1)   # ~6
 KERNEL_NAMES = ("ground_fused+ccl", "tile_hist+seg_offsets", "scatter", "box_fit",
                 "imm_predict_gate", "imm_update", "spawn_output")        # clustering runs in the ground kernel's last CTA (LMOT_FUSE_CCL=0: own launch)
 KERNEL_NAMES_UNFUSED = ("ground_fused", "ccl_cluster") + KERNEL_NAMES[1:]
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE ground_fused_kernel launch at the bench workload (pipeline geometry, 74 CTAs,
-# clustering fused into its tail), from the committed `ncu --set full` capture profiles/r2g_ncu_full_ground_pipeline.csv (2.07 MB read:
-# the frame once, plus the polar grid and the bit planes; 0 bytes written: the 3.9 MB of output clouds stay in the 126 MB L2 within
-# the measured launch)
-TRAFFIC_NCU = 2.07e6
-TRAFFIC_SOURCE = "constant from the committed ncu --set full capture profiles/r2g_ncu_full_ground_pipeline.csv (dram__bytes_read.sum + dram__bytes_write.sum of one launch), not measured by this run"
 KERNELS_PER_FRAME = len(KERNEL_NAMES) + 2   # ground + clustering 1 (one launch) + box 3 + tracker 3, + the tracker's gate kernel + publish_kernel
 
 
@@ -69,7 +67,7 @@ def make_frames(synth, n_frames, seed_offset=0):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons / power limit during the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -78,7 +76,7 @@ class ClockSampler:
 
     def start(self):
         q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--id={self.index}", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-lms", "100"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -93,26 +91,26 @@ class ClockSampler:
 
     def stop(self):
         if not self.proc:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
         try:
             self.proc.wait(timeout=5)
         except Exception:
             pass
-        sm, mx, reasons = [], [], set()
+        sm, mx, pl, reasons = [], [], [], set()
         for ln in self.lines:
             f = [x.strip() for x in ln.split(",")]
-            if len(f) < 7:
+            if len(f) < 8:
                 continue
             try:
-                sm.append(float(f[0])); mx.append(float(f[1]))
+                sm.append(float(f[0])); mx.append(float(f[1])); pl.append(float(f[7]))
             except ValueError:
                 continue
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[3:7]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": float(max(mx)) if mx else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "power_limit_w": float(min(pl)) if pl else None, "reasons": sorted(reasons), "samples": len(sm)}
 
 
 def measured_peak_gbs():
@@ -122,7 +120,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s at up to 700 W)"
 
 
 def host_cpu_name():
@@ -335,7 +333,7 @@ def run_native_e2e(frames, W, K, n_pts, rank, local_rank, world, windows=1, in_f
     path = None
     try:
         where = None
-        for cand in ("/dev/shm", tempfile.gettempdir(), ROOT):      # first place with room for the frames file (read once, into pinned memory)
+        for cand in ("/dev/shm", tempfile.gettempdir()):      # first place with room for the frames file (read once, into pinned memory); never the tree
             try:
                 st_ = os.statvfs(cand)
                 if os.access(cand, os.W_OK) and st_.f_bavail * st_.f_frsize > 1.2 * frames.nbytes * (world if cand == "/dev/shm" else 1):
@@ -438,6 +436,23 @@ def cpu_baseline_and_parity(ctx, oracle_mod, frames, ts, n_sample, W, K, d_frame
     return cpu, chk
 
 
+def dump_outputs(out_dir, res):
+    """What the last timed step returned to its caller (lmot_frame_fetch of the last frame), as float32 / float64 .npy files.
+    The states (targets, vandyaw) are those of the live tracks, rows `live_index` of the table: the table also carries dead tracks,
+    whose state the reference leaves as it was when they died -- NaN for a filter that diverged -- and which its tracking node skips
+    (trackManage == 0, tracking/main.cpp:204,299)."""
+    os.makedirs(out_dir, exist_ok=True)
+    live = res["track_manage"] != 0
+    arrays = {"boxes": res["boxes"].astype(np.float32), "targets": res["targets"][live].astype(np.float32),
+              "vandyaw": res["vandyaw"][live].astype(np.float64), "live_index": np.flatnonzero(live).astype(np.float64),
+              "track_manage": res["track_manage"].astype(np.float64),
+              "is_static": res["is_static"].astype(np.float32), "is_vis": res["is_vis"].astype(np.float32),
+              "vis_bb": res["vis_bb"].astype(np.float32),
+              "counts": np.array([res["n_elevated"], res["n_ground"], res["num_cluster"]], np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def pct(a, q):
     a = np.sort(np.asarray(a, np.float64))
     return float(a[min(len(a) - 1, int(q * len(a)))]) if len(a) else None
@@ -516,7 +531,8 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
-    ap.add_argument("--windows", type=int, default=0, help="repetitions of the K-step timed window (0 = auto: 5 for short runs, 1 from K = 200)")
+    ap.add_argument("--windows", type=int, default=1, help="equal windows the K timed steps are split into (`value` is the median window); must divide K")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the last timed step returned (boxes, track outputs, counts) as DIR/<name>.npy")
     ap.add_argument("--impl", default="lmot", choices=["lmot", "reference"])
     ap.add_argument("--cpu-sample", type=int, default=60, help="frames of the CPU baseline / parity sample (rank 0, N=1)")
     ap.add_argument("--tracker-stress", type=int, default=40, help="timed steps of the 1024x256 tracker-only workload (0 = skip; rank 0, N=1)")
@@ -549,10 +565,13 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     lmot = importlib.import_module(PKG)
     K, W = args.steps, max(args.warmup, 3)
-    R = args.windows if args.windows > 0 else max(1, min(5, 200 // max(K, 1)))
+    R = args.windows
+    if K < 1 or R < 1 or K % R:
+        raise SystemExit("bench.py: --steps must be a positive multiple of --windows")
+    Kw = K // R                      # steps per window: the R windows are exactly the K timed steps
 
-    # ---- inputs: W + R*K consecutive frames of this rank's sensor stream, resident in HBM and in pinned host memory
-    ts, frames = make_frames(synth, W + R * K, seed_offset=rank)
+    # ---- inputs: W + K consecutive frames of this rank's sensor stream, resident in HBM and in pinned host memory
+    ts, frames = make_frames(synth, W + K, seed_offset=rank)
     n_pts = int(frames.shape[1])
     h_frames = torch.from_numpy(frames).pin_memory()
     d_frames = h_frames.cuda(non_blocking=True)
@@ -584,22 +603,22 @@ def main():
         dist.destroy_process_group()
         return
 
-    # ---- (1) device-resident throughput: `value`.  R windows of exactly K steps, each bracketed by barrier + synchronize.
+    # ---- (1) device-resident throughput: `value`.  R windows of exactly Kw steps, each bracketed by barrier + synchronize.
     ctx.tracker_reset()
     for i in range(W):
         ctx.frame_dev(d_frames[i].data_ptr(), n_pts, ts[i])
-    # every timed step reads a frame no earlier step has read; with the default K the ring is 3x the 126 MB L2.  A short run
+    # every timed step reads a frame no earlier step has read; with the default K the ring is 8x the 50 MB L2.  A short run
     # (ring < L2) could still find its frames in L2 from the upload above: push them out with a buffer larger than L2
-    small_ring = ring_mb < 160
+    small_ring = ring_mb < 64
     if small_ring:
-        l2_flush = torch.empty(192 * 2**20, dtype=torch.uint8, device="cuda")
+        l2_flush = torch.empty(128 * 2**20, dtype=torch.uint8, device="cuda")
         l2_flush.zero_()
     win_ms = []
     for r_ in range(R):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
-        for i in range(W + r_ * K, W + (r_ + 1) * K):
+        for i in range(W + r_ * Kw, W + (r_ + 1) * Kw):
             ctx.frame_dev(d_frames[i].data_ptr(), n_pts, ts[i])
         ctx.flush()                      # device-side join of the context's internal streams into the timing stream
         e1.record(stream)
@@ -607,6 +626,8 @@ def main():
         win_ms.append(e0.elapsed_time(e1))
     res_dev = ctx.frame_fetch()
     live_tracks = int((res_dev["track_manage"] > 0).sum())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res_dev)
 
     # ---- (2) per-stage device time of the same frames, ONE frame in flight (CUDA events on the launching stream)
     ctx.tracker_reset()
@@ -714,7 +735,7 @@ def main():
     # ... and one copy PER FRAME (what lmot_frame_submit issues): the per-copy set-up cost is not negligible at 1.9 MB
     hb0.record(stream)
     for i in range(64):
-        tmp_d[i % 8].copy_(h_frames[i % (W + K)], non_blocking=True)
+        tmp_d[i % len(tmp_d)].copy_(h_frames[i % (W + K)], non_blocking=True)
     hb1.record(stream)
     torch.cuda.synchronize()
     h2d_frame_us = 1e3 * hb0.elapsed_time(hb1) / 64
@@ -732,7 +753,7 @@ def main():
     collected = 0
     t_submit = t_collect = 0.0
     in_flight = 0
-    for i in range(W, W + R * K):        # every step: H2D of its frame; every result is read back inside the region
+    for i in range(W, W + K):            # every step: H2D of its frame; every result is read back inside the region
         if in_flight == depth:
             tc = time.perf_counter(); r = ctx.frame_collect(); t_collect += time.perf_counter() - tc
             collected += 1; in_flight -= 1
@@ -742,15 +763,15 @@ def main():
         tc = time.perf_counter(); r = ctx.frame_collect(); t_collect += time.perf_counter() - tc
         collected += 1; in_flight -= 1
     barrier()
-    e2e_py_s = (time.perf_counter() - t0) / R
-    assert collected == R * K
+    e2e_py_s = (time.perf_counter() - t0) / R      # per window of Kw steps
+    assert collected == K
     d2h = 16 * 4 + r["boxes"].size * 4 + len(r["track_manage"]) * (12 + 16 + 4 + 1 + 1) + r["vis_bb"].size * 4
     py_live = int((r["track_manage"] > 0).sum())
 
     # ---- (3b) the same loop in the reference's host language: host/frame_loop.cpp (C++ over the same two C-ABI calls, pinned host
-    # frames, every result collected, R windows of K steps with lmot_sync on both sides).  This is `e2e`.
+    # frames, every result collected, R windows of Kw steps with lmot_sync on both sides).  This is `e2e`.
     barrier()
-    native, native_err = run_native_e2e(frames, W, K, n_pts, rank, local_rank, world, windows=R)
+    native, native_err = run_native_e2e(frames, W, Kw, n_pts, rank, local_rank, world, windows=R)
     if native is not None and not (native["tracks_last"] == len(r["track_manage"]) and native["live_tracks_last"] == py_live):
         # same frames, same tracker: the native loop must end in the state the Python loop ended in
         native_err, native = f"frame_loop ended in a different tracker state: {native} vs {len(r['track_manage'])} tracks / {py_live} live", None
@@ -770,8 +791,8 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     win_max = [float(x) for x in t[:R]]
     dev_ms_max, e2e_ms_max = float(np.median(win_max)) if R % 2 else float(sorted(win_max)[(R - 1) // 2]), float(t[R])
-    value = world * K / (dev_ms_max * 1e-3)
-    e2e = world * K / (e2e_ms_max * 1e-3)
+    value = world * Kw / (dev_ms_max * 1e-3)
+    e2e = world * Kw / (e2e_ms_max * 1e-3)
 
     cpu_baseline = parity = None
     if rank == 0 and world == 1 and args.cpu_sample > 0:
@@ -804,32 +825,32 @@ def main():
         ok = parity is None or parity["ok"]
         line = {
             "metric": "HDL-64 frames/sec (120K pts, 64 tracks)", "value": (value if ok else None), "unit": "frames/s", "n_gpus": world, "steps": K, "warmup": W,
-            "ms_per_step": dev_ms_max / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "windows": R, "window_values": [world * K / (w_ * 1e-3) for w_ in win_max],
+            "ms_per_step": dev_ms_max / Kw, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
+            "windows": R, "window_values": [world * Kw / (w_ * 1e-3) for w_ in win_max],
             "dtype": "f32 points / f64 tracker", "data": "synthetic",
             "config": {"workload": WORKLOAD, "points_per_frame": n_pts, "scene": SCENE, "live_tracks_end": live_tracks,
                        "tracks_in_table_end": int(len(res_dev["track_manage"])), "rule_filter": "INTENDED",
                        "parallelism": f"{world} independent sensor stream(s), one per GPU, no collective on the data path",
                        "pipeline_depth": int(ctx.params.pipeline_depth), "result_ring": int(ctx.params.result_ring),
-                       "l2_policy": (f"every step reads a different frame of a {ring_mb:.0f} MiB ring (> 126 MB L2)" if not small_ring else
-                                     f"every step reads a different frame of a {ring_mb:.0f} MiB ring, L2 flushed (192 MiB written) before the first timed window")},
+                       "l2_policy": (f"every step reads a different frame of a {ring_mb:.0f} MiB ring (> 50 MB L2)" if not small_ring else
+                                     f"every step reads a different frame of a {ring_mb:.0f} MiB ring, L2 flushed (128 MiB written) before the first timed window")},
             "parity_check": parity,
             "e2e": {"value": (e2e if ok else None), "unit": "frames/s", "h2d_bytes_per_step": frame_bytes, "d2h_bytes_per_step": int(d2h),
-                    "windows": (native["windows"] if native else 1), "window_values": ([world * K / w_ for w_ in native["window_s"]] if native else None),
+                    "windows": (native["windows"] if native else 1), "window_values": ([world * Kw / w_ for w_ in native["window_s"]] if native else None),
                     "pinned_h2d_gbs_this_box": h2d_gbs, "h2d_us_per_frame_copy_this_box": h2d_frame_us, "pcie_bound_frames_per_s": 1e6 / h2d_frame_us,
                     "driver": ("host/frame_loop.cpp: C++ loop over lmot_frame_submit / lmot_frame_collect, pinned host frames" if native else "python ctypes loop"),
                     "native_driver_error": native_err,
                     "host_us_per_step": ({"submit": native["submit_us_per_frame"], "collect_incl_wait": native["collect_us_per_frame"]} if native
-                                         else {"submit": 1e6 * t_submit / (R * K), "collect_incl_wait": 1e6 * t_collect / (R * K)}),
-                    "python_ctypes_loop": {"value": world * K / e2e_py_s, "unit": "frames/s", "note": "same two calls from a Python loop (this rank)",
-                                           "host_us_per_step": {"submit": 1e6 * t_submit / (R * K), "collect_incl_wait": 1e6 * t_collect / (R * K)}}},
-            "gpu_launches": KERNELS_PER_FRAME * K * R,
+                                         else {"submit": 1e6 * t_submit / K, "collect_incl_wait": 1e6 * t_collect / K}),
+                    "python_ctypes_loop": {"value": world * Kw / e2e_py_s, "unit": "frames/s", "note": "same two calls from a Python loop (this rank)",
+                                           "host_us_per_step": {"submit": 1e6 * t_submit / K, "collect_incl_wait": 1e6 * t_collect / K}}},
+            "gpu_launches": KERNELS_PER_FRAME * K,
             "clocks": clocks,
             "latency_us": latency,
             "roofline": {"bound": "hbm", "kernel": "ground_fused_kernel (the whole ground_removal stage: bin + polar grid + classify/partition, one launch)",
                          "achieved": achieved, "peak": peak, "peak_source": peak_src, "unit": "GB/s", "frac": achieved / peak,
                          "algorithmic_bytes_per_launch": ground_bytes, "avg_launch_ms": float(ground_launch_ms),
-                         "launches_timed": K, "traffic": TRAFFIC_NCU, "traffic_source": TRAFFIC_SOURCE,
+                         "launches_timed": K,
                          "how": "K launches back to back on one stream, CUDA events around the K; consecutive launches are chained as programmatic dependents (no event between them: the next launch's CTAs set up while the previous grid drains and wait in griddepcontrol.wait)",
                          "note": "latency bound at 120 k points: 3.84 MB is 0.6 us of HBM time, the kernel needs two frame-wide barriers and one count exchange; see roofline_dense_1m and batched_8x120k.roofline"},
             "stage_ms": {n: float(v) for n, v in zip(stage_names, stage_ms)},

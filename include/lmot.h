@@ -1,4 +1,4 @@
-/* lmot.h -- C ABI of the B200-native LiDAR multi-object-tracking hot path (liblmot.so).
+/* lmot.h -- C ABI of the H100-native LiDAR multi-object-tracking hot path (liblmot.so).
  *
  * Drop-in boundary (SURVEY.md §8b).  The reference has no FFI; its boundary is four C++ free functions
  * called from the three ROS node callbacks.  Each entry point below replaces one of them:

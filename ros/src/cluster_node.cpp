@@ -1,4 +1,4 @@
-// cluster_node.cpp -- `rosrun object_tracking cluster`, B200 edition (SURVEY.md §8(f)1).
+// cluster_node.cpp -- `rosrun object_tracking cluster`, H100 edition (SURVEY.md §8(f)1).
 //
 // Same ROS surface as the reference's node (object_tracking/src/cluster/main.cpp:237-256): node "cluster", subscribes
 // "none_ground_topic"; publishes "output" (clustered cloud), "realtime_cost_map" (nav_msgs/OccupancyGrid), "cluster_obs"

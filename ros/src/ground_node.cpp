@@ -1,4 +1,4 @@
-// ground_node.cpp -- `rosrun object_tracking ground`, B200 edition (SURVEY.md §8(f)1).
+// ground_node.cpp -- `rosrun object_tracking ground`, H100 edition (SURVEY.md §8(f)1).
 //
 // Same ROS surface as the reference's node (object_tracking/src/groundremove/main.cpp:139-157): node "ground", subscribes
 // "velodyne_points" (sensor_msgs/PointCloud2, queue 160), parameters filter_z_min / filter_z_max (-3 / 1), publishes

@@ -1,4 +1,4 @@
-// tracking_node.cpp -- `rosrun object_tracking tracking`, B200 edition (SURVEY.md §8(f)1).
+// tracking_node.cpp -- `rosrun object_tracking tracking`, H100 edition (SURVEY.md §8(f)1).
 //
 // Same ROS surface as the reference's node (object_tracking/tracking/main.cpp:413-445): node "obj_track", subscribes
 // "track_box" (object_tracking/trackbox) and "/gps/odom" (ego speed / yaw), publishes the track markers on

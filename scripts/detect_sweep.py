@@ -1,5 +1,5 @@
 """Diagnostic (not the bench contract): device time of the streaming detection kernels, CUDA events on the launching stream,
-inputs cycling through a ring larger than the 126 MB L2:
+inputs cycling through a ring larger than the 50 MB L2:
   ground_fused_kernel alone on 120 k / 1 M-point frames, and the batched tick (8 x 120 k): ground + CCL as two launches."""
 import importlib, json, os, sys
 import numpy as np
@@ -9,7 +9,7 @@ sys.path.insert(0, ROOT)
 PKG = "3d-lidar-multi-object-tracking_b200"
 lmot = importlib.import_module(PKG)
 synth = importlib.import_module(PKG + ".synth")
-peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0
 SCENE = dict(n_objects=150, lattice_pitch=3.8, ped_fraction=0.65)
 
 

@@ -14,7 +14,7 @@ ts, frames = bench.make_frames(synth, W + K)
 n = frames.shape[1]
 d = torch.from_numpy(frames).cuda()
 torch.cuda.synchronize()
-for coop, trk, fit in ((1, 592, 296), (0, 592, 296), (0, 148, 148)):
+for coop, trk, fit in ((1, 528, 264), (0, 528, 264), (0, 132, 132)):
     os.environ["LMOT_TRK_CTAS"] = str(trk); os.environ["LMOT_FIT_CTAS"] = str(fit); os.environ["LMOT_COOP"] = str(coop)
     for depth in (1, 2, 4, 8):
         prm = lmot.default_params(); prm.pipeline_depth = depth

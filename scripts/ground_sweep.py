@@ -9,7 +9,7 @@ PKG = "3d-lidar-multi-object-tracking_b200"
 lmot = importlib.import_module(PKG)
 synth = importlib.import_module(PKG + ".synth")
 
-peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0
 out = []
 sizes = [("hdl64_120k", synth.SceneConfig(n_objects=150, lattice_pitch=3.8, ped_fraction=0.65, seed=1), 120000, 80),
          ("dense_1m", synth.dense_config(n_objects=150, lattice_pitch=3.8, ped_fraction=0.65, seed=7), 1000000, 10)]

@@ -1,6 +1,6 @@
 """Key metrics of every launch in an .ncu-rep (`ncu --set full` capture) as a small CSV for profiles/.
 
-    python scripts/ncu_summary.py gpurun_out/X.ncu-rep > profiles/X.csv
+    python scripts/ncu_summary.py measure_out/X.ncu-rep > profiles/X.csv
 """
 import csv, subprocess, sys
 

@@ -1,6 +1,6 @@
 """Workload for `ncu` captures of the detection kernels: 4 stand-alone ground launches on dense 1 M-point frames, then 3 batched
 ticks (8 x 120 k: ground, CCL, counting sort, box fitting) without the tracker.
-  ncu --set full --import-source on --clock-control none -k regex:"ground_fused|ccl_|box_fit" --launch-skip 2 -c 8 -o gpurun_out/r2_detect python scripts/prof_detect.py"""
+  ncu --set full --import-source on --clock-control none -k regex:"ground_fused|ccl_|box_fit" --launch-skip 2 -c 8 -o measure_out/r2_detect python scripts/prof_detect.py"""
 import importlib, os, sys
 os.environ.setdefault("LMOT_FUSE_CCL", "0")     # profile clustering as its own kernel
 import numpy as np

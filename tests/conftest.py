@@ -12,7 +12,7 @@ PKG = "3d-lidar-multi-object-tracking_b200"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")

@@ -194,7 +194,7 @@ def test_fused_kernel_chunkings_bit_exact(pkg, ref_intended, synth):
 
 
 def test_fused_kernel_tiles_beyond_shared_memory_bit_exact(pkg, ref_intended, synth):
-    """Chunks longer than the 7 shared-memory-resident tiles (frames > ~1.06 M points on 148 SMs) re-read their tail from
+    """Chunks longer than the 8 shared-memory-resident tiles (frames > ~1.08 M points on 132 SMs) re-read their tail from
     global memory in the classification phase: 1.6 M points, bit-exact against the reference."""
     pts = synth.uniform_cloud(1_600_000, 22)
     ctx = _ctx_with(pkg, 16384, max_points=1_600_000)
