@@ -92,9 +92,9 @@ ABI_SYMBOLS = [
     "lmot_frame_dev", "lmot_frame_fetch", "lmot_frame_submit", "lmot_frame_collect", "lmot_frames_in_flight", "lmot_frame_ready", "lmot_flush",
     "lmot_ground_remove_dev", "lmot_detect_dev", "lmot_sync",
     "lmot_batch_submit", "lmot_batch_dev", "lmot_batch_detect_dev", "lmot_batch_collect", "lmot_batch_fetch", "lmot_batch", "lmot_batch_ground_ccl_dev",
-    "lmot_debug_stage_clocks", "lmot_detect_boxes_dev", "lmot_track_step_lists_dev", "lmot_tracker_counters_dev", "lmot_tracker_table_received",
+    "lmot_detect_boxes_dev", "lmot_track_step_lists_dev", "lmot_tracker_counters_dev", "lmot_tracker_table_received",
     "lmot_origin_points", "lmot_tracker_table", "lmot_tracker_set_num_tracks", "lmot_tracker_reset", "lmot_tracker_num_tracks", "lmot_tracker_dump", "lmot_tracker_load", "lmot_tracker_get_ego", "lmot_tracker_set_ego",
-    "lmot_debug_polar_grid", "lmot_debug_cell_index", "lmot_debug_label_grid", "lmot_debug_phase_clock", "lmot_debug_timeline", "lmot_debug_tracker_trace", "lmot_selftest_atan2f",
+    "lmot_debug_polar_grid", "lmot_debug_cell_index", "lmot_debug_label_grid", "lmot_selftest_atan2f",
     "lmot_enable_timing", "lmot_last_stage_ms", "lmot_last_kernel_ms", "lmot_debug_host_ns",
 ]
 
@@ -407,13 +407,6 @@ class Lmot:
         self._chk(self.lib.lmot_batch_fetch(self.h, C.byref(bo)))
         return self._batch_result(bo, bufs, want_boxes)
 
-    def debug_stage_clocks(self, which: int):
-        """which = 1: (frames, 16) stamps of the last ccl_bitmap_kernel; 2: (CTAs, 8) of the last box_fit_kernel (phase clock armed)."""
-        buf = np.zeros((4096, 16), np.uint64)
-        n = C.c_int(0); w = C.c_int(0)
-        self._chk(self.lib.lmot_debug_stage_clocks(self.h, int(which), buf.ctypes.data_as(C.POINTER(C.c_ulonglong)), 4096, C.byref(n), C.byref(w)))
-        return buf.reshape(-1)[: n.value * w.value].reshape(n.value, w.value).copy()
-
     def tracker_reset(self):
         self._chk(self.lib.lmot_tracker_reset(self.h))
 
@@ -485,34 +478,6 @@ class Lmot:
         nc = C.c_int(0)
         self._chk(self.lib.lmot_debug_label_grid(self.h, grid.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(nc)))
         return grid.reshape(250, 250), nc.value
-
-    def debug_timeline(self):
-        """(frames, 5 + kernels) float32 ms: completion of the stage boundaries and kernels of the frames still in the result ring."""
-        buf = np.full((64, 64), -1.0, np.float32)
-        n = C.c_int(0); stride = C.c_int(0)
-        self._chk(self.lib.lmot_debug_timeline(self.h, buf.ctypes.data_as(C.POINTER(C.c_float)), 64, C.byref(n), C.byref(stride)))
-        flat = buf.reshape(-1)[: n.value * stride.value].reshape(n.value, stride.value) if n.value else buf[:0]
-        return flat
-
-    def debug_tracker_trace(self):
-        """(32, 8) uint64 ns, oldest step first: TA start, TA end, TB start, TB end, TC start, TC end, latest start of a working TA CTA, same for TB."""
-        raw = np.zeros(32 * 8 + 64, np.uint64); nxt = C.c_int(0)
-        self._chk(self.lib.lmot_debug_tracker_trace(self.h, raw.ctypes.data_as(C.POINTER(C.c_ulonglong)), C.byref(nxt)))
-        buf = raw[:256].reshape(32, 8).copy()
-        self.last_tc_phases = raw[256:272].copy()
-        self.last_tb_phases = raw[272:282].copy()
-        self.last_ta_phases = raw[288:304].copy()    # CTA 0 of imm_predict_gate_kernel
-        self.last_gate_phases = raw[282:288].copy()     # [0] gate kernel entry, [1] gate kernel after its wait, [2] TA CTA 0 entry (before its wait)        # same for the first track's warp of imm_update_kernel       # %globaltimer stamps inside the last spawn_output_kernel (fast path)
-        for k in (0, 2, 4):
-            buf[:, k] = ~buf[:, k]        # starts are stored complemented (see trace_start in tracker.cu)
-        return np.roll(buf, -nxt.value, axis=0)
-
-    def debug_phase_clock(self):
-        """First call arms the phase clock of ground_fused_kernel; later calls -> (n_ctas, 8) uint64 ns stamps of the last launch."""
-        buf = np.zeros((1024, 8), np.uint64)
-        n = C.c_int(0)
-        self._chk(self.lib.lmot_debug_phase_clock(self.h, buf.ctypes.data_as(C.POINTER(C.c_ulonglong)), 1024, C.byref(n)))
-        return buf[: n.value]
 
     def debug_polar_grid(self):
         names = ["minz", "height", "smoothed", "hdiff", "hground"]

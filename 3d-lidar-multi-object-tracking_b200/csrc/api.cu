@@ -524,7 +524,6 @@ void lmot_destroy(lmot_ctx* ctx) {
   batch_destroy(c);
   for (int i = 0; i < c->n_results; ++i) result_destroy(&c->results[i]);
   tracker_free(c);
-  cudaFree(c->d_phase_clock); cudaFree(c->d_trk_trace); cudaFree(c->d_ccl_clock); cudaFree(c->d_fit_clock);
   cudaFree(c->d_mt_raw);
   if (c->trk_stream) cudaStreamDestroy(c->trk_stream);
   if (c->pub_stream) cudaStreamDestroy(c->pub_stream);
@@ -1227,94 +1226,6 @@ int lmot_debug_cell_index(lmot_ctx* ctx, int32_t* ch, int32_t* bin, int n) {
     if (cell[i] == kNoCell) { ch[i] = -1; bin[i] = -1; }
     else { ch[i] = cell[i] / kNumBin; bin[i] = cell[i] % kNumBin; }
   }
-  return LMOT_OK;
-}
-
-// diagnostic: completion times (ms, relative to the oldest frame's start) of the stage boundaries and of every kernel of the
-// frames still in the result ring, pipelined submissions included.  out[frame][0..4] = ev[0..4] (start, ground, cluster, box,
-// tracker), out[frame][5..5+n) = the kernels in launch order; row stride 5 + kMaxKernelEvents floats; -1 = not recorded.
-int lmot_debug_timeline(lmot_ctx* ctx, float* out, int cap_frames, int* n_frames, int* row_stride) {
-  if (!ctx || !out) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  int rc = lmot_sync(ctx);
-  if (rc) return rc;
-  const int stride = 5 + kMaxKernelEvents;
-  if (row_stride) *row_stride = stride;
-  int n = 0;
-  Result* base = nullptr;
-  for (int k = 0; k < c->n_results && n < cap_frames; ++k) {
-    Result* r = &c->results[(c->res_next + k) % c->n_results];      // oldest first
-    if (!r->has_tracks || r->n_kev == 0) continue;
-    if (!base) base = r;
-    float* o = out + (size_t)n * stride;
-    for (int i = 0; i < stride; ++i) o[i] = -1.f;
-    for (int i = 0; i < 5; ++i) if (cudaEventElapsedTime(&o[i], base->ev[0], r->ev[i]) != cudaSuccess) { o[i] = -1.f; cudaGetLastError(); }
-    for (int i = 0; i < r->n_kev; ++i) if (cudaEventElapsedTime(&o[5 + i], base->ev[0], r->kev[i]) != cudaSuccess) { o[5 + i] = -1.f; cudaGetLastError(); }
-    ++n;
-  }
-  if (n_frames) *n_frames = n;
-  return LMOT_OK;
-}
-
-// diagnostic: %globaltimer spans (ns) of the tracker kernels of the last 32 tracker steps: out[32][8] = TA first start, TA last end,
-// TB start, TB end, TC start, TC end, latest start of a TA CTA that had a track, same for TB; then out[256..271] = phase stamps of the last spawn_output_kernel (fast path), out[272..287] = of the first track's warp of the last imm_update_kernel; *next = ring position of the NEXT step (oldest entry)
-int lmot_debug_tracker_trace(lmot_ctx* ctx, unsigned long long* out, int* next) {
-  if (!ctx || !out) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  int rc = lmot_sync(ctx);
-  if (rc) return rc;
-  if (!c->d_trk_trace) return LMOT_ERR_STATE;
-  // the last 32 steps, oldest first (rows of steps that never ran stay zero), then the 32 phase stamps
-  for (int i = 0; i < 32; ++i) {
-    const long long f = (long long)c->trk_frames - 32 + i;
-    if (f < 0) { memset(out + i * 8, 0, 8 * sizeof(unsigned long long)); continue; }
-    LMOT_CUDA(c, cudaMemcpy(out + i * 8, c->d_trk_trace + (size_t)(f % kTraceRows) * 8, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  }
-  LMOT_CUDA(c, cudaMemcpy(out + 256, c->d_trk_trace + (size_t)kTraceRows * 8, 64 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  if (next) *next = 0;
-  return LMOT_OK;
-}
-
-// diagnostic: switch the phase clock of ground_fused_kernel on (allocates [CTAs][8] u64) and read the last launch's stamps
-int lmot_debug_phase_clock(lmot_ctx* ctx, unsigned long long* out, int cap_ctas, int* n_ctas) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  int rc = lmot_sync(ctx);
-  if (rc) return rc;
-  if (!c->d_phase_clock) {
-    LMOT_CUDA(c, cudaMalloc(&c->d_phase_clock, (size_t)c->fused_max_ctas * 8 * sizeof(unsigned long long)));
-    LMOT_CUDA(c, cudaMemset(c->d_phase_clock, 0, (size_t)c->fused_max_ctas * 8 * sizeof(unsigned long long)));
-    LMOT_CUDA(c, cudaMalloc(&c->d_trk_trace, ((size_t)kTraceRows * 8 + 64) * sizeof(unsigned long long)));
-    LMOT_CUDA(c, cudaMemset(c->d_trk_trace, 0, ((size_t)kTraceRows * 8 + 64) * sizeof(unsigned long long)));
-    LMOT_CUDA(c, cudaMalloc(&c->d_ccl_clock, (size_t)kMaxBatch * 16 * sizeof(unsigned long long)));
-    LMOT_CUDA(c, cudaMemset(c->d_ccl_clock, 0, (size_t)kMaxBatch * 16 * sizeof(unsigned long long)));
-    LMOT_CUDA(c, cudaMalloc(&c->d_fit_clock, (size_t)kFitClockCtas * 8 * sizeof(unsigned long long)));
-    LMOT_CUDA(c, cudaMemset(c->d_fit_clock, 0, (size_t)kFitClockCtas * 8 * sizeof(unsigned long long)));
-    c->trk_frames = 0;
-    if (n_ctas) *n_ctas = 0;
-    return LMOT_OK;
-  }
-  const int g = c->last_ground_ctas < cap_ctas ? c->last_ground_ctas : cap_ctas;
-  if (out && g > 0) LMOT_CUDA(c, cudaMemcpy(out, c->d_phase_clock, (size_t)g * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  if (n_ctas) *n_ctas = g;
-  return LMOT_OK;
-}
-
-// diagnostic (after the phase clock was switched on): %globaltimer stamps of the last ccl_bitmap_kernel launch (which = 1:
-// out[frames][16]) or of the last box_fit_kernel launch (which = 2: out[CTAs][8]: start, first cluster's point pass done, first
-// cluster fitted, all clusters done, end)
-int lmot_debug_stage_clocks(lmot_ctx* ctx, int which, unsigned long long* out, int cap_rows, int* n_rows, int* row_words) {
-  if (!ctx || !out || (which != 1 && which != 2)) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  int rc = lmot_sync(ctx);
-  if (rc) return rc;
-  if (!c->d_ccl_clock) return LMOT_ERR_STATE;
-  const int words = which == 1 ? 16 : 8;
-  int rows = which == 1 ? kMaxBatch : (c->last_fit_ctas < kFitClockCtas ? c->last_fit_ctas : kFitClockCtas);
-  if (rows > cap_rows) rows = cap_rows;
-  if (rows > 0) LMOT_CUDA(c, cudaMemcpy(out, which == 1 ? c->d_ccl_clock : c->d_fit_clock, (size_t)rows * words * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  if (n_rows) *n_rows = rows;
-  if (row_words) *row_words = words;
   return LMOT_OK;
 }
 

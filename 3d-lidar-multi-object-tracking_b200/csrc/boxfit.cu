@@ -300,15 +300,10 @@ __device__ bool rule_filter(const float pc[4][2], float maxZ, int n, const BoxPa
   return false;
 }
 
-__device__ __forceinline__ void fit_mark(unsigned long long* clk, int slot) {
-  if (clk && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); const unsigned row = blockIdx.y * gridDim.x + blockIdx.x; if (row < (unsigned)kFitClockCtas) clk[row * 8 + slot] = t; }
-}
-
 template <int NT>
 __global__ void __launch_bounds__(NT, 1024 / NT)     // <= 64 registers: 1,024 threads of box fitting per SM
 box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxParams P,
-               const unsigned long long* __restrict__ mt_raw, int n_raw, int max_clusters, int max_boxes,
-               unsigned long long* __restrict__ clk) {
+               const unsigned long long* __restrict__ mt_raw, int n_raw, int max_clusters, int max_boxes) {
   constexpr int kFitThreads = NT;
   fit_pdl_trigger();
   fit_pdl_wait();                          // scatter_kernel is complete
@@ -338,7 +333,6 @@ box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxPa
   const float half = P.roi / 2;
   const float pic = P.pic_scale * P.roi;     // 900
 
-  fit_mark(clk, 0);
   for (int k = blockIdx.x + 1; k <= K; k += gridDim.x) {
     const int n = seg_size[k];
     const float4* seg = sorted_pts + seg_start[k];          // the cluster's points, cloud order
@@ -429,7 +423,6 @@ box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxPa
       mxx = s_partf[4][0]; mxy = s_partf[5][0]; mxz = s_partf[6][0];
     }
 
-    if (k == (int)blockIdx.x + 1) fit_mark(clk, 1);
     // first-occurrence min / max slope points (:268-280).  If no slope beats the 999 / -999 seeds the reference
     // reads uninitialised floats; defined here as (0,0).
     float minMx = 0.f, minMy = 0.f, maxMx = 0.f, maxMy = 0.f;
@@ -665,7 +658,6 @@ box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxPa
       }
       __syncthreads();
     }
-    if (k == (int)blockIdx.x + 1) fit_mark(clk, 2);
     for (int c = 0; c < 4; ++c) { pc[c][0] = s_pc[c][0]; pc[c][1] = s_pc[c][1]; }
     const bool ok = rule_filter(pc, maxZ, n, P);
     if (tid == 0) {
@@ -683,7 +675,6 @@ box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxPa
     __syncthreads();
   }
 
-  fit_mark(clk, 3);
   // ---- the last CTA of the frame compacts the accepted boxes in cluster-id order
   __threadfence();
   __syncthreads();
@@ -727,7 +718,6 @@ box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxPa
     __syncthreads();
     if (tid == 0) { __threadfence(); atomicAdd(det_sem, 1); }
   }
-  fit_mark(clk, 4);
 }
 
 // batched submissions (one frame per sensor stream): the frames' box lists, concatenated in stream order, are ONE measurement
@@ -889,11 +879,9 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
     cfg.gridDim = dim3(gx, F); cfg.blockDim = dim3(F == 1 ? kFitThreadsFrame : kFitThreadsBatch); cfg.dynamicSmemBytes = 0; cfg.stream = st; cfg.attrs = &pdl; cfg.numAttrs = 1;
     const unsigned long long* mt = c->d_mt_raw;
     const int n_raw = c->n_mt_raw, max_boxes = c->prm.max_boxes;
-    unsigned long long* clk = c->d_fit_clock;
-    if (F == 1) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsFrame>, B, P, mt, n_raw, max_clusters, max_boxes, clk));
-    else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsBatch>, B, P, mt, n_raw, max_clusters, max_boxes, clk));
+    if (F == 1) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsFrame>, B, P, mt, n_raw, max_clusters, max_boxes));
+    else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsBatch>, B, P, mt, n_raw, max_clusters, max_boxes));
   }
-  c->last_fit_ctas = gx * F;
   kernel_mark(c, s0, st);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;

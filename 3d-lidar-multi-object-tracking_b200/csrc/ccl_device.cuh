@@ -82,10 +82,6 @@ __device__ __forceinline__ int uf_compress(volatile int* L, int x) {
   return p;
 }
 
-__device__ __forceinline__ void ccl_mark(unsigned long long* clk, int row, int slot) {
-  if (clk && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); clk[row * 16 + slot] = t; }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // Node ids are DENSE.  (Round 1 / the first version of round 2 numbered a piece word * 16 + k: the 32 lanes of a warp then hit the
 // same shared-memory bank on every parent access, each thread walked its own ragged list of pieces, and every flatten / union was a
@@ -105,7 +101,7 @@ __device__ __forceinline__ void ccl_flatten(volatile int* L, int P) {
   __syncthreads();
 }
 
-__device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char* ccl_smem, unsigned long long* __restrict__ clk, int clk_row) {
+__device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char* ccl_smem) {
   int* s_par = reinterpret_cast<int*>(ccl_smem);                       // [<= 32000] parent id, later -(cluster id) at roots
   unsigned* s_seed = reinterpret_cast<unsigned*>(s_par + kNodes);       // [2000]
   unsigned* s_occ = s_seed + kBitWords;                                 // [2000]
@@ -116,7 +112,6 @@ __device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char*
   unsigned* __restrict__ once = F.once; unsigned* __restrict__ twice = F.twice; unsigned* __restrict__ prev_occ = F.prev_occ;
   int* __restrict__ out = F.out;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  ccl_mark(clk, clk_row, 0);
   const int w0 = 2 * tid;
   const bool own = tid < kBitWords / 2;
   // A: seed = cells with more than one point (component_clustering.cpp:136); the bit planes are re-armed for the next frame
@@ -130,7 +125,6 @@ __device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char*
   }
   if (tid == 0) s_warp[40] = 0;
   __syncthreads();
-  ccl_mark(clk, clk_row, 1);
   // B: occupied = seed dilated 3x3, clipped at the border (:137-214); ids: exclusive scan of the pieces per word
   unsigned occ[2] = {0u, 0u};
   int np0 = 0, np1 = 0;
@@ -170,7 +164,6 @@ __device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char*
     P = s_warp[32];
   }
   __syncthreads();
-  ccl_mark(clk, clk_row, 2);
   // C: first parent = the smallest neighbour a piece touches (leftmost touching piece of the row above, else the piece it
   // continues from the previous word, else itself); every OTHER adjacency becomes a pair for step E
   if (own) {
@@ -226,11 +219,9 @@ __device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char*
     }
   }
   __syncthreads();
-  ccl_mark(clk, clk_row, 3);
   volatile int* Lv = s_par;
   // D: flatten
   ccl_flatten(Lv, P);
-  ccl_mark(clk, clk_row, 4);
   // E: the remaining adjacencies, one pair per thread
   if (s_warp[40] <= kPairCap) {
     const int npairs = s_warp[40];
@@ -274,10 +265,8 @@ __device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char*
     }
   }
   __syncthreads();
-  ccl_mark(clk, clk_row, 5);
   // F: flatten again
   ccl_flatten(Lv, P);
-  ccl_mark(clk, clk_row, 6);
   // G: id = 1 + rank of the root among all roots in id (= raster) order (:247-257); thread t ranks the ids [t*c, (t+1)*c)
   {
     const int c = (P + kCclThreads - 1) / kCclThreads;
@@ -304,7 +293,6 @@ __device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char*
     for (int id = i0; id < i1; ++id) if (s_par[id] == id) s_par[id] = -(++rank);
   }
   __syncthreads();
-  ccl_mark(clk, clk_row, 7);
   // H: label grid, sparse: cells occupied now get their id, cells occupied only in the previous frame are cleared
   if (own) {
 #pragma unroll
@@ -328,7 +316,6 @@ __device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char*
       }
     }
   }
-  ccl_mark(clk, clk_row, 8);
 }
 
 

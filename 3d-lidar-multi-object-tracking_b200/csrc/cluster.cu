@@ -52,9 +52,9 @@ cart_cells_kernel(const float4* __restrict__ elev, const int* __restrict__ count
 }
 
 __global__ void __launch_bounds__(kCclThreads, 1)
-ccl_dense_kernel(const __grid_constant__ CclBatch B, unsigned long long* __restrict__ clk) {
+ccl_dense_kernel(const __grid_constant__ CclBatch B) {
   extern __shared__ __align__(16) unsigned char ccl_smem[];
-  ccl_dense_body(B.f[blockIdx.x], ccl_smem, clk, (int)blockIdx.x);
+  ccl_dense_body(B.f[blockIdx.x], ccl_smem);
 }
 
 // ---- the cluster node's side outputs (src/cluster/main.cpp:62-99), SURVEY.md §8(f)3 ------------------------------
@@ -179,7 +179,7 @@ int ccl_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st) {
     B.f[i].out = s->d_label_grid; B.f[i].counters = s->d_counters;
   }
   for (int i = F; i < kMaxBatch; ++i) B.f[i] = B.f[0];
-  ccl_dense_kernel<<<F, kCclThreads, kDenseSmem, st>>>(B, c->d_ccl_clock);
+  ccl_dense_kernel<<<F, kCclThreads, kDenseSmem, st>>>(B);
   kernel_mark(c, slots[0], st);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;

@@ -277,14 +277,6 @@ __device__ __forceinline__ void polar_grid_slice(const GroundParams& p, const un
 // ---------------------------------------------------------------------------------------------------------------
 // frame-wide barrier (all CTAs of a frame co-resident).  The counter is never reset: launch k of a slot waits for
 // `target` = arrivals of all earlier launches + the arrivals this barrier needs (host-side bookkeeping).
-// diagnostic (scripts/ground_phases.py): %globaltimer of thread 0 at the phase boundaries, [CTA][8]; nullptr in production
-__device__ __forceinline__ void phase_mark(unsigned long long* clk, int slot) {
-  if (clk && threadIdx.x == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    clk[blockIdx.x * 8 + slot] = t;
-  }
-}
 
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -486,8 +478,7 @@ __device__ __forceinline__ void bin_pair(int t0, int T, int cnt, int res_tiles, 
 // memory.  With ring-major clouds a chunk spans most of the 80 channels, so every CTA redid most of the grid and the kernel
 // issued far more instructions.  The grid is evaluated ONCE, spread over the CTAs.)
 __global__ void __launch_bounds__(kFusedThreads, 1)
-ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant__ GroundParams p, float roi,
-                    unsigned long long* __restrict__ phase_clock) {
+ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant__ GroundParams p, float roi) {
   extern __shared__ __align__(128) unsigned char fsm[];
   const int Gf = B.ctas_per_frame;
   const int frame = blockIdx.x / Gf, cta = blockIdx.x - frame * Gf;
@@ -518,7 +509,6 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
   const int cnt = end - beg;
   const int T = (cnt + kTilePts - 1) / kTilePts;
 
-  phase_mark(phase_clock, 0);
   // ---- phase 0: arm the TMA copies of the resident tiles; re-arm the OTHER key grid for the slot's next frame
   // (a launch chained behind the previous ground kernel of its stream -- ground_launch_batch, `chain` -- becomes resident while that
   // kernel drains: everything up to griddep_wait() touches shared memory only; the wait returns when the preceding grid has
@@ -574,9 +564,7 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
     const int k = tid + j * kFusedThreads;
     if (k < kPolarCells) { const unsigned v = s_keys[k]; if (v != 0xFFFFFFFFu) atomicMin(&keys[k], v); }
   }
-  phase_mark(phase_clock, 1);
   grid_barrier(F.bar, F.bar_target, B.spin_limit);
-  phase_mark(phase_clock, 2);
 
   // ---- phase 2: the polar grid, channels split over the first min(Gf, 80) CTAs of the frame (one halo channel per side recomputed)
   {
@@ -586,9 +574,7 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
       polar_grid_slice(p, keys, own0, own1 - own0, s_H, s_G, (float*)nullptr, (float*)nullptr, (float*)nullptr, (float*)nullptr, F.hg, F.lim);
     }
   }
-  phase_mark(phase_clock, 3);
   grid_barrier(F.bar, F.bar_target + (unsigned)Gf, B.spin_limit);
-  phase_mark(phase_clock, 4);
 
   // ---- phase 3: labels (ground_removal.cpp:221-247), per-warp counts
   unsigned labs = 0;                                // 2 bits per tile: 0 dropped, 1 ground, 2 elevated
@@ -654,7 +640,6 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
   }
   }
   __syncthreads();
-  phase_mark(phase_clock, 5);
   if (warp < T) {                                   // warp w scans the 32 warp counts of tile w
     const unsigned v = s_cnt[warp * 32 + lane];
     unsigned inc = v;
@@ -701,7 +686,6 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
   }
   __syncthreads();
 
-  phase_mark(phase_clock, 6);
   // ---- phase 3b: order-preserving output clouds + the first pass of clustering on the elevated points
   unsigned run_e = s_base[0], run_g = s_base[1];
   const unsigned lt = (1u << lane) - 1u;
@@ -729,7 +713,6 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
     const unsigned tt = s_ttot[t];
     run_e += tt & 0xFFFFu; run_g += tt >> 16;
   }
-  phase_mark(phase_clock, 7);
 
   // ---- component clustering of this frame by the last of its CTAs to get here: no launch (and no launch latency) between ground
   // removal and clustering, and the CCL of a frame that finishes early overlaps the other frames' tails (batched launches)
@@ -741,7 +724,7 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
     __syncthreads();
     if (s_last) {
       __threadfence();
-      ccl_dense_body(F.ccl, fsm, nullptr, 0);     // 1,024 threads, reuses the kernel's dynamic shared memory (>= kDenseSmem, see ground_launch_batch)
+      ccl_dense_body(F.ccl, fsm);     // 1,024 threads, reuses the kernel's dynamic shared memory (>= kDenseSmem, see ground_launch_batch)
     }
   }
 }
@@ -903,7 +886,7 @@ int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* 
   }
   float roi = c->prm.roi_m;
   GroundParams gp = c->gp;
-  void* args[] = {(void*)&B, (void*)&gp, (void*)&roi, (void*)&c->d_phase_clock};
+  void* args[] = {(void*)&B, (void*)&gp, (void*)&roi};
   // every frame's chunk is laid out with the tile count of the longest one (the kernel derives its layout from its own chunk;
   // a shorter chunk just leaves the tail of the allocation unused)
   const int tiles = (chunk_max + kTilePts - 1) / kTilePts;
@@ -946,7 +929,6 @@ int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* 
     else { LMOT_CUDA(c, cudaEventRecord(g.done, st)); g.record_pending = false; g.recorded = true; }
     g.last = st; g.have_last = true;
   }
-  c->last_ground_ctas = G * F;
   kernel_mark(c, slots[0], st);
   return LMOT_OK;
 }

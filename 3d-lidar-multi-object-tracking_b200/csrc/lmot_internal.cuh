@@ -65,7 +65,6 @@ struct TrackerHost {
 };
 
 constexpr int kMaxKernelEvents = 20;
-constexpr int kTraceRows = 1024;      // diagnostic ring of per-frame tracker kernel spans (8 words each), then 32 phase stamps
 
 // Result block: where one frame's results land.  Pinned, device-mapped host memory written by the kernels themselves
 // (box compaction, spawn_output_kernel) -- the stores ARE the D2H transfer; the host waits on ev_done and reads.
@@ -165,7 +164,6 @@ struct Slot {
 enum HostHdr { HDR_N_ELEV = 0, HDR_N_GROUND, HDR_NUM_CLUSTER, HDR_N_BOXES, HDR_N_TRACKS, HDR_N_VIS, HDR_ERROR, HDR_WARN, HDR_N_ACT, HDR_COUNT = 16 };
 
 constexpr int kMaxSlots = 8;
-constexpr int kFitClockCtas = 4096;                  // rows of the box-fitting phase clock (diagnostic)
 constexpr int kBatchBanks = 2;                       // batched ticks: detection of tick t+1 overlaps the tracker of tick t
 constexpr int kMaxResults = 64;
 
@@ -181,14 +179,7 @@ struct Ctx {
   int max_points = 0, max_sort_tiles = 0, fit_ctas = 0, n_mt_raw = 0;   // fit_ctas / trk_ctas: from the SM count (lmot_create)
   bool coop_launch = false;            // LMOT_COOP=1: cudaLaunchCooperativeKernel for the ground kernel (A/B diagnostics)
   int fused_max_ctas = 0;              // co-residency limit of the cooperative ground kernel on this device
-  unsigned long long* d_trk_trace = nullptr;     // diagnostic: [kTraceRows][8] per-frame kernel spans of the tracker chain + 32 phase stamps (same switch)
-  unsigned long long trk_frames = 0;
-  unsigned long long* d_phase_clock = nullptr;   // diagnostic: [CTAs][8] %globaltimer stamps of the last ground launch (lmot_debug_phase_clock)
-  int last_ground_ctas = 0;
-  unsigned long long* d_fit_clock = nullptr;     // diagnostic: [CTAs][8] stamps of the last box_fit_kernel launch (same switch)
-  int last_fit_ctas = 0;
-  bool fuse_ccl = true;                // frame / batch path: clustering runs in the ground kernel's tail (LMOT_FUSE_CCL=0: separate launch, A/B + phase stamps)
-  unsigned long long* d_ccl_clock = nullptr;     // diagnostic: [frames][16] %globaltimer stamps of the last ccl_bitmap_kernel launch (same switch)
+  bool fuse_ccl = true;                // frame / batch path: clustering runs in the ground kernel's tail (LMOT_FUSE_CCL=0: separate launch, A/B)
   bool zero_copy = false;              // lmot_frame_submit: pinned host frames are read by the ground kernel directly (LMOT_ZERO_COPY=1; off: slower than the copy engine)
   bool ground_half_sms = true;         // frame pipeline: ground kernel on half of the SMs (ground.cu ground_launch; LMOT_GROUND_HALF=0 disables, A/B only)
   unsigned spin_limit = 1u << 24;      // polls after which a device-side wait traps instead of hanging the GPU (LMOT_SPIN_LIMIT, 0 = wait for ever)

@@ -52,14 +52,6 @@ constexpr double bbYawChangeThres = 0.2;                // :46
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// diagnostic (scripts/diag_timeline.py): first start / last end of a kernel's CTAs by %globaltimer; trace == nullptr in production
-__device__ __forceinline__ void trace_start(unsigned long long* trace, int k) {
-  if (trace && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); atomicMax(&trace[2 * k], ~t); }   // max of ~t == ~(earliest start): every entry rests at 0
-}
-__device__ __forceinline__ void trace_end(unsigned long long* trace, int k) {
-  if (trace && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); atomicMax(&trace[2 * k + 1], t); }
-}
-
 __device__ __forceinline__ double wrap_pi(double a) {   // the reference's while loops; NaN falls through
   // (beyond 1e4 rad the reference's loop would need thousands of iterations -- millions for a diverged filter --
   //  so the bulk is removed in one step there; such a track is already past any parity claim)
@@ -174,8 +166,7 @@ __device__ void ukf_initialize(TrackState& t, double zx, double zy) {   // UKF::
 // still outside this stream: a ground kernel that needs every one of its CTAs co-resident could starve), then waits for the
 // previous tracker step.  TA's own griddepcontrol.wait returns when this kernel has completed, i.e. when both (a) and (b) hold.
 __global__ void __launch_bounds__(32)
-tracker_gate_kernel(const int* __restrict__ det_sem, unsigned long long* __restrict__ phase, unsigned spin_limit) {
-  if (phase && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); phase[26] = t; }
+tracker_gate_kernel(const int* __restrict__ det_sem, unsigned spin_limit) {
   if (threadIdx.x == 0) {
     unsigned spin = 0;
     int v;
@@ -189,7 +180,6 @@ tracker_gate_kernel(const int* __restrict__ det_sem, unsigned long long* __restr
   // (no griddepcontrol.wait: this kernel may finish before the previous frame's spawn_output_kernel does.  TA's CTAs, resident from
   // here on, wait for that step through its completion counter -- one L2 poll after spawn_output_kernel's last store instead of two
   // grid-completion hops (TC -> this kernel -> TA).)
-  if (phase && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); phase[27] = t; }
 }
 
 // ------------------------------------------------------------------------------------------------ TA
@@ -214,11 +204,10 @@ __device__ __forceinline__ double bcast(double v, int src) { return __shfl_sync(
 __global__ void __launch_bounds__(kTAThreads, 4)     // <= 128 registers: a CTA (16 K registers) fits on an SM next to a ground-kernel CTA (47 K)
 imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
                         double dt, unsigned* __restrict__ gate, unsigned* __restrict__ setter, int* __restrict__ first_setter,
-                        uint8_t* __restrict__ skip, int words, const int* __restrict__ act_list, unsigned long long* trace,
-                        unsigned long long* __restrict__ phase, int* __restrict__ meas_n, double2* __restrict__ meas_ctr,
+                        uint8_t* __restrict__ skip, int words, const int* __restrict__ act_list,
+                        int* __restrict__ meas_n, double2* __restrict__ meas_ctr,
                         const unsigned* __restrict__ tc_seq, unsigned tc_want, unsigned spin_limit) {
   __shared__ TAShared sh;
-  if (phase && blockIdx.x == 0 && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); phase[28] = t; }
   pdl_wait();                              // (gated launch: the gate kernel, hence this frame's detection, is complete)
   pdl_launch_dependents();                 // TB's CTAs may line up behind this grid
   // the previous tracker step: spawn_output_kernel counts itself complete (release) after its last store.  It is ONE resident CTA
@@ -231,15 +220,9 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
     } while ((int)(v - tc_want) < 0);
   }
   __syncthreads();
-  trace_start(trace, 0);
-  struct TraceEnd { unsigned long long* t; __device__ ~TraceEnd() { __syncthreads(); trace_end(t, 0); } } trace_at_exit{trace};
   const int tid = threadIdx.x, lane = tid & 31, model = tid >> 5;
   const int n_act = trk[CNT_N_ACT];
   const int M = det[CNT_N_BOXES];
-  if (trace && tid == 0 && (int)blockIdx.x < n_act) { unsigned long long tn; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tn)); atomicMax(&trace[6], tn); }   // latest start of a CTA that has a track
-  // diagnostic: %globaltimer stamps of CTA 0 (thread 0 = lane 0 of the CV model's warp)
-  auto mark = [&](int i) { if (phase && blockIdx.x == 0 && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); phase[32 + i] = t; } };
-  mark(0);
   const double kStdA = (model == 2) ? 3.0 : 2.0;       // std_a_{cv,ctrv,rm}_ ukf.cpp:68-70 (= std_*_yawdd_ :71-73)
   const double lambda_aug = 3 - 7;
   const double w0 = lambda_aug / (lambda_aug + 7), wi = 0.5 / (7 + lambda_aug);
@@ -262,7 +245,6 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
     for (int e = tid; e < 75; e += kTAThreads) sh.Pp[e / 25][e % 25] = t.P[1 + e / 25][e % 25];
     const double mp0 = t.modeProb[0], mp1 = t.modeProb[1], mp2 = t.modeProb[2];
     __syncthreads();
-    mark(1);
     if (sh.flag) continue;
     // guard :828-831 on the side: the serial 5x5 LU no longer sits in front of the prediction
     if (tid == 96) sh.explode = (det_lu<5>(t.P[0]) > 10 || t.P[0][24] > 1000) ? 1 : 0;
@@ -288,7 +270,6 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
       sh.Pm[model][lane] = t0 + t1 + t2;
     }
     __syncwarp();
-    mark(2);
     // ---- Prediction (:630-772): P_aug.llt() with Eigen's early exit on a non-positive pivot (LLT.h:271-295)
     if (lane == 0) {
       // 5x5 block in registers, fully unrolled (packed lower triangle); the two augmentation rows are diagonal
@@ -333,7 +314,6 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
       L[6 * 7 + 6] = stop ? s2 : sqrt(s2);
     }
     __syncwarp();
-    mark(3);
     if (lane < 15) {      // one sigma point per lane (:682-735)
       const double sq = sqrt(lambda_aug + 7);
       double a[7];
@@ -377,7 +357,6 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
       o[0] = s0; o[1] = s1; o[2] = s2; o[3] = s3; o[4] = s4;
     }
     __syncwarp();
-    mark(4);
     // predicted mean (:737-744), every lane sums in sigma-point order
 #pragma unroll
     for (int e = 0; e < 5; ++e) {
@@ -402,7 +381,6 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
         Pe = Pe + (((i == 0) ? w0 : wi) * dr) * dc;
       }
     }
-    mark(5);
     // ---- UpdateLidar (:778-902)
 #pragma unroll
     for (int i = 0; i < 15; ++i) { const double w = (i == 0) ? w0 : wi; zp0 = zp0 + w * sh.Xs[model][i][0]; zp1 = zp1 + w * sh.Xs[model][i][1]; }
@@ -431,7 +409,6 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
     inv2_lu(sh.S[model], Si);
     if (lane == 0) sh.detS[model] = det2(sh.S[model]);     // for findMaxZandS below: each warp its own model, not every warp all three
     }   // model < 3
-    mark(6);
     __syncthreads();                      // the guard's verdict is in
     if (sh.explode) {
       if (tid == 0) { t.trackNum = 0; skip[it] = 1; }
@@ -465,7 +442,6 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
       if (tid == 0) { t.trackNum = 0; skip[it] = 1; }
       continue;
     }
-    mark(7);
     const double z0 = sh.zp[mm][0], z1 = sh.zp[mm][1];
     inv2_lu(S4, Si);
     const bool secondInit = (trackNum == 1);
@@ -519,7 +495,6 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
         }
         if (tid == 0) meas_n[it] = total;
       } else if (tid == 0) meas_n[it] = -1;
-      mark(8);
     } else if (model == 0) {
       // secondInit (:238-246): every running minimum of the NIS marks its box; chunks in order with a carried minimum
       if (lane == 0) meas_n[it] = -1;
@@ -665,21 +640,15 @@ struct TBShared {
 __global__ void __launch_bounds__(kTBThreads)
 imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
                   const unsigned* __restrict__ gate, const int* __restrict__ first_setter, const uint8_t* __restrict__ skip,
-                  int words, const int* __restrict__ act_list, ActSummary* __restrict__ summary, unsigned long long* trace,
-                  unsigned long long* __restrict__ phase, const int* __restrict__ meas_n, const double2* __restrict__ meas_ctr) {
+                  int words, const int* __restrict__ act_list, ActSummary* __restrict__ summary,
+                  const int* __restrict__ meas_n, const double2* __restrict__ meas_ctr) {
   extern __shared__ unsigned short s_list[];              // indices of the gated boxes, in box order
   __shared__ TBShared sh;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   pdl_wait();                              // TA has finished (gate rows, first_setter, predicted states are visible)
   pdl_launch_dependents();                 // TC's CTA may line up behind this grid
-  // diagnostic: %globaltimer stamps of the first track's CTA
-  auto mark = [&](int i) { if (phase && blockIdx.x == 0 && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); phase[16 + i] = t; } };
-  mark(0);
-  trace_start(trace, 1);
-  struct TraceEnd { unsigned long long* t; __device__ ~TraceEnd() { __syncthreads(); trace_end(t, 1); } } trace_at_exit{trace};
   const int n_act = trk[CNT_N_ACT];
   const int M = det[CNT_N_BOXES];
-  if (trace && tid == 0 && (int)blockIdx.x < n_act) { unsigned long long tn; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tn)); atomicMax(&trace[7], tn); }
   const int nchunk = (M + 31) >> 5;
   TrackState& t = sh.trk;
 
@@ -704,7 +673,6 @@ imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, 
       for (int u = 0; u < kIt; ++u) { const int w = tid + kTBThreads * u; if (w < kTrackWords) dst[w] = v[u]; }
     }
     __syncthreads();
-    mark(1);
     bool pda = false;                        // CTA-uniform: the track reaches filterPDA
     int nmeas = 0, mm = 0;
     double numMeas = 0;
@@ -734,7 +702,6 @@ imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, 
         }
       }
       __syncwarp();
-      mark(2);
       const int lifetime = t.lifetime + life;
 
       // measurement prediction used by the gate (same selection as TA)
@@ -900,7 +867,6 @@ imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, 
       }
     }
     __syncthreads();
-    mark(3);
     if (!skipped && warp == 0) {
       if (pda) {
         const double Vk = kPi * sqrt(gammaG * det2(t.S[mm]));     // S is untouched by the update, same max model
@@ -919,7 +885,6 @@ imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, 
           else lv = (1 - pG * pD) / powN;
           lam[0] = __shfl_sync(0xFFFFFFFFu, lv, 0); lam[1] = __shfl_sync(0xFFFFFFFFu, lv, 1); lam[2] = __shfl_sync(0xFFFFFFFFu, lv, 2);
         }
-        mark(4);
         // ---- PostProcessIMMUKF: UpdateModeProb (ukf.cpp:384-397), MergeEstimationAndCovariance (:419-437)
         double mp[3] = {t.modeProb[0], t.modeProb[1], t.modeProb[2]};
         const double sumG = lam[0] * mp[0] + lam[1] * mp[1] + lam[2] * mp[2];
@@ -969,7 +934,6 @@ imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, 
       if (lane == 0) { t.trackNum = sh.tn_out; t.lifetime = sh.life_out; }
     }
     __syncthreads();
-    mark(5);
     if (!skipped) {
       const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&sh.trk);
       unsigned long long* dst = reinterpret_cast<unsigned long long*>(&tracks[it]);
@@ -989,7 +953,6 @@ imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, 
       __syncwarp();
       if (lane < 16) reinterpret_cast<unsigned long long*>(&summary[q])[lane] = reinterpret_cast<const unsigned long long*>(&sh.sum)[lane];
     }
-    mark(6);
   }
 }
 
@@ -1162,11 +1125,8 @@ template <int NT>
 __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det,
                                         const float* __restrict__ boxes, const float* __restrict__ boxes_pub, int* __restrict__ first_setter, double ego_yaw, int max_tracks,
                                         const OutPtrs& o, const OutPtrs& prev, int* __restrict__ act_list, double4* __restrict__ pos,
-                                        const ActSummary* __restrict__ summary, int T0, int n_act0, int M, unsigned long long* __restrict__ trace,
-                                        unsigned long long* __restrict__ phase) {
+                                        const ActSummary* __restrict__ summary, int T0, int n_act0, int M) {
   const int tid = threadIdx.x, lane = tid & 31;
-  auto mark = [&](int i) { if (phase && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); phase[i] = t; } };
-  mark(0);
   const bool have = tid < n_act0;
   // ---- one round trip: the summaries, the previous result block, the spawn inputs
   ActSummary r;
@@ -1239,7 +1199,6 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
       if (e < T0) { if (cp) o.vandyaw[2 * e] = qv[u]; o.vandyaw[2 * e + 1] = wrap_pi(qz[u] + ego_yaw); }
     }
   }
-  mark(1);
   const int vis = (have && r.isVis) ? 1 : 0;
   float2 vb[12];                                     // the visible track's whole box (8 x 3 floats) for the output list
   if (vis) {
@@ -1267,7 +1226,6 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
   }
   __syncthreads();
 
-  mark(2);
   // ---- mergeOverSegmentation, pass A: imax = largest visible box index containing this (live) track
   // (track x box) pairs spread over the whole CTA: a warp takes every 8th box (broadcast loads); its lanes hold the tracks
   // jt = lane, lane + 32, ... in REGISTERS for the whole loop, so an iteration is two independent shared-memory loads and
@@ -1301,7 +1259,6 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
   }
   int imax = -1;
   __syncthreads();
-  mark(3);
   {
     const int ncand = min(S.ncand, kCandCap);
     for (int e = tid; e < ncand; e += NT) {      // the exact fp64 tests, one pair per thread
@@ -1310,7 +1267,6 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
     }
   }
   __syncthreads();
-  mark(4);
   imax = max(imax, S.imax[tid]);
   // ---- pass B: has5 for the rare visible box that sits inside another one, against EVERY track (dead ones included)
   if (vis && imax >= 0 && r.trackNum != 0) S.cont[atomicAdd(&S.ncont, 1)] = (unsigned short)vslot;
@@ -1330,7 +1286,6 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
     }
     if (ncont > 0) __syncthreads();
   }
-  mark(5);
   int trackNum = r.trackNum;
   if (have && trackNum != 0 && nv > 0) {
     const bool has5 = vis && S.h5[vslot] != 0;
@@ -1353,13 +1308,11 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
 #pragma unroll
     for (int e = 0; e < 12; ++e) dst[e] = vb[e];
   }
-  mark(6);
   int aex, atot;
   block_offsets(0, act, S.w, aex, atot);
   const int n_keep = atot >> 16;
   if (act) act_list[aex >> 16] = r.k;
 
-  mark(7);
   // ---- spawn one UKF per unmatched box, in box order (:972-989); the spawning thread also emits the new track
   for (int b0 = 0; b0 < M; b0 += NT) {
     const int b = b0 + tid;
@@ -1382,7 +1335,6 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
     if (tid == 0) S.carry += tot;
     __syncthreads();
   }
-  mark(8);
   int T = T0 + S.carry;
   if (T > max_tracks) T = max_tracks;
   if (tid == 0) {
@@ -1392,8 +1344,6 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
     o.hdr[HDR_WARN] = (T0 + S.carry > max_tracks) ? (int)LMOT_WARN_TRACK_TABLE_FULL : 0;   // existing tracks' outputs stay valid: a warning, not an error
     o.hdr[HDR_N_ACT] = n_keep + (T - T0);
     det[CNT_ERROR] = 0;
-    trace_end(trace, 2);
-    mark(9);
   }
 }
 
@@ -1412,20 +1362,18 @@ spawn_output_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int*
                     const float* __restrict__ boxes_pub, int* __restrict__ first_setter, int* __restrict__ imax_arr, int* __restrict__ vis_list,
                     uint8_t* __restrict__ has5_arr, int first_frame, int compat_first, double ego_yaw, int max_tracks, OutPtrs o,
                     OutPtrs prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
-                    unsigned long long* __restrict__ trace, unsigned long long* __restrict__ phase, int* __restrict__ det_sem,
-                    unsigned* __restrict__ tc_seq) {
+                    int* __restrict__ det_sem, unsigned* __restrict__ tc_seq) {
   pdl_launch_dependents();                 // the next frame's gate kernel may become resident
   pdl_wait();                              // TB has finished
   // every exit: this step's results are complete -> count it (release); publish_kernel, on its own stream, polls the count
   // instead of waiting for a stream event, so that nothing but kernels sits on the tracker stream
   struct Done { unsigned* p; __device__ ~Done() { __syncthreads(); if (threadIdx.x == 0) { __threadfence(); atomicAdd(p, 1u); } } } done_at_exit{tc_seq};
-  trace_start(trace, 2);
   if (det_sem && threadIdx.x == 0) atomicSub(det_sem, 1);     // this frame's detection results are being consumed (posted by box_fit_kernel)
   if (!full && !(first_frame && compat_first) && trk[CNT_N_ACT] <= NT) {
     extern __shared__ __align__(16) unsigned char tc_dyn[];          // sizeof(TCFastShared<NT>), tracker_launch
     TCFastShared<NT>& s_fast = *reinterpret_cast<TCFastShared<NT>*>(tc_dyn);
     const int M = det[CNT_N_BOXES];
-    tc_fast<NT>(s_fast, tracks, trk, det, boxes, boxes_pub, first_setter, ego_yaw, max_tracks, o, prev, act_list, pos, summary, trk[CNT_N_TRACKS], trk[CNT_N_ACT], M, trace, phase);
+    tc_fast<NT>(s_fast, tracks, trk, det, boxes, boxes_pub, first_setter, ego_yaw, max_tracks, o, prev, act_list, pos, summary, trk[CNT_N_TRACKS], trk[CNT_N_ACT], M);
     return;
   }
   __shared__ int s_w[33];
@@ -1650,7 +1598,6 @@ spawn_output_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int*
     o.hdr[HDR_WARN] = table_full ? (int)LMOT_WARN_TRACK_TABLE_FULL : 0;
     o.hdr[HDR_N_ACT] = s_carry2;
     det[CNT_ERROR] = 0;
-    trace_end(trace, 2);
   }
 }
 
@@ -1854,15 +1801,6 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
   int* det = const_cast<int*>(det_counters);
   const int first = h.init ? 0 : 1;
   const int compat = c->prm.oracle_compat_first_frame ? 1 : 0;
-  unsigned long long* trace = nullptr;     // diagnostic: [32 frames][8] first start / last end of TA, TB, TC
-  if (c->d_trk_trace) {
-    // rows are zeroed kTraceRows frames at a time: a memset in front of every step would sit between two programmatically
-    // dependent launches of the chain and serialise them
-    if (c->trk_frames % kTraceRows == 0) LMOT_CUDA(c, cudaMemsetAsync(c->d_trk_trace, 0, (size_t)kTraceRows * 8 * sizeof(unsigned long long), st));
-    trace = c->d_trk_trace + (size_t)(c->trk_frames % kTraceRows) * 8;
-  }
-  unsigned long long* phase = c->d_trk_trace ? c->d_trk_trace + (size_t)kTraceRows * 8 : nullptr;
-  ++c->trk_frames;
   // `gate` (frame submissions): the detection stages of this frame post sl->d_det_sem.  Either the gate kernel waits for it on
   // the device (see tracker_gate_kernel), or -- timing mode, the reference's first-frame quirk -- the stream waits for the event.
   const bool use_gate = gate && !c->timing && !(first && compat);
@@ -1888,12 +1826,12 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
       if (use_gate) {
         cudaLaunchConfig_t gc = {};
         gc.gridDim = dim3(1); gc.blockDim = dim3(32); gc.dynamicSmemBytes = 0; gc.stream = st; gc.attrs = &pa; gc.numAttrs = 1;
-        LMOT_CUDA(c, cudaLaunchKernelEx(&gc, tracker_gate_kernel, (const int*)det_sem, phase, c->spin_limit));
+        LMOT_CUDA(c, cudaLaunchKernelEx(&gc, tracker_gate_kernel, (const int*)det_sem, c->spin_limit));
       }
       cudaLaunchConfig_t ac = {};
       ac.gridDim = dim3(c->trk_ctas); ac.blockDim = dim3(kTAThreads); ac.dynamicSmemBytes = 0; ac.stream = st; ac.attrs = &pa; ac.numAttrs = 1;
       LMOT_CUDA(c, cudaLaunchKernelEx(&ac, imm_predict_gate_kernel, c->d_tracks, (const int*)c->d_trk_counters, (const int*)det, d_boxes, dt,
-                                      c->d_gate, c->d_setter, c->d_first_setter, c->d_skip, c->gate_words, (const int*)c->d_act_list, trace, phase,
+                                      c->d_gate, c->d_setter, c->d_first_setter, c->d_skip, c->gate_words, (const int*)c->d_act_list,
                                       c->d_meas_n, reinterpret_cast<double2*>(c->d_meas_ctr), (const unsigned*)c->d_tc_seq, c->tc_launched, c->spin_limit));
     }
     kernel_mark(c, sl, st);
@@ -1907,7 +1845,7 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
     cfg.attrs = &pdl; cfg.numAttrs = 1;
     LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_kernel, c->d_tracks, (const int*)c->d_trk_counters, (const int*)det, d_boxes,
                                     (const unsigned*)c->d_gate, (const int*)c->d_first_setter, (const uint8_t*)c->d_skip, c->gate_words,
-                                    (const int*)c->d_act_list, reinterpret_cast<ActSummary*>(c->d_summary), trace, phase,
+                                    (const int*)c->d_act_list, reinterpret_cast<ActSummary*>(c->d_summary),
                                     (const int*)c->d_meas_n, reinterpret_cast<const double2*>(c->d_meas_ctr)));
     kernel_mark(c, sl, st);
   }
@@ -1927,7 +1865,7 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
     cfg.attrs = &pdl; cfg.numAttrs = 1;
     LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_kernel<kTCWide> : spawn_output_kernel<kTCThreads>, c->d_tracks, c->d_trk_counters, det, d_boxes, d_boxes_pub, c->d_first_setter, c->d_new_num,
                                     c->d_vis_list, c->d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->d_act_list,
-                                    c->d_pos, reinterpret_cast<const ActSummary*>(c->d_summary), trace, phase, det_sem, c->d_tc_seq));
+                                    c->d_pos, reinterpret_cast<const ActSummary*>(c->d_summary), det_sem, c->d_tc_seq));
     ++c->tc_launched;
   }
   kernel_mark(c, sl, st);

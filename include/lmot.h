@@ -298,22 +298,6 @@ int lmot_debug_cell_index(lmot_ctx* ctx, int32_t* ch, int32_t* bin, int n);
 /* label grid and per-elevated-point cluster id of the last clustering / box fitting */
 int lmot_debug_label_grid(lmot_ctx* ctx, int32_t* grid, int* num_cluster);
 
-/* diagnostic (after lmot_enable_timing): completion times in ms, relative to the start of the oldest frame still in the result
- * ring, of the stage boundaries [0..4] and of every kernel [5..] of each of those frames -- pipelined submissions included */
-int lmot_debug_timeline(lmot_ctx* ctx, float* out, int cap_frames, int* n_frames, int* row_stride);
-
-/* diagnostic (after the phase clock was switched on): %globaltimer spans of the tracker kernels of the last 32 tracker steps,
- * out[32][8], followed by 64 phase stamps of the last launches of the chain's kernels: out must hold 320 words */
-int lmot_debug_tracker_trace(lmot_ctx* ctx, unsigned long long* out, int* next);
-
-/* diagnostic: first call switches on the phase clock of ground_fused_kernel; later calls return the %globaltimer stamps
- * (ns) thread 0 of every CTA took at its 8 phase boundaries during the last launch: out[n_ctas][8] */
-int lmot_debug_phase_clock(lmot_ctx* ctx, unsigned long long* out, int cap_ctas, int* n_ctas);
-
-/* diagnostic (phase clock on): %globaltimer stamps of the last ccl_bitmap_kernel (which = 1, rows = frames, 16 words each) or
- * box_fit_kernel launch (which = 2, rows = CTAs, 8 words each) */
-int lmot_debug_stage_clocks(lmot_ctx* ctx, int which, unsigned long long* out, int cap_rows, int* n_rows, int* row_words);
-
 /* host-side self test of the bit-exact atan2f restatement against the host libm (no GPU needed) */
 int lmot_selftest_atan2f(const float* y, const float* x, int n, float* out);
 

@@ -1,80 +1,72 @@
-"""Diagnostic: GPU timeline of the pipelined frames (completion time of every kernel of the last frames), device-resident input."""
-import importlib, os, sys
-os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
-import numpy as np
-import torch
+"""Diagnostic: the tracker chain of the frame pipeline, from a torch.profiler trace.
+
+K pipelined lmot_frame_dev steps in production mode (timing events off, frames resident on the device) are traced with CUDA
+activities only: every kernel's start and end, nothing added to the streams.  The trace goes to measure_out/<tag>.pt.trace.json.
+Printed, as the mean over the K steps in us: TA = imm_predict_gate_kernel, TB = imm_update_kernel, TC = spawn_output_kernel, the
+gaps between them (negative: the programmatic dependent's CTAs were resident before its predecessor ended), TA start to the next
+TA start (the chain's period, which bounds frames/s), and detection start (ground_fused_kernel) to box_fit_kernel end.  Then the
+same loop runs without the profiler, timed with CUDA events: tracing lengthens every step, so the trace gives the chain's shape
+and this last line its production length.
+
+    python scripts/diag_timeline.py [tag]        # DIAG_K = steps (default 200)
+"""
+import importlib, json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-lmot = importlib.import_module("3d-lidar-multi-object-tracking_b200")
-synth = importlib.import_module("3d-lidar-multi-object-tracking_b200.synth")
-import bench
-K, W = int(os.environ.get("DIAG_K", "120")), 20
+import bench                     # (sets CUDA_DEVICE_MAX_CONNECTIONS before CUDA initialises)
+import numpy as np
+import torch
+from torch.profiler import ProfilerActivity, profile
+
+if not torch.cuda.is_available():
+    raise SystemExit("diag_timeline.py: no CUDA device -- the timeline is measured on the GPU only")
+lmot = importlib.import_module(bench.PKG)
+synth = importlib.import_module(bench.PKG + ".synth")
+tag = sys.argv[1] if len(sys.argv) > 1 else "timeline"
+K, W = int(os.environ.get("DIAG_K", "200")), 20
 ts, frames = bench.make_frames(synth, W + K)
 n = frames.shape[1]
 d = torch.from_numpy(frames).cuda()
-torch.cuda.synchronize()
-BRIEF = os.environ.get("DIAG_BRIEF", "0") == "1"
-for depth in [int(x) for x in os.environ.get("DIAG_DEPTHS", "1,4").split(",")]:
-    prm = lmot.default_params(); prm.pipeline_depth = depth
-    ctx = lmot.Lmot(prm)
-    st = torch.cuda.Stream(); torch.cuda.set_stream(st); ctx.set_stream(st.cuda_stream)
-    ctx.tracker_reset(); ctx.enable_timing(True); ctx.debug_phase_clock()
-    for i in range(W + K): ctx.frame_dev(d[i].data_ptr(), n, ts[i])
-    ctx.sync()
-    tl = ctx.debug_timeline() * 1e3          # us
-    names = ["start", "ground", "cluster", "box", "tracker"] + list(bench.KERNEL_NAMES)
-    print(f"--- pipeline_depth {depth}: {len(tl)} frames; columns = completion time (us) relative to the oldest frame's start")
-    print("frame " + " ".join(f"{x[:9]:>9s}" for x in names))
-    for f, row in enumerate(tl[-14:] if not BRIEF else []):
-        print(f"{f:5d} " + " ".join(f"{v:9.1f}" for v in row[: len(names)]))
-    if len(tl) > 12:
-        per = (tl[-1, 4] - tl[-11, 4]) / 10
-        print(f"tracker completion to tracker completion: {per:.1f} us per frame")
-        ta = tl[-10:, 11] - tl[-11:-1, 4]; tb = tl[-10:, 12] - tl[-10:, 11]; tc = tl[-10:, 13] - tl[-10:, 12]; tail = tl[-10:, 4] - tl[-10:, 13]
-        print(f"  mean over the last 10 frames: prev tracker done -> TA done {ta.mean():.1f}, TA -> TB {tb.mean():.1f}, TB -> TC {tc.mean():.1f}, TC -> stage event {tail.mean():.1f} us")
-        det = tl[-10:, 10] - tl[-10:, 0]
-        print(f"  detection start -> box_fit done {det.mean():.1f} us; box_fit done -> TA done {(tl[-10:, 11] - tl[-10:, 10]).mean():.1f} us")
-    tr = ctx.debug_phase_clock()
-    if len(tr): print(f"last frame: ground kernel span {(tr[:, 7].max() - tr[:, 0].min()) / 1e3:.2f} us (CTA stamps)")
-    ctx.enable_timing(False)
-    # the same loop without timing events: frames/s as bench.py measures `value`
-    ctx.tracker_reset()
-    HOST = os.environ.get("DIAG_HOST", "0") == "1"
-    if HOST:
-        h_pin = torch.from_numpy(frames).pin_memory(); h_np = h_pin.numpy()
-        for i in range(W): ctx.frame(h_np[i], ts[i])
-    else:
-        for i in range(W): ctx.frame_dev(d[i].data_ptr(), n, ts[i])
-    torch.cuda.synchronize(); ctx.sync()
-    import time
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0 = time.perf_counter(); e0.record(st)
-    if HOST:      # the e2e path: pinned HOST frames through frame_submit / frame_collect
-        infl = 0
-        for i in range(W, W + K):
-            if infl == 31: ctx.frame_collect(); infl -= 1
-            ctx.frame_submit(h_np[i], ts[i]); infl += 1
-        while infl: ctx.frame_collect(); infl -= 1
-    else:
-        for i in range(W, W + K): ctx.frame_dev(d[i].data_ptr(), n, ts[i])
-    th = time.perf_counter() - t0
-    ctx.flush(); e1.record(st); torch.cuda.synchronize()
-    hn = ctx.debug_host_ns()
-    tt = ctx.debug_tracker_trace().astype(np.int64)[-12:]
-    ph = ctx.last_tc_phases.astype(np.int64); ph = ph[ph > 0]
-    pb = ctx.last_tb_phases.astype(np.int64); pb = pb[pb > 0]
-    gp = ctx.last_gate_phases.astype(np.int64)
-    full = ctx.debug_tracker_trace().astype(np.int64)
-    if gp[0] > 0: print(f"  last step: gate entry {(gp[0] - full[-2, 5]) / 1e3:.2f} us after the PREVIOUS step's TC end, gate released {(gp[1] - full[-2, 5]) / 1e3:.2f}, TA CTA 0 entry {(gp[2] - full[-2, 5]) / 1e3:.2f}, TA start {(full[-1, 0] - full[-2, 5]) / 1e3:.2f}; previous TC start {(full[-2, 4] - full[-2, 5]) / 1e3:.2f}, previous TB start {(full[-2, 2] - full[-2, 5]) / 1e3:.2f}")
-    pa = ctx.last_ta_phases.astype(np.int64); pa = pa[pa > 0]
-    if len(pa) > 1: print("  TA phases of CTA 0 (us after its start: staged, mixed, Cholesky, sigma points, mean+cov, S/Tc/S^-1, written back, gated):", " ".join(f"{(x - pa[0]) / 1e3:.2f}" for x in pa[1:]))
-    if len(pb) > 1: print("  TB phases of CTA 0 (us after its start: staged, gate list, model warps + box warp done, lambda, merged, written back):", " ".join(f"{(x - pb[0]) / 1e3:.2f}" for x in pb[1:]))
-    if len(ph) > 1: print("  TC phases (us after its start: loads issued, summaries in, boxes staged, pass A, exact tests, pass B, emit, act list, spawn, end):", " ".join(f"{(x - ph[0]) / 1e3:.2f}" for x in ph[1:]))
-    ta, tb, tc = (tt[:, 1] - tt[:, 0]) / 1e3, (tt[:, 3] - tt[:, 2]) / 1e3, (tt[:, 5] - tt[:, 4]) / 1e3
-    g1, g2, g3 = (tt[:, 2] - tt[:, 1]) / 1e3, (tt[:, 4] - tt[:, 3]) / 1e3, (tt[1:, 0] - tt[:-1, 5]) / 1e3
-    la, lb = (tt[:, 6] - tt[:, 0]) / 1e3, (tt[:, 7] - tt[:, 2]) / 1e3
-    print(f"  tracker chain by %globaltimer, no events in the streams (mean of the last 12 steps, us): TA {ta.mean():.1f} | gap {g1.mean():.1f} | "
-          f"TB {tb.mean():.1f} | gap {g2.mean():.1f} | TC {tc.mean():.1f} | gap to the next frame's TA {g3.mean():.1f}  "
-          f"(TA start to next TA start {((tt[1:, 0] - tt[:-1, 0]) / 1e3).mean():.1f}); last working CTA starts {la.mean():.1f} after TA's first, {lb.mean():.1f} after TB's first")
-    print(f"  no timing events: {K / (e0.elapsed_time(e1) * 1e-3):.0f} frames/s ({1e3 * e0.elapsed_time(e1) / K:.1f} us/frame); python loop {1e6 * th / K:.1f} us/frame, inside the library {hn[0] / 1e3 / (W + K):.1f} us/frame")
-    ctx.close()
+ctx = lmot.Lmot(lmot.default_params())
+st = torch.cuda.Stream(); torch.cuda.set_stream(st); ctx.set_stream(st.cuda_stream)
+clock = bench.ClockSampler(torch.cuda.current_device()); clock.start()
+
+
+def steps(lo, hi):
+    for i in range(lo, hi):
+        ctx.frame_dev(d[i].data_ptr(), n, ts[i])
+    ctx.flush()
+
+
+def warm_up():
+    ctx.tracker_reset(); steps(0, W); torch.cuda.synchronize()
+
+
+warm_up()
+with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    steps(W, W + K); torch.cuda.synchronize()
+os.makedirs(os.path.join(ROOT, "measure_out"), exist_ok=True)
+path = os.path.join(ROOT, "measure_out", f"{tag}.pt.trace.json")
+prof.export_chrome_trace(path)
+kern = [e for e in json.load(open(path))["traceEvents"] if e.get("cat") == "kernel"]
+span = {k: np.array(sorted((e["ts"], e["ts"] + e["dur"]) for e in kern if k in e["name"])).reshape(-1, 2)
+        for k in ("ground_fused_kernel", "box_fit_kernel", "imm_predict_gate_kernel", "imm_update_kernel", "spawn_output_kernel")}
+if any(len(v) != K for v in span.values()):
+    raise SystemExit(f"diag_timeline.py: expected {K} launches of each kernel in {path}, found {({k: len(v) for k, v in span.items()})}")
+ta, tb, tc = span["imm_predict_gate_kernel"], span["imm_update_kernel"], span["spawn_output_kernel"]
+det, fit = span["ground_fused_kernel"], span["box_fit_kernel"]
+
+warm_up()
+e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+e0.record(st); steps(W, W + K); e1.record(st); torch.cuda.synchronize()
+ms = e0.elapsed_time(e1)
+clk = clock.stop()
+ctx.close()
+
+m = lambda x: f"{np.mean(x):.1f}"
+print(f"{torch.cuda.get_device_name()}, power limit {clk['power_limit_w']} W, median SM clock {clk['sm_mhz']} MHz; "
+      f"{K} pipelined steps, pipeline_depth {lmot.default_params().pipeline_depth}, trace {os.path.relpath(path, ROOT)}")
+print(f"tracker chain per step, mean (us): TA {m(ta[:, 1] - ta[:, 0])} | gap {m(tb[:, 0] - ta[:, 1])} | TB {m(tb[:, 1] - tb[:, 0])} | "
+      f"gap {m(tc[:, 0] - tb[:, 1])} | TC {m(tc[:, 1] - tc[:, 0])} | gap to the next TA {m(ta[1:, 0] - tc[:-1, 1])}")
+print(f"  TA start to next TA start {m(np.diff(ta[:, 0]))} us; detection start -> box_fit_kernel end {m(fit[:, 1] - det[:, 0])} us")
+print(f"no profiler: {K / (ms * 1e-3):.0f} frames/s ({1e3 * ms / K:.1f} us/frame), CUDA events around the {K} steps")
