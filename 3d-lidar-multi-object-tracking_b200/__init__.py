@@ -333,6 +333,12 @@ class Lmot:
         self._chk(self.lib.lmot_frame_fetch(self.h, C.byref(fo)))
         return self._frame_result(fo, bufs, want_boxes)
 
+    def track_step_lists_dev(self, d_lists: int, d_counts: int, n_lists: int, cap_per_list: int, timestamp_us, v_gps=0.0, yaw_gps=0.0):
+        """Asynchronous: n_lists padded device box lists (cap_per_list boxes each, lengths in the device ints at d_counts) as one
+        tracker step; results with frame_fetch()."""
+        self._chk(self.lib.lmot_track_step_lists_dev(self.h, C.c_void_p(d_lists), C.c_void_p(d_counts), int(n_lists), int(cap_per_list),
+                                                     C.c_double(timestamp_us), C.c_double(v_gps), C.c_double(yaw_gps)))
+
     # ---- batched ticks: F sensor streams, one frame each, one shared track table (BASELINE.json configs[3]) --------
     def batch_prepare(self, dev_frames):
         """Marshal a tick's (device pointer, n) list ONCE: the returned handle can be passed to batch_dev / batch_detect_dev /
