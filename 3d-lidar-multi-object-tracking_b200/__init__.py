@@ -78,6 +78,11 @@ class BatchOut(C.Structure):
     ]
 
 
+class Sensor(C.Structure):
+    """lmot_sensor: where one sensor of a rig is mounted (pose = sensor -> vehicle frame, row-major 3x4 [R | t])."""
+    _fields_ = [("pose", C.c_float * 12), ("h_sensor", C.c_float), ("t_hmin", C.c_float), ("t_hmax", C.c_float), ("sensor_height", C.c_float)]
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -92,6 +97,7 @@ ABI_SYMBOLS = [
     "lmot_frame_dev", "lmot_frame_fetch", "lmot_frame_submit", "lmot_frame_collect", "lmot_frames_in_flight", "lmot_frame_ready", "lmot_flush",
     "lmot_ground_remove_dev", "lmot_detect_dev", "lmot_sync",
     "lmot_batch_submit", "lmot_batch_dev", "lmot_batch_detect_dev", "lmot_batch_collect", "lmot_batch_fetch", "lmot_batch", "lmot_batch_ground_ccl_dev",
+    "lmot_default_sensor", "lmot_set_sensors", "lmot_get_sensors",
     "lmot_detect_boxes_dev", "lmot_track_step_lists_dev", "lmot_tracker_counters_dev", "lmot_tracker_table_received",
     "lmot_origin_points", "lmot_tracker_table", "lmot_tracker_set_num_tracks", "lmot_tracker_reset", "lmot_tracker_num_tracks", "lmot_tracker_dump", "lmot_tracker_load", "lmot_tracker_get_ego", "lmot_tracker_set_ego",
     "lmot_debug_polar_grid", "lmot_debug_cell_index", "lmot_debug_label_grid", "lmot_selftest_atan2f",
@@ -412,6 +418,33 @@ class Lmot:
         bo, bufs = self._batch_out(cap or self.params.max_tracks, want_boxes)
         self._chk(self.lib.lmot_batch_fetch(self.h, C.byref(bo)))
         return self._batch_result(bo, bufs, want_boxes)
+
+    # ---- sensor rig: sensor k = frame k of a batched tick / list k of track_step_lists_dev (lmot_set_sensors) ----------------
+    def set_sensors(self, poses, h_sensor=None, t_hmin=None, t_hmax=None, sensor_height=None):
+        """poses: (n, 3, 4) or (n, 12) sensor -> vehicle transforms [R | t] (n = 0 or None: no sensors).  The four thresholds are
+        per-sensor sequences (or one value for all); None keeps this context's lmot_params value."""
+        if poses is None or len(poses) == 0:
+            self._chk(self.lib.lmot_set_sensors(self.h, None, 0))
+            return
+        P = np.asarray(poses, np.float32).reshape(len(poses), 12)
+        n = P.shape[0]
+        arr = (Sensor * n)()
+        for k in range(n):
+            self.lib.lmot_default_sensor(C.byref(self.params), C.byref(arr[k]))
+            arr[k].pose[:] = [float(v) for v in P[k]]
+            for name, val in (("h_sensor", h_sensor), ("t_hmin", t_hmin), ("t_hmax", t_hmax), ("sensor_height", sensor_height)):
+                if val is not None:
+                    setattr(arr[k], name, float(np.broadcast_to(np.asarray(val, np.float32), (n,))[k]))
+        self._chk(self.lib.lmot_set_sensors(self.h, arr, n))
+
+    def get_sensors(self):
+        """-> dict(poses (n, 3, 4) f32, h_sensor, t_hmin, t_hmax, sensor_height: (n,) f32 each)"""
+        arr = (Sensor * MAX_BATCH)()
+        n = C.c_int(0)
+        self._chk(self.lib.lmot_get_sensors(self.h, arr, MAX_BATCH, C.byref(n)))
+        s = arr[: n.value]
+        return dict(poses=np.array([list(e.pose) for e in s], np.float32).reshape(-1, 3, 4),
+                    **{k: np.array([getattr(e, k) for e in s], np.float32) for k in ("h_sensor", "t_hmin", "t_hmax", "sensor_height")})
 
     def tracker_reset(self):
         self._chk(self.lib.lmot_tracker_reset(self.h))

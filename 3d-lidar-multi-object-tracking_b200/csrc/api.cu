@@ -240,20 +240,21 @@ int batch_submit(Ctx* c, int bank_i, Result* r, const float4* const* d_pts, cons
   Slot* sl[kMaxBatch];
   const float4* pp[kMaxBatch];
   for (int i = 0; i < F; ++i) { sl[i] = &c->bslots[bank_i * c->batch_frames + i]; pp[i] = d_pts[i] ? d_pts[i] : sl[i]->d_points; }
+  const lmot_sensor* rig = c->n_sensors > 0 ? c->sensors : nullptr;     // copied into the launches' parameters: later changes leave this tick alone
   cudaStream_t st = sl[0]->stream;
   k->res = r; sl[0]->res = r;
   r->n_kev = 0;
   r->batch_frames = F;
   if (c->timing) cudaEventRecord(r->ev[0], st);
-  if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, c->fuse_ccl))) return rc;
+  if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, c->fuse_ccl, false, rig))) return rc;
   if (c->timing) cudaEventRecord(r->ev[1], st);
   if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
   if (c->timing) cudaEventRecord(r->ev[2], st);
-  if ((rc = boxfit_launch_batch(c, sl, F, st, n, false))) return rc;
+  if ((rc = boxfit_launch_batch(c, sl, F, st, n, false, rig))) return rc;
   int* d_fc = nullptr;                       // the per-frame counts go straight into the result's pinned, device-mapped block
   LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&d_fc, r->h_frame_counts, 0));
   const bool gf = with_tracker && c->prm.global_frame;
-  if ((rc = boxes_concat_launch(c, sl, F, st, k->d_boxes, k->d_counters, d_fc, (with_tracker && !gf) ? k->d_det_sem : nullptr))) return rc;
+  if ((rc = boxes_concat_launch(c, sl, F, st, k->d_boxes, k->d_counters, d_fc, (with_tracker && !gf) ? k->d_det_sem : nullptr, rig))) return rc;
   if (gf && (rc = boxes_to_global_launch(c, k, st, k->d_boxes, k->d_counters, ts, v, yaw, true))) return rc;
   if (c->timing) cudaEventRecord(r->ev[3], st);
   LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, st));
@@ -847,6 +848,7 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
                         double ts, double v, double yaw) {
   if (!ctx || !points || !n || n_frames < 1 || n_frames > kMaxBatch) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
+  if (c->n_sensors > 0 && n_frames > c->n_sensors) return LMOT_ERR_INVALID;     // a frame without a sensor pose
   cudaSetDevice(c->device);
   for (int i = 0; i < n_frames; ++i) {
     if (n[i] < 0 || (n[i] > 0 && !points[i])) return LMOT_ERR_INVALID;
@@ -898,6 +900,7 @@ int lmot_batch_detect_dev(lmot_ctx* ctx, const float* const* d_points, const int
 int lmot_batch_ground_ccl_dev(lmot_ctx* ctx, const float* const* d_points, const int* n, int n_frames) {
   if (!ctx || !d_points || !n || n_frames < 1 || n_frames > kMaxBatch) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
+  if (c->n_sensors > 0 && n_frames > c->n_sensors) return LMOT_ERR_INVALID;
   cudaSetDevice(c->device);
   int rc = batch_ensure(c, n_frames);
   if (rc) return rc;
@@ -910,7 +913,7 @@ int lmot_batch_ground_ccl_dev(lmot_ctx* ctx, const float* const* d_points, const
   }
   sl[0]->res = &c->results[0];
   c->results[0].n_kev = 0;
-  if ((rc = ground_launch_batch(c, sl, n_frames, pp, n, c->stream, true, false, c->fuse_ccl, c->fuse_ccl))) return rc;
+  if ((rc = ground_launch_batch(c, sl, n_frames, pp, n, c->stream, true, false, c->fuse_ccl, c->fuse_ccl, c->n_sensors > 0 ? c->sensors : nullptr))) return rc;
   return c->fuse_ccl ? LMOT_OK : ccl_launch_batch(c, sl, n_frames, c->stream);
 }
 
@@ -993,6 +996,7 @@ int lmot_track_step_lists_dev(lmot_ctx* ctx, const float* d_lists, const int* d_
                               double v_gps, double yaw_gps) {
   if (!ctx || !d_lists || !d_counts || n_lists < 1 || n_lists > kMaxBatch || cap_per_list < 1) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
+  if (c->n_sensors > 0 && n_lists > c->n_sensors) return LMOT_ERR_INVALID;     // a list without a sensor pose
   cudaSetDevice(c->device);
   int rc = batch_ensure(c, 1);              // the bank's box buffer + counters are the tracker's input
   if (rc) return rc;
@@ -1001,7 +1005,8 @@ int lmot_track_step_lists_dev(lmot_ctx* ctx, const float* d_lists, const int* d_
   k->res = r;
   r->n_kev = 0; r->batch_frames = 0;
   cudaStream_t st = c->stream;
-  if ((rc = boxes_pack_lists_launch(c, st, d_lists, d_counts, n_lists, cap_per_list, k->d_boxes, k->d_counters))) return rc;
+  if ((rc = boxes_pack_lists_launch(c, st, d_lists, d_counts, n_lists, cap_per_list, k->d_boxes, k->d_counters, c->n_sensors > 0 ? c->sensors : nullptr)))
+    return rc;
   if (c->prm.global_frame && (rc = boxes_to_global_launch(c, k, st, k->d_boxes, k->d_counters, timestamp_us, v_gps, yaw_gps, false))) return rc;
   if ((rc = tracker_launch(c, k, st, k->d_boxes, k->d_counters, timestamp_us, v_gps, yaw_gps))) return rc;
   if ((rc = tracker_publish(c, r, st))) return rc;
@@ -1010,6 +1015,46 @@ int lmot_track_step_lists_dev(lmot_ctx* ctx, const float* d_lists, const int* d_
   LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, st));
   r->has_tracks = true;
   if (!r->in_flight) { r->in_flight = true; ++c->n_in_flight; }
+  return LMOT_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- sensor rig
+int lmot_default_sensor(const lmot_params* p, lmot_sensor* out) {
+  if (!out) return LMOT_ERR_INVALID;
+  lmot_params d;
+  if (!p) { lmot_default_params(&d); p = &d; }
+  memset(out, 0, sizeof(*out));
+  out->pose[0] = out->pose[5] = out->pose[10] = 1.f;
+  out->h_sensor = p->h_sensor; out->t_hmin = p->t_hmin; out->t_hmax = p->t_hmax; out->sensor_height = p->sensor_height;
+  return LMOT_OK;
+}
+
+// the table only changes host state: ticks already submitted carry their own copy in their launch parameters
+int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n) {
+  if (!ctx || n < 0 || n > kMaxBatch || (n > 0 && !s)) return LMOT_ERR_INVALID;
+  for (int k = 0; k < n; ++k) {
+    const lmot_sensor& e = s[k];
+    const float v[4] = {e.h_sensor, e.t_hmin, e.t_hmax, e.sensor_height};
+    for (float x : e.pose) if (!std::isfinite(x)) return LMOT_ERR_INVALID;
+    for (float x : v) if (!std::isfinite(x)) return LMOT_ERR_INVALID;
+    for (int i = 0; i < 3; ++i)           // R^T R == I within 1e-5 per element (columns of the row-major 3x4)
+      for (int j = 0; j < 3; ++j) {
+        double d = 0.0;
+        for (int r = 0; r < 3; ++r) d += (double)e.pose[4 * r + i] * (double)e.pose[4 * r + j];
+        if (std::fabs(d - (i == j ? 1.0 : 0.0)) > 1e-5) return LMOT_ERR_INVALID;
+      }
+  }
+  Ctx* c = &ctx->c;
+  for (int k = 0; k < n; ++k) c->sensors[k] = s[k];
+  c->n_sensors = n;
+  return LMOT_OK;
+}
+
+int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n) {
+  if (!ctx || cap < 0 || (cap > 0 && !s)) return LMOT_ERR_INVALID;
+  const Ctx* c = &ctx->c;
+  if (n) *n = c->n_sensors;
+  for (int k = 0; k < c->n_sensors && k < cap; ++k) s[k] = c->sensors[k];
   return LMOT_OK;
 }
 

@@ -21,6 +21,7 @@
 // against OpenCV itself, bit-exact against the contract).
 #include <cfloat>
 #include <climits>
+#include <cstring>
 #include <random>
 #include "lmot_internal.cuh"
 
@@ -52,6 +53,7 @@ struct FitFrame {
   float* cl_box; float* cl_marker; uint8_t* cl_ok;
   float* boxes; float* markers; int* done; int* det_sem;
   unsigned* hist_ctr;      // atomicInc counter of finished tile_hist CTAs (wraps at the grid size: needs no reset)
+  float sensor_height;     // box_fit_kernel<., true>: this frame's sensor's (lmot_set_sensors); unread otherwise
 };
 struct FitBatch { FitFrame f[kMaxBatch]; };
 
@@ -275,14 +277,14 @@ struct MinI { __device__ int operator()(int a, int b) const { return a < b ? a :
 struct MaxI { __device__ int operator()(int a, int b) const { return a > b ? a : b; } };
 
 // ruleBasedFilter, box_fitting.cpp:97-158 (see lmot_rule_filter in lmot.h for the two modes)
-__device__ bool rule_filter(const float pc[4][2], float maxZ, int n, const BoxParams& P) {
+__device__ bool rule_filter(const float pc[4][2], float maxZ, int n, const BoxParams& P, float sensor_height) {
   if (n < P.min_points) return false;
   const float x1 = pc[0][0], y1 = pc[0][1], x2 = pc[1][0], y2 = pc[1][1], x3 = pc[2][0], y3 = pc[2][1];
   const float dist1 = sqrtf((x1 - x2) * (x1 - x2) + (y1 - y2) * (y1 - y2));
   const float dist2 = sqrtf((x3 - x2) * (x3 - x2) + (y3 - y2) * (y3 - y2));
   float length, width;
   if (dist1 > dist2) { length = dist1; width = dist2; } else { length = dist2; width = dist1; }
-  const float height = maxZ + P.sensor_height;
+  const float height = maxZ + sensor_height;
   const float area = dist1 * dist2;
   const float mass = area * height;
   const float ratio = length / width;
@@ -300,7 +302,8 @@ __device__ bool rule_filter(const float pc[4][2], float maxZ, int n, const BoxPa
   return false;
 }
 
-template <int NT>
+// kRig: sensor_height from the frame's FitFrame (a sensor rig, lmot_set_sensors) instead of P
+template <int NT, bool kRig>
 __global__ void __launch_bounds__(NT, 1024 / NT)     // <= 64 registers: 1,024 threads of box fitting per SM
 box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxParams P,
                const unsigned long long* __restrict__ mt_raw, int n_raw, int max_clusters, int max_boxes) {
@@ -659,13 +662,13 @@ box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxPa
       __syncthreads();
     }
     for (int c = 0; c < 4; ++c) { pc[c][0] = s_pc[c][0]; pc[c][1] = s_pc[c][1]; }
-    const bool ok = rule_filter(pc, maxZ, n, P);
+    const bool ok = rule_filter(pc, maxZ, n, P, kRig ? F.sensor_height : P.sensor_height);
     if (tid == 0) {
       cl_ok[k] = ok ? 1 : 0;
       if (ok) {
         float* b = cl_box + (size_t)k * 24;
         for (int h = 0; h < 2; ++h)
-          for (int c = 0; c < 4; ++c) { b[(h * 4 + c) * 3] = pc[c][0]; b[(h * 4 + c) * 3 + 1] = pc[c][1]; b[(h * 4 + c) * 3 + 2] = h == 0 ? -P.sensor_height : maxZ; }
+          for (int c = 0; c < 4; ++c) { b[(h * 4 + c) * 3] = pc[c][0]; b[(h * 4 + c) * 3 + 1] = pc[c][1]; b[(h * 4 + c) * 3 + 2] = h == 0 ? -(kRig ? F.sensor_height : P.sensor_height) : maxZ; }
         float* mk = cl_marker + (size_t)k * 6;      // mark_cluster (:161-209); zero extents become 0.1
         mk[0] = (float)(sx / n); mk[1] = (float)(sy / n); mk[2] = (float)(sz / n);
         float ex = mxx - mnx, ey = mxy - mny, ez = mxz - mnz;
@@ -720,11 +723,27 @@ box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxPa
   }
 }
 
+// p' = [R | t] p (lmot_set_sensors): ((r0 x + r1 y) + r2 z) + t per row in float, no contraction -- pcl::transformPointCloud's
+// evaluation with an Affine3f.  m = row-major 3x4.
+__device__ __forceinline__ void rig_apply(const float* m, float& x, float& y, float& z) {
+  const float ox = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[0], x), __fmul_rn(m[1], y)), __fmul_rn(m[2], z)), m[3]);
+  const float oy = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[4], x), __fmul_rn(m[5], y)), __fmul_rn(m[6], z)), m[7]);
+  const float oz = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[8], x), __fmul_rn(m[9], y)), __fmul_rn(m[10], z)), m[11]);
+  x = ox; y = oy; z = oz;
+}
+
+// one box (8 corners, 24 floats) moved by pose m
+__device__ __forceinline__ void rig_apply_box(const float* m, float* b) {
+#pragma unroll
+  for (int c = 0; c < 8; ++c) rig_apply(m, b[3 * c], b[3 * c + 1], b[3 * c + 2]);
+}
+
 // batched submissions (one frame per sensor stream): the frames' box lists, concatenated in stream order, are ONE measurement
-// list for the tracker (tracking/main.cpp:98-141 unpacks whatever the trackbox message holds; one immUkfJpdaf call per tick)
-__global__ void __launch_bounds__(256)
-concat_boxes_kernel(const __grid_constant__ FitBatch B, int n_frames, int max_boxes, float* __restrict__ boxes, int* __restrict__ counters,
-                    int* __restrict__ frame_counts, int* __restrict__ det_sem) {
+// list for the tracker (tracking/main.cpp:98-141 unpacks whatever the trackbox message holds; one immUkfJpdaf call per tick).
+// kRig: frame w's boxes are moved into the vehicle frame by its sensor's pose R->m[w] on the way.
+template <bool kRig>
+__device__ __forceinline__ void concat_boxes_body(const FitBatch& B, const RigPoses* R, int n_frames, int max_boxes, float* __restrict__ boxes,
+                                                  int* __restrict__ counters, int* __restrict__ frame_counts, int* __restrict__ det_sem) {
   __shared__ int s_off[kMaxBatch + 1];
   __shared__ int s_fc[kMaxBatch][5];
   // thread f fetches frame f's five counters (independent loads: one L2 round trip for the whole tick; a single thread walking the
@@ -762,13 +781,27 @@ concat_boxes_kernel(const __grid_constant__ FitBatch B, int n_frames, int max_bo
       const int off = s_off[w], cnt = min(s_off[w + 1], max_boxes) - off;
       const uint4* src = reinterpret_cast<const uint4*>(B.f[w].boxes);
       uint4* dst = reinterpret_cast<uint4*>(boxes + (size_t)off * 24);
-      const int nw = cnt > 0 ? cnt * 6 : 0;
-      for (int e0 = lane; e0 < nw; e0 += 128) {
-        uint4 v[4];
+      if (!kRig) {
+        const int nw = cnt > 0 ? cnt * 6 : 0;
+        for (int e0 = lane; e0 < nw; e0 += 128) {
+          uint4 v[4];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) { const int e = e0 + 32 * u; if (e < nw) v[u] = src[e]; }
+          for (int u = 0; u < 4; ++u) { const int e = e0 + 32 * u; if (e < nw) v[u] = src[e]; }
 #pragma unroll
-        for (int u = 0; u < 4; ++u) { const int e = e0 + 32 * u; if (e < nw) dst[e] = v[u]; }
+          for (int u = 0; u < 4; ++u) { const int e = e0 + 32 * u; if (e < nw) dst[e] = v[u]; }
+        }
+      } else {
+        // a whole box per lane: its six words in flight, then its eight corners through the pose
+        const float* m = R->m[w];
+        for (int j = lane; j < cnt; j += 32) {
+          uint4 v[6];
+#pragma unroll
+          for (int u = 0; u < 6; ++u) v[u] = src[6 * j + u];
+          float* b = reinterpret_cast<float*>(v);
+          rig_apply_box(m, b);
+#pragma unroll
+          for (int u = 0; u < 6; ++u) dst[6 * j + u] = v[u];
+        }
       }
     }
   }
@@ -777,6 +810,18 @@ concat_boxes_kernel(const __grid_constant__ FitBatch B, int n_frames, int max_bo
     __threadfence_system();                // frame_counts lives in pinned host memory: the host reads it after the tick's completion event
     if (det_sem) atomicAdd(det_sem, 1);
   }
+}
+
+__global__ void __launch_bounds__(256)
+concat_boxes_kernel(const __grid_constant__ FitBatch B, int n_frames, int max_boxes, float* __restrict__ boxes, int* __restrict__ counters,
+                    int* __restrict__ frame_counts, int* __restrict__ det_sem) {
+  concat_boxes_body<false>(B, nullptr, n_frames, max_boxes, boxes, counters, frame_counts, det_sem);
+}
+
+__global__ void __launch_bounds__(256)
+concat_boxes_rig_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ RigPoses R, int n_frames, int max_boxes, float* __restrict__ boxes,
+                        int* __restrict__ counters, int* __restrict__ frame_counts, int* __restrict__ det_sem) {
+  concat_boxes_body<true>(B, &R, n_frames, max_boxes, boxes, counters, frame_counts, det_sem);
 }
 
 }  // namespace
@@ -827,7 +872,13 @@ void boxfit_free(Slot* s) {
   cudaFree(s->d_done); cudaFree(s->d_det_sem);
 }
 
+static void rig_poses_of(const lmot_sensor* rig, int n, RigPoses& R) {
+  memset(&R, 0, sizeof(R));
+  for (int i = 0; i < n; ++i) memcpy(R.m[i], rig[i].pose, sizeof(R.m[i]));
+}
+
 static void fit_frame_of(const Slot* s, FitFrame& f, bool post_sem) {
+  f.sensor_height = 0.f;
   f.cart = s->d_cart; f.label_grid = s->d_label_grid; f.counters = s->d_counters;
   f.pcid = s->d_pcid; f.table = s->d_table; f.seg_start = s->d_seg_start; f.seg_size = s->d_seg_size;
   f.elev = s->d_elev; f.sorted_pts = s->d_sorted_pts;
@@ -838,14 +889,14 @@ static void fit_frame_of(const Slot* s, FitFrame& f, bool post_sem) {
 
 // inputs per frame: s->d_elev / CNT_N_ELEV, s->d_cart (from clustering), s->d_label_grid / CNT_NUM_CLUSTER.
 // F > 1: one frame per sensor stream; the four kernels run over the union of the frames' clusters (blockIdx.y = frame).
-int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem) {
+int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig) {
   if (F < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   const int K1 = c->prm.max_clusters + 1;
   int tiles = 0;
   for (int i = 0; i < F; ++i) { const int t = (n_upper[i] + kTile - 1) / kTile; if (t > tiles) tiles = t; }
   const size_t sh = (size_t)K1 * sizeof(int);
   FitBatch B;
-  for (int i = 0; i < F; ++i) fit_frame_of(slots[i], B.f[i], post_sem && F == 1);
+  for (int i = 0; i < F; ++i) { fit_frame_of(slots[i], B.f[i], post_sem && F == 1); if (rig) B.f[i].sensor_height = rig[i].sensor_height; }
   for (int i = F; i < kMaxBatch; ++i) B.f[i] = B.f[0];
   Slot* s0 = slots[0];
   if (tiles > 0) tile_hist_kernel<<<dim3(tiles, F), kTile, sh, st>>>(B, c->prm.max_clusters);     // + segment offsets by its last CTA per frame
@@ -879,8 +930,13 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
     cfg.gridDim = dim3(gx, F); cfg.blockDim = dim3(F == 1 ? kFitThreadsFrame : kFitThreadsBatch); cfg.dynamicSmemBytes = 0; cfg.stream = st; cfg.attrs = &pdl; cfg.numAttrs = 1;
     const unsigned long long* mt = c->d_mt_raw;
     const int n_raw = c->n_mt_raw, max_boxes = c->prm.max_boxes;
-    if (F == 1) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsFrame>, B, P, mt, n_raw, max_clusters, max_boxes));
-    else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsBatch>, B, P, mt, n_raw, max_clusters, max_boxes));
+    if (rig) {
+      if (F == 1) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsFrame, true>, B, P, mt, n_raw, max_clusters, max_boxes));
+      else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsBatch, true>, B, P, mt, n_raw, max_clusters, max_boxes));
+    } else {
+      if (F == 1) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsFrame, false>, B, P, mt, n_raw, max_clusters, max_boxes));
+      else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsBatch, false>, B, P, mt, n_raw, max_clusters, max_boxes));
+    }
   }
   kernel_mark(c, s0, st);
   LMOT_CUDA(c, cudaGetLastError());
@@ -888,21 +944,29 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
 }
 
 // the frames' box lists concatenated in stream order -> d_boxes / counters of the batch (the tracker's measurement list)
-int boxes_concat_launch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, float* d_boxes, int* d_counters, int* d_frame_counts, int* det_sem) {
+// rig: frame i's boxes moved by sensor i's pose (vehicle frame)
+int boxes_concat_launch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, float* d_boxes, int* d_counters, int* d_frame_counts, int* det_sem,
+                        const lmot_sensor* rig) {
   FitBatch B;
   for (int i = 0; i < F; ++i) fit_frame_of(slots[i], B.f[i], false);
   for (int i = F; i < kMaxBatch; ++i) B.f[i] = B.f[0];
-  concat_boxes_kernel<<<1, 256, 0, st>>>(B, F, c->prm.max_boxes, d_boxes, d_counters, d_frame_counts, det_sem);
+  if (rig) {
+    RigPoses R;
+    rig_poses_of(rig, F, R);
+    concat_boxes_rig_kernel<<<1, 256, 0, st>>>(B, R, F, c->prm.max_boxes, d_boxes, d_counters, d_frame_counts, det_sem);
+  } else {
+    concat_boxes_kernel<<<1, 256, 0, st>>>(B, F, c->prm.max_boxes, d_boxes, d_counters, d_frame_counts, det_sem);
+  }
   kernel_mark(c, slots[0], st);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
 }
 
 // n_lists padded device box lists (capacity cap boxes each, lengths in d_counts) -> one contiguous list + the counter block the
-// tracker reads (multi-GPU hand-over: the lists arrived by ncclAllGather)
-__global__ void __launch_bounds__(256)
-pack_lists_kernel(const float* __restrict__ lists, const int* __restrict__ counts, int n_lists, int cap, int max_boxes, float* __restrict__ boxes,
-                  int* __restrict__ counters) {
+// tracker reads (multi-GPU hand-over: the lists arrived by ncclAllGather).  kRig: list l's boxes moved by pose R->m[l].
+template <bool kRig>
+__device__ __forceinline__ void pack_lists_body(const RigPoses* R, const float* __restrict__ lists, const int* __restrict__ counts, int n_lists, int cap,
+                                                int max_boxes, float* __restrict__ boxes, int* __restrict__ counters) {
   __shared__ int s_off[kMaxBatch + 1];
   if (threadIdx.x == 0) {
     int acc = 0;
@@ -916,12 +980,45 @@ pack_lists_kernel(const float* __restrict__ lists, const int* __restrict__ count
   for (int l = 0; l < n_lists; ++l) {
     const int off = s_off[l], cnt = min(s_off[l + 1], max_boxes) - off;
     const float* src = lists + (size_t)l * cap * 24;
-    for (int e = threadIdx.x; e < cnt * 24; e += 256) boxes[(size_t)off * 24 + e] = src[e];
+    if (!kRig) {
+      for (int e = threadIdx.x; e < cnt * 24; e += 256) boxes[(size_t)off * 24 + e] = src[e];
+    } else {
+      // a whole box per thread: its 24 floats in flight (the caller's lists need only 4-byte alignment), then the pose
+      const float* m = R->m[l];
+      for (int j = threadIdx.x; j < cnt; j += 256) {
+        float b[24];
+#pragma unroll
+        for (int u = 0; u < 24; ++u) b[u] = src[(size_t)j * 24 + u];
+        rig_apply_box(m, b);
+        float4* d = reinterpret_cast<float4*>(boxes + (size_t)(off + j) * 24);
+#pragma unroll
+        for (int u = 0; u < 6; ++u) d[u] = make_float4(b[4 * u], b[4 * u + 1], b[4 * u + 2], b[4 * u + 3]);
+      }
+    }
   }
 }
 
-int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int n_lists, int cap, float* d_boxes, int* d_counters) {
-  pack_lists_kernel<<<1, 256, 0, st>>>(d_lists, d_counts, n_lists, cap, c->prm.max_boxes, d_boxes, d_counters);
+__global__ void __launch_bounds__(256)
+pack_lists_kernel(const float* __restrict__ lists, const int* __restrict__ counts, int n_lists, int cap, int max_boxes, float* __restrict__ boxes,
+                  int* __restrict__ counters) {
+  pack_lists_body<false>(nullptr, lists, counts, n_lists, cap, max_boxes, boxes, counters);
+}
+
+__global__ void __launch_bounds__(256)
+pack_lists_rig_kernel(const __grid_constant__ RigPoses R, const float* __restrict__ lists, const int* __restrict__ counts, int n_lists, int cap,
+                      int max_boxes, float* __restrict__ boxes, int* __restrict__ counters) {
+  pack_lists_body<true>(&R, lists, counts, n_lists, cap, max_boxes, boxes, counters);
+}
+
+int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int n_lists, int cap, float* d_boxes, int* d_counters,
+                            const lmot_sensor* rig) {
+  if (rig) {
+    RigPoses R;
+    rig_poses_of(rig, n_lists, R);
+    pack_lists_rig_kernel<<<1, 256, 0, st>>>(R, d_lists, d_counts, n_lists, cap, c->prm.max_boxes, d_boxes, d_counters);
+  } else {
+    pack_lists_kernel<<<1, 256, 0, st>>>(d_lists, d_counts, n_lists, cap, c->prm.max_boxes, d_boxes, d_counters);
+  }
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
 }

@@ -137,7 +137,8 @@ __device__ __forceinline__ float label_limit(float h, bool is_ground, double tol
   return f;
 }
 
-__device__ __forceinline__ void polar_grid_slice(const GroundParams& p, const unsigned* __restrict__ keys, int own0, int n_own,
+// t_hmin / t_hmax / h_sensor: lmot_params' values, or the frame's sensor's in a rig launch (lmot_set_sensors)
+__device__ __forceinline__ void polar_grid_slice(const GroundParams& p, float t_hmin, float t_hmax, float h_sensor, const unsigned* __restrict__ keys, int own0, int n_own,
                                                  float* H, uint8_t* G, float* __restrict__ o_minz, float* __restrict__ o_height,
                                                  float* __restrict__ o_smoothed, float* __restrict__ o_hdiff,
                                                  float* __restrict__ o_hg, float* __restrict__ o_lim = nullptr) {
@@ -155,9 +156,9 @@ __device__ __forceinline__ void polar_grid_slice(const GroundParams& p, const un
       if (ch >= 0 && ch < kNumChannel) {
         const float zi = fkey_inv(__ldcg(&keys[ch * kNumBin + b]));
         if (lc >= 1 && lc <= n_own && o_minz) o_minz[ch * kNumBin + b] = zi;
-        if (zi > p.t_hmin && zi < p.t_hmax) h = zi;
-        else if (zi > p.t_hmax) h = p.h_sensor;
-        else h = p.t_hmin;
+        if (zi > t_hmin && zi < t_hmax) h = zi;
+        else if (zi > t_hmax) h = h_sensor;
+        else h = t_hmin;
       }
       H[l] = h;
     }
@@ -186,7 +187,7 @@ __device__ __forceinline__ void polar_grid_slice(const GroundParams& p, const un
           hd = (pre > post) ? pre : post;
         }
         if (lc >= 1 && lc <= n_own && o_smoothed) { o_smoothed[ch * kNumBin + b] = sm; o_hdiff[ch * kNumBin + b] = hd; }
-        g = ((sm < p.t_hmax && hd < p.t_hdiff) || (h < p.t_hmax && hd < p.t_hdiff)) ? 1 : 0;  // :205-214
+        g = ((sm < t_hmax && hd < p.t_hdiff) || (h < t_hmax && hd < p.t_hdiff)) ? 1 : 0;  // :205-214
       }
       G[l] = g;
     }
@@ -228,7 +229,7 @@ __device__ __forceinline__ void polar_grid_slice(const GroundParams& p, const un
   // force H[b-1]==H[b]==T and H[b+1]!=T, which rules out a rewrite at b-2 (its b+2 is H[b]==T, its b+1 is T): the chain
   // is at most two cells long, so every cell's final value is a closed form of the ORIGINAL H[b-2..b+2], G[b-2..b+2].
   {
-    const float T = p.t_hmin;
+    const float T = t_hmin;
     float newh[kCellsPerThread];
     unsigned mod = 0;
 #pragma unroll
@@ -360,6 +361,7 @@ struct GroundBatch {
   int n_frames, ctas_per_frame;
   unsigned spin_limit;
   FrameIO f[kMaxBatch];
+  float mount[kMaxBatch][3];  // ground_fused_rig_kernel: t_hmin, t_hmax, h_sensor of each frame's sensor (phase 2); unread otherwise
 };
 
 // the fast evaluation of polar_cell(): cell id, kNoCell (certainly outside the range window) or kPending (within the guard band
@@ -477,8 +479,9 @@ __device__ __forceinline__ void bin_pair(int t0, int T, int cnt, int res_tiles, 
 // ("No second barrier" was tried: every CTA evaluating the polar grid for the channels its own points fall into, in shared
 // memory.  With ring-major clouds a chunk spans most of the 80 channels, so every CTA redid most of the grid and the kernel
 // issued far more instructions.  The grid is evaluated ONCE, spread over the CTAs.)
-__global__ void __launch_bounds__(kFusedThreads, 1)
-ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant__ GroundParams p, float roi) {
+// kRig: phase 2 takes each frame's t_hmin / t_hmax / h_sensor from B.mount (a sensor rig, lmot_set_sensors) instead of p
+template <bool kRig>
+__device__ __forceinline__ void ground_fused_body(const GroundBatch& B, const GroundParams& p, float roi) {
   extern __shared__ __align__(128) unsigned char fsm[];
   const int Gf = B.ctas_per_frame;
   const int frame = blockIdx.x / Gf, cta = blockIdx.x - frame * Gf;
@@ -571,7 +574,10 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
     const int gc = Gf < kNumChannel ? Gf : kNumChannel;
     if (cta < gc) {
       const int own0 = cta * kNumChannel / gc, own1 = (cta + 1) * kNumChannel / gc;
-      polar_grid_slice(p, keys, own0, own1 - own0, s_H, s_G, (float*)nullptr, (float*)nullptr, (float*)nullptr, (float*)nullptr, F.hg, F.lim);
+      if (kRig) polar_grid_slice(p, B.mount[frame][0], B.mount[frame][1], B.mount[frame][2], keys, own0, own1 - own0, s_H, s_G, (float*)nullptr,
+                                 (float*)nullptr, (float*)nullptr, (float*)nullptr, F.hg, F.lim);
+      else polar_grid_slice(p, p.t_hmin, p.t_hmax, p.h_sensor, keys, own0, own1 - own0, s_H, s_G, (float*)nullptr, (float*)nullptr, (float*)nullptr,
+                            (float*)nullptr, F.hg, F.lim);
     }
   }
   grid_barrier(F.bar, F.bar_target + (unsigned)Gf, B.spin_limit);
@@ -729,6 +735,13 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
   }
 }
 
+__global__ void __launch_bounds__(kFusedThreads, 1)
+ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant__ GroundParams p, float roi) { ground_fused_body<false>(B, p, roi); }
+
+// batched ticks of a sensor rig: the same kernel with every frame's ground thresholds from its own sensor
+__global__ void __launch_bounds__(kFusedThreads, 1)
+ground_fused_rig_kernel(const __grid_constant__ GroundBatch B, const __grid_constant__ GroundParams p, float roi) { ground_fused_body<true>(B, p, roi); }
+
 // inspection only (lmot_debug_polar_grid): all five 80x120 grids of the reference from the min-z keys of the last launch, ten
 // channels per CTA.  (The fused kernel evaluates, per CTA, only the channels that CTA's points need, and keeps them in shared memory.)
 __global__ void __launch_bounds__(kFusedThreads)
@@ -738,7 +751,7 @@ polar_grid_debug_kernel(GroundParams p, const unsigned* __restrict__ keys, float
   __shared__ uint8_t s_G[kMaxLocCells];
   const int gc = gridDim.x;
   const int own0 = blockIdx.x * kNumChannel / gc, own1 = (blockIdx.x + 1) * kNumChannel / gc;
-  polar_grid_slice(p, keys, own0, own1 - own0, s_H, s_G, o_minz, o_height, o_smoothed, o_hdiff, o_hg);
+  polar_grid_slice(p, p.t_hmin, p.t_hmax, p.h_sensor, keys, own0, own1 - own0, s_H, s_G, o_minz, o_height, o_smoothed, o_hdiff, o_hg);
 }
 
 // inspection only (lmot_debug_cell_index): the fused kernel keeps the cell ids in shared memory
@@ -765,6 +778,7 @@ int ground_alloc(Ctx* c, Slot* s) {
   // co-residency limit of the cooperative kernel on this device (1 CTA per SM at this shared-memory size)
   if (c->fused_max_ctas == 0) {
     LMOT_CUDA(c, cudaFuncSetAttribute(ground_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFusedSmem));
+    LMOT_CUDA(c, cudaFuncSetAttribute(ground_fused_rig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFusedSmem));
     int sms = 0, per_sm = 0, coop = 0;
     LMOT_CUDA(c, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
     LMOT_CUDA(c, cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, c->device));
@@ -835,7 +849,7 @@ bool ground_reads_input_once(const Ctx* c, int n) {
 // One launch for F frames (F = 1: the frame pipeline and the stage entry points; F > 1: one frame per sensor stream, api.cu
 // lmot_batch_*).  Frame i runs on slots[i]'s buffers; its CTAs are [i * G, (i + 1) * G) of the grid and synchronise among themselves.
 int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* pts, const int* n, cudaStream_t st, bool fuse_count,
-                        bool want_labels, bool fuse_ccl, bool chain) {
+                        bool want_labels, bool fuse_ccl, bool chain, const lmot_sensor* rig) {
   if (fuse_ccl && !fuse_count) return LMOT_ERR_INVALID;
   if (F < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   int n_max = 0;
@@ -884,6 +898,9 @@ int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* 
     f.out.counters = s->d_counters;
     s->bar_base += 2u * (unsigned)G;
   }
+  if (rig)
+    for (int i = 0; i < F; ++i) { B.mount[i][0] = rig[i].t_hmin; B.mount[i][1] = rig[i].t_hmax; B.mount[i][2] = rig[i].h_sensor; }
+  const void* kern = rig ? (const void*)ground_fused_rig_kernel : (const void*)ground_fused_kernel;
   float roi = c->prm.roi_m;
   GroundParams gp = c->gp;
   void* args[] = {(void*)&B, (void*)&gp, (void*)&roi};
@@ -893,7 +910,7 @@ int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* 
   size_t smem = (size_t)fused_smem_bytes(tiles < kMaxResTiles ? tiles : kMaxResTiles, tiles > 0 ? tiles : 1);
   if (fuse_ccl && smem < (size_t)kDenseSmem) smem = kDenseSmem;
   if (c->coop_launch) {
-    LMOT_CUDA(c, cudaLaunchCooperativeKernel((const void*)ground_fused_kernel, dim3(G * F), dim3(kFusedThreads), args, smem, st));
+    LMOT_CUDA(c, cudaLaunchCooperativeKernel(kern, dim3(G * F), dim3(kFusedThreads), args, smem, st));
   } else {
     // Ordinary launch + the guarantee a cooperative launch would give, obtained differently.  A cooperative launch makes
     // the driver wait for an idle device, i.e. it serialises the frame pipeline's streams (measured: the detection stages of
@@ -924,7 +941,7 @@ int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* 
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = (chain && same_stream && g.record_pending && !c->timing) ? 1 : 0;
-    LMOT_CUDA(c, cudaLaunchKernelExC(&cfg, (const void*)ground_fused_kernel, args));
+    LMOT_CUDA(c, cudaLaunchKernelExC(&cfg, kern, args));
     if (chain) g.record_pending = true;
     else { LMOT_CUDA(c, cudaEventRecord(g.done, st)); g.record_pending = false; g.recorded = true; }
     g.last = st; g.have_last = true;

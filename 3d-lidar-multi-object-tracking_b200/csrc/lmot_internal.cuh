@@ -56,6 +56,10 @@ struct TrackState {
 // planar rigid transform, rows (m0 m1 . m2) / (m3 m4 . m5) of a 4x4 whose third row is (0 0 1 0): lmot_params.global_frame
 struct Xf2 { int on = 0; float m[6] = {1.f, 0.f, 0.f, 0.f, 1.f, 0.f}; };
 
+// sensor -> vehicle poses of a batched tick (lmot_set_sensors), copied into the launch parameters of the kernels that concatenate
+// the tracker's measurement list: frame / list k uses m[k] (row-major 3x4 [R | t])
+struct RigPoses { float m[kMaxBatch][12]; };
+
 // frame-level scalars of imm_ukf_jpda.cpp:19-24,56-58 (host side: a handful of doubles per frame)
 struct TrackerHost {
   bool init = false;
@@ -195,6 +199,9 @@ struct Ctx {
   Slot bslots[kBatchBanks * kMaxBatch];
   int n_bslots = 0, batch_frames = 0, next_bank = 0;
   Slot bank[kBatchBanks];              // pseudo-slots: concatenated boxes + counters + semaphore + events of a bank
+  // ---- sensor rig (lmot_set_sensors): sensor k = frame k of a batched tick / list k of lmot_track_step_lists_dev; read at submission
+  int n_sensors = 0;                   // 0: every frame uses prm, the rig kernels are never launched
+  lmot_sensor sensors[kMaxBatch];
 
   // ---- result ring
   int n_results = 1;
@@ -275,7 +282,8 @@ void ground_free(Slot* s);
 // `chain`: stand-alone entry points -- nothing of the library follows on `st` before the next ground launch; consecutive launches on
 // one stream then run as programmatic dependents without an event between them (ground.cu, GroundChain)
 int ground_launch(Ctx* c, Slot* s, cudaStream_t st, const float4* pts, int n, bool fuse_count = false, bool want_labels = true, bool fuse_ccl = false, bool chain = false);
-int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* pts, const int* n, cudaStream_t st, bool fuse_count, bool want_labels, bool fuse_ccl = false, bool chain = false);
+// rig (nullable): sensor i's h_sensor / t_hmin / t_hmax for frame i (lmot_set_sensors); nullptr: lmot_params' values for every frame
+int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* pts, const int* n, cudaStream_t st, bool fuse_count, bool want_labels, bool fuse_ccl = false, bool chain = false, const lmot_sensor* rig = nullptr);
 void ground_chain_forget(int device, bool device_idle);
 int ground_cells_debug(Ctx* c, Slot* s, cudaStream_t st);
 int ground_grids_debug(Ctx* c, Slot* s, cudaStream_t st);   // d_minz / d_height / d_smoothed / d_hdiff / d_hg_dbg from the last launch's keys
@@ -291,9 +299,12 @@ int boxfit_alloc(Ctx* c, Slot* s);
 int boxfit_alloc_shared(Ctx* c);
 void boxfit_free(Slot* s);
 int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem = false);
-int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem);
-int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int n_lists, int cap, float* d_boxes, int* d_counters);
-int boxes_concat_launch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, float* d_boxes, int* d_counters, int* d_frame_counts, int* det_sem);
+// rig (nullable): sensor i's sensor_height for frame i (box fitting) / sensor i's pose for list i (concatenation)
+int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig = nullptr);
+int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int n_lists, int cap, float* d_boxes, int* d_counters,
+                            const lmot_sensor* rig = nullptr);
+int boxes_concat_launch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, float* d_boxes, int* d_counters, int* d_frame_counts, int* det_sem,
+                        const lmot_sensor* rig = nullptr);
 void origin_points_fold(TrackerHost& h, double timestamp, double v_gps, double yaw_gps);
 int tracker_alloc(Ctx* c);
 void tracker_free(Ctx* c);

@@ -101,7 +101,9 @@ typedef struct lmot_params {
    * targetPoints / visBBs back afterwards (tracking/main.cpp:76-83,142-158,182-195).  1: lmot_track_step / lmot_frame* / lmot_batch*
    * do the same on the device: boxes in, targets / vis_bb out stay in the SENSOR frame, the tracker state (and what lmot_tracker_dump
    * shows) is in the global frame.  0 (default): immUkfJpdaf as a function, boxes used as given.  The transform arithmetic is
-   * pcl_ros::transformPointCloud's (float 4x4 from a double tf::Transform); tf and pcl_ros are not part of the reference tree. */
+   * pcl_ros::transformPointCloud's (float 4x4 from a double tf::Transform); tf and pcl_ros are not part of the reference tree.
+   * With a sensor rig (lmot_set_sensors) the batched ticks first move each sensor's boxes into the vehicle frame with the same
+   * evaluation, ((r00*x + r01*y) + r02*z) + t0 per row in float without contraction, and this step then runs on that list. */
   int global_frame;          /* 0 */
   /* frames in flight inside one context: detection stages of frame f+1.. overlap the tracker of frame f (1..8, default 4) */
   int pipeline_depth;
@@ -254,6 +256,33 @@ int lmot_batch(lmot_ctx* ctx, const float* const* points, const int* n, int n_fr
                double v_gps, double yaw_gps, lmot_batch_out* out);   /* submit + collect */
 /* ground removal + connected components only, two launches on the caller stream, results stay on the device (roofline measurement) */
 int lmot_batch_ground_ccl_dev(lmot_ctx* ctx, const float* const* d_points, const int* n, int n_frames);
+
+/* ---- sensor rig: where each sensor of a batched tick is mounted ------------------------------------------------------------------
+ * Sensor k is frame k of a batched tick (lmot_batch, lmot_batch_submit, lmot_batch_dev, lmot_batch_detect_dev,
+ * lmot_batch_ground_ccl_dev) and list k of lmot_track_step_lists_dev (rank k of lmot_shared_tick_dev in LMOT_SHARED_STREAMS mode;
+ * in LMOT_SHARED_FRAMES mode every step is one list and uses sensor 0).  With sensors set:
+ *   - frame k's ground removal uses sensor k's h_sensor / t_hmin / t_hmax and its box fitting sensor k's sensor_height in place of
+ *     lmot_params' values: per-frame results equal lmot_ground_remove / lmot_box_fit on a context created with those four values;
+ *   - where the tracker's measurement list is concatenated, every corner of list k's boxes is moved by sensor k's pose (sensor ->
+ *     vehicle frame, row-major 3x4 [R | t]) as pcl::transformPointCloud evaluates it with an Affine3f, in float, without contraction:
+ *         x' = ((r00*x + r01*y) + r02*z) + t0,  y' = ((r10*x + r11*y) + r12*z) + t1,  z' = ((r20*x + r21*y) + r22*z) + t2
+ *     so the concatenated list, the tracker's input and lmot_batch_out.boxes are in the VEHICLE frame.  With global_frame = 1 the
+ *     vehicle-frame list then takes the sensor -> global step of lmot_params.global_frame (the dead-reckoned ego pose is the
+ *     vehicle's): two roundings in sequence, not one premultiplied matrix; targets and vis_bb come back in the vehicle frame.
+ * The table is captured by value when a tick is submitted: ticks already in flight keep the table they were submitted with.  A tick or
+ * list step with more frames than sensors is LMOT_ERR_INVALID while sensors are set.  Not affected: the stage entry points,
+ * lmot_track_step and the single-stream lmot_frame* calls.  Detections of one object by two sensors with overlapping fields of view
+ * stay two measurements (the reference has no fusion step). */
+typedef struct lmot_sensor {
+  float pose[12];                 /* sensor -> vehicle frame, row-major 3x4 [R | t]; R orthonormal (|R^T R - I| <= 1e-5 elementwise) */
+  float h_sensor, t_hmin, t_hmax; /* ground removal: replace lmot_params' values for this sensor's frames */
+  float sensor_height;            /* box fitting: likewise */
+} lmot_sensor;
+int lmot_default_sensor(const lmot_params* p, lmot_sensor* out);      /* identity pose + p's four values (p NULL: the defaults) */
+/* n = 0 (s may be NULL): no sensors, every frame uses lmot_params.  LMOT_ERR_INVALID, table unchanged: n < 0, n > LMOT_MAX_BATCH,
+ * a non-finite value, a rotation that is not orthonormal */
+int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n);
+int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n);   /* *n = sensors set; copies min(n, cap) of them */
 
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
