@@ -90,6 +90,10 @@ class FrameOut(C.Structure):
     ]
 
 
+class SeqOut(C.Structure):
+    _fields_ = [("n_seq", C.c_int), ("seq", FrameOut * MAX_BATCH)]
+
+
 # every symbol include/lmot.h declares (tests assert the library exports all of them)
 ABI_SYMBOLS = [
     "lmot_default_params", "lmot_create", "lmot_destroy", "lmot_get_params", "lmot_strerror", "lmot_last_error", "lmot_build_info",
@@ -98,6 +102,8 @@ ABI_SYMBOLS = [
     "lmot_ground_remove_dev", "lmot_detect_dev", "lmot_sync",
     "lmot_batch_submit", "lmot_batch_dev", "lmot_batch_detect_dev", "lmot_batch_collect", "lmot_batch_fetch", "lmot_batch", "lmot_batch_ground_ccl_dev",
     "lmot_default_sensor", "lmot_set_sensors", "lmot_get_sensors",
+    "lmot_seq_open", "lmot_seq_submit", "lmot_seq_dev", "lmot_seq_collect", "lmot_seq_fetch", "lmot_seq", "lmot_seq_tracker_reset",
+    "lmot_seq_tracker_dump", "lmot_seq_tracker_get_ego",
     "lmot_detect_boxes_dev", "lmot_track_step_lists_dev", "lmot_tracker_counters_dev", "lmot_tracker_table_received",
     "lmot_origin_points", "lmot_tracker_table", "lmot_tracker_set_num_tracks", "lmot_tracker_reset", "lmot_tracker_num_tracks", "lmot_tracker_dump", "lmot_tracker_load", "lmot_tracker_get_ego", "lmot_tracker_set_ego",
     "lmot_debug_polar_grid", "lmot_debug_cell_index", "lmot_debug_label_grid", "lmot_selftest_atan2f",
@@ -232,19 +238,23 @@ class Lmot:
         return boxes[: nb.value].copy(), markers[: nb.value].copy()
 
     # ---- getOriginPoints + immUkfJpdaf -------------------------------------------------------------------
+    def _new_track_bufs(self, cap):
+        bufs = dict(targets=np.zeros((cap, 3), np.float32), vandyaw=np.zeros((cap, 2), np.float64),
+                    track_manage=np.zeros(cap, np.int32), is_static=np.zeros(cap, np.uint8), is_vis=np.zeros(cap, np.uint8),
+                    vis_bb=np.zeros((cap, 8, 3), np.float32), boxes=np.zeros((self.params.max_boxes, 8, 3), np.float32))
+        to = TrackOut()
+        to.cap = cap
+        to.targets = _fp(bufs["targets"]); to.vandyaw = bufs["vandyaw"].ctypes.data_as(C.POINTER(C.c_double))
+        to.track_manage = bufs["track_manage"].ctypes.data_as(C.POINTER(C.c_int32))
+        to.is_static = bufs["is_static"].ctypes.data_as(C.POINTER(C.c_uint8))
+        to.is_vis = bufs["is_vis"].ctypes.data_as(C.POINTER(C.c_uint8)); to.vis_bb = _fp(bufs["vis_bb"])
+        return to, bufs
+
     def _track_out(self, cap):
         """Output buffers are allocated once per (context, cap) and reused: the hot loop must not allocate megabytes."""
         cache = self.__dict__.setdefault("_out_cache", {})
         if cap not in cache:
-            bufs = dict(targets=np.zeros((cap, 3), np.float32), vandyaw=np.zeros((cap, 2), np.float64),
-                        track_manage=np.zeros(cap, np.int32), is_static=np.zeros(cap, np.uint8), is_vis=np.zeros(cap, np.uint8),
-                        vis_bb=np.zeros((cap, 8, 3), np.float32), boxes=np.zeros((self.params.max_boxes, 8, 3), np.float32))
-            to = TrackOut()
-            to.cap = cap
-            to.targets = _fp(bufs["targets"]); to.vandyaw = bufs["vandyaw"].ctypes.data_as(C.POINTER(C.c_double))
-            to.track_manage = bufs["track_manage"].ctypes.data_as(C.POINTER(C.c_int32))
-            to.is_static = bufs["is_static"].ctypes.data_as(C.POINTER(C.c_uint8))
-            to.is_vis = bufs["is_vis"].ctypes.data_as(C.POINTER(C.c_uint8)); to.vis_bb = _fp(bufs["vis_bb"])
+            to, bufs = self._new_track_bufs(cap)
             fo = FrameOut()
             fo.boxes = _fp(bufs["boxes"]); fo.max_boxes = self.params.max_boxes
             fo_nb = FrameOut()
@@ -445,6 +455,90 @@ class Lmot:
         s = arr[: n.value]
         return dict(poses=np.array([list(e.pose) for e in s], np.float32).reshape(-1, 3, 4),
                     **{k: np.array([getattr(e, k) for e in s], np.float32) for k in ("h_sensor", "t_hmin", "t_hmax", "sensor_height")})
+
+    # ---- independent sequences: one frame of each sequence per tick, one track table per sequence (lmot_seq_*) ---------------
+    def seq_open(self, n_seq: int, ring: int = 8):
+        """n_seq (1..8) empty sequences and a ring of `ring` ticks (n_seq = 0 frees the set); drains the context."""
+        self._chk(self.lib.lmot_seq_open(self.h, int(n_seq), int(ring)))
+
+    def seq_prepare(self, dev_frames):
+        """Marshal a tick's (device pointer, n) list ONCE for seq_dev (a timing loop must not build ctypes arrays on every call)."""
+        return self.batch_prepare(dev_frames)
+
+    @staticmethod
+    def seq_scalars(n_seq, values, default=0.0):
+        """Per-sequence doubles (timestamps / ego speeds / ego yaws) as the C array the seq_* calls take; one value is broadcast."""
+        if isinstance(values, C.Array):
+            return values
+        v = np.broadcast_to(np.asarray(default if values is None else values, np.float64), (n_seq,))
+        return (C.c_double * n_seq)(*[float(x) for x in v])
+
+    def _seq_call_args(self, ptrs_ns_n, timestamps, v_gps, yaw_gps):
+        ptrs, ns, S = ptrs_ns_n
+        return ptrs, ns, S, self.seq_scalars(S, timestamps), self.seq_scalars(S, v_gps), self.seq_scalars(S, yaw_gps)
+
+    def _seq_out(self, cap, want_boxes=True):
+        cache = self.__dict__.setdefault("_seq_cache", {})
+        if cap not in cache:
+            so = SeqOut()
+            sets = [self._new_track_bufs(cap) for _ in range(MAX_BATCH)]
+            for k, (to, bufs) in enumerate(sets):
+                so.seq[k].tracks = to
+                so.seq[k].max_boxes = self.params.max_boxes
+            cache[cap] = (so, sets)
+        so, sets = cache[cap]
+        for k, (_, bufs) in enumerate(sets):
+            so.seq[k].boxes = _fp(bufs["boxes"]) if want_boxes else None
+        return so, sets
+
+    def _seq_result(self, so, sets, want_boxes=True):
+        return [self._frame_result(so.seq[k], sets[k][1], want_boxes) for k in range(so.n_seq)]
+
+    def seq(self, frames, timestamps, v_gps=None, yaw_gps=None, cap: int | None = None):
+        """One tick, synchronous: `frames` = one (N_k, >=3) host array per sequence; timestamps / v_gps / yaw_gps per sequence.
+        -> list of per-sequence dicts as frame() returns."""
+        ptrs, ns, S, stride, keep = self._batch_args(frames, False)
+        so, sets = self._seq_out(cap or self.params.max_tracks)
+        ptrs, ns, S, ts, v, yaw = self._seq_call_args((ptrs, ns, S), timestamps, v_gps, yaw_gps)
+        self._chk(self.lib.lmot_seq(self.h, ptrs, ns, S, stride, ts, v, yaw, C.byref(so)))
+        return self._seq_result(so, sets)
+
+    def seq_submit(self, frames, timestamps, v_gps=None, yaw_gps=None):
+        ptrs, ns, S, stride, keep = self._batch_args(frames, False)
+        self._keep = keep          # the copies are asynchronous: the host arrays must outlive the call
+        ptrs, ns, S, ts, v, yaw = self._seq_call_args((ptrs, ns, S), timestamps, v_gps, yaw_gps)
+        self._chk(self.lib.lmot_seq_submit(self.h, ptrs, ns, S, stride, ts, v, yaw))
+
+    def seq_dev(self, dev_frames, timestamps, v_gps=None, yaw_gps=None):
+        """dev_frames = list of (device pointer, n) of stride-4 float frames, one per sequence (or a seq_prepare handle)."""
+        ptrs, ns, S, _, _ = self._batch_args(dev_frames, True)
+        ptrs, ns, S, ts, v, yaw = self._seq_call_args((ptrs, ns, S), timestamps, v_gps, yaw_gps)
+        self._chk(self.lib.lmot_seq_dev(self.h, ptrs, ns, S, ts, v, yaw))
+
+    def seq_collect(self, cap: int | None = None, want_boxes: bool = True):
+        so, sets = self._seq_out(cap or self.params.max_tracks, want_boxes)
+        self._chk(self.lib.lmot_seq_collect(self.h, C.byref(so)))
+        return self._seq_result(so, sets, want_boxes)
+
+    def seq_fetch(self, cap: int | None = None, want_boxes: bool = True):
+        so, sets = self._seq_out(cap or self.params.max_tracks, want_boxes)
+        self._chk(self.lib.lmot_seq_fetch(self.h, C.byref(so)))
+        return self._seq_result(so, sets, want_boxes)
+
+    def seq_tracker_reset(self, k: int):
+        self._chk(self.lib.lmot_seq_tracker_reset(self.h, int(k)))
+
+    def seq_tracker_dump(self, k: int) -> np.ndarray:
+        n = C.c_int(0)
+        self._chk(self.lib.lmot_seq_tracker_dump(self.h, int(k), None, 0, C.byref(n)))
+        out = np.zeros((max(n.value, 1), TRACK_DUMP_DOUBLES), np.float64)
+        self._chk(self.lib.lmot_seq_tracker_dump(self.h, int(k), out.ctypes.data_as(C.POINTER(C.c_double)), max(n.value, 1), C.byref(n)))
+        return out[: n.value]
+
+    def seq_tracker_get_ego(self, k: int) -> np.ndarray:
+        e = np.zeros(8, np.float64)
+        self._chk(self.lib.lmot_seq_tracker_get_ego(self.h, int(k), e.ctypes.data_as(C.POINTER(C.c_double))))
+        return e
 
     def tracker_reset(self):
         self._chk(self.lib.lmot_tracker_reset(self.h))

@@ -289,8 +289,8 @@ int copy_track_outputs(const Result* s, lmot_track_out* out) {
   return (wants && T > out->cap) ? LMOT_ERR_CAPACITY : LMOT_OK;      // a zero-initialised lmot_track_out asks for the counts only
 }
 
-// results of a finished frame from its pinned host block
-int collect_result(Ctx* c, Result* r, lmot_frame_out* out) {
+// results of a finished frame from its pinned host block; `trk`: the tracker whose step the block holds (nullptr: the context's own)
+int collect_result(Ctx* c, Result* r, lmot_frame_out* out, Tracker* trk = nullptr) {
   const double t0 = now_ns();
   LMOT_CUDA(c, cudaEventSynchronize(r->ev_done));
   const double t1 = now_ns();
@@ -308,7 +308,7 @@ int collect_result(Ctx* c, Result* r, lmot_frame_out* out) {
   }
   const int err = r->h_hdr[HDR_ERROR];
   const int warn = r->has_tracks ? r->h_hdr[HDR_WARN] : 0;
-  if (r->has_tracks) c->last_n_act = r->h_hdr[HDR_N_ACT];
+  if (r->has_tracks) (trk ? trk : &c->own)->last_n_act = r->h_hdr[HDR_N_ACT];
   if (out) {
     out->n_elevated = r->h_hdr[HDR_N_ELEV]; out->n_ground = r->h_hdr[HDR_N_GROUND];
     out->num_cluster = r->h_hdr[HDR_NUM_CLUSTER]; out->n_boxes = r->h_hdr[HDR_N_BOXES];
@@ -374,6 +374,52 @@ void result_destroy(Result* r) {
   if (r->ev_done) cudaEventDestroy(r->ev_done);
   for (int i = 0; i < 5; ++i) if (r->ev[i]) cudaEventDestroy(r->ev[i]);
   for (int i = 0; i < kMaxKernelEvents; ++i) if (r->kev[i]) cudaEventDestroy(r->kev[i]);
+}
+
+// ---- independent sequences (lmot_seq_*): S frame streams, one frame each per tick, S track tables ---------------------------------
+// Detection runs on the batch banks (batch_ensure) exactly as a batched tick without a sensor rig; the box lists are NOT concatenated:
+// sequence k's tracker reads slot k's own list and counters (seq_tracker_launch, tracker.cu).
+void seq_destroy(Ctx* c) {
+  for (int k = 0; k < c->n_seq; ++k) tracker_free(c->seq[k]);
+  for (int i = 0; i < c->seq_ring; ++i)
+    for (int k = 0; k < c->n_seq; ++k) result_destroy(&c->seq_ticks[i].blocks[k]);
+  delete[] c->seq_ticks;
+  c->seq_ticks = nullptr; c->seq_last = nullptr;
+  c->n_seq = 0; c->seq_ring = 0; c->seq_next = 0; c->seq_oldest = 0; c->seq_in_flight = 0;
+}
+
+// uncollected sequence ticks are dropped (after drain(): nothing is running)
+void seq_forget(Ctx* c) {
+  for (int i = 0; i < c->seq_ring; ++i) c->seq_ticks[i].in_flight = false;
+  c->seq_in_flight = 0;
+  c->seq_oldest = c->seq_next;
+}
+
+// next tick of the sequence ring; `drop_oldest` as acquire_result
+SeqTick* seq_acquire(Ctx* c, bool drop_oldest) {
+  SeqTick* t = &c->seq_ticks[c->seq_next];
+  if (t->in_flight) {
+    if (!drop_oldest) return nullptr;
+    cudaEventSynchronize(t->blocks[0].ev_done);
+    t->in_flight = false;
+    --c->seq_in_flight;
+    c->seq_oldest = (c->seq_next + 1) % c->seq_ring;
+  }
+  c->seq_next = (c->seq_next + 1) % c->seq_ring;
+  c->seq_last = t;
+  return t;
+}
+
+// the tick's results: blocks[0].ev_done is recorded after the one publish launch that writes every block
+int seq_collect_tick(Ctx* c, SeqTick* t, lmot_seq_out* out) {
+  LMOT_CUDA(c, cudaEventSynchronize(t->blocks[0].ev_done));
+  int rc = LMOT_OK;
+  if (out) out->n_seq = c->n_seq;
+  for (int k = 0; k < c->n_seq; ++k) {
+    const int r = collect_result(c, &t->blocks[k], out ? &out->seq[k] : nullptr, &c->seq[k]);
+    if (r < 0 ? (rc >= 0) : (rc == LMOT_OK)) rc = r;       // the first error, else the first warning
+  }
+  return rc;
 }
 
 int slot_create(Ctx* c, Slot* s, int index) {
@@ -508,7 +554,7 @@ int lmot_create(lmot_ctx** out, const lmot_params* params, int device) {
   for (int i = 0; i < c->n_results && rc == LMOT_OK; ++i) rc = result_create(c, &c->results[i]);
   for (int i = 0; i < c->n_slots && rc == LMOT_OK; ++i) rc = slot_create(c, &c->slots[i], i);
   c->last_res = &c->results[0];
-  if (rc == LMOT_OK) rc = tracker_alloc(c);
+  if (rc == LMOT_OK) rc = tracker_alloc(c, c->own);
   if (rc == LMOT_OK) rc = (cudaDeviceSynchronize() == cudaSuccess) ? LMOT_OK : LMOT_ERR_CUDA;
   if (rc != LMOT_OK) { lmot_destroy(h); return rc; }
   *out = h;
@@ -524,7 +570,8 @@ void lmot_destroy(lmot_ctx* ctx) {
   for (int i = 0; i < c->n_slots; ++i) slot_destroy(&c->slots[i]);
   batch_destroy(c);
   for (int i = 0; i < c->n_results; ++i) result_destroy(&c->results[i]);
-  tracker_free(c);
+  tracker_free(c->own);
+  seq_destroy(c);
   cudaFree(c->d_mt_raw);
   if (c->trk_stream) cudaStreamDestroy(c->trk_stream);
   if (c->pub_stream) cudaStreamDestroy(c->pub_stream);
@@ -731,7 +778,7 @@ int lmot_track_step(lmot_ctx* ctx, const float* boxes, int m, double timestamp_u
     for (int i = 0; i < s->res->n_kev; ++i) cudaEventElapsedTime(&c->kernel_ms[i], i == 0 ? s->res->ev[3] : s->res->kev[i - 1], s->res->kev[i]);
   }
   const int err = s->res->h_hdr[HDR_ERROR];
-  c->last_n_act = s->res->h_hdr[HDR_N_ACT];
+  c->own.last_n_act = s->res->h_hdr[HDR_N_ACT];
   rc = copy_track_outputs(s->res, out);
   return err ? err : (rc ? rc : s->res->h_hdr[HDR_WARN]);
 }
@@ -971,6 +1018,128 @@ int lmot_batch(lmot_ctx* ctx, const float* const* points, const int* n, int n_fr
   return lmot_batch_collect(ctx, out);
 }
 
+// ---------------------------------------------------------------------------------------------- independent sequences
+int lmot_seq_open(lmot_ctx* ctx, int n_seq, int ring) {
+  if (!ctx || n_seq < 0 || n_seq > kMaxBatch || (n_seq > 0 && (ring < 1 || ring > kMaxResults))) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  cudaSetDevice(c->device);
+  int rc = drain(c);
+  if (rc) return rc;
+  seq_destroy(c);
+  if (n_seq == 0) return LMOT_OK;
+  c->seq_ticks = new (std::nothrow) SeqTick[ring];
+  if (!c->seq_ticks) return LMOT_ERR_INVALID;
+  c->seq_ring = ring;
+  c->n_seq = n_seq;                    // (set before the allocations: seq_destroy frees whatever was allocated on failure)
+  for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = tracker_alloc(c, c->seq[k]);
+  for (int i = 0; i < ring && rc == LMOT_OK; ++i)
+    for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = result_create(c, &c->seq_ticks[i].blocks[k]);
+  if (rc == LMOT_OK) rc = (cudaDeviceSynchronize() == cudaSuccess) ? LMOT_OK : LMOT_ERR_CUDA;
+  if (rc) seq_destroy(c);
+  return rc;
+}
+
+static int seq_common(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride, bool host, const double* ts,
+                      const double* v, const double* yaw) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  if (c->n_seq == 0 || n_seq != c->n_seq || !points || !n || !ts || !v || !yaw) return LMOT_ERR_INVALID;
+  if (c->timing) return LMOT_ERR_STATE;
+  cudaSetDevice(c->device);
+  for (int i = 0; i < n_seq; ++i) {
+    if (n[i] < 0 || (n[i] > 0 && !points[i])) return LMOT_ERR_INVALID;
+    if (n[i] > c->max_points) return LMOT_ERR_CAPACITY;
+    if (!host && n[i] > 0 && (reinterpret_cast<uintptr_t>(points[i]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies need 16-byte alignment
+  }
+  if (host && (stride < 3 || c->seq_in_flight >= c->seq_ring)) return stride < 3 ? LMOT_ERR_INVALID : LMOT_ERR_STATE;
+  int rc = batch_ensure(c, n_seq);
+  if (rc) return rc;
+  SeqTick* t = seq_acquire(c, !host);
+  if (!t) return LMOT_ERR_STATE;
+  const int b = c->next_bank;
+  c->next_bank = (c->next_bank + 1) % kBatchBanks;
+  Slot* k = &c->bank[b];
+  Slot* sl[kMaxBatch];
+  const float4* pp[kMaxBatch];
+  for (int i = 0; i < n_seq; ++i) sl[i] = &c->bslots[b * c->batch_frames + i];
+  cudaStream_t st = sl[0]->stream;
+  // the bank's previous tick must have been consumed by the tracker; device frames: ordered after the caller's stream
+  LMOT_CUDA(c, cudaStreamWaitEvent(st, k->ev_trk_done, 0));
+  if (host) {
+    for (int i = 0; i < n_seq; ++i) {
+      if ((rc = upload_points(c, sl[i], st, points[i], n[i], stride, sl[i]->d_points))) return rc;
+      pp[i] = sl[i]->d_points;
+    }
+  } else {
+    LMOT_CUDA(c, cudaEventRecord(k->ev_fork, c->stream));
+    LMOT_CUDA(c, cudaStreamWaitEvent(st, k->ev_fork, 0));
+    for (int i = 0; i < n_seq; ++i) pp[i] = reinterpret_cast<const float4*>(points[i]);
+  }
+  struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
+  for (int i = 0; i < n_seq; ++i) { t->blocks[i].n_kev = 0; t->blocks[i].batch_frames = 0; t->blocks[i].has_tracks = true; }
+  k->res = &t->blocks[0]; sl[0]->res = &t->blocks[0];
+  // detection: the batched launches of lmot_batch_* without a rig; each frame's last box-fitting CTA (or, global_frame, its
+  // boxes_to_global CTA) posts its own slot's semaphore, which the tick's gate kernel polls
+  const bool gf = c->prm.global_frame != 0;
+  if ((rc = ground_launch_batch(c, sl, n_seq, pp, n, st, true, false, c->fuse_ccl, false, nullptr))) return rc;
+  if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, n_seq, st))) return rc;
+  if ((rc = boxfit_launch_batch(c, sl, n_seq, st, n, !gf, nullptr))) return rc;
+  if (gf && (rc = seq_global_launch(c, sl, n_seq, st, ts, v, yaw))) return rc;
+  LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, st));
+  if ((rc = seq_tracker_launch(c, sl, t, n_seq, ts, v, yaw))) return rc;
+  LMOT_CUDA(c, cudaEventRecord(t->blocks[0].ev_done, c->pub_stream));
+  LMOT_CUDA(c, cudaEventRecord(k->ev_trk_done, c->pub_stream));
+  if (!t->in_flight) { t->in_flight = true; ++c->seq_in_flight; }
+  return LMOT_OK;
+}
+
+int lmot_seq_submit(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride_floats, const double* timestamp_us,
+                    const double* v_gps, const double* yaw_gps) {
+  return seq_common(ctx, points, n, n_seq, stride_floats, true, timestamp_us, v_gps, yaw_gps);
+}
+
+int lmot_seq_dev(lmot_ctx* ctx, const float* const* d_points, const int* n, int n_seq, const double* timestamp_us, const double* v_gps,
+                 const double* yaw_gps) {
+  return seq_common(ctx, d_points, n, n_seq, 4, false, timestamp_us, v_gps, yaw_gps);
+}
+
+int lmot_seq_collect(lmot_ctx* ctx, lmot_seq_out* out) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  if (c->seq_in_flight <= 0) return LMOT_ERR_STATE;
+  SeqTick* t = &c->seq_ticks[c->seq_oldest];
+  int guard = 0;
+  while (!t->in_flight && guard++ < c->seq_ring) { c->seq_oldest = (c->seq_oldest + 1) % c->seq_ring; t = &c->seq_ticks[c->seq_oldest]; }
+  if (!t->in_flight) return LMOT_ERR_STATE;
+  const int rc = seq_collect_tick(c, t, out);
+  t->in_flight = false;
+  --c->seq_in_flight;
+  c->seq_oldest = (c->seq_oldest + 1) % c->seq_ring;
+  return rc;
+}
+
+int lmot_seq_fetch(lmot_ctx* ctx, lmot_seq_out* out) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  if (!c->seq_last) return LMOT_ERR_STATE;
+  const int rc = seq_collect_tick(c, c->seq_last, out);
+  seq_forget(c);
+  return rc;
+}
+
+int lmot_seq(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride_floats, const double* timestamp_us,
+             const double* v_gps, const double* yaw_gps, lmot_seq_out* out) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  if (c->seq_in_flight > 0) {          // uncollected ticks are dropped, as lmot_batch drops uncollected results
+    LMOT_CUDA(c, cudaEventSynchronize(c->seq_last->blocks[0].ev_done));    // (ticks are published in submission order)
+    seq_forget(c);
+  }
+  int rc = lmot_seq_submit(ctx, points, n, n_seq, stride_floats, timestamp_us, v_gps, yaw_gps);
+  if (rc) return rc;
+  return lmot_seq_collect(ctx, out);
+}
+
 // ---------------------------------------------------------------------------------------------- device-side hand-over (multi-GPU)
 // Several sensor streams on several GPUs feeding ONE tracker (SURVEY.md §8e, host/shared_tracker.cpp): detection leaves its box
 // list on the device, the lists travel rank to rank with NCCL, the owner folds them in WITHOUT a host bounce.
@@ -985,7 +1154,7 @@ int lmot_detect_boxes_dev(lmot_ctx* ctx, const float** d_boxes, const int** d_n_
 
 int lmot_tracker_counters_dev(lmot_ctx* ctx, int** d_n_tracks) {
   if (!ctx || !d_n_tracks) return LMOT_ERR_INVALID;
-  *d_n_tracks = ctx->c.d_trk_counters + CNT_N_TRACKS;
+  *d_n_tracks = ctx->c.own.d_trk_counters + CNT_N_TRACKS;
   return LMOT_OK;
 }
 
@@ -1063,15 +1232,15 @@ int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n) {
 int lmot_tracker_table_received(lmot_ctx* ctx, int n) {
   if (!ctx || n < 0 || n > ctx->c.prm.max_tracks) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  c->h_trk_counters[CNT_N_TRACKS] = n;
-  c->act_valid = false;
-  c->last_trk_res = nullptr;
+  c->own.h_trk_counters[CNT_N_TRACKS] = n;
+  c->own.act_valid = false;
+  c->own.last_trk_res = nullptr;
   return LMOT_OK;
 }
 
 int lmot_origin_points(lmot_ctx* ctx, double timestamp_us, double v_gps, double yaw_gps, double out6[6]) {
   if (!ctx || !out6) return LMOT_ERR_INVALID;
-  TrackerHost h = ctx->c.th;                       // peek: fold on a copy
+  TrackerHost h = ctx->c.own.th;                       // peek: fold on a copy
   origin_points_fold(h, timestamp_us, v_gps, yaw_gps);
   out6[0] = h.egoPoint[0]; out6[1] = h.egoPoint[1]; out6[2] = h.egoPoint[2];
   out6[3] = h.egoPoint[0]; out6[4] = h.egoPoint[1]; out6[5] = h.egoPoint[2] + M_PI / 2;
@@ -1079,37 +1248,40 @@ int lmot_origin_points(lmot_ctx* ctx, double timestamp_us, double v_gps, double 
 }
 
 // ---------------------------------------------------------------------------------------------- tracker state
-int lmot_tracker_reset(lmot_ctx* ctx) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
+static int tracker_reset(Ctx* c, Tracker& t) {
   int rc = drain(c);
   if (rc) return rc;
-  c->th = TrackerHost();
-  c->act_valid = false;
-  LMOT_CUDA(c, cudaMemsetAsync(c->d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
+  t.th = TrackerHost();
+  t.act_valid = false;
+  LMOT_CUDA(c, cudaMemsetAsync(t.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
   return LMOT_OK;
 }
 
-static int fetch_trk_counters(Ctx* c) {
+int lmot_tracker_reset(lmot_ctx* ctx) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  return tracker_reset(&ctx->c, ctx->c.own);
+}
+
+static int fetch_trk_counters(Ctx* c, Tracker& t) {
   int rc = drain(c);
   if (rc) return rc;
-  LMOT_CUDA(c, cudaMemcpyAsync(c->h_trk_counters, c->d_trk_counters, CNT_COUNT * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  LMOT_CUDA(c, cudaMemcpyAsync(t.h_trk_counters, t.d_trk_counters, CNT_COUNT * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
   return LMOT_OK;
 }
 
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n) {
   if (!ctx || !n) return LMOT_ERR_INVALID;
-  int rc = fetch_trk_counters(&ctx->c);
+  int rc = fetch_trk_counters(&ctx->c, ctx->c.own);
   if (rc) return rc;
-  *n = ctx->c.h_trk_counters[CNT_N_TRACKS];
+  *n = ctx->c.own.h_trk_counters[CNT_N_TRACKS];
   return LMOT_OK;
 }
 
 int lmot_tracker_table(lmot_ctx* ctx, void** dev_ptr, int* bytes_per_track, int* capacity) {
   if (!ctx) return LMOT_ERR_INVALID;
-  if (dev_ptr) *dev_ptr = ctx->c.d_tracks;
+  if (dev_ptr) *dev_ptr = ctx->c.own.d_tracks;
   if (bytes_per_track) *bytes_per_track = (int)sizeof(TrackState);
   if (capacity) *capacity = ctx->c.prm.max_tracks;
   return LMOT_OK;
@@ -1120,9 +1292,9 @@ int lmot_tracker_set_num_tracks(lmot_ctx* ctx, int n) {
   Ctx* c = &ctx->c;
   int rc = drain(c);
   if (rc) return rc;
-  c->h_trk_counters[CNT_N_TRACKS] = n;
-  c->act_valid = false;
-  LMOT_CUDA(c, cudaMemcpyAsync(c->d_trk_counters + CNT_N_TRACKS, c->h_trk_counters + CNT_N_TRACKS, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  c->own.h_trk_counters[CNT_N_TRACKS] = n;
+  c->own.act_valid = false;
+  LMOT_CUDA(c, cudaMemcpyAsync(c->own.d_trk_counters + CNT_N_TRACKS, c->own.h_trk_counters + CNT_N_TRACKS, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
   return LMOT_OK;
 }
@@ -1132,17 +1304,15 @@ enum { D_TRACKNUM = 0, D_LIFETIME = 1, D_STATIC = 2, D_VIS = 3, D_X = 4, D_P = 2
        D_K = 145, D_BESTYAW = 175, D_BBYAW = 176, D_BBAREA = 177, D_DISTINIT = 178, D_XMERGEYAW = 179, D_INITMEAS = 180,
        D_VELON = 182, D_VELO = 183, D_BBN = 186, D_BB = 187, D_BESTBBN = 211, D_BESTBB = 212, D_TOTAL = LMOT_TRACK_DUMP_DOUBLES };
 
-int lmot_tracker_dump(lmot_ctx* ctx, double* dumps, int cap, int* n_out) {
-  if (!ctx || cap < 0) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  int rc = fetch_trk_counters(c);
+static int tracker_dump(Ctx* c, Tracker& trk, double* dumps, int cap, int* n_out) {
+  int rc = fetch_trk_counters(c, trk);
   if (rc) return rc;
-  const int T = c->h_trk_counters[CNT_N_TRACKS];
+  const int T = trk.h_trk_counters[CNT_N_TRACKS];
   if (n_out) *n_out = T;
   const int n = T < cap ? T : cap;
   if (n == 0 || !dumps) return LMOT_OK;
   std::vector<TrackState> h((size_t)n);
-  LMOT_CUDA(c, cudaMemcpyAsync(h.data(), c->d_tracks, (size_t)n * sizeof(TrackState), cudaMemcpyDeviceToHost, c->stream));
+  LMOT_CUDA(c, cudaMemcpyAsync(h.data(), trk.d_tracks, (size_t)n * sizeof(TrackState), cudaMemcpyDeviceToHost, c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
   for (int i = 0; i < n; ++i) {
     const TrackState& t = h[i];
@@ -1161,6 +1331,11 @@ int lmot_tracker_dump(lmot_ctx* ctx, double* dumps, int cap, int* n_out) {
     d[D_BESTBBN] = t.nBest; for (int p = 0; p < t.nBest && p < 8; ++p) for (int q = 0; q < 3; ++q) d[D_BESTBB + 3 * p + q] = t.bestBBox[p][q];
   }
   return T > cap ? LMOT_ERR_CAPACITY : LMOT_OK;
+}
+
+int lmot_tracker_dump(lmot_ctx* ctx, double* dumps, int cap, int* n_out) {
+  if (!ctx || cap < 0) return LMOT_ERR_INVALID;
+  return tracker_dump(&ctx->c, ctx->c.own, dumps, cap, n_out);
 }
 
 int lmot_tracker_load(lmot_ctx* ctx, const double* dumps, int n, int init, double timestamp_us, double ego_velo,
@@ -1187,15 +1362,15 @@ int lmot_tracker_load(lmot_ctx* ctx, const double* dumps, int n, int init, doubl
     t.nBBox = (int)d[D_BBN]; for (int p = 0; p < t.nBBox && p < 8; ++p) for (int q = 0; q < 3; ++q) t.BBox[p][q] = (float)d[D_BB + 3 * p + q];
     t.nBest = (int)d[D_BESTBBN]; for (int p = 0; p < t.nBest && p < 8; ++p) for (int q = 0; q < 3; ++q) t.bestBBox[p][q] = (float)d[D_BESTBB + 3 * p + q];
   }
-  if (n > 0) LMOT_CUDA(c, cudaMemcpyAsync(c->d_tracks, h.data(), (size_t)n * sizeof(TrackState), cudaMemcpyHostToDevice, c->stream));
-  c->h_trk_counters[CNT_N_TRACKS] = n;
-  LMOT_CUDA(c, cudaMemsetAsync(c->d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
-  LMOT_CUDA(c, cudaMemcpyAsync(c->d_trk_counters + CNT_N_TRACKS, c->h_trk_counters + CNT_N_TRACKS, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  if (n > 0) LMOT_CUDA(c, cudaMemcpyAsync(c->own.d_tracks, h.data(), (size_t)n * sizeof(TrackState), cudaMemcpyHostToDevice, c->stream));
+  c->own.h_trk_counters[CNT_N_TRACKS] = n;
+  LMOT_CUDA(c, cudaMemsetAsync(c->own.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
+  LMOT_CUDA(c, cudaMemcpyAsync(c->own.d_trk_counters + CNT_N_TRACKS, c->own.h_trk_counters + CNT_N_TRACKS, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->act_valid = false;
-  c->th = TrackerHost();
-  c->th.init = init != 0; c->th.timestamp = timestamp_us; c->th.egoVelo = ego_velo; c->th.egoYaw = ego_yaw;
-  c->th.egoPreYaw = ego_pre_yaw; c->th.egoPoint[2] = ego_point_yaw;
+  c->own.act_valid = false;
+  c->own.th = TrackerHost();
+  c->own.th.init = init != 0; c->own.th.timestamp = timestamp_us; c->own.th.egoVelo = ego_velo; c->own.th.egoYaw = ego_yaw;
+  c->own.th.egoPreYaw = ego_pre_yaw; c->own.th.egoPoint[2] = ego_point_yaw;
   // (like the oracle's ref_tracker_load, which clears egoDeltaHis_: the dead-reckoning fold restarts from (0, 0, -pi/2) and
   //  ego_point_yaw is only egoPoints_[0][2] until the next step recomputes it.  A checkpoint that must keep the accumulated ego
   //  pose restores it with lmot_tracker_set_ego.)
@@ -1203,11 +1378,34 @@ int lmot_tracker_load(lmot_ctx* ctx, const double* dumps, int n, int init, doubl
 }
 
 // the frame-level scalars of getOriginPoints / immUkfJpdaf (imm_ukf_jpda.cpp:19-24,56-58) incl. the accumulated dead-reckoning pose
-int lmot_tracker_get_ego(lmot_ctx* ctx, double ego8[8]) {
-  if (!ctx || !ego8) return LMOT_ERR_INVALID;
-  const TrackerHost& h = ctx->c.th;
+static void get_ego(const TrackerHost& h, double ego8[8]) {
   ego8[0] = h.init ? 1.0 : 0.0; ego8[1] = h.timestamp; ego8[2] = h.egoVelo; ego8[3] = h.egoYaw; ego8[4] = h.egoPreYaw;
   ego8[5] = h.fold[0]; ego8[6] = h.fold[1]; ego8[7] = h.fold[2];
+}
+
+int lmot_tracker_get_ego(lmot_ctx* ctx, double ego8[8]) {
+  if (!ctx || !ego8) return LMOT_ERR_INVALID;
+  get_ego(ctx->c.own.th, ego8);
+  return LMOT_OK;
+}
+
+// ---- per-sequence state (lmot_seq_*)
+int lmot_seq_tracker_reset(lmot_ctx* ctx, int k) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  const int rc = tracker_reset(c, c->seq[k]);
+  seq_forget(c);
+  return rc;
+}
+
+int lmot_seq_tracker_dump(lmot_ctx* ctx, int k, double* dumps, int cap, int* n_out) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq || cap < 0) return LMOT_ERR_INVALID;
+  return tracker_dump(&ctx->c, ctx->c.seq[k], dumps, cap, n_out);
+}
+
+int lmot_seq_tracker_get_ego(lmot_ctx* ctx, int k, double ego8[8]) {
+  if (!ctx || !ego8 || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  get_ego(ctx->c.seq[k].th, ego8);
   return LMOT_OK;
 }
 
@@ -1216,7 +1414,7 @@ int lmot_tracker_set_ego(lmot_ctx* ctx, const double ego8[8]) {
   Ctx* c = &ctx->c;
   int rc = drain(c);
   if (rc) return rc;
-  TrackerHost& h = c->th;
+  TrackerHost& h = c->own.th;
   h.init = ego8[0] != 0.0; h.timestamp = ego8[1]; h.egoVelo = ego8[2]; h.egoYaw = ego8[3]; h.egoPreYaw = ego8[4];
   h.fold[0] = ego8[5]; h.fold[1] = ego8[6]; h.fold[2] = ego8[7];
   h.egoPoint[0] = h.fold[0]; h.egoPoint[1] = h.fold[1]; h.egoPoint[2] = h.fold[2];

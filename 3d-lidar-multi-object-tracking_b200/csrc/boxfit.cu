@@ -896,7 +896,7 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
   for (int i = 0; i < F; ++i) { const int t = (n_upper[i] + kTile - 1) / kTile; if (t > tiles) tiles = t; }
   const size_t sh = (size_t)K1 * sizeof(int);
   FitBatch B;
-  for (int i = 0; i < F; ++i) { fit_frame_of(slots[i], B.f[i], post_sem && F == 1); if (rig) B.f[i].sensor_height = rig[i].sensor_height; }
+  for (int i = 0; i < F; ++i) { fit_frame_of(slots[i], B.f[i], post_sem); if (rig) B.f[i].sensor_height = rig[i].sensor_height; }
   for (int i = F; i < kMaxBatch; ++i) B.f[i] = B.f[0];
   Slot* s0 = slots[0];
   if (tiles > 0) tile_hist_kernel<<<dim3(tiles, F), kTile, sh, st>>>(B, c->prm.max_clusters);     // + segment offsets by its last CTA per frame

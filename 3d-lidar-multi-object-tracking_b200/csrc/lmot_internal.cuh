@@ -171,6 +171,38 @@ constexpr int kMaxSlots = 8;
 constexpr int kBatchBanks = 2;                       // batched ticks: detection of tick t+1 overlaps the tracker of tick t
 constexpr int kMaxResults = 64;
 
+// One track table and everything the tracker chain carries from one step to the next.  The context's own tracker is one; every
+// sequence of lmot_seq_* (an independent frame stream) is another.
+struct Tracker {
+  TrackerHost th;
+  TrackState* d_tracks = nullptr;      // [max_tracks] append-only table; dead tracks keep their slot
+  int* d_trk_counters = nullptr;       // [CNT_COUNT] CNT_N_TRACKS / CNT_N_VIS / CNT_ERROR of the track table
+  int* h_trk_counters = nullptr;       // pinned mirror
+  unsigned* d_gate = nullptr;          // [max_tracks][gate_words] chi-square gate bits per (track, box)
+  unsigned* d_setter = nullptr;        // [max_tracks][gate_words] boxes this track marks as matched
+  int* d_first_setter = nullptr;       // [max_boxes] lowest track index that matched the box (INT_MAX = unmatched)
+  uint8_t* d_skip = nullptr;           // [max_tracks] track did not reach measurementValidation this frame
+  int* d_new_num = nullptr;            // [max_tracks] mergeOverSegmentation: largest visible container index per live track
+  int* d_live_list = nullptr;          // [max_tracks] scratch: indices of live tracks
+  int* d_vis_list = nullptr;           // [max_tracks] scratch: indices of tracks with a visible box
+  int* d_act_list = nullptr;           // [max_tracks] tracks to visit next frame (built by spawn_output_kernel)
+  double4* d_pos = nullptr;            // [max_tracks] packed (x, y, yaw, -) of every track's merged state
+  void* d_summary = nullptr;           // [max_tracks] ActSummary (tracker.cu): what TC needs of each active track, written by TB
+  int* d_meas_n = nullptr;             // [max_tracks] TA -> TB: number of gated boxes of the track (-1: not provided)
+  void* d_meas_ctr = nullptr;          // [max_tracks][32] double2: centre points of the first 32 gated boxes, box order
+  unsigned* d_tc_seq = nullptr;        // tracker steps completed (counted by spawn_output_kernel, polled by publish_kernel)
+  unsigned tc_launched = 0;            // host: tracker steps launched
+  bool act_valid = false;              // false after the table was written from the host: rebuilt before the next step
+  Result* last_trk_res = nullptr;      // result block of the previous tracker step (its device copy seeds the next one)
+  int last_n_act = 0;                  // active tracks (live or visible) in the last result the host has read: picks spawn_output_kernel's variant
+};
+
+// one tick of lmot_seq_*: a result block per sequence; blocks[0].ev_done marks the whole tick published
+struct SeqTick {
+  Result blocks[kMaxBatch];
+  bool in_flight = false;
+};
+
 struct Ctx {
   lmot_params prm;
   int device = 0;
@@ -210,32 +242,19 @@ struct Ctx {
   Result* last_res = nullptr;
 
   // ---- tracker
-  TrackerHost th;
+  Tracker own;                         // the context's own track table (lmot_frame*, lmot_batch*, lmot_track_step*, lmot_tracker_*)
   cudaStream_t trk_stream = nullptr;
   cudaStream_t pub_stream = nullptr;   // device -> host publication of finished frames
-  int* d_act_list = nullptr;           // [max_tracks] tracks to visit next frame (built by spawn_output_kernel)
-  double4* d_pos = nullptr;            // [max_tracks] packed (x, y, yaw, -) of every track's merged state
-  int* d_meas_n = nullptr;             // [max_tracks] TA -> TB: number of gated boxes of the track (-1: not provided)
-  void* d_meas_ctr = nullptr;          // [max_tracks][32] double2: centre points of the first 32 gated boxes, box order
-  unsigned* d_tc_seq = nullptr;        // tracker steps completed (counted by spawn_output_kernel, polled by publish_kernel)
-  unsigned tc_launched = 0;            // host: tracker steps launched
-  void* d_summary = nullptr;           // [max_tracks] ActSummary (tracker.cu): what TC needs of each active track, written by TB
-  Result* last_trk_res = nullptr;      // result block of the previous tracker step (its device copy seeds the next one)
-  bool act_valid = false;              // false after the table was written from the host: rebuilt before the next step
   int trk_ctas = 0, gate_words = 0;
-  int last_n_act = 0;          // active tracks (live or visible) in the last result the host has read: picks spawn_output_kernel's variant
   bool tc_wide = false;
   int tc_force = -1;           // LMOT_TC_WIDE: -1 by count, 0 / 1 pinned
-  TrackState* d_tracks = nullptr;      // [max_tracks] append-only table; dead tracks keep their slot
-  int* d_trk_counters = nullptr;       // [CNT_COUNT] CNT_N_TRACKS / CNT_N_VIS / CNT_ERROR of the track table
-  int* h_trk_counters = nullptr;       // pinned mirror
-  unsigned* d_gate = nullptr;          // [max_tracks][gate_words] chi-square gate bits per (track, box)
-  unsigned* d_setter = nullptr;        // [max_tracks][gate_words] boxes this track marks as matched
-  int* d_first_setter = nullptr;       // [max_boxes] lowest track index that matched the box (INT_MAX = unmatched)
-  uint8_t* d_skip = nullptr;           // [max_tracks] track did not reach measurementValidation this frame
-  int* d_new_num = nullptr;            // [max_tracks] mergeOverSegmentation: largest visible container index per live track
-  int* d_live_list = nullptr;          // [max_tracks] scratch: indices of live tracks
-  int* d_vis_list = nullptr;           // [max_tracks] scratch: indices of tracks with a visible box
+  // ---- independent sequences (lmot_seq_*): one Tracker each, a ring of ticks of n_seq result blocks; detection on the batch banks
+  int n_seq = 0;
+  Tracker seq[kMaxBatch];
+  SeqTick* seq_ticks = nullptr;        // [seq_ring]
+  int seq_ring = 0, seq_next = 0, seq_oldest = 0, seq_in_flight = 0;
+  SeqTick* seq_last = nullptr;         // most recent submission (lmot_seq_fetch)
+  bool seq_wide = false;               // spawn_output_kernel's variant of the sequence ticks (largest last_n_act of the set)
 
   // ---- timing
   bool timing = false;
@@ -306,14 +325,17 @@ int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const
 int boxes_concat_launch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, float* d_boxes, int* d_counters, int* d_frame_counts, int* det_sem,
                         const lmot_sensor* rig = nullptr);
 void origin_points_fold(TrackerHost& h, double timestamp, double v_gps, double yaw_gps);
-int tracker_alloc(Ctx* c);
-void tracker_free(Ctx* c);
+int tracker_alloc(Ctx* c, Tracker& t);
+void tracker_free(Tracker& t);
 // boxes: device float[M][8][3] with M in det_counters[CNT_N_BOXES]; results into the slot's pinned host block
 int tracker_launch(Ctx* c, Slot* s, cudaStream_t st, const float* d_boxes, const int* det_counters, double timestamp, double v_gps,
                    double yaw_gps, bool gate = false, bool* gated = nullptr);   // gate: wait for the slot's detection semaphore on the device (tracker.cu)
 int boxes_to_global_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, const int* det_counters, double timestamp, double v_gps,
                            double yaw_gps, bool post_sem);
 int tracker_publish(Ctx* c, Result* r, cudaStream_t st);            // device block of r -> pinned host block
+// sequence ticks: frame k of the tick = slot sl[k] -> track table c->seq[k] -> tick->blocks[k] (tracker.cu)
+int seq_global_launch(Ctx* c, Slot* const* sl, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw);
+int seq_tracker_launch(Ctx* c, Slot* const* sl, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw);
 int boxes_publish(Ctx* c, Slot* s, Result* r, cudaStream_t st);     // detection-only: slot box list -> pinned host block
 
 }  // namespace lmot

@@ -165,21 +165,34 @@ __device__ void ukf_initialize(TrackState& t, double zx, double zy) {   // UKF::
 // polls it, THEN lets TA's CTAs come (they hold SM resources, so they must not be resident while anything they wait for is
 // still outside this stream: a ground kernel that needs every one of its CTAs co-resident could starve), then waits for the
 // previous tracker step.  TA's own griddepcontrol.wait returns when this kernel has completed, i.e. when both (a) and (b) hold.
+__device__ __forceinline__ void wait_det_sem(const int* det_sem, unsigned spin_limit) {
+  unsigned spin = 0;
+  int v;
+  do {
+    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(det_sem) : "memory");
+    if (spin_limit && ++spin > spin_limit) __trap();       // detection never finished (seconds): fail loudly instead of hanging the stream (0: wait for ever)
+  } while (v < 1);
+}
+
 __global__ void __launch_bounds__(32)
 tracker_gate_kernel(const int* __restrict__ det_sem, unsigned spin_limit) {
-  if (threadIdx.x == 0) {
-    unsigned spin = 0;
-    int v;
-    do {
-      asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(det_sem) : "memory");
-      if (spin_limit && ++spin > spin_limit) __trap();       // detection never finished (seconds): fail loudly instead of hanging the stream (0: wait for ever)
-    } while (v < 1);
-  }
+  if (threadIdx.x == 0) wait_det_sem(det_sem, spin_limit);
   __syncwarp();
   pdl_launch_dependents();
   // (no griddepcontrol.wait: this kernel may finish before the previous frame's spawn_output_kernel does.  TA's CTAs, resident from
   // here on, wait for that step through its completion counter -- one L2 poll after spawn_output_kernel's last store instead of two
   // grid-completion hops (TC -> this kernel -> TA).)
+}
+
+// Sequence ticks (lmot_seq_*): lane k waits for sequence k's detection (its slot's semaphore, posted by box fitting or by
+// boxes_to_global_seq_kernel), so TA's CTAs are released only once every frame of the tick has its boxes.
+struct GateSeq { const int* sem[kMaxBatch]; int n; };
+
+__global__ void __launch_bounds__(32)
+tracker_gate_seq_kernel(const __grid_constant__ GateSeq g, unsigned spin_limit) {
+  if ((int)threadIdx.x < g.n) wait_det_sem(g.sem[threadIdx.x], spin_limit);
+  __syncwarp();
+  pdl_launch_dependents();
 }
 
 // ------------------------------------------------------------------------------------------------ TA
@@ -201,12 +214,13 @@ struct TAShared {
 
 __device__ __forceinline__ double bcast(double v, int src) { return __shfl_sync(0xFFFFFFFFu, v, src); }
 
-__global__ void __launch_bounds__(kTAThreads, 4)     // <= 128 registers: a CTA (16 K registers) fits on an SM next to a ground-kernel CTA (47 K)
-imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
-                        double dt, unsigned* __restrict__ gate, unsigned* __restrict__ setter, int* __restrict__ first_setter,
-                        uint8_t* __restrict__ skip, int words, const int* __restrict__ act_list,
-                        int* __restrict__ meas_n, double2* __restrict__ meas_ctr,
-                        const unsigned* __restrict__ tc_seq, unsigned tc_want, unsigned spin_limit) {
+// TA for one track table; the single-stream kernel and the sequence kernel (one table per blockIdx.y) share it
+__device__ __forceinline__ void
+imm_predict_gate_body(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
+                      double dt, unsigned* __restrict__ gate, unsigned* __restrict__ setter, int* __restrict__ first_setter,
+                      uint8_t* __restrict__ skip, int words, const int* __restrict__ act_list,
+                      int* __restrict__ meas_n, double2* __restrict__ meas_ctr,
+                      const unsigned* __restrict__ tc_seq, unsigned tc_want, unsigned spin_limit) {
   __shared__ TAShared sh;
   pdl_wait();                              // (gated launch: the gate kernel, hence this frame's detection, is complete)
   pdl_launch_dependents();                 // TB's CTAs may line up behind this grid
@@ -527,6 +541,33 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
   }
 }
 
+__global__ void __launch_bounds__(kTAThreads, 4)     // <= 128 registers: a CTA (16 K registers) fits on an SM next to a ground-kernel CTA (47 K)
+imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
+                        double dt, unsigned* __restrict__ gate, unsigned* __restrict__ setter, int* __restrict__ first_setter,
+                        uint8_t* __restrict__ skip, int words, const int* __restrict__ act_list,
+                        int* __restrict__ meas_n, double2* __restrict__ meas_ctr,
+                        const unsigned* __restrict__ tc_seq, unsigned tc_want, unsigned spin_limit) {
+  imm_predict_gate_body(tracks, trk, det, boxes, dt, gate, setter, first_setter, skip, words, act_list, meas_n, meas_ctr, tc_seq, tc_want, spin_limit);
+}
+
+// Sequence ticks: one launch steps every sequence's table, sequence = blockIdx.y.  `run` = 0: the sequence is on its compat first
+// frame, where the single-stream path launches neither TA nor TB (its CTAs leave at once; TC spawns the quirk's track).
+struct TASeq {
+  TrackState* tracks; const int* trk; const int* det; const float* boxes; double dt;
+  unsigned* gate; unsigned* setter; int* first_setter; uint8_t* skip; const int* act_list;
+  int* meas_n; double2* meas_ctr; const unsigned* tc_seq; unsigned tc_want; int run;
+};
+struct TASeqParams { TASeq s[kMaxBatch]; int words; unsigned spin_limit; };
+static_assert(sizeof(TASeqParams) <= 4096, "kernel parameter block");
+
+__global__ void __launch_bounds__(kTAThreads, 4)
+imm_predict_gate_seq_kernel(const __grid_constant__ TASeqParams p) {
+  const TASeq& q = p.s[blockIdx.y];
+  if (!q.run) return;
+  imm_predict_gate_body(q.tracks, q.trk, q.det, q.boxes, q.dt, q.gate, q.setter, q.first_setter, q.skip, p.words, q.act_list, q.meas_n,
+                        q.meas_ctr, q.tc_seq, q.tc_want, p.spin_limit);
+}
+
 // ------------------------------------------------------------------------------------------------ TB
 
 // What TC needs of an active track, 128 bytes per entry of the active list, written by TB (which has the record staged in
@@ -637,11 +678,11 @@ struct TBShared {
 // runs on different warps: the PDA update of the three motion models (each its own S^-1, Gaussian kernels, beta weights,
 // K nu, covariance update -- identical code, different model) on warps 0..2, measurement bookkeeping / box association /
 // updateBB on warp 3; then warp 0 alone: association likelihoods, mode probabilities, merged estimate.
-__global__ void __launch_bounds__(kTBThreads)
-imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
-                  const unsigned* __restrict__ gate, const int* __restrict__ first_setter, const uint8_t* __restrict__ skip,
-                  int words, const int* __restrict__ act_list, ActSummary* __restrict__ summary,
-                  const int* __restrict__ meas_n, const double2* __restrict__ meas_ctr) {
+__device__ __forceinline__ void
+imm_update_body(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
+                const unsigned* __restrict__ gate, const int* __restrict__ first_setter, const uint8_t* __restrict__ skip,
+                int words, const int* __restrict__ act_list, ActSummary* __restrict__ summary,
+                const int* __restrict__ meas_n, const double2* __restrict__ meas_ctr) {
   extern __shared__ unsigned short s_list[];              // indices of the gated boxes, in box order
   __shared__ TBShared sh;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -954,6 +995,29 @@ imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, 
       if (lane < 16) reinterpret_cast<unsigned long long*>(&summary[q])[lane] = reinterpret_cast<const unsigned long long*>(&sh.sum)[lane];
     }
   }
+}
+
+__global__ void __launch_bounds__(kTBThreads)
+imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
+                  const unsigned* __restrict__ gate, const int* __restrict__ first_setter, const uint8_t* __restrict__ skip,
+                  int words, const int* __restrict__ act_list, ActSummary* __restrict__ summary,
+                  const int* __restrict__ meas_n, const double2* __restrict__ meas_ctr) {
+  imm_update_body(tracks, trk, det, boxes, gate, first_setter, skip, words, act_list, summary, meas_n, meas_ctr);
+}
+
+// sequence ticks: sequence = blockIdx.y, `run` as for TA
+struct TBSeq {
+  TrackState* tracks; const int* trk; const int* det; const float* boxes; const unsigned* gate; const int* first_setter;
+  const uint8_t* skip; const int* act_list; ActSummary* summary; const int* meas_n; const double2* meas_ctr; int run;
+};
+struct TBSeqParams { TBSeq s[kMaxBatch]; int words; };
+static_assert(sizeof(TBSeqParams) <= 4096, "kernel parameter block");
+
+__global__ void __launch_bounds__(kTBThreads)
+imm_update_seq_kernel(const __grid_constant__ TBSeqParams p) {
+  const TBSeq& q = p.s[blockIdx.y];
+  if (!q.run) return;
+  imm_update_body(q.tracks, q.trk, q.det, q.boxes, q.gate, q.first_setter, q.skip, p.words, q.act_list, q.summary, q.meas_n, q.meas_ctr);
 }
 
 // ------------------------------------------------------------------------------------------------ TC: over-segmentation test
@@ -1357,12 +1421,12 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
 //     active tracks only.
 // `full` (first step after the table was written from the host): everything is rebuilt from the records.
 template <int NT>
-__global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
-spawn_output_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det, const float* __restrict__ boxes,
-                    const float* __restrict__ boxes_pub, int* __restrict__ first_setter, int* __restrict__ imax_arr, int* __restrict__ vis_list,
-                    uint8_t* __restrict__ has5_arr, int first_frame, int compat_first, double ego_yaw, int max_tracks, OutPtrs o,
-                    OutPtrs prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
-                    int* __restrict__ det_sem, unsigned* __restrict__ tc_seq) {
+__device__ __forceinline__ void
+spawn_output_body(TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det, const float* __restrict__ boxes,
+                  const float* __restrict__ boxes_pub, int* __restrict__ first_setter, int* __restrict__ imax_arr, int* __restrict__ vis_list,
+                  uint8_t* __restrict__ has5_arr, int first_frame, int compat_first, double ego_yaw, int max_tracks, const OutPtrs& o,
+                  const OutPtrs& prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
+                  int* __restrict__ det_sem, unsigned* __restrict__ tc_seq) {
   pdl_launch_dependents();                 // the next frame's gate kernel may become resident
   pdl_wait();                              // TB has finished
   // every exit: this step's results are complete -> count it (release); publish_kernel, on its own stream, polls the count
@@ -1601,6 +1665,35 @@ spawn_output_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int*
   }
 }
 
+template <int NT>
+__global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
+spawn_output_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det, const float* __restrict__ boxes,
+                    const float* __restrict__ boxes_pub, int* __restrict__ first_setter, int* __restrict__ imax_arr, int* __restrict__ vis_list,
+                    uint8_t* __restrict__ has5_arr, int first_frame, int compat_first, double ego_yaw, int max_tracks, OutPtrs o,
+                    OutPtrs prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
+                    int* __restrict__ det_sem, unsigned* __restrict__ tc_seq) {
+  spawn_output_body<NT>(tracks, trk, det, boxes, boxes_pub, first_setter, imax_arr, vis_list, has5_arr, first_frame, compat_first, ego_yaw,
+                        max_tracks, o, prev, full, act_list, pos, summary, det_sem, tc_seq);
+}
+
+// sequence ticks: one CTA per sequence (blockIdx.x); each picks the fast or the general path from its own sequence's counts
+struct TCSeq {
+  TrackState* tracks; int* trk; int* det; const float* boxes; const float* boxes_pub; int* first_setter; int* imax_arr; int* vis_list;
+  uint8_t* has5_arr; int* act_list; double4* pos; const ActSummary* summary; int* det_sem; unsigned* tc_seq;
+  OutPtrs o, prev;
+  double ego_yaw; int first_frame, full;
+};
+struct TCSeqParams { TCSeq s[kMaxBatch]; int compat_first, max_tracks; };
+static_assert(sizeof(TCSeqParams) <= 4096, "kernel parameter block");
+
+template <int NT>
+__global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
+spawn_output_seq_kernel(const __grid_constant__ TCSeqParams p) {
+  const TCSeq& q = p.s[blockIdx.x];
+  spawn_output_body<NT>(q.tracks, q.trk, q.det, q.boxes, q.boxes_pub, q.first_setter, q.imax_arr, q.vis_list, q.has5_arr, q.first_frame,
+                        p.compat_first, q.ego_yaw, p.max_tracks, q.o, q.prev, q.full, q.act_list, q.pos, q.summary, q.det_sem, q.tc_seq);
+}
+
 // device copy of a frame's results -> pinned, device-mapped host block.  16 bytes per thread, consecutive threads ->
 // consecutive addresses: every store instruction of a warp is four full 128-byte lines on the PCIe side.
 __device__ __forceinline__ void copy16(void* dst, const void* src, size_t bytes, int tid, int nthreads) {
@@ -1619,8 +1712,8 @@ __device__ __forceinline__ void xf_apply(const Xf2& M, float x, float y, float z
 }
 
 constexpr int kPubThreads = 128;    // small on purpose: it may sit on an SM polling while detection kernels need that SM's registers
-__global__ void __launch_bounds__(kPubThreads)
-publish_kernel(OutPtrs d, OutPtrs h, const unsigned* __restrict__ tc_seq, unsigned want, unsigned spin_limit, Xf2 back) {
+__device__ __forceinline__ void
+publish_body(const OutPtrs& d, const OutPtrs& h, const unsigned* __restrict__ tc_seq, unsigned want, unsigned spin_limit, const Xf2& back) {
   const int tid = threadIdx.x;
   if (tid == 0) {              // wait until `want` tracker steps have completed (spawn_output_kernel counts them)
     unsigned spin = 0, v;
@@ -1648,17 +1741,48 @@ publish_kernel(OutPtrs d, OutPtrs h, const unsigned* __restrict__ tc_seq, unsign
   copy16(h.hdr, d.hdr, HDR_COUNT * sizeof(int), tid, kPubThreads);
 }
 
+__global__ void __launch_bounds__(kPubThreads)
+publish_kernel(OutPtrs d, OutPtrs h, const unsigned* __restrict__ tc_seq, unsigned want, unsigned spin_limit, Xf2 back) {
+  publish_body(d, h, tc_seq, want, spin_limit, back);
+}
+
+// sequence ticks: one CTA per sequence, each waits for its own sequence's step count
+struct PubSeq { OutPtrs d, h; const unsigned* tc_seq; unsigned want; Xf2 back; };
+struct PubSeqParams { PubSeq s[kMaxBatch]; unsigned spin_limit; };
+static_assert(sizeof(PubSeqParams) <= 4096, "kernel parameter block");
+
+__global__ void __launch_bounds__(kPubThreads)
+publish_seq_kernel(const __grid_constant__ PubSeqParams p) {
+  const PubSeq& q = p.s[blockIdx.x];
+  publish_body(q.d, q.h, q.tc_seq, q.want, p.spin_limit, q.back);
+}
+
 // lmot_params.global_frame: the frame's boxes (sensor frame) -> the dead-reckoned global frame the tracker works in
 // (tracking/main.cpp:142-158: pcl_ros::transformPointCloud("/global", bBoxes[i], ...)).  One CTA; also takes over posting the
 // detection semaphore from box fitting, because the tracker must not start before this list exists.
-__global__ void __launch_bounds__(256)
-boxes_to_global_kernel(const float* __restrict__ boxes, const int* __restrict__ det, float* __restrict__ boxes_g, Xf2 fwd, int* __restrict__ det_sem) {
+__device__ __forceinline__ void
+boxes_to_global_body(const float* __restrict__ boxes, const int* __restrict__ det, float* __restrict__ boxes_g, const Xf2& fwd, int* __restrict__ det_sem) {
   const int M = det[CNT_N_BOXES];
   for (int i = threadIdx.x; i < M * 8; i += 256) xf_apply(fwd, boxes[3 * i], boxes[3 * i + 1], boxes[3 * i + 2], boxes_g[3 * i], boxes_g[3 * i + 1], boxes_g[3 * i + 2]);
   if (det_sem) {
     __syncthreads();
     if (threadIdx.x == 0) { __threadfence(); atomicAdd(det_sem, 1); }
   }
+}
+
+__global__ void __launch_bounds__(256)
+boxes_to_global_kernel(const float* __restrict__ boxes, const int* __restrict__ det, float* __restrict__ boxes_g, Xf2 fwd, int* __restrict__ det_sem) {
+  boxes_to_global_body(boxes, det, boxes_g, fwd, det_sem);
+}
+
+// sequence ticks: one CTA per sequence, each with its own ego pose; posts its sequence's slot semaphore
+struct GlobalSeq { const float* boxes; const int* det; float* boxes_g; int* det_sem; Xf2 fwd; };
+struct GlobalSeqParams { GlobalSeq s[kMaxBatch]; };
+
+__global__ void __launch_bounds__(256)
+boxes_to_global_seq_kernel(const __grid_constant__ GlobalSeqParams p) {
+  const GlobalSeq& q = p.s[blockIdx.x];
+  boxes_to_global_body(q.boxes, q.det, q.boxes_g, q.fwd, q.det_sem);
 }
 
 // detection-only submissions: the box list of the slot -> the result's host block
@@ -1680,48 +1804,52 @@ __global__ void fill_int_kernel(int* p, int n, int v) {
 
 }  // namespace
 
-int tracker_alloc(Ctx* c) {
+int tracker_alloc(Ctx* c, Tracker& t) {
   const int TC = c->prm.max_tracks, MB = c->prm.max_boxes;
   c->gate_words = (MB + 31) / 32;
-  LMOT_CUDA(c, cudaMalloc(&c->d_tracks, (size_t)TC * sizeof(TrackState)));
-  LMOT_CUDA(c, cudaMemsetAsync(c->d_tracks, 0, (size_t)TC * sizeof(TrackState), c->trk_stream));
-  LMOT_CUDA(c, cudaMalloc(&c->d_trk_counters, CNT_COUNT * sizeof(int)));
-  LMOT_CUDA(c, cudaMemsetAsync(c->d_trk_counters, 0, CNT_COUNT * sizeof(int), c->trk_stream));
-  LMOT_CUDA(c, cudaHostAlloc(&c->h_trk_counters, CNT_COUNT * sizeof(int), cudaHostAllocDefault));
-  LMOT_CUDA(c, cudaMalloc(&c->d_gate, (size_t)TC * c->gate_words * sizeof(unsigned)));
-  LMOT_CUDA(c, cudaMalloc(&c->d_setter, (size_t)TC * c->gate_words * sizeof(unsigned)));
-  LMOT_CUDA(c, cudaMalloc(&c->d_first_setter, (size_t)MB * sizeof(int)));
-  LMOT_CUDA(c, cudaMalloc(&c->d_skip, TC));
-  LMOT_CUDA(c, cudaMalloc(&c->d_new_num, (size_t)TC * sizeof(int)));
-  LMOT_CUDA(c, cudaMalloc(&c->d_live_list, (size_t)TC * sizeof(int)));
-  LMOT_CUDA(c, cudaMalloc(&c->d_vis_list, (size_t)TC * sizeof(int)));
-  LMOT_CUDA(c, cudaMalloc(&c->d_act_list, (size_t)TC * sizeof(int)));
-  LMOT_CUDA(c, cudaMalloc(&c->d_pos, (size_t)TC * sizeof(double4)));
-  LMOT_CUDA(c, cudaMalloc(&c->d_summary, (size_t)TC * sizeof(ActSummary)));
-  LMOT_CUDA(c, cudaMalloc(&c->d_meas_n, (size_t)TC * sizeof(int)));
-  LMOT_CUDA(c, cudaMemsetAsync(c->d_meas_n, 0xFF, (size_t)TC * sizeof(int), c->trk_stream));
-  LMOT_CUDA(c, cudaMalloc(&c->d_meas_ctr, (size_t)TC * 32 * sizeof(double2)));
-  LMOT_CUDA(c, cudaMemsetAsync(c->d_meas_ctr, 0, (size_t)TC * 32 * sizeof(double2), c->trk_stream));
-  LMOT_CUDA(c, cudaMalloc(&c->d_tc_seq, sizeof(unsigned)));
-  LMOT_CUDA(c, cudaMemsetAsync(c->d_tc_seq, 0, sizeof(unsigned), c->trk_stream));
-  c->tc_launched = 0;
-  LMOT_CUDA(c, cudaMemsetAsync(c->d_pos, 0, (size_t)TC * sizeof(double4), c->trk_stream));
-  c->last_trk_res = nullptr;
-  c->act_valid = false;
-  fill_int_kernel<<<(MB + 255) / 256, 256, 0, c->trk_stream>>>(c->d_first_setter, MB, INT_MAX);
+  LMOT_CUDA(c, cudaMalloc(&t.d_tracks, (size_t)TC * sizeof(TrackState)));
+  LMOT_CUDA(c, cudaMemsetAsync(t.d_tracks, 0, (size_t)TC * sizeof(TrackState), c->trk_stream));
+  LMOT_CUDA(c, cudaMalloc(&t.d_trk_counters, CNT_COUNT * sizeof(int)));
+  LMOT_CUDA(c, cudaMemsetAsync(t.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->trk_stream));
+  LMOT_CUDA(c, cudaHostAlloc(&t.h_trk_counters, CNT_COUNT * sizeof(int), cudaHostAllocDefault));
+  LMOT_CUDA(c, cudaMalloc(&t.d_gate, (size_t)TC * c->gate_words * sizeof(unsigned)));
+  LMOT_CUDA(c, cudaMalloc(&t.d_setter, (size_t)TC * c->gate_words * sizeof(unsigned)));
+  LMOT_CUDA(c, cudaMalloc(&t.d_first_setter, (size_t)MB * sizeof(int)));
+  LMOT_CUDA(c, cudaMalloc(&t.d_skip, TC));
+  LMOT_CUDA(c, cudaMalloc(&t.d_new_num, (size_t)TC * sizeof(int)));
+  LMOT_CUDA(c, cudaMalloc(&t.d_live_list, (size_t)TC * sizeof(int)));
+  LMOT_CUDA(c, cudaMalloc(&t.d_vis_list, (size_t)TC * sizeof(int)));
+  LMOT_CUDA(c, cudaMalloc(&t.d_act_list, (size_t)TC * sizeof(int)));
+  LMOT_CUDA(c, cudaMalloc(&t.d_pos, (size_t)TC * sizeof(double4)));
+  LMOT_CUDA(c, cudaMalloc(&t.d_summary, (size_t)TC * sizeof(ActSummary)));
+  LMOT_CUDA(c, cudaMalloc(&t.d_meas_n, (size_t)TC * sizeof(int)));
+  LMOT_CUDA(c, cudaMemsetAsync(t.d_meas_n, 0xFF, (size_t)TC * sizeof(int), c->trk_stream));
+  LMOT_CUDA(c, cudaMalloc(&t.d_meas_ctr, (size_t)TC * 32 * sizeof(double2)));
+  LMOT_CUDA(c, cudaMemsetAsync(t.d_meas_ctr, 0, (size_t)TC * 32 * sizeof(double2), c->trk_stream));
+  LMOT_CUDA(c, cudaMalloc(&t.d_tc_seq, sizeof(unsigned)));
+  LMOT_CUDA(c, cudaMemsetAsync(t.d_tc_seq, 0, sizeof(unsigned), c->trk_stream));
+  t.tc_launched = 0;
+  LMOT_CUDA(c, cudaMemsetAsync(t.d_pos, 0, (size_t)TC * sizeof(double4), c->trk_stream));
+  t.last_trk_res = nullptr;
+  t.act_valid = false;
+  fill_int_kernel<<<(MB + 255) / 256, 256, 0, c->trk_stream>>>(t.d_first_setter, MB, INT_MAX);
   LMOT_CUDA(c, cudaGetLastError());
   const size_t sh = (size_t)c->gate_words * 32 * sizeof(unsigned short);
   LMOT_CUDA(c, cudaFuncSetAttribute(imm_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
   LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
   LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
-  c->last_n_act = 0; c->tc_wide = false;
+  LMOT_CUDA(c, cudaFuncSetAttribute(imm_update_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
+  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
+  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
+  t.last_n_act = 0;
   return LMOT_OK;
 }
 
-void tracker_free(Ctx* c) {
-  cudaFree(c->d_tracks); cudaFree(c->d_trk_counters); cudaFree(c->d_gate); cudaFree(c->d_setter); cudaFree(c->d_first_setter);
-  cudaFree(c->d_skip); cudaFree(c->d_new_num); cudaFree(c->d_live_list); cudaFree(c->d_vis_list); cudaFree(c->d_act_list); cudaFree(c->d_pos); cudaFree(c->d_summary); cudaFree(c->d_tc_seq); cudaFree(c->d_meas_n); cudaFree(c->d_meas_ctr);
-  if (c->h_trk_counters) cudaFreeHost(c->h_trk_counters);
+void tracker_free(Tracker& t) {
+  cudaFree(t.d_tracks); cudaFree(t.d_trk_counters); cudaFree(t.d_gate); cudaFree(t.d_setter); cudaFree(t.d_first_setter);
+  cudaFree(t.d_skip); cudaFree(t.d_new_num); cudaFree(t.d_live_list); cudaFree(t.d_vis_list); cudaFree(t.d_act_list); cudaFree(t.d_pos); cudaFree(t.d_summary); cudaFree(t.d_tc_seq); cudaFree(t.d_meas_n); cudaFree(t.d_meas_ctr);
+  if (t.h_trk_counters) cudaFreeHost(t.h_trk_counters);
+  t = Tracker();
 }
 
 // getOriginPoints (imm_ukf_jpda.cpp:74-172) is scalar bookkeeping on three doubles per frame; it stays on the host.
@@ -1778,7 +1906,7 @@ void global_frame_xf(const double ego[3], Xf2* fwd, Xf2* back) {
 // post_sem: post the slot's detection semaphore afterwards (frame pipeline)
 int boxes_to_global_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, const int* det_counters, double timestamp, double v_gps,
                            double yaw_gps, bool post_sem) {
-  TrackerHost peek = c->th;
+  TrackerHost peek = c->own.th;
   origin_points_fold(peek, timestamp, v_gps, yaw_gps);
   Xf2 fwd, back;
   global_frame_xf(peek.egoPoint, &fwd, &back);
@@ -1790,12 +1918,12 @@ int boxes_to_global_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_box
 
 int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, const int* det_counters, double timestamp, double v_gps,
                    double yaw_gps, bool gate, bool* gated) {
-  origin_points_fold(c->th, timestamp, v_gps, yaw_gps);
+  origin_points_fold(c->own.th, timestamp, v_gps, yaw_gps);
   // global_frame: the tracker reads the list boxes_to_global_launch prepared, the results carry the sensor-frame list
   const float* d_boxes_pub = d_boxes;
-  if (c->prm.global_frame) { d_boxes = sl->d_boxes_g; Xf2 fwd; global_frame_xf(c->th.egoPoint, &fwd, &sl->res->back); }
+  if (c->prm.global_frame) { d_boxes = sl->d_boxes_g; Xf2 fwd; global_frame_xf(c->own.th.egoPoint, &fwd, &sl->res->back); }
   else sl->res->back.on = 0;
-  TrackerHost& h = c->th;
+  TrackerHost& h = c->own.th;
   Result* r = sl->res;
   OutPtrs o{r->d_targets, r->d_vandyaw, r->d_manage, r->d_static, r->d_vis, r->d_visbb, r->d_hdr, r->d_boxes};
   int* det = const_cast<int*>(det_counters);
@@ -1807,15 +1935,15 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
   if (gate && !use_gate) LMOT_CUDA(c, cudaStreamWaitEvent(st, sl->ev_det_done, 0));
   int* det_sem = gate ? sl->d_det_sem : nullptr;
   if (gated) *gated = use_gate;
-  const int full = c->act_valid ? 0 : 1;   // the table was written from the host since the last frame: rebuild the side arrays
+  const int full = c->own.act_valid ? 0 : 1;   // the table was written from the host since the last frame: rebuild the side arrays
   if (full) {
-    LMOT_CUDA(c, cudaMemsetAsync(c->d_trk_counters + CNT_N_ACT, 0, sizeof(int), st));
-    build_active_kernel<<<(c->prm.max_tracks + 255) / 256, 256, 0, st>>>(c->d_tracks, c->d_trk_counters, c->d_act_list);
-    c->act_valid = true;
+    LMOT_CUDA(c, cudaMemsetAsync(c->own.d_trk_counters + CNT_N_ACT, 0, sizeof(int), st));
+    build_active_kernel<<<(c->prm.max_tracks + 255) / 256, 256, 0, st>>>(c->own.d_tracks, c->own.d_trk_counters, c->own.d_act_list);
+    c->own.act_valid = true;
   }
-  Result* pr = (full || !c->last_trk_res) ? r : c->last_trk_res;
+  Result* pr = (full || !c->own.last_trk_res) ? r : c->own.last_trk_res;
   OutPtrs po{pr->d_targets, pr->d_vandyaw, pr->d_manage, pr->d_static, pr->d_vis, pr->d_visbb, pr->d_hdr, pr->d_boxes};
-  c->last_trk_res = r;
+  c->own.last_trk_res = r;
   if (!(first && compat)) {
     const double dt = first ? 0.0 : (timestamp - h.timestamp) / 1000000.0;     // :807
     const size_t sh = (size_t)c->gate_words * 32 * sizeof(unsigned short);
@@ -1830,9 +1958,9 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
       }
       cudaLaunchConfig_t ac = {};
       ac.gridDim = dim3(c->trk_ctas); ac.blockDim = dim3(kTAThreads); ac.dynamicSmemBytes = 0; ac.stream = st; ac.attrs = &pa; ac.numAttrs = 1;
-      LMOT_CUDA(c, cudaLaunchKernelEx(&ac, imm_predict_gate_kernel, c->d_tracks, (const int*)c->d_trk_counters, (const int*)det, d_boxes, dt,
-                                      c->d_gate, c->d_setter, c->d_first_setter, c->d_skip, c->gate_words, (const int*)c->d_act_list,
-                                      c->d_meas_n, reinterpret_cast<double2*>(c->d_meas_ctr), (const unsigned*)c->d_tc_seq, c->tc_launched, c->spin_limit));
+      LMOT_CUDA(c, cudaLaunchKernelEx(&ac, imm_predict_gate_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes, dt,
+                                      c->own.d_gate, c->own.d_setter, c->own.d_first_setter, c->own.d_skip, c->gate_words, (const int*)c->own.d_act_list,
+                                      c->own.d_meas_n, reinterpret_cast<double2*>(c->own.d_meas_ctr), (const unsigned*)c->own.d_tc_seq, c->own.tc_launched, c->spin_limit));
     }
     kernel_mark(c, sl, st);
     // TB and TC: programmatic dependent launches (their CTAs wait on the device for the preceding grid, see pdl_wait); timing
@@ -1843,10 +1971,10 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(c->trk_ctas); cfg.blockDim = dim3(kTBThreads); cfg.dynamicSmemBytes = sh; cfg.stream = st;
     cfg.attrs = &pdl; cfg.numAttrs = 1;
-    LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_kernel, c->d_tracks, (const int*)c->d_trk_counters, (const int*)det, d_boxes,
-                                    (const unsigned*)c->d_gate, (const int*)c->d_first_setter, (const uint8_t*)c->d_skip, c->gate_words,
-                                    (const int*)c->d_act_list, reinterpret_cast<ActSummary*>(c->d_summary),
-                                    (const int*)c->d_meas_n, reinterpret_cast<const double2*>(c->d_meas_ctr)));
+    LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes,
+                                    (const unsigned*)c->own.d_gate, (const int*)c->own.d_first_setter, (const uint8_t*)c->own.d_skip, c->gate_words,
+                                    (const int*)c->own.d_act_list, reinterpret_cast<ActSummary*>(c->own.d_summary),
+                                    (const int*)c->own.d_meas_n, reinterpret_cast<const double2*>(c->own.d_meas_ctr)));
     kernel_mark(c, sl, st);
   }
   {
@@ -1856,17 +1984,17 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
     // variant: one active track per thread on the fast path.  The host only knows the active count of the last result it has read
     // (a few frames old inside the pipeline; the count moves by a handful per frame): switch early, with hysteresis.  A count above
     // the variant's width runs the kernel's general path -- slower, same results.
-    if (c->last_n_act > 208) c->tc_wide = true;
-    else if (c->last_n_act < 144) c->tc_wide = false;
+    if (c->own.last_n_act > 208) c->tc_wide = true;
+    else if (c->own.last_n_act < 144) c->tc_wide = false;
     const bool wide = c->tc_force >= 0 ? c->tc_force != 0 : c->tc_wide;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(1); cfg.blockDim = dim3(wide ? kTCWide : kTCThreads); cfg.stream = st;
     cfg.dynamicSmemBytes = wide ? sizeof(TCFastShared<kTCWide>) : sizeof(TCFastShared<kTCThreads>);
     cfg.attrs = &pdl; cfg.numAttrs = 1;
-    LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_kernel<kTCWide> : spawn_output_kernel<kTCThreads>, c->d_tracks, c->d_trk_counters, det, d_boxes, d_boxes_pub, c->d_first_setter, c->d_new_num,
-                                    c->d_vis_list, c->d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->d_act_list,
-                                    c->d_pos, reinterpret_cast<const ActSummary*>(c->d_summary), det_sem, c->d_tc_seq));
-    ++c->tc_launched;
+    LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_kernel<kTCWide> : spawn_output_kernel<kTCThreads>, c->own.d_tracks, c->own.d_trk_counters, det, d_boxes, d_boxes_pub, c->own.d_first_setter, c->own.d_new_num,
+                                    c->own.d_vis_list, c->own.d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->own.d_act_list,
+                                    c->own.d_pos, reinterpret_cast<const ActSummary*>(c->own.d_summary), det_sem, c->own.d_tc_seq));
+    ++c->own.tc_launched;
   }
   kernel_mark(c, sl, st);
   LMOT_CUDA(c, cudaGetLastError());
@@ -1880,13 +2008,113 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
 int tracker_publish(Ctx* c, Result* r, cudaStream_t st) {
   OutPtrs d{r->d_targets, r->d_vandyaw, r->d_manage, r->d_static, r->d_vis, r->d_visbb, r->d_hdr, r->d_boxes};
   OutPtrs h{r->h_targets, r->h_vandyaw, r->h_manage, r->h_static, r->h_vis, r->h_visbb, r->h_hdr, r->h_boxes};
-  publish_kernel<<<1, kPubThreads, 0, st>>>(d, h, c->d_tc_seq, c->tc_launched, c->spin_limit, r->back);
+  publish_kernel<<<1, kPubThreads, 0, st>>>(d, h, c->own.d_tc_seq, c->own.tc_launched, c->spin_limit, r->back);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
 }
 
 int boxes_publish(Ctx* c, Slot* s, Result* r, cudaStream_t st) {
   publish_boxes_kernel<<<1, 256, 0, st>>>(s->d_boxes, s->d_counters, r->h_boxes);
+  LMOT_CUDA(c, cudaGetLastError());
+  return LMOT_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- sequence ticks (lmot_seq_*)
+// Sequence k of a tick: slot sl[k]'s box list and counters, track table c->seq[k], result block tick->blocks[k].  Every launch
+// below covers all S sequences; per-sequence arguments travel in __grid_constant__ parameter blocks.
+
+// global_frame: sequence k's sensor-frame boxes -> sl[k]->d_boxes_g with THIS tick's ego pose of sequence k (peeked:
+// seq_tracker_launch folds it), posting sl[k]'s detection semaphore
+int seq_global_launch(Ctx* c, Slot* const* sl, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw) {
+  GlobalSeqParams p{};
+  for (int k = 0; k < S; ++k) {
+    TrackerHost peek = c->seq[k].th;
+    origin_points_fold(peek, ts[k], v[k], yaw[k]);
+    Xf2 back;
+    global_frame_xf(peek.egoPoint, &p.s[k].fwd, &back);
+    p.s[k].boxes = sl[k]->d_boxes; p.s[k].det = sl[k]->d_counters; p.s[k].boxes_g = sl[k]->d_boxes_g; p.s[k].det_sem = sl[k]->d_det_sem;
+  }
+  boxes_to_global_seq_kernel<<<S, 256, 0, st>>>(p);
+  LMOT_CUDA(c, cudaGetLastError());
+  return LMOT_OK;
+}
+
+// gate -> TA -> TB -> TC once for all S sequences on the tracker stream (programmatic dependent launches, as the single-stream
+// chain), then one publish launch on the publish stream.  The caller records the tick's events on the publish stream afterwards.
+int seq_tracker_launch(Ctx* c, Slot* const* sl, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw) {
+  cudaStream_t st = c->trk_stream;
+  const int compat = c->prm.oracle_compat_first_frame ? 1 : 0;
+  const bool gf = c->prm.global_frame != 0;
+  GateSeq g{};
+  TASeqParams ta{};
+  TBSeqParams tb{};
+  TCSeqParams tcp{};
+  PubSeqParams pub{};
+  g.n = S;
+  ta.words = c->gate_words; ta.spin_limit = c->spin_limit;
+  tb.words = c->gate_words;
+  tcp.compat_first = compat; tcp.max_tracks = c->prm.max_tracks;
+  pub.spin_limit = c->spin_limit;
+  int n_act_max = 0;
+  for (int k = 0; k < S; ++k) {
+    Tracker& t = c->seq[k];
+    Slot* s = sl[k];
+    Result* r = &tick->blocks[k];
+    const int first = t.th.init ? 0 : 1;
+    const double dt = first ? 0.0 : (ts[k] - t.th.timestamp) / 1000000.0;     // :807, from this sequence's own previous stamp
+    origin_points_fold(t.th, ts[k], v[k], yaw[k]);
+    if (gf) { Xf2 fwd; global_frame_xf(t.th.egoPoint, &fwd, &r->back); }
+    else r->back.on = 0;
+    const float* boxes = gf ? s->d_boxes_g : s->d_boxes;
+    const int full = t.act_valid ? 0 : 1;
+    if (full) {
+      LMOT_CUDA(c, cudaMemsetAsync(t.d_trk_counters + CNT_N_ACT, 0, sizeof(int), st));
+      build_active_kernel<<<(c->prm.max_tracks + 255) / 256, 256, 0, st>>>(t.d_tracks, t.d_trk_counters, t.d_act_list);
+      t.act_valid = true;
+    }
+    Result* pr = (full || !t.last_trk_res) ? r : t.last_trk_res;
+    t.last_trk_res = r;
+    const int run = (first && compat) ? 0 : 1;
+    ActSummary* sum = reinterpret_cast<ActSummary*>(t.d_summary);
+    double2* mc = reinterpret_cast<double2*>(t.d_meas_ctr);
+    g.sem[k] = s->d_det_sem;
+    ta.s[k] = TASeq{t.d_tracks, t.d_trk_counters, s->d_counters, boxes, dt, t.d_gate, t.d_setter, t.d_first_setter, t.d_skip, t.d_act_list,
+                    t.d_meas_n, mc, t.d_tc_seq, t.tc_launched, run};
+    tb.s[k] = TBSeq{t.d_tracks, t.d_trk_counters, s->d_counters, boxes, t.d_gate, t.d_first_setter, t.d_skip, t.d_act_list, sum, t.d_meas_n, mc, run};
+    OutPtrs o{r->d_targets, r->d_vandyaw, r->d_manage, r->d_static, r->d_vis, r->d_visbb, r->d_hdr, r->d_boxes};
+    OutPtrs po{pr->d_targets, pr->d_vandyaw, pr->d_manage, pr->d_static, pr->d_vis, pr->d_visbb, pr->d_hdr, pr->d_boxes};
+    tcp.s[k] = TCSeq{t.d_tracks, t.d_trk_counters, s->d_counters, boxes, s->d_boxes, t.d_first_setter, t.d_new_num, t.d_vis_list, t.d_skip,
+                     t.d_act_list, t.d_pos, sum, s->d_det_sem, t.d_tc_seq, o, po, t.th.egoPoint[2], first, full};
+    ++t.tc_launched;
+    OutPtrs h{r->h_targets, r->h_vandyaw, r->h_manage, r->h_static, r->h_vis, r->h_visbb, r->h_hdr, r->h_boxes};
+    pub.s[k] = PubSeq{o, h, t.d_tc_seq, t.tc_launched, r->back};
+    if (t.last_n_act > n_act_max) n_act_max = t.last_n_act;
+    t.th.timestamp = ts[k];
+    t.th.egoPreYaw = t.th.egoYaw;
+    t.th.init = true;
+  }
+  cudaLaunchAttribute pdl;
+  pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  pdl.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.stream = st; cfg.attrs = &pdl; cfg.numAttrs = 1;
+  cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); cfg.dynamicSmemBytes = 0;
+  LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, tracker_gate_seq_kernel, g, c->spin_limit));
+  // the single-stream chain's CTA count, shared by the sequences (grid-stride over each sequence's active tracks)
+  const int gx = (c->trk_ctas + S - 1) / S;
+  cfg.gridDim = dim3(gx, S); cfg.blockDim = dim3(kTAThreads); cfg.dynamicSmemBytes = 0;
+  LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_predict_gate_seq_kernel, ta));
+  cfg.gridDim = dim3(gx, S); cfg.blockDim = dim3(kTBThreads); cfg.dynamicSmemBytes = (size_t)c->gate_words * 32 * sizeof(unsigned short);
+  LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_seq_kernel, tb));
+  // spawn_output_kernel's variant for the whole launch from the largest active count of the set (hysteresis as tracker_launch);
+  // either variant is correct for any count
+  if (n_act_max > 208) c->seq_wide = true;
+  else if (n_act_max < 144) c->seq_wide = false;
+  const bool wide = c->tc_force >= 0 ? c->tc_force != 0 : c->seq_wide;
+  cfg.gridDim = dim3(S); cfg.blockDim = dim3(wide ? kTCWide : kTCThreads);
+  cfg.dynamicSmemBytes = wide ? sizeof(TCFastShared<kTCWide>) : sizeof(TCFastShared<kTCThreads>);
+  LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_kernel<kTCWide> : spawn_output_seq_kernel<kTCThreads>, tcp));
+  publish_seq_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(pub);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
 }

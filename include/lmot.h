@@ -284,6 +284,51 @@ int lmot_default_sensor(const lmot_params* p, lmot_sensor* out);      /* identit
 int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n);
 int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n);   /* *n = sensors set; copies min(n, cap) of them */
 
+/* ---- independent sequences: up to LMOT_MAX_BATCH frame streams per tick, each with its OWN track table ---------------------------
+ * A sequence is an independent frame stream (one vehicle, one replayed log): it has its own track table, its own getOriginPoints
+ * state (timestamp, ego velocity and yaw, dead-reckoning fold, first-frame flag), its own global_frame pose and its own result block.
+ * One tick carries exactly one frame of each of the n_seq sequences.  Detection of all frames runs as the batched launches of
+ * lmot_batch_*, then ONE tracker chain steps all n_seq tables (one gate, TA, TB and TC launch per tick, whatever n_seq is).
+ *
+ * Sequence k of a tick gives bit for bit the results of a separate context created with the same lmot_params that receives sequence
+ * k's frames through lmot_frame: the counts, the boxes (sensor frame), targets, vandyaw, trackManage, the static and visible flags,
+ * vis_bb, the warning status and lmot_seq_tracker_dump (= that context's lmot_tracker_dump).  Sequences never interact, and the
+ * context's own tracker (lmot_frame*, lmot_batch*, lmot_track_step*, lmot_tracker_*) is a separate table: sequence ticks and those
+ * calls may be interleaved on one context without disturbing each other.  The sensor-rig table does not apply: every frame uses
+ * lmot_params' thresholds, as lmot_frame does.  Timing mode (lmot_enable_timing) is not supported: LMOT_ERR_STATE while it is on.
+ *
+ * lmot_seq_open(ctx, n_seq, ring): drains the context and replaces the set with n_seq (1..LMOT_MAX_BATCH) empty sequences, each at
+ *   its first frame, and a ring of `ring` (1..64) ticks.  n_seq = 0 frees the set.  Memory: n_seq track tables (device, max_tracks x
+ *   ~2.6 KB incl. side arrays at max_boxes 1024) plus ring x n_seq result blocks (each max_boxes x 96 B + max_tracks x 130 B of pinned host memory and
+ *   the same again on the device) -- size max_tracks and ring for it.
+ * lmot_seq_submit : HOST frames (stride in floats), LMOT_ERR_STATE if `ring` ticks wait to be collected.
+ * lmot_seq_dev    : DEVICE frames (stride 4 floats, 16-byte aligned), ordered after the caller stream; a full ring drops the oldest tick.
+ * timestamp_us / v_gps / yaw_gps are arrays of n_seq: each sequence's dt comes from its own previous stamp.  n[k] = 0 is an empty
+ * frame; that sequence's tracker still steps.  LMOT_ERR_INVALID: no open set, n_seq of the call != the set's, null or misaligned
+ * pointers; LMOT_ERR_CAPACITY: a frame above max_points.
+ * lmot_seq_collect: the OLDEST submitted tick (blocks until done); lmot_seq_fetch: the MOST RECENT one, older uncollected ticks are
+ * dropped; lmot_seq: submit + collect.  out->seq[k] is an lmot_frame_out with the usual rules: caller-owned buffers and capacities; the
+ * status is the first error of the tick's sequences, else its first warning.
+ * lmot_seq_tracker_reset(k) drains first, like lmot_tracker_reset: the next tick is sequence k's first frame (with the
+ * oracle_compat_first_frame quirk if that is on).  lmot_seq_tracker_dump uses lmot_tracker_dump's layout, lmot_seq_tracker_get_ego
+ * lmot_tracker_get_ego's.  k out of range: LMOT_ERR_INVALID. */
+typedef struct lmot_seq_out {
+  int n_seq;                                      /* out */
+  lmot_frame_out seq[LMOT_MAX_BATCH];             /* per sequence: caller sets boxes / max_boxes / tracks as for lmot_frame */
+} lmot_seq_out;
+int lmot_seq_open(lmot_ctx* ctx, int n_seq, int ring);
+int lmot_seq_submit(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride_floats, const double* timestamp_us,
+                    const double* v_gps, const double* yaw_gps);
+int lmot_seq_dev(lmot_ctx* ctx, const float* const* d_points, const int* n, int n_seq, const double* timestamp_us, const double* v_gps,
+                 const double* yaw_gps);
+int lmot_seq_collect(lmot_ctx* ctx, lmot_seq_out* out);
+int lmot_seq_fetch(lmot_ctx* ctx, lmot_seq_out* out);
+int lmot_seq(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride_floats, const double* timestamp_us,
+             const double* v_gps, const double* yaw_gps, lmot_seq_out* out);
+int lmot_seq_tracker_reset(lmot_ctx* ctx, int k);
+int lmot_seq_tracker_dump(lmot_ctx* ctx, int k, double* dumps, int cap, int* n);
+int lmot_seq_tracker_get_ego(lmot_ctx* ctx, int k, double ego8[8]);
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);
