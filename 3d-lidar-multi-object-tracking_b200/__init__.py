@@ -103,7 +103,7 @@ ABI_SYMBOLS = [
     "lmot_batch_submit", "lmot_batch_dev", "lmot_batch_detect_dev", "lmot_batch_collect", "lmot_batch_fetch", "lmot_batch", "lmot_batch_ground_ccl_dev",
     "lmot_default_sensor", "lmot_set_sensors", "lmot_get_sensors",
     "lmot_seq_open", "lmot_seq_submit", "lmot_seq_dev", "lmot_seq_collect", "lmot_seq_fetch", "lmot_seq", "lmot_seq_tracker_reset",
-    "lmot_seq_tracker_dump", "lmot_seq_tracker_get_ego",
+    "lmot_seq_tracker_dump", "lmot_seq_tracker_get_ego", "lmot_seq_set_sensors", "lmot_seq_get_sensors", "lmot_seq_frame_counts",
     "lmot_detect_boxes_dev", "lmot_track_step_lists_dev", "lmot_tracker_counters_dev", "lmot_tracker_table_received",
     "lmot_origin_points", "lmot_tracker_table", "lmot_tracker_set_num_tracks", "lmot_tracker_reset", "lmot_tracker_num_tracks", "lmot_tracker_dump", "lmot_tracker_load", "lmot_tracker_get_ego", "lmot_tracker_set_ego",
     "lmot_debug_polar_grid", "lmot_debug_cell_index", "lmot_debug_label_grid", "lmot_selftest_atan2f",
@@ -433,9 +433,13 @@ class Lmot:
     def set_sensors(self, poses, h_sensor=None, t_hmin=None, t_hmax=None, sensor_height=None):
         """poses: (n, 3, 4) or (n, 12) sensor -> vehicle transforms [R | t] (n = 0 or None: no sensors).  The four thresholds are
         per-sensor sequences (or one value for all); None keeps this context's lmot_params value."""
+        arr, n = self._sensor_table(poses, h_sensor, t_hmin, t_hmax, sensor_height)
+        self._chk(self.lib.lmot_set_sensors(self.h, arr, n))
+
+    def _sensor_table(self, poses, h_sensor, t_hmin, t_hmax, sensor_height):
+        """(lmot_sensor array or None, n) for set_sensors / seq_set_sensors"""
         if poses is None or len(poses) == 0:
-            self._chk(self.lib.lmot_set_sensors(self.h, None, 0))
-            return
+            return None, 0
         P = np.asarray(poses, np.float32).reshape(len(poses), 12)
         n = P.shape[0]
         arr = (Sensor * n)()
@@ -445,16 +449,19 @@ class Lmot:
             for name, val in (("h_sensor", h_sensor), ("t_hmin", t_hmin), ("t_hmax", t_hmax), ("sensor_height", sensor_height)):
                 if val is not None:
                     setattr(arr[k], name, float(np.broadcast_to(np.asarray(val, np.float32), (n,))[k]))
-        self._chk(self.lib.lmot_set_sensors(self.h, arr, n))
+        return arr, n
+
+    @staticmethod
+    def _sensor_dict(s):
+        return dict(poses=np.array([list(e.pose) for e in s], np.float32).reshape(-1, 3, 4),
+                    **{k: np.array([getattr(e, k) for e in s], np.float32) for k in ("h_sensor", "t_hmin", "t_hmax", "sensor_height")})
 
     def get_sensors(self):
         """-> dict(poses (n, 3, 4) f32, h_sensor, t_hmin, t_hmax, sensor_height: (n,) f32 each)"""
         arr = (Sensor * MAX_BATCH)()
         n = C.c_int(0)
         self._chk(self.lib.lmot_get_sensors(self.h, arr, MAX_BATCH, C.byref(n)))
-        s = arr[: n.value]
-        return dict(poses=np.array([list(e.pose) for e in s], np.float32).reshape(-1, 3, 4),
-                    **{k: np.array([getattr(e, k) for e in s], np.float32) for k in ("h_sensor", "t_hmin", "t_hmax", "sensor_height")})
+        return self._sensor_dict(arr[: n.value])
 
     # ---- independent sequences: one frame of each sequence per tick, one track table per sequence (lmot_seq_*) ---------------
     def seq_open(self, n_seq: int, ring: int = 8):
@@ -462,8 +469,48 @@ class Lmot:
         self._chk(self.lib.lmot_seq_open(self.h, int(n_seq), int(ring)))
 
     def seq_prepare(self, dev_frames):
-        """Marshal a tick's (device pointer, n) list ONCE for seq_dev (a timing loop must not build ctypes arrays on every call)."""
-        return self.batch_prepare(dev_frames)
+        """Marshal a tick's per-sequence (device pointer, n) entries ONCE for seq_dev (a timing loop must not build ctypes arrays on
+        every call).  Entries as seq_dev takes them."""
+        return ("seq_prepared",) + tuple(self._seq_args(dev_frames, True))
+
+    @staticmethod
+    def _frame_list(entry, device: bool) -> bool:
+        """True if a sequence's entry is a Python list of frames (a sequence with a sensor table) rather than one frame"""
+        if not isinstance(entry, list) or not entry:
+            return False
+        return all(isinstance(x, tuple) for x in entry) if device else all(np.ndim(x) == 2 for x in entry)
+
+    def _seq_args(self, frames, device: bool):
+        """per-sequence entries -> (ptrs, ns, n_seq, stride, keep) over the tick's frames in sequence order"""
+        if isinstance(frames, tuple) and frames and frames[0] == "seq_prepared":
+            return frames[1:]
+        if isinstance(frames, tuple) and frames and frames[0] == "prepared":      # a batch_prepare handle: one frame per sequence
+            return frames[1:]
+        flat = []
+        for e in frames:
+            flat.extend(e if self._frame_list(e, device) else [e])
+        ptrs, ns, _, stride, keep = self._batch_args(flat, device)
+        return ptrs, ns, len(frames), stride, keep
+
+    # ---- sensor tables of sequences (lmot_seq_set_sensors): sequence k sends one frame per sensor each tick ------------------
+    def seq_set_sensors(self, k: int, poses, h_sensor=None, t_hmin=None, t_hmax=None, sensor_height=None):
+        """Sequence k's sensor table, arguments as set_sensors (poses None or empty: no table, one frame per tick)."""
+        arr, n = self._sensor_table(poses, h_sensor, t_hmin, t_hmax, sensor_height)
+        self._chk(self.lib.lmot_seq_set_sensors(self.h, int(k), arr, n))
+
+    def seq_get_sensors(self, k: int):
+        """-> dict as get_sensors, for sequence k"""
+        arr = (Sensor * MAX_BATCH)()
+        n = C.c_int(0)
+        self._chk(self.lib.lmot_seq_get_sensors(self.h, int(k), arr, MAX_BATCH, C.byref(n)))
+        return self._sensor_dict(arr[: n.value])
+
+    def seq_frame_counts(self, k: int) -> np.ndarray:
+        """(n_frames, 4) int32: n_elevated, n_ground, num_cluster, n_boxes of each of sequence k's frames in the tick collected last"""
+        out = np.zeros((MAX_BATCH, 4), np.int32)
+        n = C.c_int(0)
+        self._chk(self.lib.lmot_seq_frame_counts(self.h, int(k), out.ctypes.data_as(C.POINTER(C.c_int)), C.byref(n)))
+        return out[: n.value].copy()
 
     @staticmethod
     def seq_scalars(n_seq, values, default=0.0):
@@ -495,23 +542,24 @@ class Lmot:
         return [self._frame_result(so.seq[k], sets[k][1], want_boxes) for k in range(so.n_seq)]
 
     def seq(self, frames, timestamps, v_gps=None, yaw_gps=None, cap: int | None = None):
-        """One tick, synchronous: `frames` = one (N_k, >=3) host array per sequence; timestamps / v_gps / yaw_gps per sequence.
-        -> list of per-sequence dicts as frame() returns."""
-        ptrs, ns, S, stride, keep = self._batch_args(frames, False)
+        """One tick, synchronous: `frames` = per sequence one (N, >=3) host array, or a list of them (one per sensor of a sequence with
+        a sensor table); timestamps / v_gps / yaw_gps per sequence.  -> list of per-sequence dicts as frame() returns."""
+        ptrs, ns, S, stride, keep = self._seq_args(frames, False)
         so, sets = self._seq_out(cap or self.params.max_tracks)
         ptrs, ns, S, ts, v, yaw = self._seq_call_args((ptrs, ns, S), timestamps, v_gps, yaw_gps)
         self._chk(self.lib.lmot_seq(self.h, ptrs, ns, S, stride, ts, v, yaw, C.byref(so)))
         return self._seq_result(so, sets)
 
     def seq_submit(self, frames, timestamps, v_gps=None, yaw_gps=None):
-        ptrs, ns, S, stride, keep = self._batch_args(frames, False)
+        ptrs, ns, S, stride, keep = self._seq_args(frames, False)
         self._keep = keep          # the copies are asynchronous: the host arrays must outlive the call
         ptrs, ns, S, ts, v, yaw = self._seq_call_args((ptrs, ns, S), timestamps, v_gps, yaw_gps)
         self._chk(self.lib.lmot_seq_submit(self.h, ptrs, ns, S, stride, ts, v, yaw))
 
     def seq_dev(self, dev_frames, timestamps, v_gps=None, yaw_gps=None):
-        """dev_frames = list of (device pointer, n) of stride-4 float frames, one per sequence (or a seq_prepare handle)."""
-        ptrs, ns, S, _, _ = self._batch_args(dev_frames, True)
+        """dev_frames = per sequence one (device pointer, n) tuple of a stride-4 float frame, or a list of them (a sequence with a
+        sensor table); or a seq_prepare handle."""
+        ptrs, ns, S, _, _ = self._seq_args(dev_frames, True)
         ptrs, ns, S, ts, v, yaw = self._seq_call_args((ptrs, ns, S), timestamps, v_gps, yaw_gps)
         self._chk(self.lib.lmot_seq_dev(self.h, ptrs, ns, S, ts, v, yaw))
 

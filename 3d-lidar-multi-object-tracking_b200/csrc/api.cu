@@ -376,11 +376,19 @@ void result_destroy(Result* r) {
   for (int i = 0; i < kMaxKernelEvents; ++i) if (r->kev[i]) cudaEventDestroy(r->kev[i]);
 }
 
-// ---- independent sequences (lmot_seq_*): S frame streams, one frame each per tick, S track tables ---------------------------------
-// Detection runs on the batch banks (batch_ensure) exactly as a batched tick without a sensor rig; the box lists are NOT concatenated:
-// sequence k's tracker reads slot k's own list and counters (seq_tracker_launch, tracker.cu).
+// ---- independent sequences (lmot_seq_*): S frame streams, one or more frames each per tick, S track tables ---------------------------
+// Detection runs on the batch banks (batch_ensure).  Without sensor tables the box lists are NOT concatenated: sequence k's tracker
+// reads slot k's own list and counters (seq_tracker_launch, tracker.cu).  With any table set, concat_boxes_seq_kernel concatenates each
+// sequence's frames into that sequence's list on the bank (seq_meas) and the tracker reads those.
 void seq_destroy(Ctx* c) {
   for (int k = 0; k < c->n_seq; ++k) tracker_free(c->seq[k]);
+  for (int b = 0; b < kBatchBanks; ++b)
+    for (int k = 0; k < kMaxBatch; ++k) {
+      SeqMeas& m = c->seq_meas[b][k];
+      cudaFree(m.d_boxes); cudaFree(m.d_boxes_g); cudaFree(m.d_counters); cudaFree(m.d_det_sem);
+      m = SeqMeas{};
+    }
+  for (int k = 0; k < kMaxBatch; ++k) { c->seq_n_sensors[k] = 0; c->seq_fc_n[k] = 0; }
   for (int i = 0; i < c->seq_ring; ++i)
     for (int k = 0; k < c->n_seq; ++k) result_destroy(&c->seq_ticks[i].blocks[k]);
   delete[] c->seq_ticks;
@@ -416,8 +424,17 @@ int seq_collect_tick(Ctx* c, SeqTick* t, lmot_seq_out* out) {
   int rc = LMOT_OK;
   if (out) out->n_seq = c->n_seq;
   for (int k = 0; k < c->n_seq; ++k) {
-    const int r = collect_result(c, &t->blocks[k], out ? &out->seq[k] : nullptr, &c->seq[k]);
+    Result* b = &t->blocks[k];
+    const int r = collect_result(c, b, out ? &out->seq[k] : nullptr, &c->seq[k]);
     if (r < 0 ? (rc >= 0) : (rc == LMOT_OK)) rc = r;       // the first error, else the first warning
+    // per-frame counts (lmot_seq_frame_counts): the concatenation wrote them into the block (ticks with tables); else the one frame's
+    if (b->batch_frames > 0) {
+      c->seq_fc_n[k] = b->batch_frames;
+      memcpy(c->seq_fc[k], b->h_frame_counts, (size_t)b->batch_frames * 4 * sizeof(int));
+    } else {
+      c->seq_fc_n[k] = 1;
+      for (int j = 0; j < 4; ++j) c->seq_fc[k][0][j] = b->h_hdr[HDR_N_ELEV + j];
+    }
   }
   return rc;
 }
@@ -1019,6 +1036,17 @@ int lmot_batch(lmot_ctx* ctx, const float* const* points, const int* n, int n_fr
 }
 
 // ---------------------------------------------------------------------------------------------- independent sequences
+static int seq_meas_alloc(Ctx* c, SeqMeas& m) {
+  const size_t lb = (size_t)c->prm.max_boxes * 24 * sizeof(float);
+  LMOT_CUDA(c, cudaMalloc(&m.d_boxes, lb));
+  LMOT_CUDA(c, cudaMalloc(&m.d_boxes_g, lb));
+  LMOT_CUDA(c, cudaMalloc(&m.d_counters, CNT_COUNT * sizeof(int)));
+  LMOT_CUDA(c, cudaMemset(m.d_counters, 0, CNT_COUNT * sizeof(int)));
+  LMOT_CUDA(c, cudaMalloc(&m.d_det_sem, sizeof(int)));
+  LMOT_CUDA(c, cudaMemset(m.d_det_sem, 0, sizeof(int)));
+  return LMOT_OK;
+}
+
 int lmot_seq_open(lmot_ctx* ctx, int n_seq, int ring) {
   if (!ctx || n_seq < 0 || n_seq > kMaxBatch || (n_seq > 0 && (ring < 1 || ring > kMaxResults))) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
@@ -1032,6 +1060,8 @@ int lmot_seq_open(lmot_ctx* ctx, int n_seq, int ring) {
   c->seq_ring = ring;
   c->n_seq = n_seq;                    // (set before the allocations: seq_destroy frees whatever was allocated on failure)
   for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = tracker_alloc(c, c->seq[k]);
+  for (int b = 0; b < kBatchBanks && rc == LMOT_OK; ++b)         // (nothing is in flight: drained above)
+    for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = seq_meas_alloc(c, c->seq_meas[b][k]);
   for (int i = 0; i < ring && rc == LMOT_OK; ++i)
     for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = result_create(c, &c->seq_ticks[i].blocks[k]);
   if (rc == LMOT_OK) rc = (cudaDeviceSynchronize() == cudaSuccess) ? LMOT_OK : LMOT_ERR_CUDA;
@@ -1046,13 +1076,24 @@ static int seq_common(lmot_ctx* ctx, const float* const* points, const int* n, i
   if (c->n_seq == 0 || n_seq != c->n_seq || !points || !n || !ts || !v || !yaw) return LMOT_ERR_INVALID;
   if (c->timing) return LMOT_ERR_STATE;
   cudaSetDevice(c->device);
-  for (int i = 0; i < n_seq; ++i) {
+  // the tick's frames: sequence k's sensors in table order, frames [f0[k], f0[k + 1]); one frame for a sequence without a table
+  // (lmot_seq_set_sensors keeps the total at or below kMaxBatch)
+  int f0[kMaxBatch + 1];
+  bool rig_on[kMaxBatch], rigged = false;
+  f0[0] = 0;
+  for (int k = 0; k < n_seq; ++k) {
+    rig_on[k] = c->seq_n_sensors[k] > 0;
+    rigged |= rig_on[k];
+    f0[k + 1] = f0[k] + (rig_on[k] ? c->seq_n_sensors[k] : 1);
+  }
+  const int F = f0[n_seq];
+  for (int i = 0; i < F; ++i) {
     if (n[i] < 0 || (n[i] > 0 && !points[i])) return LMOT_ERR_INVALID;
     if (n[i] > c->max_points) return LMOT_ERR_CAPACITY;
     if (!host && n[i] > 0 && (reinterpret_cast<uintptr_t>(points[i]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies need 16-byte alignment
   }
   if (host && (stride < 3 || c->seq_in_flight >= c->seq_ring)) return stride < 3 ? LMOT_ERR_INVALID : LMOT_ERR_STATE;
-  int rc = batch_ensure(c, n_seq);
+  int rc = batch_ensure(c, F);
   if (rc) return rc;
   SeqTick* t = seq_acquire(c, !host);
   if (!t) return LMOT_ERR_STATE;
@@ -1061,32 +1102,56 @@ static int seq_common(lmot_ctx* ctx, const float* const* points, const int* n, i
   Slot* k = &c->bank[b];
   Slot* sl[kMaxBatch];
   const float4* pp[kMaxBatch];
-  for (int i = 0; i < n_seq; ++i) sl[i] = &c->bslots[b * c->batch_frames + i];
+  for (int i = 0; i < F; ++i) sl[i] = &c->bslots[b * c->batch_frames + i];
   cudaStream_t st = sl[0]->stream;
   // the bank's previous tick must have been consumed by the tracker; device frames: ordered after the caller's stream
   LMOT_CUDA(c, cudaStreamWaitEvent(st, k->ev_trk_done, 0));
   if (host) {
-    for (int i = 0; i < n_seq; ++i) {
+    for (int i = 0; i < F; ++i) {
       if ((rc = upload_points(c, sl[i], st, points[i], n[i], stride, sl[i]->d_points))) return rc;
       pp[i] = sl[i]->d_points;
     }
   } else {
     LMOT_CUDA(c, cudaEventRecord(k->ev_fork, c->stream));
     LMOT_CUDA(c, cudaStreamWaitEvent(st, k->ev_fork, 0));
-    for (int i = 0; i < n_seq; ++i) pp[i] = reinterpret_cast<const float4*>(points[i]);
+    for (int i = 0; i < F; ++i) pp[i] = reinterpret_cast<const float4*>(points[i]);
   }
   struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
-  for (int i = 0; i < n_seq; ++i) { t->blocks[i].n_kev = 0; t->blocks[i].batch_frames = 0; t->blocks[i].has_tracks = true; }
+  for (int i = 0; i < n_seq; ++i) {
+    t->blocks[i].n_kev = 0; t->blocks[i].has_tracks = true;
+    t->blocks[i].batch_frames = rigged ? f0[i + 1] - f0[i] : 0;     // > 0: the concatenation writes the block's per-frame counts
+  }
   k->res = &t->blocks[0]; sl[0]->res = &t->blocks[0];
-  // detection: the batched launches of lmot_batch_* without a rig; each frame's last box-fitting CTA (or, global_frame, its
-  // boxes_to_global CTA) posts its own slot's semaphore, which the tick's gate kernel polls
   const bool gf = c->prm.global_frame != 0;
-  if ((rc = ground_launch_batch(c, sl, n_seq, pp, n, st, true, false, c->fuse_ccl, false, nullptr))) return rc;
-  if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, n_seq, st))) return rc;
-  if ((rc = boxfit_launch_batch(c, sl, n_seq, st, n, !gf, nullptr))) return rc;
-  if (gf && (rc = seq_global_launch(c, sl, n_seq, st, ts, v, yaw))) return rc;
+  SeqMeas m[kMaxBatch];
+  if (!rigged) {
+    // detection: the batched launches of lmot_batch_* without a rig; each frame's last box-fitting CTA (or, global_frame, its
+    // boxes_to_global CTA) posts its own slot's semaphore, which the tick's gate kernel polls
+    for (int i = 0; i < n_seq; ++i) m[i] = SeqMeas{sl[i]->d_boxes, sl[i]->d_boxes_g, sl[i]->d_counters, sl[i]->d_det_sem};
+    if ((rc = ground_launch_batch(c, sl, n_seq, pp, n, st, true, false, c->fuse_ccl, false, nullptr))) return rc;
+    if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, n_seq, st))) return rc;
+    if ((rc = boxfit_launch_batch(c, sl, n_seq, st, n, !gf, nullptr))) return rc;
+  } else {
+    // detection with one sensor per frame (sequences without a table: lmot_params' values), copied into the launch parameters (later
+    // table changes leave this tick alone); then each sequence's frames into its own list, whose semaphore the gate kernel polls
+    lmot_sensor rig[kMaxBatch];
+    int* fc[kMaxBatch];
+    for (int i = 0; i < n_seq; ++i) {
+      for (int j = f0[i]; j < f0[i + 1]; ++j) {
+        if (rig_on[i]) rig[j] = c->seq_sensors[i][j - f0[i]];
+        else lmot_default_sensor(&c->prm, &rig[j]);
+      }
+      m[i] = c->seq_meas[b][i];
+      LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc[i], t->blocks[i].h_frame_counts, 0));
+    }
+    if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, c->fuse_ccl, false, rig))) return rc;
+    if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
+    if ((rc = boxfit_launch_batch(c, sl, F, st, n, false, rig))) return rc;
+    if ((rc = boxes_concat_seq_launch(c, sl, n_seq, f0, rig_on, rig, m, fc, !gf, st))) return rc;
+  }
+  if (gf && (rc = seq_global_launch(c, m, n_seq, st, ts, v, yaw))) return rc;
   LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, st));
-  if ((rc = seq_tracker_launch(c, sl, t, n_seq, ts, v, yaw))) return rc;
+  if ((rc = seq_tracker_launch(c, m, t, n_seq, ts, v, yaw))) return rc;
   LMOT_CUDA(c, cudaEventRecord(t->blocks[0].ev_done, c->pub_stream));
   LMOT_CUDA(c, cudaEventRecord(k->ev_trk_done, c->pub_stream));
   if (!t->in_flight) { t->in_flight = true; ++c->seq_in_flight; }
@@ -1198,21 +1263,27 @@ int lmot_default_sensor(const lmot_params* p, lmot_sensor* out) {
   return LMOT_OK;
 }
 
-// the table only changes host state: ticks already submitted carry their own copy in their launch parameters
-int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n) {
-  if (!ctx || n < 0 || n > kMaxBatch || (n > 0 && !s)) return LMOT_ERR_INVALID;
+// a sensor table of n (0..kMaxBatch) entries: finite values, orthonormal rotations
+static bool sensors_valid(const lmot_sensor* s, int n) {
+  if (n < 0 || n > kMaxBatch || (n > 0 && !s)) return false;
   for (int k = 0; k < n; ++k) {
     const lmot_sensor& e = s[k];
     const float v[4] = {e.h_sensor, e.t_hmin, e.t_hmax, e.sensor_height};
-    for (float x : e.pose) if (!std::isfinite(x)) return LMOT_ERR_INVALID;
-    for (float x : v) if (!std::isfinite(x)) return LMOT_ERR_INVALID;
+    for (float x : e.pose) if (!std::isfinite(x)) return false;
+    for (float x : v) if (!std::isfinite(x)) return false;
     for (int i = 0; i < 3; ++i)           // R^T R == I within 1e-5 per element (columns of the row-major 3x4)
       for (int j = 0; j < 3; ++j) {
         double d = 0.0;
         for (int r = 0; r < 3; ++r) d += (double)e.pose[4 * r + i] * (double)e.pose[4 * r + j];
-        if (std::fabs(d - (i == j ? 1.0 : 0.0)) > 1e-5) return LMOT_ERR_INVALID;
+        if (std::fabs(d - (i == j ? 1.0 : 0.0)) > 1e-5) return false;
       }
   }
+  return true;
+}
+
+// the table only changes host state: ticks already submitted carry their own copy in their launch parameters
+int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n) {
+  if (!ctx || !sensors_valid(s, n)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   for (int k = 0; k < n; ++k) c->sensors[k] = s[k];
   c->n_sensors = n;
@@ -1224,6 +1295,38 @@ int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n) {
   const Ctx* c = &ctx->c;
   if (n) *n = c->n_sensors;
   for (int k = 0; k < c->n_sensors && k < cap; ++k) s[k] = c->sensors[k];
+  return LMOT_OK;
+}
+
+// sequence k's table (host state only, as lmot_set_sensors): its frames of later ticks, in table order
+int lmot_seq_set_sensors(lmot_ctx* ctx, int k, const lmot_sensor* s, int n) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq || !sensors_valid(s, n)) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  int frames = 0;                                  // frames per tick with the new table: one per sequence without a table
+  for (int j = 0; j < c->n_seq; ++j) {
+    const int nj = j == k ? n : c->seq_n_sensors[j];
+    frames += nj > 0 ? nj : 1;
+  }
+  if (frames > kMaxBatch) return LMOT_ERR_INVALID;
+  for (int j = 0; j < n; ++j) c->seq_sensors[k][j] = s[j];
+  c->seq_n_sensors[k] = n;
+  return LMOT_OK;
+}
+
+int lmot_seq_get_sensors(const lmot_ctx* ctx, int k, lmot_sensor* s, int cap, int* n) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq || cap < 0 || (cap > 0 && !s)) return LMOT_ERR_INVALID;
+  const Ctx* c = &ctx->c;
+  if (n) *n = c->seq_n_sensors[k];
+  for (int j = 0; j < c->seq_n_sensors[k] && j < cap; ++j) s[j] = c->seq_sensors[k][j];
+  return LMOT_OK;
+}
+
+int lmot_seq_frame_counts(lmot_ctx* ctx, int k, int counts[LMOT_MAX_BATCH][4], int* n_frames) {
+  if (!ctx || !counts || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  const Ctx* c = &ctx->c;
+  if (n_frames) *n_frames = c->seq_fc_n[k];
+  for (int j = 0; j < c->seq_fc_n[k]; ++j)
+    for (int i = 0; i < 4; ++i) counts[j][i] = c->seq_fc[k][j][i];
   return LMOT_OK;
 }
 

@@ -738,11 +738,11 @@ __device__ __forceinline__ void rig_apply_box(const float* m, float* b) {
   for (int c = 0; c < 8; ++c) rig_apply(m, b[3 * c], b[3 * c + 1], b[3 * c + 2]);
 }
 
-// batched submissions (one frame per sensor stream): the frames' box lists, concatenated in stream order, are ONE measurement
-// list for the tracker (tracking/main.cpp:98-141 unpacks whatever the trackbox message holds; one immUkfJpdaf call per tick).
-// kRig: frame w's boxes are moved into the vehicle frame by its sensor's pose R->m[w] on the way.
+// batched submissions (one frame per sensor stream): the box lists of frames [f0, f0 + n_frames), concatenated in stream order, are ONE
+// measurement list for the tracker (tracking/main.cpp:98-141 unpacks whatever the trackbox message holds; one immUkfJpdaf call per tick).
+// kRig: frame f0 + w's boxes are moved into the vehicle frame by its sensor's pose R->m[f0 + w] on the way.  frame_counts row w = frame f0 + w.
 template <bool kRig>
-__device__ __forceinline__ void concat_boxes_body(const FitBatch& B, const RigPoses* R, int n_frames, int max_boxes, float* __restrict__ boxes,
+__device__ __forceinline__ void concat_boxes_body(const FitBatch& B, const RigPoses* R, int f0, int n_frames, int max_boxes, float* __restrict__ boxes,
                                                   int* __restrict__ counters, int* __restrict__ frame_counts, int* __restrict__ det_sem) {
   __shared__ int s_off[kMaxBatch + 1];
   __shared__ int s_fc[kMaxBatch][5];
@@ -750,7 +750,7 @@ __device__ __forceinline__ void concat_boxes_body(const FitBatch& B, const RigPo
   // frames was 40 dependent round trips)
   if (threadIdx.x < n_frames) {
     const int f = threadIdx.x;
-    int* fc = B.f[f].counters;
+    int* fc = B.f[f0 + f].counters;
     const int ne = fc[CNT_N_ELEV], ng = fc[CNT_N_GROUND], nc = fc[CNT_NUM_CLUSTER], nb = fc[CNT_N_BOXES], er = fc[CNT_ERROR];
     s_fc[f][0] = ne; s_fc[f][1] = ng; s_fc[f][2] = nc; s_fc[f][3] = nb; s_fc[f][4] = er;
     frame_counts[4 * f] = ne; frame_counts[4 * f + 1] = ng; frame_counts[4 * f + 2] = nc; frame_counts[4 * f + 3] = nb;
@@ -779,7 +779,7 @@ __device__ __forceinline__ void concat_boxes_body(const FitBatch& B, const RigPo
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (w < n_frames) {
       const int off = s_off[w], cnt = min(s_off[w + 1], max_boxes) - off;
-      const uint4* src = reinterpret_cast<const uint4*>(B.f[w].boxes);
+      const uint4* src = reinterpret_cast<const uint4*>(B.f[f0 + w].boxes);
       uint4* dst = reinterpret_cast<uint4*>(boxes + (size_t)off * 24);
       if (!kRig) {
         const int nw = cnt > 0 ? cnt * 6 : 0;
@@ -792,7 +792,7 @@ __device__ __forceinline__ void concat_boxes_body(const FitBatch& B, const RigPo
         }
       } else {
         // a whole box per lane: its six words in flight, then its eight corners through the pose
-        const float* m = R->m[w];
+        const float* m = R->m[f0 + w];
         for (int j = lane; j < cnt; j += 32) {
           uint4 v[6];
 #pragma unroll
@@ -815,13 +815,27 @@ __device__ __forceinline__ void concat_boxes_body(const FitBatch& B, const RigPo
 __global__ void __launch_bounds__(256)
 concat_boxes_kernel(const __grid_constant__ FitBatch B, int n_frames, int max_boxes, float* __restrict__ boxes, int* __restrict__ counters,
                     int* __restrict__ frame_counts, int* __restrict__ det_sem) {
-  concat_boxes_body<false>(B, nullptr, n_frames, max_boxes, boxes, counters, frame_counts, det_sem);
+  concat_boxes_body<false>(B, nullptr, 0, n_frames, max_boxes, boxes, counters, frame_counts, det_sem);
 }
 
 __global__ void __launch_bounds__(256)
 concat_boxes_rig_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ RigPoses R, int n_frames, int max_boxes, float* __restrict__ boxes,
                         int* __restrict__ counters, int* __restrict__ frame_counts, int* __restrict__ det_sem) {
-  concat_boxes_body<true>(B, &R, n_frames, max_boxes, boxes, counters, frame_counts, det_sem);
+  concat_boxes_body<true>(B, &R, 0, n_frames, max_boxes, boxes, counters, frame_counts, det_sem);
+}
+
+// sequence ticks with sensor tables (lmot_seq_set_sensors): CTA k concatenates sequence k's frames [f0, f0 + n_frames) into the
+// sequence's own measurement list.  A sequence with a table moves each box by its sensor's pose; a sequence without one has a single
+// frame, copied unchanged.  det_sem: posted after the list is complete (nullptr with global_frame: boxes_to_global_seq_kernel posts it).
+struct ConcatSeq { int f0, n_frames, rig; float* boxes; int* counters; int* frame_counts; int* det_sem; };
+struct ConcatSeqParams { ConcatSeq s[kMaxBatch]; };
+
+__global__ void __launch_bounds__(256)
+concat_boxes_seq_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ RigPoses R, const __grid_constant__ ConcatSeqParams P,
+                        int max_boxes) {
+  const ConcatSeq& q = P.s[blockIdx.x];
+  if (q.rig) concat_boxes_body<true>(B, &R, q.f0, q.n_frames, max_boxes, q.boxes, q.counters, q.frame_counts, q.det_sem);
+  else concat_boxes_body<false>(B, nullptr, q.f0, q.n_frames, max_boxes, q.boxes, q.counters, q.frame_counts, q.det_sem);
 }
 
 }  // namespace
@@ -958,6 +972,25 @@ int boxes_concat_launch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, floa
     concat_boxes_kernel<<<1, 256, 0, st>>>(B, F, c->prm.max_boxes, d_boxes, d_counters, d_frame_counts, det_sem);
   }
   kernel_mark(c, slots[0], st);
+  LMOT_CUDA(c, cudaGetLastError());
+  return LMOT_OK;
+}
+
+// sequence ticks with sensor tables: sequence k's frames [f0[k], f0[k + 1]) of `slots` -> m[k]'s list and counters, per-frame counts into
+// frame_counts[k] (device view of the tick's pinned block k).  rig: one entry per frame of the tick; sequence k's poses apply iff rig_on[k].
+int boxes_concat_seq_launch(Ctx* c, Slot* const* slots, int S, const int* f0, const bool* rig_on, const lmot_sensor* rig, const SeqMeas* m,
+                            int* const* frame_counts, bool post_sem, cudaStream_t st) {
+  const int F = f0[S];
+  if (S < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
+  FitBatch B;
+  for (int i = 0; i < F; ++i) fit_frame_of(slots[i], B.f[i], false);
+  for (int i = F; i < kMaxBatch; ++i) B.f[i] = B.f[0];
+  RigPoses R;
+  rig_poses_of(rig, F, R);
+  ConcatSeqParams P{};
+  for (int k = 0; k < S; ++k)
+    P.s[k] = ConcatSeq{f0[k], f0[k + 1] - f0[k], rig_on[k] ? 1 : 0, m[k].d_boxes, m[k].d_counters, frame_counts[k], post_sem ? m[k].d_det_sem : nullptr};
+  concat_boxes_seq_kernel<<<S, 256, 0, st>>>(B, R, P, c->prm.max_boxes);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
 }

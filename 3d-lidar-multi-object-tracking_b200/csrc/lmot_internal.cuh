@@ -197,6 +197,11 @@ struct Tracker {
   int last_n_act = 0;                  // active tracks (live or visible) in the last result the host has read: picks spawn_output_kernel's variant
 };
 
+// what the tracker chain of a sequence tick reads for sequence k: its measurement list, the list in the dead-reckoned global frame
+// (global_frame), its counter block and its detection semaphore.  Without sensor tables these are slot k's own buffers; with any table
+// set, the bank's per-sequence lists (Ctx::seq_meas) that concat_boxes_seq_kernel fills.
+struct SeqMeas { float* d_boxes = nullptr; float* d_boxes_g = nullptr; int* d_counters = nullptr; int* d_det_sem = nullptr; };
+
 // one tick of lmot_seq_*: a result block per sequence; blocks[0].ev_done marks the whole tick published
 struct SeqTick {
   Result blocks[kMaxBatch];
@@ -255,6 +260,13 @@ struct Ctx {
   int seq_ring = 0, seq_next = 0, seq_oldest = 0, seq_in_flight = 0;
   SeqTick* seq_last = nullptr;         // most recent submission (lmot_seq_fetch)
   bool seq_wide = false;               // spawn_output_kernel's variant of the sequence ticks (largest last_n_act of the set)
+  // sensor tables of the sequences (lmot_seq_set_sensors): sequence k's frames of a tick are its sensors in table order; 0 sensors: one
+  // frame with lmot_params' thresholds.  Read at submission; the context's own table (sensors[]) never applies to sequence ticks.
+  int seq_n_sensors[kMaxBatch] = {};
+  lmot_sensor seq_sensors[kMaxBatch][kMaxBatch];
+  SeqMeas seq_meas[kBatchBanks][kMaxBatch];    // per-sequence measurement lists of each batch bank, allocated by lmot_seq_open
+  int seq_fc_n[kMaxBatch] = {};                // lmot_seq_frame_counts: frames of sequence k in the tick collected last
+  int seq_fc[kMaxBatch][kMaxBatch][4] = {};    // ... and their n_elev, n_ground, num_cluster, n_boxes (host copies: the ring slot is reused)
 
   // ---- timing
   bool timing = false;
@@ -333,9 +345,12 @@ int tracker_launch(Ctx* c, Slot* s, cudaStream_t st, const float* d_boxes, const
 int boxes_to_global_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, const int* det_counters, double timestamp, double v_gps,
                            double yaw_gps, bool post_sem);
 int tracker_publish(Ctx* c, Result* r, cudaStream_t st);            // device block of r -> pinned host block
-// sequence ticks: frame k of the tick = slot sl[k] -> track table c->seq[k] -> tick->blocks[k] (tracker.cu)
-int seq_global_launch(Ctx* c, Slot* const* sl, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw);
-int seq_tracker_launch(Ctx* c, Slot* const* sl, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw);
+// sequence ticks with sensor tables: sequence k's frames [f0[k], f0[k + 1]) of `slots` -> m[k] (boxfit.cu)
+int boxes_concat_seq_launch(Ctx* c, Slot* const* slots, int S, const int* f0, const bool* rig_on, const lmot_sensor* rig, const SeqMeas* m,
+                            int* const* frame_counts, bool post_sem, cudaStream_t st);
+// sequence ticks: measurement list m[k] -> track table c->seq[k] -> tick->blocks[k] (tracker.cu)
+int seq_global_launch(Ctx* c, const SeqMeas* m, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw);
+int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw);
 int boxes_publish(Ctx* c, Slot* s, Result* r, cudaStream_t st);     // detection-only: slot box list -> pinned host block
 
 }  // namespace lmot

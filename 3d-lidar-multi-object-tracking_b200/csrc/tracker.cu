@@ -2020,19 +2020,19 @@ int boxes_publish(Ctx* c, Slot* s, Result* r, cudaStream_t st) {
 }
 
 // ---------------------------------------------------------------------------------------------- sequence ticks (lmot_seq_*)
-// Sequence k of a tick: slot sl[k]'s box list and counters, track table c->seq[k], result block tick->blocks[k].  Every launch
-// below covers all S sequences; per-sequence arguments travel in __grid_constant__ parameter blocks.
+// Sequence k of a tick: measurement list m[k] (box list, counters, semaphore), track table c->seq[k], result block tick->blocks[k].
+// Every launch below covers all S sequences; per-sequence arguments travel in __grid_constant__ parameter blocks.
 
-// global_frame: sequence k's sensor-frame boxes -> sl[k]->d_boxes_g with THIS tick's ego pose of sequence k (peeked:
-// seq_tracker_launch folds it), posting sl[k]'s detection semaphore
-int seq_global_launch(Ctx* c, Slot* const* sl, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw) {
+// global_frame: sequence k's sensor- (or vehicle-) frame boxes -> m[k].d_boxes_g with THIS tick's ego pose of sequence k (peeked:
+// seq_tracker_launch folds it), posting m[k]'s detection semaphore
+int seq_global_launch(Ctx* c, const SeqMeas* m, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw) {
   GlobalSeqParams p{};
   for (int k = 0; k < S; ++k) {
     TrackerHost peek = c->seq[k].th;
     origin_points_fold(peek, ts[k], v[k], yaw[k]);
     Xf2 back;
     global_frame_xf(peek.egoPoint, &p.s[k].fwd, &back);
-    p.s[k].boxes = sl[k]->d_boxes; p.s[k].det = sl[k]->d_counters; p.s[k].boxes_g = sl[k]->d_boxes_g; p.s[k].det_sem = sl[k]->d_det_sem;
+    p.s[k].boxes = m[k].d_boxes; p.s[k].det = m[k].d_counters; p.s[k].boxes_g = m[k].d_boxes_g; p.s[k].det_sem = m[k].d_det_sem;
   }
   boxes_to_global_seq_kernel<<<S, 256, 0, st>>>(p);
   LMOT_CUDA(c, cudaGetLastError());
@@ -2041,7 +2041,7 @@ int seq_global_launch(Ctx* c, Slot* const* sl, int S, cudaStream_t st, const dou
 
 // gate -> TA -> TB -> TC once for all S sequences on the tracker stream (programmatic dependent launches, as the single-stream
 // chain), then one publish launch on the publish stream.  The caller records the tick's events on the publish stream afterwards.
-int seq_tracker_launch(Ctx* c, Slot* const* sl, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw) {
+int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw) {
   cudaStream_t st = c->trk_stream;
   const int compat = c->prm.oracle_compat_first_frame ? 1 : 0;
   const bool gf = c->prm.global_frame != 0;
@@ -2058,14 +2058,14 @@ int seq_tracker_launch(Ctx* c, Slot* const* sl, SeqTick* tick, int S, const doub
   int n_act_max = 0;
   for (int k = 0; k < S; ++k) {
     Tracker& t = c->seq[k];
-    Slot* s = sl[k];
+    const SeqMeas& s = m[k];
     Result* r = &tick->blocks[k];
     const int first = t.th.init ? 0 : 1;
     const double dt = first ? 0.0 : (ts[k] - t.th.timestamp) / 1000000.0;     // :807, from this sequence's own previous stamp
     origin_points_fold(t.th, ts[k], v[k], yaw[k]);
     if (gf) { Xf2 fwd; global_frame_xf(t.th.egoPoint, &fwd, &r->back); }
     else r->back.on = 0;
-    const float* boxes = gf ? s->d_boxes_g : s->d_boxes;
+    const float* boxes = gf ? s.d_boxes_g : s.d_boxes;
     const int full = t.act_valid ? 0 : 1;
     if (full) {
       LMOT_CUDA(c, cudaMemsetAsync(t.d_trk_counters + CNT_N_ACT, 0, sizeof(int), st));
@@ -2077,14 +2077,14 @@ int seq_tracker_launch(Ctx* c, Slot* const* sl, SeqTick* tick, int S, const doub
     const int run = (first && compat) ? 0 : 1;
     ActSummary* sum = reinterpret_cast<ActSummary*>(t.d_summary);
     double2* mc = reinterpret_cast<double2*>(t.d_meas_ctr);
-    g.sem[k] = s->d_det_sem;
-    ta.s[k] = TASeq{t.d_tracks, t.d_trk_counters, s->d_counters, boxes, dt, t.d_gate, t.d_setter, t.d_first_setter, t.d_skip, t.d_act_list,
+    g.sem[k] = s.d_det_sem;
+    ta.s[k] = TASeq{t.d_tracks, t.d_trk_counters, s.d_counters, boxes, dt, t.d_gate, t.d_setter, t.d_first_setter, t.d_skip, t.d_act_list,
                     t.d_meas_n, mc, t.d_tc_seq, t.tc_launched, run};
-    tb.s[k] = TBSeq{t.d_tracks, t.d_trk_counters, s->d_counters, boxes, t.d_gate, t.d_first_setter, t.d_skip, t.d_act_list, sum, t.d_meas_n, mc, run};
+    tb.s[k] = TBSeq{t.d_tracks, t.d_trk_counters, s.d_counters, boxes, t.d_gate, t.d_first_setter, t.d_skip, t.d_act_list, sum, t.d_meas_n, mc, run};
     OutPtrs o{r->d_targets, r->d_vandyaw, r->d_manage, r->d_static, r->d_vis, r->d_visbb, r->d_hdr, r->d_boxes};
     OutPtrs po{pr->d_targets, pr->d_vandyaw, pr->d_manage, pr->d_static, pr->d_vis, pr->d_visbb, pr->d_hdr, pr->d_boxes};
-    tcp.s[k] = TCSeq{t.d_tracks, t.d_trk_counters, s->d_counters, boxes, s->d_boxes, t.d_first_setter, t.d_new_num, t.d_vis_list, t.d_skip,
-                     t.d_act_list, t.d_pos, sum, s->d_det_sem, t.d_tc_seq, o, po, t.th.egoPoint[2], first, full};
+    tcp.s[k] = TCSeq{t.d_tracks, t.d_trk_counters, s.d_counters, boxes, s.d_boxes, t.d_first_setter, t.d_new_num, t.d_vis_list, t.d_skip,
+                     t.d_act_list, t.d_pos, sum, s.d_det_sem, t.d_tc_seq, o, po, t.th.egoPoint[2], first, full};
     ++t.tc_launched;
     OutPtrs h{r->h_targets, r->h_vandyaw, r->h_manage, r->h_static, r->h_vis, r->h_visbb, r->h_hdr, r->h_boxes};
     pub.s[k] = PubSeq{o, h, t.d_tc_seq, t.tc_launched, r->back};

@@ -271,7 +271,8 @@ int lmot_batch_ground_ccl_dev(lmot_ctx* ctx, const float* const* d_points, const
  *     vehicle's): two roundings in sequence, not one premultiplied matrix; targets and vis_bb come back in the vehicle frame.
  * The table is captured by value when a tick is submitted: ticks already in flight keep the table they were submitted with.  A tick or
  * list step with more frames than sensors is LMOT_ERR_INVALID while sensors are set.  Not affected: the stage entry points,
- * lmot_track_step and the single-stream lmot_frame* calls.  Detections of one object by two sensors with overlapping fields of view
+ * lmot_track_step, the single-stream lmot_frame* calls and sequence ticks (lmot_seq_*: each sequence has its own table,
+ * lmot_seq_set_sensors).  Detections of one object by two sensors with overlapping fields of view
  * stay two measurements (the reference has no fusion step). */
 typedef struct lmot_sensor {
   float pose[12];                 /* sensor -> vehicle frame, row-major 3x4 [R | t]; R orthonormal (|R^T R - I| <= 1e-5 elementwise) */
@@ -287,31 +288,50 @@ int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n);   /*
 /* ---- independent sequences: up to LMOT_MAX_BATCH frame streams per tick, each with its OWN track table ---------------------------
  * A sequence is an independent frame stream (one vehicle, one replayed log): it has its own track table, its own getOriginPoints
  * state (timestamp, ego velocity and yaw, dead-reckoning fold, first-frame flag), its own global_frame pose and its own result block.
- * One tick carries exactly one frame of each of the n_seq sequences.  Detection of all frames runs as the batched launches of
- * lmot_batch_*, then ONE tracker chain steps all n_seq tables (one gate, TA, TB and TC launch per tick, whatever n_seq is).
+ * One tick carries one frame of each of the n_seq sequences (one per sensor for a sequence with a sensor table, at most LMOT_MAX_BATCH
+ * frames in all).  Detection of all frames runs as the batched launches of lmot_batch_*, then ONE tracker chain steps all n_seq tables (one gate, TA, TB and TC launch per tick, whatever n_seq is).
  *
  * Sequence k of a tick gives bit for bit the results of a separate context created with the same lmot_params that receives sequence
  * k's frames through lmot_frame: the counts, the boxes (sensor frame), targets, vandyaw, trackManage, the static and visible flags,
  * vis_bb, the warning status and lmot_seq_tracker_dump (= that context's lmot_tracker_dump).  Sequences never interact, and the
  * context's own tracker (lmot_frame*, lmot_batch*, lmot_track_step*, lmot_tracker_*) is a separate table: sequence ticks and those
- * calls may be interleaved on one context without disturbing each other.  The sensor-rig table does not apply: every frame uses
- * lmot_params' thresholds, as lmot_frame does.  Timing mode (lmot_enable_timing) is not supported: LMOT_ERR_STATE while it is on.
+ * calls may be interleaved on one context without disturbing each other.  Timing mode (lmot_enable_timing) is not supported:
+ * LMOT_ERR_STATE while it is on.
+ *
+ * Multi-sensor sequences (one vehicle with several LiDARs, or one LiDAR not mounted at lmot_params' height): lmot_seq_set_sensors(k)
+ * gives sequence k its own sensor table, in lmot_set_sensors' format and with its rules.  Sequence k then has one frame per sensor in
+ * every tick, and behaves bit for bit like a separate context with the same lmot_params and lmot_set_sensors(that table) that receives
+ * those frames through lmot_batch: ground removal and box fitting with each sensor's thresholds, the frames' box lists concatenated in
+ * table order and moved into the VEHICLE frame, one tracker step on that list.  out->seq[k] then follows lmot_batch_out's rules: the
+ * counts are summed over its frames, boxes / n_boxes are the concatenated vehicle-frame list (LMOT_ERR_CAPACITY if it exceeds
+ * max_boxes); lmot_seq_frame_counts gives the per-frame counts.  A sequence without a table keeps one frame per tick with lmot_params'
+ * thresholds (its results stay those of lmot_frame), and with no table set a tick runs exactly the launches it always did.  The
+ * context's own table (lmot_set_sensors) never applies to sequence ticks.
  *
  * lmot_seq_open(ctx, n_seq, ring): drains the context and replaces the set with n_seq (1..LMOT_MAX_BATCH) empty sequences, each at
  *   its first frame, and a ring of `ring` (1..64) ticks.  n_seq = 0 frees the set.  Memory: n_seq track tables (device, max_tracks x
  *   ~2.6 KB incl. side arrays at max_boxes 1024) plus ring x n_seq result blocks (each max_boxes x 96 B + max_tracks x 130 B of pinned host memory and
- *   the same again on the device) -- size max_tracks and ring for it.
+ *   the same again on the device), and per sequence 2 x 2 x max_boxes x 96 B of device memory (a measurement list and its global-frame
+ *   copy for each of the two detection banks) -- size max_tracks and ring for it.  Reopening (or closing) also clears every sequence's sensor table.
  * lmot_seq_submit : HOST frames (stride in floats), LMOT_ERR_STATE if `ring` ticks wait to be collected.
  * lmot_seq_dev    : DEVICE frames (stride 4 floats, 16-byte aligned), ordered after the caller stream; a full ring drops the oldest tick.
- * timestamp_us / v_gps / yaw_gps are arrays of n_seq: each sequence's dt comes from its own previous stamp.  n[k] = 0 is an empty
- * frame; that sequence's tracker still steps.  LMOT_ERR_INVALID: no open set, n_seq of the call != the set's, null or misaligned
- * pointers; LMOT_ERR_CAPACITY: a frame above max_points.
+ * points / n hold one entry per FRAME of the tick, in sequence order: sequence 0's frames (its sensors in table order, or its one
+ * frame), then sequence 1's, and so on.  timestamp_us / v_gps / yaw_gps are arrays of n_seq (one per sequence): each sequence's dt
+ * comes from its own previous stamp.  n[i] = 0 is an empty frame; that sequence's tracker still steps.  LMOT_ERR_INVALID: no open
+ * set, n_seq of the call != the set's, null or misaligned pointers; LMOT_ERR_CAPACITY: a frame above max_points.
  * lmot_seq_collect: the OLDEST submitted tick (blocks until done); lmot_seq_fetch: the MOST RECENT one, older uncollected ticks are
  * dropped; lmot_seq: submit + collect.  out->seq[k] is an lmot_frame_out with the usual rules: caller-owned buffers and capacities; the
  * status is the first error of the tick's sequences, else its first warning.
  * lmot_seq_tracker_reset(k) drains first, like lmot_tracker_reset: the next tick is sequence k's first frame (with the
  * oracle_compat_first_frame quirk if that is on).  lmot_seq_tracker_dump uses lmot_tracker_dump's layout, lmot_seq_tracker_get_ego
- * lmot_tracker_get_ego's.  k out of range: LMOT_ERR_INVALID. */
+ * lmot_tracker_get_ego's.  k out of range: LMOT_ERR_INVALID.
+ * lmot_seq_set_sensors(k, s, n): sequence k's table; n = 0 (s may be NULL) removes it.  LMOT_ERR_INVALID, every table unchanged: k out
+ *   of range (or no open set), lmot_set_sensors' rejections, or more than LMOT_MAX_BATCH frames per tick over the set (a sequence
+ *   without a table counts one).  Host state only: submitted ticks keep the tables they were submitted with (copied into their launch
+ *   parameters); lmot_seq_tracker_reset leaves the table alone.  lmot_seq_get_sensors reads it back as lmot_get_sensors does.
+ * lmot_seq_frame_counts(k): (n_elevated, n_ground, num_cluster, n_boxes) of each of sequence k's frames in the tick most recently
+ *   returned by lmot_seq_collect / lmot_seq_fetch / lmot_seq, and their number (0 before the first); a one-frame sequence's row equals
+ *   out->seq[k]'s counts. */
 typedef struct lmot_seq_out {
   int n_seq;                                      /* out */
   lmot_frame_out seq[LMOT_MAX_BATCH];             /* per sequence: caller sets boxes / max_boxes / tracks as for lmot_frame */
@@ -328,6 +348,9 @@ int lmot_seq(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq,
 int lmot_seq_tracker_reset(lmot_ctx* ctx, int k);
 int lmot_seq_tracker_dump(lmot_ctx* ctx, int k, double* dumps, int cap, int* n);
 int lmot_seq_tracker_get_ego(lmot_ctx* ctx, int k, double ego8[8]);
+int lmot_seq_set_sensors(lmot_ctx* ctx, int k, const lmot_sensor* s, int n);
+int lmot_seq_get_sensors(const lmot_ctx* ctx, int k, lmot_sensor* s, int cap, int* n);
+int lmot_seq_frame_counts(lmot_ctx* ctx, int k, int counts[LMOT_MAX_BATCH][4], int* n_frames);
 
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
