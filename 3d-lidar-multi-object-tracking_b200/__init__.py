@@ -104,6 +104,7 @@ ABI_SYMBOLS = [
     "lmot_default_sensor", "lmot_set_sensors", "lmot_get_sensors",
     "lmot_seq_open", "lmot_seq_submit", "lmot_seq_dev", "lmot_seq_collect", "lmot_seq_fetch", "lmot_seq", "lmot_seq_tracker_reset",
     "lmot_seq_tracker_dump", "lmot_seq_tracker_get_ego", "lmot_seq_set_sensors", "lmot_seq_get_sensors", "lmot_seq_frame_counts",
+    "lmot_seq_track_submit", "lmot_seq_track_dev", "lmot_seq_track", "lmot_seq_tracker_load", "lmot_seq_tracker_set_ego",
     "lmot_detect_boxes_dev", "lmot_track_step_lists_dev", "lmot_tracker_counters_dev", "lmot_tracker_table_received",
     "lmot_origin_points", "lmot_tracker_table", "lmot_tracker_set_num_tracks", "lmot_tracker_reset", "lmot_tracker_num_tracks", "lmot_tracker_dump", "lmot_tracker_load", "lmot_tracker_get_ego", "lmot_tracker_set_ego",
     "lmot_debug_polar_grid", "lmot_debug_cell_index", "lmot_debug_label_grid", "lmot_selftest_atan2f",
@@ -467,6 +468,7 @@ class Lmot:
     def seq_open(self, n_seq: int, ring: int = 8):
         """n_seq (1..8) empty sequences and a ring of `ring` ticks (n_seq = 0 frees the set); drains the context."""
         self._chk(self.lib.lmot_seq_open(self.h, int(n_seq), int(ring)))
+        self.n_seq = int(n_seq)
 
     def seq_prepare(self, dev_frames):
         """Marshal a tick's per-sequence (device pointer, n) entries ONCE for seq_dev (a timing loop must not build ctypes arrays on
@@ -572,6 +574,61 @@ class Lmot:
         so, sets = self._seq_out(cap or self.params.max_tracks, want_boxes)
         self._chk(self.lib.lmot_seq_fetch(self.h, C.byref(so)))
         return self._seq_result(so, sets, want_boxes)
+
+    # ---- tracking-only sequence ticks: caller box lists instead of frames (lmot_seq_track*) -----------------------------------------
+    @staticmethod
+    def _seq_lists(lists):
+        """per-sequence entries -- one (m, 8, 3) box array, or a list of them for a sequence with a sensor table -- -> (ptrs, ms, n_seq,
+        keep) over the tick's lists in sequence order"""
+        flat = []
+        for e in lists:
+            flat.extend(e if isinstance(e, list) and e and all(np.ndim(x) == 3 for x in e) else [e])
+        ptrs = (C.c_void_p * len(flat))()
+        ms = (C.c_int * len(flat))()
+        keep = []
+        for i, b in enumerate(flat):
+            a = np.ascontiguousarray(b, np.float32).reshape(-1, 8, 3)
+            keep.append(a)
+            ptrs[i], ms[i] = (a.ctypes.data if len(a) else None), len(a)
+        return ptrs, ms, len(lists), keep
+
+    def seq_track(self, lists, timestamps, v_gps=None, yaw_gps=None, cap: int | None = None):
+        """One tracking-only tick, synchronous: `lists` = per sequence one (m, 8, 3) box array, or a list of them (one per sensor of a
+        sequence with a sensor table).  -> list of per-sequence dicts as seq() returns (counts 0, boxes = the list that was tracked)."""
+        ptrs, ms, S, keep = self._seq_lists(lists)
+        so, sets = self._seq_out(cap or self.params.max_tracks)
+        ptrs, ms, S, ts, v, yaw = self._seq_call_args((ptrs, ms, S), timestamps, v_gps, yaw_gps)
+        self._chk(self.lib.lmot_seq_track(self.h, ptrs, ms, S, ts, v, yaw, C.byref(so)))
+        return self._seq_result(so, sets)
+
+    def seq_track_submit(self, lists, timestamps, v_gps=None, yaw_gps=None):
+        """Asynchronous seq_track; results with seq_collect() / seq_fetch()."""
+        ptrs, ms, S, keep = self._seq_lists(lists)
+        self._keep = keep
+        ptrs, ms, S, ts, v, yaw = self._seq_call_args((ptrs, ms, S), timestamps, v_gps, yaw_gps)
+        self._chk(self.lib.lmot_seq_track_submit(self.h, ptrs, ms, S, ts, v, yaw))
+
+    def seq_track_dev(self, d_lists: int, d_counts: int, cap_per_list: int, timestamps, v_gps=None, yaw_gps=None):
+        """Asynchronous tracking-only tick from padded device lists (list i at d_lists + i * cap_per_list * 96 bytes, its length in the
+        device int d_counts[i]), one list per frame of the tick in sequence order; ordered after the context's stream."""
+        S = getattr(self, "n_seq", 0)
+        ts, v, yaw = (self.seq_scalars(max(S, 1), x) for x in (timestamps, v_gps, yaw_gps))
+        self._chk(self.lib.lmot_seq_track_dev(self.h, C.c_void_p(d_lists), C.c_void_p(d_counts), S, int(cap_per_list), ts, v, yaw))
+
+    def seq_tracker_load(self, k: int, dumps, init, timestamp_us, ego_velo=0.0, ego_yaw=0.0, ego_pre_yaw=0.0, ego_point_yaw=-np.pi / 2):
+        """tracker_load for sequence k"""
+        d = np.ascontiguousarray(dumps, np.float64).reshape(-1, TRACK_DUMP_DOUBLES)
+        n = d.shape[0]
+        if n == 0:
+            d = np.zeros((1, TRACK_DUMP_DOUBLES), np.float64)
+        self._chk(self.lib.lmot_seq_tracker_load(self.h, int(k), d.ctypes.data_as(C.POINTER(C.c_double)), n, int(init), C.c_double(timestamp_us),
+                                                 C.c_double(ego_velo), C.c_double(ego_yaw), C.c_double(ego_pre_yaw), C.c_double(ego_point_yaw)))
+
+    def seq_tracker_set_ego(self, k: int, ego8):
+        """tracker_set_ego for sequence k"""
+        e = np.ascontiguousarray(ego8, np.float64)
+        assert e.shape == (8,)
+        self._chk(self.lib.lmot_seq_tracker_set_ego(self.h, int(k), e.ctypes.data_as(C.POINTER(C.c_double))))
 
     def seq_tracker_reset(self, k: int):
         self._chk(self.lib.lmot_seq_tracker_reset(self.h, int(k)))

@@ -89,6 +89,7 @@ int check_device_error(Ctx* c, Slot* s, cudaStream_t st) {
 int drain(Ctx* c) {
   for (int i = 0; i < c->n_slots; ++i) LMOT_CUDA(c, cudaStreamSynchronize(c->slots[i].stream));
   for (int i = 0; i < c->n_bslots; ++i) LMOT_CUDA(c, cudaStreamSynchronize(c->bslots[i].stream));
+  for (int b = 0; b < kBatchBanks; ++b) if (c->bank[b].stream) LMOT_CUDA(c, cudaStreamSynchronize(c->bank[b].stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->trk_stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->pub_stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -187,17 +188,8 @@ int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tra
 int slot_create(Ctx* c, Slot* s, int index);
 void slot_destroy(Slot* s);
 
-int batch_ensure(Ctx* c, int F) {
-  if (F <= c->batch_frames) return LMOT_OK;
-  // (re)allocate for the larger batch: nothing of the old banks may be in flight
-  for (int i = 0; i < c->n_bslots; ++i) LMOT_CUDA(c, cudaStreamSynchronize(c->bslots[i].stream));
-  LMOT_CUDA(c, cudaStreamSynchronize(c->trk_stream));
-  LMOT_CUDA(c, cudaStreamSynchronize(c->pub_stream));
-  for (int i = c->n_bslots; i < kBatchBanks * F; ++i) {
-    int rc = slot_create(c, &c->bslots[i], 1000 + i);
-    if (rc) return rc;
-    c->n_bslots = i + 1;
-  }
+// the banks' pseudo-slots (once per context); the caller synchronises the device afterwards
+int bank_ensure(Ctx* c) {
   for (int b = 0; b < kBatchBanks; ++b) {
     Slot* k = &c->bank[b];
     if (k->d_boxes) continue;
@@ -213,8 +205,25 @@ int batch_ensure(Ctx* c, int F) {
     LMOT_CUDA(c, cudaEventCreateWithFlags(&k->ev_fork, cudaEventDisableTiming));
     LMOT_CUDA(c, cudaEventRecord(k->ev_trk_done, c->stream));
     LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, c->stream));
+    LMOT_CUDA(c, cudaStreamCreateWithFlags(&k->stream, cudaStreamNonBlocking));
     k->res = &c->results[0];
   }
+  return LMOT_OK;
+}
+
+int batch_ensure(Ctx* c, int F) {
+  if (F <= c->batch_frames) return LMOT_OK;
+  // (re)allocate for the larger batch: nothing of the old banks may be in flight
+  for (int i = 0; i < c->n_bslots; ++i) LMOT_CUDA(c, cudaStreamSynchronize(c->bslots[i].stream));
+  LMOT_CUDA(c, cudaStreamSynchronize(c->trk_stream));
+  LMOT_CUDA(c, cudaStreamSynchronize(c->pub_stream));
+  for (int i = c->n_bslots; i < kBatchBanks * F; ++i) {
+    int rc = slot_create(c, &c->bslots[i], 1000 + i);
+    if (rc) return rc;
+    c->n_bslots = i + 1;
+  }
+  int rc = bank_ensure(c);
+  if (rc) return rc;
   LMOT_CUDA(c, cudaDeviceSynchronize());
   c->batch_frames = F;
   return LMOT_OK;
@@ -228,6 +237,7 @@ void batch_destroy(Ctx* c) {
     if (k->ev_det_done) cudaEventDestroy(k->ev_det_done);
     if (k->ev_trk_done) cudaEventDestroy(k->ev_trk_done);
     if (k->ev_fork) cudaEventDestroy(k->ev_fork);
+    if (k->stream) cudaStreamDestroy(k->stream);
   }
 }
 
@@ -388,6 +398,7 @@ void seq_destroy(Ctx* c) {
       cudaFree(m.d_boxes); cudaFree(m.d_boxes_g); cudaFree(m.d_counters); cudaFree(m.d_det_sem);
       m = SeqMeas{};
     }
+  for (int b = 0; b < kBatchBanks; ++b) { cudaFree(c->seq_stage[b]); c->seq_stage[b] = nullptr; }
   for (int k = 0; k < kMaxBatch; ++k) { c->seq_n_sensors[k] = 0; c->seq_fc_n[k] = 0; }
   for (int i = 0; i < c->seq_ring; ++i)
     for (int k = 0; k < c->n_seq; ++k) result_destroy(&c->seq_ticks[i].blocks[k]);
@@ -617,6 +628,7 @@ int lmot_sync(lmot_ctx* ctx) {
   Ctx* c = &ctx->c;
   for (int i = 0; i < c->n_slots; ++i) LMOT_CUDA(c, cudaStreamSynchronize(c->slots[i].stream));
   for (int i = 0; i < c->n_bslots; ++i) LMOT_CUDA(c, cudaStreamSynchronize(c->bslots[i].stream));
+  for (int b = 0; b < kBatchBanks; ++b) if (c->bank[b].stream) LMOT_CUDA(c, cudaStreamSynchronize(c->bank[b].stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->trk_stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->pub_stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -631,7 +643,7 @@ int lmot_flush(lmot_ctx* ctx) {
     LMOT_CUDA(c, cudaStreamWaitEvent(c->stream, c->slots[i].ev_det_done, 0));
     LMOT_CUDA(c, cudaStreamWaitEvent(c->stream, c->slots[i].ev_trk_done, 0));
   }
-  for (int b = 0; b < kBatchBanks && c->batch_frames > 0; ++b) {
+  for (int b = 0; b < kBatchBanks && c->bank[b].ev_det_done; ++b) {      // (the banks exist once a batched or sequence tick ran)
     LMOT_CUDA(c, cudaStreamWaitEvent(c->stream, c->bank[b].ev_det_done, 0));
     LMOT_CUDA(c, cudaStreamWaitEvent(c->stream, c->bank[b].ev_trk_done, 0));
   }
@@ -1062,6 +1074,8 @@ int lmot_seq_open(lmot_ctx* ctx, int n_seq, int ring) {
   for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = tracker_alloc(c, c->seq[k]);
   for (int b = 0; b < kBatchBanks && rc == LMOT_OK; ++b)         // (nothing is in flight: drained above)
     for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = seq_meas_alloc(c, c->seq_meas[b][k]);
+  for (int b = 0; b < kBatchBanks && rc == LMOT_OK; ++b)
+    if (cudaMalloc(&c->seq_stage[b], (size_t)kMaxBatch * c->prm.max_boxes * 24 * sizeof(float) + kMaxBatch * sizeof(int)) != cudaSuccess) rc = LMOT_ERR_CUDA;
   for (int i = 0; i < ring && rc == LMOT_OK; ++i)
     for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = result_create(c, &c->seq_ticks[i].blocks[k]);
   if (rc == LMOT_OK) rc = (cudaDeviceSynchronize() == cudaSuccess) ? LMOT_OK : LMOT_ERR_CUDA;
@@ -1069,6 +1083,51 @@ int lmot_seq_open(lmot_ctx* ctx, int n_seq, int ring) {
   return rc;
 }
 
+// ---- sequence ticks: two front ends -- detection (frames -> ground removal, clustering, box fitting) and tracking-only (caller box
+// lists, lmot_seq_track*) -- fill each sequence's measurement list; one back end steps the tables.  Both kinds share the ring and the
+// bank alternation, so a set may mix them tick by tick; each table folds its steps in submission order.
+
+// the tick's frames / lists: sequence k's sensors in table order, [f0[k], f0[k + 1]); one for a sequence without a table
+// (lmot_seq_set_sensors keeps the total at or below kMaxBatch).  -> whether any sequence has a table
+static bool seq_layout(const Ctx* c, int* f0, bool* rig_on) {
+  bool rigged = false;
+  f0[0] = 0;
+  for (int k = 0; k < c->n_seq; ++k) {
+    rig_on[k] = c->seq_n_sensors[k] > 0;
+    rigged |= rig_on[k];
+    f0[k + 1] = f0[k] + (rig_on[k] ? c->seq_n_sensors[k] : 1);
+  }
+  return rigged;
+}
+
+// back end, first half: the tick's ring slot and bank.  *st: the stream the front end runs on -- the bank's first detection slot's for
+// detection, the bank's own for tracking-only ticks -- made to wait until the bank's previous tick has been consumed by the tracker.
+static int seq_begin(Ctx* c, bool drop_oldest, bool lists, SeqTick** t, int* bank, cudaStream_t* st) {
+  *t = seq_acquire(c, drop_oldest);
+  if (!*t) return LMOT_ERR_STATE;
+  const int b = c->next_bank;
+  c->next_bank = (c->next_bank + 1) % kBatchBanks;
+  *bank = b;
+  *st = lists ? c->bank[b].stream : c->bslots[b * c->batch_frames].stream;
+  LMOT_CUDA(c, cudaStreamWaitEvent(*st, c->bank[b].ev_trk_done, 0));
+  return LMOT_OK;
+}
+
+// back end, second half: the measurement lists m[] (complete on `st`, or posting their semaphores there) -> global-frame step, ONE tracker
+// chain for all tables, publication; the tick's events
+static int seq_finish(Ctx* c, SeqTick* t, int bank, cudaStream_t st, const SeqMeas* m, const double* ts, const double* v, const double* yaw) {
+  int rc;
+  Slot* k = &c->bank[bank];
+  if (c->prm.global_frame && (rc = seq_global_launch(c, m, c->n_seq, st, ts, v, yaw))) return rc;
+  LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, st));
+  if ((rc = seq_tracker_launch(c, m, t, c->n_seq, ts, v, yaw))) return rc;
+  LMOT_CUDA(c, cudaEventRecord(t->blocks[0].ev_done, c->pub_stream));
+  LMOT_CUDA(c, cudaEventRecord(k->ev_trk_done, c->pub_stream));
+  if (!t->in_flight) { t->in_flight = true; ++c->seq_in_flight; }
+  return LMOT_OK;
+}
+
+// detection front end (lmot_seq_submit / lmot_seq_dev)
 static int seq_common(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride, bool host, const double* ts,
                       const double* v, const double* yaw) {
   if (!ctx) return LMOT_ERR_INVALID;
@@ -1076,16 +1135,9 @@ static int seq_common(lmot_ctx* ctx, const float* const* points, const int* n, i
   if (c->n_seq == 0 || n_seq != c->n_seq || !points || !n || !ts || !v || !yaw) return LMOT_ERR_INVALID;
   if (c->timing) return LMOT_ERR_STATE;
   cudaSetDevice(c->device);
-  // the tick's frames: sequence k's sensors in table order, frames [f0[k], f0[k + 1]); one frame for a sequence without a table
-  // (lmot_seq_set_sensors keeps the total at or below kMaxBatch)
   int f0[kMaxBatch + 1];
-  bool rig_on[kMaxBatch], rigged = false;
-  f0[0] = 0;
-  for (int k = 0; k < n_seq; ++k) {
-    rig_on[k] = c->seq_n_sensors[k] > 0;
-    rigged |= rig_on[k];
-    f0[k + 1] = f0[k] + (rig_on[k] ? c->seq_n_sensors[k] : 1);
-  }
+  bool rig_on[kMaxBatch];
+  const bool rigged = seq_layout(c, f0, rig_on);
   const int F = f0[n_seq];
   for (int i = 0; i < F; ++i) {
     if (n[i] < 0 || (n[i] > 0 && !points[i])) return LMOT_ERR_INVALID;
@@ -1095,17 +1147,15 @@ static int seq_common(lmot_ctx* ctx, const float* const* points, const int* n, i
   if (host && (stride < 3 || c->seq_in_flight >= c->seq_ring)) return stride < 3 ? LMOT_ERR_INVALID : LMOT_ERR_STATE;
   int rc = batch_ensure(c, F);
   if (rc) return rc;
-  SeqTick* t = seq_acquire(c, !host);
-  if (!t) return LMOT_ERR_STATE;
-  const int b = c->next_bank;
-  c->next_bank = (c->next_bank + 1) % kBatchBanks;
+  SeqTick* t;
+  int b;
+  cudaStream_t st;
+  if ((rc = seq_begin(c, !host, false, &t, &b, &st))) return rc;
   Slot* k = &c->bank[b];
   Slot* sl[kMaxBatch];
   const float4* pp[kMaxBatch];
   for (int i = 0; i < F; ++i) sl[i] = &c->bslots[b * c->batch_frames + i];
-  cudaStream_t st = sl[0]->stream;
-  // the bank's previous tick must have been consumed by the tracker; device frames: ordered after the caller's stream
-  LMOT_CUDA(c, cudaStreamWaitEvent(st, k->ev_trk_done, 0));
+  // device frames: ordered after the caller's stream
   if (host) {
     for (int i = 0; i < F; ++i) {
       if ((rc = upload_points(c, sl[i], st, points[i], n[i], stride, sl[i]->d_points))) return rc;
@@ -1149,12 +1199,79 @@ static int seq_common(lmot_ctx* ctx, const float* const* points, const int* n, i
     if ((rc = boxfit_launch_batch(c, sl, F, st, n, false, rig))) return rc;
     if ((rc = boxes_concat_seq_launch(c, sl, n_seq, f0, rig_on, rig, m, fc, !gf, st))) return rc;
   }
-  if (gf && (rc = seq_global_launch(c, m, n_seq, st, ts, v, yaw))) return rc;
-  LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, st));
-  if ((rc = seq_tracker_launch(c, m, t, n_seq, ts, v, yaw))) return rc;
-  LMOT_CUDA(c, cudaEventRecord(t->blocks[0].ev_done, c->pub_stream));
-  LMOT_CUDA(c, cudaEventRecord(k->ev_trk_done, c->pub_stream));
-  if (!t->in_flight) { t->in_flight = true; ++c->seq_in_flight; }
+  return seq_finish(c, t, b, st, m, ts, v, yaw);
+}
+
+// tracking-only front end (lmot_seq_track_submit / lmot_seq_track_dev): host lists (boxes / m, staged on the device first) or padded
+// device lists (d_lists / d_counts, cap boxes each) -> pack_lists_seq_kernel into each sequence's measurement list on the bank
+static int seq_lists_common(lmot_ctx* ctx, const float* const* boxes, const int* m, const float* d_lists, const int* d_counts, int cap, int n_seq,
+                            bool host, const double* ts, const double* v, const double* yaw) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  if (c->n_seq == 0 || n_seq != c->n_seq || !ts || !v || !yaw) return LMOT_ERR_INVALID;
+  if (host ? (!boxes || !m) : (!d_lists || !d_counts || cap < 1)) return LMOT_ERR_INVALID;
+  if (c->timing) return LMOT_ERR_STATE;
+  cudaSetDevice(c->device);
+  int f0[kMaxBatch + 1];
+  bool rig_on[kMaxBatch];
+  seq_layout(c, f0, rig_on);
+  const int F = f0[n_seq];
+  if (host) {
+    for (int i = 0; i < F; ++i) if (m[i] < 0 || (m[i] > 0 && !boxes[i])) return LMOT_ERR_INVALID;
+    for (int i = 0; i < F; ++i) if (m[i] > c->prm.max_boxes) return LMOT_ERR_CAPACITY;
+    if (c->seq_in_flight >= c->seq_ring) return LMOT_ERR_STATE;
+  }
+  int rc;
+  if (!c->bank[0].stream) {            // a tracking tick needs the banks' events and streams, not their detection slots
+    if ((rc = bank_ensure(c))) return rc;
+    LMOT_CUDA(c, cudaDeviceSynchronize());
+  }
+  SeqTick* t;
+  int b;
+  cudaStream_t st;
+  if ((rc = seq_begin(c, !host, true, &t, &b, &st))) return rc;
+  struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
+  if (host) {
+    // list i at i * max_boxes boxes of the bank's staging buffer (16-byte aligned), the counts behind the lists.  The copies are
+    // ordered after the bank's previous tick (seq_begin), whose pack kernel was the last reader.
+    const int MB = c->prm.max_boxes;
+    float* stage = c->seq_stage[b];
+    int* counts = reinterpret_cast<int*>(stage + (size_t)kMaxBatch * MB * 24);
+    for (int i = 0; i < F; ++i)
+      if (m[i] > 0) LMOT_CUDA(c, cudaMemcpyAsync(stage + (size_t)i * MB * 24, boxes[i], (size_t)m[i] * 24 * sizeof(float), cudaMemcpyHostToDevice, st));
+    LMOT_CUDA(c, cudaMemcpyAsync(counts, m, (size_t)F * sizeof(int), cudaMemcpyHostToDevice, st));
+    d_lists = stage; d_counts = counts; cap = MB;
+  } else {
+    LMOT_CUDA(c, cudaEventRecord(c->bank[b].ev_fork, c->stream));      // the caller's stream produced the lists
+    LMOT_CUDA(c, cudaStreamWaitEvent(st, c->bank[b].ev_fork, 0));
+  }
+  // sequence k's lists: poses of its table (copied into the launch parameters), its measurement list on the bank, per-list counts into
+  // its result block
+  lmot_sensor rig[kMaxBatch];
+  int* fc[kMaxBatch];
+  SeqMeas mm[kMaxBatch];
+  for (int k = 0; k < n_seq; ++k) {
+    for (int j = f0[k]; j < f0[k + 1]; ++j) {
+      if (rig_on[k]) rig[j] = c->seq_sensors[k][j - f0[k]];
+      else lmot_default_sensor(&c->prm, &rig[j]);
+    }
+    mm[k] = c->seq_meas[b][k];
+    Result* r = &t->blocks[k];
+    r->n_kev = 0; r->has_tracks = true;
+    r->batch_frames = f0[k + 1] - f0[k];
+    LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc[k], r->h_frame_counts, 0));
+  }
+  const bool gf = c->prm.global_frame != 0;
+  if ((rc = boxes_pack_lists_seq_launch(c, st, d_lists, d_counts, cap, n_seq, f0, rig_on, rig, mm, fc, !gf))) return rc;
+  return seq_finish(c, t, b, st, mm, ts, v, yaw);
+}
+
+// uncollected ticks are dropped, as lmot_batch drops uncollected results
+static int seq_drop_uncollected(Ctx* c) {
+  if (c->seq_in_flight > 0) {
+    LMOT_CUDA(c, cudaEventSynchronize(c->seq_last->blocks[0].ev_done));    // (ticks are published in submission order)
+    seq_forget(c);
+  }
   return LMOT_OK;
 }
 
@@ -1195,12 +1312,29 @@ int lmot_seq_fetch(lmot_ctx* ctx, lmot_seq_out* out) {
 int lmot_seq(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride_floats, const double* timestamp_us,
              const double* v_gps, const double* yaw_gps, lmot_seq_out* out) {
   if (!ctx) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  if (c->seq_in_flight > 0) {          // uncollected ticks are dropped, as lmot_batch drops uncollected results
-    LMOT_CUDA(c, cudaEventSynchronize(c->seq_last->blocks[0].ev_done));    // (ticks are published in submission order)
-    seq_forget(c);
-  }
-  int rc = lmot_seq_submit(ctx, points, n, n_seq, stride_floats, timestamp_us, v_gps, yaw_gps);
+  int rc = seq_drop_uncollected(&ctx->c);
+  if (rc) return rc;
+  rc = lmot_seq_submit(ctx, points, n, n_seq, stride_floats, timestamp_us, v_gps, yaw_gps);
+  if (rc) return rc;
+  return lmot_seq_collect(ctx, out);
+}
+
+int lmot_seq_track_submit(lmot_ctx* ctx, const float* const* boxes, const int* m, int n_seq, const double* timestamp_us, const double* v_gps,
+                          const double* yaw_gps) {
+  return seq_lists_common(ctx, boxes, m, nullptr, nullptr, 0, n_seq, true, timestamp_us, v_gps, yaw_gps);
+}
+
+int lmot_seq_track_dev(lmot_ctx* ctx, const float* d_lists, const int* d_counts, int n_seq, int cap_per_list, const double* timestamp_us,
+                       const double* v_gps, const double* yaw_gps) {
+  return seq_lists_common(ctx, nullptr, nullptr, d_lists, d_counts, cap_per_list, n_seq, false, timestamp_us, v_gps, yaw_gps);
+}
+
+int lmot_seq_track(lmot_ctx* ctx, const float* const* boxes, const int* m, int n_seq, const double* timestamp_us, const double* v_gps,
+                   const double* yaw_gps, lmot_seq_out* out) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  int rc = seq_drop_uncollected(&ctx->c);
+  if (rc) return rc;
+  rc = lmot_seq_track_submit(ctx, boxes, m, n_seq, timestamp_us, v_gps, yaw_gps);
   if (rc) return rc;
   return lmot_seq_collect(ctx, out);
 }
@@ -1441,10 +1575,9 @@ int lmot_tracker_dump(lmot_ctx* ctx, double* dumps, int cap, int* n_out) {
   return tracker_dump(&ctx->c, ctx->c.own, dumps, cap, n_out);
 }
 
-int lmot_tracker_load(lmot_ctx* ctx, const double* dumps, int n, int init, double timestamp_us, double ego_velo,
-                      double ego_yaw, double ego_pre_yaw, double ego_point_yaw) {
-  if (!ctx || n < 0 || (n > 0 && !dumps)) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
+static int tracker_load(Ctx* c, Tracker& trk, const double* dumps, int n, int init, double timestamp_us, double ego_velo, double ego_yaw,
+                        double ego_pre_yaw, double ego_point_yaw) {
+  if (n < 0 || (n > 0 && !dumps)) return LMOT_ERR_INVALID;
   if (n > c->prm.max_tracks) return LMOT_ERR_CAPACITY;
   int rc = drain(c);
   if (rc) return rc;
@@ -1465,19 +1598,25 @@ int lmot_tracker_load(lmot_ctx* ctx, const double* dumps, int n, int init, doubl
     t.nBBox = (int)d[D_BBN]; for (int p = 0; p < t.nBBox && p < 8; ++p) for (int q = 0; q < 3; ++q) t.BBox[p][q] = (float)d[D_BB + 3 * p + q];
     t.nBest = (int)d[D_BESTBBN]; for (int p = 0; p < t.nBest && p < 8; ++p) for (int q = 0; q < 3; ++q) t.bestBBox[p][q] = (float)d[D_BESTBB + 3 * p + q];
   }
-  if (n > 0) LMOT_CUDA(c, cudaMemcpyAsync(c->own.d_tracks, h.data(), (size_t)n * sizeof(TrackState), cudaMemcpyHostToDevice, c->stream));
-  c->own.h_trk_counters[CNT_N_TRACKS] = n;
-  LMOT_CUDA(c, cudaMemsetAsync(c->own.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
-  LMOT_CUDA(c, cudaMemcpyAsync(c->own.d_trk_counters + CNT_N_TRACKS, c->own.h_trk_counters + CNT_N_TRACKS, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  if (n > 0) LMOT_CUDA(c, cudaMemcpyAsync(trk.d_tracks, h.data(), (size_t)n * sizeof(TrackState), cudaMemcpyHostToDevice, c->stream));
+  trk.h_trk_counters[CNT_N_TRACKS] = n;
+  LMOT_CUDA(c, cudaMemsetAsync(trk.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
+  LMOT_CUDA(c, cudaMemcpyAsync(trk.d_trk_counters + CNT_N_TRACKS, trk.h_trk_counters + CNT_N_TRACKS, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->own.act_valid = false;
-  c->own.th = TrackerHost();
-  c->own.th.init = init != 0; c->own.th.timestamp = timestamp_us; c->own.th.egoVelo = ego_velo; c->own.th.egoYaw = ego_yaw;
-  c->own.th.egoPreYaw = ego_pre_yaw; c->own.th.egoPoint[2] = ego_point_yaw;
+  trk.act_valid = false;
+  trk.th = TrackerHost();
+  trk.th.init = init != 0; trk.th.timestamp = timestamp_us; trk.th.egoVelo = ego_velo; trk.th.egoYaw = ego_yaw;
+  trk.th.egoPreYaw = ego_pre_yaw; trk.th.egoPoint[2] = ego_point_yaw;
   // (like the oracle's ref_tracker_load, which clears egoDeltaHis_: the dead-reckoning fold restarts from (0, 0, -pi/2) and
   //  ego_point_yaw is only egoPoints_[0][2] until the next step recomputes it.  A checkpoint that must keep the accumulated ego
   //  pose restores it with lmot_tracker_set_ego.)
   return LMOT_OK;
+}
+
+int lmot_tracker_load(lmot_ctx* ctx, const double* dumps, int n, int init, double timestamp_us, double ego_velo,
+                      double ego_yaw, double ego_pre_yaw, double ego_point_yaw) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  return tracker_load(&ctx->c, ctx->c.own, dumps, n, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw);
 }
 
 // the frame-level scalars of getOriginPoints / immUkfJpdaf (imm_ukf_jpda.cpp:19-24,56-58) incl. the accumulated dead-reckoning pose
@@ -1512,16 +1651,36 @@ int lmot_seq_tracker_get_ego(lmot_ctx* ctx, int k, double ego8[8]) {
   return LMOT_OK;
 }
 
-int lmot_tracker_set_ego(lmot_ctx* ctx, const double ego8[8]) {
-  if (!ctx || !ego8) return LMOT_ERR_INVALID;
+int lmot_seq_tracker_load(lmot_ctx* ctx, int k, const double* dumps, int n, int init, double timestamp_us, double ego_velo, double ego_yaw,
+                          double ego_pre_yaw, double ego_point_yaw) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
+  const int rc = tracker_load(c, c->seq[k], dumps, n, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw);
+  if (rc == LMOT_OK) seq_forget(c);        // (as lmot_seq_tracker_reset: the drained ticks are dropped)
+  return rc;
+}
+
+static int tracker_set_ego(Ctx* c, Tracker& t, const double ego8[8]) {
   int rc = drain(c);
   if (rc) return rc;
-  TrackerHost& h = c->own.th;
+  TrackerHost& h = t.th;
   h.init = ego8[0] != 0.0; h.timestamp = ego8[1]; h.egoVelo = ego8[2]; h.egoYaw = ego8[3]; h.egoPreYaw = ego8[4];
   h.fold[0] = ego8[5]; h.fold[1] = ego8[6]; h.fold[2] = ego8[7];
   h.egoPoint[0] = h.fold[0]; h.egoPoint[1] = h.fold[1]; h.egoPoint[2] = h.fold[2];
   return LMOT_OK;
+}
+
+int lmot_tracker_set_ego(lmot_ctx* ctx, const double ego8[8]) {
+  if (!ctx || !ego8) return LMOT_ERR_INVALID;
+  return tracker_set_ego(&ctx->c, ctx->c.own, ego8);
+}
+
+int lmot_seq_tracker_set_ego(lmot_ctx* ctx, int k, const double ego8[8]) {
+  if (!ctx || !ego8 || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  const int rc = tracker_set_ego(c, c->seq[k], ego8);
+  if (rc == LMOT_OK) seq_forget(c);
+  return rc;
 }
 
 // ---------------------------------------------------------------------------------------------- inspection

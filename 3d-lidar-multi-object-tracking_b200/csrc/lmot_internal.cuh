@@ -235,7 +235,8 @@ struct Ctx {
   // ---- batched ticks (lmot_batch_*): own detection slots, kBatchBanks x batch_frames, allocated on first use
   Slot bslots[kBatchBanks * kMaxBatch];
   int n_bslots = 0, batch_frames = 0, next_bank = 0;
-  Slot bank[kBatchBanks];              // pseudo-slots: concatenated boxes + counters + semaphore + events of a bank
+  Slot bank[kBatchBanks];              // pseudo-slots: concatenated boxes + counters + semaphore + events of a bank, and the stream its
+                                       // tracking-only sequence ticks (lmot_seq_track*) run on
   // ---- sensor rig (lmot_set_sensors): sensor k = frame k of a batched tick / list k of lmot_track_step_lists_dev; read at submission
   int n_sensors = 0;                   // 0: every frame uses prm, the rig kernels are never launched
   lmot_sensor sensors[kMaxBatch];
@@ -265,6 +266,8 @@ struct Ctx {
   int seq_n_sensors[kMaxBatch] = {};
   lmot_sensor seq_sensors[kMaxBatch][kMaxBatch];
   SeqMeas seq_meas[kBatchBanks][kMaxBatch];    // per-sequence measurement lists of each batch bank, allocated by lmot_seq_open
+  // staging of lmot_seq_track_submit's host lists, per bank: kMaxBatch lists of max_boxes boxes, then kMaxBatch counts (lmot_seq_open)
+  float* seq_stage[kBatchBanks] = {};
   int seq_fc_n[kMaxBatch] = {};                // lmot_seq_frame_counts: frames of sequence k in the tick collected last
   int seq_fc[kMaxBatch][kMaxBatch][4] = {};    // ... and their n_elev, n_ground, num_cluster, n_boxes (host copies: the ring slot is reused)
 
@@ -348,6 +351,9 @@ int tracker_publish(Ctx* c, Result* r, cudaStream_t st);            // device bl
 // sequence ticks with sensor tables: sequence k's frames [f0[k], f0[k + 1]) of `slots` -> m[k] (boxfit.cu)
 int boxes_concat_seq_launch(Ctx* c, Slot* const* slots, int S, const int* f0, const bool* rig_on, const lmot_sensor* rig, const SeqMeas* m,
                             int* const* frame_counts, bool post_sem, cudaStream_t st);
+// tracking-only sequence ticks: sequence k's padded lists [f0[k], f0[k + 1]) of d_lists (cap boxes each, lengths in d_counts) -> m[k] (boxfit.cu)
+int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int cap, int S, const int* f0, const bool* rig_on,
+                                const lmot_sensor* rig, const SeqMeas* m, int* const* frame_counts, bool post_sem);
 // sequence ticks: measurement list m[k] -> track table c->seq[k] -> tick->blocks[k] (tracker.cu)
 int seq_global_launch(Ctx* c, const SeqMeas* m, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw);
 int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw);

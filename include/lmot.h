@@ -311,8 +311,9 @@ int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n);   /*
  * lmot_seq_open(ctx, n_seq, ring): drains the context and replaces the set with n_seq (1..LMOT_MAX_BATCH) empty sequences, each at
  *   its first frame, and a ring of `ring` (1..64) ticks.  n_seq = 0 frees the set.  Memory: n_seq track tables (device, max_tracks x
  *   ~2.6 KB incl. side arrays at max_boxes 1024) plus ring x n_seq result blocks (each max_boxes x 96 B + max_tracks x 130 B of pinned host memory and
- *   the same again on the device), and per sequence 2 x 2 x max_boxes x 96 B of device memory (a measurement list and its global-frame
- *   copy for each of the two detection banks) -- size max_tracks and ring for it.  Reopening (or closing) also clears every sequence's sensor table.
+ *   the same again on the device), per sequence 2 x 2 x max_boxes x 96 B of device memory (a measurement list and its global-frame
+ *   copy for each of the two detection banks), and 2 x 8 x max_boxes x 96 B of device memory (~1.5 MB at max_boxes 1024) staging the
+ *   host lists of lmot_seq_track_submit -- size max_tracks and ring for it.  Reopening (or closing) also clears every sequence's sensor table.
  * lmot_seq_submit : HOST frames (stride in floats), LMOT_ERR_STATE if `ring` ticks wait to be collected.
  * lmot_seq_dev    : DEVICE frames (stride 4 floats, 16-byte aligned), ordered after the caller stream; a full ring drops the oldest tick.
  * points / n hold one entry per FRAME of the tick, in sequence order: sequence 0's frames (its sensors in table order, or its one
@@ -351,6 +352,48 @@ int lmot_seq_tracker_get_ego(lmot_ctx* ctx, int k, double ego8[8]);
 int lmot_seq_set_sensors(lmot_ctx* ctx, int k, const lmot_sensor* s, int n);
 int lmot_seq_get_sensors(const lmot_ctx* ctx, int k, lmot_sensor* s, int cap, int* n);
 int lmot_seq_frame_counts(lmot_ctx* ctx, int k, int counts[LMOT_MAX_BATCH][4], int* n_frames);
+
+/* ---- tracking-only sequence ticks: each sequence's tracker fed with box lists from elsewhere (another detector, a detection log) -----
+ * The sequence form of lmot_track_step: one tick carries the box lists of all n_seq sequences, and ONE tracker chain steps all tables
+ * (no ground removal, clustering or box fitting runs).  Lists follow the frame layout of a detection tick: one list per sensor of a
+ * sequence with a table (table order), one list for a sequence without one, in sequence order.  A box is float[8*3] as for
+ * lmot_track_step; timestamp_us / v_gps / yaw_gps are arrays of n_seq as for lmot_seq_submit.
+ *
+ * Sequence k gives bit for bit what a separate context with the same lmot_params gives: without a table, lmot_track_step on its list;
+ * with a table, lmot_set_sensors(that table) and lmot_track_step_lists_dev on its lists (each list's boxes moved into the VEHICLE
+ * frame by its sensor's pose, as lmot_track_step_lists_dev does) -- targets, vandyaw, trackManage, static / visible flags, vis_bb,
+ * the status and lmot_seq_tracker_dump, with global_frame 0 or 1.  out->seq[k]: boxes / n_boxes are the list that was tracked,
+ * before the global-frame step (the caller's list, or the concatenated vehicle-frame list); n_elevated, n_ground and num_cluster are
+ * 0; lmot_seq_frame_counts(k) gives one row (0, 0, 0, length) per list.  A sequence whose lists together exceed max_boxes reports
+ * LMOT_ERR_CAPACITY at collect with its list cut at max_boxes, as its lmot_track_step_lists_dev twin does; the other sequences of the
+ * tick are unaffected.
+ *
+ * Ticks use the ring of lmot_seq_*: lmot_seq_collect / lmot_seq_fetch, the same LMOT_ERR_STATE (host lists) and drop-oldest (device
+ * lists) rules.  A set may mix detection ticks (lmot_seq*) and tracking ticks in any order; each table folds its steps in submission
+ * order.  One tick is all-detection or all-tracking: a tick that feeds some sequences frames and others box lists is not supported.
+ * lmot_seq_track_submit: HOST lists boxes[i] of m[i] boxes.  LMOT_ERR_CAPACITY, nothing submitted: a list above max_boxes.  The
+ *   lists and m are copied to a device staging buffer of the bank during the call (copies from pageable memory complete before the
+ *   call returns; page-locked lists must stay untouched until lmot_flush has joined or the tick has been collected).
+ * lmot_seq_track_dev: padded DEVICE lists as lmot_track_step_lists_dev takes them: list i at d_lists + i * cap_per_list * 24 floats
+ *   (4-byte alignment suffices), its length in d_counts[i], clamped to [0, cap_per_list].  The tick is ordered after the work queued on
+ *   the caller stream; the caller may overwrite the lists once lmot_flush has made its stream wait for the tick (or the tick has been
+ *   collected), as for the frames of lmot_seq_dev.
+ * lmot_seq_track: submit + collect, dropping uncollected ticks as lmot_seq does.
+ * LMOT_ERR_INVALID: no open set, n_seq != the set's, null pointers, a negative m[i], cap_per_list < 1.  LMOT_ERR_STATE: timing mode.
+ *
+ * lmot_seq_tracker_load / lmot_seq_tracker_set_ego: lmot_tracker_load / lmot_tracker_set_ego applied to sequence k (same arguments
+ * and rules; they drain first and drop uncollected sequence ticks, as lmot_seq_tracker_reset does).  k out of range: LMOT_ERR_INVALID;
+ * n > max_tracks: LMOT_ERR_CAPACITY.  With lmot_seq_tracker_dump / lmot_seq_tracker_get_ego they move a sequence's checkpoint between
+ * sequences and contexts (and to or from a context's own tracker). */
+int lmot_seq_track_submit(lmot_ctx* ctx, const float* const* boxes, const int* m, int n_seq, const double* timestamp_us, const double* v_gps,
+                          const double* yaw_gps);
+int lmot_seq_track_dev(lmot_ctx* ctx, const float* d_lists, const int* d_counts, int n_seq, int cap_per_list, const double* timestamp_us,
+                       const double* v_gps, const double* yaw_gps);
+int lmot_seq_track(lmot_ctx* ctx, const float* const* boxes, const int* m, int n_seq, const double* timestamp_us, const double* v_gps,
+                   const double* yaw_gps, lmot_seq_out* out);
+int lmot_seq_tracker_load(lmot_ctx* ctx, int k, const double* dumps, int n, int init, double timestamp_us, double ego_velo,
+                          double ego_yaw, double ego_pre_yaw, double ego_point_yaw);
+int lmot_seq_tracker_set_ego(lmot_ctx* ctx, int k, const double ego8[8]);
 
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
