@@ -83,6 +83,57 @@ class Sensor(C.Structure):
     _fields_ = [("pose", C.c_float * 12), ("h_sensor", C.c_float), ("t_hmin", C.c_float), ("t_hmax", C.c_float), ("sensor_height", C.c_float)]
 
 
+class TrackerParams(C.Structure):
+    """lmot_tracker_params: the IMM-UKF-PDA noise, gating and track-management constants of one track table."""
+    _fields_ = [
+        ("gamma_g", C.c_double), ("p_g", C.c_double), ("p_d", C.c_double), ("distance_thres", C.c_double), ("lifetime_thres", C.c_int),
+        ("bb_yaw_change_thres", C.c_double), ("second_init_v", C.c_double), ("static_lifetime", C.c_int), ("static_dist", C.c_double),
+        ("std_a", C.c_double * 3), ("std_yawdd", C.c_double * 3), ("std_las_x", C.c_double), ("std_las_y", C.c_double),
+        ("trans", (C.c_double * 3) * 3), ("mode_prob0", C.c_double * 3), ("p0_diag", C.c_double * 5),
+    ]
+
+
+def _tracker_params_dict(p: TrackerParams) -> dict:
+    out = {}
+    for name, _ in TrackerParams._fields_:
+        v = getattr(p, name)
+        if name == "trans":
+            out[name] = [list(row) for row in v]
+        elif isinstance(v, C.Array):
+            out[name] = list(v)
+        else:
+            out[name] = v
+    return out
+
+
+def default_tracker_params() -> dict:
+    """lmot_default_tracker_params as a dict of field -> value (lists for the array fields)"""
+    p = TrackerParams()
+    load_library().lmot_default_tracker_params(C.byref(p))
+    return _tracker_params_dict(p)
+
+
+def _tracker_params(fields: dict) -> TrackerParams:
+    """the defaults with `fields` replaced (unknown names raise)"""
+    p = TrackerParams()
+    load_library().lmot_default_tracker_params(C.byref(p))
+    names = dict(TrackerParams._fields_)
+    for name, val in fields.items():
+        if name not in names:
+            raise ValueError(f"unknown tracker parameter {name!r}")
+        if name == "trans":
+            a = np.asarray(val, np.float64).reshape(3, 3)
+            for i in range(3):
+                p.trans[i][:] = [float(x) for x in a[i]]
+        elif name in ("std_a", "std_yawdd", "mode_prob0", "p0_diag"):
+            getattr(p, name)[:] = [float(x) for x in np.asarray(val, np.float64).reshape(-1)]
+        elif names[name] is C.c_int:
+            setattr(p, name, int(val))
+        else:
+            setattr(p, name, float(val))
+    return p
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -105,6 +156,8 @@ ABI_SYMBOLS = [
     "lmot_seq_open", "lmot_seq_submit", "lmot_seq_dev", "lmot_seq_collect", "lmot_seq_fetch", "lmot_seq", "lmot_seq_tracker_reset",
     "lmot_seq_tracker_dump", "lmot_seq_tracker_get_ego", "lmot_seq_set_sensors", "lmot_seq_get_sensors", "lmot_seq_frame_counts",
     "lmot_seq_track_submit", "lmot_seq_track_dev", "lmot_seq_track", "lmot_seq_tracker_load", "lmot_seq_tracker_set_ego",
+    "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
+    "lmot_seq_get_tracker_params",
     "lmot_detect_boxes_dev", "lmot_track_step_lists_dev", "lmot_tracker_counters_dev", "lmot_tracker_table_received",
     "lmot_origin_points", "lmot_tracker_table", "lmot_tracker_set_num_tracks", "lmot_tracker_reset", "lmot_tracker_num_tracks", "lmot_tracker_dump", "lmot_tracker_load", "lmot_tracker_get_ego", "lmot_tracker_set_ego",
     "lmot_debug_polar_grid", "lmot_debug_cell_index", "lmot_debug_label_grid", "lmot_selftest_atan2f",
@@ -506,6 +559,26 @@ class Lmot:
         n = C.c_int(0)
         self._chk(self.lib.lmot_seq_get_sensors(self.h, int(k), arr, MAX_BATCH, C.byref(n)))
         return self._sensor_dict(arr[: n.value])
+
+    # ---- tracker parameters (lmot_set_tracker_params / lmot_seq_set_tracker_params) --------------------------------------------
+    def set_tracker_params(self, **fields):
+        """The context's own track table: the given fields, every other one at its default (no fields: the defaults).
+        Array fields take sequences (std_a (3,), trans (3, 3), ...).  Applies from the next submitted step on."""
+        self._chk(self.lib.lmot_set_tracker_params(self.h, C.byref(_tracker_params(fields)) if fields else None))
+
+    def get_tracker_params(self) -> dict:
+        p = TrackerParams()
+        self._chk(self.lib.lmot_get_tracker_params(self.h, C.byref(p)))
+        return _tracker_params_dict(p)
+
+    def seq_set_tracker_params(self, k: int, **fields):
+        """Sequence k's parameters, arguments as set_tracker_params."""
+        self._chk(self.lib.lmot_seq_set_tracker_params(self.h, int(k), C.byref(_tracker_params(fields)) if fields else None))
+
+    def seq_get_tracker_params(self, k: int) -> dict:
+        p = TrackerParams()
+        self._chk(self.lib.lmot_seq_get_tracker_params(self.h, int(k), C.byref(p)))
+        return _tracker_params_dict(p)
 
     def seq_frame_counts(self, k: int) -> np.ndarray:
         """(n_frames, 4) int32: n_elevated, n_ground, num_cluster, n_boxes of each of sequence k's frames in the tick collected last"""

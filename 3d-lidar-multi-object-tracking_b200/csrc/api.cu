@@ -1464,6 +1464,72 @@ int lmot_seq_frame_counts(lmot_ctx* ctx, int k, int counts[LMOT_MAX_BATCH][4], i
   return LMOT_OK;
 }
 
+// ---------------------------------------------------------------------------------------------- tracker parameters
+int lmot_default_tracker_params(lmot_tracker_params* p) {
+  if (!p) return LMOT_ERR_INVALID;
+  *p = tracker_params_defaults();
+  return LMOT_OK;
+}
+
+static bool tracker_params_valid(const lmot_tracker_params& p) {
+  const double pos[] = {p.gamma_g, p.std_a[0], p.std_a[1], p.std_a[2], p.std_yawdd[0], p.std_yawdd[1], p.std_yawdd[2], p.std_las_x,
+                        p.std_las_y, p.p0_diag[0], p.p0_diag[1], p.p0_diag[2], p.p0_diag[3], p.p0_diag[4]};
+  const double prob[] = {p.p_g, p.p_d, p.mode_prob0[0], p.mode_prob0[1], p.mode_prob0[2]};
+  const double other[] = {p.distance_thres, p.bb_yaw_change_thres, p.second_init_v, p.static_dist};
+  for (double v : pos) if (!std::isfinite(v) || !(v > 0)) return false;
+  for (double v : prob) if (!std::isfinite(v) || !(v > 0 && v <= 1)) return false;
+  for (double v : other) if (!std::isfinite(v)) return false;
+  for (int j = 0; j < 3; ++j) {
+    bool any = false;
+    for (int i = 0; i < 3; ++i) {
+      const double v = p.trans[i][j];
+      if (!std::isfinite(v) || v < 0 || v > 1) return false;
+      any |= v > 0;
+    }
+    if (!any) return false;
+  }
+  return p.lifetime_thres >= 0 && p.static_lifetime >= 0;
+}
+
+// host state only, as the sensor tables: submitted steps carry their own copy in their launch parameters
+static int tracker_params_set(Tracker& t, const lmot_tracker_params* p) {
+  const lmot_tracker_params d = tracker_params_defaults();
+  if (p && !tracker_params_valid(*p)) return LMOT_ERR_INVALID;
+  t.prm = p ? *p : d;
+  // field by field (a caller's struct may carry anything in its padding)
+  const lmot_tracker_params& q = t.prm;
+  bool same = q.gamma_g == d.gamma_g && q.p_g == d.p_g && q.p_d == d.p_d && q.distance_thres == d.distance_thres &&
+              q.lifetime_thres == d.lifetime_thres && q.bb_yaw_change_thres == d.bb_yaw_change_thres && q.second_init_v == d.second_init_v &&
+              q.static_lifetime == d.static_lifetime && q.static_dist == d.static_dist && q.std_las_x == d.std_las_x && q.std_las_y == d.std_las_y;
+  for (int m = 0; m < 3; ++m) same = same && q.std_a[m] == d.std_a[m] && q.std_yawdd[m] == d.std_yawdd[m] && q.mode_prob0[m] == d.mode_prob0[m];
+  for (int i = 0; i < 9; ++i) same = same && q.trans[i / 3][i % 3] == d.trans[i / 3][i % 3];
+  for (int i = 0; i < 5; ++i) same = same && q.p0_diag[i] == d.p0_diag[i];
+  t.tuned = !same;
+  return LMOT_OK;
+}
+
+int lmot_set_tracker_params(lmot_ctx* ctx, const lmot_tracker_params* p) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  return tracker_params_set(ctx->c.own, p);
+}
+
+int lmot_get_tracker_params(const lmot_ctx* ctx, lmot_tracker_params* p) {
+  if (!ctx || !p) return LMOT_ERR_INVALID;
+  *p = ctx->c.own.prm;
+  return LMOT_OK;
+}
+
+int lmot_seq_set_tracker_params(lmot_ctx* ctx, int k, const lmot_tracker_params* p) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  return tracker_params_set(ctx->c.seq[k], p);
+}
+
+int lmot_seq_get_tracker_params(const lmot_ctx* ctx, int k, lmot_tracker_params* p) {
+  if (!ctx || !p || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  *p = ctx->c.seq[k].prm;
+  return LMOT_OK;
+}
+
 // after the table was received from another rank (NCCL broadcast into lmot_tracker_table's pointer, count already in the device
 // counter lmot_tracker_counters_dev points at): rebuild the side arrays before the next step.  n = the count, as the host knows it.
 int lmot_tracker_table_received(lmot_ctx* ctx, int n) {

@@ -171,10 +171,30 @@ constexpr int kMaxSlots = 8;
 constexpr int kBatchBanks = 2;                       // batched ticks: detection of tick t+1 overlaps the tracker of tick t
 constexpr int kMaxResults = 64;
 
+// lmot_default_tracker_params: the reference's constants (citations in include/lmot.h)
+inline lmot_tracker_params tracker_params_defaults() {
+  lmot_tracker_params p = {};
+  p.gamma_g = 9.22; p.p_g = 0.99; p.p_d = 0.9;
+  p.distance_thres = 99; p.lifetime_thres = 3;
+  p.bb_yaw_change_thres = 0.2;
+  p.second_init_v = 2;
+  p.static_lifetime = 8; p.static_dist = 3.0;
+  for (int m = 0; m < 3; ++m) { p.std_a[m] = (m == 2) ? 3 : 2; p.std_yawdd[m] = (m == 2) ? 3 : 2; }
+  p.std_las_x = 0.15; p.std_las_y = 0.15;
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) p.trans[i][j] = (i == j) ? 0.9 : 0.05;
+  for (int m = 0; m < 3; ++m) p.mode_prob0[m] = 0.33;
+  const double d[5] = {0.5, 0.5, 3, 10, 1};
+  for (int i = 0; i < 5; ++i) p.p0_diag[i] = d[i];
+  return p;
+}
+
 // One track table and everything the tracker chain carries from one step to the next.  The context's own tracker is one; every
 // sequence of lmot_seq_* (an independent frame stream) is another.
 struct Tracker {
   TrackerHost th;
+  lmot_tracker_params prm = tracker_params_defaults();   // lmot_set_tracker_params / lmot_seq_set_tracker_params; read at submission
+  bool tuned = false;                  // prm differs from the defaults: the chain runs the kernels that read it (tracker.cu)
   TrackState* d_tracks = nullptr;      // [max_tracks] append-only table; dead tracks keep their slot
   int* d_trk_counters = nullptr;       // [CNT_COUNT] CNT_N_TRACKS / CNT_N_VIS / CNT_ERROR of the track table
   int* h_trk_counters = nullptr;       // pinned mirror

@@ -45,6 +45,57 @@ constexpr int lifeTimeThres = 3;                        // :42
 constexpr double distanceThres = 99;                    // :38
 constexpr double bbYawChangeThres = 0.2;                // :46
 
+// ---- where the tracker's constants come from (lmot_tracker_params).  TA, TB and TC are templates on a parameter source: the
+// Def* sources return the reference's constants as compile-time values (the kernels every table at the defaults runs); the Tun*
+// sources read the stage's own slice of a table's parameters, which travels by value in the launch's parameter block.
+struct TAPrm { double gamma_g, std_a[3], std_yawdd[3], std_las_x, std_las_y, trans[3][3]; };
+struct TBPrm { double gamma_g, p_g, p_d, distance_thres, bb_yaw_change_thres, second_init_v; int lifetime_thres; };
+struct TCPrm { double p0_diag[5], mode_prob0[3], static_dist; int static_lifetime; };
+
+struct DefTA {
+  __device__ static constexpr double gamma_g() { return gammaG; }
+  __device__ static constexpr double std_a(int m) { return (m == 2) ? 3.0 : 2.0; }       // std_a_{cv,ctrv,rm}_ ukf.cpp:68-70
+  __device__ static constexpr double std_yawdd(int m) { return (m == 2) ? 3.0 : 2.0; }   // std_*_yawdd_ :71-73
+  __device__ static constexpr double r(int i) { return 0.15 * 0.15; }                   // std_laspx_ / std_laspy_ squared, :91-94
+  __device__ static constexpr double trans(int i, int j) { return (i == j) ? 0.9 : 0.05; }   // p{i+1}_[j], :144-154
+};
+struct TunTA {
+  const TAPrm& p;
+  __device__ double gamma_g() const { return p.gamma_g; }
+  __device__ double std_a(int m) const { return p.std_a[m]; }
+  __device__ double std_yawdd(int m) const { return p.std_yawdd[m]; }
+  __device__ double r(int i) const { return i == 0 ? p.std_las_x * p.std_las_x : p.std_las_y * p.std_las_y; }
+  __device__ double trans(int i, int j) const { return p.trans[i][j]; }
+};
+struct DefTB {
+  __device__ static constexpr double gamma_g() { return gammaG; }
+  __device__ static constexpr double p_g() { return pG; }
+  __device__ static constexpr double p_d() { return pD; }
+  __device__ static constexpr double distance_thres() { return distanceThres; }
+  __device__ static constexpr int lifetime_thres() { return lifeTimeThres; }
+  __device__ static constexpr double second_init_v() { return 2; }                     // targetV, imm_ukf_jpda.cpp:902
+};
+struct TunTB {
+  const TBPrm& p;
+  __device__ double gamma_g() const { return p.gamma_g; }
+  __device__ double p_g() const { return p.p_g; }
+  __device__ double p_d() const { return p.p_d; }
+  __device__ double distance_thres() const { return p.distance_thres; }
+  __device__ int lifetime_thres() const { return p.lifetime_thres; }
+  __device__ double second_init_v() const { return p.second_init_v; }
+};
+struct DefTC {
+  __device__ static constexpr double mode_prob0(int m) { return 0.33; }                // ukf.cpp:180-182
+  __device__ static constexpr int static_lifetime() { return 8; }                      // imm_ukf_jpda.cpp:1064
+  __device__ static constexpr double static_dist() { return 3.0; }                     // :1067
+};
+struct TunTC {
+  const TCPrm& p;
+  __device__ double mode_prob0(int m) const { return p.mode_prob0[m]; }
+  __device__ int static_lifetime() const { return p.static_lifetime; }
+  __device__ double static_dist() const { return p.static_dist; }
+};
+
 // Programmatic dependent launch (sm_90+): the three kernels of the tracker chain are launched back to back on one stream.
 // A kernel calls pdl_launch_dependents() at its start so that the NEXT kernel's CTAs may already become resident and run up to
 // their pdl_wait(), which returns once the whole preceding grid has finished and its writes are visible -- the dependent
@@ -136,16 +187,16 @@ __device__ __forceinline__ void cp_from_box(const float* b, double& cx, double& 
   cp_from_corners(b[0], b[1], b[3], b[4], b[6], b[7], b[9], b[10], cx, cy);
 }
 
-__device__ void ukf_initialize(TrackState& t, double zx, double zy) {   // UKF::UKF + Initialize, ukf.cpp:20-322
+// UKF::UKF + Initialize, ukf.cpp:20-322; d = P_merge_'s diagonal (:275-279), mp = the initial mode probabilities (:180-182)
+__device__ __forceinline__ void ukf_init_body(TrackState& t, double zx, double zy, const double* d, const double* mp) {
   const double x0[5] = {zx, zy, 0, 0, 0.1};
-  const double d[5] = {0.5, 0.5, 3, 10, 1};
   for (int m = 0; m < 4; ++m) {
     for (int i = 0; i < 5; ++i) t.x[m][i] = x0[i];
     for (int e = 0; e < 25; ++e) t.P[m][e] = 0;
     for (int i = 0; i < 5; ++i) t.P[m][i * 5 + i] = d[i];
   }
   for (int m = 0; m < 3; ++m) {
-    t.modeProb[m] = 0.33;
+    t.modeProb[m] = mp[m];
     t.zPred[m][0] = zx; t.zPred[m][1] = zy;
     t.S[m][0] = 1; t.S[m][1] = 0; t.S[m][2] = 0; t.S[m][3] = 1;
     for (int e = 0; e < 10; ++e) t.K[m][e] = 0;
@@ -155,6 +206,14 @@ __device__ void ukf_initialize(TrackState& t, double zx, double zy) {   // UKF::
   for (int p = 0; p < 8; ++p) for (int c = 0; c < 3; ++c) { t.BBox[p][c] = 0; t.bestBBox[p][c] = 0; }
   t.trackNum = 1; t.lifetime = 0; t.nVelo = 0; t.nBBox = 0; t.nBest = 0; t.isStatic = 0; t.isVisBB = 0;
 }
+__device__ void ukf_initialize(TrackState& t, double zx, double zy) {
+  const double d[5] = {0.5, 0.5, 3, 10, 1};
+  const double mp[3] = {0.33, 0.33, 0.33};
+  ukf_init_body(t, zx, zy, d, mp);
+}
+__device__ void ukf_initialize(TrackState& t, double zx, double zy, const TCPrm& p) { ukf_init_body(t, zx, zy, p.p0_diag, p.mode_prob0); }
+__device__ __forceinline__ void ukf_initialize(TrackState& t, double zx, double zy, DefTC) { ukf_initialize(t, zx, zy); }
+__device__ __forceinline__ void ukf_initialize(TrackState& t, double zx, double zy, TunTC s) { ukf_initialize(t, zx, zy, s.p); }
 
 // ------------------------------------------------------------------------------------------------ gate
 // The tracker of frame f+1 needs (a) the tracker of frame f (same stream) and (b) the detection stages of frame f+1 (another
@@ -214,13 +273,14 @@ struct TAShared {
 
 __device__ __forceinline__ double bcast(double v, int src) { return __shfl_sync(0xFFFFFFFFu, v, src); }
 
-// TA for one track table; the single-stream kernel and the sequence kernel (one table per blockIdx.y) share it
+// TA for one track table; the single-stream kernel and the sequence kernel (one table per blockIdx.y) share it.  P: DefTA / TunTA
+template <class TP>
 __device__ __forceinline__ void
 imm_predict_gate_body(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
                       double dt, unsigned* __restrict__ gate, unsigned* __restrict__ setter, int* __restrict__ first_setter,
                       uint8_t* __restrict__ skip, int words, const int* __restrict__ act_list,
                       int* __restrict__ meas_n, double2* __restrict__ meas_ctr,
-                      const unsigned* __restrict__ tc_seq, unsigned tc_want, unsigned spin_limit) {
+                      const unsigned* __restrict__ tc_seq, unsigned tc_want, unsigned spin_limit, const TP& P) {
   __shared__ TAShared sh;
   pdl_wait();                              // (gated launch: the gate kernel, hence this frame's detection, is complete)
   pdl_launch_dependents();                 // TB's CTAs may line up behind this grid
@@ -237,7 +297,6 @@ imm_predict_gate_body(TrackState* __restrict__ tracks, const int* __restrict__ t
   const int tid = threadIdx.x, lane = tid & 31, model = tid >> 5;
   const int n_act = trk[CNT_N_ACT];
   const int M = det[CNT_N_BOXES];
-  const double kStdA = (model == 2) ? 3.0 : 2.0;       // std_a_{cv,ctrv,rm}_ ukf.cpp:68-70 (= std_*_yawdd_ :71-73)
   const double lambda_aug = 3 - 7;
   const double w0 = lambda_aug / (lambda_aug + 7), wi = 0.5 / (7 + lambda_aug);
 
@@ -267,7 +326,7 @@ imm_predict_gate_body(TrackState* __restrict__ tracks, const int* __restrict__ t
     double Si[4] = {0, 0, 0, 0};
     if (model < 3) {
     // ---- MixingProbability (ukf.cpp:439-455) for this warp's model column j = model
-    const double pj0 = (model == 0) ? 0.9 : 0.05, pj1 = (model == 1) ? 0.9 : 0.05, pj2 = (model == 2) ? 0.9 : 0.05;
+    const double pj0 = P.trans(0, model), pj1 = P.trans(1, model), pj2 = P.trans(2, model);
     const double sumProb = mp0 * pj0 + mp1 * pj1 + mp2 * pj2;
     const double mu0 = mp0 * pj0 / sumProb, mu1 = mp1 * pj1 / sumProb, mu2 = mp2 * pj2 / sumProb;
     // ---- Interaction (:458-500)
@@ -323,9 +382,11 @@ imm_predict_gate_body(TrackState* __restrict__ tracks, const int* __restrict__ t
 #pragma unroll
         for (int c = 0; c < 7; ++c) L[r * 7 + c] = (r < 5 && c <= r) ? a[r * (r + 1) / 2 + c] : 0.0;
       // columns 5 and 6: pivot = sigma^2 - 0 > 0 -> sqrt, unless the factorisation stopped earlier (then raw sigma^2)
-      const double s2 = kStdA * kStdA;
-      L[5 * 7 + 5] = stop ? s2 : sqrt(s2);
-      L[6 * 7 + 6] = stop ? s2 : sqrt(s2);
+      // (std_a, std_yawdd of this warp's model: ukf.cpp:642-657)
+      const double sa = P.std_a(model), sy = P.std_yawdd(model);
+      const double s2a = sa * sa, s2y = sy * sy;
+      L[5 * 7 + 5] = stop ? s2a : sqrt(s2a);
+      L[6 * 7 + 6] = stop ? s2y : sqrt(s2y);
     }
     __syncwarp();
     if (lane < 15) {      // one sigma point per lane (:682-735)
@@ -406,7 +467,7 @@ imm_predict_gate_body(TrackState* __restrict__ tracks, const int* __restrict__ t
         const double dzr = sh.Xs[model][i][r] - (r ? zp1 : zp0), dzc = sh.Xs[model][i][c] - (c ? zp1 : zp0);
         acc = acc + (((i == 0) ? w0 : wi) * dzr) * dzc;
       }
-      const double R = (r == c) ? 0.15 * 0.15 : 0.0;
+      const double R = (r == c) ? P.r(r) : 0.0;
       sh.S[model][lane] = acc + R;
     } else if (lane < 14) {
       const int e = lane - 4, r = e >> 1, c = e & 1;
@@ -469,7 +530,7 @@ imm_predict_gate_body(TrackState* __restrict__ tracks, const int* __restrict__ t
           cp_from_box(boxes + (size_t)b * 24, cx, cy);
           const double d0 = cx - z0, d1 = cy - z1;
           const double nis = (d0 * Si[0] + d1 * Si[2]) * d0 + (d0 * Si[1] + d1 * Si[3]) * d1;
-          g = nis < gammaG;
+          g = nis < P.gamma_g();
         }
         const unsigned bits = __ballot_sync(0xFFFFFFFFu, g);
         if (lane == 0) { gate[(size_t)it * words + ch] = bits; setter[(size_t)it * words + ch] = bits; }
@@ -522,7 +583,7 @@ imm_predict_gate_body(TrackState* __restrict__ tracks, const int* __restrict__ t
           cp_from_box(boxes + (size_t)b * 24, cx, cy);
           const double d0 = cx - z0, d1 = cy - z1;
           nis = (d0 * Si[0] + d1 * Si[2]) * d0 + (d0 * Si[1] + d1 * Si[3]) * d1;
-          g = nis < gammaG;
+          g = nis < P.gamma_g();
         }
         const double v = g ? nis : DBL_MAX;
         double pm = v;     // inclusive prefix minimum over lanes
@@ -547,7 +608,17 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
                         uint8_t* __restrict__ skip, int words, const int* __restrict__ act_list,
                         int* __restrict__ meas_n, double2* __restrict__ meas_ctr,
                         const unsigned* __restrict__ tc_seq, unsigned tc_want, unsigned spin_limit) {
-  imm_predict_gate_body(tracks, trk, det, boxes, dt, gate, setter, first_setter, skip, words, act_list, meas_n, meas_ctr, tc_seq, tc_want, spin_limit);
+  imm_predict_gate_body(tracks, trk, det, boxes, dt, gate, setter, first_setter, skip, words, act_list, meas_n, meas_ctr, tc_seq, tc_want, spin_limit, DefTA{});
+}
+
+// a table with its own parameters (lmot_set_tracker_params)
+__global__ void __launch_bounds__(kTAThreads, 4)
+imm_predict_gate_tuned_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
+                              double dt, unsigned* __restrict__ gate, unsigned* __restrict__ setter, int* __restrict__ first_setter,
+                              uint8_t* __restrict__ skip, int words, const int* __restrict__ act_list,
+                              int* __restrict__ meas_n, double2* __restrict__ meas_ctr,
+                              const unsigned* __restrict__ tc_seq, unsigned tc_want, unsigned spin_limit, const __grid_constant__ TAPrm tp) {
+  imm_predict_gate_body(tracks, trk, det, boxes, dt, gate, setter, first_setter, skip, words, act_list, meas_n, meas_ctr, tc_seq, tc_want, spin_limit, TunTA{tp});
 }
 
 // Sequence ticks: one launch steps every sequence's table, sequence = blockIdx.y.  `run` = 0: the sequence is on its compat first
@@ -559,13 +630,24 @@ struct TASeq {
 };
 struct TASeqParams { TASeq s[kMaxBatch]; int words; unsigned spin_limit; };
 static_assert(sizeof(TASeqParams) <= 4096, "kernel parameter block");
+struct TASeqTunedParams { TASeqParams b; TAPrm tp[kMaxBatch]; };
+static_assert(sizeof(TASeqTunedParams) <= 4096, "kernel parameter block");
 
 __global__ void __launch_bounds__(kTAThreads, 4)
 imm_predict_gate_seq_kernel(const __grid_constant__ TASeqParams p) {
   const TASeq& q = p.s[blockIdx.y];
   if (!q.run) return;
   imm_predict_gate_body(q.tracks, q.trk, q.det, q.boxes, q.dt, q.gate, q.setter, q.first_setter, q.skip, p.words, q.act_list, q.meas_n,
-                        q.meas_ctr, q.tc_seq, q.tc_want, p.spin_limit);
+                        q.meas_ctr, q.tc_seq, q.tc_want, p.spin_limit, DefTA{});
+}
+
+// ... a tick where some table has its own parameters: every sequence of it, each with its own slice
+__global__ void __launch_bounds__(kTAThreads, 4)
+imm_predict_gate_seq_tuned_kernel(const __grid_constant__ TASeqTunedParams p) {
+  const TASeq& q = p.b.s[blockIdx.y];
+  if (!q.run) return;
+  imm_predict_gate_body(q.tracks, q.trk, q.det, q.boxes, q.dt, q.gate, q.setter, q.first_setter, q.skip, p.b.words, q.act_list, q.meas_n,
+                        q.meas_ctr, q.tc_seq, q.tc_want, p.b.spin_limit, TunTA{p.tp[blockIdx.y]});
 }
 
 // ------------------------------------------------------------------------------------------------ TB
@@ -612,7 +694,8 @@ __device__ double bbox_yaw(const float b[][3], double ukfYaw) {
 // order; what is independent runs on different lanes: the two centre points and the two areas (lane 0: BBox, lane 1:
 // bestBBox -- same code, different operand), the sixteen corner rotations (lane = corner).  getBBoxYaw of an UNCHANGED box
 // (deltaArea >= 0) is the same pure function of the same operands as the first evaluation and is not repeated.
-__device__ void update_bb_warp(TrackState& t, int lane) {
+// thres = bbYawChangeThres_ (:617-621)
+__device__ __forceinline__ void update_bb_warp_body(TrackState& t, int lane, double thres) {
   if (!t.isVisBB) return;
   if (t.nBest == 0) {
     const float v = (lane < 24) ? (&t.BBox[0][0])[lane] : 0.f;
@@ -647,8 +730,8 @@ __device__ void update_bb_warp(TrackState& t, int lane) {
   __syncwarp();
   const double currentYaw = (deltaArea < 0) ? bbox_yaw(t.BBox, ukfYaw) : yaw;
   const double DiffYaw = yaw - currentYaw;
-  if (fabs(DiffYaw) > bbYawChangeThres) {
-  } else if (fabs(DiffYaw) < bbYawChangeThres) {
+  if (fabs(DiffYaw) > thres) {
+  } else if (fabs(DiffYaw) < thres) {
     const double cd = cos(DiffYaw), sd = sin(DiffYaw);
     // updateBoxYaw :512-532 on both boxes (n = nBBox for both, like the reference): lane < 8 -> BBox, 8 <= lane < 16 -> bestBBox
     const int i = lane & 7;
@@ -662,8 +745,12 @@ __device__ void update_bb_warp(TrackState& t, int lane) {
   }
   __syncwarp();
 }
+__device__ void update_bb_warp(TrackState& t, int lane) { update_bb_warp_body(t, lane, bbYawChangeThres); }
+__device__ void update_bb_warp(TrackState& t, int lane, double thres) { update_bb_warp_body(t, lane, thres); }
+__device__ __forceinline__ void update_bb_warp(TrackState& t, int lane, DefTB) { update_bb_warp(t, lane); }
+__device__ __forceinline__ void update_bb_warp(TrackState& t, int lane, TunTB s) { update_bb_warp(t, lane, s.p.bb_yaw_change_thres); }
 
-constexpr int kTBThreads = 128;     // warps 0-2: PDA update of one motion model each; warp 3: box association + updateBB
+constexpr int kTBThreads = 128;    // warps 0-2: PDA update of one motion model each; warp 3: box association + updateBB
 
 struct TBShared {
   TrackState trk;                   // the track, staged (1.6 KB)
@@ -677,12 +764,13 @@ struct TBShared {
 // One CTA per active track.  What the reference does one after the other for a track, and what does not depend on each other,
 // runs on different warps: the PDA update of the three motion models (each its own S^-1, Gaussian kernels, beta weights,
 // K nu, covariance update -- identical code, different model) on warps 0..2, measurement bookkeeping / box association /
-// updateBB on warp 3; then warp 0 alone: association likelihoods, mode probabilities, merged estimate.
+// updateBB on warp 3; then warp 0 alone: association likelihoods, mode probabilities, merged estimate.  P: DefTB / TunTB
+template <class TP>
 __device__ __forceinline__ void
 imm_update_body(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
                 const unsigned* __restrict__ gate, const int* __restrict__ first_setter, const uint8_t* __restrict__ skip,
                 int words, const int* __restrict__ act_list, ActSummary* __restrict__ summary,
-                const int* __restrict__ meas_n, const double2* __restrict__ meas_ctr) {
+                const int* __restrict__ meas_n, const double2* __restrict__ meas_ctr, const TP& P) {
   extern __shared__ unsigned short s_list[];              // indices of the gated boxes, in box order
   __shared__ TBShared sh;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -776,7 +864,7 @@ imm_update_body(TrackState* __restrict__ tracks, const int* __restrict__ trk, co
               t.initMeas[0] = t.x[0][0]; t.initMeas[1] = t.x[0][1];
               const double dX = bx - t.x[0][0], dY = by - t.x[0][1];
               const double targetYaw = wrap_pi(atan2(dY, dX));
-              for (int m = 0; m < 4; ++m) { t.x[m][0] = bx; t.x[m][1] = by; t.x[m][2] = 2; t.x[m][3] = targetYaw; }
+              for (int m = 0; m < 4; ++m) { t.x[m][0] = bx; t.x[m][1] = by; t.x[m][2] = P.second_init_v(); t.x[m][3] = targetYaw; }
               sh.tn_out = trackNum0 + 1;
             }
           }
@@ -798,7 +886,7 @@ imm_update_body(TrackState* __restrict__ tracks, const int* __restrict__ trk, co
           // ---- associateBB (:416-463) + getNearestEuclidBBox (:396-413): int minDist => first box with the smallest
           // floor(distance)
           int isVis = 0;
-          if (nmeas > 0 && trackNum0 == 5 && lifetime > lifeTimeThres) {
+          if (nmeas > 0 && trackNum0 == 5 && lifetime > P.lifetime_thres()) {
             const double px = t.x[0][0], py = t.x[0][1];
             long long key = LLONG_MAX;      // (floor(dist) << 32) | position
             for (int k = lane; k < nmeas; k += 32) {
@@ -811,7 +899,7 @@ imm_update_body(TrackState* __restrict__ tracks, const int* __restrict__ trk, co
             for (int o = 16; o > 0; o >>= 1) { const long long ok = __shfl_xor_sync(0xFFFFFFFFu, key, o); key = key < ok ? key : ok; }
             int minDist = 999, minInd = 0;
             if (key != LLONG_MAX) { minDist = (int)(key >> 32); minInd = (int)(key & 0xFFFFFFFFll); }
-            if (minDist < distanceThres) {
+            if (minDist < P.distance_thres()) {
               const float* b = boxes + (size_t)s_list[minInd] * 24;
               if (lane < 8) {
                 const int c = lane & 3;
@@ -826,10 +914,11 @@ imm_update_body(TrackState* __restrict__ tracks, const int* __restrict__ trk, co
             if (isVis) { t.isVisBB = 1; t.nBBox = 8; }
           }
           __syncwarp();
-          update_bb_warp(t, lane);                          // :877 (reads x_merge_ before warp 0 replaces it below)
+          update_bb_warp(t, lane, P);                       // :877 (reads x_merge_ before warp 0 replaces it below)
         } else if (pda) {
           // ---- filterPDA (:259-394) for model `warp`; scalars replicated on every lane
           const int m = warp;
+          const double pD = P.p_d(), pG = P.p_g(), gammaG = P.gamma_g();
           const double bb = 2 * numMeas * (1 - pD * pG) / (gammaG * pD);
           // centre point of every gated box once (lane k <-> measurement k; beyond 32 measurements recomputed on the fly)
           double mcx = 0, mcy = 0;
@@ -910,6 +999,7 @@ imm_update_body(TrackState* __restrict__ tracks, const int* __restrict__ trk, co
     __syncthreads();
     if (!skipped && warp == 0) {
       if (pda) {
+        const double pD = P.p_d(), pG = P.p_g(), gammaG = P.gamma_g();
         const double Vk = kPi * sqrt(gammaG * det2(t.S[mm]));     // S is untouched by the update, same max model
         double lam[3];
         {
@@ -1002,7 +1092,16 @@ imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, 
                   const unsigned* __restrict__ gate, const int* __restrict__ first_setter, const uint8_t* __restrict__ skip,
                   int words, const int* __restrict__ act_list, ActSummary* __restrict__ summary,
                   const int* __restrict__ meas_n, const double2* __restrict__ meas_ctr) {
-  imm_update_body(tracks, trk, det, boxes, gate, first_setter, skip, words, act_list, summary, meas_n, meas_ctr);
+  imm_update_body(tracks, trk, det, boxes, gate, first_setter, skip, words, act_list, summary, meas_n, meas_ctr, DefTB{});
+}
+
+// a table with its own parameters (lmot_set_tracker_params)
+__global__ void __launch_bounds__(kTBThreads)
+imm_update_tuned_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
+                        const unsigned* __restrict__ gate, const int* __restrict__ first_setter, const uint8_t* __restrict__ skip,
+                        int words, const int* __restrict__ act_list, ActSummary* __restrict__ summary,
+                        const int* __restrict__ meas_n, const double2* __restrict__ meas_ctr, const __grid_constant__ TBPrm tp) {
+  imm_update_body(tracks, trk, det, boxes, gate, first_setter, skip, words, act_list, summary, meas_n, meas_ctr, TunTB{tp});
 }
 
 // sequence ticks: sequence = blockIdx.y, `run` as for TA
@@ -1012,12 +1111,23 @@ struct TBSeq {
 };
 struct TBSeqParams { TBSeq s[kMaxBatch]; int words; };
 static_assert(sizeof(TBSeqParams) <= 4096, "kernel parameter block");
+struct TBSeqTunedParams { TBSeqParams b; TBPrm tp[kMaxBatch]; };
+static_assert(sizeof(TBSeqTunedParams) <= 4096, "kernel parameter block");
 
 __global__ void __launch_bounds__(kTBThreads)
 imm_update_seq_kernel(const __grid_constant__ TBSeqParams p) {
   const TBSeq& q = p.s[blockIdx.y];
   if (!q.run) return;
-  imm_update_body(q.tracks, q.trk, q.det, q.boxes, q.gate, q.first_setter, q.skip, p.words, q.act_list, q.summary, q.meas_n, q.meas_ctr);
+  imm_update_body(q.tracks, q.trk, q.det, q.boxes, q.gate, q.first_setter, q.skip, p.words, q.act_list, q.summary, q.meas_n, q.meas_ctr, DefTB{});
+}
+
+// ... a tick where some table has its own parameters: every sequence of it, each with its own slice
+__global__ void __launch_bounds__(kTBThreads)
+imm_update_seq_tuned_kernel(const __grid_constant__ TBSeqTunedParams p) {
+  const TBSeq& q = p.b.s[blockIdx.y];
+  if (!q.run) return;
+  imm_update_body(q.tracks, q.trk, q.det, q.boxes, q.gate, q.first_setter, q.skip, p.b.words, q.act_list, q.summary, q.meas_n, q.meas_ctr,
+                  TunTB{p.tp[blockIdx.y]});
 }
 
 // ------------------------------------------------------------------------------------------------ TC: over-segmentation test
@@ -1084,7 +1194,8 @@ __device__ __forceinline__ void block_offsets(int a, int b, int* s_w, int& excl,
 }
 
 // per-track outputs of one track (:995-1041) + static flag (:1045-1081) into the frame's result block; returns isVisBB
-__device__ __forceinline__ int emit_track(TrackState& t, int i, double ego_yaw, const OutPtrs& o, double4* __restrict__ pos) {
+template <class TP>
+__device__ __forceinline__ int emit_track(TrackState& t, int i, double ego_yaw, const OutPtrs& o, double4* __restrict__ pos, const TP& P) {
   const double tx = t.x[0][0], ty = t.x[0][1];
   const double mx = t.initMeas[0], my = t.initMeas[1];
   t.distFromInit = sqrt((tx - mx) * (tx - mx) + (ty - my) * (ty - my));
@@ -1097,8 +1208,8 @@ __device__ __forceinline__ int emit_track(TrackState& t, int i, double ego_yaw, 
   o.is_vis[i] = (uint8_t)vis;
   int st = 0;
   if (t.isStatic) st = 1;
-  else if (t.trackNum == 5 && t.lifetime > 8) {
-    if ((t.distFromInit < 3.0) && (t.modeProb[2] > t.modeProb[0] || t.modeProb[2] > t.modeProb[1])) { st = 1; t.isStatic = 1; }
+  else if (t.trackNum == 5 && t.lifetime > P.static_lifetime()) {
+    if ((t.distFromInit < P.static_dist()) &&(t.modeProb[2] > t.modeProb[0] || t.modeProb[2] > t.modeProb[1])) { st = 1; t.isStatic = 1; }
   }
   o.is_static[i] = (uint8_t)st;
   o.track_manage[i] = t.trackNum;
@@ -1134,9 +1245,10 @@ __device__ __forceinline__ void cta_store(T* dst, const T (&v)[U], int n) {
 
 // per-track outputs (:995-1041) + static flag (:1045-1081) from values instead of the record (the fast path of TC holds an
 // active track's fields in registers); same statements as emit_track.  Returns the new isStatic.
+template <class TP>
 __device__ __forceinline__ int emit_values(int i, double tx, double ty, double yaw, double v, double mx, double my, double mp0, double mp1,
                                            double mp2, int trackNum, int lifetime, int isStatic, int vis, double ego_yaw, const OutPtrs& o,
-                                           double4* __restrict__ pos, double& distFromInit) {
+                                           double4* __restrict__ pos, double& distFromInit, const TP& P) {
   distFromInit = sqrt((tx - mx) * (tx - mx) + (ty - my) * (ty - my));
   double tyaw = yaw;
   tyaw += ego_yaw;
@@ -1146,8 +1258,8 @@ __device__ __forceinline__ int emit_values(int i, double tx, double ty, double y
   o.is_vis[i] = (uint8_t)vis;
   int st = 0;
   if (isStatic) st = 1;
-  else if (trackNum == 5 && lifetime > 8) {
-    if ((distFromInit < 3.0) && (mp2 > mp0 || mp2 > mp1)) st = 1;
+  else if (trackNum == 5 && lifetime > P.static_lifetime()) {
+    if ((distFromInit < P.static_dist()) &&(mp2 > mp0 || mp2 > mp1)) st = 1;
   }
   o.is_static[i] = (uint8_t)st;
   o.track_manage[i] = trackNum;
@@ -1185,11 +1297,11 @@ __device__ __noinline__ void tc_candidate(TCFastShared<NT>& S, int v, int jt) {
   else if (overseg_cond(S.bx[v], reinterpret_cast<const float*>(&S.ab[v]), S.px[jt], S.py[jt])) atomicMax(&S.imax[jt], S.vid[v]);
 }
 
-template <int NT>
+template <int NT, class TP>
 __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det,
                                         const float* __restrict__ boxes, const float* __restrict__ boxes_pub, int* __restrict__ first_setter, double ego_yaw, int max_tracks,
                                         const OutPtrs& o, const OutPtrs& prev, int* __restrict__ act_list, double4* __restrict__ pos,
-                                        const ActSummary* __restrict__ summary, int T0, int n_act0, int M) {
+                                        const ActSummary* __restrict__ summary, int T0, int n_act0, int M, const TP& P) {
   const int tid = threadIdx.x, lane = tid & 31;
   const bool have = tid < n_act0;
   // ---- one round trip: the summaries, the previous result block, the spawn inputs
@@ -1362,7 +1474,7 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
   int act = 0;
   if (have) {
     double dfi;
-    const int st = emit_values(r.k, r.x, r.y, r.yaw, r.v, r.initx, r.inity, r.mp0, r.mp1, r.mp2, trackNum, r.lifetime, r.isStatic, vis, ego_yaw, o, pos, dfi);
+    const int st = emit_values(r.k, r.x, r.y, r.yaw, r.v, r.initx, r.inity, r.mp0, r.mp1, r.mp2, trackNum, r.lifetime, r.isStatic, vis, ego_yaw, o, pos, dfi, P);
     tracks[r.k].distFromInit = dfi;
     if (st && !r.isStatic) tracks[r.k].isStatic = 1;
     act = (trackNum != 0 || vis) ? 1 : 0;
@@ -1388,9 +1500,9 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
       double cx, cy;
       if (b0 == 0) cp_from_corners(bc[0], bc[1], bc[2], bc[3], bc[4], bc[5], bc[6], bc[7], cx, cy);
       else cp_from_box(boxes + (size_t)b * 24, cx, cy);
-      ukf_initialize(tracks[p], cx, cy);
+      ukf_initialize(tracks[p], cx, cy, P);
       double dfi;
-      emit_values(p, cx, cy, 0.0, 0.0, 0.0, 0.0, 0.33, 0.33, 0.33, 1, 0, 0, 0, ego_yaw, o, pos, dfi);
+      emit_values(p, cx, cy, 0.0, 0.0, 0.0, 0.0, P.mode_prob0(0), P.mode_prob0(1), P.mode_prob0(2), 1, 0, 0, 0, ego_yaw, o, pos, dfi, P);
       tracks[p].distFromInit = dfi;
       act_list[n_keep + (p - T0)] = p;
     }
@@ -1420,13 +1532,14 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
 //     of every track is its state's yaw plus THIS frame's ego yaw: `pos`, a packed (x, y, yaw) per track, refreshed for the
 //     active tracks only.
 // `full` (first step after the table was written from the host): everything is rebuilt from the records.
-template <int NT>
+// P: DefTC / TunTC
+template <int NT, class TP>
 __device__ __forceinline__ void
 spawn_output_body(TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det, const float* __restrict__ boxes,
                   const float* __restrict__ boxes_pub, int* __restrict__ first_setter, int* __restrict__ imax_arr, int* __restrict__ vis_list,
                   uint8_t* __restrict__ has5_arr, int first_frame, int compat_first, double ego_yaw, int max_tracks, const OutPtrs& o,
                   const OutPtrs& prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
-                  int* __restrict__ det_sem, unsigned* __restrict__ tc_seq) {
+                  int* __restrict__ det_sem, unsigned* __restrict__ tc_seq, const TP& P) {
   pdl_launch_dependents();                 // the next frame's gate kernel may become resident
   pdl_wait();                              // TB has finished
   // every exit: this step's results are complete -> count it (release); publish_kernel, on its own stream, polls the count
@@ -1437,7 +1550,7 @@ spawn_output_body(TrackState* __restrict__ tracks, int* __restrict__ trk, int* _
     extern __shared__ __align__(16) unsigned char tc_dyn[];          // sizeof(TCFastShared<NT>), tracker_launch
     TCFastShared<NT>& s_fast = *reinterpret_cast<TCFastShared<NT>*>(tc_dyn);
     const int M = det[CNT_N_BOXES];
-    tc_fast<NT>(s_fast, tracks, trk, det, boxes, boxes_pub, first_setter, ego_yaw, max_tracks, o, prev, act_list, pos, summary, trk[CNT_N_TRACKS], trk[CNT_N_ACT], M);
+    tc_fast<NT>(s_fast, tracks, trk, det, boxes, boxes_pub, first_setter, ego_yaw, max_tracks, o, prev, act_list, pos, summary, trk[CNT_N_TRACKS], trk[CNT_N_ACT], M, P);
     return;
   }
   __shared__ int s_w[33];
@@ -1460,7 +1573,7 @@ spawn_output_body(TrackState* __restrict__ tracks, int* __restrict__ trk, int* _
     if (tid == 0) {
       int T = 0;
       if (M >= 2) {
-        ukf_initialize(tracks[0], -1.5125, -8.975);
+        ukf_initialize(tracks[0], -1.5125, -8.975, P);
         o.targets[0] = (float)-1.5125; o.targets[1] = (float)-8.975; o.targets[2] = (float)(-1.73 / 2);
         o.vandyaw[0] = 0; o.vandyaw[1] = 0; o.is_static[0] = 0; o.is_vis[0] = 0; o.track_manage[0] = 1;
         pos[0] = make_double4(-1.5125, -8.975, 0.0, 0.0);
@@ -1614,7 +1727,7 @@ spawn_output_body(TrackState* __restrict__ tracks, int* __restrict__ trk, int* _
     if (un && p < max_tracks) {
       double cx, cy;
       cp_from_box(boxes + (size_t)b * 24, cx, cy);
-      ukf_initialize(tracks[p], cx, cy);
+      ukf_initialize(tracks[p], cx, cy, P);
     }
     if (b < M) first_setter[b] = INT_MAX;        // ready for the next frame
     __syncthreads();
@@ -1638,7 +1751,7 @@ spawn_output_body(TrackState* __restrict__ tracks, int* __restrict__ trk, int* _
     if (q < n_emit) {
       i = (q < n_scan) ? (full ? q : act_list[q]) : T0 + (q - n_scan);
       TrackState& t = tracks[i];
-      vis = emit_track(t, i, ego_yaw, o, pos);
+      vis = emit_track(t, i, ego_yaw, o, pos, P);
       act = (t.trackNum != 0 || vis) ? 1 : 0;
     }
     int ex, tot;
@@ -1673,7 +1786,19 @@ spawn_output_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int*
                     OutPtrs prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
                     int* __restrict__ det_sem, unsigned* __restrict__ tc_seq) {
   spawn_output_body<NT>(tracks, trk, det, boxes, boxes_pub, first_setter, imax_arr, vis_list, has5_arr, first_frame, compat_first, ego_yaw,
-                        max_tracks, o, prev, full, act_list, pos, summary, det_sem, tc_seq);
+                        max_tracks, o, prev, full, act_list, pos, summary, det_sem, tc_seq, DefTC{});
+}
+
+// a table with its own parameters (lmot_set_tracker_params)
+template <int NT>
+__global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
+spawn_output_tuned_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det, const float* __restrict__ boxes,
+                          const float* __restrict__ boxes_pub, int* __restrict__ first_setter, int* __restrict__ imax_arr, int* __restrict__ vis_list,
+                          uint8_t* __restrict__ has5_arr, int first_frame, int compat_first, double ego_yaw, int max_tracks, OutPtrs o,
+                          OutPtrs prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
+                          int* __restrict__ det_sem, unsigned* __restrict__ tc_seq, const __grid_constant__ TCPrm tp) {
+  spawn_output_body<NT>(tracks, trk, det, boxes, boxes_pub, first_setter, imax_arr, vis_list, has5_arr, first_frame, compat_first, ego_yaw,
+                        max_tracks, o, prev, full, act_list, pos, summary, det_sem, tc_seq, TunTC{tp});
 }
 
 // sequence ticks: one CTA per sequence (blockIdx.x); each picks the fast or the general path from its own sequence's counts
@@ -1685,13 +1810,25 @@ struct TCSeq {
 };
 struct TCSeqParams { TCSeq s[kMaxBatch]; int compat_first, max_tracks; };
 static_assert(sizeof(TCSeqParams) <= 4096, "kernel parameter block");
+struct TCSeqTunedParams { TCSeqParams b; TCPrm tp[kMaxBatch]; };
+static_assert(sizeof(TCSeqTunedParams) <= 4096, "kernel parameter block");
 
 template <int NT>
 __global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
 spawn_output_seq_kernel(const __grid_constant__ TCSeqParams p) {
   const TCSeq& q = p.s[blockIdx.x];
   spawn_output_body<NT>(q.tracks, q.trk, q.det, q.boxes, q.boxes_pub, q.first_setter, q.imax_arr, q.vis_list, q.has5_arr, q.first_frame,
-                        p.compat_first, q.ego_yaw, p.max_tracks, q.o, q.prev, q.full, q.act_list, q.pos, q.summary, q.det_sem, q.tc_seq);
+                        p.compat_first, q.ego_yaw, p.max_tracks, q.o, q.prev, q.full, q.act_list, q.pos, q.summary, q.det_sem, q.tc_seq, DefTC{});
+}
+
+// ... a tick where some table has its own parameters: every sequence of it, each with its own slice
+template <int NT>
+__global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
+spawn_output_seq_tuned_kernel(const __grid_constant__ TCSeqTunedParams p) {
+  const TCSeq& q = p.b.s[blockIdx.x];
+  spawn_output_body<NT>(q.tracks, q.trk, q.det, q.boxes, q.boxes_pub, q.first_setter, q.imax_arr, q.vis_list, q.has5_arr, q.first_frame,
+                        p.b.compat_first, q.ego_yaw, p.b.max_tracks, q.o, q.prev, q.full, q.act_list, q.pos, q.summary, q.det_sem, q.tc_seq,
+                        TunTC{p.tp[blockIdx.x]});
 }
 
 // device copy of a frame's results -> pinned, device-mapped host block.  16 bytes per thread, consecutive threads ->
@@ -1802,6 +1939,25 @@ __global__ void fill_int_kernel(int* p, int n, int v) {
   if (i < n) p[i] = v;
 }
 
+// each stage's slice of a table's parameters
+TAPrm ta_prm(const lmot_tracker_params& p) {
+  TAPrm a;
+  a.gamma_g = p.gamma_g; a.std_las_x = p.std_las_x; a.std_las_y = p.std_las_y;
+  for (int m = 0; m < 3; ++m) { a.std_a[m] = p.std_a[m]; a.std_yawdd[m] = p.std_yawdd[m]; }
+  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) a.trans[i][j] = p.trans[i][j];
+  return a;
+}
+TBPrm tb_prm(const lmot_tracker_params& p) {
+  return TBPrm{p.gamma_g, p.p_g, p.p_d, p.distance_thres, p.bb_yaw_change_thres, p.second_init_v, p.lifetime_thres};
+}
+TCPrm tc_prm(const lmot_tracker_params& p) {
+  TCPrm a;
+  for (int i = 0; i < 5; ++i) a.p0_diag[i] = p.p0_diag[i];
+  for (int m = 0; m < 3; ++m) a.mode_prob0[m] = p.mode_prob0[m];
+  a.static_dist = p.static_dist; a.static_lifetime = p.static_lifetime;
+  return a;
+}
+
 }  // namespace
 
 int tracker_alloc(Ctx* c, Tracker& t) {
@@ -1841,6 +1997,12 @@ int tracker_alloc(Ctx* c, Tracker& t) {
   LMOT_CUDA(c, cudaFuncSetAttribute(imm_update_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
   LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
   LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
+  LMOT_CUDA(c, cudaFuncSetAttribute(imm_update_tuned_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
+  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_tuned_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
+  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_tuned_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
+  LMOT_CUDA(c, cudaFuncSetAttribute(imm_update_seq_tuned_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
+  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_tuned_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
+  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_tuned_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
   t.last_n_act = 0;
   return LMOT_OK;
 }
@@ -1936,6 +2098,7 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
   int* det_sem = gate ? sl->d_det_sem : nullptr;
   if (gated) *gated = use_gate;
   const int full = c->own.act_valid ? 0 : 1;   // the table was written from the host since the last frame: rebuild the side arrays
+  const bool tuned = c->own.tuned;             // lmot_set_tracker_params: the kernels that read the table's values (copied into the launches)
   if (full) {
     LMOT_CUDA(c, cudaMemsetAsync(c->own.d_trk_counters + CNT_N_ACT, 0, sizeof(int), st));
     build_active_kernel<<<(c->prm.max_tracks + 255) / 256, 256, 0, st>>>(c->own.d_tracks, c->own.d_trk_counters, c->own.d_act_list);
@@ -1958,9 +2121,15 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
       }
       cudaLaunchConfig_t ac = {};
       ac.gridDim = dim3(c->trk_ctas); ac.blockDim = dim3(kTAThreads); ac.dynamicSmemBytes = 0; ac.stream = st; ac.attrs = &pa; ac.numAttrs = 1;
-      LMOT_CUDA(c, cudaLaunchKernelEx(&ac, imm_predict_gate_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes, dt,
-                                      c->own.d_gate, c->own.d_setter, c->own.d_first_setter, c->own.d_skip, c->gate_words, (const int*)c->own.d_act_list,
-                                      c->own.d_meas_n, reinterpret_cast<double2*>(c->own.d_meas_ctr), (const unsigned*)c->own.d_tc_seq, c->own.tc_launched, c->spin_limit));
+      if (tuned)
+        LMOT_CUDA(c, cudaLaunchKernelEx(&ac, imm_predict_gate_tuned_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes, dt,
+                                        c->own.d_gate, c->own.d_setter, c->own.d_first_setter, c->own.d_skip, c->gate_words, (const int*)c->own.d_act_list,
+                                        c->own.d_meas_n, reinterpret_cast<double2*>(c->own.d_meas_ctr), (const unsigned*)c->own.d_tc_seq, c->own.tc_launched, c->spin_limit,
+                                        ta_prm(c->own.prm)));
+      else
+        LMOT_CUDA(c, cudaLaunchKernelEx(&ac, imm_predict_gate_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes, dt,
+                                        c->own.d_gate, c->own.d_setter, c->own.d_first_setter, c->own.d_skip, c->gate_words, (const int*)c->own.d_act_list,
+                                        c->own.d_meas_n, reinterpret_cast<double2*>(c->own.d_meas_ctr), (const unsigned*)c->own.d_tc_seq, c->own.tc_launched, c->spin_limit));
     }
     kernel_mark(c, sl, st);
     // TB and TC: programmatic dependent launches (their CTAs wait on the device for the preceding grid, see pdl_wait); timing
@@ -1971,10 +2140,16 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(c->trk_ctas); cfg.blockDim = dim3(kTBThreads); cfg.dynamicSmemBytes = sh; cfg.stream = st;
     cfg.attrs = &pdl; cfg.numAttrs = 1;
-    LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes,
-                                    (const unsigned*)c->own.d_gate, (const int*)c->own.d_first_setter, (const uint8_t*)c->own.d_skip, c->gate_words,
-                                    (const int*)c->own.d_act_list, reinterpret_cast<ActSummary*>(c->own.d_summary),
-                                    (const int*)c->own.d_meas_n, reinterpret_cast<const double2*>(c->own.d_meas_ctr)));
+    if (tuned)
+      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_tuned_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes,
+                                      (const unsigned*)c->own.d_gate, (const int*)c->own.d_first_setter, (const uint8_t*)c->own.d_skip, c->gate_words,
+                                      (const int*)c->own.d_act_list, reinterpret_cast<ActSummary*>(c->own.d_summary),
+                                      (const int*)c->own.d_meas_n, reinterpret_cast<const double2*>(c->own.d_meas_ctr), tb_prm(c->own.prm)));
+    else
+      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes,
+                                      (const unsigned*)c->own.d_gate, (const int*)c->own.d_first_setter, (const uint8_t*)c->own.d_skip, c->gate_words,
+                                      (const int*)c->own.d_act_list, reinterpret_cast<ActSummary*>(c->own.d_summary),
+                                      (const int*)c->own.d_meas_n, reinterpret_cast<const double2*>(c->own.d_meas_ctr)));
     kernel_mark(c, sl, st);
   }
   {
@@ -1991,9 +2166,14 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
     cfg.gridDim = dim3(1); cfg.blockDim = dim3(wide ? kTCWide : kTCThreads); cfg.stream = st;
     cfg.dynamicSmemBytes = wide ? sizeof(TCFastShared<kTCWide>) : sizeof(TCFastShared<kTCThreads>);
     cfg.attrs = &pdl; cfg.numAttrs = 1;
-    LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_kernel<kTCWide> : spawn_output_kernel<kTCThreads>, c->own.d_tracks, c->own.d_trk_counters, det, d_boxes, d_boxes_pub, c->own.d_first_setter, c->own.d_new_num,
-                                    c->own.d_vis_list, c->own.d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->own.d_act_list,
-                                    c->own.d_pos, reinterpret_cast<const ActSummary*>(c->own.d_summary), det_sem, c->own.d_tc_seq));
+    if (tuned)
+      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_tuned_kernel<kTCWide> : spawn_output_tuned_kernel<kTCThreads>, c->own.d_tracks, c->own.d_trk_counters, det, d_boxes, d_boxes_pub, c->own.d_first_setter, c->own.d_new_num,
+                                      c->own.d_vis_list, c->own.d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->own.d_act_list,
+                                      c->own.d_pos, reinterpret_cast<const ActSummary*>(c->own.d_summary), det_sem, c->own.d_tc_seq, tc_prm(c->own.prm)));
+    else
+      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_kernel<kTCWide> : spawn_output_kernel<kTCThreads>, c->own.d_tracks, c->own.d_trk_counters, det, d_boxes, d_boxes_pub, c->own.d_first_setter, c->own.d_new_num,
+                                      c->own.d_vis_list, c->own.d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->own.d_act_list,
+                                      c->own.d_pos, reinterpret_cast<const ActSummary*>(c->own.d_summary), det_sem, c->own.d_tc_seq));
     ++c->own.tc_launched;
   }
   kernel_mark(c, sl, st);
@@ -2046,10 +2226,14 @@ int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const dou
   const int compat = c->prm.oracle_compat_first_frame ? 1 : 0;
   const bool gf = c->prm.global_frame != 0;
   GateSeq g{};
-  TASeqParams ta{};
-  TBSeqParams tb{};
-  TCSeqParams tcp{};
+  TASeqTunedParams tat{};      // (the parameter blocks of the kernels that read the tables' values: the blocks below + a slice per sequence)
+  TBSeqTunedParams tbt{};
+  TCSeqTunedParams tct{};
+  TASeqParams& ta = tat.b;
+  TBSeqParams& tb = tbt.b;
+  TCSeqParams& tcp = tct.b;
   PubSeqParams pub{};
+  bool tuned = false;          // some table of the set has its own values: every sequence of the tick runs those kernels
   g.n = S;
   ta.words = c->gate_words; ta.spin_limit = c->spin_limit;
   tb.words = c->gate_words;
@@ -2085,6 +2269,8 @@ int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const dou
     OutPtrs po{pr->d_targets, pr->d_vandyaw, pr->d_manage, pr->d_static, pr->d_vis, pr->d_visbb, pr->d_hdr, pr->d_boxes};
     tcp.s[k] = TCSeq{t.d_tracks, t.d_trk_counters, s.d_counters, boxes, s.d_boxes, t.d_first_setter, t.d_new_num, t.d_vis_list, t.d_skip,
                      t.d_act_list, t.d_pos, sum, s.d_det_sem, t.d_tc_seq, o, po, t.th.egoPoint[2], first, full};
+    tat.tp[k] = ta_prm(t.prm); tbt.tp[k] = tb_prm(t.prm); tct.tp[k] = tc_prm(t.prm);
+    tuned |= t.tuned;
     ++t.tc_launched;
     OutPtrs h{r->h_targets, r->h_vandyaw, r->h_manage, r->h_static, r->h_vis, r->h_visbb, r->h_hdr, r->h_boxes};
     pub.s[k] = PubSeq{o, h, t.d_tc_seq, t.tc_launched, r->back};
@@ -2103,9 +2289,11 @@ int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const dou
   // the single-stream chain's CTA count, shared by the sequences (grid-stride over each sequence's active tracks)
   const int gx = (c->trk_ctas + S - 1) / S;
   cfg.gridDim = dim3(gx, S); cfg.blockDim = dim3(kTAThreads); cfg.dynamicSmemBytes = 0;
-  LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_predict_gate_seq_kernel, ta));
+  if (tuned) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_predict_gate_seq_tuned_kernel, tat));
+  else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_predict_gate_seq_kernel, ta));
   cfg.gridDim = dim3(gx, S); cfg.blockDim = dim3(kTBThreads); cfg.dynamicSmemBytes = (size_t)c->gate_words * 32 * sizeof(unsigned short);
-  LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_seq_kernel, tb));
+  if (tuned) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_seq_tuned_kernel, tbt));
+  else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_seq_kernel, tb));
   // spawn_output_kernel's variant for the whole launch from the largest active count of the set (hysteresis as tracker_launch);
   // either variant is correct for any count
   if (n_act_max > 208) c->seq_wide = true;
@@ -2113,7 +2301,8 @@ int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const dou
   const bool wide = c->tc_force >= 0 ? c->tc_force != 0 : c->seq_wide;
   cfg.gridDim = dim3(S); cfg.blockDim = dim3(wide ? kTCWide : kTCThreads);
   cfg.dynamicSmemBytes = wide ? sizeof(TCFastShared<kTCWide>) : sizeof(TCFastShared<kTCThreads>);
-  LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_kernel<kTCWide> : spawn_output_seq_kernel<kTCThreads>, tcp));
+  if (tuned) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_tuned_kernel<kTCWide> : spawn_output_seq_tuned_kernel<kTCThreads>, tct));
+  else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_kernel<kTCWide> : spawn_output_seq_kernel<kTCThreads>, tcp));
   publish_seq_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(pub);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;

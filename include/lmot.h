@@ -395,6 +395,50 @@ int lmot_seq_tracker_load(lmot_ctx* ctx, int k, const double* dumps, int n, int 
                           double ego_yaw, double ego_pre_yaw, double ego_point_yaw);
 int lmot_seq_tracker_set_ego(lmot_ctx* ctx, int k, const double ego8[8]);
 
+/* ---- tracker parameters: the IMM-UKF-PDA noise, gating and track-management constants of one track table ------------------------
+ * The defaults (lmot_default_tracker_params) are the reference's values; citations are file:line under object_tracking/tracking/.
+ * A separate struct rather than fields of lmot_params, so that callers compiled against an older lmot_params keep working. */
+typedef struct lmot_tracker_params {
+  double gamma_g;              /* 9.22  chi-square gate, gammaG_ imm_ukf_jpda.cpp:26 (gate :230, PDA :263, likelihoods :374-388) */
+  double p_g;                  /* 0.99  gate probability, pG_ :30 */
+  double p_d;                  /* 0.9   detection probability, pD_ :34 */
+  double distance_thres;       /* 99    box association distance (m), distanceThres_ :38 (associateBB :427-432) */
+  int lifetime_thres;          /* 3     lifetime a track needs before a box is associated, lifeTimeThres_ :41 */
+  double bb_yaw_change_thres;  /* 0.2   box yaw change (rad) below which the box is rotated, bbYawChangeThres_ :45 (updateBB :617-621) */
+  double second_init_v;        /* 2     speed (m/s) of a track at its second initialisation, targetV :902 */
+  int static_lifetime;         /* 8     lifetime above which a track may be flagged static, :1064 */
+  double static_dist;          /* 3.0   distance (m) from the first position below which it is, distThres :1067 */
+  double std_a[3];             /* 2, 2, 3  process noise, longitudinal acceleration (m/s^2) of CV, CTRV, RM: std_a_*_ ukf.cpp:68-70 */
+  double std_yawdd[3];         /* 2, 2, 3  process noise, yaw acceleration (rad/s^2) of CV, CTRV, RM: std_*_yawdd_ ukf.cpp:71-73 */
+  double std_las_x, std_las_y; /* 0.15, 0.15  lidar noise (m), std_laspx_ / std_laspy_ ukf.cpp:91-94 (R :841-842) */
+  double trans[3][3];          /* IMM transition matrix, row i = p{i+1}_ (from model i to model j): 0.9 on the diagonal, 0.05 elsewhere,
+                                  ukf.cpp:144-154 (MixingProbability :440-451) */
+  double mode_prob0[3];        /* 0.33 each  initial mode probabilities of a new track, ukf.cpp:180-182 */
+  double p0_diag[5];           /* 0.5, 0.5, 3, 10, 1  diagonal of a new track's covariance, P_merge_ ukf.cpp:275-279 */
+} lmot_tracker_params;
+/* Not parameters: the explosion guards (det > 10, P(4,4) > 1000, det(S) > 10), the mode-probability floor and the gate's S * 4, and
+ * the UKF members gammaG_ / pD_ / pG_ (ukf.cpp:216-218: only UKF::PDAupdate reads them, which the tracker never calls).
+ *
+ * lmot_default_tracker_params(p): the defaults above.
+ * lmot_set_tracker_params(ctx, p): the context's own track table (lmot_frame*, lmot_batch*, lmot_track_step, lmot_track_step_lists_dev,
+ *   and through it the owner rank of lmot_shared_*).  p == NULL restores the defaults.  lmot_get_tracker_params reads them back.
+ * lmot_seq_set_tracker_params(ctx, k, p) / lmot_seq_get_tracker_params: sequence k of the open set, for detection and tracking-only
+ *   ticks alike.  lmot_seq_open (reopening the set) resets every sequence to the defaults; lmot_seq_tracker_reset / _load keep them.
+ * Like the sensor tables, the parameters are host state captured by value when a step or tick is submitted: steps in flight keep the
+ * values they were submitted with, and a change applies to every track of the table -- those that already exist included -- from the
+ * next submitted step on.  (The reference fixes std_a, std_yawdd, the lidar noise and the transition matrix when a track's UKF is
+ * constructed; a mid-run change here equals a reference whose constants are the new values, reloaded from lmot_tracker_dump.)
+ * A table at the defaults runs the kernels it always ran; a tick in which any table has other values runs all of its tables through
+ * kernels that read each table's values, with bit-identical results for the tables at the defaults.
+ * LMOT_ERR_INVALID, parameters unchanged: a non-finite value; a standard deviation, gamma_g or p0_diag entry <= 0; p_g, p_d or a
+ * mode_prob0 entry outside (0, 1]; a trans entry outside [0, 1] or a trans column that is all zero (the mixing divides by its weighted
+ * sum); a negative lifetime_thres or static_lifetime; k out of range or no open set. */
+int lmot_default_tracker_params(lmot_tracker_params* p);
+int lmot_set_tracker_params(lmot_ctx* ctx, const lmot_tracker_params* p);
+int lmot_get_tracker_params(const lmot_ctx* ctx, lmot_tracker_params* p);
+int lmot_seq_set_tracker_params(lmot_ctx* ctx, int k, const lmot_tracker_params* p);
+int lmot_seq_get_tracker_params(const lmot_ctx* ctx, int k, lmot_tracker_params* p);
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);

@@ -12,5 +12,6 @@ timeout 300 python bench.py --impl reference --steps 20 --warmup 5 > measure_out
 timeout 600 python scripts/seq_measure.py > measure_out/${T}_seq.txt 2>&1; tail -9 measure_out/${T}_seq.txt
 timeout 600 python scripts/seq_rig_measure.py > measure_out/${T}_seq_rig.txt 2>&1; tail -7 measure_out/${T}_seq_rig.txt
 timeout 600 python scripts/seq_track_measure.py > measure_out/${T}_seq_track.txt 2>&1; tail -11 measure_out/${T}_seq_track.txt
+timeout 600 python scripts/tracker_params_measure.py > measure_out/${T}_tracker_params.txt 2>&1; tail -9 measure_out/${T}_tracker_params.txt
 timeout 300 python scripts/diag_timeline.py ${T}_timeline > measure_out/${T}_timeline.txt 2>&1; tail -5 measure_out/${T}_timeline.txt
 ls -la measure_out/${T}*
