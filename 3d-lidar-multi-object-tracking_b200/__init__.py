@@ -134,6 +134,43 @@ def _tracker_params(fields: dict) -> TrackerParams:
     return p
 
 
+class DetectParams(C.Structure):
+    """lmot_detect_params: ground removal, clustering ROI and box-fitting values of one sequence."""
+    _fields_ = [
+        ("r_min", C.c_float), ("r_max", C.c_float), ("t_hmin", C.c_float), ("t_hmax", C.c_float),
+        ("t_hdiff", C.c_float), ("h_sensor", C.c_float), ("ground_tolerance", C.c_double),
+        ("node_prefilter", C.c_int), ("filter_z_min", C.c_float), ("filter_z_max", C.c_float),
+        ("filter_x_min", C.c_float), ("filter_x_max", C.c_float), ("filter_y_min", C.c_float), ("filter_y_max", C.c_float),
+        ("roi_m", C.c_float),
+        ("ram_points", C.c_int), ("l_slope_dist", C.c_int), ("l_num_points", C.c_int), ("sensor_height", C.c_float),
+        ("t_height_min", C.c_float), ("t_height_max", C.c_float), ("t_width_min", C.c_float), ("t_width_max", C.c_float),
+        ("t_len_min", C.c_float), ("t_len_max", C.c_float), ("t_area_max", C.c_float),
+        ("t_ratio_min", C.c_float), ("t_ratio_max", C.c_float), ("min_len_ratio", C.c_float), ("t_pt_per_m3", C.c_float),
+        ("min_cluster_points", C.c_int), ("rule_filter", C.c_int),
+    ]
+
+
+MAX_RAM_POINTS = 1024
+
+
+def default_detect_params(params: Params | None = None) -> dict:
+    """lmot_default_detect_params: `params`' detection fields (None: the defaults) as a dict of field -> value"""
+    d = DetectParams()
+    load_library().lmot_default_detect_params(C.byref(params) if params is not None else None, C.byref(d))
+    return {name: getattr(d, name) for name, _ in DetectParams._fields_}
+
+
+def _detect_params(base: dict, fields: dict) -> DetectParams:
+    """`base` (a default_detect_params dict) with `fields` replaced (unknown names raise)"""
+    d = DetectParams()
+    names = dict(DetectParams._fields_)
+    for name, val in {**base, **fields}.items():
+        if name not in names:
+            raise ValueError(f"unknown detection parameter {name!r}")
+        setattr(d, name, int(val) if names[name] is C.c_int else float(val))
+    return d
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -157,7 +194,7 @@ ABI_SYMBOLS = [
     "lmot_seq_tracker_dump", "lmot_seq_tracker_get_ego", "lmot_seq_set_sensors", "lmot_seq_get_sensors", "lmot_seq_frame_counts",
     "lmot_seq_track_submit", "lmot_seq_track_dev", "lmot_seq_track", "lmot_seq_tracker_load", "lmot_seq_tracker_set_ego",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
-    "lmot_seq_get_tracker_params",
+    "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_detect_boxes_dev", "lmot_track_step_lists_dev", "lmot_tracker_counters_dev", "lmot_tracker_table_received",
     "lmot_origin_points", "lmot_tracker_table", "lmot_tracker_set_num_tracks", "lmot_tracker_reset", "lmot_tracker_num_tracks", "lmot_tracker_dump", "lmot_tracker_load", "lmot_tracker_get_ego", "lmot_tracker_set_ego",
     "lmot_debug_polar_grid", "lmot_debug_cell_index", "lmot_debug_label_grid", "lmot_selftest_atan2f",
@@ -579,6 +616,17 @@ class Lmot:
         p = TrackerParams()
         self._chk(self.lib.lmot_seq_get_tracker_params(self.h, int(k), C.byref(p)))
         return _tracker_params_dict(p)
+
+    # ---- detection parameters of a sequence (lmot_seq_set_detect_params) --------------------------------------------------------
+    def seq_set_detect_params(self, k: int, **fields):
+        """Sequence k detects with this context's lmot_params values, `fields` replaced; no fields: it follows lmot_params again."""
+        arg = C.byref(_detect_params(default_detect_params(self.params), fields)) if fields else None
+        self._chk(self.lib.lmot_seq_set_detect_params(self.h, int(k), arg))
+
+    def seq_get_detect_params(self, k: int) -> dict:
+        d = DetectParams()
+        self._chk(self.lib.lmot_seq_get_detect_params(self.h, int(k), C.byref(d)))
+        return {name: getattr(d, name) for name, _ in DetectParams._fields_}
 
     def seq_frame_counts(self, k: int) -> np.ndarray:
         """(n_frames, 4) int32: n_elevated, n_ground, num_cluster, n_boxes of each of sequence k's frames in the tick collected last"""

@@ -399,7 +399,7 @@ void seq_destroy(Ctx* c) {
       m = SeqMeas{};
     }
   for (int b = 0; b < kBatchBanks; ++b) { cudaFree(c->seq_stage[b]); c->seq_stage[b] = nullptr; }
-  for (int k = 0; k < kMaxBatch; ++k) { c->seq_n_sensors[k] = 0; c->seq_fc_n[k] = 0; }
+  for (int k = 0; k < kMaxBatch; ++k) { c->seq_n_sensors[k] = 0; c->seq_fc_n[k] = 0; c->seq_det_on[k] = false; }
   for (int i = 0; i < c->seq_ring; ++i)
     for (int k = 0; k < c->n_seq; ++k) result_destroy(&c->seq_ticks[i].blocks[k]);
   delete[] c->seq_ticks;
@@ -551,15 +551,11 @@ int lmot_create(lmot_ctx** out, const lmot_params* params, int device) {
   c->max_points = p.max_points;
   c->n_slots = p.pipeline_depth;
   c->n_results = p.result_ring;
-  c->gp.r_min = p.r_min; c->gp.r_max = p.r_max; c->gp.t_hmin = p.t_hmin; c->gp.t_hmax = p.t_hmax;
-  c->gp.t_hdiff = p.t_hdiff; c->gp.h_sensor = p.h_sensor;
-  { volatile float span = p.r_max - p.r_min; c->gp.r_span = span; }
-  c->gp.prefilter = p.node_prefilter ? 1 : 0;
-  c->gp.fz0 = p.filter_z_min; c->gp.fz1 = p.filter_z_max; c->gp.fx0 = p.filter_x_min; c->gp.fx1 = p.filter_x_max;
-  c->gp.fy0 = p.filter_y_min; c->gp.fy1 = p.filter_y_max;
-  c->gp.bin_scale = (float)((double)LMOT_NUM_BIN / (double)c->gp.r_span);
-  c->gp.tol = p.ground_tolerance;
-  gauss_taps(c->gp.tap);
+  {
+    double tap[3];
+    gauss_taps(tap);
+    c->gp = ground_params_of(detect_params_of(p), tap);
+  }
   if (const char* e = getenv("LMOT_COOP")) c->coop_launch = atoi(e) != 0;
   if (const char* e = getenv("LMOT_FUSE_CCL")) c->fuse_ccl = atoi(e) != 0;
   if (const char* e = getenv("LMOT_SPIN_LIMIT")) c->spin_limit = (unsigned)strtoul(e, nullptr, 0);   // 0: device-side waits never trap (debuggers, MPS)
@@ -1174,13 +1170,29 @@ static int seq_common(lmot_ctx* ctx, const float* const* points, const int* n, i
   k->res = &t->blocks[0]; sl[0]->res = &t->blocks[0];
   const bool gf = c->prm.global_frame != 0;
   SeqMeas m[kMaxBatch];
+  // sequences with their own detection values: every frame of the tick gets its entry (copied into the launch parameters), the values
+  // of its sequence -- or lmot_params' -- with its sensor's four mounting values in place of h_sensor / t_hmin / t_hmax / sensor_height
+  bool own_det = false;
+  for (int i = 0; i < n_seq; ++i) own_det |= c->seq_det_on[i];
+  lmot_detect_params det[kMaxBatch];
+  if (own_det) {
+    const lmot_detect_params base = detect_params_of(c->prm);
+    for (int i = 0; i < n_seq; ++i)
+      for (int j = f0[i]; j < f0[i + 1]; ++j) {
+        det[j] = c->seq_det_on[i] ? c->seq_det[i] : base;
+        if (rig_on[i]) {
+          const lmot_sensor& e = c->seq_sensors[i][j - f0[i]];
+          det[j].h_sensor = e.h_sensor; det[j].t_hmin = e.t_hmin; det[j].t_hmax = e.t_hmax; det[j].sensor_height = e.sensor_height;
+        }
+      }
+  }
   if (!rigged) {
     // detection: the batched launches of lmot_batch_* without a rig; each frame's last box-fitting CTA (or, global_frame, its
     // boxes_to_global CTA) posts its own slot's semaphore, which the tick's gate kernel polls
     for (int i = 0; i < n_seq; ++i) m[i] = SeqMeas{sl[i]->d_boxes, sl[i]->d_boxes_g, sl[i]->d_counters, sl[i]->d_det_sem};
-    if ((rc = ground_launch_batch(c, sl, n_seq, pp, n, st, true, false, c->fuse_ccl, false, nullptr))) return rc;
+    if ((rc = ground_launch_batch(c, sl, n_seq, pp, n, st, true, false, c->fuse_ccl, false, nullptr, own_det ? det : nullptr))) return rc;
     if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, n_seq, st))) return rc;
-    if ((rc = boxfit_launch_batch(c, sl, n_seq, st, n, !gf, nullptr))) return rc;
+    if ((rc = boxfit_launch_batch(c, sl, n_seq, st, n, !gf, nullptr, own_det ? det : nullptr))) return rc;
   } else {
     // detection with one sensor per frame (sequences without a table: lmot_params' values), copied into the launch parameters (later
     // table changes leave this tick alone); then each sequence's frames into its own list, whose semaphore the gate kernel polls
@@ -1194,9 +1206,9 @@ static int seq_common(lmot_ctx* ctx, const float* const* points, const int* n, i
       m[i] = c->seq_meas[b][i];
       LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc[i], t->blocks[i].h_frame_counts, 0));
     }
-    if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, c->fuse_ccl, false, rig))) return rc;
+    if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, c->fuse_ccl, false, rig, own_det ? det : nullptr))) return rc;
     if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
-    if ((rc = boxfit_launch_batch(c, sl, F, st, n, false, rig))) return rc;
+    if ((rc = boxfit_launch_batch(c, sl, F, st, n, false, rig, own_det ? det : nullptr))) return rc;
     if ((rc = boxes_concat_seq_launch(c, sl, n_seq, f0, rig_on, rig, m, fc, !gf, st))) return rc;
   }
   return seq_finish(c, t, b, st, m, ts, v, yaw);
@@ -1527,6 +1539,49 @@ int lmot_seq_set_tracker_params(lmot_ctx* ctx, int k, const lmot_tracker_params*
 int lmot_seq_get_tracker_params(const lmot_ctx* ctx, int k, lmot_tracker_params* p) {
   if (!ctx || !p || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
   *p = ctx->c.seq[k].prm;
+  return LMOT_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- detection parameters of a sequence
+int lmot_default_detect_params(const lmot_params* p, lmot_detect_params* out) {
+  if (!out) return LMOT_ERR_INVALID;
+  lmot_params d;
+  if (!p) { lmot_default_params(&d); p = &d; }
+  *out = detect_params_of(*p);
+  return LMOT_OK;
+}
+
+// What the kernels evaluate exactly.  The range window: the guarded fast path of the polar cell index (ground.cu polar_cell_fast) has
+// an error in bin units that grows with r_max / (r_max - r_min) (DESIGN.md §6d); a window of at least r_max / 5 keeps it below half
+// of the guard band.  ram_points: box fitting's table of mt19937_64 draws (boxfit.cu boxfit_alloc_shared).
+static bool detect_params_valid(const lmot_detect_params& d) {
+  const float f[] = {d.r_min, d.r_max, d.t_hmin, d.t_hmax, d.t_hdiff, d.h_sensor, d.filter_z_min, d.filter_z_max, d.filter_x_min,
+                     d.filter_x_max, d.filter_y_min, d.filter_y_max, d.roi_m, d.sensor_height, d.t_height_min, d.t_height_max,
+                     d.t_width_min, d.t_width_max, d.t_len_min, d.t_len_max, d.t_area_max, d.t_ratio_min, d.t_ratio_max, d.min_len_ratio,
+                     d.t_pt_per_m3};
+  for (float v : f) if (!std::isfinite(v)) return false;
+  if (!std::isfinite(d.ground_tolerance)) return false;
+  if (!(d.r_min >= 0.f) || !(d.r_max > d.r_min)) return false;
+  if (!((double)d.r_max - (double)d.r_min >= (double)d.r_max / 5.0)) return false;
+  if (!(d.roi_m > 0.f)) return false;
+  if (d.rule_filter != LMOT_RULE_INTENDED && d.rule_filter != LMOT_RULE_GCC13_O2_COMPAT) return false;
+  return d.ram_points >= 1 && d.ram_points <= LMOT_MAX_RAM_POINTS;
+}
+
+// host state only, as the sensor tables: submitted ticks carry their own copy in their launch parameters
+int lmot_seq_set_detect_params(lmot_ctx* ctx, int k, const lmot_detect_params* p) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  if (p && !detect_params_valid(*p)) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  c->seq_det_on[k] = p != nullptr;
+  if (p) c->seq_det[k] = *p;
+  return LMOT_OK;
+}
+
+int lmot_seq_get_detect_params(const lmot_ctx* ctx, int k, lmot_detect_params* p) {
+  if (!ctx || !p || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  const Ctx* c = &ctx->c;
+  *p = c->seq_det_on[k] ? c->seq_det[k] : detect_params_of(c->prm);
   return LMOT_OK;
 }
 

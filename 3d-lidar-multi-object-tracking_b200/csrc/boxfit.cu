@@ -23,6 +23,7 @@
 #include <climits>
 #include <cstring>
 #include <random>
+#include <vector>
 #include "lmot_internal.cuh"
 
 namespace lmot {
@@ -307,420 +308,23 @@ template <int NT, bool kRig>
 __global__ void __launch_bounds__(NT, 1024 / NT)     // <= 64 registers: 1,024 threads of box fitting per SM
 box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxParams P,
                const unsigned long long* __restrict__ mt_raw, int n_raw, int max_clusters, int max_boxes) {
-  constexpr int kFitThreads = NT;
-  fit_pdl_trigger();
-  fit_pdl_wait();                          // scatter_kernel is complete
-  const FitFrame& F = B.f[blockIdx.y];
-  const float4* __restrict__ sorted_pts = F.sorted_pts; const int* __restrict__ seg_start = F.seg_start; const int* __restrict__ seg_size = F.seg_size;
-  int* __restrict__ counters = F.counters;
-  float* __restrict__ cl_box = F.cl_box; float* __restrict__ cl_marker = F.cl_marker; uint8_t* __restrict__ cl_ok = F.cl_ok;
-  float* __restrict__ boxes = F.boxes; float* __restrict__ markers = F.markers; int* __restrict__ done = F.done; int* __restrict__ det_sem = F.det_sem;
-  __shared__ int s_lo[kCols], s_hi[kCols];
-  __shared__ short s_hx[kHullCap], s_hy[kHullCap];
-  __shared__ short s_cx[kCols], s_clo[kCols], s_chi[kCols];     // occupied pixel columns, compacted
-  __shared__ uint8_t s_flag8[kCols];
-  __shared__ unsigned long long s_red64[kFitThreads / 32];
-  __shared__ unsigned long long s_part64[2][kFitThreads / 32];
-  __shared__ double s_partd[3][kFitThreads / 32];
-  __shared__ float s_partf[7][kFitThreads / 32];
-  __shared__ int s_redi[kFitThreads / 32];
-  __shared__ int s_m;                        // hull size
-  __shared__ int s_best;                     // best edge
-  __shared__ unsigned long long s_bnum[kFitThreads / 32], s_bl[kFitThreads / 32];
-  __shared__ int s_bidx[kFitThreads / 32];
-  __shared__ float s_pc[4][2];
-  __shared__ int s_flag;
-  __shared__ int s_src[kFitThreads];         // compaction: cluster id of the j-th accepted box of the current batch
-  const int tid = threadIdx.x;
-  const int K = min(counters[CNT_NUM_CLUSTER], max_clusters);
-  const float half = P.roi / 2;
-  const float pic = P.pic_scale * P.roi;     // 900
+  // box_fit_body.inc reads: B, P, NT, kRig, mt_raw, n_raw, max_clusters, max_boxes
+#include "box_fit_body.inc"
+}
 
-  for (int k = blockIdx.x + 1; k <= K; k += gridDim.x) {
-    const int n = seg_size[k];
-    const float4* seg = sorted_pts + seg_start[k];          // the cluster's points, cloud order
-    if (tid == 0) cl_ok[k] = 0;
-    if (n < P.min_points || n <= 0) continue;      // ruleBasedFilter's first test (:100) rejects it whatever the fit
+// sequence ticks with their own detection values (lmot_seq_set_detect_params): frame blockIdx.y's whole BoxParams -- ROI and picScale,
+// L-shape gates, ram_points, min_points, rule mode and window, the sensor's height folded in on the host
+struct BoxFrameParams { BoxParams p[kMaxBatch]; };
+static_assert(sizeof(FitBatch) + sizeof(BoxFrameParams) + 32 <= 4096, "box_fit_frame_kernel: parameter block");
 
-    // ---- point #0 and the pixel offsets (:218-225)
-    const float4 q0 = __ldg(&seg[0]);
-    const int initX = (int)floorf((q0.x + half) * P.pic_scale);
-    const int initY = (int)floorf((q0.y + half) * P.pic_scale);
-    const int initPicX = initX;
-    const int initPicY = (int)(pic - (float)initY);
-    const int offsetInitX = (int)(P.roi * P.pic_scale / 2 - (float)initPicX);
-    const int offsetInitY = (int)(P.roi * P.pic_scale / 2 - (float)initPicY);
-
-    // ---- per-point pass (:239-293): column extremes for the hull, slope extremes, max z, centroid, AABB
-    for (int c = tid; c < kCols; c += kFitThreads) { s_lo[c] = INT_MAX; s_hi[c] = INT_MIN; }
-    __syncthreads();
-    unsigned long long kmin = ~0ull, kmax = 0ull;
-    float maxZ = -99.f;
-    double sx = 0, sy = 0, sz = 0;
-    float mnx = FLT_MAX, mny = FLT_MAX, mnz = FLT_MAX, mxx = -FLT_MAX, mxy = -FLT_MAX, mxz = -FLT_MAX;
-    // four points per thread in flight: as a plain loop this was one L2 round trip per iteration
-    for (int j0 = tid; j0 < n; j0 += 4 * kFitThreads) {
-      float4 qq[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) { const int j = j0 + u * kFitThreads; qq[u] = (j < n) ? __ldg(&seg[j]) : make_float4(0.f, 0.f, 0.f, 0.f); }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const int j = j0 + u * kFitThreads;
-        if (j >= n) break;
-        const float4 q = qq[u];
-        const int x = (int)floorf((q.x + half) * P.pic_scale);
-        const int y = (int)floorf((q.y + half) * P.pic_scale);
-        const int picX = x, picY = (int)(pic - (float)y);
-        const int offX = picX + offsetInitX, offY = picY + offsetInitY;
-        const int col = offX + kColShift;
-        if (col >= 0 && col < kCols) { atomicMin(&s_lo[col], offY); atomicMax(&s_hi[col], offY); }
-        const float m = q.y / q.x;
-        if (m < 999.f) { const unsigned long long key = ((unsigned long long)okey(m) << 32) | (unsigned)j; kmin = kmin < key ? kmin : key; }
-        if (m > -999.f) { const unsigned long long key = ((unsigned long long)okey(m) << 32) | (0xFFFFFFFFu - (unsigned)j); kmax = kmax > key ? kmax : key; }
-        if (q.z > maxZ) maxZ = q.z;
-        sx += q.x; sy += q.y; sz += q.z;
-        mnx = fminf(mnx, q.x); mny = fminf(mny, q.y); mnz = fminf(mnz, q.z);
-        mxx = fmaxf(mxx, q.x); mxy = fmaxf(mxy, q.y); mxz = fmaxf(mxz, q.z);
-      }
-    }
-    // thirteen block-wide reductions as ONE: shuffles inside the warp, one exchange of the per-warp partials through shared
-    // memory, threads 0..12 fold one quantity each (26 CTA barriers before, 2 now)
-    {
-      const int lane = tid & 31, warp = tid >> 5;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long a = __shfl_xor_sync(0xFFFFFFFFu, kmin, o), b = __shfl_xor_sync(0xFFFFFFFFu, kmax, o);
-        kmin = kmin < a ? kmin : a; kmax = kmax > b ? kmax : b;
-        maxZ = fmaxf(maxZ, __shfl_xor_sync(0xFFFFFFFFu, maxZ, o));
-        sx += __shfl_xor_sync(0xFFFFFFFFu, sx, o); sy += __shfl_xor_sync(0xFFFFFFFFu, sy, o); sz += __shfl_xor_sync(0xFFFFFFFFu, sz, o);
-        mnx = fminf(mnx, __shfl_xor_sync(0xFFFFFFFFu, mnx, o)); mny = fminf(mny, __shfl_xor_sync(0xFFFFFFFFu, mny, o)); mnz = fminf(mnz, __shfl_xor_sync(0xFFFFFFFFu, mnz, o));
-        mxx = fmaxf(mxx, __shfl_xor_sync(0xFFFFFFFFu, mxx, o)); mxy = fmaxf(mxy, __shfl_xor_sync(0xFFFFFFFFu, mxy, o)); mxz = fmaxf(mxz, __shfl_xor_sync(0xFFFFFFFFu, mxz, o));
-      }
-      __syncthreads();                       // (the previous cluster's readers of s_part are done)
-      if (lane == 0) {
-        s_part64[0][warp] = kmin; s_part64[1][warp] = kmax;
-        s_partd[0][warp] = sx; s_partd[1][warp] = sy; s_partd[2][warp] = sz;
-        s_partf[0][warp] = maxZ; s_partf[1][warp] = mnx; s_partf[2][warp] = mny; s_partf[3][warp] = mnz;
-        s_partf[4][warp] = mxx; s_partf[5][warp] = mxy; s_partf[6][warp] = mxz;
-      }
-      __syncthreads();
-      constexpr int NW = kFitThreads / 32;
-      if (tid < 2) {
-        unsigned long long r = s_part64[tid][0];
-        for (int w = 1; w < NW; ++w) { const unsigned long long v = s_part64[tid][w]; r = (tid == 0) ? (r < v ? r : v) : (r > v ? r : v); }
-        s_part64[tid][0] = r;
-      } else if (tid < 5) {
-        double r = s_partd[tid - 2][0];
-        for (int w = 1; w < NW; ++w) r += s_partd[tid - 2][w];
-        s_partd[tid - 2][0] = r;
-      } else if (tid < 12) {
-        const int q = tid - 5;
-        float r = s_partf[q][0];
-        for (int w = 1; w < NW; ++w) r = (q == 0 || q >= 4) ? fmaxf(r, s_partf[q][w]) : fminf(r, s_partf[q][w]);
-        s_partf[q][0] = r;
-      }
-      __syncthreads();
-      kmin = s_part64[0][0]; kmax = s_part64[1][0];
-      sx = s_partd[0][0]; sy = s_partd[1][0]; sz = s_partd[2][0];
-      maxZ = s_partf[0][0]; mnx = s_partf[1][0]; mny = s_partf[2][0]; mnz = s_partf[3][0];
-      mxx = s_partf[4][0]; mxy = s_partf[5][0]; mxz = s_partf[6][0];
-    }
-
-    // first-occurrence min / max slope points (:268-280).  If no slope beats the 999 / -999 seeds the reference
-    // reads uninitialised floats; defined here as (0,0).
-    float minMx = 0.f, minMy = 0.f, maxMx = 0.f, maxMy = 0.f;
-    if (kmin != ~0ull) { const float4 q = __ldg(&seg[(unsigned)(kmin & 0xFFFFFFFFull)]); minMx = q.x; minMy = q.y; }
-    if (kmax != 0ull) { const float4 q = __ldg(&seg[0xFFFFFFFFu - (unsigned)(kmax & 0xFFFFFFFFull)]); maxMx = q.x; maxMy = q.y; }
-    const float xDist = maxMx - minMx, yDist = maxMy - minMy;
-    const float slopeDist = sqrtf(xDist * xDist + yDist * yDist);
-    const float slope = (maxMy - minMy) / (maxMx - minMx);
-
-    float pc[4][2];
-    if (slopeDist > (float)P.l_slope_dist && n > P.l_num_points && (maxMy > 8.f || maxMy < -5.f)) {
-      // ---- L-shape (:303-356): 80 draws of uniform_int_distribution<>(0,n-1) over mt19937_64(0), Lemire mapping
-      // (libstdc++ >= 11): idx = hi64(raw*n), redraw while lo64 < 2^64 mod n.  First strictly larger distance wins.
-      const float den = sqrtf(slope * slope + 1);
-      const unsigned long long un = (unsigned long long)n;
-      const unsigned long long thr = (0ull - un) % un;
-      // one draw per thread; a Lemire redraw (probability n / 2^64) shifts the stream, then thread 0 replays it in order
-      bool redraw = false;
-      unsigned long long key = 0ull;                       // (dist bits << 32) | (~draw index): max = first largest dist
-      float myx = 0.f, myy = 0.f;
-      if (tid < P.ram_points) {
-        const unsigned long long raw = mt_raw[tid % n_raw];
-        redraw = raw * un < thr;
-        const unsigned pInd = (unsigned)__umul64hi(raw, un);
-        const float4 q = __ldg(&seg[pInd]);
-        const float dist = fabsf(slope * q.x - 1 * q.y + maxMy - slope * maxMx) / den;
-        myx = q.x; myy = q.y;
-        if (dist > 0.f) key = ((unsigned long long)__float_as_uint(dist) << 32) | (0xFFFFFFFFu - (unsigned)tid);
-      }
-      const bool slow = __syncthreads_or(redraw) || P.ram_points > kFitThreads;
-      if (!slow) {
-        const unsigned long long best = block_reduce(key, MaxU64(), s_red64);
-        const unsigned win = 0xFFFFFFFFu - (unsigned)(best & 0xFFFFFFFFull);
-        if (best == 0ull) { if (tid == 0) { s_pc[1][0] = 0.f; s_pc[1][1] = 0.f; } }   // no dist > 0: uninitialised in the reference
-        else if ((unsigned)tid == win) { s_pc[1][0] = myx; s_pc[1][1] = myy; }
-      } else if (tid == 0) {
-        float maxDist = 0.f, maxDx = 0.f, maxDy = 0.f;
-        int cur = 0;
-        for (int i = 0; i < P.ram_points; ++i) {
-          unsigned long long raw = mt_raw[cur % n_raw]; ++cur;
-          unsigned long long lo = raw * un;
-          while (lo < thr) { raw = mt_raw[cur % n_raw]; ++cur; lo = raw * un; }
-          const unsigned pInd = (unsigned)__umul64hi(raw, un);
-          const float4 q = __ldg(&seg[pInd]);
-          const float dist = fabsf(slope * q.x - 1 * q.y + maxMy - slope * maxMx) / den;
-          if (dist > maxDist) { maxDist = dist; maxDx = q.x; maxDy = q.y; }
-        }
-        s_pc[1][0] = maxDx; s_pc[1][1] = maxDy;
-      }
-      __syncthreads();
-      if (tid == 0) {
-        const float maxDx = s_pc[1][0], maxDy = s_pc[1][1];
-        const float maxMvecX = maxMx - maxDx, maxMvecY = maxMy - maxDy;
-        const float minMvecX = minMx - maxDx, minMvecY = minMy - maxDy;
-        s_pc[0][0] = minMx; s_pc[0][1] = minMy;
-        s_pc[2][0] = maxMx; s_pc[2][1] = maxMy;
-        s_pc[3][0] = maxDx + maxMvecX + minMvecX; s_pc[3][1] = maxDy + maxMvecY + minMvecY;
-      }
-      __syncthreads();
-    } else {
-      // ---- MAR contract (oracle/mar_contract.cpp): strict hull of the pixel set from the column extremes
-      // strict convex hull of the pixel set, same canonical sequence as Andrew's monotone chain in
-      // oracle/mar_contract.cpp (start = lexicographic minimum, lower chain left to right, upper chain right to left),
-      // computed in parallel from the per-column extremes:
-      //   (c, lo[c]) is a lower-hull vertex  <=>  max slope from any column on its left  <  min slope to any column on its right
-      //   (c, hi[c]) is an upper-hull vertex <=>  min slope from the left                >  max slope to the right
-      // (first / last occupied columns always are); slopes are compared exactly as integer cross products.
-      int W;
-      {
-        // compact the occupied columns: thread t owns columns [8t, 8t+8)
-        int cnt = 0;
-#pragma unroll
-        for (int u = 0; u < 8; ++u) { const int c = tid * 8 + u; if (c < kCols && s_lo[c] != INT_MAX) ++cnt; }
-        int incl = cnt;
-        const int lane = tid & 31, warp = tid >> 5;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= o) incl += t; }
-        if (lane == 31) s_redi[warp] = incl;
-        __syncthreads();
-        int wbase = 0, tot = 0;
-        for (int w = 0; w < kFitThreads / 32; ++w) { if (w < warp) wbase += s_redi[w]; tot += s_redi[w]; }
-        int pos = wbase + incl - cnt;
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const int c = tid * 8 + u;
-          if (c < kCols && s_lo[c] != INT_MAX) { s_cx[pos] = (short)(c - kColShift); s_clo[pos] = (short)s_lo[c]; s_chi[pos] = (short)s_hi[c]; ++pos; }
-        }
-        W = tot;
-        __syncthreads();
-      }
-      for (int i = tid; i < W; i += kFitThreads) {
-        const int xi = s_cx[i], li = s_clo[i], hi = s_chi[i];
-        bool lowv = true, upv = true;
-        if (i > 0 && i < W - 1) {
-          // left side: running extreme slopes as (dy, dx), dx > 0
-          int lmax_n = 0, lmax_d = 0, umin_n = 0, umin_d = 0;
-          for (int j = 0; j < i; ++j) {
-            const int dx = xi - s_cx[j];
-            const int dl = li - s_clo[j], du = hi - s_chi[j];
-            if (lmax_d == 0 || (long long)dl * lmax_d > (long long)lmax_n * dx) { lmax_n = dl; lmax_d = dx; }
-            if (umin_d == 0 || (long long)du * umin_d < (long long)umin_n * dx) { umin_n = du; umin_d = dx; }
-          }
-          for (int k = i + 1; k < W && (lowv || upv); ++k) {
-            const int dx = s_cx[k] - xi;
-            const int dl = s_clo[k] - li, du = s_chi[k] - hi;
-            if (!((long long)lmax_n * dx < (long long)dl * lmax_d)) lowv = false;   // need lmax < slope to k
-            if (!((long long)umin_n * dx > (long long)du * umin_d)) upv = false;    // need umin > slope to k
-          }
-        }
-        s_flag8[i] = (lowv ? 1 : 0) | (upv ? 2 : 0);
-      }
-      __syncthreads();
-      // hull sequence = lower-chain vertices left to right, then upper-chain vertices right to left: positions from two block-wide
-      // counts (thread t owns the compacted columns [8t, 8t+8)); as a loop on thread 0 this was 2 W dependent shared-memory
-      // round trips, the longest phase of the slowest CTA
-      if (W == 1) {
-        if (tid == 0) {
-          int m = 1;
-          s_hx[0] = s_cx[0]; s_hy[0] = s_clo[0];
-          if (s_chi[0] != s_clo[0]) { s_hx[1] = s_cx[0]; s_hy[1] = s_chi[0]; m = 2; }
-          s_m = m;
-        }
-      } else {
-        const int lane = tid & 31, warp = tid >> 5;
-        unsigned lowm = 0, upm = 0;
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const int i = tid * 8 + u;
-          if (i < W) {
-            const int fl = s_flag8[i];
-            if (fl & 1) lowm |= 1u << u;
-            // the lo point of the first / last column already sits in the lower chain
-            if ((fl & 2) && !((i == 0 || i == W - 1) && s_chi[i] == s_clo[i])) upm |= 1u << u;
-          }
-        }
-        const int cl = __popc(lowm), cu = __popc(upm);
-        int il = cl, iu = cu;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const int a = __shfl_up_sync(0xFFFFFFFFu, il, o), b = __shfl_up_sync(0xFFFFFFFFu, iu, o);
-          if (lane >= o) { il += a; iu += b; }
-        }
-        if (lane == 31) { s_redi[warp] = il; s_bidx[warp] = iu; }
-        __syncthreads();
-        int bl = 0, bu = 0, tl = 0, tu = 0;
-        for (int w = 0; w < kFitThreads / 32; ++w) { if (w < warp) { bl += s_redi[w]; bu += s_bidx[w]; } tl += s_redi[w]; tu += s_bidx[w]; }
-        int pl = bl + il - cl;                        // lower-chain vertices before this thread's columns
-        int pu_after = tu - (bu + iu);                // upper-chain vertices AFTER this thread's columns (they come first, right to left)
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const int i = tid * 8 + u;
-          if ((lowm >> u) & 1u) { if (pl < kHullCap) { s_hx[pl] = s_cx[i]; s_hy[pl] = s_clo[i]; } ++pl; }
-        }
-#pragma unroll
-        for (int u = 7; u >= 0; --u) {
-          const int i = tid * 8 + u;
-          if ((upm >> u) & 1u) { const int pos = tl + pu_after; if (pos < kHullCap) { s_hx[pos] = s_cx[i]; s_hy[pos] = s_chi[i]; } ++pu_after; }
-        }
-        if (tid == 0) {
-          int m = tl + tu;
-          if (m > kHullCap) { counters[CNT_ERROR] = LMOT_ERR_CAPACITY; m = kHullCap; }
-          s_m = m;
-        }
-      }
-      __syncthreads();
-      const int m = s_m;
-      float rc[4][2];
-      if (m == 1) {
-        for (int c = 0; c < 4; ++c) { rc[c][0] = (float)s_hx[0]; rc[c][1] = (float)s_hy[0]; }
-      } else if (m == 2) {
-        rc[0][0] = rc[1][0] = (float)s_hx[0]; rc[0][1] = rc[1][1] = (float)s_hy[0];
-        rc[2][0] = rc[3][0] = (float)s_hx[1]; rc[2][1] = rc[3][1] = (float)s_hy[1];
-      } else {
-        // exact min-area edge: area_i = W*T/l compared as rationals, ties -> lowest edge index
-        unsigned long long bnum = 0, bl = 1; int bidx = INT_MAX;
-        for (int i = tid; i < m; i += kFitThreads) {
-          const int i1 = (i + 1 == m) ? 0 : i + 1;
-          const int dx = s_hx[i1] - s_hx[i], dy = s_hy[i1] - s_hy[i];
-          int smin = INT_MAX, smax = INT_MIN, tmin = INT_MAX, tmax = INT_MIN;
-          for (int j = 0; j < m; ++j) {
-            const int s = s_hx[j] * dx + s_hy[j] * dy, t = -s_hx[j] * dy + s_hy[j] * dx;
-            smin = min(smin, s); smax = max(smax, s); tmin = min(tmin, t); tmax = max(tmax, t);
-          }
-          const unsigned long long num = (unsigned long long)(smax - smin) * (unsigned long long)(tmax - tmin);
-          const unsigned long long l = (unsigned long long)((long long)dx * dx + (long long)dy * dy);
-          if (bidx == INT_MAX || num * bl < bnum * l) { bnum = num; bl = l; bidx = i; }   // i ascending per thread
-        }
-        // warp then block argmin with the same comparator (index breaks ties)
-        for (int o = 16; o > 0; o >>= 1) {
-          const unsigned long long onum = __shfl_xor_sync(0xFFFFFFFFu, bnum, o), ol = __shfl_xor_sync(0xFFFFFFFFu, bl, o);
-          const int oidx = __shfl_xor_sync(0xFFFFFFFFu, bidx, o);
-          if (oidx != INT_MAX) {
-            const bool better = (bidx == INT_MAX) || (onum * bl < bnum * ol) || (onum * bl == bnum * ol && oidx < bidx);
-            if (better) { bnum = onum; bl = ol; bidx = oidx; }
-          }
-        }
-        if ((tid & 31) == 0) { s_bnum[tid >> 5] = bnum; s_bl[tid >> 5] = bl; s_bidx[tid >> 5] = bidx; }
-        __syncthreads();
-        if (tid == 0) {
-          for (int w = 1; w < kFitThreads / 32; ++w) {
-            if (s_bidx[w] == INT_MAX) continue;
-            const bool better = (bidx == INT_MAX) || (s_bnum[w] * bl < bnum * s_bl[w]) || (s_bnum[w] * bl == bnum * s_bl[w] && s_bidx[w] < bidx);
-            if (better) { bnum = s_bnum[w]; bl = s_bl[w]; bidx = s_bidx[w]; }
-          }
-          s_best = bidx;
-        }
-        __syncthreads();
-        const int best = s_best, b1 = (best + 1 == m) ? 0 : best + 1;
-        long long ux = s_hx[b1] - s_hx[best], uy = s_hy[b1] - s_hy[best];
-        for (int r = 0; r < 4 && !(ux >= 0 && uy < 0); ++r) { const long long t = ux; ux = -uy; uy = t; }
-        const long long l = ux * ux + uy * uy;
-        int smin = INT_MAX, smax = INT_MIN, tmin = INT_MAX, tmax = INT_MIN;
-        for (int j = tid; j < m; j += kFitThreads) {
-          const int s = (int)(s_hx[j] * ux + s_hy[j] * uy), t = (int)(-s_hx[j] * uy + s_hy[j] * ux);
-          smin = min(smin, s); smax = max(smax, s); tmin = min(tmin, t); tmax = max(tmax, t);
-        }
-        smin = block_reduce(smin, MinI(), s_redi); smax = block_reduce(smax, MaxI(), s_redi);
-        tmin = block_reduce(tmin, MinI(), s_redi); tmax = block_reduce(tmax, MaxI(), s_redi);
-        const long long S[4] = {smin, smin, smax, smax}, T[4] = {tmax, tmin, tmin, tmax};
-        for (int c = 0; c < 4; ++c) {
-          rc[c][0] = (float)((double)(S[c] * ux - T[c] * uy) / (double)l);
-          rc[c][1] = (float)((double)(S[c] * uy + T[c] * ux) / (double)l);
-        }
-      }
-      // getPointsInPcFrame (:75-95)
-      if (tid == 0) {
-        for (int c = 0; c < 4; ++c) {
-          const float rOffsetX = rc[c][0] - (float)offsetInitX, rOffsetY = rc[c][1] - (float)offsetInitY;
-          const float rX = rOffsetX, rY = P.pic_scale * P.roi - rOffsetY;
-          const float rmX = rX / P.pic_scale, rmY = rY / P.pic_scale;
-          s_pc[c][0] = rmX - P.roi / 2; s_pc[c][1] = rmY - P.roi / 2;
-        }
-      }
-      __syncthreads();
-    }
-    for (int c = 0; c < 4; ++c) { pc[c][0] = s_pc[c][0]; pc[c][1] = s_pc[c][1]; }
-    const bool ok = rule_filter(pc, maxZ, n, P, kRig ? F.sensor_height : P.sensor_height);
-    if (tid == 0) {
-      cl_ok[k] = ok ? 1 : 0;
-      if (ok) {
-        float* b = cl_box + (size_t)k * 24;
-        for (int h = 0; h < 2; ++h)
-          for (int c = 0; c < 4; ++c) { b[(h * 4 + c) * 3] = pc[c][0]; b[(h * 4 + c) * 3 + 1] = pc[c][1]; b[(h * 4 + c) * 3 + 2] = h == 0 ? -(kRig ? F.sensor_height : P.sensor_height) : maxZ; }
-        float* mk = cl_marker + (size_t)k * 6;      // mark_cluster (:161-209); zero extents become 0.1
-        mk[0] = (float)(sx / n); mk[1] = (float)(sy / n); mk[2] = (float)(sz / n);
-        float ex = mxx - mnx, ey = mxy - mny, ez = mxz - mnz;
-        mk[3] = ex == 0.f ? 0.1f : ex; mk[4] = ey == 0.f ? 0.1f : ey; mk[5] = ez == 0.f ? 0.1f : ez;
-      }
-    }
-    __syncthreads();
-  }
-
-  // ---- the last CTA of the frame compacts the accepted boxes in cluster-id order
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) s_flag = (atomicAdd(done, 1) == (int)gridDim.x - 1);
-  __syncthreads();
-  if (!s_flag) return;
-  __threadfence();
-  int carry = 0;
-  for (int k0 = 1; k0 <= K; k0 += kFitThreads) {
-    const int k = k0 + tid;
-    const int f = (k <= K) ? __ldcg((const unsigned char*)&cl_ok[k]) : 0;
-    const unsigned bal = __ballot_sync(0xFFFFFFFFu, f);
-    if ((tid & 31) == 0) s_redi[tid >> 5] = __popc(bal);
-    __syncthreads();
-    int wbase = 0, tot = 0;
-    for (int w = 0; w < kFitThreads / 32; ++w) { if (w < (tid >> 5)) wbase += s_redi[w]; tot += s_redi[w]; }
-    const int pos = carry + wbase + __popc(bal & ((1u << (tid & 31)) - 1u));
-    if (f && pos < max_boxes) s_src[pos - carry] = k;
-    __syncthreads();
-    // cooperative copy: consecutive threads move consecutive floats
-    const int nacc = min(tot, max_boxes - carry);
-    for (int e = tid; e < nacc * 24; e += kFitThreads) {
-      const int j = e / 24, w = e - j * 24;
-      const float v = __ldcg(&cl_box[(size_t)s_src[j] * 24 + w]);
-      boxes[(size_t)(carry + j) * 24 + w] = v;
-    }
-    for (int e = tid; e < nacc * 6; e += kFitThreads) {
-      const int j = e / 6, w = e - j * 6;
-      markers[(size_t)(carry + j) * 6 + w] = __ldcg(&cl_marker[(size_t)s_src[j] * 6 + w]);
-    }
-    carry += tot;
-    __syncthreads();
-  }
-  if (tid == 0) {
-    if (carry > max_boxes) { counters[CNT_ERROR] = LMOT_ERR_CAPACITY; carry = max_boxes; }
-    counters[CNT_N_BOXES] = carry;
-  }
-  // the frame's detection stages are complete: post the slot's semaphore for the tracker's gate kernel (tracker.cu), which takes
-  // the place of a stream-level event wait in front of the tracker chain
-  if (det_sem) {
-    __syncthreads();
-    if (tid == 0) { __threadfence(); atomicAdd(det_sem, 1); }
-  }
+template <int NT>
+__global__ void __launch_bounds__(NT, 1024 / NT)
+box_fit_frame_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxFrameParams PF,
+                     const unsigned long long* __restrict__ mt_raw, int n_raw, int max_clusters, int max_boxes) {
+  constexpr bool kRig = false;                 // (the sensor's height is folded into the frame's entry)
+  const BoxParams& P = PF.p[blockIdx.y];
+  // box_fit_body.inc reads: B, P, NT, kRig, mt_raw, n_raw, max_clusters, max_boxes
+#include "box_fit_body.inc"
 }
 
 // p' = [R | t] p (lmot_set_sensors): ((r0 x + r1 y) + r2 z) + t per row in float, no contraction -- pcl::transformPointCloud's
@@ -841,15 +445,16 @@ concat_boxes_seq_kernel(const __grid_constant__ FitBatch B, const __grid_constan
 }  // namespace
 
 int boxfit_alloc_shared(Ctx* c) {
-  // raw mt19937_64(0) stream (box_fitting.cpp:303 re-seeds per cluster, so every cluster sees the same draws)
-  constexpr int kRaw = 256;
+  // raw mt19937_64(0) stream (box_fitting.cpp:303 re-seeds per cluster, so every cluster sees the same draws): LMOT_MAX_RAM_POINTS
+  // draws and 64 spare ones for Lemire redraws (odds n / 2^64 each).  The first 256 values are the table's earlier extent.
+  constexpr int kRaw = LMOT_MAX_RAM_POINTS + 64;
   std::mt19937_64 mt(0);
-  unsigned long long raw[kRaw];
+  std::vector<unsigned long long> raw(kRaw);
   for (int i = 0; i < kRaw; ++i) raw[i] = mt();
   c->n_mt_raw = kRaw;
   c->max_sort_tiles = (c->max_points + kTile - 1) / kTile;
-  LMOT_CUDA(c, cudaMalloc(&c->d_mt_raw, sizeof(raw)));
-  LMOT_CUDA(c, cudaMemcpy(c->d_mt_raw, raw, sizeof(raw), cudaMemcpyHostToDevice));
+  LMOT_CUDA(c, cudaMalloc(&c->d_mt_raw, kRaw * sizeof(unsigned long long)));
+  LMOT_CUDA(c, cudaMemcpy(c->d_mt_raw, raw.data(), kRaw * sizeof(unsigned long long), cudaMemcpyHostToDevice));
   // tile_hist / scatter keep one int per cluster id in dynamic shared memory (lmot_create bounds max_clusters accordingly)
   const int sh = (c->prm.max_clusters + 1) * (int)sizeof(int);
   if (sh > 48 * 1024) {
@@ -903,7 +508,21 @@ static void fit_frame_of(const Slot* s, FitFrame& f, bool post_sem) {
 
 // inputs per frame: s->d_elev / CNT_N_ELEV, s->d_cart (from clustering), s->d_label_grid / CNT_NUM_CLUSTER.
 // F > 1: one frame per sensor stream; the four kernels run over the union of the frames' clusters (blockIdx.y = frame).
-int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig) {
+// BoxParams of detection values d (the context's, or a frame's own)
+static BoxParams box_params_of(const lmot_detect_params& p) {
+  BoxParams P;
+  P.roi = p.roi_m;
+  { volatile float ps = 900 / p.roi_m; P.pic_scale = ps; }   // float picScale = 900/roiM (box_fitting.cpp:18)
+  P.sensor_height = p.sensor_height; P.ram_points = p.ram_points; P.l_slope_dist = p.l_slope_dist;
+  P.l_num_points = p.l_num_points; P.min_points = p.min_cluster_points; P.rule_mode = p.rule_filter;
+  P.t_height_min = p.t_height_min; P.t_height_max = p.t_height_max; P.t_width_min = p.t_width_min; P.t_width_max = p.t_width_max;
+  P.t_len_min = p.t_len_min; P.t_len_max = p.t_len_max; P.t_area_max = p.t_area_max; P.t_ratio_min = p.t_ratio_min;
+  P.t_ratio_max = p.t_ratio_max; P.min_len_ratio = p.min_len_ratio; P.t_pt_per_m3 = p.t_pt_per_m3;
+  return P;
+}
+
+int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig,
+                        const lmot_detect_params* det) {
   if (F < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   const int K1 = c->prm.max_clusters + 1;
   int tiles = 0;
@@ -928,15 +547,7 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
     LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, scatter_kernel, B, max_clusters));
     kernel_mark(c, s0, st);
   }
-  BoxParams P;
-  const lmot_params& p = c->prm;
-  P.roi = p.roi_m;
-  { volatile float ps = 900 / p.roi_m; P.pic_scale = ps; }   // float picScale = 900/roiM (box_fitting.cpp:18)
-  P.sensor_height = p.sensor_height; P.ram_points = p.ram_points; P.l_slope_dist = p.l_slope_dist;
-  P.l_num_points = p.l_num_points; P.min_points = p.min_cluster_points; P.rule_mode = p.rule_filter;
-  P.t_height_min = p.t_height_min; P.t_height_max = p.t_height_max; P.t_width_min = p.t_width_min; P.t_width_max = p.t_width_max;
-  P.t_len_min = p.t_len_min; P.t_len_max = p.t_len_max; P.t_area_max = p.t_area_max; P.t_ratio_min = p.t_ratio_min;
-  P.t_ratio_max = p.t_ratio_max; P.min_len_ratio = p.min_len_ratio; P.t_pt_per_m3 = p.t_pt_per_m3;
+  const BoxParams P = box_params_of(detect_params_of(c->prm));
   // one CTA per cluster: a frame rarely holds more than a few hundred clusters, F frames share the grid
   const int gx = F == 1 ? c->fit_ctas : (c->fit_ctas / 2 > 8 ? c->fit_ctas / 2 : 8);
   {
@@ -944,7 +555,13 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
     cfg.gridDim = dim3(gx, F); cfg.blockDim = dim3(F == 1 ? kFitThreadsFrame : kFitThreadsBatch); cfg.dynamicSmemBytes = 0; cfg.stream = st; cfg.attrs = &pdl; cfg.numAttrs = 1;
     const unsigned long long* mt = c->d_mt_raw;
     const int n_raw = c->n_mt_raw, max_boxes = c->prm.max_boxes;
-    if (rig) {
+    if (det) {
+      BoxFrameParams FP;
+      memset(&FP, 0, sizeof(FP));
+      for (int i = 0; i < F; ++i) FP.p[i] = box_params_of(det[i]);
+      if (F == 1) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_frame_kernel<kFitThreadsFrame>, B, FP, mt, n_raw, max_clusters, max_boxes));
+      else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_frame_kernel<kFitThreadsBatch>, B, FP, mt, n_raw, max_clusters, max_boxes));
+    } else if (rig) {
       if (F == 1) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsFrame, true>, B, P, mt, n_raw, max_clusters, max_boxes));
       else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsBatch, true>, B, P, mt, n_raw, max_clusters, max_boxes));
     } else {

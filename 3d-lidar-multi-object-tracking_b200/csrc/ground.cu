@@ -21,6 +21,7 @@
 //
 // Everything that decides a cell index or a label is IEEE round-to-nearest without FMA contraction, so the
 // results are bit-identical to the reference built for x86-64.
+#include <climits>
 #include <cstring>
 #include <mutex>
 #include "lmot_internal.cuh"
@@ -53,6 +54,9 @@ __device__ __forceinline__ float fkey_inv(unsigned k) {
 
 // ground_removal.cpp:46-64 (range filter) + :67-76 (getCellIndexFromPoints) + :89 (index guard), evaluated exactly as the
 // reference does: IEEE sqrt and divisions, glibc's atan2f (fdlibm restatement, exact_math.cuh), the double add / divide.
+// kClone: ground_fused_frame_kernel calls its own copy -- one shared non-inlined function would be compiled for the most general of its
+// callers' arguments (a frame's entry of a parameter array) and change the code of the other kernels
+template <int kClone = 0>
 __device__ __noinline__ uint16_t polar_cell_exact(float x, float y, const GroundParams& p) {
   const float d = fsqrt(fadd(fmul(x, x), fmul(y, y)));
   if (d <= p.r_min || d >= p.r_max || d != d) return kNoCell;
@@ -398,7 +402,7 @@ __device__ __forceinline__ void smem_min_u32(uint32_t addr, unsigned v) {
 
 // Two tiles of phase 1 (see the kernel).  FULL: both tiles exist, are resident in shared memory and hold kTilePts points each;
 // PRE: the node's pre-filters are on.
-template <bool FULL, bool PRE>
+template <bool FULL, bool PRE, int kClone>
 __device__ __forceinline__ void bin_pair(int t0, int T, int cnt, int res_tiles, int beg, const float4* __restrict__ pts, const float4* s_pts,
                                          uint16_t* s_cell, uint64_t* s_full, unsigned* s_meta, uint16_t* s_pend, uint32_t keys_sa,
                                          const GroundParams& p) {
@@ -457,7 +461,7 @@ __device__ __forceinline__ void bin_pair(int t0, int T, int cnt, int res_tiles, 
       if (cc == kPending) {
         const unsigned slot = base + __popc(pm & ((1u << lane) - 1u));
         if (slot < (unsigned)kPendCap) s_pend[slot] = (uint16_t)li;
-        else cc = polar_cell_exact(q[u].x, q[u].y, p);       // queue full (adversarial clouds): evaluate here
+        else cc = polar_cell_exact<kClone>(q[u].x, q[u].y, p);   // queue full (adversarial clouds): evaluate here
       }
     }
     s_cell[li] = (PRE && pre[u]) ? kPreFiltered : (uint16_t)cc;
@@ -480,7 +484,7 @@ __device__ __forceinline__ void bin_pair(int t0, int T, int cnt, int res_tiles, 
 // memory.  With ring-major clouds a chunk spans most of the 80 channels, so every CTA redid most of the grid and the kernel
 // issued far more instructions.  The grid is evaluated ONCE, spread over the CTAs.)
 // kRig: phase 2 takes each frame's t_hmin / t_hmax / h_sensor from B.mount (a sensor rig, lmot_set_sensors) instead of p
-template <bool kRig>
+template <bool kRig, int kClone = 0>
 __device__ __forceinline__ void ground_fused_body(const GroundBatch& B, const GroundParams& p, float roi) {
   extern __shared__ __align__(128) unsigned char fsm[];
   const int Gf = B.ctas_per_frame;
@@ -541,9 +545,9 @@ __device__ __forceinline__ void ground_fused_body(const GroundBatch& B, const Gr
     const uint32_t keys_sa = smem_u32(s_keys);
     const int full_end = p.prefilter ? 0 : (min(cnt / kTilePts, res_tiles) & ~1);
     int t0 = 0;
-    for (; t0 < full_end; t0 += 2) bin_pair<true, false>(t0, T, cnt, res_tiles, beg, pts, s_pts, s_cell, s_full, s_meta, s_pend, keys_sa, p);
-    if (p.prefilter) for (; t0 < T; t0 += 2) bin_pair<false, true>(t0, T, cnt, res_tiles, beg, pts, s_pts, s_cell, s_full, s_meta, s_pend, keys_sa, p);
-    else for (; t0 < T; t0 += 2) bin_pair<false, false>(t0, T, cnt, res_tiles, beg, pts, s_pts, s_cell, s_full, s_meta, s_pend, keys_sa, p);
+    for (; t0 < full_end; t0 += 2) bin_pair<true, false, kClone>(t0, T, cnt, res_tiles, beg, pts, s_pts, s_cell, s_full, s_meta, s_pend, keys_sa, p);
+    if (p.prefilter) for (; t0 < T; t0 += 2) bin_pair<false, true, kClone>(t0, T, cnt, res_tiles, beg, pts, s_pts, s_cell, s_full, s_meta, s_pend, keys_sa, p);
+    else for (; t0 < T; t0 += 2) bin_pair<false, false, kClone>(t0, T, cnt, res_tiles, beg, pts, s_pts, s_cell, s_full, s_meta, s_pend, keys_sa, p);
   }
   __syncthreads();
   {
@@ -551,7 +555,7 @@ __device__ __forceinline__ void ground_fused_body(const GroundBatch& B, const Gr
     for (int i = tid; i < np; i += kFusedThreads) {
       const int li = s_pend[i];
       const float4 q = ((li >> 10) < res_tiles) ? s_pts[li] : __ldg(&pts[beg + li]);
-      const unsigned cc = polar_cell_exact(q.x, q.y, p);
+      const unsigned cc = polar_cell_exact<kClone>(q.x, q.y, p);
       s_cell[li] = (uint16_t)cc;
       if (cc != kNoCell) {
         float z = q.z;
@@ -742,6 +746,23 @@ ground_fused_kernel(const __grid_constant__ GroundBatch B, const __grid_constant
 __global__ void __launch_bounds__(kFusedThreads, 1)
 ground_fused_rig_kernel(const __grid_constant__ GroundBatch B, const __grid_constant__ GroundParams p, float roi) { ground_fused_body<true>(B, p, roi); }
 
+// sequence ticks with their own detection values (lmot_seq_set_detect_params): every frame's whole GroundParams and clustering ROI, the
+// sensor's four mounting values folded in on the host.  A separate parameter block, so that GroundBatch -- and with it the parameter
+// layout of the two kernels above -- stays as it was.
+struct GroundFrameParams {
+  GroundParams p[kMaxBatch];
+  float roi[kMaxBatch];
+};
+static_assert(sizeof(GroundBatch) + sizeof(GroundFrameParams) <= 4096, "ground_fused_frame_kernel: parameter block");
+
+// the same kernel with every frame's parameters from its own entry: range filter, fast path, pre-filters (phase 1), clamp, flags,
+// outlier filter and label limits (phase 2), cartesian cell (phase 3)
+__global__ void __launch_bounds__(kFusedThreads, 1)
+ground_fused_frame_kernel(const __grid_constant__ GroundBatch B, const __grid_constant__ GroundFrameParams P) {
+  const int frame = blockIdx.x / B.ctas_per_frame;
+  ground_fused_body<false, 1>(B, P.p[frame], P.roi[frame]);
+}
+
 // inspection only (lmot_debug_polar_grid): all five 80x120 grids of the reference from the min-z keys of the last launch, ten
 // channels per CTA.  (The fused kernel evaluates, per CTA, only the channels that CTA's points need, and keeps them in shared memory.)
 __global__ void __launch_bounds__(kFusedThreads)
@@ -779,10 +800,18 @@ int ground_alloc(Ctx* c, Slot* s) {
   if (c->fused_max_ctas == 0) {
     LMOT_CUDA(c, cudaFuncSetAttribute(ground_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFusedSmem));
     LMOT_CUDA(c, cudaFuncSetAttribute(ground_fused_rig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFusedSmem));
+    LMOT_CUDA(c, cudaFuncSetAttribute(ground_fused_frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFusedSmem));
     int sms = 0, per_sm = 0, coop = 0;
     LMOT_CUDA(c, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
     LMOT_CUDA(c, cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, c->device));
-    LMOT_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ground_fused_kernel, kFusedThreads, kFusedSmem));
+    // the grid barrier needs every CTA co-resident: the limit is the smallest over the three variants a launch may pick
+    const void* variants[] = {(const void*)ground_fused_kernel, (const void*)ground_fused_rig_kernel, (const void*)ground_fused_frame_kernel};
+    per_sm = INT_MAX;
+    for (const void* k : variants) {
+      int v = 0;
+      LMOT_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k, kFusedThreads, kFusedSmem));
+      if (v < per_sm) per_sm = v;
+    }
     if (!coop || per_sm < 1 || sms * per_sm < kMinCtas) { c->last_error = "device cannot run the cooperative ground kernel"; return LMOT_ERR_CUDA; }
     c->fused_max_ctas = sms * per_sm;
     if ((long long)c->fused_max_ctas * kMaxTiles * kTilePts < (long long)c->max_points) {
@@ -849,7 +878,7 @@ bool ground_reads_input_once(const Ctx* c, int n) {
 // One launch for F frames (F = 1: the frame pipeline and the stage entry points; F > 1: one frame per sensor stream, api.cu
 // lmot_batch_*).  Frame i runs on slots[i]'s buffers; its CTAs are [i * G, (i + 1) * G) of the grid and synchronise among themselves.
 int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* pts, const int* n, cudaStream_t st, bool fuse_count,
-                        bool want_labels, bool fuse_ccl, bool chain, const lmot_sensor* rig) {
+                        bool want_labels, bool fuse_ccl, bool chain, const lmot_sensor* rig, const lmot_detect_params* det) {
   if (fuse_ccl && !fuse_count) return LMOT_ERR_INVALID;
   if (F < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   int n_max = 0;
@@ -900,10 +929,17 @@ int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* 
   }
   if (rig)
     for (int i = 0; i < F; ++i) { B.mount[i][0] = rig[i].t_hmin; B.mount[i][1] = rig[i].t_hmax; B.mount[i][2] = rig[i].h_sensor; }
-  const void* kern = rig ? (const void*)ground_fused_rig_kernel : (const void*)ground_fused_kernel;
+  const void* kern = det ? (const void*)ground_fused_frame_kernel : rig ? (const void*)ground_fused_rig_kernel : (const void*)ground_fused_kernel;
   float roi = c->prm.roi_m;
   GroundParams gp = c->gp;
-  void* args[] = {(void*)&B, (void*)&gp, (void*)&roi};
+  void* args3[] = {(void*)&B, (void*)&gp, (void*)&roi};
+  GroundFrameParams FP;
+  void* args2[] = {(void*)&B, (void*)&FP};
+  if (det) {
+    memset(&FP, 0, sizeof(FP));
+    for (int i = 0; i < F; ++i) { FP.p[i] = ground_params_of(det[i], c->gp.tap); FP.roi[i] = det[i].roi_m; }
+  }
+  void** args = det ? args2 : args3;
   // every frame's chunk is laid out with the tile count of the longest one (the kernel derives its layout from its own chunk;
   // a shorter chunk just leaves the tail of the allocation unused)
   const int tiles = (chunk_max + kTilePts - 1) / kTilePts;

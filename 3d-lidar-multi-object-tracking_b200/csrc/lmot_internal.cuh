@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
+#include <cstring>
 #include <string>
 #include "../../include/lmot.h"
 
@@ -34,6 +35,39 @@ struct GroundParams {
   double tol;            // 0.25
   double tap[3];         // gaussKernel(3, 1.0) computed on the host with the host libm (gaus_blur.cpp:26-49)
 };
+
+// lmot_params' detection fields (lmot_default_detect_params)
+inline lmot_detect_params detect_params_of(const lmot_params& p) {
+  lmot_detect_params d;
+  memset(&d, 0, sizeof(d));
+  d.r_min = p.r_min; d.r_max = p.r_max; d.t_hmin = p.t_hmin; d.t_hmax = p.t_hmax; d.t_hdiff = p.t_hdiff; d.h_sensor = p.h_sensor;
+  d.ground_tolerance = p.ground_tolerance;
+  d.node_prefilter = p.node_prefilter;
+  d.filter_z_min = p.filter_z_min; d.filter_z_max = p.filter_z_max; d.filter_x_min = p.filter_x_min; d.filter_x_max = p.filter_x_max;
+  d.filter_y_min = p.filter_y_min; d.filter_y_max = p.filter_y_max;
+  d.roi_m = p.roi_m;
+  d.ram_points = p.ram_points; d.l_slope_dist = p.l_slope_dist; d.l_num_points = p.l_num_points; d.sensor_height = p.sensor_height;
+  d.t_height_min = p.t_height_min; d.t_height_max = p.t_height_max; d.t_width_min = p.t_width_min; d.t_width_max = p.t_width_max;
+  d.t_len_min = p.t_len_min; d.t_len_max = p.t_len_max; d.t_area_max = p.t_area_max; d.t_ratio_min = p.t_ratio_min;
+  d.t_ratio_max = p.t_ratio_max; d.min_len_ratio = p.min_len_ratio; d.t_pt_per_m3 = p.t_pt_per_m3;
+  d.min_cluster_points = p.min_cluster_points; d.rule_filter = p.rule_filter;
+  return d;
+}
+
+// the ground kernel's parameter block of detection values d (lmot_create for the context, the sequence launches per frame: one
+// evaluation of r_span / bin_scale for both, so equal values give equal bits).  tap: the Gaussian taps (gauss_taps, api.cu).
+inline GroundParams ground_params_of(const lmot_detect_params& d, const double tap[3]) {
+  GroundParams g;
+  memset(&g, 0, sizeof(g));
+  g.r_min = d.r_min; g.r_max = d.r_max; g.t_hmin = d.t_hmin; g.t_hmax = d.t_hmax; g.t_hdiff = d.t_hdiff; g.h_sensor = d.h_sensor;
+  { volatile float span = d.r_max - d.r_min; g.r_span = span; }      // float, as ground_removal.cpp:71 evaluates it
+  g.prefilter = d.node_prefilter ? 1 : 0;
+  g.fz0 = d.filter_z_min; g.fz1 = d.filter_z_max; g.fx0 = d.filter_x_min; g.fx1 = d.filter_x_max; g.fy0 = d.filter_y_min; g.fy1 = d.filter_y_max;
+  g.bin_scale = (float)((double)LMOT_NUM_BIN / (double)g.r_span);
+  g.tol = d.ground_tolerance;
+  for (int i = 0; i < 3; ++i) g.tap[i] = tap[i];
+  return g;
+}
 
 // one track == one UKF object of the reference (ukf.h:15-263) + its trackNumVec_ entry; x/P index 0 = merge,
 // 1 = cv, 2 = ctrv, 3 = rm.  Xsig_pred_* is transient (recomputed by every Prediction) and not stored.
@@ -288,6 +322,10 @@ struct Ctx {
   SeqMeas seq_meas[kBatchBanks][kMaxBatch];    // per-sequence measurement lists of each batch bank, allocated by lmot_seq_open
   // staging of lmot_seq_track_submit's host lists, per bank: kMaxBatch lists of max_boxes boxes, then kMaxBatch counts (lmot_seq_open)
   float* seq_stage[kBatchBanks] = {};
+  // detection parameters of the sequences (lmot_seq_set_detect_params): seq_det_on[k] false = lmot_params' values.  Read at submission;
+  // a detection tick with any of them on runs every frame through the per-frame kernel variants (ground.cu, boxfit.cu)
+  bool seq_det_on[kMaxBatch] = {};
+  lmot_detect_params seq_det[kMaxBatch] = {};
   int seq_fc_n[kMaxBatch] = {};                // lmot_seq_frame_counts: frames of sequence k in the tick collected last
   int seq_fc[kMaxBatch][kMaxBatch][4] = {};    // ... and their n_elev, n_ground, num_cluster, n_boxes (host copies: the ring slot is reused)
 
@@ -337,7 +375,10 @@ void ground_free(Slot* s);
 // one stream then run as programmatic dependents without an event between them (ground.cu, GroundChain)
 int ground_launch(Ctx* c, Slot* s, cudaStream_t st, const float4* pts, int n, bool fuse_count = false, bool want_labels = true, bool fuse_ccl = false, bool chain = false);
 // rig (nullable): sensor i's h_sensor / t_hmin / t_hmax for frame i (lmot_set_sensors); nullptr: lmot_params' values for every frame
-int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* pts, const int* n, cudaStream_t st, bool fuse_count, bool want_labels, bool fuse_ccl = false, bool chain = false, const lmot_sensor* rig = nullptr);
+// det (nullable): frame i's own detection values (sensor values already folded in; lmot_seq_set_detect_params) -> the per-frame kernel
+// variant; rig is then unused
+int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* pts, const int* n, cudaStream_t st, bool fuse_count, bool want_labels, bool fuse_ccl = false, bool chain = false, const lmot_sensor* rig = nullptr,
+                        const lmot_detect_params* det = nullptr);
 void ground_chain_forget(int device, bool device_idle);
 int ground_cells_debug(Ctx* c, Slot* s, cudaStream_t st);
 int ground_grids_debug(Ctx* c, Slot* s, cudaStream_t st);   // d_minz / d_height / d_smoothed / d_hdiff / d_hg_dbg from the last launch's keys
@@ -354,7 +395,9 @@ int boxfit_alloc_shared(Ctx* c);
 void boxfit_free(Slot* s);
 int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem = false);
 // rig (nullable): sensor i's sensor_height for frame i (box fitting) / sensor i's pose for list i (concatenation)
-int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig = nullptr);
+// det (nullable): frame i's own detection values, as ground_launch_batch's; rig is then unused
+int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig = nullptr,
+                        const lmot_detect_params* det = nullptr);
 int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int n_lists, int cap, float* d_boxes, int* d_counters,
                             const lmot_sensor* rig = nullptr);
 int boxes_concat_launch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, float* d_boxes, int* d_counters, int* d_frame_counts, int* det_sem,

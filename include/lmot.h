@@ -439,6 +439,59 @@ int lmot_get_tracker_params(const lmot_ctx* ctx, lmot_tracker_params* p);
 int lmot_seq_set_tracker_params(lmot_ctx* ctx, int k, const lmot_tracker_params* p);
 int lmot_seq_get_tracker_params(const lmot_ctx* ctx, int k, lmot_tracker_params* p);
 
+/* ---- detection parameters of one sequence: ground removal, clustering ROI and box fitting ------------------------------------------
+ * lmot_params' detection fields, as a separate struct (callers compiled against today's lmot_params keep working).  Defaults are
+ * lmot_default_params' values; citations are file:line under object_tracking/src/. */
+typedef struct lmot_detect_params {
+  /* ground removal -- groundremove/ground_removal.cpp */
+  float r_min, r_max;               /* 3.4, 120   range window, rMin / rMax :24-25 (filter :53, bin :71) */
+  float t_hmin, t_hmax;             /* -2.0, -0.4 height clamp, tHmin / tHmax :27,29 (:194-196) */
+  float t_hdiff;                    /* 0.4        hDiff threshold, tHDiff :32 */
+  float h_sensor;                   /* 2.0        clamp value above t_hmax, hSeonsor :33 (:195) */
+  double ground_tolerance;          /* 0.25       label margin above hGround, a literal at :239 */
+  /* pre-filters of the `ground` node (groundremove/main.cpp:56-89,104-112), as lmot_params.node_prefilter */
+  int node_prefilter;               /* 0 */
+  float filter_z_min, filter_z_max; /* -3.0, 1.0 */
+  float filter_x_min, filter_x_max; /* -15, 5 */
+  float filter_y_min, filter_y_max; /* -50, 50 */
+  /* clustering */
+  float roi_m;                      /* 50         roiM cluster/component_clustering.cpp:11 (and box fitting's picScale = 900/roiM,
+                                                  cluster/box_fitting.cpp:18) */
+  /* box fitting -- cluster/box_fitting.cpp */
+  int ram_points;                   /* 80         L-shape draws, ramPoints :19 (:314); 1..LMOT_MAX_RAM_POINTS */
+  int l_slope_dist;                 /* 1          lSlopeDist :20 */
+  int l_num_points;                 /* 5          lnumPoints :23 */
+  float sensor_height;              /* 2          sensorHeight :26 */
+  float t_height_min, t_height_max; /* 0.8, 2.6   tHeightMin / tHeightMax :28-29 */
+  float t_width_min, t_width_max;   /* 0.2, 3.5   tWidthMin / tWidthMax :32-33 */
+  float t_len_min, t_len_max;       /* 0.2, 14    tLenMin / tLenMax :34-35 */
+  float t_area_max;                 /* 20         tAreaMax :36 */
+  float t_ratio_min, t_ratio_max;   /* 1, 8       tRatioMin / tRatioMax :40-41 */
+  float min_len_ratio;              /* 3          minLenRatio :43 */
+  float t_pt_per_m3;                /* 8          tPtPerM3 :44 */
+  int min_cluster_points;           /* 30         a literal at :100 (`numPoints < 30`) */
+  int rule_filter;                  /* lmot_rule_filter, LMOT_RULE_INTENDED */
+} lmot_detect_params;
+/* box fitting evaluates the first LMOT_MAX_RAM_POINTS draws of the reference's mt19937_64(0) stream exactly; a Lemire redraw (odds
+ * n / 2^64 per draw) needs one draw more, and the library's table covers those too */
+#define LMOT_MAX_RAM_POINTS 1024
+/* lmot_default_detect_params(p, out): p's detection fields (p NULL: lmot_default_params' values).
+ * lmot_seq_set_detect_params(ctx, k, p): sequence k of the open set detects with p from the next submitted tick on.  Sequence k then
+ *   gives bit for bit what a separate context gives that was created with the same lmot_params except that its detection fields are p:
+ *   through lmot_frame for a sequence without a sensor table, through lmot_set_sensors(table) + lmot_batch for one with a table (the
+ *   table's four mounting values still replace h_sensor / t_hmin / t_hmax / sensor_height of p for that sensor's frames).  p == NULL:
+ *   the sequence follows lmot_params again.  lmot_seq_get_detect_params reads the values back (lmot_params' own while it follows them).
+ * Like the sensor tables and tracker parameters, the values are host state captured by value when a tick is submitted: ticks in flight
+ * keep theirs.  lmot_seq_open resets every sequence to lmot_params; lmot_seq_tracker_reset / _load keep them; tracking-only ticks
+ * (lmot_seq_track*) do not read them.  A tick in which no sequence has its own values runs exactly the kernels it always ran; a tick in
+ * which any has runs all of its frames through kernels that read each frame's values (bit-identical for sequences following lmot_params).
+ * LMOT_ERR_INVALID, every sequence unchanged: no open set or k out of range; a non-finite value; r_min < 0 or r_max <= r_min; a range
+ * window shorter than a fifth of r_max (r_max - r_min < r_max / 5: the guarded fast path of the polar cell index is only exact for
+ * wider windows, DESIGN.md §6d); roi_m <= 0; rule_filter not an lmot_rule_filter; ram_points outside [1, LMOT_MAX_RAM_POINTS]. */
+int lmot_default_detect_params(const lmot_params* p, lmot_detect_params* out);
+int lmot_seq_set_detect_params(lmot_ctx* ctx, int k, const lmot_detect_params* p);
+int lmot_seq_get_detect_params(const lmot_ctx* ctx, int k, lmot_detect_params* p);
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);
