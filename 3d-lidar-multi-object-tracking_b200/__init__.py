@@ -195,6 +195,8 @@ ABI_SYMBOLS = [
     "lmot_seq_track_submit", "lmot_seq_track_dev", "lmot_seq_track", "lmot_seq_tracker_load", "lmot_seq_tracker_set_ego",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
+    "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
+    "lmot_track_ids", "lmot_seq_track_ids",
     "lmot_detect_boxes_dev", "lmot_track_step_lists_dev", "lmot_tracker_counters_dev", "lmot_tracker_table_received",
     "lmot_origin_points", "lmot_tracker_table", "lmot_tracker_set_num_tracks", "lmot_tracker_reset", "lmot_tracker_num_tracks", "lmot_tracker_dump", "lmot_tracker_load", "lmot_tracker_get_ego", "lmot_tracker_set_ego",
     "lmot_debug_polar_grid", "lmot_debug_cell_index", "lmot_debug_label_grid", "lmot_selftest_atan2f",
@@ -616,6 +618,40 @@ class Lmot:
         p = TrackerParams()
         self._chk(self.lib.lmot_seq_get_tracker_params(self.h, int(k), C.byref(p)))
         return _tracker_params_dict(p)
+
+    # ---- track retirement and track IDs (lmot_set_track_retirement / lmot_track_ids) -------------------------------------------
+    def set_track_retirement(self, on: bool):
+        """The context's own table: end every step by removing the tracks with trackManage 0.  Applies from the next submitted step on."""
+        self._chk(self.lib.lmot_set_track_retirement(self.h, 1 if on else 0))
+
+    def get_track_retirement(self) -> bool:
+        v = C.c_int(0)
+        self._chk(self.lib.lmot_get_track_retirement(self.h, C.byref(v)))
+        return bool(v.value)
+
+    def seq_set_track_retirement(self, k: int, on: bool):
+        self._chk(self.lib.lmot_seq_set_track_retirement(self.h, int(k), 1 if on else 0))
+
+    def seq_get_track_retirement(self, k: int) -> bool:
+        v = C.c_int(0)
+        self._chk(self.lib.lmot_seq_get_track_retirement(self.h, int(k), C.byref(v)))
+        return bool(v.value)
+
+    def _ids(self, fn, *k) -> np.ndarray:
+        n = C.c_int(0)
+        fn.argtypes = [C.c_void_p] + [C.c_int] * len(k) + [C.c_void_p, C.c_int, C.POINTER(C.c_int)]
+        self._chk(fn(self.h, *k, None, 0, C.byref(n)))
+        ids = np.zeros(n.value, np.int64)
+        self._chk(fn(self.h, *k, ids.ctypes.data_as(C.c_void_p), n.value, C.byref(n)))
+        return ids
+
+    def track_ids(self) -> np.ndarray:
+        """int64 IDs of the rows of the result most recently returned for the context's own table, in the order of its outputs."""
+        return self._ids(self.lib.lmot_track_ids)
+
+    def seq_track_ids(self, k: int) -> np.ndarray:
+        """As track_ids, for sequence k of the tick most recently returned."""
+        return self._ids(self.lib.lmot_seq_track_ids, int(k))
 
     # ---- detection parameters of a sequence (lmot_seq_set_detect_params) --------------------------------------------------------
     def seq_set_detect_params(self, k: int, **fields):

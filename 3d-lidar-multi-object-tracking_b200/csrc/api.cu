@@ -281,6 +281,14 @@ int batch_submit(Ctx* c, int bank_i, Result* r, const float4* const* d_pts, cons
   return LMOT_OK;
 }
 
+// the IDs of a result being returned (lmot_track_ids): copied now, the block is reused by later submissions
+void note_ids(Tracker& t, const Result* r) {
+  const int T = r->h_hdr[HDR_N_TRACKS];
+  t.ids_n = T;
+  t.ids_rows = !r->ids;
+  if (r->ids) t.ids_last.assign(r->h_ids, r->h_ids + T);
+}
+
 int copy_track_outputs(const Result* s, lmot_track_out* out) {
   const int T = s->h_hdr[HDR_N_TRACKS], nv = s->h_hdr[HDR_N_VIS];
   if (!out) return LMOT_OK;
@@ -318,7 +326,11 @@ int collect_result(Ctx* c, Result* r, lmot_frame_out* out, Tracker* trk = nullpt
   }
   const int err = r->h_hdr[HDR_ERROR];
   const int warn = r->has_tracks ? r->h_hdr[HDR_WARN] : 0;
-  if (r->has_tracks) (trk ? trk : &c->own)->last_n_act = r->h_hdr[HDR_N_ACT];
+  if (r->has_tracks) {
+    Tracker& t = trk ? *trk : c->own;
+    t.last_n_act = r->h_hdr[HDR_N_ACT];
+    note_ids(t, r);
+  }
   if (out) {
     out->n_elevated = r->h_hdr[HDR_N_ELEV]; out->n_ground = r->h_hdr[HDR_N_GROUND];
     out->num_cluster = r->h_hdr[HDR_NUM_CLUSTER]; out->n_boxes = r->h_hdr[HDR_N_BOXES];
@@ -347,6 +359,8 @@ int result_create(Ctx* c, Result* r) {
   LMOT_CUDA(c, cudaHostAlloc(&r->h_static, (size_t)TC + 16, fl));
   LMOT_CUDA(c, cudaHostAlloc(&r->h_vis, (size_t)TC + 16, fl));
   LMOT_CUDA(c, cudaHostAlloc(&r->h_visbb, (size_t)TC * 24 * sizeof(float) + 16, fl));
+  LMOT_CUDA(c, cudaHostAlloc(&r->h_ids, ((size_t)TC + 2) * sizeof(long long), fl));
+  LMOT_CUDA(c, cudaMalloc(&r->d_ids, ((size_t)TC + 2) * sizeof(long long)));
   {   // device copy of the block, one allocation, every array 256-byte aligned with 16 bytes of slack
     auto al = [](size_t b) { return (b + 16 + 255) & ~(size_t)255; };
     const size_t sz[8] = {al(HDR_COUNT * sizeof(int)), al((size_t)MB * 96), al((size_t)TC * 12), al((size_t)TC * 16), al((size_t)TC * 4),
@@ -379,6 +393,8 @@ void result_destroy(Result* r) {
   if (r->h_static) cudaFreeHost(r->h_static);
   if (r->h_vis) cudaFreeHost(r->h_vis);
   if (r->h_visbb) cudaFreeHost(r->h_visbb);
+  if (r->h_ids) cudaFreeHost(r->h_ids);
+  if (r->d_ids) cudaFree(r->d_ids);
   if (r->d_block) cudaFree(r->d_block);
   if (r->ev_tc) cudaEventDestroy(r->ev_tc);
   if (r->ev_done) cudaEventDestroy(r->ev_done);
@@ -804,6 +820,7 @@ int lmot_track_step(lmot_ctx* ctx, const float* boxes, int m, double timestamp_u
   }
   const int err = s->res->h_hdr[HDR_ERROR];
   c->own.last_n_act = s->res->h_hdr[HDR_N_ACT];
+  note_ids(c->own, s->res);
   rc = copy_track_outputs(s->res, out);
   return err ? err : (rc ? rc : s->res->h_hdr[HDR_WARN]);
 }
@@ -1592,6 +1609,7 @@ int lmot_tracker_table_received(lmot_ctx* ctx, int n) {
   Ctx* c = &ctx->c;
   c->own.h_trk_counters[CNT_N_TRACKS] = n;
   c->own.act_valid = false;
+  c->own.ids_identity = true;
   c->own.last_trk_res = nullptr;
   return LMOT_OK;
 }
@@ -1611,6 +1629,7 @@ static int tracker_reset(Ctx* c, Tracker& t) {
   if (rc) return rc;
   t.th = TrackerHost();
   t.act_valid = false;
+  t.ids_identity = true;               // the spawn counter restarts at 0 (the retirement switch is kept)
   LMOT_CUDA(c, cudaMemsetAsync(t.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
   return LMOT_OK;
@@ -1652,6 +1671,7 @@ int lmot_tracker_set_num_tracks(lmot_ctx* ctx, int n) {
   if (rc) return rc;
   c->own.h_trk_counters[CNT_N_TRACKS] = n;
   c->own.act_valid = false;
+  c->own.ids_identity = true;
   LMOT_CUDA(c, cudaMemcpyAsync(c->own.d_trk_counters + CNT_N_TRACKS, c->own.h_trk_counters + CNT_N_TRACKS, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
   return LMOT_OK;
@@ -1725,6 +1745,7 @@ static int tracker_load(Ctx* c, Tracker& trk, const double* dumps, int n, int in
   LMOT_CUDA(c, cudaMemcpyAsync(trk.d_trk_counters + CNT_N_TRACKS, trk.h_trk_counters + CNT_N_TRACKS, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
   trk.act_valid = false;
+  trk.ids_identity = true;             // the loaded rows are numbered 0..n-1, the counter continues at n
   trk.th = TrackerHost();
   trk.th.init = init != 0; trk.th.timestamp = timestamp_us; trk.th.egoVelo = ego_velo; trk.th.egoYaw = ego_yaw;
   trk.th.egoPreYaw = ego_pre_yaw; trk.th.egoPoint[2] = ego_point_yaw;
@@ -1750,6 +1771,50 @@ int lmot_tracker_get_ego(lmot_ctx* ctx, double ego8[8]) {
   if (!ctx || !ego8) return LMOT_ERR_INVALID;
   get_ego(ctx->c.own.th, ego8);
   return LMOT_OK;
+}
+
+// ---- track retirement and track IDs
+int lmot_set_track_retirement(lmot_ctx* ctx, int on) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  ctx->c.own.retire = on != 0;
+  return LMOT_OK;
+}
+
+int lmot_get_track_retirement(const lmot_ctx* ctx, int* on) {
+  if (!ctx || !on) return LMOT_ERR_INVALID;
+  *on = ctx->c.own.retire ? 1 : 0;
+  return LMOT_OK;
+}
+
+int lmot_seq_set_track_retirement(lmot_ctx* ctx, int k, int on) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  ctx->c.seq[k].retire = on != 0;
+  return LMOT_OK;
+}
+
+int lmot_seq_get_track_retirement(const lmot_ctx* ctx, int k, int* on) {
+  if (!ctx || !on || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  *on = ctx->c.seq[k].retire ? 1 : 0;
+  return LMOT_OK;
+}
+
+static int track_ids(const Tracker& t, long long* ids, int cap, int* n) {
+  if (!n || cap < 0 || (cap > 0 && !ids)) return LMOT_ERR_INVALID;
+  if (t.ids_n < 0) return LMOT_ERR_STATE;
+  *n = t.ids_n;
+  const int m = t.ids_n < cap ? t.ids_n : cap;
+  for (int i = 0; i < m; ++i) ids[i] = t.ids_rows ? (long long)i : t.ids_last[i];
+  return LMOT_OK;
+}
+
+int lmot_track_ids(lmot_ctx* ctx, int64_t* ids, int cap, int* n) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  return track_ids(ctx->c.own, reinterpret_cast<long long*>(ids), cap, n);
+}
+
+int lmot_seq_track_ids(lmot_ctx* ctx, int k, int64_t* ids, int cap, int* n) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  return track_ids(ctx->c.seq[k], reinterpret_cast<long long*>(ids), cap, n);
 }
 
 // ---- per-sequence state (lmot_seq_*)

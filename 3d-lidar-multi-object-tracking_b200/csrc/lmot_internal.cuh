@@ -5,6 +5,7 @@
 #include <cstdio>
 #include <cstring>
 #include <string>
+#include <vector>
 #include "../../include/lmot.h"
 
 namespace lmot {
@@ -125,6 +126,10 @@ struct Result {
   bool in_flight = false;              // submitted and not yet collected / dropped
   bool has_tracks = false;             // went through the tracker (frame) or not (detect only)
   Xf2 back;                            // global_frame: global -> sensor transform of this frame, applied by publish_kernel
+  // track IDs (lmot_track_ids): written by the retire-capable TC (device) and moved to the host block by publish_ids_kernel
+  long long* d_ids = nullptr;          // [max_tracks + 2]
+  long long* h_ids = nullptr;          // [max_tracks + 2] pinned
+  bool ids = false;                    // the step wrote ID rows; false: the IDs are the row indices
   // timing (lmot_enable_timing): stage boundaries and one event after every kernel
   cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t kev[kMaxKernelEvents] = {};
@@ -229,7 +234,7 @@ struct Tracker {
   TrackerHost th;
   lmot_tracker_params prm = tracker_params_defaults();   // lmot_set_tracker_params / lmot_seq_set_tracker_params; read at submission
   bool tuned = false;                  // prm differs from the defaults: the chain runs the kernels that read it (tracker.cu)
-  TrackState* d_tracks = nullptr;      // [max_tracks] append-only table; dead tracks keep their slot
+  TrackState* d_tracks = nullptr;      // [max_tracks] append-only table, dead tracks keep their slot (without retirement)
   int* d_trk_counters = nullptr;       // [CNT_COUNT] CNT_N_TRACKS / CNT_N_VIS / CNT_ERROR of the track table
   int* h_trk_counters = nullptr;       // pinned mirror
   unsigned* d_gate = nullptr;          // [max_tracks][gate_words] chi-square gate bits per (track, box)
@@ -249,6 +254,13 @@ struct Tracker {
   bool act_valid = false;              // false after the table was written from the host: rebuilt before the next step
   Result* last_trk_res = nullptr;      // result block of the previous tracker step (its device copy seeds the next one)
   int last_n_act = 0;                  // active tracks (live or visible) in the last result the host has read: picks spawn_output_kernel's variant
+  // track retirement (lmot_set_track_retirement) and track IDs.  Read at submission (tracker.cu ret_prm)
+  bool retire = false;                 // every step ends by removing the tracks with trackNum 0 (the retire-capable TC)
+  bool ids_identity = true;            // every row's ID is its index: no retirement since the table's last reset / load / open
+  long long* d_ids = nullptr;          // [max_tracks + 1] the ID of every row, then the table's spawn counter (retire-capable TC only)
+  int ids_n = -1;                      // IDs of the result most recently returned for this table: count (-1: none yet) ...
+  bool ids_rows = true;                // ... the row indices, or
+  std::vector<long long> ids_last;     // ... these
 };
 
 // what the tracker chain of a sequence tick reads for sequence k: its measurement list, the list in the dead-reckoned global frame

@@ -31,6 +31,7 @@
 #include <cfloat>
 #include <cstdlib>
 #include <climits>
+#include <type_traits>
 #include <vector>
 #include "lmot_internal.cuh"
 #include "exact_math.cuh"
@@ -1523,7 +1524,106 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
   }
 }
 
-// TC.  The track table only ever grows (dead tracks keep their slot, like targets_), and the reference re-emits every track
+// ------------------------------------------------------------------------------------------------ TC: track retirement
+// (lmot_set_track_retirement, DESIGN.md section 6e).  The retire-capable instantiations of TC end every step with this phase: after
+// the step's outputs, before done_at_exit counts the step -- the next step's TA and publish_kernel poll that count, so neither ever
+// sees a half-compacted table.  Per table of the launch:
+//   on      the table numbers its tracks: this step's ID rows go into the result block (pre-compaction order, the order of its
+//           outputs); the spawns take the next values of the table's spawn counter;
+//   init    the table's IDs are still its row indices (no retirement since its last reset / load / open): derived from the rows;
+//   retire  remove every row with trackNum 0.  The survivors move down in place, in order: their records, packed positions (d_pos)
+//           and IDs; the active list becomes the identity over them.  A retained table has no dead rows, so TA / TB run unchanged.
+struct RetPrm { long long* ids; long long* next; long long* out_ids; int* keep; int on, init, retire; };
+
+// the default kernels: no phase at all
+struct NoRetire {
+  __device__ __forceinline__ void begin(const int*) {}
+  __device__ __forceinline__ void end(bool, TrackState*, int*, const OutPtrs&, int*, double4*) {}
+};
+
+template <int NT>
+__device__ __noinline__ void retire_phase(const RetPrm& p, int T0, TrackState* __restrict__ tracks, int* __restrict__ trk,
+                                          const int* __restrict__ track_manage, int* __restrict__ act_list, double4* __restrict__ pos) {
+  __shared__ int s_w[33];
+  __shared__ int s_carry, s_first;
+  const int tid = threadIdx.x;
+  if (tid == 0) { s_carry = 0; s_first = INT_MAX; }
+  __syncthreads();                               // (also: every record and output of this step is written)
+  const int T = trk[CNT_N_TRACKS];
+  const int n_new = T > T0 ? T - T0 : 0;
+  const long long next = p.init ? (long long)T0 : *p.next;
+  // ID rows; with retirement the stable in-place compaction of IDs and positions (a tile is read completely -- the barrier inside
+  // block_offsets -- before anything at or below its range is written) and the list of kept rows
+  for (int q0 = 0; q0 < T; q0 += NT) {
+    const int i = q0 + tid;
+    long long id = 0;
+    int keep = 0;
+    double4 ps = make_double4(0.0, 0.0, 0.0, 0.0);
+    if (i < T) {
+      id = (i >= T0) ? next + (i - T0) : (p.init ? (long long)i : p.ids[i]);
+      p.out_ids[i] = id;
+      keep = track_manage[i] != 0 ? 1 : 0;
+      ps = pos[i];
+    }
+    if (!p.retire) {                             // (uniform) the table keeps its rows: only the spawns' IDs are new
+      if (i < T && i >= T0) p.ids[i] = id;
+      continue;
+    }
+    int ex, tot;
+    block_offsets(keep, 0, s_w, ex, tot);
+    if (keep) {
+      const int d = s_carry + ex;
+      p.ids[d] = id; pos[d] = ps; p.keep[d] = i; act_list[d] = d;
+      if (d != i) atomicMin(&s_first, d);
+    }
+    __syncthreads();
+    if (tid == 0) s_carry += tot;
+    __syncthreads();
+  }
+  const int n = p.retire ? s_carry : T;
+  if (p.retire) {
+    // the records of the kept rows from the first moved one on, as one stream of words: dst word e <- src word keep[e / W] * W + e % W,
+    // src >= dst throughout, so a chunk read completely before it is written never overwrites a word a later chunk still reads
+    using Word = typename std::conditional<sizeof(TrackState) % 16 == 0, uint4, uint2>::type;
+    constexpr int W = (int)(sizeof(TrackState) / sizeof(Word)), U = 4;
+    static_assert(sizeof(TrackState) % sizeof(Word) == 0, "TrackState is a whole number of words");
+    Word* rec = reinterpret_cast<Word*>(tracks);
+    const int f = min(s_first, n);
+    const int e1 = n * W;
+    for (int base = f * W; base < e1; base += NT * U) {
+      Word v[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int e = base + u * NT + tid;
+        if (e < e1) { const int d = e / W; v[u] = rec[(size_t)p.keep[d] * W + (e - d * W)]; }
+      }
+      __syncthreads();
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int e = base + u * NT + tid;
+        if (e < e1) rec[e] = v[u];
+      }
+      __syncthreads();
+    }
+  }
+  if (tid == 0) {
+    *p.next = next + n_new;
+    if (p.retire) { trk[CNT_N_TRACKS] = n; trk[CNT_N_ACT] = n; }
+  }
+}
+
+template <int NT>
+struct Retire {
+  const RetPrm& p;
+  int T0;
+  __device__ __forceinline__ void begin(const int* trk) { T0 = trk[CNT_N_TRACKS]; }
+  // fresh: the step rebuilt the table from nothing (the reference's first-call quirk): every row is a spawn
+  __device__ __forceinline__ void end(bool fresh, TrackState* tracks, int* trk, const OutPtrs& o, int* act_list, double4* pos) {
+    if (p.on) retire_phase<NT>(p, fresh ? 0 : T0, tracks, trk, o.track_manage, act_list, pos);
+  }
+};
+
+// TC.  The track table only ever grows (dead tracks keep their slot, like targets_; retirement is the phase above), and the reference re-emits every track
 // every frame.  Everything here that walks the table does so through coalesced side arrays; everything that touches the
 // 1.6 KB TrackState records is limited to the ACTIVE tracks:
 //   * the per-track outputs of a dead track never change, so the frame's result block starts as a copy of the previous
@@ -1532,16 +1632,17 @@ __device__ __forceinline__ void tc_fast(TCFastShared<NT>& S, TrackState* __restr
 //     of every track is its state's yaw plus THIS frame's ego yaw: `pos`, a packed (x, y, yaw) per track, refreshed for the
 //     active tracks only.
 // `full` (first step after the table was written from the host): everything is rebuilt from the records.
-// P: DefTC / TunTC
-template <int NT, class TP>
+// P: DefTC / TunTC; R: NoRetire / Retire<NT>
+template <int NT, class TP, class RH = NoRetire>
 __device__ __forceinline__ void
 spawn_output_body(TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det, const float* __restrict__ boxes,
                   const float* __restrict__ boxes_pub, int* __restrict__ first_setter, int* __restrict__ imax_arr, int* __restrict__ vis_list,
                   uint8_t* __restrict__ has5_arr, int first_frame, int compat_first, double ego_yaw, int max_tracks, const OutPtrs& o,
                   const OutPtrs& prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
-                  int* __restrict__ det_sem, unsigned* __restrict__ tc_seq, const TP& P) {
+                  int* __restrict__ det_sem, unsigned* __restrict__ tc_seq, const TP& P, RH R = RH{}) {
   pdl_launch_dependents();                 // the next frame's gate kernel may become resident
   pdl_wait();                              // TB has finished
+  R.begin(trk);
   // every exit: this step's results are complete -> count it (release); publish_kernel, on its own stream, polls the count
   // instead of waiting for a stream event, so that nothing but kernels sits on the tracker stream
   struct Done { unsigned* p; __device__ ~Done() { __syncthreads(); if (threadIdx.x == 0) { __threadfence(); atomicAdd(p, 1u); } } } done_at_exit{tc_seq};
@@ -1551,6 +1652,7 @@ spawn_output_body(TrackState* __restrict__ tracks, int* __restrict__ trk, int* _
     TCFastShared<NT>& s_fast = *reinterpret_cast<TCFastShared<NT>*>(tc_dyn);
     const int M = det[CNT_N_BOXES];
     tc_fast<NT>(s_fast, tracks, trk, det, boxes, boxes_pub, first_setter, ego_yaw, max_tracks, o, prev, act_list, pos, summary, trk[CNT_N_TRACKS], trk[CNT_N_ACT], M, P);
+    R.end(false, tracks, trk, o, act_list, pos);
     return;
   }
   __shared__ int s_w[33];
@@ -1586,6 +1688,7 @@ spawn_output_body(TrackState* __restrict__ tracks, int* __restrict__ trk, int* _
     }
     for (int b = tid; b < M; b += NT) first_setter[b] = INT_MAX;
     for (int e = tid; e < M * 24; e += NT) o.boxes[e] = boxes_pub[e];
+    R.end(true, tracks, trk, o, act_list, pos);
     return;
   }
   for (int e = tid; e < M * 24; e += NT) o.boxes[e] = boxes_pub[e];     // the frame's box list travels with its results
@@ -1776,6 +1879,7 @@ spawn_output_body(TrackState* __restrict__ tracks, int* __restrict__ trk, int* _
     o.hdr[HDR_N_ACT] = s_carry2;
     det[CNT_ERROR] = 0;
   }
+  R.end(false, tracks, trk, o, act_list, pos);
 }
 
 template <int NT>
@@ -1829,6 +1933,34 @@ spawn_output_seq_tuned_kernel(const __grid_constant__ TCSeqTunedParams p) {
   spawn_output_body<NT>(q.tracks, q.trk, q.det, q.boxes, q.boxes_pub, q.first_setter, q.imax_arr, q.vis_list, q.has5_arr, q.first_frame,
                         p.b.compat_first, q.ego_yaw, p.b.max_tracks, q.o, q.prev, q.full, q.act_list, q.pos, q.summary, q.det_sem, q.tc_seq,
                         TunTC{p.tp[blockIdx.x]});
+}
+
+// track retirement / track IDs (lmot_set_track_retirement): a table that retires, or whose IDs are no longer its row indices.  On the
+// tuned parameter source (bit-identical to the defaults at the default values, DESIGN.md section 6c), so that there is one retire
+// variant per launch shape instead of two
+template <int NT>
+__global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
+spawn_output_retire_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det, const float* __restrict__ boxes,
+                           const float* __restrict__ boxes_pub, int* __restrict__ first_setter, int* __restrict__ imax_arr, int* __restrict__ vis_list,
+                           uint8_t* __restrict__ has5_arr, int first_frame, int compat_first, double ego_yaw, int max_tracks, OutPtrs o,
+                           OutPtrs prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
+                           int* __restrict__ det_sem, unsigned* __restrict__ tc_seq, const __grid_constant__ TCPrm tp,
+                           const __grid_constant__ RetPrm rp) {
+  spawn_output_body<NT>(tracks, trk, det, boxes, boxes_pub, first_setter, imax_arr, vis_list, has5_arr, first_frame, compat_first, ego_yaw,
+                        max_tracks, o, prev, full, act_list, pos, summary, det_sem, tc_seq, TunTC{tp}, Retire<NT>{rp, 0});
+}
+
+// ... a tick where some sequence retires or numbers its tracks: every sequence of it, each with its own flags (all off: no phase)
+struct TCSeqRetireParams { TCSeqTunedParams t; RetPrm rp[kMaxBatch]; };
+static_assert(sizeof(TCSeqRetireParams) <= 4096, "kernel parameter block");
+
+template <int NT>
+__global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
+spawn_output_seq_retire_kernel(const __grid_constant__ TCSeqRetireParams p) {
+  const TCSeq& q = p.t.b.s[blockIdx.x];
+  spawn_output_body<NT>(q.tracks, q.trk, q.det, q.boxes, q.boxes_pub, q.first_setter, q.imax_arr, q.vis_list, q.has5_arr, q.first_frame,
+                        p.t.b.compat_first, q.ego_yaw, p.t.b.max_tracks, q.o, q.prev, q.full, q.act_list, q.pos, q.summary, q.det_sem, q.tc_seq,
+                        TunTC{p.t.tp[blockIdx.x]}, Retire<NT>{p.rp[blockIdx.x], 0});
 }
 
 // device copy of a frame's results -> pinned, device-mapped host block.  16 bytes per thread, consecutive threads ->
@@ -1894,6 +2026,17 @@ publish_seq_kernel(const __grid_constant__ PubSeqParams p) {
   publish_body(q.d, q.h, q.tc_seq, q.want, p.spin_limit, q.back);
 }
 
+// the ID rows of results whose table numbers its tracks (retire-capable TC): launched on the publish stream right behind the publish
+// launch of the same step, which has waited for it; one CTA per result block (nullptr: the block's IDs are its row indices)
+struct PubIds { const int* hdr; const long long* d_ids; long long* h_ids; };
+struct PubIdsParams { PubIds s[kMaxBatch]; };
+
+__global__ void __launch_bounds__(kPubThreads)
+publish_ids_kernel(const __grid_constant__ PubIdsParams p) {
+  const PubIds& q = p.s[blockIdx.x];
+  if (q.d_ids) copy16(q.h_ids, q.d_ids, (size_t)q.hdr[HDR_N_TRACKS] * sizeof(long long), threadIdx.x, kPubThreads);
+}
+
 // lmot_params.global_frame: the frame's boxes (sensor frame) -> the dead-reckoned global frame the tracker works in
 // (tracking/main.cpp:142-158: pcl_ros::transformPointCloud("/global", bBoxes[i], ...)).  One CTA; also takes over posting the
 // detection semaphore from box fitting, because the tracker must not start before this list exists.
@@ -1950,6 +2093,19 @@ TAPrm ta_prm(const lmot_tracker_params& p) {
 TBPrm tb_prm(const lmot_tracker_params& p) {
   return TBPrm{p.gamma_g, p.p_g, p.p_d, p.distance_thres, p.bb_yaw_change_thres, p.second_init_v, p.lifetime_thres};
 }
+// the retire phase's flags and arrays of table t for a step into result block r; r->ids: the step writes ID rows.  A table whose IDs
+// are its row indices and that does not retire needs neither (the default kernels); after a retiring step its IDs stay the table's own
+// until reset / load / reopen.
+RetPrm ret_prm(const Ctx* c, Tracker& t, Result* r) {
+  RetPrm a{t.d_ids, t.d_ids + c->prm.max_tracks, r->d_ids, t.d_live_list, 0, 0, 0};
+  a.retire = t.retire ? 1 : 0;
+  a.on = (t.retire || !t.ids_identity) ? 1 : 0;
+  a.init = t.ids_identity ? 1 : 0;
+  r->ids = a.on != 0;
+  if (t.retire) t.ids_identity = false;
+  return a;
+}
+
 TCPrm tc_prm(const lmot_tracker_params& p) {
   TCPrm a;
   for (int i = 0; i < 5; ++i) a.p0_diag[i] = p.p0_diag[i];
@@ -1984,6 +2140,7 @@ int tracker_alloc(Ctx* c, Tracker& t) {
   LMOT_CUDA(c, cudaMemsetAsync(t.d_meas_ctr, 0, (size_t)TC * 32 * sizeof(double2), c->trk_stream));
   LMOT_CUDA(c, cudaMalloc(&t.d_tc_seq, sizeof(unsigned)));
   LMOT_CUDA(c, cudaMemsetAsync(t.d_tc_seq, 0, sizeof(unsigned), c->trk_stream));
+  LMOT_CUDA(c, cudaMalloc(&t.d_ids, ((size_t)TC + 1) * sizeof(long long)));
   t.tc_launched = 0;
   LMOT_CUDA(c, cudaMemsetAsync(t.d_pos, 0, (size_t)TC * sizeof(double4), c->trk_stream));
   t.last_trk_res = nullptr;
@@ -2003,6 +2160,10 @@ int tracker_alloc(Ctx* c, Tracker& t) {
   LMOT_CUDA(c, cudaFuncSetAttribute(imm_update_seq_tuned_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
   LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_tuned_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
   LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_tuned_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
+  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_retire_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
+  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_retire_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
+  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_retire_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
+  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_retire_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
   t.last_n_act = 0;
   return LMOT_OK;
 }
@@ -2010,6 +2171,7 @@ int tracker_alloc(Ctx* c, Tracker& t) {
 void tracker_free(Tracker& t) {
   cudaFree(t.d_tracks); cudaFree(t.d_trk_counters); cudaFree(t.d_gate); cudaFree(t.d_setter); cudaFree(t.d_first_setter);
   cudaFree(t.d_skip); cudaFree(t.d_new_num); cudaFree(t.d_live_list); cudaFree(t.d_vis_list); cudaFree(t.d_act_list); cudaFree(t.d_pos); cudaFree(t.d_summary); cudaFree(t.d_tc_seq); cudaFree(t.d_meas_n); cudaFree(t.d_meas_ctr);
+  cudaFree(t.d_ids);
   if (t.h_trk_counters) cudaFreeHost(t.h_trk_counters);
   t = Tracker();
 }
@@ -2166,7 +2328,12 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
     cfg.gridDim = dim3(1); cfg.blockDim = dim3(wide ? kTCWide : kTCThreads); cfg.stream = st;
     cfg.dynamicSmemBytes = wide ? sizeof(TCFastShared<kTCWide>) : sizeof(TCFastShared<kTCThreads>);
     cfg.attrs = &pdl; cfg.numAttrs = 1;
-    if (tuned)
+    const RetPrm rp = ret_prm(c, c->own, r);
+    if (rp.on)
+      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_retire_kernel<kTCWide> : spawn_output_retire_kernel<kTCThreads>, c->own.d_tracks, c->own.d_trk_counters, det, d_boxes, d_boxes_pub, c->own.d_first_setter, c->own.d_new_num,
+                                      c->own.d_vis_list, c->own.d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->own.d_act_list,
+                                      c->own.d_pos, reinterpret_cast<const ActSummary*>(c->own.d_summary), det_sem, c->own.d_tc_seq, tc_prm(c->own.prm), rp));
+    else if (tuned)
       LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_tuned_kernel<kTCWide> : spawn_output_tuned_kernel<kTCThreads>, c->own.d_tracks, c->own.d_trk_counters, det, d_boxes, d_boxes_pub, c->own.d_first_setter, c->own.d_new_num,
                                       c->own.d_vis_list, c->own.d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->own.d_act_list,
                                       c->own.d_pos, reinterpret_cast<const ActSummary*>(c->own.d_summary), det_sem, c->own.d_tc_seq, tc_prm(c->own.prm)));
@@ -2189,6 +2356,11 @@ int tracker_publish(Ctx* c, Result* r, cudaStream_t st) {
   OutPtrs d{r->d_targets, r->d_vandyaw, r->d_manage, r->d_static, r->d_vis, r->d_visbb, r->d_hdr, r->d_boxes};
   OutPtrs h{r->h_targets, r->h_vandyaw, r->h_manage, r->h_static, r->h_vis, r->h_visbb, r->h_hdr, r->h_boxes};
   publish_kernel<<<1, kPubThreads, 0, st>>>(d, h, c->own.d_tc_seq, c->own.tc_launched, c->spin_limit, r->back);
+  if (r->ids) {
+    PubIdsParams p{};
+    p.s[0] = PubIds{r->d_hdr, r->d_ids, r->h_ids};
+    publish_ids_kernel<<<1, kPubThreads, 0, st>>>(p);
+  }
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
 }
@@ -2228,7 +2400,10 @@ int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const dou
   GateSeq g{};
   TASeqTunedParams tat{};      // (the parameter blocks of the kernels that read the tables' values: the blocks below + a slice per sequence)
   TBSeqTunedParams tbt{};
-  TCSeqTunedParams tct{};
+  TCSeqRetireParams tcr{};    // (the retire-capable TC: the tuned block + a phase per sequence)
+  TCSeqTunedParams& tct = tcr.t;
+  PubIdsParams pids{};
+  bool retire = false;         // some table of the set retires or numbers its tracks: every sequence of the tick runs the retire-capable TC
   TASeqParams& ta = tat.b;
   TBSeqParams& tb = tbt.b;
   TCSeqParams& tcp = tct.b;
@@ -2271,6 +2446,8 @@ int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const dou
                      t.d_act_list, t.d_pos, sum, s.d_det_sem, t.d_tc_seq, o, po, t.th.egoPoint[2], first, full};
     tat.tp[k] = ta_prm(t.prm); tbt.tp[k] = tb_prm(t.prm); tct.tp[k] = tc_prm(t.prm);
     tuned |= t.tuned;
+    tcr.rp[k] = ret_prm(c, t, r);
+    if (tcr.rp[k].on) { retire = true; pids.s[k] = PubIds{r->d_hdr, r->d_ids, r->h_ids}; }
     ++t.tc_launched;
     OutPtrs h{r->h_targets, r->h_vandyaw, r->h_manage, r->h_static, r->h_vis, r->h_visbb, r->h_hdr, r->h_boxes};
     pub.s[k] = PubSeq{o, h, t.d_tc_seq, t.tc_launched, r->back};
@@ -2301,9 +2478,11 @@ int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const dou
   const bool wide = c->tc_force >= 0 ? c->tc_force != 0 : c->seq_wide;
   cfg.gridDim = dim3(S); cfg.blockDim = dim3(wide ? kTCWide : kTCThreads);
   cfg.dynamicSmemBytes = wide ? sizeof(TCFastShared<kTCWide>) : sizeof(TCFastShared<kTCThreads>);
-  if (tuned) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_tuned_kernel<kTCWide> : spawn_output_seq_tuned_kernel<kTCThreads>, tct));
+  if (retire) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_retire_kernel<kTCWide> : spawn_output_seq_retire_kernel<kTCThreads>, tcr));
+  else if (tuned) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_tuned_kernel<kTCWide> : spawn_output_seq_tuned_kernel<kTCThreads>, tct));
   else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_kernel<kTCWide> : spawn_output_seq_kernel<kTCThreads>, tcp));
   publish_seq_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(pub);
+  if (retire) publish_ids_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(pids);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
 }

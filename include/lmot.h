@@ -46,10 +46,13 @@ typedef enum lmot_status {
   LMOT_ERR_CAPACITY = -3,  /* input exceeds a capacity fixed at lmot_create (points, clusters, boxes, tracks) */
   LMOT_ERR_STATE = -4,     /* call sequence error (e.g. fetch before run) */
   /* positive = warning: the call did its work and every output is valid */
-  LMOT_WARN_TRACK_TABLE_FULL = 1   /* max_tracks tracks exist (dead ones keep their slot, like the reference's targets_): boxes no track
-                                      matched spawn no new track this frame; existing tracks are updated and reported as usual.  At the
-                                      default 8192 and ~3 spawns per frame that is ~4.5 min of a 10 Hz stream; size max_tracks for the
-                                      session (1.6 KB of device memory per track) or call lmot_tracker_reset between sequences. */
+  LMOT_WARN_TRACK_TABLE_FULL = 1   /* the step's rows -- the rows the table held at its start plus this step's spawns -- would exceed
+                                      max_tracks: boxes no track matched beyond that spawn no new track this frame; existing tracks are
+                                      updated and reported as usual.  Without track retirement dead tracks keep their row (like the
+                                      reference's targets_), so the table fills: at the default 8192 and ~3 spawns per frame that is
+                                      ~4.5 min of a 10 Hz stream.  Turn retirement on (lmot_set_track_retirement: the table then holds
+                                      the live tracks only), size max_tracks for the session (1.6 KB of device memory per track) or call
+                                      lmot_tracker_reset between sequences. */
 } lmot_status;
 
 /* ruleBasedFilter (box_fitting.cpp:97-158) falls off its end without a return when a nested size check fails:
@@ -88,7 +91,8 @@ typedef struct lmot_params {
   int max_points;            /* per frame, default 1<<20 */
   int max_clusters;          /* default 4096 (a 250x250 grid with 3x3 dilation cannot hold more) */
   int max_boxes;             /* default 1024 */
-  int max_tracks;            /* tracks ever created (dead ones keep their slot), default 8192 */
+  int max_tracks;            /* rows of a track table: tracks ever created (dead ones keep their slot), or with track retirement
+                                the live tracks plus one step's spawns; default 8192 */
   /* pre-filters of the reference's `ground` ROS node, applied BEFORE groundRemove (src/groundremove/main.cpp:56-89,104-112):
    * pcl::PassThrough on z (limits inclusive, non-finite points removed) then pcl::ConditionalRemoval x in (x_min,x_max) AND
    * y in (y_min,y_max) (strict).  Off by default: the hot path is groundRemove itself.  Fused into the first load. */
@@ -310,7 +314,7 @@ int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n);   /*
  *
  * lmot_seq_open(ctx, n_seq, ring): drains the context and replaces the set with n_seq (1..LMOT_MAX_BATCH) empty sequences, each at
  *   its first frame, and a ring of `ring` (1..64) ticks.  n_seq = 0 frees the set.  Memory: n_seq track tables (device, max_tracks x
- *   ~2.6 KB incl. side arrays at max_boxes 1024) plus ring x n_seq result blocks (each max_boxes x 96 B + max_tracks x 130 B of pinned host memory and
+ *   ~2.6 KB incl. side arrays at max_boxes 1024) plus ring x n_seq result blocks (each max_boxes x 96 B + max_tracks x 138 B of pinned host memory and
  *   the same again on the device), per sequence 2 x 2 x max_boxes x 96 B of device memory (a measurement list and its global-frame
  *   copy for each of the two detection banks), and 2 x 8 x max_boxes x 96 B of device memory (~1.5 MB at max_boxes 1024) staging the
  *   host lists of lmot_seq_track_submit -- size max_tracks and ring for it.  Reopening (or closing) also clears every sequence's sensor table.
@@ -438,6 +442,41 @@ int lmot_set_tracker_params(lmot_ctx* ctx, const lmot_tracker_params* p);
 int lmot_get_tracker_params(const lmot_ctx* ctx, lmot_tracker_params* p);
 int lmot_seq_set_tracker_params(lmot_ctx* ctx, int k, const lmot_tracker_params* p);
 int lmot_seq_get_tracker_params(const lmot_ctx* ctx, int k, lmot_tracker_params* p);
+
+/* ---- track retirement and track IDs: track a stream indefinitely ---------------------------------------------------------------------
+ * By default a track table is append-only like the reference's targets_ / trackNumVec_: a dead track (trackManage 0) keeps its row and
+ * is reported in every later frame, so a long stream fills max_tracks (LMOT_WARN_TRACK_TABLE_FULL) and every step costs more.
+ * With retirement on, every step of the table ends by removing each track whose trackManage is 0; the remaining rows keep their
+ * relative order and the next step's spawns are appended after them.  The results equal the reference with one extra operation after
+ * every immUkfJpdaf: stably erase every i with trackNumVec_[i] == 0 from targets_ and trackNumVec_ (the ego state is not touched) --
+ * the same trackManage, lifetime, static and visible flags, box and vis_bb rows bit for bit, UKF states to 1e-4 relative.
+ *   Outputs: step f lists every row present during step f -- the rows retained after step f-1, then this step's spawns.  A track that
+ *   dies in step f appears once with trackManage 0 (possibly visible) and is gone from step f+1.  lmot_tracker_num_tracks and
+ *   lmot_tracker_dump (and the sequence forms) describe the retained table; the result's n_tracks is the number of its rows.
+ *   max_tracks bounds the rows a step holds: the retained rows plus that step's spawns.
+ *   The one deviation from the unbounded reference: mergeOverSegmentation (imm_ukf_jpda.cpp:682-695) tests every track, dead ones
+ *   included, so there a visible box that contains the frozen position of a long-dead track promotes that visible track to 5.  Once
+ *   the dead track is erased, that promotion does not happen.  Nothing else of the reference reads dead rows.
+ * Track IDs.  Once rows move, a row index no longer names a track.  Every track has an int64 ID: the table's spawn counter at its
+ *   spawn, 0, 1, 2, ... from the table's last reset / open / load (lmot_tracker_load numbers the loaded rows 0..n-1 and continues at n).
+ *   A table that never retired has IDs equal to its row indices.
+ * lmot_set_track_retirement(ctx, on) / lmot_get_track_retirement: the context's own table; lmot_seq_set_track_retirement(ctx, k, on) /
+ *   lmot_seq_get_track_retirement: sequence k of the open set.  Off by default.  Host state captured by value when a step or tick is
+ *   submitted, like the tracker parameters: steps in flight keep the setting they were submitted with.  lmot_seq_open turns it off for
+ *   every sequence; lmot_tracker_reset / _load and lmot_seq_tracker_reset / _load keep it (and return the IDs to the row indices).
+ *   A table that retired and is then switched off keeps numbering its tracks (its IDs stay right) until reset, load or reopen.
+ * lmot_track_ids(ctx, ids, cap, n): the IDs of the rows of the result most recently returned for the context's own table (lmot_track_step,
+ *   lmot_frame, lmot_frame_collect / _fetch, lmot_batch, lmot_batch_collect / _fetch, lmot_track_step_lists_dev), in the order of its
+ *   outputs; *n = their number, min(*n, cap) are copied.  lmot_seq_track_ids(ctx, k, ...): sequence k of the tick most recently returned
+ *   by lmot_seq_collect / lmot_seq_fetch / lmot_seq / lmot_seq_track.
+ * LMOT_ERR_INVALID: k out of range, no open set, a null pointer (ids may be NULL when cap is 0).  LMOT_ERR_STATE: no result yet.
+ * Not supported: retirement on a context driven by lmot_shared_tick_dev of liblmot_shared.so -- its receiving ranks hold no IDs. */
+int lmot_set_track_retirement(lmot_ctx* ctx, int on);
+int lmot_get_track_retirement(const lmot_ctx* ctx, int* on);
+int lmot_seq_set_track_retirement(lmot_ctx* ctx, int k, int on);
+int lmot_seq_get_track_retirement(const lmot_ctx* ctx, int k, int* on);
+int lmot_track_ids(lmot_ctx* ctx, int64_t* ids, int cap, int* n);
+int lmot_seq_track_ids(lmot_ctx* ctx, int k, int64_t* ids, int cap, int* n);
 
 /* ---- detection parameters of one sequence: ground removal, clustering ROI and box fitting ------------------------------------------
  * lmot_params' detection fields, as a separate struct (callers compiled against today's lmot_params keep working).  Defaults are

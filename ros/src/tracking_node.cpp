@@ -11,6 +11,10 @@
 // Timestamp: the reference node passes header.stamp.toSec() -- SECONDS -- to a tracker that divides by 1e6 (imm_ukf_jpda.cpp:807),
 // i.e. the deployed reference runs with dt ~ 1e-7 s.  Default here = the same (drop-in for what is deployed); the private parameter
 // ~stamp_in_microseconds:=true feeds the physically meaningful value instead.
+// Track table: like the reference, dead tracks keep their row by default, so the table (kCap rows) fills after a few minutes of
+// driving and new objects are no longer tracked.  ~retire_dead_tracks:=true turns track retirement on (lmot_set_track_retirement):
+// dead tracks are removed after every step, the node can run indefinitely, and the arrow markers take their ids from the stable
+// track IDs (lmot_track_ids) instead of the row index.
 // Needs ROS (catkin) and the package's generated message headers.
 #include <ros/ros.h>
 #include <nav_msgs/Odometry.h>
@@ -28,11 +32,13 @@ lmot_ctx* g_ctx = nullptr;
 ros::Publisher g_pub_markers, g_pub_boxes;
 double g_v_gps = 0.0, g_yaw_gps = 0.0;
 bool g_stamp_us = false;
+bool g_retire = false;
 constexpr int kCap = 8192;
 std::vector<float> g_boxes, g_targets((size_t)kCap * 3), g_visbb((size_t)kCap * 24);
 std::vector<double> g_vy((size_t)kCap * 2);
 std::vector<int32_t> g_manage(kCap);
 std::vector<uint8_t> g_static(kCap), g_vis(kCap);
+std::vector<int64_t> g_ids(kCap);
 
 void on_odom(const nav_msgs::Odometry& odom) {
   const auto& t = odom.twist.twist.linear;
@@ -69,13 +75,15 @@ void on_boxes(const object_tracking::trackbox& in) {
   const int rc = lmot_track_step(g_ctx, g_boxes.data(), m, stamp, g_v_gps, g_yaw_gps, &o);
   if (rc < 0) { ROS_ERROR_THROTTLE(1.0, "lmot_track_step: %s (%s)", lmot_strerror(rc), lmot_last_error(g_ctx)); return; }
   if (rc > 0) ROS_WARN_THROTTLE(10.0, "lmot_track_step: %s", lmot_strerror(rc));      // e.g. track table full: outputs are valid, keep publishing
+  int n_ids = 0;
+  if (g_retire) lmot_track_ids(g_ctx, g_ids.data(), kCap, &n_ids);      // row i -> its track's ID (rows move once dead tracks are removed)
 
   // arrows: moving, visible, live tracks (speed = length, yaw = direction)
   for (int i = 0; i < o.n_tracks; ++i) {
     if (g_manage[i] == 0 || !g_vis[i] || g_static[i]) continue;
     visualization_msgs::Marker a;
     a.header.frame_id = "/velodyne"; a.header.stamp = ros::Time::now();
-    a.ns = "arrows"; a.id = i; a.type = visualization_msgs::Marker::ARROW; a.action = visualization_msgs::Marker::ADD;
+    a.ns = "arrows"; a.id = (g_retire && i < n_ids) ? (int)(g_ids[i] % 2147483647) : i; a.type = visualization_msgs::Marker::ARROW; a.action = visualization_msgs::Marker::ADD;
     a.lifetime = ros::Duration(0.1);
     a.pose.position.x = g_targets[3 * i]; a.pose.position.y = g_targets[3 * i + 1]; a.pose.position.z = -1.73 / 2;
     a.pose.orientation = tf::createQuaternionMsgFromYaw(g_vy[2 * i + 1]);
@@ -113,8 +121,10 @@ int main(int argc, char** argv) {
   int device = 0;
   nh.param<int>("cuda_device", device, 0);
   ros::NodeHandle("~").param<bool>("stamp_in_microseconds", g_stamp_us, false);
+  ros::NodeHandle("~").param<bool>("retire_dead_tracks", g_retire, false);      // false: the reference's append-only table (drop-in)
   const int rc = lmot_create(&g_ctx, &prm, device);
   if (rc != LMOT_OK) { ROS_FATAL("lmot_create: %s -- this node has no CPU path", lmot_strerror(rc)); return 1; }
+  if (g_retire) lmot_set_track_retirement(g_ctx, 1);
   g_pub_markers = nh.advertise<visualization_msgs::Marker>("visualization_marker", 0);
   g_pub_boxes = nh.advertise<visualization_msgs::Marker>("visualization_marker2", 0);
   ros::Subscriber sub_boxes = nh.subscribe("track_box", 160, on_boxes);

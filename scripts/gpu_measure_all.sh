@@ -14,5 +14,6 @@ timeout 600 python scripts/seq_rig_measure.py > measure_out/${T}_seq_rig.txt 2>&
 timeout 600 python scripts/seq_track_measure.py > measure_out/${T}_seq_track.txt 2>&1; tail -11 measure_out/${T}_seq_track.txt
 timeout 600 python scripts/tracker_params_measure.py > measure_out/${T}_tracker_params.txt 2>&1; tail -9 measure_out/${T}_tracker_params.txt
 timeout 600 python scripts/seq_detect_params_measure.py > measure_out/${T}_seq_detect_params.txt 2>&1; tail -6 measure_out/${T}_seq_detect_params.txt
+timeout 900 python scripts/retire_measure.py > measure_out/${T}_retire.txt 2>&1; tail -30 measure_out/${T}_retire.txt
 timeout 300 python scripts/diag_timeline.py ${T}_timeline > measure_out/${T}_timeline.txt 2>&1; tail -5 measure_out/${T}_timeline.txt
 ls -la measure_out/${T}*
