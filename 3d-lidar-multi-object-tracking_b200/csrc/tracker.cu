@@ -26,6 +26,13 @@
 // G -> TA -> TB -> TC are programmatic dependent launches of one another (griddepcontrol); in steady state the tracker
 // stream carries nothing else (DESIGN.md section 6).
 //
+// Each stage has one kernel per family, all from the stage's one body; chain_launch picks the family for a step of 1..8 tables:
+//   the kernels above        the context's own table at the default parameters, not numbering its tracks (lmot_frame*, lmot_batch*,
+//                            lmot_track_step*, lmot_shared_*);
+//   *_seq_kernel             a sequence tick whose tables are all of that kind: one table per blockIdx.y (TA, TB) / blockIdx.x (TC);
+//   *_seq_tuned_kernel       every other step, the own table's included (S = 1): each table's own parameters (DESIGN.md section 6c),
+//                            and a TC whose track-retirement phase is on for each table that numbers its tracks (section 6e).
+//
 // All state is fp64 like the reference (Eigen::MatrixXd); this file is compiled with -fmad=false so that the
 // operation sequence matches the x86-64 build of the reference except for libm (sin/cos/exp/pow/atan2 <= 2 ulp).
 #include <cfloat>
@@ -612,16 +619,6 @@ imm_predict_gate_kernel(TrackState* __restrict__ tracks, const int* __restrict__
   imm_predict_gate_body(tracks, trk, det, boxes, dt, gate, setter, first_setter, skip, words, act_list, meas_n, meas_ctr, tc_seq, tc_want, spin_limit, DefTA{});
 }
 
-// a table with its own parameters (lmot_set_tracker_params)
-__global__ void __launch_bounds__(kTAThreads, 4)
-imm_predict_gate_tuned_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
-                              double dt, unsigned* __restrict__ gate, unsigned* __restrict__ setter, int* __restrict__ first_setter,
-                              uint8_t* __restrict__ skip, int words, const int* __restrict__ act_list,
-                              int* __restrict__ meas_n, double2* __restrict__ meas_ctr,
-                              const unsigned* __restrict__ tc_seq, unsigned tc_want, unsigned spin_limit, const __grid_constant__ TAPrm tp) {
-  imm_predict_gate_body(tracks, trk, det, boxes, dt, gate, setter, first_setter, skip, words, act_list, meas_n, meas_ctr, tc_seq, tc_want, spin_limit, TunTA{tp});
-}
-
 // Sequence ticks: one launch steps every sequence's table, sequence = blockIdx.y.  `run` = 0: the sequence is on its compat first
 // frame, where the single-stream path launches neither TA nor TB (its CTAs leave at once; TC spawns the quirk's track).
 struct TASeq {
@@ -642,7 +639,8 @@ imm_predict_gate_seq_kernel(const __grid_constant__ TASeqParams p) {
                         q.meas_ctr, q.tc_seq, q.tc_want, p.spin_limit, DefTA{});
 }
 
-// ... a tick where some table has its own parameters: every sequence of it, each with its own slice
+// ... every other chain (a table with its own parameters, or one that numbers its tracks; the context's own table too, S = 1): every
+// table of it, each with its own slice
 __global__ void __launch_bounds__(kTAThreads, 4)
 imm_predict_gate_seq_tuned_kernel(const __grid_constant__ TASeqTunedParams p) {
   const TASeq& q = p.b.s[blockIdx.y];
@@ -1096,15 +1094,6 @@ imm_update_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, 
   imm_update_body(tracks, trk, det, boxes, gate, first_setter, skip, words, act_list, summary, meas_n, meas_ctr, DefTB{});
 }
 
-// a table with its own parameters (lmot_set_tracker_params)
-__global__ void __launch_bounds__(kTBThreads)
-imm_update_tuned_kernel(TrackState* __restrict__ tracks, const int* __restrict__ trk, const int* __restrict__ det, const float* __restrict__ boxes,
-                        const unsigned* __restrict__ gate, const int* __restrict__ first_setter, const uint8_t* __restrict__ skip,
-                        int words, const int* __restrict__ act_list, ActSummary* __restrict__ summary,
-                        const int* __restrict__ meas_n, const double2* __restrict__ meas_ctr, const __grid_constant__ TBPrm tp) {
-  imm_update_body(tracks, trk, det, boxes, gate, first_setter, skip, words, act_list, summary, meas_n, meas_ctr, TunTB{tp});
-}
-
 // sequence ticks: sequence = blockIdx.y, `run` as for TA
 struct TBSeq {
   TrackState* tracks; const int* trk; const int* det; const float* boxes; const unsigned* gate; const int* first_setter;
@@ -1122,7 +1111,7 @@ imm_update_seq_kernel(const __grid_constant__ TBSeqParams p) {
   imm_update_body(q.tracks, q.trk, q.det, q.boxes, q.gate, q.first_setter, q.skip, p.words, q.act_list, q.summary, q.meas_n, q.meas_ctr, DefTB{});
 }
 
-// ... a tick where some table has its own parameters: every sequence of it, each with its own slice
+// ... every other chain (as imm_predict_gate_seq_tuned_kernel's)
 __global__ void __launch_bounds__(kTBThreads)
 imm_update_seq_tuned_kernel(const __grid_constant__ TBSeqTunedParams p) {
   const TBSeq& q = p.b.s[blockIdx.y];
@@ -1160,7 +1149,7 @@ __device__ __forceinline__ bool overseg_cond(const float* c, const float* ab, do
 constexpr int kTCThreads = 256;      // ONE small CTA: 16 K registers, so it starts on any SM next to the resident detection kernels
                                      // instead of waiting for a whole SM to drain (a 1024-thread CTA needs the full register file)
 constexpr int kTCWide = 512;         // the same kernel for scenes with 257..512 active tracks (multi-sensor ticks, dense traffic): the
-                                     // fast path holds one active track per thread (tracker_launch picks the variant from the last
+                                     // fast path holds one active track per thread (chain_launch picks the variant from the last
                                      // active-track count the host has seen; either variant is correct for any count)
 constexpr int kVisChunk = 128;       // visible boxes staged in shared memory per pass
 constexpr int kCandCap = 1024;       // (box, track) pairs that pass the bounds pre-test, per pass (more: tested inline)
@@ -1893,18 +1882,6 @@ spawn_output_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int*
                         max_tracks, o, prev, full, act_list, pos, summary, det_sem, tc_seq, DefTC{});
 }
 
-// a table with its own parameters (lmot_set_tracker_params)
-template <int NT>
-__global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
-spawn_output_tuned_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det, const float* __restrict__ boxes,
-                          const float* __restrict__ boxes_pub, int* __restrict__ first_setter, int* __restrict__ imax_arr, int* __restrict__ vis_list,
-                          uint8_t* __restrict__ has5_arr, int first_frame, int compat_first, double ego_yaw, int max_tracks, OutPtrs o,
-                          OutPtrs prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
-                          int* __restrict__ det_sem, unsigned* __restrict__ tc_seq, const __grid_constant__ TCPrm tp) {
-  spawn_output_body<NT>(tracks, trk, det, boxes, boxes_pub, first_setter, imax_arr, vis_list, has5_arr, first_frame, compat_first, ego_yaw,
-                        max_tracks, o, prev, full, act_list, pos, summary, det_sem, tc_seq, TunTC{tp});
-}
-
 // sequence ticks: one CTA per sequence (blockIdx.x); each picks the fast or the general path from its own sequence's counts
 struct TCSeq {
   TrackState* tracks; int* trk; int* det; const float* boxes; const float* boxes_pub; int* first_setter; int* imax_arr; int* vis_list;
@@ -1914,8 +1891,6 @@ struct TCSeq {
 };
 struct TCSeqParams { TCSeq s[kMaxBatch]; int compat_first, max_tracks; };
 static_assert(sizeof(TCSeqParams) <= 4096, "kernel parameter block");
-struct TCSeqTunedParams { TCSeqParams b; TCPrm tp[kMaxBatch]; };
-static_assert(sizeof(TCSeqTunedParams) <= 4096, "kernel parameter block");
 
 template <int NT>
 __global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
@@ -1925,38 +1900,17 @@ spawn_output_seq_kernel(const __grid_constant__ TCSeqParams p) {
                         p.compat_first, q.ego_yaw, p.max_tracks, q.o, q.prev, q.full, q.act_list, q.pos, q.summary, q.det_sem, q.tc_seq, DefTC{});
 }
 
-// ... a tick where some table has its own parameters: every sequence of it, each with its own slice
+// ... every other chain (as imm_predict_gate_seq_tuned_kernel's): each table with its own slice, and the retire-capable TC (track
+// retirement / track IDs, lmot_set_track_retirement) with each table's own flags -- all off: no phase.  One TC on the tuned parameter
+// source (bit-identical to the defaults at the default values, DESIGN.md section 6c) instead of a tuned and a retire variant.
+// (the _seq block + a parameter slice per table, then a retire phase per table)
+struct TCSeqPrmParams { TCSeqParams b; TCPrm tp[kMaxBatch]; };
+struct TCSeqTunedParams { TCSeqPrmParams t; RetPrm rp[kMaxBatch]; };
+static_assert(sizeof(TCSeqTunedParams) <= 4096, "kernel parameter block");
+
 template <int NT>
 __global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
 spawn_output_seq_tuned_kernel(const __grid_constant__ TCSeqTunedParams p) {
-  const TCSeq& q = p.b.s[blockIdx.x];
-  spawn_output_body<NT>(q.tracks, q.trk, q.det, q.boxes, q.boxes_pub, q.first_setter, q.imax_arr, q.vis_list, q.has5_arr, q.first_frame,
-                        p.b.compat_first, q.ego_yaw, p.b.max_tracks, q.o, q.prev, q.full, q.act_list, q.pos, q.summary, q.det_sem, q.tc_seq,
-                        TunTC{p.tp[blockIdx.x]});
-}
-
-// track retirement / track IDs (lmot_set_track_retirement): a table that retires, or whose IDs are no longer its row indices.  On the
-// tuned parameter source (bit-identical to the defaults at the default values, DESIGN.md section 6c), so that there is one retire
-// variant per launch shape instead of two
-template <int NT>
-__global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
-spawn_output_retire_kernel(TrackState* __restrict__ tracks, int* __restrict__ trk, int* __restrict__ det, const float* __restrict__ boxes,
-                           const float* __restrict__ boxes_pub, int* __restrict__ first_setter, int* __restrict__ imax_arr, int* __restrict__ vis_list,
-                           uint8_t* __restrict__ has5_arr, int first_frame, int compat_first, double ego_yaw, int max_tracks, OutPtrs o,
-                           OutPtrs prev, int full, int* __restrict__ act_list, double4* __restrict__ pos, const ActSummary* __restrict__ summary,
-                           int* __restrict__ det_sem, unsigned* __restrict__ tc_seq, const __grid_constant__ TCPrm tp,
-                           const __grid_constant__ RetPrm rp) {
-  spawn_output_body<NT>(tracks, trk, det, boxes, boxes_pub, first_setter, imax_arr, vis_list, has5_arr, first_frame, compat_first, ego_yaw,
-                        max_tracks, o, prev, full, act_list, pos, summary, det_sem, tc_seq, TunTC{tp}, Retire<NT>{rp, 0});
-}
-
-// ... a tick where some sequence retires or numbers its tracks: every sequence of it, each with its own flags (all off: no phase)
-struct TCSeqRetireParams { TCSeqTunedParams t; RetPrm rp[kMaxBatch]; };
-static_assert(sizeof(TCSeqRetireParams) <= 4096, "kernel parameter block");
-
-template <int NT>
-__global__ void __launch_bounds__(NT, NT == kTCThreads ? 2 : 1)
-spawn_output_seq_retire_kernel(const __grid_constant__ TCSeqRetireParams p) {
   const TCSeq& q = p.t.b.s[blockIdx.x];
   spawn_output_body<NT>(q.tracks, q.trk, q.det, q.boxes, q.boxes_pub, q.first_setter, q.imax_arr, q.vis_list, q.has5_arr, q.first_frame,
                         p.t.b.compat_first, q.ego_yaw, p.t.b.max_tracks, q.o, q.prev, q.full, q.act_list, q.pos, q.summary, q.det_sem, q.tc_seq,
@@ -2154,16 +2108,9 @@ int tracker_alloc(Ctx* c, Tracker& t) {
   LMOT_CUDA(c, cudaFuncSetAttribute(imm_update_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
   LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
   LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
-  LMOT_CUDA(c, cudaFuncSetAttribute(imm_update_tuned_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
-  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_tuned_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
-  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_tuned_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
   LMOT_CUDA(c, cudaFuncSetAttribute(imm_update_seq_tuned_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
   LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_tuned_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
   LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_tuned_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
-  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_retire_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
-  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_retire_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
-  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_retire_kernel<kTCThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCThreads>)));
-  LMOT_CUDA(c, cudaFuncSetAttribute(spawn_output_seq_retire_kernel<kTCWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TCFastShared<kTCWide>)));
   t.last_n_act = 0;
   return LMOT_OK;
 }
@@ -2240,115 +2187,154 @@ int boxes_to_global_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_box
   return LMOT_OK;
 }
 
+// ---------------------------------------------------------------------------------------------- the tracker chain
+// One step of 1 <= S <= 8 track tables: gate -> TA -> TB -> TC, as programmatic dependent launches on one stream.  The context's own
+// table (tracker_launch) and the tables of a sequence tick (seq_tracker_launch) are prepared by chain_prepare and launched by
+// chain_launch, which picks the kernel family (see the head of this file).
+namespace {
+
+// table k's slice of every parameter block (the default kernels take their arguments from slice 0); the _seq kernels take the
+// `.b` blocks (`tc.t.b`), the _seq_tuned kernels the whole blocks
+struct Chain {
+  int S = 0;
+  GateSeq g{};
+  TASeqTunedParams ta{};
+  TBSeqTunedParams tb{};
+  TCSeqTunedParams tc{};
+  PubSeqParams pub{};
+  PubIdsParams ids{};
+  bool tuned = false;          // some table has its own values ...
+  bool ids_on = false;         // ... or numbers its tracks (RetPrm::on): the chain runs the _seq_tuned kernels
+  int n_act_max = 0;           // the largest last_n_act of the tables: TC's width
+  explicit Chain(const Ctx* c) {
+    ta.b.words = tb.b.words = c->gate_words;
+    ta.b.spin_limit = pub.spin_limit = c->spin_limit;
+    tc.t.b.compat_first = c->prm.oracle_compat_first_frame ? 1 : 0;
+    tc.t.b.max_tracks = c->prm.max_tracks;
+  }
+};
+
+// table t's step on measurement list m (box list, counters, semaphore: nullptr for an ungated step) into result block r at the ego pose
+// (ts, v, yaw) -> slot ch.S of the blocks.  Advances the table's host state; a table written from the host since its last step gets its
+// active list rebuilt on `st` first.
+int chain_prepare(Ctx* c, Tracker& t, const SeqMeas& m, Result* r, cudaStream_t st, double ts, double v, double yaw, Chain& ch) {
+  const int k = ch.S++;
+  const int first = t.th.init ? 0 : 1;
+  const double dt = first ? 0.0 : (ts - t.th.timestamp) / 1000000.0;     // :807, from this table's own previous stamp
+  origin_points_fold(t.th, ts, v, yaw);
+  // global_frame: the tracker reads the list boxes_to_global_launch / seq_global_launch prepared, the results carry the sensor-frame list
+  const bool gf = c->prm.global_frame != 0;
+  if (gf) { Xf2 fwd; global_frame_xf(t.th.egoPoint, &fwd, &r->back); }
+  else r->back.on = 0;
+  const float* boxes = gf ? m.d_boxes_g : m.d_boxes;
+  const int full = t.act_valid ? 0 : 1;   // the table was written from the host since its last step: rebuild the side arrays
+  if (full) {
+    LMOT_CUDA(c, cudaMemsetAsync(t.d_trk_counters + CNT_N_ACT, 0, sizeof(int), st));
+    build_active_kernel<<<(c->prm.max_tracks + 255) / 256, 256, 0, st>>>(t.d_tracks, t.d_trk_counters, t.d_act_list);
+    t.act_valid = true;
+  }
+  Result* pr = (full || !t.last_trk_res) ? r : t.last_trk_res;
+  t.last_trk_res = r;
+  const int run = (first && ch.tc.t.b.compat_first) ? 0 : 1;
+  ActSummary* sum = reinterpret_cast<ActSummary*>(t.d_summary);
+  double2* mc = reinterpret_cast<double2*>(t.d_meas_ctr);
+  ch.g.sem[k] = m.d_det_sem;
+  ch.ta.b.s[k] = TASeq{t.d_tracks, t.d_trk_counters, m.d_counters, boxes, dt, t.d_gate, t.d_setter, t.d_first_setter, t.d_skip, t.d_act_list,
+                       t.d_meas_n, mc, t.d_tc_seq, t.tc_launched, run};
+  ch.tb.b.s[k] = TBSeq{t.d_tracks, t.d_trk_counters, m.d_counters, boxes, t.d_gate, t.d_first_setter, t.d_skip, t.d_act_list, sum, t.d_meas_n, mc, run};
+  OutPtrs o{r->d_targets, r->d_vandyaw, r->d_manage, r->d_static, r->d_vis, r->d_visbb, r->d_hdr, r->d_boxes};
+  OutPtrs po{pr->d_targets, pr->d_vandyaw, pr->d_manage, pr->d_static, pr->d_vis, pr->d_visbb, pr->d_hdr, pr->d_boxes};
+  ch.tc.t.b.s[k] = TCSeq{t.d_tracks, t.d_trk_counters, m.d_counters, boxes, m.d_boxes, t.d_first_setter, t.d_new_num, t.d_vis_list, t.d_skip,
+                       t.d_act_list, t.d_pos, sum, m.d_det_sem, t.d_tc_seq, o, po, t.th.egoPoint[2], first, full};
+  ch.ta.tp[k] = ta_prm(t.prm); ch.tb.tp[k] = tb_prm(t.prm); ch.tc.t.tp[k] = tc_prm(t.prm);
+  ch.tuned |= t.tuned;
+  ch.tc.rp[k] = ret_prm(c, t, r);
+  if (ch.tc.rp[k].on) { ch.ids_on = true; ch.ids.s[k] = PubIds{r->d_hdr, r->d_ids, r->h_ids}; }
+  ++t.tc_launched;
+  OutPtrs h{r->h_targets, r->h_vandyaw, r->h_manage, r->h_static, r->h_vis, r->h_visbb, r->h_hdr, r->h_boxes};
+  ch.pub.s[k] = PubSeq{o, h, t.d_tc_seq, t.tc_launched, r->back};
+  if (t.last_n_act > ch.n_act_max) ch.n_act_max = t.last_n_act;
+  t.th.timestamp = ts;
+  t.th.egoPreYaw = t.th.egoYaw;
+  t.th.init = true;
+  return LMOT_OK;
+}
+
+enum class ChainGate { none, one, seq };   // tracker_gate_kernel on the one semaphore of slice 0, tracker_gate_seq_kernel on all S
+
+// launches the prepared chain on `st`.  own: the context's own table (the single-table default kernels where the family is the
+// default one; `tc_wide` holds TC's width) or a sequence tick (`seq_wide`).  gate: how the chain waits for its measurement lists on the
+// device (none: the caller ordered the stream, or nothing to wait for); TA follows a gate kernel as its programmatic dependent.
+// pdl: TB and TC as programmatic dependents (timing mode records an event between the kernels, which needs the ordinary full
+// serialisation).  mark: the slot whose kernel_marks to record (nullptr: none).  ta_tb: false on the own table's compat first frame,
+// where TC alone runs, fully serialised.
+int chain_launch(Ctx* c, Chain& ch, cudaStream_t st, bool own, ChainGate gate, bool pdl, Slot* mark, bool ta_tb) {
+  const int S = ch.S;
+  const bool def = !ch.tuned && !ch.ids_on;
+  cudaLaunchAttribute pa;
+  pa.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  cudaLaunchConfig_t cfg = {};
+  cfg.stream = st; cfg.attrs = &pa; cfg.numAttrs = 1;
+  if (ta_tb) {
+    pa.val.programmaticStreamSerializationAllowed = gate != ChainGate::none ? 1 : 0;
+    cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); cfg.dynamicSmemBytes = 0;
+    if (gate == ChainGate::one) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, tracker_gate_kernel, (const int*)ch.g.sem[0], c->spin_limit));
+    if (gate == ChainGate::seq) { ch.g.n = S; LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, tracker_gate_seq_kernel, ch.g, c->spin_limit)); }
+    // the single-stream chain's CTA count, shared by the tables (grid-stride over each table's active tracks)
+    cfg.gridDim = dim3((c->trk_ctas + S - 1) / S, S); cfg.blockDim = dim3(kTAThreads);
+    const TASeq& a = ch.ta.b.s[0];
+    if (own && def)
+      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_predict_gate_kernel, a.tracks, a.trk, a.det, a.boxes, a.dt, a.gate, a.setter, a.first_setter, a.skip,
+                                      ch.ta.b.words, a.act_list, a.meas_n, a.meas_ctr, a.tc_seq, a.tc_want, ch.ta.b.spin_limit));
+    else if (def) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_predict_gate_seq_kernel, ch.ta.b));
+    else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_predict_gate_seq_tuned_kernel, ch.ta));
+    if (mark) kernel_mark(c, mark, st);
+    pa.val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
+    cfg.blockDim = dim3(kTBThreads); cfg.dynamicSmemBytes = (size_t)c->gate_words * 32 * sizeof(unsigned short);
+    const TBSeq& b = ch.tb.b.s[0];
+    if (own && def)
+      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_kernel, b.tracks, b.trk, b.det, b.boxes, b.gate, b.first_setter, b.skip, ch.tb.b.words,
+                                      b.act_list, b.summary, b.meas_n, b.meas_ctr));
+    else if (def) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_seq_kernel, ch.tb.b));
+    else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_seq_tuned_kernel, ch.tb));
+    if (mark) kernel_mark(c, mark, st);
+  }
+  pa.val.programmaticStreamSerializationAllowed = (pdl && ta_tb) ? 1 : 0;
+  // TC's width: one active track per thread on the fast path.  The host only knows the active count of the last result it has read
+  // (a few frames old inside the pipeline; the count moves by a handful per frame): switch early, with hysteresis.  A count above the
+  // width runs the kernel's general path -- slower, same results.
+  bool& wide_now = own ? c->tc_wide : c->seq_wide;
+  if (ch.n_act_max > 208) wide_now = true;
+  else if (ch.n_act_max < 144) wide_now = false;
+  const bool wide = c->tc_force >= 0 ? c->tc_force != 0 : wide_now;
+  cfg.gridDim = dim3(S); cfg.blockDim = dim3(wide ? kTCWide : kTCThreads);
+  cfg.dynamicSmemBytes = wide ? sizeof(TCFastShared<kTCWide>) : sizeof(TCFastShared<kTCThreads>);
+  const TCSeq& q = ch.tc.t.b.s[0];
+  if (own && def)
+    LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_kernel<kTCWide> : spawn_output_kernel<kTCThreads>, q.tracks, q.trk, q.det, q.boxes,
+                                    q.boxes_pub, q.first_setter, q.imax_arr, q.vis_list, q.has5_arr, q.first_frame, ch.tc.t.b.compat_first, q.ego_yaw,
+                                    ch.tc.t.b.max_tracks, q.o, q.prev, q.full, q.act_list, q.pos, q.summary, q.det_sem, q.tc_seq));
+  else if (def) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_kernel<kTCWide> : spawn_output_seq_kernel<kTCThreads>, ch.tc.t.b));
+  else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_tuned_kernel<kTCWide> : spawn_output_seq_tuned_kernel<kTCThreads>, ch.tc));
+  if (mark) kernel_mark(c, mark, st);
+  LMOT_CUDA(c, cudaGetLastError());
+  return LMOT_OK;
+}
+
+}  // namespace
+
 int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, const int* det_counters, double timestamp, double v_gps,
                    double yaw_gps, bool gate, bool* gated) {
-  origin_points_fold(c->own.th, timestamp, v_gps, yaw_gps);
-  // global_frame: the tracker reads the list boxes_to_global_launch prepared, the results carry the sensor-frame list
-  const float* d_boxes_pub = d_boxes;
-  if (c->prm.global_frame) { d_boxes = sl->d_boxes_g; Xf2 fwd; global_frame_xf(c->own.th.egoPoint, &fwd, &sl->res->back); }
-  else sl->res->back.on = 0;
-  TrackerHost& h = c->own.th;
-  Result* r = sl->res;
-  OutPtrs o{r->d_targets, r->d_vandyaw, r->d_manage, r->d_static, r->d_vis, r->d_visbb, r->d_hdr, r->d_boxes};
-  int* det = const_cast<int*>(det_counters);
-  const int first = h.init ? 0 : 1;
-  const int compat = c->prm.oracle_compat_first_frame ? 1 : 0;
+  const bool compat_first = !c->own.th.init && c->prm.oracle_compat_first_frame;   // the reference's first-frame quirk: TC alone
   // `gate` (frame submissions): the detection stages of this frame post sl->d_det_sem.  Either the gate kernel waits for it on
   // the device (see tracker_gate_kernel), or -- timing mode, the reference's first-frame quirk -- the stream waits for the event.
-  const bool use_gate = gate && !c->timing && !(first && compat);
+  const bool use_gate = gate && !c->timing && !compat_first;
   if (gate && !use_gate) LMOT_CUDA(c, cudaStreamWaitEvent(st, sl->ev_det_done, 0));
-  int* det_sem = gate ? sl->d_det_sem : nullptr;
   if (gated) *gated = use_gate;
-  const int full = c->own.act_valid ? 0 : 1;   // the table was written from the host since the last frame: rebuild the side arrays
-  const bool tuned = c->own.tuned;             // lmot_set_tracker_params: the kernels that read the table's values (copied into the launches)
-  if (full) {
-    LMOT_CUDA(c, cudaMemsetAsync(c->own.d_trk_counters + CNT_N_ACT, 0, sizeof(int), st));
-    build_active_kernel<<<(c->prm.max_tracks + 255) / 256, 256, 0, st>>>(c->own.d_tracks, c->own.d_trk_counters, c->own.d_act_list);
-    c->own.act_valid = true;
-  }
-  Result* pr = (full || !c->own.last_trk_res) ? r : c->own.last_trk_res;
-  OutPtrs po{pr->d_targets, pr->d_vandyaw, pr->d_manage, pr->d_static, pr->d_vis, pr->d_visbb, pr->d_hdr, pr->d_boxes};
-  c->own.last_trk_res = r;
-  if (!(first && compat)) {
-    const double dt = first ? 0.0 : (timestamp - h.timestamp) / 1000000.0;     // :807
-    const size_t sh = (size_t)c->gate_words * 32 * sizeof(unsigned short);
-    {
-      cudaLaunchAttribute pa;
-      pa.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      pa.val.programmaticStreamSerializationAllowed = use_gate ? 1 : 0;
-      if (use_gate) {
-        cudaLaunchConfig_t gc = {};
-        gc.gridDim = dim3(1); gc.blockDim = dim3(32); gc.dynamicSmemBytes = 0; gc.stream = st; gc.attrs = &pa; gc.numAttrs = 1;
-        LMOT_CUDA(c, cudaLaunchKernelEx(&gc, tracker_gate_kernel, (const int*)det_sem, c->spin_limit));
-      }
-      cudaLaunchConfig_t ac = {};
-      ac.gridDim = dim3(c->trk_ctas); ac.blockDim = dim3(kTAThreads); ac.dynamicSmemBytes = 0; ac.stream = st; ac.attrs = &pa; ac.numAttrs = 1;
-      if (tuned)
-        LMOT_CUDA(c, cudaLaunchKernelEx(&ac, imm_predict_gate_tuned_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes, dt,
-                                        c->own.d_gate, c->own.d_setter, c->own.d_first_setter, c->own.d_skip, c->gate_words, (const int*)c->own.d_act_list,
-                                        c->own.d_meas_n, reinterpret_cast<double2*>(c->own.d_meas_ctr), (const unsigned*)c->own.d_tc_seq, c->own.tc_launched, c->spin_limit,
-                                        ta_prm(c->own.prm)));
-      else
-        LMOT_CUDA(c, cudaLaunchKernelEx(&ac, imm_predict_gate_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes, dt,
-                                        c->own.d_gate, c->own.d_setter, c->own.d_first_setter, c->own.d_skip, c->gate_words, (const int*)c->own.d_act_list,
-                                        c->own.d_meas_n, reinterpret_cast<double2*>(c->own.d_meas_ctr), (const unsigned*)c->own.d_tc_seq, c->own.tc_launched, c->spin_limit));
-    }
-    kernel_mark(c, sl, st);
-    // TB and TC: programmatic dependent launches (their CTAs wait on the device for the preceding grid, see pdl_wait); timing
-    // mode records an event between the kernels, which needs the ordinary full serialisation
-    cudaLaunchAttribute pdl;
-    pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    pdl.val.programmaticStreamSerializationAllowed = c->timing ? 0 : 1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(c->trk_ctas); cfg.blockDim = dim3(kTBThreads); cfg.dynamicSmemBytes = sh; cfg.stream = st;
-    cfg.attrs = &pdl; cfg.numAttrs = 1;
-    if (tuned)
-      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_tuned_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes,
-                                      (const unsigned*)c->own.d_gate, (const int*)c->own.d_first_setter, (const uint8_t*)c->own.d_skip, c->gate_words,
-                                      (const int*)c->own.d_act_list, reinterpret_cast<ActSummary*>(c->own.d_summary),
-                                      (const int*)c->own.d_meas_n, reinterpret_cast<const double2*>(c->own.d_meas_ctr), tb_prm(c->own.prm)));
-    else
-      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_kernel, c->own.d_tracks, (const int*)c->own.d_trk_counters, (const int*)det, d_boxes,
-                                      (const unsigned*)c->own.d_gate, (const int*)c->own.d_first_setter, (const uint8_t*)c->own.d_skip, c->gate_words,
-                                      (const int*)c->own.d_act_list, reinterpret_cast<ActSummary*>(c->own.d_summary),
-                                      (const int*)c->own.d_meas_n, reinterpret_cast<const double2*>(c->own.d_meas_ctr)));
-    kernel_mark(c, sl, st);
-  }
-  {
-    cudaLaunchAttribute pdl;
-    pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    pdl.val.programmaticStreamSerializationAllowed = (c->timing || (first && compat)) ? 0 : 1;
-    // variant: one active track per thread on the fast path.  The host only knows the active count of the last result it has read
-    // (a few frames old inside the pipeline; the count moves by a handful per frame): switch early, with hysteresis.  A count above
-    // the variant's width runs the kernel's general path -- slower, same results.
-    if (c->own.last_n_act > 208) c->tc_wide = true;
-    else if (c->own.last_n_act < 144) c->tc_wide = false;
-    const bool wide = c->tc_force >= 0 ? c->tc_force != 0 : c->tc_wide;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(1); cfg.blockDim = dim3(wide ? kTCWide : kTCThreads); cfg.stream = st;
-    cfg.dynamicSmemBytes = wide ? sizeof(TCFastShared<kTCWide>) : sizeof(TCFastShared<kTCThreads>);
-    cfg.attrs = &pdl; cfg.numAttrs = 1;
-    const RetPrm rp = ret_prm(c, c->own, r);
-    if (rp.on)
-      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_retire_kernel<kTCWide> : spawn_output_retire_kernel<kTCThreads>, c->own.d_tracks, c->own.d_trk_counters, det, d_boxes, d_boxes_pub, c->own.d_first_setter, c->own.d_new_num,
-                                      c->own.d_vis_list, c->own.d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->own.d_act_list,
-                                      c->own.d_pos, reinterpret_cast<const ActSummary*>(c->own.d_summary), det_sem, c->own.d_tc_seq, tc_prm(c->own.prm), rp));
-    else if (tuned)
-      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_tuned_kernel<kTCWide> : spawn_output_tuned_kernel<kTCThreads>, c->own.d_tracks, c->own.d_trk_counters, det, d_boxes, d_boxes_pub, c->own.d_first_setter, c->own.d_new_num,
-                                      c->own.d_vis_list, c->own.d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->own.d_act_list,
-                                      c->own.d_pos, reinterpret_cast<const ActSummary*>(c->own.d_summary), det_sem, c->own.d_tc_seq, tc_prm(c->own.prm)));
-    else
-      LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_kernel<kTCWide> : spawn_output_kernel<kTCThreads>, c->own.d_tracks, c->own.d_trk_counters, det, d_boxes, d_boxes_pub, c->own.d_first_setter, c->own.d_new_num,
-                                      c->own.d_vis_list, c->own.d_skip, first, compat, h.egoPoint[2], c->prm.max_tracks, o, po, full, c->own.d_act_list,
-                                      c->own.d_pos, reinterpret_cast<const ActSummary*>(c->own.d_summary), det_sem, c->own.d_tc_seq));
-    ++c->own.tc_launched;
-  }
-  kernel_mark(c, sl, st);
-  LMOT_CUDA(c, cudaGetLastError());
-  h.timestamp = timestamp;
-  h.egoPreYaw = h.egoYaw;
-  h.init = true;
-  return LMOT_OK;
+  Chain ch(c);
+  const SeqMeas m{const_cast<float*>(d_boxes), sl->d_boxes_g, const_cast<int*>(det_counters), gate ? sl->d_det_sem : nullptr};
+  if (int rc = chain_prepare(c, c->own, m, sl->res, st, timestamp, v_gps, yaw_gps, ch)) return rc;
+  return chain_launch(c, ch, st, true, use_gate ? ChainGate::one : ChainGate::none, !c->timing, sl, !compat_first);
 }
 
 // device block of `r` -> its pinned host block (asynchronous on st)
@@ -2391,98 +2377,15 @@ int seq_global_launch(Ctx* c, const SeqMeas* m, int S, cudaStream_t st, const do
   return LMOT_OK;
 }
 
-// gate -> TA -> TB -> TC once for all S sequences on the tracker stream (programmatic dependent launches, as the single-stream
-// chain), then one publish launch on the publish stream.  The caller records the tick's events on the publish stream afterwards.
+// gate -> TA -> TB -> TC once for all S sequences on the tracker stream (chain_launch), then one publish launch on the publish stream.
+// The caller records the tick's events on the publish stream afterwards.
 int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw) {
-  cudaStream_t st = c->trk_stream;
-  const int compat = c->prm.oracle_compat_first_frame ? 1 : 0;
-  const bool gf = c->prm.global_frame != 0;
-  GateSeq g{};
-  TASeqTunedParams tat{};      // (the parameter blocks of the kernels that read the tables' values: the blocks below + a slice per sequence)
-  TBSeqTunedParams tbt{};
-  TCSeqRetireParams tcr{};    // (the retire-capable TC: the tuned block + a phase per sequence)
-  TCSeqTunedParams& tct = tcr.t;
-  PubIdsParams pids{};
-  bool retire = false;         // some table of the set retires or numbers its tracks: every sequence of the tick runs the retire-capable TC
-  TASeqParams& ta = tat.b;
-  TBSeqParams& tb = tbt.b;
-  TCSeqParams& tcp = tct.b;
-  PubSeqParams pub{};
-  bool tuned = false;          // some table of the set has its own values: every sequence of the tick runs those kernels
-  g.n = S;
-  ta.words = c->gate_words; ta.spin_limit = c->spin_limit;
-  tb.words = c->gate_words;
-  tcp.compat_first = compat; tcp.max_tracks = c->prm.max_tracks;
-  pub.spin_limit = c->spin_limit;
-  int n_act_max = 0;
-  for (int k = 0; k < S; ++k) {
-    Tracker& t = c->seq[k];
-    const SeqMeas& s = m[k];
-    Result* r = &tick->blocks[k];
-    const int first = t.th.init ? 0 : 1;
-    const double dt = first ? 0.0 : (ts[k] - t.th.timestamp) / 1000000.0;     // :807, from this sequence's own previous stamp
-    origin_points_fold(t.th, ts[k], v[k], yaw[k]);
-    if (gf) { Xf2 fwd; global_frame_xf(t.th.egoPoint, &fwd, &r->back); }
-    else r->back.on = 0;
-    const float* boxes = gf ? s.d_boxes_g : s.d_boxes;
-    const int full = t.act_valid ? 0 : 1;
-    if (full) {
-      LMOT_CUDA(c, cudaMemsetAsync(t.d_trk_counters + CNT_N_ACT, 0, sizeof(int), st));
-      build_active_kernel<<<(c->prm.max_tracks + 255) / 256, 256, 0, st>>>(t.d_tracks, t.d_trk_counters, t.d_act_list);
-      t.act_valid = true;
-    }
-    Result* pr = (full || !t.last_trk_res) ? r : t.last_trk_res;
-    t.last_trk_res = r;
-    const int run = (first && compat) ? 0 : 1;
-    ActSummary* sum = reinterpret_cast<ActSummary*>(t.d_summary);
-    double2* mc = reinterpret_cast<double2*>(t.d_meas_ctr);
-    g.sem[k] = s.d_det_sem;
-    ta.s[k] = TASeq{t.d_tracks, t.d_trk_counters, s.d_counters, boxes, dt, t.d_gate, t.d_setter, t.d_first_setter, t.d_skip, t.d_act_list,
-                    t.d_meas_n, mc, t.d_tc_seq, t.tc_launched, run};
-    tb.s[k] = TBSeq{t.d_tracks, t.d_trk_counters, s.d_counters, boxes, t.d_gate, t.d_first_setter, t.d_skip, t.d_act_list, sum, t.d_meas_n, mc, run};
-    OutPtrs o{r->d_targets, r->d_vandyaw, r->d_manage, r->d_static, r->d_vis, r->d_visbb, r->d_hdr, r->d_boxes};
-    OutPtrs po{pr->d_targets, pr->d_vandyaw, pr->d_manage, pr->d_static, pr->d_vis, pr->d_visbb, pr->d_hdr, pr->d_boxes};
-    tcp.s[k] = TCSeq{t.d_tracks, t.d_trk_counters, s.d_counters, boxes, s.d_boxes, t.d_first_setter, t.d_new_num, t.d_vis_list, t.d_skip,
-                     t.d_act_list, t.d_pos, sum, s.d_det_sem, t.d_tc_seq, o, po, t.th.egoPoint[2], first, full};
-    tat.tp[k] = ta_prm(t.prm); tbt.tp[k] = tb_prm(t.prm); tct.tp[k] = tc_prm(t.prm);
-    tuned |= t.tuned;
-    tcr.rp[k] = ret_prm(c, t, r);
-    if (tcr.rp[k].on) { retire = true; pids.s[k] = PubIds{r->d_hdr, r->d_ids, r->h_ids}; }
-    ++t.tc_launched;
-    OutPtrs h{r->h_targets, r->h_vandyaw, r->h_manage, r->h_static, r->h_vis, r->h_visbb, r->h_hdr, r->h_boxes};
-    pub.s[k] = PubSeq{o, h, t.d_tc_seq, t.tc_launched, r->back};
-    if (t.last_n_act > n_act_max) n_act_max = t.last_n_act;
-    t.th.timestamp = ts[k];
-    t.th.egoPreYaw = t.th.egoYaw;
-    t.th.init = true;
-  }
-  cudaLaunchAttribute pdl;
-  pdl.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  pdl.val.programmaticStreamSerializationAllowed = 1;
-  cudaLaunchConfig_t cfg = {};
-  cfg.stream = st; cfg.attrs = &pdl; cfg.numAttrs = 1;
-  cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); cfg.dynamicSmemBytes = 0;
-  LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, tracker_gate_seq_kernel, g, c->spin_limit));
-  // the single-stream chain's CTA count, shared by the sequences (grid-stride over each sequence's active tracks)
-  const int gx = (c->trk_ctas + S - 1) / S;
-  cfg.gridDim = dim3(gx, S); cfg.blockDim = dim3(kTAThreads); cfg.dynamicSmemBytes = 0;
-  if (tuned) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_predict_gate_seq_tuned_kernel, tat));
-  else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_predict_gate_seq_kernel, ta));
-  cfg.gridDim = dim3(gx, S); cfg.blockDim = dim3(kTBThreads); cfg.dynamicSmemBytes = (size_t)c->gate_words * 32 * sizeof(unsigned short);
-  if (tuned) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_seq_tuned_kernel, tbt));
-  else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, imm_update_seq_kernel, tb));
-  // spawn_output_kernel's variant for the whole launch from the largest active count of the set (hysteresis as tracker_launch);
-  // either variant is correct for any count
-  if (n_act_max > 208) c->seq_wide = true;
-  else if (n_act_max < 144) c->seq_wide = false;
-  const bool wide = c->tc_force >= 0 ? c->tc_force != 0 : c->seq_wide;
-  cfg.gridDim = dim3(S); cfg.blockDim = dim3(wide ? kTCWide : kTCThreads);
-  cfg.dynamicSmemBytes = wide ? sizeof(TCFastShared<kTCWide>) : sizeof(TCFastShared<kTCThreads>);
-  if (retire) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_retire_kernel<kTCWide> : spawn_output_seq_retire_kernel<kTCThreads>, tcr));
-  else if (tuned) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_tuned_kernel<kTCWide> : spawn_output_seq_tuned_kernel<kTCThreads>, tct));
-  else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, wide ? spawn_output_seq_kernel<kTCWide> : spawn_output_seq_kernel<kTCThreads>, tcp));
-  publish_seq_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(pub);
-  if (retire) publish_ids_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(pids);
+  Chain ch(c);
+  for (int k = 0; k < S; ++k)
+    if (int rc = chain_prepare(c, c->seq[k], m[k], &tick->blocks[k], c->trk_stream, ts[k], v[k], yaw[k], ch)) return rc;
+  if (int rc = chain_launch(c, ch, c->trk_stream, false, ChainGate::seq, true, nullptr, true)) return rc;
+  publish_seq_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(ch.pub);
+  if (ch.ids_on) publish_ids_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(ch.ids);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
 }

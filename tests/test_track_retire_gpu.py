@@ -133,10 +133,10 @@ print(json.dumps(names))
 
 
 # ------------------------------------------------------------------------------------------------ 1. off is today's path
-def test_off_is_todays_path(pkg):
-    """Catches a context that never called the API, or switched retirement off, running the retire-capable TC or the ID publication
-    (kernel names through torch.profiler, in a process of its own), outputs that differ from such a context, and IDs that are not the
-    row indices."""
+def test_off_runs_the_default_kernels(pkg):
+    """Catches a context that never called the API, or switched retirement off, running the tuned kernels, the retire-capable TC or the
+    ID publication (kernel names through torch.profiler, in a process of its own), outputs that differ from such a context, and IDs
+    that are not the row indices.  A retiring context runs the sequence family's TC at S = 1 and publishes its IDs."""
     import json
     import subprocess
     here = os.path.dirname(os.path.abspath(__file__))
@@ -145,8 +145,8 @@ def test_off_is_todays_path(pkg):
     names = json.loads(r.stdout.strip().splitlines()[-1])
     print(names)
     for arm in ("never", "off"):
-        assert names[arm] and not any("retire" in n or "publish_ids" in n for n in names[arm]), (arm, names[arm])
-    assert any("spawn_output_retire" in n for n in names["on"]) and any("publish_ids" in n for n in names["on"]), names["on"]
+        assert names[arm] and not any("tuned" in n or "retire" in n or "publish_ids" in n for n in names[arm]), (arm, names[arm])
+    assert any("spawn_output_seq_tuned" in n for n in names["on"]) and any("publish_ids" in n for n in names["on"]), names["on"]
     a, b = pkg.Lmot(_params(pkg)), pkg.Lmot(_params(pkg))
     try:
         b.set_track_retirement(False)
@@ -497,7 +497,41 @@ def test_switching_in_flight_reset_load_reopen(pkg):
         a.close(); b.close()
 
 
-# ------------------------------------------------------------------------------------------------ 7. validation
+# ------------------------------------------------------------------------------------------------ 7. timing mode
+@pytest.mark.parametrize("gf", [0, 1])
+def test_timing_mode_kernel_times(pkg, gf):
+    """Catches a tuned or retiring table whose tracker chain marks a different set of kernels in timing mode (lmot_enable_timing: TA, TB
+    and TC each followed by an event, launched without programmatic dependence) than a table at the defaults, and timing mode changing a
+    result.  lmot_track_step over 30 frames of the bench scene with a moving ego, compat first frame included: a default, a tuned (every
+    association at 99 m also happens at 1e9 m) and a retiring context, timed, each against an untimed twin with the same settings."""
+    scene = bench_scene(30)
+    arms = ("default", "tuned", "retire")
+    ctx = {}
+    try:
+        for arm in arms:
+            for timed in (True, False):
+                c = _ctx(pkg, retire=arm == "retire", gf=gf)
+                if arm == "tuned":
+                    c.set_tracker_params(distance_thres=1e9)
+                c.enable_timing(timed)
+                ctx[arm, timed] = c
+        for f, (ts, boxes, v, y) in enumerate(scene):
+            out, n_times = {}, {}
+            for arm in arms:
+                out[arm] = ctx[arm, True].track_step(boxes, ts, v, y)
+                n_times[arm] = len(ctx[arm, True].last_kernel_ms())
+                _same_outputs(out[arm], ctx[arm, False].track_step(boxes, ts, v, y), (arm, f))
+                assert np.array_equal(ctx[arm, True].track_ids(), ctx[arm, False].track_ids()), (arm, f)
+            _same_outputs(out["tuned"], out["default"], ("tuned vs default", f))
+            assert n_times["default"] > 0 and n_times["tuned"] == n_times["default"] == n_times["retire"], (f, n_times)
+        for arm in arms:
+            assert np.array_equal(_bits(ctx[arm, True].tracker_dump()), _bits(ctx[arm, False].tracker_dump())), arm
+    finally:
+        for c in ctx.values():
+            c.close()
+
+
+# ------------------------------------------------------------------------------------------------ 8. validation
 def test_validation(pkg):
     """Catches a missing argument check of the new calls."""
     c = pkg.Lmot(_params(pkg))

@@ -203,7 +203,7 @@ REGIME_SET = dict(ALL_MOVED, static_lifetime=4, static_dist=6.0)     # slow latt
 
 
 @pytest.mark.parametrize("n_tracks", [400, 700])
-def test_tuned_regimes(pkg, ref_tunable, n_tracks):
+def test_tuned_regimes_on_sequence_tc(pkg, ref_tunable, n_tracks):
     """Catches a TC path or width that still uses the literals.  Free-running from a reset over 14 frames of a slowly moving lattice:
     a compat first frame (ukf_initialize's p0_diag and mode_prob0), then more than 256 active tracks (400: the 512-thread fast path,
     emit_values) or more than 512 (700: the general path, emit_track), where every track turns static (static_lifetime /
@@ -237,7 +237,7 @@ def test_tuned_regimes(pkg, ref_tunable, n_tracks):
         print(n_tracks, "tracks: TC kernels", sorted({n.split("(")[0] for n in names if "spawn_output" in n}),
               "static at the end:", int(b["is_static"].sum()))
         assert names, "the profiler recorded none of the tracker's kernels"
-        assert any("spawn_output_tuned_kernel<512>" in n for n in names), names
+        assert any("spawn_output_seq_tuned_kernel<512>" in n for n in names), names
         _teacher_forced(lm, ref_tunable, seq[:8], ("lattice, teacher-forced", n_tracks))
     finally:
         ref_tunable.set_tracker_params(None)
