@@ -178,6 +178,27 @@ class FrameOut(C.Structure):
     ]
 
 
+MAX_PRED_TIMES = 32                    # LMOT_MAX_PRED_TIMES
+PRED_VALID, PRED_DEAD, PRED_GUARD_P, PRED_GUARD_S = 1, 2, 4, 8
+PRED_FIELDS = (("x", 5), ("P", 25), ("mode_prob", 3), ("gate_z", 2), ("gate_S", 4))   # per (time, row), float64
+
+
+class PredOut(C.Structure):
+    _fields_ = [("cap", C.c_int), ("n_rows", C.c_int), ("ids", C.c_void_p), ("track_manage", C.c_void_p), ("flags", C.c_void_p),
+                ("x", C.c_void_p), ("P", C.c_void_p), ("mode_prob", C.c_void_p), ("gate_z", C.c_void_p), ("gate_S", C.c_void_p)]
+
+
+def pred_out(cap: int, ptrs: dict) -> PredOut:
+    """lmot_pred_out of `cap` rows over the given array addresses (keys ids, track_manage, flags, x, P, mode_prob, optional gate_z /
+    gate_S; device addresses for the _dev forms).  Layout: ids / track_manage [cap], flags [n_t][cap], x [n_t][cap][5], P [n_t][cap][25],
+    mode_prob [n_t][cap][3], gate_z [n_t][cap][2], gate_S [n_t][cap][4]."""
+    o = PredOut()
+    o.cap = int(cap)
+    for name, _ in PredOut._fields_[2:]:
+        setattr(o, name, int(ptrs[name]) if ptrs.get(name) else None)
+    return o
+
+
 class SeqOut(C.Structure):
     _fields_ = [("n_seq", C.c_int), ("seq", FrameOut * MAX_BATCH)]
 
@@ -197,6 +218,7 @@ ABI_SYMBOLS = [
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
     "lmot_track_ids", "lmot_seq_track_ids",
+    "lmot_predict_tracks", "lmot_predict_tracks_dev", "lmot_seq_predict_tracks", "lmot_seq_predict_tracks_dev",
     "lmot_detect_boxes_dev", "lmot_track_step_lists_dev", "lmot_tracker_counters_dev", "lmot_tracker_table_received",
     "lmot_origin_points", "lmot_tracker_table", "lmot_tracker_set_num_tracks", "lmot_tracker_reset", "lmot_tracker_num_tracks", "lmot_tracker_dump", "lmot_tracker_load", "lmot_tracker_get_ego", "lmot_tracker_set_ego",
     "lmot_debug_polar_grid", "lmot_debug_cell_index", "lmot_debug_label_grid", "lmot_selftest_atan2f",
@@ -652,6 +674,55 @@ class Lmot:
     def seq_track_ids(self, k: int) -> np.ndarray:
         """As track_ids, for sequence k of the tick most recently returned."""
         return self._ids(self.lib.lmot_seq_track_ids, int(k))
+
+    # ---- track prediction (lmot_predict_tracks*) ----------------------------------------------------------------------------------
+    def _predict(self, fn, k, t_us, cap):
+        t = np.ascontiguousarray(np.atleast_1d(np.asarray(t_us, np.float64)))
+        n_t = int(t.shape[0])
+        fn.argtypes = [C.c_void_p] + [C.c_int] * len(k) + [C.c_void_p, C.c_int, C.POINTER(PredOut)]
+        while True:
+            cap = max(int(cap), 0)
+            r = {"ids": np.zeros(cap, np.int64), "track_manage": np.zeros(cap, np.int32), "flags": np.zeros((n_t, cap), np.uint8)}
+            for name, w in PRED_FIELDS:
+                r[name] = np.zeros((n_t, cap, w), np.float64)
+            r["P"] = r["P"].reshape(n_t, cap, 5, 5)
+            o = pred_out(cap, {name: a.ctypes.data for name, a in r.items()})
+            st = fn(self.h, *k, t.ctypes.data_as(C.c_void_p), n_t, C.byref(o))
+            if st == ERR_CAPACITY and o.n_rows > cap:
+                cap = o.n_rows
+                continue
+            self._chk(st)
+            n = o.n_rows
+            return {name: a[:n] if name in ("ids", "track_manage") else a[:, :n] for name, a in r.items()}
+
+    def predict_tracks(self, t_us, cap: int = 1024) -> dict:
+        """Every row of the context's own table predicted at the times t_us (us, 1..32 of them): ids [n], track_manage [n],
+        flags [n_t, n] (PRED_*), x [n_t, n, 5], P [n_t, n, 5, 5], mode_prob [n_t, n, 3], gate_z [n_t, n, 2], gate_S [n_t, n, 4]
+        (include/lmot.h, track prediction).  cap: first guess of the row count."""
+        return self._predict(self.lib.lmot_predict_tracks, (), t_us, cap)
+
+    def seq_predict_tracks(self, k: int, t_us, cap: int = 1024) -> dict:
+        """As predict_tracks, for sequence k of the open set."""
+        return self._predict(self.lib.lmot_seq_predict_tracks, (int(k),), t_us, cap)
+
+    def predict_tracks_dev(self, t_us, out: PredOut, d_n_rows: int | None = None):
+        """lmot_predict_tracks_dev: the own table into the device arrays of `out` (pred_out), the row count into the device int at
+        d_n_rows; ordered on the context's caller stream."""
+        t = np.ascontiguousarray(np.atleast_1d(np.asarray(t_us, np.float64)))
+        fn = self.lib.lmot_predict_tracks_dev
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(PredOut), C.c_void_p]
+        self._chk(fn(self.h, t.ctypes.data_as(C.c_void_p), int(t.shape[0]), C.byref(out), C.c_void_p(d_n_rows or 0)))
+
+    def seq_predict_tracks_dev(self, t_us, outs, d_n_rows: int | None = None):
+        """lmot_seq_predict_tracks_dev: every sequence in one launch; t_us [n_seq, n_t], outs = one PredOut per sequence, d_n_rows = device
+        int[n_seq] (or None)."""
+        t = np.ascontiguousarray(np.asarray(t_us, np.float64))
+        if t.ndim != 2:
+            raise ValueError("t_us must be [n_seq, n_t]")
+        arr = (PredOut * len(outs))(*outs)
+        fn = self.lib.lmot_seq_predict_tracks_dev
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(PredOut), C.c_void_p]
+        self._chk(fn(self.h, t.ctypes.data_as(C.c_void_p), int(t.shape[1]), arr, C.c_void_p(d_n_rows or 0)))
 
     # ---- detection parameters of a sequence (lmot_seq_set_detect_params) --------------------------------------------------------
     def seq_set_detect_params(self, k: int, **fields):

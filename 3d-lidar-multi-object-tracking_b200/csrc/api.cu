@@ -613,6 +613,10 @@ void lmot_destroy(lmot_ctx* ctx) {
   tracker_free(c->own);
   seq_destroy(c);
   cudaFree(c->d_mt_raw);
+  if (c->ev_pred) cudaEventDestroy(c->ev_pred);
+  if (c->ev_pred_in) cudaEventDestroy(c->ev_pred_in);
+  cudaFree(c->d_pred_stage);
+  if (c->h_pred_n) cudaFreeHost(c->h_pred_n);
   if (c->trk_stream) cudaStreamDestroy(c->trk_stream);
   if (c->pub_stream) cudaStreamDestroy(c->pub_stream);
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
@@ -1628,6 +1632,7 @@ static int tracker_reset(Ctx* c, Tracker& t) {
   int rc = drain(c);
   if (rc) return rc;
   t.th = TrackerHost();
+  t.pred_ok = false;                   // no stamp to predict from until the next step or load
   t.act_valid = false;
   t.ids_identity = true;               // the spawn counter restarts at 0 (the retirement switch is kept)
   LMOT_CUDA(c, cudaMemsetAsync(t.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
@@ -1749,6 +1754,7 @@ static int tracker_load(Ctx* c, Tracker& trk, const double* dumps, int n, int in
   trk.th = TrackerHost();
   trk.th.init = init != 0; trk.th.timestamp = timestamp_us; trk.th.egoVelo = ego_velo; trk.th.egoYaw = ego_yaw;
   trk.th.egoPreYaw = ego_pre_yaw; trk.th.egoPoint[2] = ego_point_yaw;
+  trk.pred_ok = true;                  // predictions start from timestamp_us
   // (like the oracle's ref_tracker_load, which clears egoDeltaHis_: the dead-reckoning fold restarts from (0, 0, -pi/2) and
   //  ego_point_yaw is only egoPoints_[0][2] until the next step recomputes it.  A checkpoint that must keep the accumulated ego
   //  pose restores it with lmot_tracker_set_ego.)
@@ -1815,6 +1821,120 @@ int lmot_track_ids(lmot_ctx* ctx, int64_t* ids, int cap, int* n) {
 int lmot_seq_track_ids(lmot_ctx* ctx, int k, int64_t* ids, int cap, int* n) {
   if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
   return track_ids(ctx->c.seq[k], reinterpret_cast<long long*>(ids), cap, n);
+}
+
+// ---- track prediction (lmot_predict_tracks*; tracker.cu predict_launch)
+static bool pred_out_valid(const lmot_pred_out& o) {
+  return o.cap >= 0 && (o.cap == 0 || (o.ids && o.track_manage && o.flags && o.x && o.P && o.mode_prob));
+}
+
+// n_t in range, finite stamps, a table with a stamp, no stamp before it
+static int pred_times_valid(const Tracker& t, const double* t_us, int n_t) {
+  if (!t_us || n_t < 1 || n_t > LMOT_MAX_PRED_TIMES) return LMOT_ERR_INVALID;
+  for (int j = 0; j < n_t; ++j) if (!std::isfinite(t_us[j])) return LMOT_ERR_INVALID;
+  if (!t.pred_ok) return LMOT_ERR_STATE;
+  for (int j = 0; j < n_t; ++j) if (t_us[j] < t.th.timestamp) return LMOT_ERR_INVALID;
+  return LMOT_OK;
+}
+
+// the stream of the table's latest step (the prediction is ordered behind it there)
+static cudaStream_t pred_stream_of(const Ctx* c, const Tracker& t) { return t.last_st ? t.last_st : c->trk_stream; }
+
+// device outputs: the caller stream's earlier work on them comes first, and the caller stream waits for the prediction
+static int predict_dev(Ctx* c, Tracker* const* tabs, int S, const double* t_us, int n_t, const lmot_pred_out* d_outs, int* const* d_n_rows,
+                       cudaStream_t st) {
+  if (st != c->stream) {
+    if (!c->ev_pred_in) LMOT_CUDA(c, cudaEventCreateWithFlags(&c->ev_pred_in, cudaEventDisableTiming));
+    LMOT_CUDA(c, cudaEventRecord(c->ev_pred_in, c->stream));
+    LMOT_CUDA(c, cudaStreamWaitEvent(st, c->ev_pred_in, 0));
+  }
+  if (int rc = predict_launch(c, tabs, S, t_us, n_t, d_outs, d_n_rows, st)) return rc;
+  if (st != c->stream) LMOT_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_pred, 0));
+  return LMOT_OK;
+}
+
+// host outputs: the kernel writes a device staging area (grown to the largest request), then the rows that fit are copied out
+static int predict_host(Ctx* c, Tracker& t, const double* t_us, int n_t, lmot_pred_out* out, cudaStream_t st) {
+  if (!out || !pred_out_valid(*out)) return LMOT_ERR_INVALID;
+  if (int rc = pred_times_valid(t, t_us, n_t)) return rc;
+  const size_t cap = (size_t)out->cap, rows = (size_t)n_t * cap;
+  auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t o_ids = 256, o_tm = o_ids + up(cap * 8), o_fl = o_tm + up(cap * 4), o_x = o_fl + up(rows), o_P = o_x + up(rows * 40),
+               o_mp = o_P + up(rows * 200), o_gz = o_mp + up(rows * 24), o_gS = o_gz + up(rows * 16), bytes = o_gS + up(rows * 32);
+  if (bytes > c->pred_stage_bytes) {
+    cudaFree(c->d_pred_stage);           // (a host form has waited for its copies: nothing reads the old area)
+    c->d_pred_stage = nullptr; c->pred_stage_bytes = 0;
+    LMOT_CUDA(c, cudaMalloc(&c->d_pred_stage, bytes));
+    c->pred_stage_bytes = bytes;
+  }
+  if (!c->h_pred_n) LMOT_CUDA(c, cudaHostAlloc(&c->h_pred_n, sizeof(int), cudaHostAllocDefault));
+  unsigned char* b = c->d_pred_stage;
+  lmot_pred_out d{out->cap, 0, reinterpret_cast<int64_t*>(b + o_ids), reinterpret_cast<int32_t*>(b + o_tm), b + o_fl,
+                  reinterpret_cast<double*>(b + o_x), reinterpret_cast<double*>(b + o_P), reinterpret_cast<double*>(b + o_mp),
+                  out->gate_z ? reinterpret_cast<double*>(b + o_gz) : nullptr, out->gate_S ? reinterpret_cast<double*>(b + o_gS) : nullptr};
+  int* dn = reinterpret_cast<int*>(b);
+  Tracker* tabs[1] = {&t};
+  if (int rc = predict_launch(c, tabs, 1, t_us, n_t, &d, &dn, st)) return rc;
+  LMOT_CUDA(c, cudaMemcpyAsync(c->h_pred_n, dn, sizeof(int), cudaMemcpyDeviceToHost, st));
+  LMOT_CUDA(c, cudaEventRecord(c->ev_pred, st));
+  LMOT_CUDA(c, cudaEventSynchronize(c->ev_pred));
+  const int n = *c->h_pred_n;
+  out->n_rows = n;
+  const size_t m = (size_t)(n < out->cap ? n : out->cap);
+  if (m > 0) {
+    auto rows2d = [&](void* dst, const void* src, size_t k) {    // [n_t][cap][k] -> the first m rows of every time
+      return cudaMemcpy2DAsync(dst, cap * k, src, cap * k, m * k, n_t, cudaMemcpyDeviceToHost, st);
+    };
+    LMOT_CUDA(c, cudaMemcpyAsync(out->ids, d.ids, m * 8, cudaMemcpyDeviceToHost, st));
+    LMOT_CUDA(c, cudaMemcpyAsync(out->track_manage, d.track_manage, m * 4, cudaMemcpyDeviceToHost, st));
+    LMOT_CUDA(c, rows2d(out->flags, d.flags, 1));
+    LMOT_CUDA(c, rows2d(out->x, d.x, 40));
+    LMOT_CUDA(c, rows2d(out->P, d.P, 200));
+    LMOT_CUDA(c, rows2d(out->mode_prob, d.mode_prob, 24));
+    if (out->gate_z) LMOT_CUDA(c, rows2d(out->gate_z, d.gate_z, 16));
+    if (out->gate_S) LMOT_CUDA(c, rows2d(out->gate_S, d.gate_S, 32));
+    LMOT_CUDA(c, cudaEventRecord(c->ev_pred, st));
+    LMOT_CUDA(c, cudaEventSynchronize(c->ev_pred));
+  }
+  return n > out->cap ? LMOT_ERR_CAPACITY : LMOT_OK;
+}
+
+int lmot_predict_tracks(lmot_ctx* ctx, const double* t_us, int n_t, lmot_pred_out* out) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  cudaSetDevice(c->device);
+  return predict_host(c, c->own, t_us, n_t, out, pred_stream_of(c, c->own));
+}
+
+int lmot_predict_tracks_dev(lmot_ctx* ctx, const double* t_us, int n_t, const lmot_pred_out* d_out, int* d_n_rows) {
+  if (!ctx || !d_out || !pred_out_valid(*d_out)) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  if (int rc = pred_times_valid(c->own, t_us, n_t)) return rc;
+  cudaSetDevice(c->device);
+  Tracker* tabs[1] = {&c->own};
+  return predict_dev(c, tabs, 1, t_us, n_t, d_out, &d_n_rows, pred_stream_of(c, c->own));
+}
+
+int lmot_seq_predict_tracks(lmot_ctx* ctx, int k, const double* t_us, int n_t, lmot_pred_out* out) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  if (c->timing) return LMOT_ERR_STATE;
+  cudaSetDevice(c->device);
+  return predict_host(c, c->seq[k], t_us, n_t, out, c->trk_stream);
+}
+
+int lmot_seq_predict_tracks_dev(lmot_ctx* ctx, const double* t_us, int n_t, const lmot_pred_out* d_outs, int* d_n_rows) {
+  if (!ctx || ctx->c.n_seq < 1 || !d_outs || !t_us || n_t < 1 || n_t > LMOT_MAX_PRED_TIMES) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  const int S = c->n_seq;
+  for (int k = 0; k < S; ++k) if (!pred_out_valid(d_outs[k])) return LMOT_ERR_INVALID;
+  if (c->timing) return LMOT_ERR_STATE;
+  for (int k = 0; k < S; ++k) if (int rc = pred_times_valid(c->seq[k], t_us + (size_t)k * n_t, n_t)) return rc;
+  cudaSetDevice(c->device);
+  Tracker* tabs[kMaxBatch];
+  int* dn[kMaxBatch];
+  for (int k = 0; k < S; ++k) { tabs[k] = &c->seq[k]; dn[k] = d_n_rows ? d_n_rows + k : nullptr; }
+  return predict_dev(c, tabs, S, t_us, n_t, d_outs, dn, c->trk_stream);
 }
 
 // ---- per-sequence state (lmot_seq_*)

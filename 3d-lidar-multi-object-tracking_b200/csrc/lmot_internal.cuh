@@ -261,6 +261,9 @@ struct Tracker {
   int ids_n = -1;                      // IDs of the result most recently returned for this table: count (-1: none yet) ...
   bool ids_rows = true;                // ... the row indices, or
   std::vector<long long> ids_last;     // ... these
+  // track prediction (lmot_predict_tracks): the table's stamp th.timestamp is meaningful once it stepped or was loaded
+  bool pred_ok = false;
+  cudaStream_t last_st = nullptr;      // the stream of the table's latest submitted step (nullptr: none since open)
 };
 
 // what the tracker chain of a sequence tick reads for sequence k: its measurement list, the list in the dead-reckoned global frame
@@ -340,6 +343,15 @@ struct Ctx {
   lmot_detect_params seq_det[kMaxBatch] = {};
   int seq_fc_n[kMaxBatch] = {};                // lmot_seq_frame_counts: frames of sequence k in the tick collected last
   int seq_fc[kMaxBatch][kMaxBatch][4] = {};    // ... and their n_elev, n_ground, num_cluster, n_boxes (host copies: the ring slot is reused)
+
+  // ---- track prediction (lmot_predict_tracks*, tracker.cu predict_launch)
+  bool pred_pending = false;           // a prediction was queued since the last tracker step: the next step's first kernel waits for it
+  cudaStream_t pred_stream = nullptr;  // ... on this stream
+  cudaEvent_t ev_pred = nullptr;       // recorded after every prediction (created on first use)
+  cudaEvent_t ev_pred_in = nullptr;    // _dev forms on another stream: the caller stream's work so far (created on first use)
+  unsigned char* d_pred_stage = nullptr;   // host forms: device staging of the outputs, grown to the largest request
+  size_t pred_stage_bytes = 0;
+  int* h_pred_n = nullptr;             // pinned: the staged row count
 
   // ---- timing
   bool timing = false;
@@ -432,6 +444,10 @@ int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const float* d_lists, c
 // sequence ticks: measurement list m[k] -> track table c->seq[k] -> tick->blocks[k] (tracker.cu)
 int seq_global_launch(Ctx* c, const SeqMeas* m, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw);
 int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw);
+// track prediction of S tables (1..kMaxBatch) at n_t times each (t_us[k * n_t + j]) into outs[k] (device arrays), row counts into
+// d_n_rows[k] (nullable), on stream st behind the tables' latest steps; records c->ev_pred after the kernel (tracker.cu)
+int predict_launch(Ctx* c, Tracker* const* tabs, int S, const double* t_us, int n_t, const lmot_pred_out* outs, int* const* d_n_rows,
+                   cudaStream_t st);
 int boxes_publish(Ctx* c, Slot* s, Result* r, cudaStream_t st);     // detection-only: slot box list -> pinned host block
 
 }  // namespace lmot

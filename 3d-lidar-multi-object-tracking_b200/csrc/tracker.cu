@@ -333,164 +333,9 @@ imm_predict_gate_body(TrackState* __restrict__ tracks, const int* __restrict__ t
     double Pe = 0.0, zp0 = 0.0, zp1 = 0.0;
     double Si[4] = {0, 0, 0, 0};
     if (model < 3) {
-    // ---- MixingProbability (ukf.cpp:439-455) for this warp's model column j = model
-    const double pj0 = P.trans(0, model), pj1 = P.trans(1, model), pj2 = P.trans(2, model);
-    const double sumProb = mp0 * pj0 + mp1 * pj1 + mp2 * pj2;
-    const double mu0 = mp0 * pj0 / sumProb, mu1 = mp1 * pj1 / sumProb, mu2 = mp2 * pj2 / sumProb;
-    // ---- Interaction (:458-500)
-#pragma unroll
-    for (int e = 0; e < 5; ++e) x[e] = mu0 * sh.xp[0][e] + mu1 * sh.xp[1][e] + mu2 * sh.xp[2][e];
-    x[3] = wrap_pi(sh.xp[model][3]);
-    if (lane < 25) {
-      const int r = lane / 5, c = lane % 5;
-      const double xr = (r == 0) ? x[0] : (r == 1) ? x[1] : (r == 2) ? x[2] : (r == 3) ? x[3] : x[4];
-      const double xc = (c == 0) ? x[0] : (c == 1) ? x[1] : (c == 2) ? x[2] : (c == 3) ? x[3] : x[4];
-      const double t0 = mu0 * (sh.Pp[0][lane] + (sh.xp[0][r] - xr) * (sh.xp[0][c] - xc));
-      const double t1 = mu1 * (sh.Pp[1][lane] + (sh.xp[1][r] - xr) * (sh.xp[1][c] - xc));
-      const double t2 = mu2 * (sh.Pp[2][lane] + (sh.xp[2][r] - xr) * (sh.xp[2][c] - xc));
-      sh.Pm[model][lane] = t0 + t1 + t2;
-    }
+#include "imm_mix.inc"
     __syncwarp();
-    // ---- Prediction (:630-772): P_aug.llt() with Eigen's early exit on a non-positive pivot (LLT.h:271-295)
-    if (lane == 0) {
-      // 5x5 block in registers, fully unrolled (packed lower triangle); the two augmentation rows are diagonal
-      double a[15];
-#pragma unroll
-      for (int r = 0; r < 5; ++r)
-#pragma unroll
-        for (int c = 0; c <= r; ++c) a[r * (r + 1) / 2 + c] = sh.Pm[model][r * 5 + c];
-      bool stop = false;
-#pragma unroll
-      for (int k = 0; k < 5; ++k) {
-        if (!stop) {
-          double xk = a[k * (k + 1) / 2 + k];
-          if (k > 0) {
-            double sq = a[k * (k + 1) / 2] * a[k * (k + 1) / 2];
-#pragma unroll
-            for (int j = 1; j < k; ++j) sq += a[k * (k + 1) / 2 + j] * a[k * (k + 1) / 2 + j];
-            xk -= sq;
-          }
-          if (xk <= 0.0) stop = true;                        // Eigen returns here; the rest stays unfactored
-          else {
-            xk = sqrt(xk);
-            a[k * (k + 1) / 2 + k] = xk;
-#pragma unroll
-            for (int r = k + 1; r < 5; ++r) {
-              double acc = a[r * (r + 1) / 2 + k];
-#pragma unroll
-              for (int j = 0; j < k; ++j) acc -= a[r * (r + 1) / 2 + j] * a[k * (k + 1) / 2 + j];
-              a[r * (r + 1) / 2 + k] = qdiv(acc, xk);
-            }
-          }
-        }
-      }
-      double* L = sh.L[model];
-#pragma unroll
-      for (int r = 0; r < 7; ++r)
-#pragma unroll
-        for (int c = 0; c < 7; ++c) L[r * 7 + c] = (r < 5 && c <= r) ? a[r * (r + 1) / 2 + c] : 0.0;
-      // columns 5 and 6: pivot = sigma^2 - 0 > 0 -> sqrt, unless the factorisation stopped earlier (then raw sigma^2)
-      // (std_a, std_yawdd of this warp's model: ukf.cpp:642-657)
-      const double sa = P.std_a(model), sy = P.std_yawdd(model);
-      const double s2a = sa * sa, s2y = sy * sy;
-      L[5 * 7 + 5] = stop ? s2a : sqrt(s2a);
-      L[6 * 7 + 6] = stop ? s2y : sqrt(s2y);
-    }
-    __syncwarp();
-    if (lane < 15) {      // one sigma point per lane (:682-735)
-      const double sq = sqrt(lambda_aug + 7);
-      double a[7];
-#pragma unroll
-      for (int e = 0; e < 5; ++e) a[e] = x[e];
-      a[5] = 0; a[6] = 0;
-      if (lane >= 1) {
-        const int col = (lane - 1) % 7;
-        const double* L = sh.L[model];
-#pragma unroll
-        for (int e = 0; e < 7; ++e) a[e] = (lane <= 7) ? a[e] + sq * L[e * 7 + col] : a[e] - sq * L[e * 7 + col];
-      }
-      const double p_x = a[0], p_y = a[1], v = a[2], yaw = a[3], yawd = a[4], nu_a = a[5], nu_yawdd = a[6];
-      double s0, s1, s2, s3, s4;
-      if (model == 2) { s0 = p_x; s1 = p_y; s2 = v; s3 = yaw; s4 = yawd; }      // randomMotion :589-606
-      else {
-        double px_p, py_p, yaw_p;
-        if (model == 0) {                                                         // Cv :564-588
-          px_p = p_x + v * cos(yaw) * dt;
-          py_p = p_y + v * sin(yaw) * dt;
-          yaw_p = yaw;
-        } else {                                                                  // Ctrv :539-563
-          if (fabs(yawd) > 0.001) {
-            px_p = p_x + v / yawd * (sin(yaw + yawd * dt) - sin(yaw));
-            py_p = p_y + v / yawd * (cos(yaw) - cos(yaw + yawd * dt));
-          } else {
-            px_p = p_x + v * dt * cos(yaw);
-            py_p = p_y + v * dt * sin(yaw);
-          }
-          yaw_p = yaw + yawd * dt;
-        }
-        double v_p = v, yawd_p = yawd;
-        px_p = px_p + 0.5 * nu_a * dt * dt * cos(yaw);
-        py_p = py_p + 0.5 * nu_a * dt * dt * sin(yaw);
-        v_p = v_p + nu_a * dt;
-        yaw_p = yaw_p + 0.5 * nu_yawdd * dt * dt;
-        yawd_p = yawd_p + nu_yawdd * dt;
-        s0 = px_p; s1 = py_p; s2 = v_p; s3 = yaw_p; s4 = yawd_p;
-      }
-      double* o = sh.Xs[model][lane];
-      o[0] = s0; o[1] = s1; o[2] = s2; o[3] = s3; o[4] = s4;
-    }
-    __syncwarp();
-    // predicted mean (:737-744), every lane sums in sigma-point order
-#pragma unroll
-    for (int e = 0; e < 5; ++e) {
-      double acc = 0.0;
-#pragma unroll
-      for (int i = 0; i < 15; ++i) acc = acc + ((i == 0) ? w0 : wi) * sh.Xs[model][i][e];
-      x[e] = acc;
-    }
-    x[3] = wrap_pi(x[3]);
-    // the yaw residual of sigma point i is wrapped once (lane = sigma point) instead of inside the 15-term sums of the
-    // nine covariance elements that use it: same operands, same operations, same bits
-    if (lane < 15) sh.dyaw[model][lane] = wrap_pi(sh.Xs[model][lane][3] - x[3]);
-    __syncwarp();
-    if (lane < 25) {      // predicted covariance element (:746-755)
-      const int r = lane / 5, c = lane % 5;
-      const double xr = (r == 0) ? x[0] : (r == 1) ? x[1] : (r == 2) ? x[2] : (r == 3) ? x[3] : x[4];
-      const double xc = (c == 0) ? x[0] : (c == 1) ? x[1] : (c == 2) ? x[2] : (c == 3) ? x[3] : x[4];
-#pragma unroll
-      for (int i = 0; i < 15; ++i) {
-        const double dr = (r == 3) ? sh.dyaw[model][i] : sh.Xs[model][i][r] - xr;
-        const double dc = (c == 3) ? sh.dyaw[model][i] : sh.Xs[model][i][c] - xc;
-        Pe = Pe + (((i == 0) ? w0 : wi) * dr) * dc;
-      }
-    }
-    // ---- UpdateLidar (:778-902)
-#pragma unroll
-    for (int i = 0; i < 15; ++i) { const double w = (i == 0) ? w0 : wi; zp0 = zp0 + w * sh.Xs[model][i][0]; zp1 = zp1 + w * sh.Xs[model][i][1]; }
-    if (lane < 4) {
-      const int r = lane >> 1, c = lane & 1;
-      double acc = 0.0;
-#pragma unroll
-      for (int i = 0; i < 15; ++i) {
-        const double dzr = sh.Xs[model][i][r] - (r ? zp1 : zp0), dzc = sh.Xs[model][i][c] - (c ? zp1 : zp0);
-        acc = acc + (((i == 0) ? w0 : wi) * dzr) * dzc;
-      }
-      const double R = (r == c) ? P.r(r) : 0.0;
-      sh.S[model][lane] = acc + R;
-    } else if (lane < 14) {
-      const int e = lane - 4, r = e >> 1, c = e & 1;
-      const double xr = (r == 0) ? x[0] : (r == 1) ? x[1] : (r == 2) ? x[2] : (r == 3) ? x[3] : x[4];
-      double acc = 0.0;
-#pragma unroll
-      for (int i = 0; i < 15; ++i) {
-        const double xd = sh.Xs[model][i][r] - xr, dz = sh.Xs[model][i][c] - (c ? zp1 : zp0);
-        acc = acc + (((i == 0) ? w0 : wi) * xd) * dz;
-      }
-      sh.Tc[model][e] = acc;
-    }
-    __syncwarp();
-    inv2_lu(sh.S[model], Si);
-    if (lane == 0) sh.detS[model] = det2(sh.S[model]);     // for findMaxZandS below: each warp its own model, not every warp all three
+#include "imm_propagate.inc"
     }   // model < 3
     __syncthreads();                      // the guard's verdict is in
     if (sh.explode) {
@@ -511,14 +356,7 @@ imm_predict_gate_body(TrackState* __restrict__ tracks, const int* __restrict__ t
     __syncthreads();
 
     // ---- findMaxZandS (:176-203), gate scale x4 and explosion guard (:843-851)
-    const double dcv = sh.detS[0], dctrv = sh.detS[1], drm = sh.detS[2];
-    int mm;
-    if (dcv > dctrv) mm = (dcv > drm) ? 0 : 2; else mm = (dctrv > drm) ? 1 : 2;
-    double S4[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) S4[e] = sh.S[mm][e] * 4;
-    const double detS = det2(S4);
-    const bool dead = isnan(detS) || detS > 10;
+#include "imm_max_s.inc"
     const int trackNum = t.trackNum;
     __syncthreads();                      // everyone has read t.trackNum / sh before thread 0 may change it
     if (dead) {
@@ -1017,34 +855,9 @@ imm_update_body(TrackState* __restrict__ tracks, const int* __restrict__ trk, co
         }
         // ---- PostProcessIMMUKF: UpdateModeProb (ukf.cpp:384-397), MergeEstimationAndCovariance (:419-437)
         double mp[3] = {t.modeProb[0], t.modeProb[1], t.modeProb[2]};
-        const double sumG = lam[0] * mp[0] + lam[1] * mp[1] + lam[2] * mp[2];
-#pragma unroll
-        for (int m = 0; m < 3; ++m) { mp[m] = (lam[m] * mp[m]) / sumG; }
-#pragma unroll
-        for (int m = 0; m < 3; ++m) if (fabs(mp[m]) < 0.0001) mp[m] = 0.0001;
-        double xnew[3][5];
-#pragma unroll
-        for (int m = 0; m < 3; ++m)
-#pragma unroll
-          for (int e = 0; e < 5; ++e) xnew[m][e] = sh.xnew[m][e];
-        double xm[5];
-#pragma unroll
-        for (int e = 0; e < 5; ++e) xm[e] = mp[0] * xnew[0][e] + mp[1] * xnew[1][e] + mp[2] * xnew[2][e];
-        xm[3] = wrap_pi(xm[3]);
-        double myaw;
-        if (mp[0] > mp[1]) myaw = (mp[0] > mp[2]) ? xnew[0][3] : xnew[2][3];
-        else               myaw = (mp[1] > mp[2]) ? xnew[1][3] : xnew[2][3];
-        xm[3] = myaw;
+#include "imm_merge.inc"
         if (lane < 25) {
-          const int r = lane / 5, c = lane % 5;
-          const double Pn0 = sh.Pnew[0][lane], Pn1 = sh.Pnew[1][lane], Pn2 = sh.Pnew[2][lane];
-          const double xr0 = sh.xnew[0][r], xr1 = sh.xnew[1][r], xr2 = sh.xnew[2][r];
-          const double xc0 = sh.xnew[0][c], xc1 = sh.xnew[1][c], xc2 = sh.xnew[2][c];
-          const double xmr = (r == 0) ? xm[0] : (r == 1) ? xm[1] : (r == 2) ? xm[2] : (r == 3) ? xm[3] : xm[4];
-          const double xmc = (c == 0) ? xm[0] : (c == 1) ? xm[1] : (c == 2) ? xm[2] : (c == 3) ? xm[3] : xm[4];
-          const double a0 = mp[0] * (Pn0 + (xr0 - xmr) * (xc0 - xmc));
-          const double a1 = mp[1] * (Pn1 + (xr1 - xmr) * (xc1 - xmc));
-          const double a2 = mp[2] * (Pn2 + (xr2 - xmr) * (xc2 - xmc));
+#include "imm_merge_p.inc"
           t.P[0][lane] = a0 + a1 + a2;
           t.P[1][lane] = Pn0; t.P[2][lane] = Pn1; t.P[3][lane] = Pn2;
         }
@@ -1118,6 +931,125 @@ imm_update_seq_tuned_kernel(const __grid_constant__ TBSeqTunedParams p) {
   if (!q.run) return;
   imm_update_body(q.tracks, q.trk, q.det, q.boxes, q.gate, q.first_setter, q.skip, p.b.words, q.act_list, q.summary, q.meas_n, q.meas_ctr,
                   TunTB{p.tp[blockIdx.y]});
+}
+
+// ------------------------------------------------------------------------------------------------ track prediction
+// lmot_predict_tracks*: on a COPY of every row of 1..8 tables, at up to LMOT_MAX_PRED_TIMES query times: ProcessIMMUKF(dt), findMaxZandS,
+// PostProcessIMMUKF({1, 1, 1}) (DESIGN.md section 6f).  Read-only: the table is never written.  One CTA per row (grid-stride over the
+// table's row count, read on the device), table = blockIdx.y.  Warps 0-2 = the models CV / CTRV / RM, as in TA: the mixing, interaction
+// and Cholesky of P_aug once per row (imm_mix.inc -- they do not depend on dt), then per query time the propagation, predicted mean /
+// covariance and S (imm_propagate.inc) into one of two buffers.  Warp 3 works one time behind: findMaxZandS and the gate guard
+// (imm_max_s.inc), TB's merge (imm_merge.inc, imm_merge_p.inc) and the outputs of time j - 1 while warps 0-2 predict time j.
+// No polling of any kind: it never holds SMs that something outside its stream has to reach.
+struct PredTab {
+  const TrackState* tracks; const int* trk;
+  const long long* ids;              // the rows' track IDs; nullptr: the row indices (a table that never retired)
+  lmot_pred_out o; int* n_rows;      // device arrays; n_rows nullable
+  TAPrm tp;
+};
+struct PredParams { PredTab s[kMaxBatch]; double dt[kMaxBatch][LMOT_MAX_PRED_TIMES]; int n_t; };
+static_assert(sizeof(PredParams) <= 4096, "kernel parameter block");
+
+struct PredBuf { double xnew[3][5], Pnew[3][25], S[3][4], zp[3][2], detS[3]; };   // the three models at one query time (TB's names)
+struct PredShared {                  // TA's staging (TAShared's names: the shared bodies read them), two PredBufs, the row's verdict
+  double xp[3][5];
+  double Pp[3][25];
+  double L[3][49];
+  double Xs[3][15][5];
+  double Pm[3][25];
+  double S[3][4], Tc[3][10];
+  double dyaw[3][15];
+  double detS[3];
+  PredBuf buf[2];
+  int flag;                          // 0: predict; LMOT_PRED_DEAD / LMOT_PRED_GUARD_P: not predicted
+};
+
+__global__ void __launch_bounds__(kTAThreads, 4)     // <= 128 registers, like TA: fits on an SM next to a ground-kernel CTA
+predict_tracks_kernel(const __grid_constant__ PredParams p) {
+  __shared__ PredShared sh_all;
+  PredShared& sh = sh_all;
+  PredBuf* const bufs = sh_all.buf;
+  pdl_wait();                              // the latest step (TC, its retire phase included) has completed
+  const PredTab& q = p.s[blockIdx.y];
+  const TunTA P{q.tp};
+  const int tid = threadIdx.x, lane = tid & 31, model = tid >> 5;
+  const int n_t = p.n_t, cap = q.o.cap;
+  const int T = q.trk[CNT_N_TRACKS];
+  if (blockIdx.x == 0 && tid == 0 && q.n_rows) *q.n_rows = T;
+  const int n = T < cap ? T : cap;         // rows beyond cap are not written
+  const double lambda_aug = 3 - 7;
+  const double w0 = lambda_aug / (lambda_aug + 7), wi = 0.5 / (7 + lambda_aug);
+  const double qnan = __longlong_as_double(0x7FF8000000000000ll);
+
+  for (int i = blockIdx.x; i < n; i += gridDim.x) {
+    const TrackState& t = q.tracks[i];
+    __syncthreads();                       // the previous row's readers are done with the shared copy
+    if (tid == 0) {
+      const int tn = t.trackNum;
+      sh.flag = (tn == 0) ? LMOT_PRED_DEAD : (det_lu<5>(t.P[0]) > 10 || t.P[0][24] > 1000) ? LMOT_PRED_GUARD_P : 0;   // :826, :828-831
+      q.o.ids[i] = q.ids ? q.ids[i] : (long long)i;
+      q.o.track_manage[i] = tn;
+    }
+    for (int e = tid; e < 15; e += kTAThreads) sh.xp[e / 5][e % 5] = t.x[1 + e / 5][e % 5];
+    for (int e = tid; e < 75; e += kTAThreads) sh.Pp[e / 25][e % 25] = t.P[1 + e / 25][e % 25];
+    const double mp0 = t.modeProb[0], mp1 = t.modeProb[1], mp2 = t.modeProb[2];
+    __syncthreads();
+    const int flag = sh.flag;
+    if (flag) {                            // not predicted: the flag, and NaN for every value, at every time
+      for (int e = tid; e < n_t * 40; e += kTAThreads) {
+        const int j = e / 40, k = e % 40;
+        const size_t row = (size_t)j * cap + i;
+        if (k < 5) q.o.x[row * 5 + k] = qnan;
+        else if (k < 30) q.o.P[row * 25 + (k - 5)] = qnan;
+        else if (k < 33) q.o.mode_prob[row * 3 + (k - 30)] = qnan;
+        else if (k < 35) { if (q.o.gate_z) q.o.gate_z[row * 2 + (k - 33)] = qnan; }
+        else if (k < 39) { if (q.o.gate_S) q.o.gate_S[row * 4 + (k - 35)] = qnan; }
+        else q.o.flags[row] = (uint8_t)flag;
+      }
+      continue;
+    }
+    double x[5] = {0, 0, 0, 0, 0};
+    double Pe = 0.0, zp0 = 0.0, zp1 = 0.0;
+    double Si[4] = {0, 0, 0, 0};
+    double xi[5];                          // the mixed mean every query time starts from
+    if (model < 3) {
+#include "imm_mix.inc"
+    __syncwarp();
+    }
+#pragma unroll
+    for (int e = 0; e < 5; ++e) xi[e] = x[e];
+    for (int j = 0; j <= n_t; ++j) {
+      if (model < 3 && j < n_t) {
+        const double dt = p.dt[blockIdx.y][j];
+#pragma unroll
+        for (int e = 0; e < 5; ++e) x[e] = xi[e];
+        Pe = 0.0; zp0 = 0.0; zp1 = 0.0;
+#include "imm_propagate.inc"
+        PredBuf& b = bufs[j & 1];
+        if (lane < 5) b.xnew[model][lane] = (lane == 0) ? x[0] : (lane == 1) ? x[1] : (lane == 2) ? x[2] : (lane == 3) ? x[3] : x[4];
+        if (lane < 25) b.Pnew[model][lane] = Pe;
+        if (lane < 4) b.S[model][lane] = sh.S[model][lane];
+        if (lane == 0) { b.zp[model][0] = zp0; b.zp[model][1] = zp1; b.detS[model] = sh.detS[model]; }
+      } else if (model == 3 && j > 0) {
+        const PredBuf& sh = bufs[(j - 1) & 1];     // (the shared bodies read `sh`: here the buffer of time j - 1)
+#include "imm_max_s.inc"
+        double lam[3] = {1.0, 1.0, 1.0};           // PostProcessIMMUKF({1, 1, 1}): a step without information
+        double mp[3] = {mp0, mp1, mp2};
+#include "imm_merge.inc"
+        const size_t row = (size_t)(j - 1) * cap + i;
+        if (lane < 25) {
+#include "imm_merge_p.inc"
+          q.o.P[row * 25 + lane] = a0 + a1 + a2;
+        }
+        if (lane < 5) q.o.x[row * 5 + lane] = (lane == 0) ? xm[0] : (lane == 1) ? xm[1] : (lane == 2) ? xm[2] : (lane == 3) ? xm[3] : xm[4];
+        if (lane < 3) q.o.mode_prob[row * 3 + lane] = (lane == 0) ? mp[0] : (lane == 1) ? mp[1] : mp[2];
+        if (q.o.gate_z && lane < 2) q.o.gate_z[row * 2 + lane] = sh.zp[mm][lane];
+        if (q.o.gate_S && lane < 4) q.o.gate_S[row * 4 + lane] = sh.S[mm][lane];
+        if (lane == 0) q.o.flags[row] = (uint8_t)(LMOT_PRED_VALID | (dead ? LMOT_PRED_GUARD_S : 0));
+      }
+      __syncthreads();                     // buffer j is complete / buffer j - 1 is consumed
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ TC: over-segmentation test
@@ -2257,6 +2189,8 @@ int chain_prepare(Ctx* c, Tracker& t, const SeqMeas& m, Result* r, cudaStream_t 
   t.th.timestamp = ts;
   t.th.egoPreYaw = t.th.egoYaw;
   t.th.init = true;
+  t.pred_ok = true;
+  t.last_st = st;
   return LMOT_OK;
 }
 
@@ -2275,11 +2209,17 @@ int chain_launch(Ctx* c, Chain& ch, cudaStream_t st, bool own, ChainGate gate, b
   pa.id = cudaLaunchAttributeProgrammaticStreamSerialization;
   cudaLaunchConfig_t cfg = {};
   cfg.stream = st; cfg.attrs = &pa; cfg.numAttrs = 1;
+  // a prediction queued since the last step reads the table this step writes, and TA waits for the previous TC, not for the grid in
+  // front of the gate kernel: the step's first kernel runs fully serialised behind it (behind its event when it ran on another stream)
+  const bool after_pred = c->pred_pending;
+  c->pred_pending = false;
+  if (after_pred && c->pred_stream != st) LMOT_CUDA(c, cudaStreamWaitEvent(st, c->ev_pred, 0));
   if (ta_tb) {
-    pa.val.programmaticStreamSerializationAllowed = gate != ChainGate::none ? 1 : 0;
+    pa.val.programmaticStreamSerializationAllowed = (gate != ChainGate::none && !after_pred) ? 1 : 0;
     cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); cfg.dynamicSmemBytes = 0;
     if (gate == ChainGate::one) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, tracker_gate_kernel, (const int*)ch.g.sem[0], c->spin_limit));
     if (gate == ChainGate::seq) { ch.g.n = S; LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, tracker_gate_seq_kernel, ch.g, c->spin_limit)); }
+    pa.val.programmaticStreamSerializationAllowed = gate != ChainGate::none ? 1 : 0;      // TA: the gate kernel's programmatic dependent
     // the single-stream chain's CTA count, shared by the tables (grid-stride over each table's active tracks)
     cfg.gridDim = dim3((c->trk_ctas + S - 1) / S, S); cfg.blockDim = dim3(kTAThreads);
     const TASeq& a = ch.ta.b.s[0];
@@ -2387,6 +2327,32 @@ int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const dou
   publish_seq_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(ch.pub);
   if (ch.ids_on) publish_ids_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(ch.ids);
   LMOT_CUDA(c, cudaGetLastError());
+  return LMOT_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- track prediction (lmot_predict_tracks*)
+// One launch for the S tables, on st behind their latest steps: a programmatic dependent of the step's TC, whose griddepcontrol.wait
+// returns once TC (retire phase included) has completed.  The next chain_launch serialises its first kernel behind it (pred_pending).
+int predict_launch(Ctx* c, Tracker* const* tabs, int S, const double* t_us, int n_t, const lmot_pred_out* outs, int* const* d_n_rows,
+                   cudaStream_t st) {
+  PredParams p{};
+  p.n_t = n_t;
+  for (int k = 0; k < S; ++k) {
+    const Tracker& t = *tabs[k];
+    p.s[k] = PredTab{t.d_tracks, t.d_trk_counters, t.ids_identity ? nullptr : t.d_ids, outs[k], d_n_rows ? d_n_rows[k] : nullptr, ta_prm(t.prm)};
+    for (int j = 0; j < n_t; ++j) p.dt[k][j] = (t_us[k * n_t + j] - t.th.timestamp) / 1000000.0;     // as chain_prepare's dt (:807)
+  }
+  if (!c->ev_pred) LMOT_CUDA(c, cudaEventCreateWithFlags(&c->ev_pred, cudaEventDisableTiming));
+  cudaLaunchAttribute pa;
+  pa.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  pa.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.stream = st; cfg.attrs = &pa; cfg.numAttrs = 1;
+  cfg.gridDim = dim3((c->trk_ctas + S - 1) / S, S); cfg.blockDim = dim3(kTAThreads);
+  LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, predict_tracks_kernel, p));
+  LMOT_CUDA(c, cudaEventRecord(c->ev_pred, st));
+  c->pred_pending = true;
+  c->pred_stream = st;
   return LMOT_OK;
 }
 

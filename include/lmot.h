@@ -478,6 +478,63 @@ int lmot_seq_get_track_retirement(const lmot_ctx* ctx, int k, int* on);
 int lmot_track_ids(lmot_ctx* ctx, int64_t* ids, int cap, int* n);
 int lmot_seq_track_ids(lmot_ctx* ctx, int k, int64_t* ids, int cap, int* n);
 
+/* ---- track prediction: every track's IMM-UKF state, covariance and gate at caller-given later times ---------------------------------
+ * For a track table, query time t (us, the clock of lmot_track_step) and row i, on a COPY of the track (the table is never modified):
+ *   dt = (t - ts_last) / 1e6, ts_last = the stamp of the table's most recently SUBMITTED step, or the stamp given to lmot_tracker_load
+ *   (computed as a step computes its dt, imm_ukf_jpda.cpp:807).
+ *   trackManage 0: nothing is predicted, flag LMOT_PRED_DEAD.
+ *   det(P_merge) > 10 || P_merge(4,4) > 1000 (the explosion guard, :828): nothing is predicted, flag LMOT_PRED_GUARD_P (a step would kill
+ *   the track before predicting it).
+ *   Otherwise ProcessIMMUKF(dt) (ukf.cpp:507-527: mixing, interaction, Prediction(dt, 0..2), UpdateLidar(0..2), which only sets zPred /
+ *   S / K), findMaxZandS (imm_ukf_jpda.cpp:176), then PostProcessIMMUKF({1, 1, 1}) (ukf.cpp:529-535): the merge of a step that brings no
+ *   information -- mode probabilities renormalised with the 1e-4 floor, merged mean and covariance, the yaw of the most probable model.
+ *   Reported: x (x, y, v, yaw, yaw rate) and P (5x5, row-major) of the merge, the three mode probabilities, gate_z / gate_S = the
+ *   max-det(S) model's predicted measurement and S (before the x4 of :844); flag LMOT_PRED_VALID, plus LMOT_PRED_GUARD_S if
+ *   isnan(det(4 S)) || det(4 S) > 10 (:848: a step at t would kill the track).  dt = 0 is allowed: it is the mixed state, not the posterior.
+ *   The values of rows that are not predicted are NaN.
+ * Rows: the table as lmot_tracker_dump sees it, in that order, each with its int64 track ID (lmot_track_ids: the row index for a table
+ * that never retired) and its trackManage.  Frame: the tracker's -- the dead-reckoned global frame with global_frame = 1, else the frame
+ * the boxes came in (lmot_tracker_get_ego gives the pose).  Parameters: the table's current tracker parameters (std_a, std_yawdd, the lidar
+ * noise and trans of lmot_set_tracker_params), the values the next submitted step would use.
+ * Output layout (lmot_pred_out): ids / track_manage [cap]; flags [n_t][cap]; x [n_t][cap][5]; P [n_t][cap][25]; mode_prob [n_t][cap][3];
+ * gate_z [n_t][cap][2]; gate_S [n_t][cap][4] (gate_z / gate_S nullable).  Rows beyond cap are not written; the row count is still
+ * returned (n_rows / d_n_rows), and the host forms then return LMOT_ERR_CAPACITY.
+ * lmot_predict_tracks(ctx, t_us, n_t, out): the context's own table, host outputs, out->n_rows = the row count.  Waits only for the
+ *   prediction, which is ordered after the latest submitted step on the device; it does not drain the detection slots.
+ * lmot_predict_tracks_dev(ctx, t_us, n_t, d_out, d_n_rows): the same into DEVICE arrays (d_out itself is a host struct), row count into
+ *   the device int d_n_rows (nullable); asynchronous: the caller stream (lmot_set_stream) waits for it on the device.
+ * lmot_seq_predict_tracks(ctx, k, t_us, n_t, out): sequence k of the open set, host outputs.
+ * lmot_seq_predict_tracks_dev(ctx, t_us, n_t, d_outs, d_n_rows): every sequence in ONE launch; t_us [n_seq][n_t] (host), d_outs [n_seq]
+ *   host structs of device arrays, d_n_rows [n_seq] device ints (nullable).
+ * A prediction runs on the tracker chain's stream right behind the latest submitted step; the next step of the context then starts one
+ * launch latency later (its first kernel waits for the prediction to finish).  Contexts that never predict run unchanged.
+ * LMOT_ERR_INVALID: n_t outside [1, LMOT_MAX_PRED_TIMES], a non-finite t or t before ts_last, cap < 0, a required array null while
+ * cap > 0, k out of range / no open set.  LMOT_ERR_STATE: the table has neither stepped nor been loaded since reset or open; the
+ * sequence forms in timing mode. */
+#define LMOT_MAX_PRED_TIMES 32
+enum {
+  LMOT_PRED_VALID = 1,     /* predicted */
+  LMOT_PRED_DEAD = 2,      /* trackManage 0: not predicted */
+  LMOT_PRED_GUARD_P = 4,   /* the P_merge explosion guard holds: not predicted */
+  LMOT_PRED_GUARD_S = 8    /* predicted, but det(4 S) is NaN or > 10: a step at t would kill the track */
+};
+typedef struct lmot_pred_out {
+  int cap;                 /* rows the arrays hold */
+  int n_rows;              /* host forms: rows of the table (may exceed cap) */
+  int64_t* ids;            /* [cap] */
+  int32_t* track_manage;   /* [cap] */
+  uint8_t* flags;          /* [n_t][cap] LMOT_PRED_* bits */
+  double* x;               /* [n_t][cap][5] */
+  double* P;               /* [n_t][cap][25] */
+  double* mode_prob;       /* [n_t][cap][3] */
+  double* gate_z;          /* [n_t][cap][2], nullable */
+  double* gate_S;          /* [n_t][cap][4], nullable */
+} lmot_pred_out;
+int lmot_predict_tracks(lmot_ctx* ctx, const double* t_us, int n_t, lmot_pred_out* out);
+int lmot_predict_tracks_dev(lmot_ctx* ctx, const double* t_us, int n_t, const lmot_pred_out* d_out, int* d_n_rows);
+int lmot_seq_predict_tracks(lmot_ctx* ctx, int k, const double* t_us, int n_t, lmot_pred_out* out);
+int lmot_seq_predict_tracks_dev(lmot_ctx* ctx, const double* t_us, int n_t, const lmot_pred_out* d_outs, int* d_n_rows);
+
 /* ---- detection parameters of one sequence: ground removal, clustering ROI and box fitting ------------------------------------------
  * lmot_params' detection fields, as a separate struct (callers compiled against today's lmot_params keep working).  Defaults are
  * lmot_default_params' values; citations are file:line under object_tracking/src/. */
