@@ -203,6 +203,15 @@ class SeqOut(C.Structure):
     _fields_ = [("n_seq", C.c_int), ("seq", FrameOut * MAX_BATCH)]
 
 
+SEQ_SKIP, SEQ_FRAMES, SEQ_LISTS = 0, 1, 2          # lmot_seq_entry.kind
+SEQ_RESTART = 1                                     # lmot_seq_entry.flags
+
+
+class SeqEntry(C.Structure):
+    _fields_ = [("kind", C.c_int), ("flags", C.c_int), ("timestamp_us", C.c_double), ("v_gps", C.c_double), ("yaw_gps", C.c_double),
+                ("data", C.POINTER(C.c_void_p)), ("n", C.POINTER(C.c_int)), ("d_counts", C.c_void_p), ("cap_per_list", C.c_int)]
+
+
 # every symbol include/lmot.h declares (tests assert the library exports all of them)
 ABI_SYMBOLS = [
     "lmot_default_params", "lmot_create", "lmot_destroy", "lmot_get_params", "lmot_strerror", "lmot_last_error", "lmot_build_info",
@@ -214,6 +223,7 @@ ABI_SYMBOLS = [
     "lmot_seq_open", "lmot_seq_submit", "lmot_seq_dev", "lmot_seq_collect", "lmot_seq_fetch", "lmot_seq", "lmot_seq_tracker_reset",
     "lmot_seq_tracker_dump", "lmot_seq_tracker_get_ego", "lmot_seq_set_sensors", "lmot_seq_get_sensors", "lmot_seq_frame_counts",
     "lmot_seq_track_submit", "lmot_seq_track_dev", "lmot_seq_track", "lmot_seq_tracker_load", "lmot_seq_tracker_set_ego",
+    "lmot_seq_tick_submit", "lmot_seq_tick_dev", "lmot_seq_tick", "lmot_seq_stepped",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
@@ -769,7 +779,7 @@ class Lmot:
         return so, sets
 
     def _seq_result(self, so, sets, want_boxes=True):
-        return [self._frame_result(so.seq[k], sets[k][1], want_boxes) for k in range(so.n_seq)]
+        return self._seq_tick_result(so, sets, want_boxes)
 
     def seq(self, frames, timestamps, v_gps=None, yaw_gps=None, cap: int | None = None):
         """One tick, synchronous: `frames` = per sequence one (N, >=3) host array, or a list of them (one per sensor of a sequence with
@@ -842,6 +852,68 @@ class Lmot:
         S = getattr(self, "n_seq", 0)
         ts, v, yaw = (self.seq_scalars(max(S, 1), x) for x in (timestamps, v_gps, yaw_gps))
         self._chk(self.lib.lmot_seq_track_dev(self.h, C.c_void_p(d_lists), C.c_void_p(d_counts), S, int(cap_per_list), ts, v, yaw))
+
+    # ---- sequence ticks on each stream's own clock (lmot_seq_tick*): any subset of the sequences, each from frames or box lists -----
+    def _seq_entries(self, entries, device: bool):
+        """per-sequence entries -> (SeqEntry array, stride, keep).  An entry is None (the sequence skips the tick) or a dict with
+        `frames=` (as one sequence's entry of seq() / seq_dev()) or `lists=` (host: as one sequence's entry of seq_track(); device: one
+        device address per list, with `d_counts=` the device address of their int lengths and `cap=` boxes per list), `timestamp=`,
+        `v_gps=`, `yaw_gps=` (default 0) and `restart=` (the sequence starts over with this step)."""
+        arr = (SeqEntry * len(entries))()
+        keep, stride = [], 4
+        for k, d in enumerate(entries):
+            if d is None:
+                continue
+            q = arr[k]
+            q.flags = SEQ_RESTART if d.get("restart") else 0
+            q.timestamp_us, q.v_gps, q.yaw_gps = (float(d.get(x) or 0.0) for x in ("timestamp", "v_gps", "yaw_gps"))
+            if "frames" in d:
+                q.kind = SEQ_FRAMES
+                fr = d["frames"]
+                ptrs, ns, _, st, kp = self._batch_args(fr if self._frame_list(fr, device) else [fr], device)
+                stride = st
+            elif device:
+                q.kind = SEQ_LISTS
+                ls = d["lists"] if isinstance(d["lists"], (list, tuple)) else [d["lists"]]
+                ptrs, ns, kp = (C.c_void_p * len(ls))(*[int(x) for x in ls]), None, None
+                q.d_counts, q.cap_per_list = int(d["d_counts"]), int(d["cap"])
+            else:
+                q.kind = SEQ_LISTS
+                ptrs, ns, _, kp = self._seq_lists([d["lists"]])
+            q.data = C.cast(ptrs, C.POINTER(C.c_void_p))
+            if ns is not None:
+                q.n = C.cast(ns, C.POINTER(C.c_int))
+            keep += [ptrs, ns, kp]
+        return arr, stride, keep
+
+    def seq_tick(self, entries, cap: int | None = None):
+        """One tick, synchronous, over host data: `entries` = one per sequence (see _seq_entries).  -> list of per-sequence dicts as
+        seq() returns, None for a sequence that skipped the tick."""
+        arr, stride, keep = self._seq_entries(entries, False)
+        so, sets = self._seq_out(cap or self.params.max_tracks)
+        self._chk(self.lib.lmot_seq_tick(self.h, arr, len(entries), stride, C.byref(so)))
+        return self._seq_tick_result(so, sets)
+
+    def seq_tick_submit(self, entries):
+        """Asynchronous seq_tick; results with seq_collect() / seq_fetch()."""
+        arr, stride, keep = self._seq_entries(entries, False)
+        self._keep = keep          # the copies are asynchronous: the host arrays must outlive the call
+        self._chk(self.lib.lmot_seq_tick_submit(self.h, arr, len(entries), stride))
+
+    def seq_tick_dev(self, entries):
+        """Asynchronous tick over device data (frames as seq_dev's entries; lists see _seq_entries), ordered after the context's stream."""
+        arr, _, keep = self._seq_entries(entries, True)
+        self._chk(self.lib.lmot_seq_tick_dev(self.h, arr, len(entries)))
+
+    def seq_stepped(self) -> int:
+        """Bit k: sequence k stepped in the tick most recently returned."""
+        m = C.c_uint32(0)
+        self._chk(self.lib.lmot_seq_stepped(self.h, C.byref(m)))
+        return int(m.value)
+
+    def _seq_tick_result(self, so, sets, want_boxes=True):
+        mask = self.seq_stepped()
+        return [self._frame_result(so.seq[k], sets[k][1], want_boxes) if mask >> k & 1 else None for k in range(so.n_seq)]
 
     def seq_tracker_load(self, k: int, dumps, init, timestamp_us, ego_velo=0.0, ego_yaw=0.0, ego_pre_yaw=0.0, ego_point_yaw=-np.pi / 2):
         """tracker_load for sequence k"""

@@ -403,9 +403,9 @@ void result_destroy(Result* r) {
 }
 
 // ---- independent sequences (lmot_seq_*): S frame streams, one or more frames each per tick, S track tables ---------------------------
-// Detection runs on the batch banks (batch_ensure).  Without sensor tables the box lists are NOT concatenated: sequence k's tracker
-// reads slot k's own list and counters (seq_tracker_launch, tracker.cu).  With any table set, concat_boxes_seq_kernel concatenates each
-// sequence's frames into that sequence's list on the bank (seq_meas) and the tracker reads those.
+// Detection runs on the batch banks (batch_ensure).  Without sensor tables the box lists are NOT concatenated: a FRAMES sequence's tracker
+// reads its detection slot's own list and counters (seq_tick_common's map).  With a table among the tick's FRAMES sequences,
+// concat_boxes_seq_kernel concatenates each of their frames into that sequence's list on the bank (seq_meas) and the tracker reads those.
 void seq_destroy(Ctx* c) {
   for (int k = 0; k < c->n_seq; ++k) tracker_free(c->seq[k]);
   for (int b = 0; b < kBatchBanks; ++b)
@@ -419,7 +419,7 @@ void seq_destroy(Ctx* c) {
   for (int i = 0; i < c->seq_ring; ++i)
     for (int k = 0; k < c->n_seq; ++k) result_destroy(&c->seq_ticks[i].blocks[k]);
   delete[] c->seq_ticks;
-  c->seq_ticks = nullptr; c->seq_last = nullptr;
+  c->seq_ticks = nullptr; c->seq_last = nullptr; c->seq_stepped = 0;
   c->n_seq = 0; c->seq_ring = 0; c->seq_next = 0; c->seq_oldest = 0; c->seq_in_flight = 0;
 }
 
@@ -445,16 +445,19 @@ SeqTick* seq_acquire(Ctx* c, bool drop_oldest) {
   return t;
 }
 
-// the tick's results: blocks[0].ev_done is recorded after the one publish launch that writes every block
+// the tick's results: blocks[0].ev_done is recorded after the one publish launch that writes every stepped block.  A skipped sequence's
+// block is stale (an earlier tick's step on this ring slot): its output, counts, IDs and last_n_act are left alone.
 int seq_collect_tick(Ctx* c, SeqTick* t, lmot_seq_out* out) {
   LMOT_CUDA(c, cudaEventSynchronize(t->blocks[0].ev_done));
   int rc = LMOT_OK;
   if (out) out->n_seq = c->n_seq;
+  c->seq_stepped = t->stepped;
   for (int k = 0; k < c->n_seq; ++k) {
+    if (!(t->stepped >> k & 1u)) { c->seq_fc_n[k] = 0; continue; }
     Result* b = &t->blocks[k];
     const int r = collect_result(c, b, out ? &out->seq[k] : nullptr, &c->seq[k]);
     if (r < 0 ? (rc >= 0) : (rc == LMOT_OK)) rc = r;       // the first error, else the first warning
-    // per-frame counts (lmot_seq_frame_counts): the concatenation wrote them into the block (ticks with tables); else the one frame's
+    // per-frame counts (lmot_seq_frame_counts): the concatenation / pack wrote them into the block; else the one frame's
     if (b->batch_frames > 0) {
       c->seq_fc_n[k] = b->batch_frames;
       memcpy(c->seq_fc[k], b->h_frame_counts, (size_t)b->batch_frames * 4 * sizeof(int));
@@ -1100,12 +1103,18 @@ int lmot_seq_open(lmot_ctx* ctx, int n_seq, int ring) {
   return rc;
 }
 
-// ---- sequence ticks: two front ends -- detection (frames -> ground removal, clustering, box fitting) and tracking-only (caller box
-// lists, lmot_seq_track*) -- fill each sequence's measurement list; one back end steps the tables.  Both kinds share the ring and the
-// bank alternation, so a set may mix them tick by tick; each table folds its steps in submission order.
+// ---- sequence ticks: one builder (seq_tick_common) for lmot_seq_tick_*, lmot_seq* (every entry FRAMES) and lmot_seq_track* (every entry
+// LISTS).  A tick's entries say, per sequence, whether it steps this tick and from what: FRAMES entries go through detection (ground
+// removal, clustering, box fitting), LISTS entries through one pack launch; both fill the stepped sequences' measurement lists, and ONE
+// tracker chain steps the stepped tables.  Every tick shares the ring and the bank alternation; each table folds its steps in submission
+// order.
+//
+// The map: the stepped sequences, in sequence order, are the chain positions 0..S-1 (seq[pos] = sequence).  The FRAMES entries' frames
+// are the detection slots in that order, the LISTS entries' lists the pack's lists in that order.  Every per-sequence array handed to a
+// launch (measurement lists, ego values, rig poses, frame-count pointers, result blocks, detection values) is built through it.
 
-// the tick's frames / lists: sequence k's sensors in table order, [f0[k], f0[k + 1]); one for a sequence without a table
-// (lmot_seq_set_sensors keeps the total at or below kMaxBatch).  -> whether any sequence has a table
+// the set's layout: sequence k's sensors in table order, [f0[k], f0[k + 1]); one for a sequence without a table (lmot_seq_set_sensors
+// keeps the total at or below kMaxBatch).  -> whether any sequence has a table
 static bool seq_layout(const Ctx* c, int* f0, bool* rig_on) {
   bool rigged = false;
   f0[0] = 0;
@@ -1117,186 +1126,246 @@ static bool seq_layout(const Ctx* c, int* f0, bool* rig_on) {
   return rigged;
 }
 
-// back end, first half: the tick's ring slot and bank.  *st: the stream the front end runs on -- the bank's first detection slot's for
-// detection, the bank's own for tracking-only ticks -- made to wait until the bank's previous tick has been consumed by the tracker.
-static int seq_begin(Ctx* c, bool drop_oldest, bool lists, SeqTick** t, int* bank, cudaStream_t* st) {
-  *t = seq_acquire(c, drop_oldest);
-  if (!*t) return LMOT_ERR_STATE;
-  const int b = c->next_bank;
-  c->next_bank = (c->next_bank + 1) % kBatchBanks;
-  *bank = b;
-  *st = lists ? c->bank[b].stream : c->bslots[b * c->batch_frames].stream;
-  LMOT_CUDA(c, cudaStreamWaitEvent(*st, c->bank[b].ev_trk_done, 0));
-  return LMOT_OK;
+// LMOT_SEQ_RESTART: lmot_seq_tracker_reset's host state, and the table's counters cleared on the tracker stream ahead of the chain (in
+// stream order: the table's earlier steps and predictions queued before come first).  act_valid = false: the chain rebuilds the active
+// list (chain_prepare's `full` path) and seeds TC from this step's own block.
+static void tracker_restart_host(Tracker& t) {
+  t.th = TrackerHost();
+  t.pred_ok = false;                   // no stamp to predict from until the next step or load
+  t.act_valid = false;
+  t.ids_identity = true;               // the spawn counter restarts at 0 (the retirement switch is kept)
 }
 
-// back end, second half: the measurement lists m[] (complete on `st`, or posting their semaphores there) -> global-frame step, ONE tracker
-// chain for all tables, publication; the tick's events
-static int seq_finish(Ctx* c, SeqTick* t, int bank, cudaStream_t st, const SeqMeas* m, const double* ts, const double* v, const double* yaw) {
+// host form: frames with `stride` floats per point and host lists; device form (host = false): device frames (stride 4) and lists
+static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, int stride, bool host) {
+  if (!ctx || !e) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  if (c->n_seq == 0 || n_seq != c->n_seq) return LMOT_ERR_INVALID;
+  if (c->timing) return LMOT_ERR_STATE;
+  int f0[kMaxBatch + 1];
+  bool rig_on[kMaxBatch];
+  seq_layout(c, f0, rig_on);
+  // validation: nothing is submitted unless the whole tick is valid
+  int S = 0, F = 0, FL = 0;            // stepped sequences, detection frames, lists
+  bool rigged = false, own_det = false;
+  for (int k = 0; k < n_seq; ++k) {
+    const lmot_seq_entry& q = e[k];
+    const int nk = f0[k + 1] - f0[k];
+    if (q.flags & ~LMOT_SEQ_RESTART) return LMOT_ERR_INVALID;
+    if (q.kind == LMOT_SEQ_SKIP) { if (q.flags) return LMOT_ERR_INVALID; continue; }
+    if (q.kind != LMOT_SEQ_FRAMES && q.kind != LMOT_SEQ_LISTS) return LMOT_ERR_INVALID;
+    const bool dev_lists = !host && q.kind == LMOT_SEQ_LISTS;
+    if (!q.data || (dev_lists ? (!q.d_counts || q.cap_per_list < 1) : !q.n)) return LMOT_ERR_INVALID;
+    for (int j = 0; j < nk; ++j) {
+      if (dev_lists) { if (!q.data[j]) return LMOT_ERR_INVALID; continue; }
+      if (q.n[j] < 0 || (q.n[j] > 0 && !q.data[j])) return LMOT_ERR_INVALID;
+      if (!host && q.kind == LMOT_SEQ_FRAMES && q.n[j] > 0 && (reinterpret_cast<uintptr_t>(q.data[j]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies
+    }
+    ++S;
+    if (q.kind == LMOT_SEQ_FRAMES) { F += nk; rigged |= rig_on[k]; own_det |= c->seq_det_on[k]; }
+    else FL += nk;
+  }
+  if (S == 0 || (host && F > 0 && stride < 3)) return LMOT_ERR_INVALID;
+  for (int k = 0; k < n_seq; ++k) {
+    const lmot_seq_entry& q = e[k];
+    if (q.kind == LMOT_SEQ_SKIP || (!host && q.kind == LMOT_SEQ_LISTS)) continue;
+    const int cap = q.kind == LMOT_SEQ_FRAMES ? c->max_points : c->prm.max_boxes;
+    for (int j = 0; j < f0[k + 1] - f0[k]; ++j) if (q.n[j] > cap) return LMOT_ERR_CAPACITY;
+  }
+  if (host && c->seq_in_flight >= c->seq_ring) return LMOT_ERR_STATE;
+  cudaSetDevice(c->device);
   int rc;
-  Slot* k = &c->bank[bank];
-  if (c->prm.global_frame && (rc = seq_global_launch(c, m, c->n_seq, st, ts, v, yaw))) return rc;
-  LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, st));
-  if ((rc = seq_tracker_launch(c, m, t, c->n_seq, ts, v, yaw))) return rc;
+  if (F > 0) {
+    if ((rc = batch_ensure(c, F))) return rc;
+  } else if (!c->bank[0].stream) {     // a tracking tick needs the banks' events and streams, not their detection slots
+    if ((rc = bank_ensure(c))) return rc;
+    LMOT_CUDA(c, cudaDeviceSynchronize());
+  }
+  // the tick's ring slot and bank; the front end runs on the bank's first detection slot's stream (on the bank's own stream when no
+  // sequence sends frames), after the bank's previous tick has been consumed by the tracker
+  SeqTick* t = seq_acquire(c, !host);
+  if (!t) return LMOT_ERR_STATE;
+  const int b = c->next_bank;
+  c->next_bank = (c->next_bank + 1) % kBatchBanks;
+  Slot* bk = &c->bank[b];
+  cudaStream_t st = F > 0 ? c->bslots[b * c->batch_frames].stream : bk->stream;
+  LMOT_CUDA(c, cudaStreamWaitEvent(st, bk->ev_trk_done, 0));
+  if (!host) {                         // device data: ordered after the caller's stream
+    LMOT_CUDA(c, cudaEventRecord(bk->ev_fork, c->stream));
+    LMOT_CUDA(c, cudaStreamWaitEvent(st, bk->ev_fork, 0));
+  }
+  struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
+  const bool gf = c->prm.global_frame != 0;
+  // the map: chain position -> sequence, and per position its measurement list and ego values
+  int seq[kMaxBatch];
+  SeqMeas m[kMaxBatch];
+  double ts[kMaxBatch], v[kMaxBatch], yaw[kMaxBatch];
+  uint32_t stepped = 0;
+  for (int k = 0, p = 0; k < n_seq; ++k) {
+    if (e[k].kind == LMOT_SEQ_SKIP) continue;
+    seq[p] = k; ts[p] = e[k].timestamp_us; v[p] = e[k].v_gps; yaw[p] = e[k].yaw_gps;
+    ++p;
+    stepped |= 1u << k;
+    if (e[k].flags & LMOT_SEQ_RESTART) {
+      tracker_restart_host(c->seq[k]);
+      LMOT_CUDA(c, cudaMemsetAsync(c->seq[k].d_trk_counters, 0, CNT_COUNT * sizeof(int), c->trk_stream));
+    }
+    Result* r = &t->blocks[k];
+    r->n_kev = 0; r->has_tracks = true;
+    // > 0: the concatenation / pack writes the block's per-frame counts; 0: one frame, counts from the header
+    r->batch_frames = (e[k].kind == LMOT_SEQ_LISTS || rigged) ? f0[k + 1] - f0[k] : 0;
+  }
+  t->stepped = stepped;
+  bk->res = &t->blocks[seq[0]];
+  // the stepped sequences' measurement lists, by sequence (gathered by chain position below)
+  SeqMeas mk[kMaxBatch];
+  if (FL > 0) {
+    // LISTS entries: host lists staged at list i * max_boxes boxes of the bank's staging buffer (16-byte aligned), their counts behind the
+    // lists (the copies are ordered after the bank's previous tick, whose pack kernel was the last reader); device lists as they are
+    const int MB = c->prm.max_boxes;
+    float* stage = c->seq_stage[b];
+    int* counts = reinterpret_cast<int*>(stage + (size_t)kMaxBatch * MB * 24);
+    SeqLists L{};
+    int lf0[kMaxBatch + 1], hn[kMaxBatch], fcount = 0, nl = 0;
+    bool lrig[kMaxBatch];
+    lmot_sensor rig[kMaxBatch];
+    int* fc[kMaxBatch];
+    SeqMeas lm[kMaxBatch];
+    lf0[0] = 0;
+    for (int k = 0; k < n_seq; ++k) {
+      if (e[k].kind != LMOT_SEQ_LISTS) continue;
+      for (int j = 0; j < f0[k + 1] - f0[k]; ++j, ++fcount) {
+        const int i = fcount;
+        if (host) {
+          hn[i] = e[k].n[j];
+          if (hn[i] > 0) LMOT_CUDA(c, cudaMemcpyAsync(stage + (size_t)i * MB * 24, e[k].data[j], (size_t)hn[i] * 24 * sizeof(float), cudaMemcpyHostToDevice, st));
+          L.lists[i] = stage + (size_t)i * MB * 24; L.counts[i] = counts + i; L.cap[i] = MB;
+        } else {
+          L.lists[i] = e[k].data[j]; L.counts[i] = e[k].d_counts + j; L.cap[i] = e[k].cap_per_list;
+        }
+        if (rig_on[k]) rig[i] = c->seq_sensors[k][j];
+        else lmot_default_sensor(&c->prm, &rig[i]);
+      }
+      lrig[nl] = rig_on[k];
+      lm[nl] = mk[k] = c->seq_meas[b][k];
+      LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc[nl], t->blocks[k].h_frame_counts, 0));
+      lf0[++nl] = fcount;
+    }
+    if (host) LMOT_CUDA(c, cudaMemcpyAsync(counts, hn, (size_t)FL * sizeof(int), cudaMemcpyHostToDevice, st));
+    if ((rc = boxes_pack_lists_seq_launch(c, st, L, nl, lf0, lrig, rig, lm, fc, !gf))) return rc;
+  }
+  if (F > 0) {
+    // FRAMES entries: the frames of the FRAMES sequences on the bank's detection slots, in sequence order
+    Slot* sl[kMaxBatch];
+    const float4* pp[kMaxBatch];
+    int nn[kMaxBatch], df0[kMaxBatch + 1], dseq[kMaxBatch], nd = 0;
+    bool drig[kMaxBatch];
+    for (int i = 0; i < F; ++i) sl[i] = &c->bslots[b * c->batch_frames + i];
+    df0[0] = 0;
+    for (int k = 0; k < n_seq; ++k) {
+      if (e[k].kind != LMOT_SEQ_FRAMES) continue;
+      for (int j = 0; j < f0[k + 1] - f0[k]; ++j) {
+        const int i = df0[nd] + j;
+        nn[i] = e[k].n[j];
+        if (host) {
+          if ((rc = upload_points(c, sl[i], st, e[k].data[j], nn[i], stride, sl[i]->d_points))) return rc;
+          pp[i] = sl[i]->d_points;
+        } else {
+          pp[i] = reinterpret_cast<const float4*>(e[k].data[j]);
+        }
+      }
+      dseq[nd] = k; drig[nd] = rig_on[k];
+      df0[nd + 1] = df0[nd] + f0[k + 1] - f0[k];
+      ++nd;
+    }
+    sl[0]->res = bk->res;
+    // sequences with their own detection values: every frame of the tick gets its entry (copied into the launch parameters), the values
+    // of its sequence -- or lmot_params' -- with its sensor's four mounting values in place of h_sensor / t_hmin / t_hmax / sensor_height
+    lmot_detect_params det[kMaxBatch];
+    if (own_det) {
+      const lmot_detect_params base = detect_params_of(c->prm);
+      for (int d = 0; d < nd; ++d) {
+        const int k = dseq[d];
+        for (int i = df0[d]; i < df0[d + 1]; ++i) {
+          det[i] = c->seq_det_on[k] ? c->seq_det[k] : base;
+          if (drig[d]) {
+            const lmot_sensor& s = c->seq_sensors[k][i - df0[d]];
+            det[i].h_sensor = s.h_sensor; det[i].t_hmin = s.t_hmin; det[i].t_hmax = s.t_hmax; det[i].sensor_height = s.sensor_height;
+          }
+        }
+      }
+    }
+    if (!rigged) {
+      // detection: the batched launches of lmot_batch_* without a rig; each frame's last box-fitting CTA (or, global_frame, its
+      // boxes_to_global CTA) posts its own slot's semaphore, which the tick's gate kernel polls
+      for (int d = 0; d < nd; ++d) {         // (one frame per sequence: slot df0[d] == d)
+        Slot* s = sl[df0[d]];
+        mk[dseq[d]] = SeqMeas{s->d_boxes, s->d_boxes_g, s->d_counters, s->d_det_sem};
+      }
+      if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, c->fuse_ccl, false, nullptr, own_det ? det : nullptr))) return rc;
+      if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
+      if ((rc = boxfit_launch_batch(c, sl, F, st, nn, !gf, nullptr, own_det ? det : nullptr))) return rc;
+    } else {
+      // detection with one sensor per frame (sequences without a table: lmot_params' values), copied into the launch parameters (later
+      // table changes leave this tick alone); then each sequence's frames into its own list, whose semaphore the gate kernel polls
+      lmot_sensor rig[kMaxBatch];
+      int* fc[kMaxBatch];
+      SeqMeas dm[kMaxBatch];
+      for (int d = 0; d < nd; ++d) {
+        const int k = dseq[d];
+        for (int i = df0[d]; i < df0[d + 1]; ++i) {
+          if (drig[d]) rig[i] = c->seq_sensors[k][i - df0[d]];
+          else lmot_default_sensor(&c->prm, &rig[i]);
+        }
+        dm[d] = mk[k] = c->seq_meas[b][k];
+        LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc[d], t->blocks[k].h_frame_counts, 0));
+      }
+      if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, c->fuse_ccl, false, rig, own_det ? det : nullptr))) return rc;
+      if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
+      if ((rc = boxfit_launch_batch(c, sl, F, st, nn, false, rig, own_det ? det : nullptr))) return rc;
+      if ((rc = boxes_concat_seq_launch(c, sl, nd, df0, drig, rig, dm, fc, !gf, st))) return rc;
+    }
+  }
+  for (int p = 0; p < S; ++p) m[p] = mk[seq[p]];
+  // the measurement lists (complete on `st`, or posting their semaphores there) -> global-frame step, ONE tracker chain for the stepped
+  // tables, publication; the tick's events
+  if (gf && (rc = seq_global_launch(c, seq, m, S, st, ts, v, yaw))) return rc;
+  LMOT_CUDA(c, cudaEventRecord(bk->ev_det_done, st));
+  if ((rc = seq_tracker_launch(c, seq, m, t, S, ts, v, yaw))) return rc;
   LMOT_CUDA(c, cudaEventRecord(t->blocks[0].ev_done, c->pub_stream));
-  LMOT_CUDA(c, cudaEventRecord(k->ev_trk_done, c->pub_stream));
+  LMOT_CUDA(c, cudaEventRecord(bk->ev_trk_done, c->pub_stream));
   if (!t->in_flight) { t->in_flight = true; ++c->seq_in_flight; }
   return LMOT_OK;
 }
 
-// detection front end (lmot_seq_submit / lmot_seq_dev)
-static int seq_common(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride, bool host, const double* ts,
-                      const double* v, const double* yaw) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  if (c->n_seq == 0 || n_seq != c->n_seq || !points || !n || !ts || !v || !yaw) return LMOT_ERR_INVALID;
-  if (c->timing) return LMOT_ERR_STATE;
-  cudaSetDevice(c->device);
+// lmot_seq_submit / lmot_seq_dev: every sequence steps from its frames (points / n in the set's frame layout)
+static int seq_frames_tick(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride, bool host, const double* ts,
+                           const double* v, const double* yaw) {
+  if (!ctx || ctx->c.n_seq == 0 || n_seq != ctx->c.n_seq || !points || !n || !ts || !v || !yaw) return LMOT_ERR_INVALID;
   int f0[kMaxBatch + 1];
   bool rig_on[kMaxBatch];
-  const bool rigged = seq_layout(c, f0, rig_on);
-  const int F = f0[n_seq];
-  for (int i = 0; i < F; ++i) {
-    if (n[i] < 0 || (n[i] > 0 && !points[i])) return LMOT_ERR_INVALID;
-    if (n[i] > c->max_points) return LMOT_ERR_CAPACITY;
-    if (!host && n[i] > 0 && (reinterpret_cast<uintptr_t>(points[i]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies need 16-byte alignment
-  }
-  if (host && (stride < 3 || c->seq_in_flight >= c->seq_ring)) return stride < 3 ? LMOT_ERR_INVALID : LMOT_ERR_STATE;
-  int rc = batch_ensure(c, F);
-  if (rc) return rc;
-  SeqTick* t;
-  int b;
-  cudaStream_t st;
-  if ((rc = seq_begin(c, !host, false, &t, &b, &st))) return rc;
-  Slot* k = &c->bank[b];
-  Slot* sl[kMaxBatch];
-  const float4* pp[kMaxBatch];
-  for (int i = 0; i < F; ++i) sl[i] = &c->bslots[b * c->batch_frames + i];
-  // device frames: ordered after the caller's stream
-  if (host) {
-    for (int i = 0; i < F; ++i) {
-      if ((rc = upload_points(c, sl[i], st, points[i], n[i], stride, sl[i]->d_points))) return rc;
-      pp[i] = sl[i]->d_points;
-    }
-  } else {
-    LMOT_CUDA(c, cudaEventRecord(k->ev_fork, c->stream));
-    LMOT_CUDA(c, cudaStreamWaitEvent(st, k->ev_fork, 0));
-    for (int i = 0; i < F; ++i) pp[i] = reinterpret_cast<const float4*>(points[i]);
-  }
-  struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
-  for (int i = 0; i < n_seq; ++i) {
-    t->blocks[i].n_kev = 0; t->blocks[i].has_tracks = true;
-    t->blocks[i].batch_frames = rigged ? f0[i + 1] - f0[i] : 0;     // > 0: the concatenation writes the block's per-frame counts
-  }
-  k->res = &t->blocks[0]; sl[0]->res = &t->blocks[0];
-  const bool gf = c->prm.global_frame != 0;
-  SeqMeas m[kMaxBatch];
-  // sequences with their own detection values: every frame of the tick gets its entry (copied into the launch parameters), the values
-  // of its sequence -- or lmot_params' -- with its sensor's four mounting values in place of h_sensor / t_hmin / t_hmax / sensor_height
-  bool own_det = false;
-  for (int i = 0; i < n_seq; ++i) own_det |= c->seq_det_on[i];
-  lmot_detect_params det[kMaxBatch];
-  if (own_det) {
-    const lmot_detect_params base = detect_params_of(c->prm);
-    for (int i = 0; i < n_seq; ++i)
-      for (int j = f0[i]; j < f0[i + 1]; ++j) {
-        det[j] = c->seq_det_on[i] ? c->seq_det[i] : base;
-        if (rig_on[i]) {
-          const lmot_sensor& e = c->seq_sensors[i][j - f0[i]];
-          det[j].h_sensor = e.h_sensor; det[j].t_hmin = e.t_hmin; det[j].t_hmax = e.t_hmax; det[j].sensor_height = e.sensor_height;
-        }
-      }
-  }
-  if (!rigged) {
-    // detection: the batched launches of lmot_batch_* without a rig; each frame's last box-fitting CTA (or, global_frame, its
-    // boxes_to_global CTA) posts its own slot's semaphore, which the tick's gate kernel polls
-    for (int i = 0; i < n_seq; ++i) m[i] = SeqMeas{sl[i]->d_boxes, sl[i]->d_boxes_g, sl[i]->d_counters, sl[i]->d_det_sem};
-    if ((rc = ground_launch_batch(c, sl, n_seq, pp, n, st, true, false, c->fuse_ccl, false, nullptr, own_det ? det : nullptr))) return rc;
-    if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, n_seq, st))) return rc;
-    if ((rc = boxfit_launch_batch(c, sl, n_seq, st, n, !gf, nullptr, own_det ? det : nullptr))) return rc;
-  } else {
-    // detection with one sensor per frame (sequences without a table: lmot_params' values), copied into the launch parameters (later
-    // table changes leave this tick alone); then each sequence's frames into its own list, whose semaphore the gate kernel polls
-    lmot_sensor rig[kMaxBatch];
-    int* fc[kMaxBatch];
-    for (int i = 0; i < n_seq; ++i) {
-      for (int j = f0[i]; j < f0[i + 1]; ++j) {
-        if (rig_on[i]) rig[j] = c->seq_sensors[i][j - f0[i]];
-        else lmot_default_sensor(&c->prm, &rig[j]);
-      }
-      m[i] = c->seq_meas[b][i];
-      LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc[i], t->blocks[i].h_frame_counts, 0));
-    }
-    if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, c->fuse_ccl, false, rig, own_det ? det : nullptr))) return rc;
-    if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
-    if ((rc = boxfit_launch_batch(c, sl, F, st, n, false, rig, own_det ? det : nullptr))) return rc;
-    if ((rc = boxes_concat_seq_launch(c, sl, n_seq, f0, rig_on, rig, m, fc, !gf, st))) return rc;
-  }
-  return seq_finish(c, t, b, st, m, ts, v, yaw);
+  seq_layout(&ctx->c, f0, rig_on);
+  lmot_seq_entry e[kMaxBatch];
+  for (int k = 0; k < n_seq; ++k) e[k] = lmot_seq_entry{LMOT_SEQ_FRAMES, 0, ts[k], v[k], yaw[k], points + f0[k], n + f0[k], nullptr, 0};
+  return seq_tick_common(ctx, e, n_seq, stride, host);
 }
 
-// tracking-only front end (lmot_seq_track_submit / lmot_seq_track_dev): host lists (boxes / m, staged on the device first) or padded
-// device lists (d_lists / d_counts, cap boxes each) -> pack_lists_seq_kernel into each sequence's measurement list on the bank
-static int seq_lists_common(lmot_ctx* ctx, const float* const* boxes, const int* m, const float* d_lists, const int* d_counts, int cap, int n_seq,
-                            bool host, const double* ts, const double* v, const double* yaw) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  if (c->n_seq == 0 || n_seq != c->n_seq || !ts || !v || !yaw) return LMOT_ERR_INVALID;
+// lmot_seq_track_submit / lmot_seq_track_dev: every sequence steps from its lists (host lists boxes / m, or padded device lists d_lists /
+// d_counts of cap boxes each, in the set's frame layout)
+static int seq_lists_tick(lmot_ctx* ctx, const float* const* boxes, const int* m, const float* d_lists, const int* d_counts, int cap, int n_seq,
+                          bool host, const double* ts, const double* v, const double* yaw) {
+  if (!ctx || ctx->c.n_seq == 0 || n_seq != ctx->c.n_seq || !ts || !v || !yaw) return LMOT_ERR_INVALID;
   if (host ? (!boxes || !m) : (!d_lists || !d_counts || cap < 1)) return LMOT_ERR_INVALID;
-  if (c->timing) return LMOT_ERR_STATE;
-  cudaSetDevice(c->device);
   int f0[kMaxBatch + 1];
   bool rig_on[kMaxBatch];
-  seq_layout(c, f0, rig_on);
-  const int F = f0[n_seq];
-  if (host) {
-    for (int i = 0; i < F; ++i) if (m[i] < 0 || (m[i] > 0 && !boxes[i])) return LMOT_ERR_INVALID;
-    for (int i = 0; i < F; ++i) if (m[i] > c->prm.max_boxes) return LMOT_ERR_CAPACITY;
-    if (c->seq_in_flight >= c->seq_ring) return LMOT_ERR_STATE;
-  }
-  int rc;
-  if (!c->bank[0].stream) {            // a tracking tick needs the banks' events and streams, not their detection slots
-    if ((rc = bank_ensure(c))) return rc;
-    LMOT_CUDA(c, cudaDeviceSynchronize());
-  }
-  SeqTick* t;
-  int b;
-  cudaStream_t st;
-  if ((rc = seq_begin(c, !host, true, &t, &b, &st))) return rc;
-  struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
-  if (host) {
-    // list i at i * max_boxes boxes of the bank's staging buffer (16-byte aligned), the counts behind the lists.  The copies are
-    // ordered after the bank's previous tick (seq_begin), whose pack kernel was the last reader.
-    const int MB = c->prm.max_boxes;
-    float* stage = c->seq_stage[b];
-    int* counts = reinterpret_cast<int*>(stage + (size_t)kMaxBatch * MB * 24);
-    for (int i = 0; i < F; ++i)
-      if (m[i] > 0) LMOT_CUDA(c, cudaMemcpyAsync(stage + (size_t)i * MB * 24, boxes[i], (size_t)m[i] * 24 * sizeof(float), cudaMemcpyHostToDevice, st));
-    LMOT_CUDA(c, cudaMemcpyAsync(counts, m, (size_t)F * sizeof(int), cudaMemcpyHostToDevice, st));
-    d_lists = stage; d_counts = counts; cap = MB;
-  } else {
-    LMOT_CUDA(c, cudaEventRecord(c->bank[b].ev_fork, c->stream));      // the caller's stream produced the lists
-    LMOT_CUDA(c, cudaStreamWaitEvent(st, c->bank[b].ev_fork, 0));
-  }
-  // sequence k's lists: poses of its table (copied into the launch parameters), its measurement list on the bank, per-list counts into
-  // its result block
-  lmot_sensor rig[kMaxBatch];
-  int* fc[kMaxBatch];
-  SeqMeas mm[kMaxBatch];
-  for (int k = 0; k < n_seq; ++k) {
-    for (int j = f0[k]; j < f0[k + 1]; ++j) {
-      if (rig_on[k]) rig[j] = c->seq_sensors[k][j - f0[k]];
-      else lmot_default_sensor(&c->prm, &rig[j]);
-    }
-    mm[k] = c->seq_meas[b][k];
-    Result* r = &t->blocks[k];
-    r->n_kev = 0; r->has_tracks = true;
-    r->batch_frames = f0[k + 1] - f0[k];
-    LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc[k], r->h_frame_counts, 0));
-  }
-  const bool gf = c->prm.global_frame != 0;
-  if ((rc = boxes_pack_lists_seq_launch(c, st, d_lists, d_counts, cap, n_seq, f0, rig_on, rig, mm, fc, !gf))) return rc;
-  return seq_finish(c, t, b, st, mm, ts, v, yaw);
+  seq_layout(&ctx->c, f0, rig_on);
+  const float* lp[kMaxBatch];
+  for (int i = 0; !host && i < f0[n_seq]; ++i) lp[i] = d_lists + (size_t)i * cap * 24;
+  lmot_seq_entry e[kMaxBatch];
+  for (int k = 0; k < n_seq; ++k)
+    e[k] = host ? lmot_seq_entry{LMOT_SEQ_LISTS, 0, ts[k], v[k], yaw[k], boxes + f0[k], m + f0[k], nullptr, 0}
+                : lmot_seq_entry{LMOT_SEQ_LISTS, 0, ts[k], v[k], yaw[k], lp + f0[k], nullptr, d_counts + f0[k], cap};
+  return seq_tick_common(ctx, e, n_seq, 0, host);
 }
 
 // uncollected ticks are dropped, as lmot_batch drops uncollected results
@@ -1310,12 +1379,12 @@ static int seq_drop_uncollected(Ctx* c) {
 
 int lmot_seq_submit(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride_floats, const double* timestamp_us,
                     const double* v_gps, const double* yaw_gps) {
-  return seq_common(ctx, points, n, n_seq, stride_floats, true, timestamp_us, v_gps, yaw_gps);
+  return seq_frames_tick(ctx, points, n, n_seq, stride_floats, true, timestamp_us, v_gps, yaw_gps);
 }
 
 int lmot_seq_dev(lmot_ctx* ctx, const float* const* d_points, const int* n, int n_seq, const double* timestamp_us, const double* v_gps,
                  const double* yaw_gps) {
-  return seq_common(ctx, d_points, n, n_seq, 4, false, timestamp_us, v_gps, yaw_gps);
+  return seq_frames_tick(ctx, d_points, n, n_seq, 4, false, timestamp_us, v_gps, yaw_gps);
 }
 
 int lmot_seq_collect(lmot_ctx* ctx, lmot_seq_out* out) {
@@ -1354,12 +1423,12 @@ int lmot_seq(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq,
 
 int lmot_seq_track_submit(lmot_ctx* ctx, const float* const* boxes, const int* m, int n_seq, const double* timestamp_us, const double* v_gps,
                           const double* yaw_gps) {
-  return seq_lists_common(ctx, boxes, m, nullptr, nullptr, 0, n_seq, true, timestamp_us, v_gps, yaw_gps);
+  return seq_lists_tick(ctx, boxes, m, nullptr, nullptr, 0, n_seq, true, timestamp_us, v_gps, yaw_gps);
 }
 
 int lmot_seq_track_dev(lmot_ctx* ctx, const float* d_lists, const int* d_counts, int n_seq, int cap_per_list, const double* timestamp_us,
                        const double* v_gps, const double* yaw_gps) {
-  return seq_lists_common(ctx, nullptr, nullptr, d_lists, d_counts, cap_per_list, n_seq, false, timestamp_us, v_gps, yaw_gps);
+  return seq_lists_tick(ctx, nullptr, nullptr, d_lists, d_counts, cap_per_list, n_seq, false, timestamp_us, v_gps, yaw_gps);
 }
 
 int lmot_seq_track(lmot_ctx* ctx, const float* const* boxes, const int* m, int n_seq, const double* timestamp_us, const double* v_gps,
@@ -1370,6 +1439,29 @@ int lmot_seq_track(lmot_ctx* ctx, const float* const* boxes, const int* m, int n
   rc = lmot_seq_track_submit(ctx, boxes, m, n_seq, timestamp_us, v_gps, yaw_gps);
   if (rc) return rc;
   return lmot_seq_collect(ctx, out);
+}
+
+int lmot_seq_tick_submit(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, int stride_floats) {
+  return seq_tick_common(ctx, e, n_seq, stride_floats, true);
+}
+
+int lmot_seq_tick_dev(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq) {
+  return seq_tick_common(ctx, e, n_seq, 4, false);
+}
+
+int lmot_seq_tick(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, int stride_floats, lmot_seq_out* out) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  int rc = seq_drop_uncollected(&ctx->c);
+  if (rc) return rc;
+  rc = lmot_seq_tick_submit(ctx, e, n_seq, stride_floats);
+  if (rc) return rc;
+  return lmot_seq_collect(ctx, out);
+}
+
+int lmot_seq_stepped(const lmot_ctx* ctx, uint32_t* mask) {
+  if (!ctx || !mask) return LMOT_ERR_INVALID;
+  *mask = ctx->c.seq_stepped;
+  return LMOT_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- device-side hand-over (multi-GPU)
@@ -1631,10 +1723,7 @@ int lmot_origin_points(lmot_ctx* ctx, double timestamp_us, double v_gps, double 
 static int tracker_reset(Ctx* c, Tracker& t) {
   int rc = drain(c);
   if (rc) return rc;
-  t.th = TrackerHost();
-  t.pred_ok = false;                   // no stamp to predict from until the next step or load
-  t.act_valid = false;
-  t.ids_identity = true;               // the spawn counter restarts at 0 (the retirement switch is kept)
+  tracker_restart_host(t);
   LMOT_CUDA(c, cudaMemsetAsync(t.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
   return LMOT_OK;

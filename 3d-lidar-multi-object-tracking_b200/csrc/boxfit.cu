@@ -612,20 +612,32 @@ int boxes_concat_seq_launch(Ctx* c, Slot* const* slots, int S, const int* f0, co
   return LMOT_OK;
 }
 
-// padded device box lists [f0, f0 + n_lists) (capacity cap boxes each, lengths in counts) -> one contiguous list + the counter block
-// the tracker reads (multi-GPU hand-over: the lists arrived by ncclAllGather; tracking-only sequence ticks: one sequence's lists).
-// kRig: list f0 + l's boxes moved by pose R->m[f0 + l].  Optional outputs of sequence ticks: frame_counts row l = (0, 0, 0, list
-// f0 + l's clamped length), det_sem posted once the list is complete.
-template <bool kRig>
-__device__ __forceinline__ void pack_lists_body(const RigPoses* R, const float* __restrict__ lists, const int* __restrict__ counts, int f0, int n_lists,
-                                                int cap, int max_boxes, float* __restrict__ boxes, int* __restrict__ counters,
-                                                int* __restrict__ frame_counts = nullptr, int* __restrict__ det_sem = nullptr) {
+// device box lists [f0, f0 + n_lists) of `src` (src.list(i): list i's boxes, src.count(i): its length clamped to its capacity) -> one
+// contiguous list + the counter block the tracker reads (multi-GPU hand-over: the lists arrived by ncclAllGather; sequence ticks: one
+// sequence's lists).  kRig: list f0 + l's boxes moved by pose R->m[f0 + l].  Optional outputs of sequence ticks: frame_counts row l =
+// (0, 0, 0, list f0 + l's clamped length), det_sem posted once the list is complete.
+// padded lists (one buffer, `cap` boxes per list)
+struct PaddedLists {
+  const float* lists; const int* counts; int cap;
+  __device__ const float* list(int i) const { return lists + (size_t)i * cap * 24; }
+  __device__ int count(int i) const { return min(max(counts[i], 0), cap); }
+};
+// a pointer and a length pointer per list (SeqLists in the parameter block)
+struct PtrLists {
+  const SeqLists* L;
+  __device__ const float* list(int i) const { return L->lists[i]; }
+  __device__ int count(int i) const { return min(max(*L->counts[i], 0), L->cap[i]); }
+};
+
+template <bool kRig, class Src>
+__device__ __forceinline__ void pack_lists_body(const RigPoses* R, const Src& src, int f0, int n_lists, int max_boxes, float* __restrict__ boxes,
+                                                int* __restrict__ counters, int* __restrict__ frame_counts = nullptr, int* __restrict__ det_sem = nullptr) {
   __shared__ int s_off[kMaxBatch + 1];
   if (threadIdx.x == 0) {
     int acc = 0;
     for (int l = 0; l < n_lists; ++l) {
       s_off[l] = acc;
-      const int n = min(max(counts[f0 + l], 0), cap);
+      const int n = src.count(f0 + l);
       acc += n;
       if (frame_counts) { frame_counts[4 * l] = 0; frame_counts[4 * l + 1] = 0; frame_counts[4 * l + 2] = 0; frame_counts[4 * l + 3] = n; }
     }
@@ -637,16 +649,16 @@ __device__ __forceinline__ void pack_lists_body(const RigPoses* R, const float* 
   __syncthreads();
   for (int l = 0; l < n_lists; ++l) {
     const int off = s_off[l], cnt = min(s_off[l + 1], max_boxes) - off;
-    const float* src = lists + (size_t)(f0 + l) * cap * 24;
+    const float* lst = src.list(f0 + l);
     if (!kRig) {
-      for (int e = threadIdx.x; e < cnt * 24; e += 256) boxes[(size_t)off * 24 + e] = src[e];
+      for (int e = threadIdx.x; e < cnt * 24; e += 256) boxes[(size_t)off * 24 + e] = lst[e];
     } else {
       // a whole box per thread: its 24 floats in flight (the caller's lists need only 4-byte alignment), then the pose
       const float* m = R->m[f0 + l];
       for (int j = threadIdx.x; j < cnt; j += 256) {
         float b[24];
 #pragma unroll
-        for (int u = 0; u < 24; ++u) b[u] = src[(size_t)j * 24 + u];
+        for (int u = 0; u < 24; ++u) b[u] = lst[(size_t)j * 24 + u];
         rig_apply_box(m, b);
         float4* d = reinterpret_cast<float4*>(boxes + (size_t)(off + j) * 24);
 #pragma unroll
@@ -666,27 +678,27 @@ __device__ __forceinline__ void pack_lists_body(const RigPoses* R, const float* 
 __global__ void __launch_bounds__(256)
 pack_lists_kernel(const float* __restrict__ lists, const int* __restrict__ counts, int n_lists, int cap, int max_boxes, float* __restrict__ boxes,
                   int* __restrict__ counters) {
-  pack_lists_body<false>(nullptr, lists, counts, 0, n_lists, cap, max_boxes, boxes, counters);
+  pack_lists_body<false>(nullptr, PaddedLists{lists, counts, cap}, 0, n_lists, max_boxes, boxes, counters);
 }
 
 __global__ void __launch_bounds__(256)
 pack_lists_rig_kernel(const __grid_constant__ RigPoses R, const float* __restrict__ lists, const int* __restrict__ counts, int n_lists, int cap,
                       int max_boxes, float* __restrict__ boxes, int* __restrict__ counters) {
-  pack_lists_body<true>(&R, lists, counts, 0, n_lists, cap, max_boxes, boxes, counters);
+  pack_lists_body<true>(&R, PaddedLists{lists, counts, cap}, 0, n_lists, max_boxes, boxes, counters);
 }
 
-// tracking-only sequence ticks (lmot_seq_track*): CTA k packs sequence k's lists [f0, f0 + n_lists) into the sequence's own measurement
-// list.  A sequence with a table moves each box by its sensor's pose; a sequence without one has a single list, copied unchanged.
+// LISTS entries of sequence ticks: CTA k packs position k's lists [f0, f0 + n_lists) of P.L into that sequence's own measurement list.  A
+// sequence with a table moves each box by its sensor's pose; a sequence without one has a single list, copied unchanged.
 // det_sem: posted after the list is complete (nullptr with global_frame: boxes_to_global_seq_kernel posts it).
 struct PackSeq { int f0, n_lists, rig; float* boxes; int* counters; int* frame_counts; int* det_sem; };
-struct PackSeqParams { PackSeq s[kMaxBatch]; };
+struct PackSeqParams { PackSeq s[kMaxBatch]; SeqLists L; };
 
 __global__ void __launch_bounds__(256)
-pack_lists_seq_kernel(const __grid_constant__ RigPoses R, const __grid_constant__ PackSeqParams P, const float* __restrict__ lists,
-                      const int* __restrict__ counts, int cap, int max_boxes) {
+pack_lists_seq_kernel(const __grid_constant__ RigPoses R, const __grid_constant__ PackSeqParams P, int max_boxes) {
   const PackSeq& q = P.s[blockIdx.x];
-  if (q.rig) pack_lists_body<true>(&R, lists, counts, q.f0, q.n_lists, cap, max_boxes, q.boxes, q.counters, q.frame_counts, q.det_sem);
-  else pack_lists_body<false>(nullptr, lists, counts, q.f0, q.n_lists, cap, max_boxes, q.boxes, q.counters, q.frame_counts, q.det_sem);
+  const PtrLists src{&P.L};
+  if (q.rig) pack_lists_body<true>(&R, src, q.f0, q.n_lists, max_boxes, q.boxes, q.counters, q.frame_counts, q.det_sem);
+  else pack_lists_body<false>(nullptr, src, q.f0, q.n_lists, max_boxes, q.boxes, q.counters, q.frame_counts, q.det_sem);
 }
 
 int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int n_lists, int cap, float* d_boxes, int* d_counters,
@@ -702,10 +714,10 @@ int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const
   return LMOT_OK;
 }
 
-// tracking-only sequence ticks: sequence k's lists [f0[k], f0[k + 1]) of d_lists / d_counts -> m[k]'s list and counters, per-list counts
-// into frame_counts[k] (device view of the tick's pinned block k).  rig: one entry per list of the tick; sequence k's poses apply iff rig_on[k].
-int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int cap, int S, const int* f0, const bool* rig_on,
-                                const lmot_sensor* rig, const SeqMeas* m, int* const* frame_counts, bool post_sem) {
+// LISTS entries of sequence ticks: position k's lists [f0[k], f0[k + 1]) of L -> m[k]'s list and counters, per-list counts into
+// frame_counts[k] (device view of that sequence's pinned result block).  rig: one entry per list; position k's poses apply iff rig_on[k].
+int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const SeqLists& L, int S, const int* f0, const bool* rig_on, const lmot_sensor* rig,
+                                const SeqMeas* m, int* const* frame_counts, bool post_sem) {
   const int F = f0[S];
   if (S < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   RigPoses R;
@@ -713,7 +725,8 @@ int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const float* d_lists, c
   PackSeqParams P{};
   for (int k = 0; k < S; ++k)
     P.s[k] = PackSeq{f0[k], f0[k + 1] - f0[k], rig_on[k] ? 1 : 0, m[k].d_boxes, m[k].d_counters, frame_counts[k], post_sem ? m[k].d_det_sem : nullptr};
-  pack_lists_seq_kernel<<<S, 256, 0, st>>>(R, P, d_lists, d_counts, cap, c->prm.max_boxes);
+  P.L = L;
+  pack_lists_seq_kernel<<<S, 256, 0, st>>>(R, P, c->prm.max_boxes);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
 }

@@ -271,9 +271,15 @@ struct Tracker {
 // set, the bank's per-sequence lists (Ctx::seq_meas) that concat_boxes_seq_kernel fills.
 struct SeqMeas { float* d_boxes = nullptr; float* d_boxes_g = nullptr; int* d_counters = nullptr; int* d_det_sem = nullptr; };
 
-// one tick of lmot_seq_*: a result block per sequence; blocks[0].ev_done marks the whole tick published
+// the box lists of a sequence tick's LISTS entries, in tick order: list i at lists[i] (device), its length in the device int counts[i],
+// clamped to [0, cap[i]] (api.cu seq_tick_common: the staged host lists, or the caller's device lists)
+struct SeqLists { const float* lists[kMaxBatch]; const int* counts[kMaxBatch]; int cap[kMaxBatch]; };
+
+// one tick of lmot_seq_*: a result block per sequence; blocks[0].ev_done marks the whole tick published.  Only the stepped sequences'
+// blocks are written: blocks[k] of a sequence the tick skipped still holds that sequence's step of an earlier tick on this ring slot.
 struct SeqTick {
   Result blocks[kMaxBatch];
+  uint32_t stepped = 0;                // bit k: sequence k stepped in this tick
   bool in_flight = false;
 };
 
@@ -329,7 +335,8 @@ struct Ctx {
   SeqTick* seq_ticks = nullptr;        // [seq_ring]
   int seq_ring = 0, seq_next = 0, seq_oldest = 0, seq_in_flight = 0;
   SeqTick* seq_last = nullptr;         // most recent submission (lmot_seq_fetch)
-  bool seq_wide = false;               // spawn_output_kernel's variant of the sequence ticks (largest last_n_act of the set)
+  uint32_t seq_stepped = 0;            // lmot_seq_stepped: the stepped mask of the tick most recently returned
+  bool seq_wide = false;               // spawn_output_kernel's variant of the sequence ticks (largest last_n_act of the stepped tables)
   // sensor tables of the sequences (lmot_seq_set_sensors): sequence k's frames of a tick are its sensors in table order; 0 sensors: one
   // frame with lmot_params' thresholds.  Read at submission; the context's own table (sensors[]) never applies to sequence ticks.
   int seq_n_sensors[kMaxBatch] = {};
@@ -438,12 +445,13 @@ int tracker_publish(Ctx* c, Result* r, cudaStream_t st);            // device bl
 // sequence ticks with sensor tables: sequence k's frames [f0[k], f0[k + 1]) of `slots` -> m[k] (boxfit.cu)
 int boxes_concat_seq_launch(Ctx* c, Slot* const* slots, int S, const int* f0, const bool* rig_on, const lmot_sensor* rig, const SeqMeas* m,
                             int* const* frame_counts, bool post_sem, cudaStream_t st);
-// tracking-only sequence ticks: sequence k's padded lists [f0[k], f0[k + 1]) of d_lists (cap boxes each, lengths in d_counts) -> m[k] (boxfit.cu)
-int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int cap, int S, const int* f0, const bool* rig_on,
-                                const lmot_sensor* rig, const SeqMeas* m, int* const* frame_counts, bool post_sem);
-// sequence ticks: measurement list m[k] -> track table c->seq[k] -> tick->blocks[k] (tracker.cu)
-int seq_global_launch(Ctx* c, const SeqMeas* m, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw);
-int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw);
+// LISTS entries of sequence ticks: position k's lists [f0[k], f0[k + 1]) of L -> m[k] (boxfit.cu)
+int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const SeqLists& L, int S, const int* f0, const bool* rig_on, const lmot_sensor* rig,
+                                const SeqMeas* m, int* const* frame_counts, bool post_sem);
+// sequence ticks over the S stepped sequences: chain position k is sequence seq[k]; measurement list m[k] and ego values ts / v / yaw[k]
+// are indexed by position -> track table c->seq[seq[k]] -> tick->blocks[seq[k]] (tracker.cu)
+int seq_global_launch(Ctx* c, const int* seq, const SeqMeas* m, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw);
+int seq_tracker_launch(Ctx* c, const int* seq, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw);
 // track prediction of S tables (1..kMaxBatch) at n_t times each (t_us[k * n_t + j]) into outs[k] (device arrays), row counts into
 // d_n_rows[k] (nullable), on stream st behind the tables' latest steps; records c->ev_pred after the kernel (tracker.cu)
 int predict_launch(Ctx* c, Tracker* const* tabs, int S, const double* t_us, int n_t, const lmot_pred_out* outs, int* const* d_n_rows,

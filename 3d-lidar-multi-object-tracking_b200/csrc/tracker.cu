@@ -2301,12 +2301,12 @@ int boxes_publish(Ctx* c, Slot* s, Result* r, cudaStream_t st) {
 // Sequence k of a tick: measurement list m[k] (box list, counters, semaphore), track table c->seq[k], result block tick->blocks[k].
 // Every launch below covers all S sequences; per-sequence arguments travel in __grid_constant__ parameter blocks.
 
-// global_frame: sequence k's sensor- (or vehicle-) frame boxes -> m[k].d_boxes_g with THIS tick's ego pose of sequence k (peeked:
+// global_frame: position k's sensor- (or vehicle-) frame boxes -> m[k].d_boxes_g with THIS tick's ego pose of sequence seq[k] (peeked:
 // seq_tracker_launch folds it), posting m[k]'s detection semaphore
-int seq_global_launch(Ctx* c, const SeqMeas* m, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw) {
+int seq_global_launch(Ctx* c, const int* seq, const SeqMeas* m, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw) {
   GlobalSeqParams p{};
   for (int k = 0; k < S; ++k) {
-    TrackerHost peek = c->seq[k].th;
+    TrackerHost peek = c->seq[seq[k]].th;
     origin_points_fold(peek, ts[k], v[k], yaw[k]);
     Xf2 back;
     global_frame_xf(peek.egoPoint, &p.s[k].fwd, &back);
@@ -2317,12 +2317,12 @@ int seq_global_launch(Ctx* c, const SeqMeas* m, int S, cudaStream_t st, const do
   return LMOT_OK;
 }
 
-// gate -> TA -> TB -> TC once for all S sequences on the tracker stream (chain_launch), then one publish launch on the publish stream.
-// The caller records the tick's events on the publish stream afterwards.
-int seq_tracker_launch(Ctx* c, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw) {
+// gate -> TA -> TB -> TC once for the S stepped sequences on the tracker stream (chain_launch), then one publish launch on the publish
+// stream.  The caller records the tick's events on the publish stream afterwards.
+int seq_tracker_launch(Ctx* c, const int* seq, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw) {
   Chain ch(c);
   for (int k = 0; k < S; ++k)
-    if (int rc = chain_prepare(c, c->seq[k], m[k], &tick->blocks[k], c->trk_stream, ts[k], v[k], yaw[k], ch)) return rc;
+    if (int rc = chain_prepare(c, c->seq[seq[k]], m[k], &tick->blocks[seq[k]], c->trk_stream, ts[k], v[k], yaw[k], ch)) return rc;
   if (int rc = chain_launch(c, ch, c->trk_stream, false, ChainGate::seq, true, nullptr, true)) return rc;
   publish_seq_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(ch.pub);
   if (ch.ids_on) publish_ids_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(ch.ids);

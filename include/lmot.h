@@ -374,7 +374,8 @@ int lmot_seq_frame_counts(lmot_ctx* ctx, int k, int counts[LMOT_MAX_BATCH][4], i
  *
  * Ticks use the ring of lmot_seq_*: lmot_seq_collect / lmot_seq_fetch, the same LMOT_ERR_STATE (host lists) and drop-oldest (device
  * lists) rules.  A set may mix detection ticks (lmot_seq*) and tracking ticks in any order; each table folds its steps in submission
- * order.  One tick is all-detection or all-tracking: a tick that feeds some sequences frames and others box lists is not supported.
+ * order.  One lmot_seq* / lmot_seq_track* tick is all-detection or all-tracking and steps every sequence; lmot_seq_tick_* (below)
+ * mixes the two kinds and steps any subset.
  * lmot_seq_track_submit: HOST lists boxes[i] of m[i] boxes.  LMOT_ERR_CAPACITY, nothing submitted: a list above max_boxes.  The
  *   lists and m are copied to a device staging buffer of the bank during the call (copies from pageable memory complete before the
  *   call returns; page-locked lists must stay untouched until lmot_flush has joined or the tick has been collected).
@@ -398,6 +399,58 @@ int lmot_seq_track(lmot_ctx* ctx, const float* const* boxes, const int* m, int n
 int lmot_seq_tracker_load(lmot_ctx* ctx, int k, const double* dumps, int n, int init, double timestamp_us, double ego_velo,
                           double ego_yaw, double ego_pre_yaw, double ego_point_yaw);
 int lmot_seq_tracker_set_ego(lmot_ctx* ctx, int k, const double ego8[8]);
+
+/* ---- sequence ticks on each stream's own clock: any subset of the sequences, each from frames or box lists, restart in place ------
+ * A tick describes each of the n_seq sequences with one lmot_seq_entry: LMOT_SEQ_SKIP (the sequence has no data this tick and does not
+ * step), LMOT_SEQ_FRAMES (its frames: one per sensor of its table, or one without a table) or LMOT_SEQ_LISTS (its box lists, in the same
+ * layout).  ONE tracker chain steps the stepped sequences' tables.  Streams at different rates, dropped frames, logs of different
+ * lengths, and vehicles that send point clouds next to vehicles that send their own detector's boxes thus share one set and one chain.
+ *
+ * Equivalence: over any schedule of ticks, sequence k gives bit for bit what a separate context with the same lmot_params, tracker
+ * parameters, retirement setting and detection parameters gives when it receives only sequence k's steps, in order, and nothing at
+ * skipped ticks: a FRAMES step through lmot_frame (lmot_set_sensors(table) + lmot_batch with a table), a LISTS step through
+ * lmot_track_step (lmot_track_step_lists_dev with the table).  This covers the counts, the boxes, every track output, the status,
+ * lmot_seq_tracker_dump, lmot_seq_track_ids and lmot_seq_tracker_get_ego, with global_frame 0 or 1.  A sequence may switch kinds
+ * from tick to tick.
+ *
+ * A skipped sequence is untouched: table, ego fold, stamp, first-frame flag, prediction stamp and IDs.  Its out->seq[k] is not written
+ * (no count field, no caller buffer); lmot_seq_frame_counts(k) reports 0 frames for that tick; lmot_seq_track_ids(k) keeps the IDs of
+ * its last returned step.  lmot_seq_stepped: bit k set iff sequence k stepped in the tick most recently returned by lmot_seq_collect /
+ * lmot_seq_fetch / lmot_seq* (every bit of the set for lmot_seq* and lmot_seq_track* ticks).  The tick's status is the first error of
+ * its stepped sequences, else their first warning.
+ *
+ * LMOT_SEQ_RESTART: the sequence first does what lmot_seq_tracker_reset(k) does -- empties its table, resets its ego state and
+ * first-frame flag (the oracle_compat_first_frame quirk applies again), numbers its IDs from 0 -- then steps.  In stream order: nothing
+ * is drained, other sequences' ticks stay in flight and their uncollected results are kept; a prediction queued before the tick sees the
+ * old table.  Sensor tables, tracker and detection parameters and retirement are host state captured at submission, so a new stream on
+ * sequence k is configured before its restarting tick without a drain.  lmot_seq_tracker_reset / _load / _set_ego still drain.
+ *
+ * Ticks use the ring of lmot_seq_* and mix freely with lmot_seq* and lmot_seq_track* ticks; each table folds its steps in submission
+ * order.  lmot_seq_tick_submit: host data (frames with stride_floats, lists staged as lmot_seq_track_submit stages them);
+ * LMOT_ERR_STATE when `ring` ticks wait to be collected.  lmot_seq_tick_dev: device data ordered after the caller stream (frames: stride
+ * 4, 16-byte aligned; lists: data[j] of up to cap_per_list boxes, 4-byte alignment, lengths in the device ints d_counts[j] clamped to
+ * [0, cap_per_list]); a full ring drops the oldest tick; a sequence whose lists together exceed max_boxes reports LMOT_ERR_CAPACITY at
+ * collect with its list cut, the other sequences are unaffected.  lmot_seq_tick: submit + collect, dropping uncollected ticks as lmot_seq
+ * does.  Timing mode: LMOT_ERR_STATE.
+ * LMOT_ERR_INVALID, nothing submitted: no open set; n_seq != the set's; an unknown kind or flag bit; every entry SKIP; SKIP with
+ * RESTART; a null data / n / d_counts where the kind needs it (a host frame or list of length > 0 needs its pointer, a device list
+ * always); a negative count; cap_per_list < 1; a device frame that is not 16-byte aligned; a host FRAMES entry with stride_floats < 3.
+ * LMOT_ERR_CAPACITY, nothing submitted: a frame above max_points, a host list above max_boxes. */
+enum { LMOT_SEQ_SKIP = 0, LMOT_SEQ_FRAMES = 1, LMOT_SEQ_LISTS = 2 };
+enum { LMOT_SEQ_RESTART = 1 };
+typedef struct lmot_seq_entry {
+  int kind;                    /* LMOT_SEQ_SKIP / _FRAMES / _LISTS */
+  int flags;                   /* LMOT_SEQ_RESTART: the sequence starts over with this step */
+  double timestamp_us, v_gps, yaw_gps;
+  const float* const* data;    /* one per sensor of the sequence's table (one without a table): point arrays (FRAMES) or box lists (LISTS) */
+  const int* n;                /* HOST ints: points per frame / boxes per list (dev form, LISTS: unused) */
+  const int* d_counts;         /* dev form, LISTS only: DEVICE ints, list lengths */
+  int cap_per_list;            /* dev form, LISTS only */
+} lmot_seq_entry;
+int lmot_seq_tick_submit(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, int stride_floats);
+int lmot_seq_tick_dev(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq);
+int lmot_seq_tick(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, int stride_floats, lmot_seq_out* out);
+int lmot_seq_stepped(const lmot_ctx* ctx, uint32_t* mask);
 
 /* ---- tracker parameters: the IMM-UKF-PDA noise, gating and track-management constants of one track table ------------------------
  * The defaults (lmot_default_tracker_params) are the reference's values; citations are file:line under object_tracking/tracking/.
