@@ -171,6 +171,53 @@ def _detect_params(base: dict, fields: dict) -> DetectParams:
     return d
 
 
+class Deskew(C.Structure):
+    """lmot_deskew: sweep deskew of a stream's frames (include/lmot.h)."""
+    _fields_ = [("on", C.c_int), ("time_field", C.c_int), ("time_scale", C.c_double), ("time_offset", C.c_double),
+                ("t_min", C.c_double), ("t_max", C.c_double)]
+
+
+DESKEW_SLICES = 256                     # LMOT_DESKEW_SLICES
+
+
+def default_deskew() -> dict:
+    """lmot_default_deskew as a dict of field -> value"""
+    d = Deskew()
+    load_library().lmot_default_deskew(C.byref(d))
+    return {name: getattr(d, name) for name, _ in Deskew._fields_}
+
+
+def _deskew(fields: dict) -> Deskew:
+    """the defaults with `fields` replaced (unknown names raise)"""
+    d = Deskew()
+    load_library().lmot_default_deskew(C.byref(d))
+    names = dict(Deskew._fields_)
+    for name, val in fields.items():
+        if name not in names:
+            raise ValueError(f"unknown deskew setting {name!r}")
+        setattr(d, name, int(val) if names[name] is C.c_int else float(val))
+    return d
+
+
+def deskew_table(v: float, omega: float, mount=None, **fields) -> np.ndarray:
+    """lmot_deskew_table: the (DESKEW_SLICES, 3, 4) float32 pose table of one frame moving at v (m/s) and turning at omega (rad/s),
+    for the settings `fields` (the defaults replaced) and a sensor mounted at `mount` ((3, 4) or (12,) [R | t]; None: identity)."""
+    lib = load_library()
+    out = np.zeros((DESKEW_SLICES, 12), np.float32)
+    m = None
+    if mount is not None:
+        m = Sensor()
+        lib.lmot_default_sensor(None, C.byref(m))
+        m.pose[:] = [float(x) for x in np.asarray(mount, np.float32).reshape(12)]
+    fn = lib.lmot_deskew_table
+    fn.argtypes = [C.POINTER(Deskew), C.c_double, C.c_double, C.c_void_p, C.c_void_p]
+    st = fn(C.byref(_deskew(fields)), float(v), float(omega), C.cast(C.byref(m), C.c_void_p) if m is not None else None,
+            out.ctypes.data_as(C.c_void_p))
+    if st != OK:
+        raise LmotError(st, lib.lmot_strerror(st).decode())
+    return out.reshape(DESKEW_SLICES, 3, 4)
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -224,6 +271,7 @@ ABI_SYMBOLS = [
     "lmot_seq_tracker_dump", "lmot_seq_tracker_get_ego", "lmot_seq_set_sensors", "lmot_seq_get_sensors", "lmot_seq_frame_counts",
     "lmot_seq_track_submit", "lmot_seq_track_dev", "lmot_seq_track", "lmot_seq_tracker_load", "lmot_seq_tracker_set_ego",
     "lmot_seq_tick_submit", "lmot_seq_tick_dev", "lmot_seq_tick", "lmot_seq_stepped",
+    "lmot_default_deskew", "lmot_set_deskew", "lmot_get_deskew", "lmot_seq_set_deskew", "lmot_seq_get_deskew", "lmot_deskew_table",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
@@ -744,6 +792,26 @@ class Lmot:
         d = DetectParams()
         self._chk(self.lib.lmot_seq_get_detect_params(self.h, int(k), C.byref(d)))
         return {name: getattr(d, name) for name, _ in DetectParams._fields_}
+
+    # ---- sweep deskew (lmot_set_deskew / lmot_seq_set_deskew) --------------------------------------------------------------------
+    def set_deskew(self, **fields):
+        """The context's frames: deskew settings with `fields` replaced (on=1 turns it on; no fields: the defaults, off).  Applies from
+        the next submitted frame on."""
+        self._chk(self.lib.lmot_set_deskew(self.h, C.byref(_deskew(fields)) if fields else None))
+
+    def get_deskew(self) -> dict:
+        d = Deskew()
+        self._chk(self.lib.lmot_get_deskew(self.h, C.byref(d)))
+        return {name: getattr(d, name) for name, _ in Deskew._fields_}
+
+    def seq_set_deskew(self, k: int, **fields):
+        """Sequence k's FRAMES steps, arguments as set_deskew."""
+        self._chk(self.lib.lmot_seq_set_deskew(self.h, int(k), C.byref(_deskew(fields)) if fields else None))
+
+    def seq_get_deskew(self, k: int) -> dict:
+        d = Deskew()
+        self._chk(self.lib.lmot_seq_get_deskew(self.h, int(k), C.byref(d)))
+        return {name: getattr(d, name) for name, _ in Deskew._fields_}
 
     def seq_frame_counts(self, k: int) -> np.ndarray:
         """(n_frames, 4) int32: n_elevated, n_ground, num_cluster, n_boxes of each of sequence k's frames in the tick collected last"""

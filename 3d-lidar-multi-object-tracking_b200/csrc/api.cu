@@ -62,6 +62,55 @@ int upload_points(Ctx* c, Slot* s, cudaStream_t st, const float* points, int n, 
   return LMOT_OK;
 }
 
+// ---- sweep deskew (deskew.cu; include/lmot.h): the frame's motion from the stream's fold, and the staging of frames and pose tables
+constexpr int kDeskewTab = LMOT_DESKEW_SLICES * 12;            // floats of one pose table
+constexpr size_t kDeskewTabBytes = kDeskewTab * sizeof(float);
+
+// omega of the frame (ts, v, yaw) of the table whose host state is th: diffYaw and dt as the tracker launch's fold will take them
+// (peeked on a copy); 0 on the table's first frame, for dt <= 0 and for anything not finite
+double deskew_omega(const TrackerHost& th, double ts, double v, double yaw) {
+  if (!th.init) return 0.0;
+  TrackerHost peek = th;
+  origin_points_fold(peek, ts, v, yaw);
+  const double diffYaw = peek.egoYaw - peek.egoPreYaw;
+  const double dt = (ts - th.timestamp) / 1000000.0;
+  if (!std::isfinite(diffYaw) || !std::isfinite(dt) || !(dt > 0.0)) return 0.0;
+  const double w = std::remainder(diffYaw, 2.0 * M_PI) / dt;
+  return std::isfinite(w) ? w : 0.0;
+}
+
+// a host frame's records (stride floats each) -> slot s's raw device staging on st: d_stage_in for stride 4, d_stage_wide (grown to the
+// largest frame seen; growing waits for the device once) for wider records
+int deskew_stage_host(Ctx* c, Slot* s, cudaStream_t st, const float* points, int n, int stride, const float** d_raw) {
+  *d_raw = nullptr;
+  if (n == 0) return LMOT_OK;
+  const size_t bytes = (size_t)n * stride * sizeof(float);
+  float* dst = s->d_stage_in;
+  if (stride > 4) {
+    if (bytes > s->stage_wide_bytes) {
+      LMOT_CUDA(c, cudaStreamSynchronize(st));       // (cudaFree waits for the device anyway: the old staging may still be read)
+      cudaFree(s->d_stage_wide);
+      s->d_stage_wide = nullptr; s->stage_wide_bytes = 0;
+      LMOT_CUDA(c, cudaMalloc(&s->d_stage_wide, bytes));
+      s->stage_wide_bytes = bytes;
+    }
+    dst = s->d_stage_wide;
+  }
+  LMOT_CUDA(c, cudaMemcpyAsync(dst, points, bytes, cudaMemcpyHostToDevice, st));
+  *d_raw = dst;
+  return LMOT_OK;
+}
+
+// a single-stream frame (lmot_frame*): its table from the context's own fold (no mount) into r's pinned block, copied to the slot's
+// table; the frame's records d_raw (stride floats each) deskewed into the slot's point buffer, all on the slot stream
+int deskew_frame(Ctx* c, Slot* s, Result* r, const float* d_raw, int n, int stride, double ts, double v, double yaw) {
+  if (n == 0) return LMOT_OK;
+  deskew_table(c->deskew, std::isfinite(v) ? v : 0.0, deskew_omega(c->own.th, ts, v, yaw), nullptr, r->h_deskew);
+  LMOT_CUDA(c, cudaMemcpyAsync(s->d_deskew, r->h_deskew, kDeskewTabBytes, cudaMemcpyHostToDevice, s->stream));
+  const DeskewJob j{d_raw, s->d_points, s->d_deskew, n, stride, c->deskew};
+  return deskew_launch(c, s->stream, &j, 1);
+}
+
 int fetch_counters(Ctx* c, Slot* s, cudaStream_t st) {
   LMOT_CUDA(c, cudaMemcpyAsync(s->h_counters, s->d_counters, CNT_COUNT * sizeof(int), cudaMemcpyDeviceToHost, st));
   LMOT_CUDA(c, cudaStreamSynchronize(st));
@@ -200,6 +249,7 @@ int bank_ensure(Ctx* c) {
     LMOT_CUDA(c, cudaMemset(k->d_counters, 0, CNT_COUNT * sizeof(int)));
     LMOT_CUDA(c, cudaMalloc(&k->d_det_sem, sizeof(int)));
     LMOT_CUDA(c, cudaMemset(k->d_det_sem, 0, sizeof(int)));
+    LMOT_CUDA(c, cudaMalloc(&k->d_deskew, kMaxBatch * kDeskewTabBytes));
     LMOT_CUDA(c, cudaEventCreateWithFlags(&k->ev_det_done, cudaEventDisableTiming));
     LMOT_CUDA(c, cudaEventCreateWithFlags(&k->ev_trk_done, cudaEventDisableTiming));
     LMOT_CUDA(c, cudaEventCreateWithFlags(&k->ev_fork, cudaEventDisableTiming));
@@ -233,7 +283,7 @@ void batch_destroy(Ctx* c) {
   for (int i = 0; i < c->n_bslots; ++i) slot_destroy(&c->bslots[i]);
   for (int b = 0; b < kBatchBanks; ++b) {
     Slot* k = &c->bank[b];
-    cudaFree(k->d_boxes); cudaFree(k->d_boxes_g); cudaFree(k->d_counters); cudaFree(k->d_det_sem);
+    cudaFree(k->d_boxes); cudaFree(k->d_boxes_g); cudaFree(k->d_counters); cudaFree(k->d_det_sem); cudaFree(k->d_deskew);
     if (k->ev_det_done) cudaEventDestroy(k->ev_det_done);
     if (k->ev_trk_done) cudaEventDestroy(k->ev_trk_done);
     if (k->ev_fork) cudaEventDestroy(k->ev_fork);
@@ -394,6 +444,7 @@ void result_destroy(Result* r) {
   if (r->h_vis) cudaFreeHost(r->h_vis);
   if (r->h_visbb) cudaFreeHost(r->h_visbb);
   if (r->h_ids) cudaFreeHost(r->h_ids);
+  if (r->h_deskew) cudaFreeHost(r->h_deskew);
   if (r->d_ids) cudaFree(r->d_ids);
   if (r->d_block) cudaFree(r->d_block);
   if (r->ev_tc) cudaEventDestroy(r->ev_tc);
@@ -415,9 +466,11 @@ void seq_destroy(Ctx* c) {
       m = SeqMeas{};
     }
   for (int b = 0; b < kBatchBanks; ++b) { cudaFree(c->seq_stage[b]); c->seq_stage[b] = nullptr; }
-  for (int k = 0; k < kMaxBatch; ++k) { c->seq_n_sensors[k] = 0; c->seq_fc_n[k] = 0; c->seq_det_on[k] = false; }
-  for (int i = 0; i < c->seq_ring; ++i)
+  for (int k = 0; k < kMaxBatch; ++k) { c->seq_n_sensors[k] = 0; c->seq_fc_n[k] = 0; c->seq_det_on[k] = false; c->seq_deskew[k] = deskew_defaults(); }
+  for (int i = 0; i < c->seq_ring; ++i) {
     for (int k = 0; k < c->n_seq; ++k) result_destroy(&c->seq_ticks[i].blocks[k]);
+    if (c->seq_ticks[i].h_deskew) cudaFreeHost(c->seq_ticks[i].h_deskew);
+  }
   delete[] c->seq_ticks;
   c->seq_ticks = nullptr; c->seq_last = nullptr; c->seq_stepped = 0;
   c->n_seq = 0; c->seq_ring = 0; c->seq_next = 0; c->seq_oldest = 0; c->seq_in_flight = 0;
@@ -479,6 +532,7 @@ int slot_create(Ctx* c, Slot* s, int index) {
   if (rc == LMOT_OK) rc = cluster_alloc(c, s);
   if (rc == LMOT_OK) rc = boxfit_alloc(c, s);
   if (rc) return rc;
+  LMOT_CUDA(c, cudaMalloc(&s->d_deskew, kDeskewTabBytes));
   LMOT_CUDA(c, cudaEventRecord(s->ev_trk_done, s->stream));   // "free" from the start
   LMOT_CUDA(c, cudaEventRecord(s->ev_det_done, s->stream));
   s->res = &c->results[0];
@@ -487,6 +541,7 @@ int slot_create(Ctx* c, Slot* s, int index) {
 
 void slot_destroy(Slot* s) {
   ground_free(s); cluster_free(s); boxfit_free(s);
+  cudaFree(s->d_deskew); cudaFree(s->d_stage_wide);
   if (s->ev_fork) cudaEventDestroy(s->ev_fork);
   if (s->ev_det_done) cudaEventDestroy(s->ev_det_done);
   if (s->ev_trk_done) cudaEventDestroy(s->ev_trk_done);
@@ -848,12 +903,21 @@ int lmot_detect_dev(lmot_ctx* ctx, const float* d_points, int n) {
 int lmot_frame_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp_us, double v_gps, double yaw_gps) {
   if (!ctx || n < 0 || (n > 0 && !d_points) || (reinterpret_cast<uintptr_t>(d_points) & 15u)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
+  const bool dsk = c->deskew.on != 0;
+  if (dsk && c->timing) return LMOT_ERR_STATE;
+  if (dsk && c->deskew.time_field != 3) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, true);
   LMOT_CUDA(c, cudaEventRecord(s->ev_fork, c->stream));          // the caller's stream produced d_points
   LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_fork, 0));
+  if (dsk) {                           // one extra pass: the caller's frame, deskewed, into the slot's own point buffer
+    LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_trk_done, 0));
+    int rc = deskew_frame(c, s, r, d_points, n, 4, timestamp_us, v_gps, yaw_gps);
+    if (rc) return rc;
+    return submit(c, s, r, s->d_points, n, true, timestamp_us, v_gps, yaw_gps);
+  }
   return submit(c, s, r, reinterpret_cast<const float4*>(d_points), n, true, timestamp_us, v_gps, yaw_gps);
 }
 
@@ -861,6 +925,12 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
+  const bool dsk = c->deskew.on != 0;
+  if (dsk) {                           // (validated before anything is submitted: upload_points checks the rest without deskew)
+    if (c->timing) return LMOT_ERR_STATE;
+    if (n < 0 || (n > 0 && !points) || stride <= c->deskew.time_field) return LMOT_ERR_INVALID;
+    if (n > c->max_points) return LMOT_ERR_CAPACITY;
+  }
   if (c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;    // result ring full: collect first
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, false);
@@ -874,15 +944,21 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   // ground_reads_input_once).  Bit-identical results (tests/test_pipeline_gpu.py) -- but SM-issued reads over the link were
   // slower than the copy engine at this copy size.  Hence off by default.  The buffer must stay untouched until
   // the frame has been collected (the same contract as the asynchronous copy).
-  if (c->zero_copy && stride == 4 && n > 0 && n <= c->max_points && (reinterpret_cast<uintptr_t>(points) & 15u) == 0 && ground_reads_input_once(c, n)) {
+  if (!dsk && c->zero_copy && stride == 4 && n > 0 && n <= c->max_points && (reinterpret_cast<uintptr_t>(points) & 15u) == 0 && ground_reads_input_once(c, n)) {
     cudaPointerAttributes pa;
     if (cudaPointerGetAttributes(&pa, points) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer)
       return submit(c, s, r, reinterpret_cast<const float4*>(pa.devicePointer), n, true, timestamp_us, v_gps, yaw_gps);
     cudaGetLastError();      // (pageable memory: not an error, take the copy path)
   }
   LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_trk_done, 0));
-  int rc = upload_points(c, s, s->stream, points, n, stride, s->d_points);
-  if (rc) return rc;
+  int rc;
+  if (dsk) {                           // the raw records to the device, then deskewed into the slot's point buffer (in place of repack_kernel)
+    const float* raw = nullptr;
+    if ((rc = deskew_stage_host(c, s, s->stream, points, n, stride, &raw))) return rc;
+    if ((rc = deskew_frame(c, s, r, raw, n, stride, timestamp_us, v_gps, yaw_gps))) return rc;
+  } else if ((rc = upload_points(c, s, s->stream, points, n, stride, s->d_points))) {
+    return rc;
+  }
   return submit(c, s, r, s->d_points, n, true, timestamp_us, v_gps, yaw_gps);
 }
 
@@ -951,6 +1027,9 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
     if (n[i] > c->max_points) return LMOT_ERR_CAPACITY;
     if (!host && n[i] > 0 && (reinterpret_cast<uintptr_t>(points[i]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies need 16-byte alignment
   }
+  const bool dsk = with_tracker && c->deskew.on != 0;               // (lmot_batch_detect_dev has no stamp: never deskewed)
+  if (dsk && c->timing) return LMOT_ERR_STATE;
+  if (dsk && (host ? stride <= c->deskew.time_field : c->deskew.time_field != 3)) return LMOT_ERR_INVALID;
   if (host && c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;
   int rc = batch_ensure(c, n_frames);
   if (rc) return rc;
@@ -964,16 +1043,31 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   // the bank's previous tick must have been consumed by the tracker; device frames: ordered after the caller's stream
   LMOT_CUDA(c, cudaStreamWaitEvent(st, k->ev_trk_done, 0));
   const float4* dp[kMaxBatch];
+  const float* raw[kMaxBatch];
   if (host) {
     for (int i = 0; i < n_frames; ++i) {
       Slot* s = &c->bslots[b * c->batch_frames + i];
-      if ((rc = upload_points(c, s, st, points[i], n[i], stride, s->d_points))) return rc;
+      if (dsk) rc = deskew_stage_host(c, s, st, points[i], n[i], stride, &raw[i]);
+      else rc = upload_points(c, s, st, points[i], n[i], stride, s->d_points);
+      if (rc) return rc;
       dp[i] = nullptr;
     }
   } else {
     LMOT_CUDA(c, cudaEventRecord(k->ev_fork, c->stream));
     LMOT_CUDA(c, cudaStreamWaitEvent(st, k->ev_fork, 0));
-    for (int i = 0; i < n_frames; ++i) dp[i] = reinterpret_cast<const float4*>(points[i]);
+    for (int i = 0; i < n_frames; ++i) { dp[i] = reinterpret_cast<const float4*>(points[i]); raw[i] = points[i]; }
+  }
+  if (dsk) {
+    // every sensor's frame with its own mount (the rig table, captured here) and the context's fold; one table copy, one launch
+    const double om = deskew_omega(c->own.th, ts, v, yaw), vv = std::isfinite(v) ? v : 0.0;
+    DeskewJob jobs[kMaxBatch];
+    for (int i = 0; i < n_frames; ++i) {
+      deskew_table(c->deskew, vv, om, c->n_sensors > 0 ? &c->sensors[i] : nullptr, r->h_deskew + (size_t)i * kDeskewTab);
+      jobs[i] = DeskewJob{raw[i], c->bslots[b * c->batch_frames + i].d_points, k->d_deskew + (size_t)i * kDeskewTab, n[i], host ? stride : 4, c->deskew};
+      dp[i] = nullptr;
+    }
+    LMOT_CUDA(c, cudaMemcpyAsync(k->d_deskew, r->h_deskew, (size_t)n_frames * kDeskewTabBytes, cudaMemcpyHostToDevice, st));
+    if ((rc = deskew_launch(c, st, jobs, n_frames))) return rc;
   }
   return batch_submit(c, b, r, dp, n, n_frames, with_tracker, ts, v, yaw);
 }
@@ -1161,6 +1255,8 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
       if (q.n[j] < 0 || (q.n[j] > 0 && !q.data[j])) return LMOT_ERR_INVALID;
       if (!host && q.kind == LMOT_SEQ_FRAMES && q.n[j] > 0 && (reinterpret_cast<uintptr_t>(q.data[j]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies
     }
+    if (q.kind == LMOT_SEQ_FRAMES && c->seq_deskew[k].on && (host ? stride <= c->seq_deskew[k].time_field : c->seq_deskew[k].time_field != 3))
+      return LMOT_ERR_INVALID;
     ++S;
     if (q.kind == LMOT_SEQ_FRAMES) { F += nk; rigged |= rig_on[k]; own_det |= c->seq_det_on[k]; }
     else FL += nk;
@@ -1262,12 +1358,23 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
     bool drig[kMaxBatch];
     for (int i = 0; i < F; ++i) sl[i] = &c->bslots[b * c->batch_frames + i];
     df0[0] = 0;
+    DeskewJob dj[kMaxBatch];           // deskewing sequences (lmot_seq_set_deskew): their frames, each with its sequence's fold and mount
+    int nj = 0;
     for (int k = 0; k < n_seq; ++k) {
       if (e[k].kind != LMOT_SEQ_FRAMES) continue;
+      const lmot_deskew& dk = c->seq_deskew[k];
+      const double om = dk.on ? deskew_omega(c->seq[k].th, e[k].timestamp_us, e[k].v_gps, e[k].yaw_gps) : 0.0;   // (after a restart above)
+      const double vv = std::isfinite(e[k].v_gps) ? e[k].v_gps : 0.0;
       for (int j = 0; j < f0[k + 1] - f0[k]; ++j) {
         const int i = df0[nd] + j;
         nn[i] = e[k].n[j];
-        if (host) {
+        if (dk.on) {
+          const float* raw = reinterpret_cast<const float*>(e[k].data[j]);
+          if (host && (rc = deskew_stage_host(c, sl[i], st, e[k].data[j], nn[i], stride, &raw))) return rc;
+          deskew_table(dk, vv, om, rig_on[k] ? &c->seq_sensors[k][j] : nullptr, t->h_deskew + (size_t)i * kDeskewTab);
+          dj[nj++] = DeskewJob{raw, sl[i]->d_points, bk->d_deskew + (size_t)i * kDeskewTab, nn[i], host ? stride : 4, dk};
+          pp[i] = sl[i]->d_points;
+        } else if (host) {
           if ((rc = upload_points(c, sl[i], st, e[k].data[j], nn[i], stride, sl[i]->d_points))) return rc;
           pp[i] = sl[i]->d_points;
         } else {
@@ -1277,6 +1384,10 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
       dseq[nd] = k; drig[nd] = rig_on[k];
       df0[nd + 1] = df0[nd] + f0[k + 1] - f0[k];
       ++nd;
+    }
+    if (nj > 0) {                      // the tick's tables in one copy (frame i's at table i of the bank), then one launch
+      LMOT_CUDA(c, cudaMemcpyAsync(bk->d_deskew, t->h_deskew, (size_t)F * kDeskewTabBytes, cudaMemcpyHostToDevice, st));
+      if ((rc = deskew_launch(c, st, dj, nj))) return rc;
     }
     sl[0]->res = bk->res;
     // sequences with their own detection values: every frame of the tick gets its entry (copied into the launch parameters), the values
@@ -1696,6 +1807,65 @@ int lmot_seq_get_detect_params(const lmot_ctx* ctx, int k, lmot_detect_params* p
   const Ctx* c = &ctx->c;
   *p = c->seq_det_on[k] ? c->seq_det[k] : detect_params_of(c->prm);
   return LMOT_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- sweep deskew
+int lmot_default_deskew(lmot_deskew* d) {
+  if (!d) return LMOT_ERR_INVALID;
+  *d = deskew_defaults();
+  return LMOT_OK;
+}
+
+static bool deskew_valid(const lmot_deskew& d) {
+  const double f[] = {d.time_scale, d.time_offset, d.t_min, d.t_max};
+  for (double x : f) if (!std::isfinite(x)) return false;
+  return d.t_min < d.t_max && d.t_max - d.t_min <= 1.0 && d.time_field >= 3;
+}
+
+// d (NULL: the defaults) validated; turning deskew on allocates the pinned table blocks `n` blocks of the ring need (once)
+static int deskew_set(Ctx* c, lmot_deskew& dst, const lmot_deskew* d, float** blocks, int n, size_t stride) {
+  lmot_deskew v = d ? *d : deskew_defaults();
+  if (!deskew_valid(v)) return LMOT_ERR_INVALID;
+  v.on = v.on ? 1 : 0;
+  if (v.on) {
+    cudaSetDevice(c->device);
+    for (int i = 0; i < n; ++i) {
+      float** p = reinterpret_cast<float**>(reinterpret_cast<char*>(blocks) + i * stride);
+      if (!*p) LMOT_CUDA(c, cudaHostAlloc((void**)p, kMaxBatch * kDeskewTabBytes, cudaHostAllocDefault));
+    }
+  }
+  dst = v;
+  return LMOT_OK;
+}
+
+// host state only, as the sensor tables: submitted frames carry their own tables and launch parameters
+int lmot_set_deskew(lmot_ctx* ctx, const lmot_deskew* d) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  return deskew_set(c, c->deskew, d, &c->results[0].h_deskew, c->n_results, sizeof(Result));
+}
+
+int lmot_get_deskew(const lmot_ctx* ctx, lmot_deskew* d) {
+  if (!ctx || !d) return LMOT_ERR_INVALID;
+  *d = ctx->c.deskew;
+  return LMOT_OK;
+}
+
+int lmot_seq_set_deskew(lmot_ctx* ctx, int k, const lmot_deskew* d) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  return deskew_set(c, c->seq_deskew[k], d, &c->seq_ticks[0].h_deskew, c->seq_ring, sizeof(SeqTick));
+}
+
+int lmot_seq_get_deskew(const lmot_ctx* ctx, int k, lmot_deskew* d) {
+  if (!ctx || !d || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  *d = ctx->c.seq_deskew[k];
+  return LMOT_OK;
+}
+
+int lmot_deskew_table(const lmot_deskew* d, double v, double omega, const lmot_sensor* mount, float out[LMOT_DESKEW_SLICES][12]) {
+  if (!d || !out || !deskew_valid(*d) || !std::isfinite(v) || !std::isfinite(omega) || (mount && !sensors_valid(mount, 1))) return LMOT_ERR_INVALID;
+  return deskew_table(*d, v, omega, mount, &out[0][0]);
 }
 
 // after the table was received from another rank (NCCL broadcast into lmot_tracker_table's pointer, count already in the device

@@ -134,6 +134,9 @@ struct Result {
   cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t kev[kMaxKernelEvents] = {};
   int n_kev = 0;
+  // deskew: pinned host source of the pose tables copied for this block's submission ([kMaxBatch][LMOT_DESKEW_SLICES * 12], allocated
+  // by lmot_set_deskew).  Reusing a block means its previous submission has completed, so the copy from it has too.
+  float* h_deskew = nullptr;
 };
 
 // Detection slot: every buffer the three detection stages (ground -> cluster -> box) touch for ONE frame, plus the
@@ -149,6 +152,9 @@ struct Slot {
   // ---- frame input (host-buffer entry points copy here; *_dev entry points use the caller's pointer)
   float4* d_points = nullptr;
   float* d_stage_in = nullptr;         // raw staging for stride != 4 inputs
+  float* d_stage_wide = nullptr;       // deskew: raw staging of host frames with stride > 4 (grown to the largest frame seen)
+  size_t stage_wide_bytes = 0;
+  float* d_deskew = nullptr;           // deskew pose tables: one on a frame slot, kMaxBatch on a bank pseudo-slot (written on its stream)
   const float4* cur_points = nullptr;
   int cur_n = 0;
 
@@ -281,7 +287,16 @@ struct SeqTick {
   Result blocks[kMaxBatch];
   uint32_t stepped = 0;                // bit k: sequence k stepped in this tick
   bool in_flight = false;
+  float* h_deskew = nullptr;           // deskew: pinned host source of the tick's pose tables, as Result::h_deskew (lmot_seq_set_deskew)
 };
+
+// lmot_default_deskew
+inline lmot_deskew deskew_defaults() {
+  lmot_deskew d;
+  memset(&d, 0, sizeof(d));
+  d.on = 0; d.time_field = 3; d.time_scale = 1.0; d.time_offset = 0.0; d.t_min = -0.1; d.t_max = 0.0;
+  return d;
+}
 
 struct Ctx {
   lmot_params prm;
@@ -350,6 +365,11 @@ struct Ctx {
   lmot_detect_params seq_det[kMaxBatch] = {};
   int seq_fc_n[kMaxBatch] = {};                // lmot_seq_frame_counts: frames of sequence k in the tick collected last
   int seq_fc[kMaxBatch][kMaxBatch][4] = {};    // ... and their n_elev, n_ground, num_cluster, n_boxes (host copies: the ring slot is reused)
+
+  // ---- sweep deskew (lmot_set_deskew / lmot_seq_set_deskew, deskew.cu): read at submission
+  lmot_deskew deskew = deskew_defaults();
+  lmot_deskew seq_deskew[kMaxBatch] = {deskew_defaults(), deskew_defaults(), deskew_defaults(), deskew_defaults(),
+                                       deskew_defaults(), deskew_defaults(), deskew_defaults(), deskew_defaults()};
 
   // ---- track prediction (lmot_predict_tracks*, tracker.cu predict_launch)
   bool pred_pending = false;           // a prediction was queued since the last tracker step: the next step's first kernel waits for it
@@ -457,5 +477,10 @@ int seq_tracker_launch(Ctx* c, const int* seq, const SeqMeas* m, SeqTick* tick, 
 int predict_launch(Ctx* c, Tracker* const* tabs, int S, const double* t_us, int n_t, const lmot_pred_out* outs, int* const* d_n_rows,
                    cudaStream_t st);
 int boxes_publish(Ctx* c, Slot* s, Result* r, cudaStream_t st);     // detection-only: slot box list -> pinned host block
+// sweep deskew (deskew.cu): one frame's pose table (out: [LMOT_DESKEW_SLICES][12]; mount nullptr: identity), and one launch over the
+// deskewed frames of a submission
+struct DeskewJob { const float* in; float4* out; const float* table; int n, stride; lmot_deskew d; };
+int deskew_table(const lmot_deskew& d, double v, double omega, const lmot_sensor* mount, float* out);
+int deskew_launch(Ctx* c, cudaStream_t st, const DeskewJob* jobs, int n_jobs);
 
 }  // namespace lmot

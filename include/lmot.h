@@ -641,6 +641,57 @@ int lmot_default_detect_params(const lmot_params* p, lmot_detect_params* out);
 int lmot_seq_set_detect_params(lmot_ctx* ctx, int k, const lmot_detect_params* p);
 int lmot_seq_get_detect_params(const lmot_ctx* ctx, int k, lmot_detect_params* p);
 
+/* ---- sweep deskew: every point of a frame moved to the frame's stamp from its own capture time and the stream's ego motion -----------
+ * A spinning LiDAR takes a whole period (100 ms at 10 Hz) to sweep; on a moving vehicle the points of one frame are seen from different
+ * poses, so static objects shift with their azimuth and an object on the sweep seam splits in two.  With deskew on, every frame is
+ * first moved point by point into the vehicle's (sensor's) frame at the frame's timestamp; detection and tracking then run exactly as
+ * on any other cloud.  The reference has no such step: deskew is opt-in, and with it off every launch and result is what it was.
+ *
+ * Definition.  Point i's time tau_i = (double)f[time_field] * time_scale + time_offset seconds relative to the frame's timestamp_us
+ * (evaluated in double, without contraction).  The frame's motion is v = its v_gps and omega = remainder(diffYaw, 2 pi) / dt, with
+ * diffYaw = egoYaw - egoPreYaw and dt = (ts - ts_prev) / 1e6 exactly as getOriginPoints' fold (lmot_origin_points) computes them for
+ * this frame of this stream; omega = 0 on the stream's first frame (after create, lmot_tracker_reset / _load with init = 0,
+ * lmot_seq_open, LMOT_SEQ_RESTART) and whenever dt <= 0 or a value is not finite (a non-finite v_gps gives v = 0).  The vehicle moves
+ * along its +x axis and turns about +z, counter-clockwise positive; its pose at tau in its frame at the stamp is th = omega * tau,
+ * tx = v * sin(th) / omega, ty = v * (1 - cos(th)) / omega (|omega| < 1e-9: tx = v * tau, ty = 0), rotation th about z.  The pose table
+ * has LMOT_DESKEW_SLICES slices over [t_min, t_max): h = (t_max - t_min) / LMOT_DESKEW_SLICES, slice s at tau_s = t_min + (s + 0.5) h,
+ * D_s = M^-1 T(tau_s) M built in double and rounded to float once per entry, M the sensor's mount pose (the rig table entry of the
+ * frame's sensor, widened from float; identity without a table), M^-1 = [R^T | -R^T t].  lmot_deskew_table returns it (no device
+ * needed).  Point i uses slice s = clamp(floor((tau_i - t_min) / h), 0, LMOT_DESKEW_SLICES - 1) and becomes, in float without
+ * contraction, x' = ((d00*x + d01*y) + d02*z) + d03 (likewise y', z'), w = 1.  A point whose tau is not finite is passed unmoved.
+ *
+ * Equivalence (bit for bit): a context with deskew on given frame P through lmot_frame / lmot_frame_submit / lmot_frame_dev returns
+ * what the same context with deskew off returns for the deskewed cloud P' (stride 4, same stamps and ego inputs): counts, boxes, every
+ * track output, the status, the tracker dump; the elevated and ground clouds are those of P'.  lmot_batch_submit / lmot_batch_dev deskew each
+ * sensor's frame with its own mount; sequences (lmot_seq_set_deskew) deskew the FRAMES steps of lmot_seq* / lmot_seq_tick* with their own
+ * fold and sensor table, as a separate context with lmot_set_deskew would.  Node pre-filters, global_frame and retirement act on P'.
+ *
+ * The setting is host state captured by value at submission, as the sensor tables: frames in flight keep theirs.  lmot_seq_open turns
+ * deskew off for every sequence; lmot_seq_tracker_reset / _load keep it; LISTS steps ignore it.  Not affected (no stamp, no ego): the
+ * stage entry points (lmot_ground_remove, lmot_component_cluster, lmot_box_fit), lmot_detect_dev, lmot_batch_detect_dev,
+ * lmot_batch_ground_ccl_dev, the tracking-only calls and lmot_shared_*.  With deskew on, LMOT_ZERO_COPY takes the copy path, and a host
+ * frame with stride_floats > 4 is staged whole on the device (its staging grows once, synchronously, to the largest frame seen).
+ *
+ * Errors.  LMOT_ERR_INVALID from lmot_set_deskew / lmot_seq_set_deskew / lmot_deskew_table, setting unchanged: a non-finite value,
+ * t_min >= t_max, t_max - t_min > 1 s, time_field < 3, k out of range (lmot_deskew_table: also non-finite v / omega, an invalid mount).
+ * At submission, nothing submitted: LMOT_ERR_INVALID for a host frame with stride_floats <= time_field or a device frame while
+ * time_field != 3; LMOT_ERR_STATE while timing mode (lmot_enable_timing) is on. */
+#define LMOT_DESKEW_SLICES 256
+typedef struct lmot_deskew {
+  int on;                    /* 0 */
+  int time_field;            /* 3: index of the float holding the point's time (device frames: must be 3, the 4th float) */
+  double time_scale;         /* 1.0: tau = field * time_scale + time_offset, in seconds relative to the frame's timestamp_us */
+  double time_offset;        /* 0.0 */
+  double t_min, t_max;       /* -0.1, 0.0: the window the pose table covers (s); t_min < t_max, both finite, t_max - t_min <= 1 */
+} lmot_deskew;
+int lmot_default_deskew(lmot_deskew* d);
+int lmot_set_deskew(lmot_ctx* ctx, const lmot_deskew* d);               /* d NULL: the defaults (off) */
+int lmot_get_deskew(const lmot_ctx* ctx, lmot_deskew* d);
+int lmot_seq_set_deskew(lmot_ctx* ctx, int k, const lmot_deskew* d);    /* sequence k of the open set; d NULL: the defaults (off) */
+int lmot_seq_get_deskew(const lmot_ctx* ctx, int k, lmot_deskew* d);
+/* the pose table of one frame: v, omega as above, mount NULL: identity */
+int lmot_deskew_table(const lmot_deskew* d, double v, double omega, const lmot_sensor* mount, float out[LMOT_DESKEW_SLICES][12]);
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);
