@@ -267,6 +267,7 @@ ABI_SYMBOLS = [
     "lmot_ground_remove_dev", "lmot_detect_dev", "lmot_sync",
     "lmot_batch_submit", "lmot_batch_dev", "lmot_batch_detect_dev", "lmot_batch_collect", "lmot_batch_fetch", "lmot_batch", "lmot_batch_ground_ccl_dev",
     "lmot_default_sensor", "lmot_set_sensors", "lmot_get_sensors",
+    "lmot_set_rig_merge", "lmot_get_rig_merge", "lmot_seq_set_rig_merge", "lmot_seq_get_rig_merge",
     "lmot_seq_open", "lmot_seq_submit", "lmot_seq_dev", "lmot_seq_collect", "lmot_seq_fetch", "lmot_seq", "lmot_seq_tracker_reset",
     "lmot_seq_tracker_dump", "lmot_seq_tracker_get_ego", "lmot_seq_set_sensors", "lmot_seq_get_sensors", "lmot_seq_frame_counts",
     "lmot_seq_track_submit", "lmot_seq_track_dev", "lmot_seq_track", "lmot_seq_tracker_load", "lmot_seq_tracker_set_ego",
@@ -635,6 +636,27 @@ class Lmot:
         n = C.c_int(0)
         self._chk(self.lib.lmot_get_sensors(self.h, arr, MAX_BATCH, C.byref(n)))
         return self._sensor_dict(arr[: n.value])
+
+    # ---- merging rigs (lmot_set_rig_merge): the sensors' elevated clouds clustered and boxed as one vehicle-frame cloud ----------
+    def set_rig_merge(self, on):
+        """Batched ticks of this context's rig: with a sensor table set, ground removal per sensor, then ONE clustering and box fitting
+        of the sensors' elevated clouds moved into the vehicle frame (an object seen by two sensors is one box).  lmot_params'
+        sensor_height is then the vehicle frame origin's height above the ground.  Applies from the next submitted tick on."""
+        self._chk(self.lib.lmot_set_rig_merge(self.h, int(on)))
+
+    def get_rig_merge(self) -> bool:
+        v = C.c_int(0)
+        self._chk(self.lib.lmot_get_rig_merge(self.h, C.byref(v)))
+        return bool(v.value)
+
+    def seq_set_rig_merge(self, k: int, on):
+        """Sequence k's FRAMES steps, as set_rig_merge (with sequence k's sensor table and detection values)."""
+        self._chk(self.lib.lmot_seq_set_rig_merge(self.h, int(k), int(on)))
+
+    def seq_get_rig_merge(self, k: int) -> bool:
+        v = C.c_int(0)
+        self._chk(self.lib.lmot_seq_get_rig_merge(self.h, int(k), C.byref(v)))
+        return bool(v.value)
 
     # ---- independent sequences: one frame of each sequence per tick, one track table per sequence (lmot_seq_*) ---------------
     def seq_open(self, n_seq: int, ring: int = 8):

@@ -169,6 +169,7 @@ Result* acquire_result(Ctx* c, bool drop_oldest) {
   }
   c->res_next = (c->res_next + 1) % c->n_results;
   c->last_res = r;
+  r->merge_rows = 0;                             // only a merging batched tick sets it (batch_submit): collect_result reads it
   return r;
 }
 
@@ -281,6 +282,7 @@ int batch_ensure(Ctx* c, int F) {
 
 void batch_destroy(Ctx* c) {
   for (int i = 0; i < c->n_bslots; ++i) slot_destroy(&c->bslots[i]);
+  for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&c->merge_unit[b]);
   for (int b = 0; b < kBatchBanks; ++b) {
     Slot* k = &c->bank[b];
     cudaFree(k->d_boxes); cudaFree(k->d_boxes_g); cudaFree(k->d_counters); cudaFree(k->d_det_sem); cudaFree(k->d_deskew);
@@ -291,8 +293,26 @@ void batch_destroy(Ctx* c) {
   }
 }
 
+// merge units of a merging rig: *units[b] of every bank, allocated on first use (one device synchronisation, as batch_ensure).  All or
+// nothing: a failed allocation frees the whole set, so a later submission retries from scratch instead of finding a half-built one.
+int merge_ensure(Ctx* c, Slot* const* units, int index) {
+  bool ready = true;
+  for (int b = 0; b < kBatchBanks; ++b) ready &= merge_unit_ready(units[b]);
+  if (ready) return LMOT_OK;
+  int rc = LMOT_OK;
+  for (int b = 0; b < kBatchBanks && rc == LMOT_OK; ++b)
+    if (!merge_unit_ready(units[b])) rc = merge_unit_create(c, units[b], index + b);
+  if (rc == LMOT_OK && cudaDeviceSynchronize() != cudaSuccess) rc = LMOT_ERR_CUDA;
+  if (rc) {
+    cudaDeviceSynchronize();           // (the allocators' memsets) before the buffers go back
+    for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(units[b]);
+  }
+  return rc;
+}
+
 // one tick: F device-resident frames (slot buffers or caller pointers) -> batched ground / CCL / box fitting -> concatenated boxes
-// -> (optionally) the tracker.  d_pts[i] == nullptr: the frame was uploaded into the slot's own buffer.
+// -> (optionally) the tracker.  d_pts[i] == nullptr: the frame was uploaded into the slot's own buffer.  A merging rig
+// (lmot_set_rig_merge, units allocated by batch_common) clusters and boxes the sensors' elevated clouds as one, in the bank's merge unit.
 int batch_submit(Ctx* c, int bank_i, Result* r, const float4* const* d_pts, const int* n, int F, bool with_tracker, double ts, double v, double yaw) {
   int rc;
   struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
@@ -305,16 +325,35 @@ int batch_submit(Ctx* c, int bank_i, Result* r, const float4* const* d_pts, cons
   k->res = r; sl[0]->res = r;
   r->n_kev = 0;
   r->batch_frames = F;
-  if (c->timing) cudaEventRecord(r->ev[0], st);
-  if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, c->fuse_ccl, false, rig))) return rc;
-  if (c->timing) cudaEventRecord(r->ev[1], st);
-  if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
-  if (c->timing) cudaEventRecord(r->ev[2], st);
-  if ((rc = boxfit_launch_batch(c, sl, F, st, n, false, rig))) return rc;
   int* d_fc = nullptr;                       // the per-frame counts go straight into the result's pinned, device-mapped block
   LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&d_fc, r->h_frame_counts, 0));
   const bool gf = with_tracker && c->prm.global_frame;
-  if ((rc = boxes_concat_launch(c, sl, F, st, k->d_boxes, k->d_counters, d_fc, (with_tracker && !gf) ? k->d_det_sem : nullptr, rig))) return rc;
+  const bool merge = rig && c->rig_merge;
+  r->merge_rows = merge ? F : 0;
+  if (!merge) {
+    if (c->timing) cudaEventRecord(r->ev[0], st);
+    if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, c->fuse_ccl, false, rig))) return rc;
+    if (c->timing) cudaEventRecord(r->ev[1], st);
+    if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
+    if (c->timing) cudaEventRecord(r->ev[2], st);
+    if ((rc = boxfit_launch_batch(c, sl, F, st, n, false, rig))) return rc;
+    if ((rc = boxes_concat_launch(c, sl, F, st, k->d_boxes, k->d_counters, d_fc, (with_tracker && !gf) ? k->d_det_sem : nullptr, rig))) return rc;
+  } else {
+    // ground per sensor (CCL not fused: nothing clusters the sensors' frames), the sensors' elevated clouds into the merge unit, then
+    // clustering and box fitting of that one cloud with lmot_params' values, and its box list as the tick's (already vehicle frame)
+    Slot* u[1] = {&c->merge_unit[bank_i]};
+    const int s0[2] = {0, F};
+    int* fcu[1] = {d_fc};
+    const float roi[1] = {c->prm.roi_m};
+    long long tot = 0;
+    for (int i = 0; i < F; ++i) tot += n[i];
+    const int nu[1] = {(int)(tot < c->max_points ? tot : c->max_points)};
+    if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, false, false, rig))) return rc;
+    if ((rc = rig_merge_launch(c, st, sl, rig, n, 1, s0, u, fcu, roi))) return rc;
+    if ((rc = ccl_launch_batch(c, u, 1, st))) return rc;
+    if ((rc = boxfit_launch_batch(c, u, 1, st, nu, false))) return rc;
+    if ((rc = boxes_concat_launch(c, u, 1, st, k->d_boxes, k->d_counters, d_fc + 4 * F, (with_tracker && !gf) ? k->d_det_sem : nullptr))) return rc;
+  }
   if (gf && (rc = boxes_to_global_launch(c, k, st, k->d_boxes, k->d_counters, ts, v, yaw, true))) return rc;
   if (c->timing) cudaEventRecord(r->ev[3], st);
   LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, st));
@@ -374,6 +413,16 @@ int collect_result(Ctx* c, Result* r, lmot_frame_out* out, Tracker* trk = nullpt
     r->h_hdr[HDR_NUM_CLUSTER] = r->h_det[CNT_NUM_CLUSTER]; r->h_hdr[HDR_N_BOXES] = r->h_det[CNT_N_BOXES];
     r->h_hdr[HDR_N_TRACKS] = 0; r->h_hdr[HDR_N_VIS] = 0; r->h_hdr[HDR_ERROR] = r->h_det[CNT_ERROR]; r->h_hdr[HDR_WARN] = 0;
   }
+  if (r->merge_rows > 0) {
+    // merging rig: row 0 takes the merged cloud's num_cluster / n_boxes (written behind the sensors' rows); n_elevated is the sensors'
+    // sum (the merged cloud's length is that, or max_points where it was cut)
+    int* fc = r->h_frame_counts;
+    const int F = r->merge_rows;
+    fc[2] = fc[4 * F + 2]; fc[3] = fc[4 * F + 3];
+    int ne = 0;
+    for (int j = 0; j < F; ++j) ne += fc[4 * j];
+    r->h_hdr[HDR_N_ELEV] = ne;
+  }
   const int err = r->h_hdr[HDR_ERROR];
   const int warn = r->has_tracks ? r->h_hdr[HDR_WARN] : 0;
   if (r->has_tracks) {
@@ -399,8 +448,8 @@ int result_create(Ctx* c, Result* r) {
   memset(r->h_hdr, 0, HDR_COUNT * sizeof(int));
   LMOT_CUDA(c, cudaHostAlloc(&r->h_det, CNT_COUNT * sizeof(int), fl));
   memset(r->h_det, 0, CNT_COUNT * sizeof(int));
-  LMOT_CUDA(c, cudaHostAlloc(&r->h_frame_counts, 4 * kMaxBatch * sizeof(int), fl));
-  memset(r->h_frame_counts, 0, 4 * kMaxBatch * sizeof(int));
+  LMOT_CUDA(c, cudaHostAlloc(&r->h_frame_counts, 4 * (kMaxBatch + 1) * sizeof(int), fl));   // + the merged cloud's row (merge_rows)
+  memset(r->h_frame_counts, 0, 4 * (kMaxBatch + 1) * sizeof(int));
   LMOT_CUDA(c, cudaHostAlloc(&r->h_boxes, (size_t)MB * 24 * sizeof(float) + 16, fl));
   // + 16 bytes: spawn_output_kernel writes whole 16-byte words
   LMOT_CUDA(c, cudaHostAlloc(&r->h_targets, (size_t)TC * 3 * sizeof(float) + 16, fl));
@@ -467,6 +516,10 @@ void seq_destroy(Ctx* c) {
     }
   for (int b = 0; b < kBatchBanks; ++b) { cudaFree(c->seq_stage[b]); c->seq_stage[b] = nullptr; }
   for (int k = 0; k < kMaxBatch; ++k) { c->seq_n_sensors[k] = 0; c->seq_fc_n[k] = 0; c->seq_det_on[k] = false; c->seq_deskew[k] = deskew_defaults(); }
+  for (int k = 0; k < kMaxBatch; ++k) {
+    c->seq_rig_merge[k] = false;
+    for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&c->seq_merge_unit[b][k]);
+  }
   for (int i = 0; i < c->seq_ring; ++i) {
     for (int k = 0; k < c->n_seq; ++k) result_destroy(&c->seq_ticks[i].blocks[k]);
     if (c->seq_ticks[i].h_deskew) cudaFreeHost(c->seq_ticks[i].h_deskew);
@@ -1030,9 +1083,13 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   const bool dsk = with_tracker && c->deskew.on != 0;               // (lmot_batch_detect_dev has no stamp: never deskewed)
   if (dsk && c->timing) return LMOT_ERR_STATE;
   if (dsk && (host ? stride <= c->deskew.time_field : c->deskew.time_field != 3)) return LMOT_ERR_INVALID;
+  const bool merge = c->rig_merge && c->n_sensors > 0;
+  if (merge && c->timing) return LMOT_ERR_STATE;
   if (host && c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;
   int rc = batch_ensure(c, n_frames);
   if (rc) return rc;
+  Slot* const units[kBatchBanks] = {&c->merge_unit[0], &c->merge_unit[1]};
+  if (merge && (rc = merge_ensure(c, units, 3000))) return rc;
   Result* r = acquire_result(c, !host);
   if (!r) return LMOT_ERR_STATE;
   const int b = c->next_bank;
@@ -1241,7 +1298,8 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
   seq_layout(c, f0, rig_on);
   // validation: nothing is submitted unless the whole tick is valid
   int S = 0, F = 0, FL = 0;            // stepped sequences, detection frames, lists
-  bool rigged = false, own_det = false;
+  bool rigged = false, own_det = false, merging = false;
+  bool merge[kMaxBatch] = {};          // FRAMES sequences with a table and lmot_seq_set_rig_merge on: one merged cloud per sequence
   for (int k = 0; k < n_seq; ++k) {
     const lmot_seq_entry& q = e[k];
     const int nk = f0[k + 1] - f0[k];
@@ -1258,7 +1316,11 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
     if (q.kind == LMOT_SEQ_FRAMES && c->seq_deskew[k].on && (host ? stride <= c->seq_deskew[k].time_field : c->seq_deskew[k].time_field != 3))
       return LMOT_ERR_INVALID;
     ++S;
-    if (q.kind == LMOT_SEQ_FRAMES) { F += nk; rigged |= rig_on[k]; own_det |= c->seq_det_on[k]; }
+    if (q.kind == LMOT_SEQ_FRAMES) {
+      F += nk; rigged |= rig_on[k]; own_det |= c->seq_det_on[k];
+      merge[k] = rig_on[k] && c->seq_rig_merge[k];
+      merging |= merge[k];
+    }
     else FL += nk;
   }
   if (S == 0 || (host && F > 0 && stride < 3)) return LMOT_ERR_INVALID;
@@ -1276,6 +1338,11 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
   } else if (!c->bank[0].stream) {     // a tracking tick needs the banks' events and streams, not their detection slots
     if ((rc = bank_ensure(c))) return rc;
     LMOT_CUDA(c, cudaDeviceSynchronize());
+  }
+  for (int k = 0; k < n_seq; ++k) {
+    if (!merge[k]) continue;
+    Slot* const units[kBatchBanks] = {&c->seq_merge_unit[0][k], &c->seq_merge_unit[1][k]};
+    if ((rc = merge_ensure(c, units, 4000 + 16 * k))) return rc;
   }
   // the tick's ring slot and bank; the front end runs on the bank's first detection slot's stream (on the bank's own stream when no
   // sequence sends frames), after the bank's previous tick has been consumed by the tracker
@@ -1310,6 +1377,7 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
     r->n_kev = 0; r->has_tracks = true;
     // > 0: the concatenation / pack writes the block's per-frame counts; 0: one frame, counts from the header
     r->batch_frames = (e[k].kind == LMOT_SEQ_LISTS || rigged) ? f0[k + 1] - f0[k] : 0;
+    r->merge_rows = merge[k] ? f0[k + 1] - f0[k] : 0;
   }
   t->stepped = stepped;
   bk->res = &t->blocks[seq[0]];
@@ -1431,10 +1499,57 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
         dm[d] = mk[k] = c->seq_meas[b][k];
         LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc[d], t->blocks[k].h_frame_counts, 0));
       }
-      if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, c->fuse_ccl, false, rig, own_det ? det : nullptr))) return rc;
-      if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
-      if ((rc = boxfit_launch_batch(c, sl, F, st, nn, false, rig, own_det ? det : nullptr))) return rc;
-      if ((rc = boxes_concat_seq_launch(c, sl, nd, df0, drig, rig, dm, fc, !gf, st))) return rc;
+      if (!merging) {
+        if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, c->fuse_ccl, false, rig, own_det ? det : nullptr))) return rc;
+        if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
+        if ((rc = boxfit_launch_batch(c, sl, F, st, nn, false, rig, own_det ? det : nullptr))) return rc;
+        if ((rc = boxes_concat_seq_launch(c, sl, nd, df0, drig, rig, dm, fc, !gf, st))) return rc;
+      } else {
+        // merging sequences (lmot_seq_set_rig_merge): ground per sensor as above (CCL not fused), then each merging sequence's elevated
+        // clouds into its merge unit of this bank (one launch for all of them).  The CCL / box-fitting units are the other frames and
+        // the merge units, in sequence order; a merge unit gets the vehicle's values (identity pose, the sequence's detection values
+        // without a sensor's) and contributes one identity-pose list to its sequence
+        Slot* src[kMaxBatch];
+        Slot* mu[kMaxBatch];
+        lmot_sensor mpose[kMaxBatch];
+        int mn[kMaxBatch], ms0[kMaxBatch + 1], *mfc[kMaxBatch], nm = 0, nsrc = 0;
+        float mroi[kMaxBatch];
+        Slot* su[kMaxBatch];
+        lmot_sensor urig[kMaxBatch];
+        lmot_detect_params udet[kMaxBatch];
+        int unn[kMaxBatch], uf0[kMaxBatch + 1], *ufc[kMaxBatch], nu = 0;
+        bool udrig[kMaxBatch];
+        const lmot_detect_params base = detect_params_of(c->prm);
+        ms0[0] = 0;
+        for (int d = 0; d < nd; ++d) {
+          const int k = dseq[d], nk = df0[d + 1] - df0[d];
+          uf0[d] = nu;
+          if (merge[k]) {
+            const lmot_detect_params& vd = c->seq_det_on[k] ? c->seq_det[k] : base;
+            long long tot = 0;
+            for (int i = df0[d]; i < df0[d + 1]; ++i) { src[nsrc] = sl[i]; mpose[nsrc] = rig[i]; mn[nsrc] = nn[i]; ++nsrc; tot += nn[i]; }
+            mu[nm] = &c->seq_merge_unit[b][k]; mfc[nm] = fc[d]; mroi[nm] = vd.roi_m;
+            ms0[++nm] = nsrc;
+            su[nu] = mu[nm - 1];
+            lmot_default_sensor(&c->prm, &urig[nu]);
+            udet[nu] = vd;
+            unn[nu] = (int)(tot < c->max_points ? tot : c->max_points);
+            ++nu;
+            udrig[d] = false;
+            ufc[d] = fc[d] + 4 * nk;
+          } else {
+            for (int i = df0[d]; i < df0[d + 1]; ++i) { su[nu] = sl[i]; urig[nu] = rig[i]; if (own_det) udet[nu] = det[i]; unn[nu] = nn[i]; ++nu; }
+            udrig[d] = drig[d];
+            ufc[d] = fc[d];
+          }
+        }
+        uf0[nd] = nu;
+        if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, false, false, rig, own_det ? det : nullptr))) return rc;
+        if ((rc = rig_merge_launch(c, st, src, mpose, mn, nm, ms0, mu, mfc, mroi))) return rc;
+        if ((rc = ccl_launch_batch(c, su, nu, st))) return rc;
+        if ((rc = boxfit_launch_batch(c, su, nu, st, unn, false, urig, own_det ? udet : nullptr))) return rc;
+        if ((rc = boxes_concat_seq_launch(c, su, nd, uf0, udrig, urig, dm, ufc, !gf, st))) return rc;
+      }
     }
   }
   for (int p = 0; p < S; ++p) m[p] = mk[seq[p]];
@@ -1688,6 +1803,31 @@ int lmot_seq_get_sensors(const lmot_ctx* ctx, int k, lmot_sensor* s, int cap, in
   const Ctx* c = &ctx->c;
   if (n) *n = c->seq_n_sensors[k];
   for (int j = 0; j < c->seq_n_sensors[k] && j < cap; ++j) s[j] = c->seq_sensors[k][j];
+  return LMOT_OK;
+}
+
+// ---- merging rigs (rig_merge.cu)
+int lmot_set_rig_merge(lmot_ctx* ctx, int on) {
+  if (!ctx || (on != 0 && on != 1)) return LMOT_ERR_INVALID;
+  ctx->c.rig_merge = on != 0;
+  return LMOT_OK;
+}
+
+int lmot_get_rig_merge(const lmot_ctx* ctx, int* on) {
+  if (!ctx || !on) return LMOT_ERR_INVALID;
+  *on = ctx->c.rig_merge ? 1 : 0;
+  return LMOT_OK;
+}
+
+int lmot_seq_set_rig_merge(lmot_ctx* ctx, int k, int on) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq || (on != 0 && on != 1)) return LMOT_ERR_INVALID;
+  ctx->c.seq_rig_merge[k] = on != 0;
+  return LMOT_OK;
+}
+
+int lmot_seq_get_rig_merge(const lmot_ctx* ctx, int k, int* on) {
+  if (!ctx || !on || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  *on = ctx->c.seq_rig_merge[k] ? 1 : 0;
   return LMOT_OK;
 }
 

@@ -327,15 +327,6 @@ box_fit_frame_kernel(const __grid_constant__ FitBatch B, const __grid_constant__
 #include "box_fit_body.inc"
 }
 
-// p' = [R | t] p (lmot_set_sensors): ((r0 x + r1 y) + r2 z) + t per row in float, no contraction -- pcl::transformPointCloud's
-// evaluation with an Affine3f.  m = row-major 3x4.
-__device__ __forceinline__ void rig_apply(const float* m, float& x, float& y, float& z) {
-  const float ox = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[0], x), __fmul_rn(m[1], y)), __fmul_rn(m[2], z)), m[3]);
-  const float oy = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[4], x), __fmul_rn(m[5], y)), __fmul_rn(m[6], z)), m[7]);
-  const float oz = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[8], x), __fmul_rn(m[9], y)), __fmul_rn(m[10], z)), m[11]);
-  x = ox; y = oy; z = oz;
-}
-
 // one box (8 corners, 24 floats) moved by pose m
 __device__ __forceinline__ void rig_apply_box(const float* m, float* b) {
 #pragma unroll

@@ -111,7 +111,7 @@ constexpr int kMaxKernelEvents = 20;
 struct Result {
   int* h_hdr = nullptr;                // [16] n_elev, n_ground, num_cluster, n_boxes, n_tracks, n_vis, error
   int* h_det = nullptr;                // [CNT_COUNT] raw detection counters (detect-only submissions)
-  int* h_frame_counts = nullptr;       // [kMaxBatch][4] batched ticks: n_elev, n_ground, num_cluster, n_boxes of every frame
+  int* h_frame_counts = nullptr;       // [kMaxBatch + 1][4] batched ticks: n_elev, n_ground, num_cluster, n_boxes of every frame
   int batch_frames = 0;                // frames of the tick this block holds (0: a single-frame submission)
   float* h_boxes = nullptr;            // [max_boxes][24]
   float* h_targets = nullptr; double* h_vandyaw = nullptr; int* h_manage = nullptr;
@@ -137,6 +137,10 @@ struct Result {
   // deskew: pinned host source of the pose tables copied for this block's submission ([kMaxBatch][LMOT_DESKEW_SLICES * 12], allocated
   // by lmot_set_deskew).  Reusing a block means its previous submission has completed, so the copy from it has too.
   float* h_deskew = nullptr;
+  // merging rig (lmot_set_rig_merge): the tick's sensors, 0 when it did not merge.  h_frame_counts rows 0..merge_rows-1 hold the
+  // sensors' (n_elev, n_ground, 0, 0) from rig_merge_kernel, row merge_rows the merged cloud's row from the concatenation; collect
+  // moves its num_cluster / n_boxes into row 0 (collect_result)
+  int merge_rows = 0;
 };
 
 // Detection slot: every buffer the three detection stages (ground -> cluster -> box) touch for ONE frame, plus the
@@ -330,6 +334,10 @@ struct Ctx {
   // ---- sensor rig (lmot_set_sensors): sensor k = frame k of a batched tick / list k of lmot_track_step_lists_dev; read at submission
   int n_sensors = 0;                   // 0: every frame uses prm, the rig kernels are never launched
   lmot_sensor sensors[kMaxBatch];
+  // merging rig (lmot_set_rig_merge): with a table set, the sensors' elevated clouds are clustered and boxed as one vehicle-frame cloud
+  // in the bank's merge unit (rig_merge.cu, allocated on the first merging submission).  Read at submission
+  bool rig_merge = false;
+  Slot merge_unit[kBatchBanks];
 
   // ---- result ring
   int n_results = 1;
@@ -363,6 +371,8 @@ struct Ctx {
   // a detection tick with any of them on runs every frame through the per-frame kernel variants (ground.cu, boxfit.cu)
   bool seq_det_on[kMaxBatch] = {};
   lmot_detect_params seq_det[kMaxBatch] = {};
+  bool seq_rig_merge[kMaxBatch] = {};         // lmot_seq_set_rig_merge; merge units per bank and merging sequence (first use)
+  Slot seq_merge_unit[kBatchBanks][kMaxBatch];
   int seq_fc_n[kMaxBatch] = {};                // lmot_seq_frame_counts: frames of sequence k in the tick collected last
   int seq_fc[kMaxBatch][kMaxBatch][4] = {};    // ... and their n_elev, n_ground, num_cluster, n_boxes (host copies: the ring slot is reused)
 
@@ -414,6 +424,15 @@ __device__ __forceinline__ void cart_mark(unsigned c, unsigned* __restrict__ onc
     if (__popc(grp) > 1) atomicOr(&twice[w], bit);
     else if (atomicOr(&once[w], bit) & bit) atomicOr(&twice[w], bit);
   }
+}
+
+// p' = [R | t] p (lmot_set_sensors): ((r0 x + r1 y) + r2 z) + t per row in float, no contraction -- pcl::transformPointCloud's
+// evaluation with an Affine3f.  m = row-major 3x4.  (Boxes of a rig: boxfit.cu; points of a merging rig: rig_merge.cu)
+__device__ __forceinline__ void rig_apply(const float* m, float& x, float& y, float& z) {
+  const float ox = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[0], x), __fmul_rn(m[1], y)), __fmul_rn(m[2], z)), m[3]);
+  const float oy = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[4], x), __fmul_rn(m[5], y)), __fmul_rn(m[6], z)), m[7]);
+  const float oz = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[8], x), __fmul_rn(m[9], y)), __fmul_rn(m[10], z)), m[11]);
+  x = ox; y = oy; z = oz;
 }
 #endif
 
@@ -482,5 +501,16 @@ int boxes_publish(Ctx* c, Slot* s, Result* r, cudaStream_t st);     // detection
 struct DeskewJob { const float* in; float4* out; const float* table; int n, stride; lmot_deskew d; };
 int deskew_table(const lmot_deskew& d, double v, double omega, const lmot_sensor* mount, float* out);
 int deskew_launch(Ctx* c, cudaStream_t st, const DeskewJob* jobs, int n_jobs);
+// merging rigs (rig_merge.cu).  A merge unit is a Slot with only the buffers clustering and box fitting of the merged cloud touch:
+// d_elev (the merged cloud), d_counters, d_cart, bit planes, label grid and the box-fitting set.
+int merge_unit_create(Ctx* c, Slot* u, int index);
+bool merge_unit_ready(const Slot* u);  // every buffer of the unit allocated (merge_unit_create succeeded)
+void merge_unit_destroy(Slot* u);      // frees whatever is allocated (also a partly created unit) and resets the slot
+// one launch over every merging unit of a submission: unit u gathers the elevated clouds of sensor slots src[s0[u] .. s0[u + 1]) moved by
+// their poses (pose[i] = sensor i's, in src order), writes its rows of the per-sensor counts to frame_counts[u] (device view of its
+// result block) and marks its own bit planes; the sensor slots' bit planes are returned to rest.  n_upper[i]: source i's frame size
+// (grid bound).  roi[u]: unit u's clustering ROI
+int rig_merge_launch(Ctx* c, cudaStream_t st, Slot* const* src, const lmot_sensor* pose, const int* n_upper, int n_units, const int* s0,
+                     Slot* const* units, int* const* frame_counts, const float* roi);
 
 }  // namespace lmot

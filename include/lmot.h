@@ -276,8 +276,8 @@ int lmot_batch_ground_ccl_dev(lmot_ctx* ctx, const float* const* d_points, const
  * The table is captured by value when a tick is submitted: ticks already in flight keep the table they were submitted with.  A tick or
  * list step with more frames than sensors is LMOT_ERR_INVALID while sensors are set.  Not affected: the stage entry points,
  * lmot_track_step, the single-stream lmot_frame* calls and sequence ticks (lmot_seq_*: each sequence has its own table,
- * lmot_seq_set_sensors).  Detections of one object by two sensors with overlapping fields of view
- * stay two measurements (the reference has no fusion step). */
+ * lmot_seq_set_sensors).  Detections of one object by two sensors with overlapping fields of view stay two measurements (the reference
+ * has no fusion step) unless the rig merges: lmot_set_rig_merge (below) clusters and boxes the sensors' elevated clouds as one. */
 typedef struct lmot_sensor {
   float pose[12];                 /* sensor -> vehicle frame, row-major 3x4 [R | t]; R orthonormal (|R^T R - I| <= 1e-5 elementwise) */
   float h_sensor, t_hmin, t_hmax; /* ground removal: replace lmot_params' values for this sensor's frames */
@@ -288,6 +288,43 @@ int lmot_default_sensor(const lmot_params* p, lmot_sensor* out);      /* identit
  * a non-finite value, a rotation that is not orthonormal */
 int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n);
 int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n);   /* *n = sensors set; copies min(n, cap) of them */
+
+/* ---- merging rigs: the sensors' elevated clouds clustered and boxed together in the VEHICLE frame ----------------------------------------
+ * With overlapping fields of view, separate detection gives an object seen by two sensors two boxes (two measurements, and a second track
+ * where the tracker spawns one for every unmatched box), and cuts an object on the edge between two fields of view in two.  A rig with
+ * merge on (off by default) and a table of F >= 1 sensors detects a tick as ONE cloud instead; a frame step of that rig gives, bit for bit:
+ *   1. ground removal per sensor, exactly as without merge: frame j (deskewed first if deskew is on) with sensor j's h_sensor / t_hmin /
+ *      t_hmax -> n_elevated[j], n_ground[j] and the order-preserving elevated cloud E_j in sensor j's frame;
+ *   2. the merged cloud E = E_0' | E_1' | ... | E_{F-1}' in table order, E_j' = every point of E_j moved by sensor j's pose with the rig's
+ *      arithmetic above (x' = ((r00*x + r01*y) + r02*z) + t0 and likewise y', z', in float without contraction), w = 1.  If |E| >
+ *      max_points, E is cut at max_points in that order and the step's status is LMOT_ERR_CAPACITY; the cut step's results and later
+ *      steps stay valid (the rule of an over-long list of lmot_seq_track_dev);
+ *   3. componentClustering(E) with roi_m, boxFitting(E, grid, numCluster) with the box-fitting values of lmot_params, or of the sequence's
+ *      lmot_detect_params if it has its own.  sensor_height is then the height of the VEHICLE frame's origin above the ground (box
+ *      bottoms and the height test); no sensor's sensor_height is read;
+ *   4. the boxes B, already in the vehicle frame, are the step's measurement list and lmot_batch_out.boxes (no pose applied again); with
+ *      global_frame = 1 they take the global-frame step as a rig's list does.
+ * That is: lmot_ground_remove(frame j) on a context created with sensor j's four values, for each j; the transform and concatenation
+ * above; lmot_component_cluster(E) + lmot_box_fit(E, ...) + lmot_track_step(B) on a context with the step's parameters.
+ * Counts: lmot_batch_out.n_elevated[j] / n_ground[j] per sensor; num_cluster[0] / n_boxes[0] the merged cloud's, the other entries 0;
+ * n_boxes_total = |B|.  lmot_seq_frame_counts(k) gives the same rows, and out->seq[k] their sums.
+ * Applies to the context's lmot_batch_submit / lmot_batch_dev / lmot_batch / lmot_batch_detect_dev while lmot_set_sensors holds a table,
+ * and to the FRAMES steps of sequence k (lmot_seq*, lmot_seq_tick*) while lmot_seq_set_sensors(k) holds one.  Without a table the setting
+ * has no effect and a tick runs exactly the launches it always did.  Never read by LISTS steps and lmot_seq_track*, the stage entry
+ * points, lmot_frame*, lmot_track_step*, lmot_batch_ground_ccl_dev and lmot_shared_*.
+ * Host state captured by value at submission, like the sensor tables: ticks in flight keep theirs.  lmot_seq_open turns it off for every
+ * sequence; lmot_seq_tracker_reset / _load and LMOT_SEQ_RESTART keep it.
+ * LMOT_ERR_INVALID, setting unchanged: on other than 0 or 1; k out of range or no open set.  LMOT_ERR_STATE, nothing submitted: a merging
+ * submission in timing mode.
+ * Memory: the first merging submission of the context allocates a merge unit per batch bank (2), and that of sequence k one per bank for
+ * it, synchronising the device once: the merged cloud and the clustering / box-fitting buffers of one frame, 36 B x max_points +
+ * 4 B x ceil(max_points / 1024) x (max_clusters + 1) + ~1 MB, about 55 MB at the default max_points and max_clusters: ~110 MB for the
+ * context's rig and ~110 MB per merging sequence (~880 MB with all 8 merging).  All or nothing: a failed allocation frees both banks' units
+ * and returns its error, and the next merging submission tries again.  Freed with the context (sequences: with the set). */
+int lmot_set_rig_merge(lmot_ctx* ctx, int on);
+int lmot_get_rig_merge(const lmot_ctx* ctx, int* on);
+int lmot_seq_set_rig_merge(lmot_ctx* ctx, int k, int on);
+int lmot_seq_get_rig_merge(const lmot_ctx* ctx, int k, int* on);
 
 /* ---- independent sequences: up to LMOT_MAX_BATCH frame streams per tick, each with its OWN track table ---------------------------
  * A sequence is an independent frame stream (one vehicle, one replayed log): it has its own track table, its own getOriginPoints
