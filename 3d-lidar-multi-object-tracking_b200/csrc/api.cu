@@ -105,9 +105,10 @@ int deskew_stage_host(Ctx* c, Slot* s, cudaStream_t st, const float* points, int
 // table; the frame's records d_raw (stride floats each) deskewed into the slot's point buffer, all on the slot stream
 int deskew_frame(Ctx* c, Slot* s, Result* r, const float* d_raw, int n, int stride, double ts, double v, double yaw) {
   if (n == 0) return LMOT_OK;
-  deskew_table(c->deskew, std::isfinite(v) ? v : 0.0, deskew_omega(c->own.th, ts, v, yaw), nullptr, r->h_deskew);
+  const lmot_deskew& d = c->own_cfg.deskew;
+  deskew_table(d, std::isfinite(v) ? v : 0.0, deskew_omega(c->own.th, ts, v, yaw), nullptr, r->h_deskew);
   LMOT_CUDA(c, cudaMemcpyAsync(s->d_deskew, r->h_deskew, kDeskewTabBytes, cudaMemcpyHostToDevice, s->stream));
-  const DeskewJob j{d_raw, s->d_points, s->d_deskew, n, stride, c->deskew};
+  const DeskewJob j{d_raw, s->d_points, s->d_deskew, n, stride, d};
   return deskew_launch(c, s->stream, &j, 1);
 }
 
@@ -169,7 +170,7 @@ Result* acquire_result(Ctx* c, bool drop_oldest) {
   }
   c->res_next = (c->res_next + 1) % c->n_results;
   c->last_res = r;
-  r->merge_rows = 0;                             // only a merging batched tick sets it (batch_submit): collect_result reads it
+  r->merge_rows = 0;                             // only a merging batched tick sets it (batch_common): collect_result reads it
   return r;
 }
 
@@ -282,7 +283,7 @@ int batch_ensure(Ctx* c, int F) {
 
 void batch_destroy(Ctx* c) {
   for (int i = 0; i < c->n_bslots; ++i) slot_destroy(&c->bslots[i]);
-  for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&c->merge_unit[b]);
+  for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&c->own_cfg.merge_unit[b]);
   for (int b = 0; b < kBatchBanks; ++b) {
     Slot* k = &c->bank[b];
     cudaFree(k->d_boxes); cudaFree(k->d_boxes_g); cudaFree(k->d_counters); cudaFree(k->d_det_sem); cudaFree(k->d_deskew);
@@ -293,81 +294,143 @@ void batch_destroy(Ctx* c) {
   }
 }
 
-// merge units of a merging rig: *units[b] of every bank, allocated on first use (one device synchronisation, as batch_ensure).  All or
-// nothing: a failed allocation frees the whole set, so a later submission retries from scratch instead of finding a half-built one.
-int merge_ensure(Ctx* c, Slot* const* units, int index) {
+// the merge units of a merging stream (StreamCfg::merge_unit, one per bank), allocated on first use (one device synchronisation, as
+// batch_ensure).  All or nothing: a failed allocation frees the whole set, so a later submission retries from scratch instead of finding
+// a half-built one.
+int merge_ensure(Ctx* c, Slot* units, int index) {
   bool ready = true;
-  for (int b = 0; b < kBatchBanks; ++b) ready &= merge_unit_ready(units[b]);
+  for (int b = 0; b < kBatchBanks; ++b) ready &= merge_unit_ready(&units[b]);
   if (ready) return LMOT_OK;
   int rc = LMOT_OK;
   for (int b = 0; b < kBatchBanks && rc == LMOT_OK; ++b)
-    if (!merge_unit_ready(units[b])) rc = merge_unit_create(c, units[b], index + b);
+    if (!merge_unit_ready(&units[b])) rc = merge_unit_create(c, &units[b], index + b);
   if (rc == LMOT_OK && cudaDeviceSynchronize() != cudaSuccess) rc = LMOT_ERR_CUDA;
   if (rc) {
     cudaDeviceSynchronize();           // (the allocators' memsets) before the buffers go back
-    for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(units[b]);
+    for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&units[b]);
   }
   return rc;
 }
 
-// one tick: F device-resident frames (slot buffers or caller pointers) -> batched ground / CCL / box fitting -> concatenated boxes
-// -> (optionally) the tracker.  d_pts[i] == nullptr: the frame was uploaded into the slot's own buffer.  A merging rig
-// (lmot_set_rig_merge, units allocated by batch_common) clusters and boxes the sensors' elevated clouds as one, in the bank's merge unit.
-int batch_submit(Ctx* c, int bank_i, Result* r, const float4* const* d_pts, const int* n, int F, bool with_tracker, double ts, double v, double yaw) {
+// ---- the detection front end of batched and sequence ticks: frames -> box-fitted units ---------------------------------------------
+// A tick's frames come in groups, one per stream: a batched tick is one group (the context's own settings and fold), a sequence tick
+// has one per FRAMES sequence.  Frame j of a group is its sensor j's.
+struct DetGroup {
+  StreamCfg* cfg;                      // the stream's settings and merge units
+  const TrackerHost* th;               // the fold the frames' motion is taken from (nullptr: frames without a stamp, never deskewed)
+  const float* const* data;            // nf frames (host: stride floats per point; device: float4) of n[j] points
+  const int* n;
+  int nf;
+  double ts, v, yaw;
+  int* fc;                             // device view of the stream's per-frame counts in its result block (nullptr: none are written)
+};
+
+// what the front end box-fitted, by group: group g's units are u[f0[g] .. f0[g + 1]) (its frames, or its merge unit), unit i with pose
+// rig[i], which applies to its boxes iff rig_on[g]; the concatenation writes the group's count rows from fc[g] on
+struct DetUnits {
+  Slot* u[kMaxBatch];
+  lmot_sensor rig[kMaxBatch];
+  int f0[kMaxBatch + 1];
+  bool rig_on[kMaxBatch];
+  int* fc[kMaxBatch];
+};
+
+// G groups of frames on bank b's detection slots, in group order, all on the first slot's stream, for the bank's result block
+// (bank[b].res): staging (host frames uploaded, device frames read in place), deskew (tables into the pinned block h_dsk, one copy, one
+// launch), ground removal, the merging groups' elevated clouds into their merge units, clustering, box fitting.  post_sem: every unit's
+// last box-fitting CTA posts the unit's semaphore (nothing concatenates its list).
+//   Ground removal gets the tick's pose table iff some group has a sensor table, box fitting iff some unit is an unmerged frame of such
+// a group (a frame without a table: lmot_default_sensor); both get per-frame detection values iff some group has its own (sensor values
+// folded in).  A merge unit is the vehicle's cloud: identity pose, the group's detection values without a sensor's, at most max_points
+// points.  Clustering runs in the ground kernel's tail (fuse_ccl) unless a group merges in between.
+int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host, float* h_dsk, bool post_sem, DetUnits& U) {
   int rc;
-  struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
-  Slot* k = &c->bank[bank_i];
+  Slot* bk = &c->bank[b];
   Slot* sl[kMaxBatch];
   const float4* pp[kMaxBatch];
-  for (int i = 0; i < F; ++i) { sl[i] = &c->bslots[bank_i * c->batch_frames + i]; pp[i] = d_pts[i] ? d_pts[i] : sl[i]->d_points; }
-  const lmot_sensor* rig = c->n_sensors > 0 ? c->sensors : nullptr;     // copied into the launches' parameters: later changes leave this tick alone
-  cudaStream_t st = sl[0]->stream;
-  k->res = r; sl[0]->res = r;
-  r->n_kev = 0;
-  r->batch_frames = F;
-  int* d_fc = nullptr;                       // the per-frame counts go straight into the result's pinned, device-mapped block
-  LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&d_fc, r->h_frame_counts, 0));
-  const bool gf = with_tracker && c->prm.global_frame;
-  const bool merge = rig && c->rig_merge;
-  r->merge_rows = merge ? F : 0;
-  if (!merge) {
-    if (c->timing) cudaEventRecord(r->ev[0], st);
-    if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, c->fuse_ccl, false, rig))) return rc;
-    if (c->timing) cudaEventRecord(r->ev[1], st);
-    if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
-    if (c->timing) cudaEventRecord(r->ev[2], st);
-    if ((rc = boxfit_launch_batch(c, sl, F, st, n, false, rig))) return rc;
-    if ((rc = boxes_concat_launch(c, sl, F, st, k->d_boxes, k->d_counters, d_fc, (with_tracker && !gf) ? k->d_det_sem : nullptr, rig))) return rc;
-  } else {
-    // ground per sensor (CCL not fused: nothing clusters the sensors' frames), the sensors' elevated clouds into the merge unit, then
-    // clustering and box fitting of that one cloud with lmot_params' values, and its box list as the tick's (already vehicle frame)
-    Slot* u[1] = {&c->merge_unit[bank_i]};
-    const int s0[2] = {0, F};
-    int* fcu[1] = {d_fc};
-    const float roi[1] = {c->prm.roi_m};
-    long long tot = 0;
-    for (int i = 0; i < F; ++i) tot += n[i];
-    const int nu[1] = {(int)(tot < c->max_points ? tot : c->max_points)};
-    if ((rc = ground_launch_batch(c, sl, F, pp, n, st, true, false, false, false, rig))) return rc;
-    if ((rc = rig_merge_launch(c, st, sl, rig, n, 1, s0, u, fcu, roi))) return rc;
-    if ((rc = ccl_launch_batch(c, u, 1, st))) return rc;
-    if ((rc = boxfit_launch_batch(c, u, 1, st, nu, false))) return rc;
-    if ((rc = boxes_concat_launch(c, u, 1, st, k->d_boxes, k->d_counters, d_fc + 4 * F, (with_tracker && !gf) ? k->d_det_sem : nullptr))) return rc;
+  int nn[kMaxBatch], F = 0, nj = 0;
+  lmot_sensor rig[kMaxBatch];
+  DeskewJob dj[kMaxBatch];
+  bool rigged = false, own_det = false, merging = false;
+  cudaStream_t st = c->bslots[b * c->batch_frames].stream;
+  c->bslots[b * c->batch_frames].res = bk->res;      // (kernel_mark)
+  for (int d = 0; d < G; ++d) {
+    const StreamCfg& q = *g[d].cfg;
+    const bool tab = q.n_sensors > 0, dsk = g[d].th && q.deskew.on;
+    rigged |= tab; own_det |= q.det_on; merging |= q.merges();
+    const double om = dsk ? deskew_omega(*g[d].th, g[d].ts, g[d].v, g[d].yaw) : 0.0, vv = std::isfinite(g[d].v) ? g[d].v : 0.0;
+    for (int j = 0; j < g[d].nf; ++j, ++F) {
+      Slot* s = sl[F] = &c->bslots[b * c->batch_frames + F];
+      nn[F] = g[d].n[j];
+      if (tab) rig[F] = q.sensors[j];
+      else lmot_default_sensor(&c->prm, &rig[F]);
+      pp[F] = s->d_points;
+      if (dsk) {                       // the frame with its sensor's mount and its stream's fold
+        const float* raw = g[d].data[j];
+        if (host && (rc = deskew_stage_host(c, s, st, g[d].data[j], nn[F], stride, &raw))) return rc;
+        deskew_table(q.deskew, vv, om, tab ? &q.sensors[j] : nullptr, h_dsk + (size_t)F * kDeskewTab);
+        dj[nj++] = DeskewJob{raw, s->d_points, bk->d_deskew + (size_t)F * kDeskewTab, nn[F], host ? stride : 4, q.deskew};
+      } else if (host) {
+        if ((rc = upload_points(c, s, st, g[d].data[j], nn[F], stride, s->d_points))) return rc;
+      } else {
+        pp[F] = reinterpret_cast<const float4*>(g[d].data[j]);
+      }
+    }
   }
-  if (gf && (rc = boxes_to_global_launch(c, k, st, k->d_boxes, k->d_counters, ts, v, yaw, true))) return rc;
-  if (c->timing) cudaEventRecord(r->ev[3], st);
-  LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, st));
-  if (with_tracker) {
-    if ((rc = submit_tracker(c, k, r, k->d_boxes, k->d_counters, ts, v, yaw))) return rc;
-  } else {
-    LMOT_CUDA(c, cudaMemcpyAsync(r->h_det, k->d_counters, CNT_COUNT * sizeof(int), cudaMemcpyDeviceToHost, st));
-    if ((rc = boxes_publish(c, k, r, st))) return rc;
-    LMOT_CUDA(c, cudaEventRecord(k->ev_trk_done, st));
-    LMOT_CUDA(c, cudaEventRecord(r->ev_done, st));
+  if (nj > 0) {                        // frame i's table at table i of the bank
+    LMOT_CUDA(c, cudaMemcpyAsync(bk->d_deskew, h_dsk, (size_t)F * kDeskewTabBytes, cudaMemcpyHostToDevice, st));
+    if ((rc = deskew_launch(c, st, dj, nj))) return rc;
   }
-  r->has_tracks = with_tracker;
-  if (!r->in_flight) { r->in_flight = true; ++c->n_in_flight; }
-  return LMOT_OK;
+  // per-frame detection values and the units (copied into the launch parameters: later setting changes leave this tick alone)
+  const lmot_detect_params base = detect_params_of(c->prm);
+  lmot_detect_params det[kMaxBatch], udet[kMaxBatch];
+  Slot* src[kMaxBatch];
+  Slot* mu[kMaxBatch];
+  lmot_sensor mpose[kMaxBatch];
+  int mn[kMaxBatch], ms0[kMaxBatch + 1], *mfc[kMaxBatch], unn[kMaxBatch], nm = 0, nsrc = 0, nu = 0;
+  float mroi[kMaxBatch];
+  bool rig_fit = false;
+  ms0[0] = 0;
+  for (int d = 0, i0 = 0; d < G; i0 += g[d].nf, ++d) {
+    StreamCfg& q = *g[d].cfg;
+    const lmot_detect_params& vd = q.det_on ? q.det : base;
+    if (own_det)
+      for (int i = i0; i < i0 + g[d].nf; ++i) {
+        det[i] = vd;
+        if (q.n_sensors > 0) {
+          const lmot_sensor& s = rig[i];
+          det[i].h_sensor = s.h_sensor; det[i].t_hmin = s.t_hmin; det[i].t_hmax = s.t_hmax; det[i].sensor_height = s.sensor_height;
+        }
+      }
+    U.f0[d] = nu;
+    U.rig_on[d] = q.n_sensors > 0 && !q.merges();
+    U.fc[d] = g[d].fc;
+    if (q.merges()) {
+      long long tot = 0;
+      for (int i = i0; i < i0 + g[d].nf; ++i) { src[nsrc] = sl[i]; mpose[nsrc] = rig[i]; mn[nsrc] = nn[i]; ++nsrc; tot += nn[i]; }
+      mu[nm] = &q.merge_unit[b]; mfc[nm] = g[d].fc; mroi[nm] = vd.roi_m;
+      ms0[++nm] = nsrc;
+      U.u[nu] = mu[nm - 1];
+      lmot_default_sensor(&c->prm, &U.rig[nu]);
+      udet[nu] = vd;
+      unn[nu] = (int)(tot < c->max_points ? tot : c->max_points);
+      ++nu;
+      U.fc[d] += 4 * g[d].nf;         // behind the sensors' rows, which rig_merge_kernel writes
+    } else {
+      for (int i = i0; i < i0 + g[d].nf; ++i) { U.u[nu] = sl[i]; U.rig[nu] = rig[i]; if (own_det) udet[nu] = det[i]; unn[nu] = nn[i]; ++nu; }
+      rig_fit |= U.rig_on[d];
+    }
+  }
+  U.f0[G] = nu;
+  const bool fuse = c->fuse_ccl && !merging;
+  Result* r = bk->res;
+  if (c->timing) cudaEventRecord(r->ev[0], st);
+  if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, fuse, false, rigged ? rig : nullptr, own_det ? det : nullptr))) return rc;
+  if (c->timing) cudaEventRecord(r->ev[1], st);
+  if (nm > 0 && (rc = rig_merge_launch(c, st, src, mpose, mn, nm, ms0, mu, mfc, mroi))) return rc;
+  if (!fuse && (rc = ccl_launch_batch(c, U.u, nu, st))) return rc;
+  if (c->timing) cudaEventRecord(r->ev[2], st);
+  return boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr);
 }
 
 // the IDs of a result being returned (lmot_track_ids): copied now, the block is reused by later submissions
@@ -515,10 +578,10 @@ void seq_destroy(Ctx* c) {
       m = SeqMeas{};
     }
   for (int b = 0; b < kBatchBanks; ++b) { cudaFree(c->seq_stage[b]); c->seq_stage[b] = nullptr; }
-  for (int k = 0; k < kMaxBatch; ++k) { c->seq_n_sensors[k] = 0; c->seq_fc_n[k] = 0; c->seq_det_on[k] = false; c->seq_deskew[k] = deskew_defaults(); }
   for (int k = 0; k < kMaxBatch; ++k) {
-    c->seq_rig_merge[k] = false;
-    for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&c->seq_merge_unit[b][k]);
+    for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&c->seq_cfg[k].merge_unit[b]);
+    c->seq_cfg[k] = StreamCfg{};
+    c->seq_fc_n[k] = 0;
   }
   for (int i = 0; i < c->seq_ring; ++i) {
     for (int k = 0; k < c->n_seq; ++k) result_destroy(&c->seq_ticks[i].blocks[k]);
@@ -956,9 +1019,9 @@ int lmot_detect_dev(lmot_ctx* ctx, const float* d_points, int n) {
 int lmot_frame_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp_us, double v_gps, double yaw_gps) {
   if (!ctx || n < 0 || (n > 0 && !d_points) || (reinterpret_cast<uintptr_t>(d_points) & 15u)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  const bool dsk = c->deskew.on != 0;
+  const bool dsk = c->own_cfg.deskew.on != 0;
   if (dsk && c->timing) return LMOT_ERR_STATE;
-  if (dsk && c->deskew.time_field != 3) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
+  if (dsk && c->own_cfg.deskew.time_field != 3) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
   Slot* s = acquire_slot(c);
@@ -978,10 +1041,10 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
-  const bool dsk = c->deskew.on != 0;
+  const bool dsk = c->own_cfg.deskew.on != 0;
   if (dsk) {                           // (validated before anything is submitted: upload_points checks the rest without deskew)
     if (c->timing) return LMOT_ERR_STATE;
-    if (n < 0 || (n > 0 && !points) || stride <= c->deskew.time_field) return LMOT_ERR_INVALID;
+    if (n < 0 || (n > 0 && !points) || stride <= c->own_cfg.deskew.time_field) return LMOT_ERR_INVALID;
     if (n > c->max_points) return LMOT_ERR_CAPACITY;
   }
   if (c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;    // result ring full: collect first
@@ -1069,64 +1132,67 @@ int lmot_frame(lmot_ctx* ctx, const float* points, int n, int stride, double tim
 }
 
 // ---------------------------------------------------------------------------------------------- batched ticks
+// one tick: F frames of the context's own stream -> the detection front end on the next bank -> concatenated boxes -> (optionally) the
+// tracker.  A merging rig (lmot_set_rig_merge) concatenates the bank's merge unit, its boxes already in the vehicle frame.
 static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n, int n_frames, int stride, bool host, bool with_tracker,
                         double ts, double v, double yaw) {
   if (!ctx || !points || !n || n_frames < 1 || n_frames > kMaxBatch) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  if (c->n_sensors > 0 && n_frames > c->n_sensors) return LMOT_ERR_INVALID;     // a frame without a sensor pose
+  StreamCfg& q = c->own_cfg;
+  if (q.n_sensors > 0 && n_frames > q.n_sensors) return LMOT_ERR_INVALID;     // a frame without a sensor pose
   cudaSetDevice(c->device);
   for (int i = 0; i < n_frames; ++i) {
     if (n[i] < 0 || (n[i] > 0 && !points[i])) return LMOT_ERR_INVALID;
     if (n[i] > c->max_points) return LMOT_ERR_CAPACITY;
     if (!host && n[i] > 0 && (reinterpret_cast<uintptr_t>(points[i]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies need 16-byte alignment
   }
-  const bool dsk = with_tracker && c->deskew.on != 0;               // (lmot_batch_detect_dev has no stamp: never deskewed)
+  const bool dsk = with_tracker && q.deskew.on != 0;                // (lmot_batch_detect_dev has no stamp: never deskewed)
   if (dsk && c->timing) return LMOT_ERR_STATE;
-  if (dsk && (host ? stride <= c->deskew.time_field : c->deskew.time_field != 3)) return LMOT_ERR_INVALID;
-  const bool merge = c->rig_merge && c->n_sensors > 0;
-  if (merge && c->timing) return LMOT_ERR_STATE;
+  if (dsk && (host ? stride <= q.deskew.time_field : q.deskew.time_field != 3)) return LMOT_ERR_INVALID;
+  if (q.merges() && c->timing) return LMOT_ERR_STATE;
   if (host && c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;
   int rc = batch_ensure(c, n_frames);
   if (rc) return rc;
-  Slot* const units[kBatchBanks] = {&c->merge_unit[0], &c->merge_unit[1]};
-  if (merge && (rc = merge_ensure(c, units, 3000))) return rc;
+  if (q.merges() && (rc = merge_ensure(c, q.merge_unit, 3000))) return rc;
   Result* r = acquire_result(c, !host);
   if (!r) return LMOT_ERR_STATE;
   const int b = c->next_bank;
   c->next_bank = (c->next_bank + 1) % kBatchBanks;
   Slot* k = &c->bank[b];
-  Slot* s0 = &c->bslots[b * c->batch_frames];
-  cudaStream_t st = s0->stream;
+  cudaStream_t st = c->bslots[b * c->batch_frames].stream;
   // the bank's previous tick must have been consumed by the tracker; device frames: ordered after the caller's stream
   LMOT_CUDA(c, cudaStreamWaitEvent(st, k->ev_trk_done, 0));
-  const float4* dp[kMaxBatch];
-  const float* raw[kMaxBatch];
-  if (host) {
-    for (int i = 0; i < n_frames; ++i) {
-      Slot* s = &c->bslots[b * c->batch_frames + i];
-      if (dsk) rc = deskew_stage_host(c, s, st, points[i], n[i], stride, &raw[i]);
-      else rc = upload_points(c, s, st, points[i], n[i], stride, s->d_points);
-      if (rc) return rc;
-      dp[i] = nullptr;
-    }
-  } else {
+  if (!host) {
     LMOT_CUDA(c, cudaEventRecord(k->ev_fork, c->stream));
     LMOT_CUDA(c, cudaStreamWaitEvent(st, k->ev_fork, 0));
-    for (int i = 0; i < n_frames; ++i) { dp[i] = reinterpret_cast<const float4*>(points[i]); raw[i] = points[i]; }
   }
-  if (dsk) {
-    // every sensor's frame with its own mount (the rig table, captured here) and the context's fold; one table copy, one launch
-    const double om = deskew_omega(c->own.th, ts, v, yaw), vv = std::isfinite(v) ? v : 0.0;
-    DeskewJob jobs[kMaxBatch];
-    for (int i = 0; i < n_frames; ++i) {
-      deskew_table(c->deskew, vv, om, c->n_sensors > 0 ? &c->sensors[i] : nullptr, r->h_deskew + (size_t)i * kDeskewTab);
-      jobs[i] = DeskewJob{raw[i], c->bslots[b * c->batch_frames + i].d_points, k->d_deskew + (size_t)i * kDeskewTab, n[i], host ? stride : 4, c->deskew};
-      dp[i] = nullptr;
-    }
-    LMOT_CUDA(c, cudaMemcpyAsync(k->d_deskew, r->h_deskew, (size_t)n_frames * kDeskewTabBytes, cudaMemcpyHostToDevice, st));
-    if ((rc = deskew_launch(c, st, jobs, n_frames))) return rc;
+  struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
+  k->res = r;
+  r->n_kev = 0;
+  r->batch_frames = n_frames;
+  r->merge_rows = q.merges() ? n_frames : 0;
+  int* d_fc = nullptr;                       // the per-frame counts go straight into the result's pinned, device-mapped block
+  LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&d_fc, r->h_frame_counts, 0));
+  const DetGroup grp{&q, with_tracker ? &c->own.th : nullptr, points, n, n_frames, ts, v, yaw, d_fc};
+  DetUnits U;
+  if ((rc = detect_front(c, b, &grp, 1, stride, host, r->h_deskew, false, U))) return rc;
+  const bool gf = with_tracker && c->prm.global_frame;
+  if ((rc = boxes_concat_launch(c, U.u, U.f0[1], st, k->d_boxes, k->d_counters, U.fc[0], (with_tracker && !gf) ? k->d_det_sem : nullptr,
+                                U.rig_on[0] ? U.rig : nullptr))) return rc;
+  if (gf && (rc = boxes_to_global_launch(c, k, st, k->d_boxes, k->d_counters, ts, v, yaw, true))) return rc;
+  if (c->timing) cudaEventRecord(r->ev[3], st);
+  LMOT_CUDA(c, cudaEventRecord(k->ev_det_done, st));
+  if (with_tracker) {
+    if ((rc = submit_tracker(c, k, r, k->d_boxes, k->d_counters, ts, v, yaw))) return rc;
+  } else {
+    LMOT_CUDA(c, cudaMemcpyAsync(r->h_det, k->d_counters, CNT_COUNT * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if ((rc = boxes_publish(c, k, r, st))) return rc;
+    LMOT_CUDA(c, cudaEventRecord(k->ev_trk_done, st));
+    LMOT_CUDA(c, cudaEventRecord(r->ev_done, st));
   }
-  return batch_submit(c, b, r, dp, n, n_frames, with_tracker, ts, v, yaw);
+  r->has_tracks = with_tracker;
+  if (!r->in_flight) { r->in_flight = true; ++c->n_in_flight; }
+  return LMOT_OK;
 }
 
 int lmot_batch_submit(lmot_ctx* ctx, const float* const* points, const int* n, int n_frames, int stride_floats, double timestamp_us,
@@ -1147,7 +1213,7 @@ int lmot_batch_detect_dev(lmot_ctx* ctx, const float* const* d_points, const int
 int lmot_batch_ground_ccl_dev(lmot_ctx* ctx, const float* const* d_points, const int* n, int n_frames) {
   if (!ctx || !d_points || !n || n_frames < 1 || n_frames > kMaxBatch) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  if (c->n_sensors > 0 && n_frames > c->n_sensors) return LMOT_ERR_INVALID;
+  if (c->own_cfg.n_sensors > 0 && n_frames > c->own_cfg.n_sensors) return LMOT_ERR_INVALID;
   cudaSetDevice(c->device);
   int rc = batch_ensure(c, n_frames);
   if (rc) return rc;
@@ -1160,7 +1226,7 @@ int lmot_batch_ground_ccl_dev(lmot_ctx* ctx, const float* const* d_points, const
   }
   sl[0]->res = &c->results[0];
   c->results[0].n_kev = 0;
-  if ((rc = ground_launch_batch(c, sl, n_frames, pp, n, c->stream, true, false, c->fuse_ccl, c->fuse_ccl, c->n_sensors > 0 ? c->sensors : nullptr))) return rc;
+  if ((rc = ground_launch_batch(c, sl, n_frames, pp, n, c->stream, true, false, c->fuse_ccl, c->fuse_ccl, c->own_cfg.n_sensors > 0 ? c->own_cfg.sensors : nullptr))) return rc;
   return c->fuse_ccl ? LMOT_OK : ccl_launch_batch(c, sl, n_frames, c->stream);
 }
 
@@ -1255,14 +1321,14 @@ int lmot_seq_open(lmot_ctx* ctx, int n_seq, int ring) {
 }
 
 // ---- sequence ticks: one builder (seq_tick_common) for lmot_seq_tick_*, lmot_seq* (every entry FRAMES) and lmot_seq_track* (every entry
-// LISTS).  A tick's entries say, per sequence, whether it steps this tick and from what: FRAMES entries go through detection (ground
-// removal, clustering, box fitting), LISTS entries through one pack launch; both fill the stepped sequences' measurement lists, and ONE
-// tracker chain steps the stepped tables.  Every tick shares the ring and the bank alternation; each table folds its steps in submission
-// order.
+// LISTS).  A tick's entries say, per sequence, whether it steps this tick and from what: FRAMES entries go through the detection front
+// end (detect_front, one group per sequence), LISTS entries through one pack launch; both fill the stepped sequences' measurement lists,
+// and ONE tracker chain steps the stepped tables.  Every tick shares the ring and the bank alternation; each table folds its steps in
+// submission order.
 //
 // The map: the stepped sequences, in sequence order, are the chain positions 0..S-1 (seq[pos] = sequence).  The FRAMES entries' frames
 // are the detection slots in that order, the LISTS entries' lists the pack's lists in that order.  Every per-sequence array handed to a
-// launch (measurement lists, ego values, rig poses, frame-count pointers, result blocks, detection values) is built through it.
+// launch (measurement lists, ego values, rig poses, frame-count pointers, result blocks) is built through it.
 
 // the set's layout: sequence k's sensors in table order, [f0[k], f0[k + 1]); one for a sequence without a table (lmot_seq_set_sensors
 // keeps the total at or below kMaxBatch).  -> whether any sequence has a table
@@ -1270,9 +1336,9 @@ static bool seq_layout(const Ctx* c, int* f0, bool* rig_on) {
   bool rigged = false;
   f0[0] = 0;
   for (int k = 0; k < c->n_seq; ++k) {
-    rig_on[k] = c->seq_n_sensors[k] > 0;
+    rig_on[k] = c->seq_cfg[k].n_sensors > 0;
     rigged |= rig_on[k];
-    f0[k + 1] = f0[k] + (rig_on[k] ? c->seq_n_sensors[k] : 1);
+    f0[k + 1] = f0[k] + (rig_on[k] ? c->seq_cfg[k].n_sensors : 1);
   }
   return rigged;
 }
@@ -1298,7 +1364,7 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
   seq_layout(c, f0, rig_on);
   // validation: nothing is submitted unless the whole tick is valid
   int S = 0, F = 0, FL = 0;            // stepped sequences, detection frames, lists
-  bool rigged = false, own_det = false, merging = false;
+  bool rigged = false;
   bool merge[kMaxBatch] = {};          // FRAMES sequences with a table and lmot_seq_set_rig_merge on: one merged cloud per sequence
   for (int k = 0; k < n_seq; ++k) {
     const lmot_seq_entry& q = e[k];
@@ -1313,14 +1379,10 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
       if (q.n[j] < 0 || (q.n[j] > 0 && !q.data[j])) return LMOT_ERR_INVALID;
       if (!host && q.kind == LMOT_SEQ_FRAMES && q.n[j] > 0 && (reinterpret_cast<uintptr_t>(q.data[j]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies
     }
-    if (q.kind == LMOT_SEQ_FRAMES && c->seq_deskew[k].on && (host ? stride <= c->seq_deskew[k].time_field : c->seq_deskew[k].time_field != 3))
-      return LMOT_ERR_INVALID;
+    const lmot_deskew& dk = c->seq_cfg[k].deskew;
+    if (q.kind == LMOT_SEQ_FRAMES && dk.on && (host ? stride <= dk.time_field : dk.time_field != 3)) return LMOT_ERR_INVALID;
     ++S;
-    if (q.kind == LMOT_SEQ_FRAMES) {
-      F += nk; rigged |= rig_on[k]; own_det |= c->seq_det_on[k];
-      merge[k] = rig_on[k] && c->seq_rig_merge[k];
-      merging |= merge[k];
-    }
+    if (q.kind == LMOT_SEQ_FRAMES) { F += nk; rigged |= rig_on[k]; merge[k] = c->seq_cfg[k].merges(); }
     else FL += nk;
   }
   if (S == 0 || (host && F > 0 && stride < 3)) return LMOT_ERR_INVALID;
@@ -1339,11 +1401,8 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
     if ((rc = bank_ensure(c))) return rc;
     LMOT_CUDA(c, cudaDeviceSynchronize());
   }
-  for (int k = 0; k < n_seq; ++k) {
-    if (!merge[k]) continue;
-    Slot* const units[kBatchBanks] = {&c->seq_merge_unit[0][k], &c->seq_merge_unit[1][k]};
-    if ((rc = merge_ensure(c, units, 4000 + 16 * k))) return rc;
-  }
+  for (int k = 0; k < n_seq; ++k)
+    if (merge[k] && (rc = merge_ensure(c, c->seq_cfg[k].merge_unit, 4000 + 16 * k))) return rc;
   // the tick's ring slot and bank; the front end runs on the bank's first detection slot's stream (on the bank's own stream when no
   // sequence sends frames), after the bank's previous tick has been consumed by the tracker
   SeqTick* t = seq_acquire(c, !host);
@@ -1407,7 +1466,7 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
         } else {
           L.lists[i] = e[k].data[j]; L.counts[i] = e[k].d_counts + j; L.cap[i] = e[k].cap_per_list;
         }
-        if (rig_on[k]) rig[i] = c->seq_sensors[k][j];
+        if (rig_on[k]) rig[i] = c->seq_cfg[k].sensors[j];
         else lmot_default_sensor(&c->prm, &rig[i]);
       }
       lrig[nl] = rig_on[k];
@@ -1419,138 +1478,26 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
     if ((rc = boxes_pack_lists_seq_launch(c, st, L, nl, lf0, lrig, rig, lm, fc, !gf))) return rc;
   }
   if (F > 0) {
-    // FRAMES entries: the frames of the FRAMES sequences on the bank's detection slots, in sequence order
-    Slot* sl[kMaxBatch];
-    const float4* pp[kMaxBatch];
-    int nn[kMaxBatch], df0[kMaxBatch + 1], dseq[kMaxBatch], nd = 0;
-    bool drig[kMaxBatch];
-    for (int i = 0; i < F; ++i) sl[i] = &c->bslots[b * c->batch_frames + i];
-    df0[0] = 0;
-    DeskewJob dj[kMaxBatch];           // deskewing sequences (lmot_seq_set_deskew): their frames, each with its sequence's fold and mount
-    int nj = 0;
+    // FRAMES entries: one group per FRAMES sequence, in sequence order.  Without a table each frame's last box-fitting CTA (or, global_frame,
+    // its boxes_to_global CTA) posts the semaphore of the frame's own list, which the tick's gate kernel polls; with one, each sequence's
+    // frames are concatenated into its own list and that semaphore is polled
+    DetGroup g[kMaxBatch];
+    int gk[kMaxBatch], G = 0;
     for (int k = 0; k < n_seq; ++k) {
       if (e[k].kind != LMOT_SEQ_FRAMES) continue;
-      const lmot_deskew& dk = c->seq_deskew[k];
-      const double om = dk.on ? deskew_omega(c->seq[k].th, e[k].timestamp_us, e[k].v_gps, e[k].yaw_gps) : 0.0;   // (after a restart above)
-      const double vv = std::isfinite(e[k].v_gps) ? e[k].v_gps : 0.0;
-      for (int j = 0; j < f0[k + 1] - f0[k]; ++j) {
-        const int i = df0[nd] + j;
-        nn[i] = e[k].n[j];
-        if (dk.on) {
-          const float* raw = reinterpret_cast<const float*>(e[k].data[j]);
-          if (host && (rc = deskew_stage_host(c, sl[i], st, e[k].data[j], nn[i], stride, &raw))) return rc;
-          deskew_table(dk, vv, om, rig_on[k] ? &c->seq_sensors[k][j] : nullptr, t->h_deskew + (size_t)i * kDeskewTab);
-          dj[nj++] = DeskewJob{raw, sl[i]->d_points, bk->d_deskew + (size_t)i * kDeskewTab, nn[i], host ? stride : 4, dk};
-          pp[i] = sl[i]->d_points;
-        } else if (host) {
-          if ((rc = upload_points(c, sl[i], st, e[k].data[j], nn[i], stride, sl[i]->d_points))) return rc;
-          pp[i] = sl[i]->d_points;
-        } else {
-          pp[i] = reinterpret_cast<const float4*>(e[k].data[j]);
-        }
-      }
-      dseq[nd] = k; drig[nd] = rig_on[k];
-      df0[nd + 1] = df0[nd] + f0[k + 1] - f0[k];
-      ++nd;
+      int* fc = nullptr;
+      if (rigged) LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc, t->blocks[k].h_frame_counts, 0));
+      gk[G] = k;
+      g[G++] = DetGroup{&c->seq_cfg[k], &c->seq[k].th, e[k].data, e[k].n, f0[k + 1] - f0[k], e[k].timestamp_us, e[k].v_gps, e[k].yaw_gps, fc};
     }
-    if (nj > 0) {                      // the tick's tables in one copy (frame i's at table i of the bank), then one launch
-      LMOT_CUDA(c, cudaMemcpyAsync(bk->d_deskew, t->h_deskew, (size_t)F * kDeskewTabBytes, cudaMemcpyHostToDevice, st));
-      if ((rc = deskew_launch(c, st, dj, nj))) return rc;
+    DetUnits U;
+    if ((rc = detect_front(c, b, g, G, stride, host, t->h_deskew, !rigged && !gf, U))) return rc;
+    SeqMeas dm[kMaxBatch];
+    for (int d = 0; d < G; ++d) {
+      const Slot* s = U.u[U.f0[d]];
+      dm[d] = mk[gk[d]] = rigged ? c->seq_meas[b][gk[d]] : SeqMeas{s->d_boxes, s->d_boxes_g, s->d_counters, s->d_det_sem};
     }
-    sl[0]->res = bk->res;
-    // sequences with their own detection values: every frame of the tick gets its entry (copied into the launch parameters), the values
-    // of its sequence -- or lmot_params' -- with its sensor's four mounting values in place of h_sensor / t_hmin / t_hmax / sensor_height
-    lmot_detect_params det[kMaxBatch];
-    if (own_det) {
-      const lmot_detect_params base = detect_params_of(c->prm);
-      for (int d = 0; d < nd; ++d) {
-        const int k = dseq[d];
-        for (int i = df0[d]; i < df0[d + 1]; ++i) {
-          det[i] = c->seq_det_on[k] ? c->seq_det[k] : base;
-          if (drig[d]) {
-            const lmot_sensor& s = c->seq_sensors[k][i - df0[d]];
-            det[i].h_sensor = s.h_sensor; det[i].t_hmin = s.t_hmin; det[i].t_hmax = s.t_hmax; det[i].sensor_height = s.sensor_height;
-          }
-        }
-      }
-    }
-    if (!rigged) {
-      // detection: the batched launches of lmot_batch_* without a rig; each frame's last box-fitting CTA (or, global_frame, its
-      // boxes_to_global CTA) posts its own slot's semaphore, which the tick's gate kernel polls
-      for (int d = 0; d < nd; ++d) {         // (one frame per sequence: slot df0[d] == d)
-        Slot* s = sl[df0[d]];
-        mk[dseq[d]] = SeqMeas{s->d_boxes, s->d_boxes_g, s->d_counters, s->d_det_sem};
-      }
-      if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, c->fuse_ccl, false, nullptr, own_det ? det : nullptr))) return rc;
-      if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
-      if ((rc = boxfit_launch_batch(c, sl, F, st, nn, !gf, nullptr, own_det ? det : nullptr))) return rc;
-    } else {
-      // detection with one sensor per frame (sequences without a table: lmot_params' values), copied into the launch parameters (later
-      // table changes leave this tick alone); then each sequence's frames into its own list, whose semaphore the gate kernel polls
-      lmot_sensor rig[kMaxBatch];
-      int* fc[kMaxBatch];
-      SeqMeas dm[kMaxBatch];
-      for (int d = 0; d < nd; ++d) {
-        const int k = dseq[d];
-        for (int i = df0[d]; i < df0[d + 1]; ++i) {
-          if (drig[d]) rig[i] = c->seq_sensors[k][i - df0[d]];
-          else lmot_default_sensor(&c->prm, &rig[i]);
-        }
-        dm[d] = mk[k] = c->seq_meas[b][k];
-        LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc[d], t->blocks[k].h_frame_counts, 0));
-      }
-      if (!merging) {
-        if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, c->fuse_ccl, false, rig, own_det ? det : nullptr))) return rc;
-        if (!c->fuse_ccl && (rc = ccl_launch_batch(c, sl, F, st))) return rc;
-        if ((rc = boxfit_launch_batch(c, sl, F, st, nn, false, rig, own_det ? det : nullptr))) return rc;
-        if ((rc = boxes_concat_seq_launch(c, sl, nd, df0, drig, rig, dm, fc, !gf, st))) return rc;
-      } else {
-        // merging sequences (lmot_seq_set_rig_merge): ground per sensor as above (CCL not fused), then each merging sequence's elevated
-        // clouds into its merge unit of this bank (one launch for all of them).  The CCL / box-fitting units are the other frames and
-        // the merge units, in sequence order; a merge unit gets the vehicle's values (identity pose, the sequence's detection values
-        // without a sensor's) and contributes one identity-pose list to its sequence
-        Slot* src[kMaxBatch];
-        Slot* mu[kMaxBatch];
-        lmot_sensor mpose[kMaxBatch];
-        int mn[kMaxBatch], ms0[kMaxBatch + 1], *mfc[kMaxBatch], nm = 0, nsrc = 0;
-        float mroi[kMaxBatch];
-        Slot* su[kMaxBatch];
-        lmot_sensor urig[kMaxBatch];
-        lmot_detect_params udet[kMaxBatch];
-        int unn[kMaxBatch], uf0[kMaxBatch + 1], *ufc[kMaxBatch], nu = 0;
-        bool udrig[kMaxBatch];
-        const lmot_detect_params base = detect_params_of(c->prm);
-        ms0[0] = 0;
-        for (int d = 0; d < nd; ++d) {
-          const int k = dseq[d], nk = df0[d + 1] - df0[d];
-          uf0[d] = nu;
-          if (merge[k]) {
-            const lmot_detect_params& vd = c->seq_det_on[k] ? c->seq_det[k] : base;
-            long long tot = 0;
-            for (int i = df0[d]; i < df0[d + 1]; ++i) { src[nsrc] = sl[i]; mpose[nsrc] = rig[i]; mn[nsrc] = nn[i]; ++nsrc; tot += nn[i]; }
-            mu[nm] = &c->seq_merge_unit[b][k]; mfc[nm] = fc[d]; mroi[nm] = vd.roi_m;
-            ms0[++nm] = nsrc;
-            su[nu] = mu[nm - 1];
-            lmot_default_sensor(&c->prm, &urig[nu]);
-            udet[nu] = vd;
-            unn[nu] = (int)(tot < c->max_points ? tot : c->max_points);
-            ++nu;
-            udrig[d] = false;
-            ufc[d] = fc[d] + 4 * nk;
-          } else {
-            for (int i = df0[d]; i < df0[d + 1]; ++i) { su[nu] = sl[i]; urig[nu] = rig[i]; if (own_det) udet[nu] = det[i]; unn[nu] = nn[i]; ++nu; }
-            udrig[d] = drig[d];
-            ufc[d] = fc[d];
-          }
-        }
-        uf0[nd] = nu;
-        if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, false, false, rig, own_det ? det : nullptr))) return rc;
-        if ((rc = rig_merge_launch(c, st, src, mpose, mn, nm, ms0, mu, mfc, mroi))) return rc;
-        if ((rc = ccl_launch_batch(c, su, nu, st))) return rc;
-        if ((rc = boxfit_launch_batch(c, su, nu, st, unn, false, urig, own_det ? udet : nullptr))) return rc;
-        if ((rc = boxes_concat_seq_launch(c, su, nd, uf0, udrig, urig, dm, ufc, !gf, st))) return rc;
-      }
-    }
+    if (rigged && (rc = boxes_concat_seq_launch(c, U.u, G, U.f0, U.rig_on, U.rig, dm, U.fc, !gf, st))) return rc;
   }
   for (int p = 0; p < S; ++p) m[p] = mk[seq[p]];
   // the measurement lists (complete on `st`, or posting their semaphores there) -> global-frame step, ONE tracker chain for the stepped
@@ -1715,7 +1662,7 @@ int lmot_track_step_lists_dev(lmot_ctx* ctx, const float* d_lists, const int* d_
                               double v_gps, double yaw_gps) {
   if (!ctx || !d_lists || !d_counts || n_lists < 1 || n_lists > kMaxBatch || cap_per_list < 1) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  if (c->n_sensors > 0 && n_lists > c->n_sensors) return LMOT_ERR_INVALID;     // a list without a sensor pose
+  if (c->own_cfg.n_sensors > 0 && n_lists > c->own_cfg.n_sensors) return LMOT_ERR_INVALID;     // a list without a sensor pose
   cudaSetDevice(c->device);
   int rc = batch_ensure(c, 1);              // the bank's box buffer + counters are the tracker's input
   if (rc) return rc;
@@ -1724,7 +1671,7 @@ int lmot_track_step_lists_dev(lmot_ctx* ctx, const float* d_lists, const int* d_
   k->res = r;
   r->n_kev = 0; r->batch_frames = 0;
   cudaStream_t st = c->stream;
-  if ((rc = boxes_pack_lists_launch(c, st, d_lists, d_counts, n_lists, cap_per_list, k->d_boxes, k->d_counters, c->n_sensors > 0 ? c->sensors : nullptr)))
+  if ((rc = boxes_pack_lists_launch(c, st, d_lists, d_counts, n_lists, cap_per_list, k->d_boxes, k->d_counters, c->own_cfg.n_sensors > 0 ? c->own_cfg.sensors : nullptr)))
     return rc;
   if (c->prm.global_frame && (rc = boxes_to_global_launch(c, k, st, k->d_boxes, k->d_counters, timestamp_us, v_gps, yaw_gps, false))) return rc;
   if ((rc = tracker_launch(c, k, st, k->d_boxes, k->d_counters, timestamp_us, v_gps, yaw_gps))) return rc;
@@ -1766,69 +1713,64 @@ static bool sensors_valid(const lmot_sensor* s, int n) {
   return true;
 }
 
-// the table only changes host state: ticks already submitted carry their own copy in their launch parameters
-int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n) {
-  if (!ctx || !sensors_valid(s, n)) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  for (int k = 0; k < n; ++k) c->sensors[k] = s[k];
-  c->n_sensors = n;
+// a stream's sensor table, host state only: ticks already submitted carry their own copy in their launch parameters
+static int sensors_set(StreamCfg& q, const lmot_sensor* s, int n) {
+  if (!sensors_valid(s, n)) return LMOT_ERR_INVALID;
+  for (int k = 0; k < n; ++k) q.sensors[k] = s[k];
+  q.n_sensors = n;
   return LMOT_OK;
 }
 
-int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n) {
-  if (!ctx || cap < 0 || (cap > 0 && !s)) return LMOT_ERR_INVALID;
-  const Ctx* c = &ctx->c;
-  if (n) *n = c->n_sensors;
-  for (int k = 0; k < c->n_sensors && k < cap; ++k) s[k] = c->sensors[k];
+static int sensors_get(const StreamCfg& q, lmot_sensor* s, int cap, int* n) {
+  if (cap < 0 || (cap > 0 && !s)) return LMOT_ERR_INVALID;
+  if (n) *n = q.n_sensors;
+  for (int k = 0; k < q.n_sensors && k < cap; ++k) s[k] = q.sensors[k];
   return LMOT_OK;
 }
 
-// sequence k's table (host state only, as lmot_set_sensors): its frames of later ticks, in table order
+int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n) { return ctx ? sensors_set(ctx->c.own_cfg, s, n) : LMOT_ERR_INVALID; }
+
+int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n) { return ctx ? sensors_get(ctx->c.own_cfg, s, cap, n) : LMOT_ERR_INVALID; }
+
+// sequence k's table: its frames of later ticks, in table order.  A tick's frames (one per sequence without a table) stay within kMaxBatch
 int lmot_seq_set_sensors(lmot_ctx* ctx, int k, const lmot_sensor* s, int n) {
   if (!ctx || k < 0 || k >= ctx->c.n_seq || !sensors_valid(s, n)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  int frames = 0;                                  // frames per tick with the new table: one per sequence without a table
+  int frames = 0;
   for (int j = 0; j < c->n_seq; ++j) {
-    const int nj = j == k ? n : c->seq_n_sensors[j];
+    const int nj = j == k ? n : c->seq_cfg[j].n_sensors;
     frames += nj > 0 ? nj : 1;
   }
-  if (frames > kMaxBatch) return LMOT_ERR_INVALID;
-  for (int j = 0; j < n; ++j) c->seq_sensors[k][j] = s[j];
-  c->seq_n_sensors[k] = n;
-  return LMOT_OK;
+  return frames > kMaxBatch ? LMOT_ERR_INVALID : sensors_set(c->seq_cfg[k], s, n);
 }
 
 int lmot_seq_get_sensors(const lmot_ctx* ctx, int k, lmot_sensor* s, int cap, int* n) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq || cap < 0 || (cap > 0 && !s)) return LMOT_ERR_INVALID;
-  const Ctx* c = &ctx->c;
-  if (n) *n = c->seq_n_sensors[k];
-  for (int j = 0; j < c->seq_n_sensors[k] && j < cap; ++j) s[j] = c->seq_sensors[k][j];
-  return LMOT_OK;
+  return ctx && k >= 0 && k < ctx->c.n_seq ? sensors_get(ctx->c.seq_cfg[k], s, cap, n) : LMOT_ERR_INVALID;
 }
 
 // ---- merging rigs (rig_merge.cu)
-int lmot_set_rig_merge(lmot_ctx* ctx, int on) {
-  if (!ctx || (on != 0 && on != 1)) return LMOT_ERR_INVALID;
-  ctx->c.rig_merge = on != 0;
+static int rig_merge_set(StreamCfg& q, int on) {
+  if (on != 0 && on != 1) return LMOT_ERR_INVALID;
+  q.rig_merge = on != 0;
   return LMOT_OK;
 }
 
-int lmot_get_rig_merge(const lmot_ctx* ctx, int* on) {
-  if (!ctx || !on) return LMOT_ERR_INVALID;
-  *on = ctx->c.rig_merge ? 1 : 0;
+static int rig_merge_get(const StreamCfg& q, int* on) {
+  if (!on) return LMOT_ERR_INVALID;
+  *on = q.rig_merge ? 1 : 0;
   return LMOT_OK;
 }
+
+int lmot_set_rig_merge(lmot_ctx* ctx, int on) { return ctx ? rig_merge_set(ctx->c.own_cfg, on) : LMOT_ERR_INVALID; }
+
+int lmot_get_rig_merge(const lmot_ctx* ctx, int* on) { return ctx ? rig_merge_get(ctx->c.own_cfg, on) : LMOT_ERR_INVALID; }
 
 int lmot_seq_set_rig_merge(lmot_ctx* ctx, int k, int on) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq || (on != 0 && on != 1)) return LMOT_ERR_INVALID;
-  ctx->c.seq_rig_merge[k] = on != 0;
-  return LMOT_OK;
+  return ctx && k >= 0 && k < ctx->c.n_seq ? rig_merge_set(ctx->c.seq_cfg[k], on) : LMOT_ERR_INVALID;
 }
 
 int lmot_seq_get_rig_merge(const lmot_ctx* ctx, int k, int* on) {
-  if (!ctx || !on || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *on = ctx->c.seq_rig_merge[k] ? 1 : 0;
-  return LMOT_OK;
+  return ctx && k >= 0 && k < ctx->c.n_seq ? rig_merge_get(ctx->c.seq_cfg[k], on) : LMOT_ERR_INVALID;
 }
 
 int lmot_seq_frame_counts(lmot_ctx* ctx, int k, int counts[LMOT_MAX_BATCH][4], int* n_frames) {
@@ -1936,16 +1878,16 @@ static bool detect_params_valid(const lmot_detect_params& d) {
 int lmot_seq_set_detect_params(lmot_ctx* ctx, int k, const lmot_detect_params* p) {
   if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
   if (p && !detect_params_valid(*p)) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  c->seq_det_on[k] = p != nullptr;
-  if (p) c->seq_det[k] = *p;
+  StreamCfg& q = ctx->c.seq_cfg[k];
+  q.det_on = p != nullptr;
+  if (p) q.det = *p;
   return LMOT_OK;
 }
 
 int lmot_seq_get_detect_params(const lmot_ctx* ctx, int k, lmot_detect_params* p) {
   if (!ctx || !p || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
   const Ctx* c = &ctx->c;
-  *p = c->seq_det_on[k] ? c->seq_det[k] : detect_params_of(c->prm);
+  *p = c->seq_cfg[k].det_on ? c->seq_cfg[k].det : detect_params_of(c->prm);
   return LMOT_OK;
 }
 
@@ -1982,24 +1924,24 @@ static int deskew_set(Ctx* c, lmot_deskew& dst, const lmot_deskew* d, float** bl
 int lmot_set_deskew(lmot_ctx* ctx, const lmot_deskew* d) {
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  return deskew_set(c, c->deskew, d, &c->results[0].h_deskew, c->n_results, sizeof(Result));
+  return deskew_set(c, c->own_cfg.deskew, d, &c->results[0].h_deskew, c->n_results, sizeof(Result));
 }
 
 int lmot_get_deskew(const lmot_ctx* ctx, lmot_deskew* d) {
   if (!ctx || !d) return LMOT_ERR_INVALID;
-  *d = ctx->c.deskew;
+  *d = ctx->c.own_cfg.deskew;
   return LMOT_OK;
 }
 
 int lmot_seq_set_deskew(lmot_ctx* ctx, int k, const lmot_deskew* d) {
   if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  return deskew_set(c, c->seq_deskew[k], d, &c->seq_ticks[0].h_deskew, c->seq_ring, sizeof(SeqTick));
+  return deskew_set(c, c->seq_cfg[k].deskew, d, &c->seq_ticks[0].h_deskew, c->seq_ring, sizeof(SeqTick));
 }
 
 int lmot_seq_get_deskew(const lmot_ctx* ctx, int k, lmot_deskew* d) {
   if (!ctx || !d || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *d = ctx->c.seq_deskew[k];
+  *d = ctx->c.seq_cfg[k].deskew;
   return LMOT_OK;
 }
 

@@ -277,12 +277,13 @@ struct Tracker {
 };
 
 // what the tracker chain of a sequence tick reads for sequence k: its measurement list, the list in the dead-reckoned global frame
-// (global_frame), its counter block and its detection semaphore.  Without sensor tables these are slot k's own buffers; with any table
-// set, the bank's per-sequence lists (Ctx::seq_meas) that concat_boxes_seq_kernel fills.
+// (global_frame), its counter block and its detection semaphore.  Without sensor tables these are the buffers of the unit the detection
+// front end (api.cu detect_front) box-fitted for it; with any table set, the bank's per-sequence lists (Ctx::seq_meas) that
+// concat_boxes_seq_kernel fills.
 struct SeqMeas { float* d_boxes = nullptr; float* d_boxes_g = nullptr; int* d_counters = nullptr; int* d_det_sem = nullptr; };
 
 // the box lists of a sequence tick's LISTS entries, in tick order: list i at lists[i] (device), its length in the device int counts[i],
-// clamped to [0, cap[i]] (api.cu seq_tick_common: the staged host lists, or the caller's device lists)
+// clamped to [0, cap[i]] (api.cu seq_tick_common packs them; the staged host lists, or the caller's device lists)
 struct SeqLists { const float* lists[kMaxBatch]; const int* counts[kMaxBatch]; int cap[kMaxBatch]; };
 
 // one tick of lmot_seq_*: a result block per sequence; blocks[0].ev_done marks the whole tick published.  Only the stepped sequences'
@@ -301,6 +302,23 @@ inline lmot_deskew deskew_defaults() {
   d.on = 0; d.time_field = 3; d.time_scale = 1.0; d.time_offset = 0.0; d.t_min = -0.1; d.t_max = 0.0;
   return d;
 }
+
+// One frame stream's detection-side settings: the context's own (lmot_set_sensors / _rig_merge / _deskew; batched ticks) and each
+// sequence's (lmot_seq_set_*).  Host state read at submission: ticks already submitted carry their own copy in their launch parameters.
+struct StreamCfg {
+  int n_sensors = 0;                   // sensor table: sensor k = frame k of a tick; 0: every frame uses lmot_params' values
+  lmot_sensor sensors[kMaxBatch] = {};
+  // merging rig: with a table set, the sensors' elevated clouds are clustered and boxed as one vehicle-frame cloud in the bank's merge
+  // unit (rig_merge.cu, allocated on the first merging submission)
+  bool rig_merge = false;
+  Slot merge_unit[kBatchBanks];
+  // own detection values (lmot_seq_set_detect_params; the context's own stream has none): off = lmot_params' values.  A tick with any
+  // of them on runs every frame through the per-frame kernel variants (ground.cu, boxfit.cu)
+  bool det_on = false;
+  lmot_detect_params det = {};
+  lmot_deskew deskew = deskew_defaults();   // sweep deskew (deskew.cu)
+  bool merges() const { return rig_merge && n_sensors > 0; }
+};
 
 struct Ctx {
   lmot_params prm;
@@ -331,13 +349,9 @@ struct Ctx {
   int n_bslots = 0, batch_frames = 0, next_bank = 0;
   Slot bank[kBatchBanks];              // pseudo-slots: concatenated boxes + counters + semaphore + events of a bank, and the stream its
                                        // tracking-only sequence ticks (lmot_seq_track*) run on
-  // ---- sensor rig (lmot_set_sensors): sensor k = frame k of a batched tick / list k of lmot_track_step_lists_dev; read at submission
-  int n_sensors = 0;                   // 0: every frame uses prm, the rig kernels are never launched
-  lmot_sensor sensors[kMaxBatch];
-  // merging rig (lmot_set_rig_merge): with a table set, the sensors' elevated clouds are clustered and boxed as one vehicle-frame cloud
-  // in the bank's merge unit (rig_merge.cu, allocated on the first merging submission).  Read at submission
-  bool rig_merge = false;
-  Slot merge_unit[kBatchBanks];
+  // the context's own stream: sensor k = frame k of a batched tick / list k of lmot_track_step_lists_dev; deskew of lmot_frame* and of
+  // batched ticks.  The sequences' records never apply to it, nor it to sequence ticks
+  StreamCfg own_cfg;
 
   // ---- result ring
   int n_results = 1;
@@ -360,26 +374,13 @@ struct Ctx {
   SeqTick* seq_last = nullptr;         // most recent submission (lmot_seq_fetch)
   uint32_t seq_stepped = 0;            // lmot_seq_stepped: the stepped mask of the tick most recently returned
   bool seq_wide = false;               // spawn_output_kernel's variant of the sequence ticks (largest last_n_act of the stepped tables)
-  // sensor tables of the sequences (lmot_seq_set_sensors): sequence k's frames of a tick are its sensors in table order; 0 sensors: one
-  // frame with lmot_params' thresholds.  Read at submission; the context's own table (sensors[]) never applies to sequence ticks.
-  int seq_n_sensors[kMaxBatch] = {};
-  lmot_sensor seq_sensors[kMaxBatch][kMaxBatch];
+  // each sequence's stream: its frames of a tick are its sensors in table order (no table: one frame)
+  StreamCfg seq_cfg[kMaxBatch];
   SeqMeas seq_meas[kBatchBanks][kMaxBatch];    // per-sequence measurement lists of each batch bank, allocated by lmot_seq_open
   // staging of lmot_seq_track_submit's host lists, per bank: kMaxBatch lists of max_boxes boxes, then kMaxBatch counts (lmot_seq_open)
   float* seq_stage[kBatchBanks] = {};
-  // detection parameters of the sequences (lmot_seq_set_detect_params): seq_det_on[k] false = lmot_params' values.  Read at submission;
-  // a detection tick with any of them on runs every frame through the per-frame kernel variants (ground.cu, boxfit.cu)
-  bool seq_det_on[kMaxBatch] = {};
-  lmot_detect_params seq_det[kMaxBatch] = {};
-  bool seq_rig_merge[kMaxBatch] = {};         // lmot_seq_set_rig_merge; merge units per bank and merging sequence (first use)
-  Slot seq_merge_unit[kBatchBanks][kMaxBatch];
   int seq_fc_n[kMaxBatch] = {};                // lmot_seq_frame_counts: frames of sequence k in the tick collected last
   int seq_fc[kMaxBatch][kMaxBatch][4] = {};    // ... and their n_elev, n_ground, num_cluster, n_boxes (host copies: the ring slot is reused)
-
-  // ---- sweep deskew (lmot_set_deskew / lmot_seq_set_deskew, deskew.cu): read at submission
-  lmot_deskew deskew = deskew_defaults();
-  lmot_deskew seq_deskew[kMaxBatch] = {deskew_defaults(), deskew_defaults(), deskew_defaults(), deskew_defaults(),
-                                       deskew_defaults(), deskew_defaults(), deskew_defaults(), deskew_defaults()};
 
   // ---- track prediction (lmot_predict_tracks*, tracker.cu predict_launch)
   bool pred_pending = false;           // a prediction was queued since the last tracker step: the next step's first kernel waits for it
