@@ -218,6 +218,46 @@ def deskew_table(v: float, omega: float, mount=None, **fields) -> np.ndarray:
     return out.reshape(DESKEW_SLICES, 3, 4)
 
 
+class Area(C.Structure):
+    """lmot_area: a detection area, polygon rings of (x, y) vertices in the vehicle frame (include/lmot.h)."""
+    _fields_ = [("n_rings", C.c_int), ("ring_len", C.c_void_p), ("xy", C.c_void_p), ("keep_outside", C.c_int)]
+
+
+AREA_MAX_RINGS, AREA_MAX_VERTICES = 64, 1024     # LMOT_AREA_MAX_RINGS / LMOT_AREA_MAX_VERTICES
+
+
+def _area(rings, keep_outside=False):
+    """(Area or None, keep-alive arrays) of `rings`: a sequence of (m, 2) vertex arrays (None or empty: no area).  Ring lengths and
+    vertices are passed as given; the library validates them."""
+    if rings is None or len(rings) == 0:
+        return None, ()
+    arrs = [np.asarray(r, np.float64).reshape(-1, 2) for r in rings]
+    lens = np.array([len(a) for a in arrs], np.int32)
+    xy = np.ascontiguousarray(np.concatenate(arrs) if len(arrs) else np.zeros((0, 2)), np.float64)
+    a = Area(len(arrs), lens.ctypes.data, xy.ctypes.data, int(keep_outside))
+    return a, (lens, xy)
+
+
+def detect_area_mask(rings, keep_outside=False, mount=None, roi_m=50.0) -> np.ndarray:
+    """lmot_detect_area_mask: the (250, 8) uint32 cell mask of the area `rings` for a unit mounted at `mount` ((3, 4) or (12,) [R | t];
+    None: identity) with clustering extent roi_m.  Row x = the grid's x cell, bit y & 31 of word y >> 5 = cell (x, y)."""
+    lib = load_library()
+    a, keep = _area(rings, keep_outside)
+    m = None
+    if mount is not None:
+        m = Sensor()
+        lib.lmot_default_sensor(None, C.byref(m))
+        m.pose[:] = [float(x) for x in np.asarray(mount, np.float32).reshape(12)]
+    out = np.zeros((250, 8), np.uint32)
+    fn = lib.lmot_detect_area_mask
+    fn.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
+    st = fn(C.cast(C.byref(a), C.c_void_p) if a is not None else None, C.cast(C.byref(m), C.c_void_p) if m is not None else None,
+            float(roi_m), out.ctypes.data_as(C.c_void_p))
+    if st != OK:
+        raise LmotError(st, lib.lmot_strerror(st).decode())
+    return out
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -273,6 +313,8 @@ ABI_SYMBOLS = [
     "lmot_seq_track_submit", "lmot_seq_track_dev", "lmot_seq_track", "lmot_seq_tracker_load", "lmot_seq_tracker_set_ego",
     "lmot_seq_tick_submit", "lmot_seq_tick_dev", "lmot_seq_tick", "lmot_seq_stepped",
     "lmot_default_deskew", "lmot_set_deskew", "lmot_get_deskew", "lmot_seq_set_deskew", "lmot_seq_get_deskew", "lmot_deskew_table",
+    "lmot_set_detect_area", "lmot_get_detect_area", "lmot_seq_set_detect_area", "lmot_seq_get_detect_area", "lmot_detect_area_mask",
+    "lmot_debug_area_masks",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
@@ -834,6 +876,50 @@ class Lmot:
         d = Deskew()
         self._chk(self.lib.lmot_seq_get_deskew(self.h, int(k), C.byref(d)))
         return {name: getattr(d, name) for name, _ in Deskew._fields_}
+
+    # ---- detection areas (lmot_set_detect_area / lmot_seq_set_detect_area) ----------------------------------------------------------
+    def set_detect_area(self, rings, keep_outside=False):
+        """The context's frames and batched ticks: cluster and box only the elevated points in cells inside `rings` (a sequence of (m, 2)
+        vertex arrays in the vehicle frame; None or empty: off), or outside them with keep_outside.  Applies from the next submission."""
+        a, keep = _area(rings, keep_outside)
+        fn = self.lib.lmot_set_detect_area
+        fn.argtypes = [C.c_void_p, C.c_void_p]
+        self._chk(fn(self.h, C.cast(C.byref(a), C.c_void_p) if a is not None else None))
+
+    def seq_set_detect_area(self, k: int, rings, keep_outside=False):
+        """Sequence k's FRAMES steps, arguments as set_detect_area."""
+        a, keep = _area(rings, keep_outside)
+        fn = self.lib.lmot_seq_set_detect_area
+        fn.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        self._chk(fn(self.h, int(k), C.cast(C.byref(a), C.c_void_p) if a is not None else None))
+
+    def _get_area(self, fn, *k):
+        lens = np.zeros(AREA_MAX_RINGS, np.int32)
+        xy = np.zeros((AREA_MAX_VERTICES, 2), np.float64)
+        nr, nv, ko = C.c_int(0), C.c_int(0), C.c_int(0)
+        fn.argtypes = [C.c_void_p] + [C.c_int] * len(k) + [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        self._chk(fn(self.h, *k, C.byref(nr), lens.ctypes.data, AREA_MAX_RINGS, C.byref(nv), xy.ctypes.data, AREA_MAX_VERTICES, C.byref(ko)))
+        rings, v0 = [], 0
+        for L in lens[: nr.value]:
+            rings.append(xy[v0 : v0 + L].copy())
+            v0 += int(L)
+        return dict(rings=rings, keep_outside=bool(ko.value))
+
+    def get_detect_area(self) -> dict:
+        """-> dict(rings: list of (m, 2) float64, keep_outside: bool); no rings: off"""
+        return self._get_area(self.lib.lmot_get_detect_area)
+
+    def seq_get_detect_area(self, k: int) -> dict:
+        return self._get_area(self.lib.lmot_seq_get_detect_area, int(k))
+
+    def debug_area_masks(self) -> np.ndarray:
+        """lmot_debug_area_masks: (n_units, 250, 8) uint32 device masks of the most recent own-stream submission (0 units: unmasked)"""
+        out = np.zeros((MAX_BATCH, 250, 8), np.uint32)
+        n = C.c_int(0)
+        fn = self.lib.lmot_debug_area_masks
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
+        self._chk(fn(self.h, out.ctypes.data, MAX_BATCH, C.byref(n)))
+        return out[: n.value]
 
     def seq_frame_counts(self, k: int) -> np.ndarray:
         """(n_frames, 4) int32: n_elevated, n_ground, num_cluster, n_boxes of each of sequence k's frames in the tick collected last"""

@@ -112,6 +112,20 @@ int deskew_frame(Ctx* c, Slot* s, Result* r, const float* d_raw, int n, int stri
   return deskew_launch(c, s->stream, &j, 1);
 }
 
+// a single-stream frame with the context's detection area: the area into r's pinned block, one copy to the slot's staging, the slot's
+// cell mask (identity pose, lmot_params.roi_m), all on the slot stream
+int area_frame(Ctx* c, Slot* s, Result* r) {
+  int rc;
+  if ((rc = area_ensure(c, s, 1))) return rc;
+  *r->h_area = c->own_cfg.area;
+  LMOT_CUDA(c, cudaMemcpyAsync(s->d_area, r->h_area, sizeof(AreaBlock), cudaMemcpyHostToDevice, s->stream));
+  AreaJob j{s->d_area, s->d_area_mask, {}, c->prm.roi_m};
+  lmot_sensor id;
+  lmot_default_sensor(&c->prm, &id);
+  memcpy(j.pose, id.pose, sizeof(j.pose));
+  return area_launch(c, s->stream, &j, 1);
+}
+
 int fetch_counters(Ctx* c, Slot* s, cudaStream_t st) {
   LMOT_CUDA(c, cudaMemcpyAsync(s->h_counters, s->d_counters, CNT_COUNT * sizeof(int), cudaMemcpyDeviceToHost, st));
   LMOT_CUDA(c, cudaStreamSynchronize(st));
@@ -208,13 +222,21 @@ int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tra
   r->batch_frames = 0;
   // the slot's previous boxes / counters must have been consumed by the tracker
   LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_trk_done, 0));
+  // detection area: the slot's cell mask first; clustering then runs as its own launch, masked, and box fitting skips masked points
+  const bool masked = c->own_cfg.masked();
+  if (masked && (rc = area_frame(c, s, r))) return rc;        // (allocates the slot's mask on first use)
+  const unsigned* mask = masked ? s->d_area_mask : nullptr;
+  s->area_last = masked;
+  c->n_area_dbg = masked ? 1 : 0;
+  c->area_dbg[0] = mask;
+  const bool fuse = c->fuse_ccl && !masked;
   if (c->timing) cudaEventRecord(r->ev[0], s->stream);
-  if ((rc = ground_launch(c, s, s->stream, d_pts, n, true, false, c->fuse_ccl))) return rc;
+  if ((rc = ground_launch(c, s, s->stream, d_pts, n, true, false, fuse))) return rc;
   if (c->timing) cudaEventRecord(r->ev[1], s->stream);
-  if (!c->fuse_ccl && (rc = cluster_launch(c, s, s->stream, n, true))) return rc;      // (fused: the ground kernel's last CTA did it)
+  if (!fuse && (rc = cluster_launch(c, s, s->stream, n, true, mask))) return rc;      // (fused: the ground kernel's last CTA did it)
   if (c->timing) cudaEventRecord(r->ev[2], s->stream);
   const bool gf = with_tracker && c->prm.global_frame;
-  if ((rc = boxfit_launch(c, s, s->stream, n, with_tracker && !gf))) return rc;      // with_tracker: posts the slot's detection semaphore
+  if ((rc = boxfit_launch(c, s, s->stream, n, with_tracker && !gf, mask))) return rc;      // with_tracker: posts the slot's detection semaphore
   if (gf && (rc = boxes_to_global_launch(c, s, s->stream, s->d_boxes, s->d_counters, ts, v, yaw, true))) return rc;   // ... or this one does
   if (c->timing) cudaEventRecord(r->ev[3], s->stream);
   LMOT_CUDA(c, cudaEventRecord(s->ev_det_done, s->stream));
@@ -286,7 +308,7 @@ void batch_destroy(Ctx* c) {
   for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&c->own_cfg.merge_unit[b]);
   for (int b = 0; b < kBatchBanks; ++b) {
     Slot* k = &c->bank[b];
-    cudaFree(k->d_boxes); cudaFree(k->d_boxes_g); cudaFree(k->d_counters); cudaFree(k->d_det_sem); cudaFree(k->d_deskew);
+    cudaFree(k->d_boxes); cudaFree(k->d_boxes_g); cudaFree(k->d_counters); cudaFree(k->d_det_sem); cudaFree(k->d_deskew); cudaFree(k->d_area);
     if (k->ev_det_done) cudaEventDestroy(k->ev_det_done);
     if (k->ev_trk_done) cudaEventDestroy(k->ev_trk_done);
     if (k->ev_fork) cudaEventDestroy(k->ev_fork);
@@ -343,7 +365,10 @@ struct DetUnits {
 // a group (a frame without a table: lmot_default_sensor); both get per-frame detection values iff some group has its own (sensor values
 // folded in).  A merge unit is the vehicle's cloud: identity pose, the group's detection values without a sensor's, at most max_points
 // points.  Clustering runs in the ground kernel's tail (fuse_ccl) unless a group merges in between.
-int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host, float* h_dsk, bool post_sem, DetUnits& U) {
+//   Detection areas: a group whose stream has one stages it into the pinned block h_area[i] (i-th masked group) -- one copy, one launch for
+// every masked unit's cell mask (unit pose: the merge unit's identity, else U.rig); clustering then runs as its own launch, and the
+// masked units cluster and box-fit through the masking kernel variants.
+int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host, float* h_dsk, AreaBlock* h_area, bool post_sem, DetUnits& U) {
   int rc;
   Slot* bk = &c->bank[b];
   Slot* sl[kMaxBatch];
@@ -422,15 +447,37 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
     }
   }
   U.f0[G] = nu;
-  const bool fuse = c->fuse_ccl && !merging;
+  AreaJob aj[kMaxBatch];
+  const unsigned* amask[kMaxBatch] = {};
+  int na = 0, nblk = 0;
+  for (int d = 0; d < G; ++d) {
+    const StreamCfg& q = *g[d].cfg;
+    if (!q.masked()) continue;
+    if ((rc = area_ensure(c, bk, kMaxBatch))) return rc;
+    h_area[nblk] = q.area;
+    const float roi = (q.det_on ? q.det : base).roi_m;
+    for (int i = U.f0[d]; i < U.f0[d + 1]; ++i) {
+      if ((rc = area_ensure(c, U.u[i], 0))) return rc;
+      aj[na] = AreaJob{bk->d_area + nblk, U.u[i]->d_area_mask, {}, roi};
+      memcpy(aj[na++].pose, U.rig[i].pose, sizeof(aj[0].pose));
+      amask[i] = U.u[i]->d_area_mask;
+    }
+    ++nblk;
+  }
+  if (nblk > 0) {
+    LMOT_CUDA(c, cudaMemcpyAsync(bk->d_area, h_area, (size_t)nblk * sizeof(AreaBlock), cudaMemcpyHostToDevice, st));
+    if ((rc = area_launch(c, st, aj, na))) return rc;
+  }
+  const unsigned* const* area = nblk > 0 ? amask : nullptr;
+  const bool fuse = c->fuse_ccl && !merging && nblk == 0;
   Result* r = bk->res;
   if (c->timing) cudaEventRecord(r->ev[0], st);
   if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, fuse, false, rigged ? rig : nullptr, own_det ? det : nullptr))) return rc;
   if (c->timing) cudaEventRecord(r->ev[1], st);
   if (nm > 0 && (rc = rig_merge_launch(c, st, src, mpose, mn, nm, ms0, mu, mfc, mroi))) return rc;
-  if (!fuse && (rc = ccl_launch_batch(c, U.u, nu, st))) return rc;
+  if (!fuse && (rc = ccl_launch_batch(c, U.u, nu, st, area))) return rc;
   if (c->timing) cudaEventRecord(r->ev[2], st);
-  return boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr);
+  return boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr, area);
 }
 
 // the IDs of a result being returned (lmot_track_ids): copied now, the block is reused by later submissions
@@ -557,6 +604,7 @@ void result_destroy(Result* r) {
   if (r->h_visbb) cudaFreeHost(r->h_visbb);
   if (r->h_ids) cudaFreeHost(r->h_ids);
   if (r->h_deskew) cudaFreeHost(r->h_deskew);
+  if (r->h_area) cudaFreeHost(r->h_area);
   if (r->d_ids) cudaFree(r->d_ids);
   if (r->d_block) cudaFree(r->d_block);
   if (r->ev_tc) cudaEventDestroy(r->ev_tc);
@@ -586,6 +634,7 @@ void seq_destroy(Ctx* c) {
   for (int i = 0; i < c->seq_ring; ++i) {
     for (int k = 0; k < c->n_seq; ++k) result_destroy(&c->seq_ticks[i].blocks[k]);
     if (c->seq_ticks[i].h_deskew) cudaFreeHost(c->seq_ticks[i].h_deskew);
+    if (c->seq_ticks[i].h_area) cudaFreeHost(c->seq_ticks[i].h_area);
   }
   delete[] c->seq_ticks;
   c->seq_ticks = nullptr; c->seq_last = nullptr; c->seq_stepped = 0;
@@ -657,7 +706,7 @@ int slot_create(Ctx* c, Slot* s, int index) {
 
 void slot_destroy(Slot* s) {
   ground_free(s); cluster_free(s); boxfit_free(s);
-  cudaFree(s->d_deskew); cudaFree(s->d_stage_wide);
+  cudaFree(s->d_deskew); cudaFree(s->d_stage_wide); cudaFree(s->d_area_mask); cudaFree(s->d_area);
   if (s->ev_fork) cudaEventDestroy(s->ev_fork);
   if (s->ev_det_done) cudaEventDestroy(s->ev_det_done);
   if (s->ev_trk_done) cudaEventDestroy(s->ev_trk_done);
@@ -888,6 +937,7 @@ int lmot_component_cluster(lmot_ctx* ctx, const float* elevated, int n, int stri
   cudaStream_t st = c->stream;
   if ((rc = upload_points(c, s, st, elevated, n, stride, s->d_elev))) return rc;
   if ((rc = set_counter(c, s, st, CNT_N_ELEV, n))) return rc;
+  s->area_last = false;
   if ((rc = cluster_launch(c, s, st, n))) return rc;
   if ((rc = fetch_counters(c, s, st))) return rc;
   if (num_cluster) *num_cluster = s->h_counters[CNT_NUM_CLUSTER];
@@ -951,6 +1001,7 @@ int lmot_box_fit(lmot_ctx* ctx, const float* elevated, int n, int stride, const 
   if ((rc = upload_points(c, s, st, elevated, n, stride, s->d_elev))) return rc;
   LMOT_CUDA(c, cudaMemcpyAsync(s->d_label_grid, grid, kCartCells * sizeof(int), cudaMemcpyHostToDevice, st));
   s->label_grid_foreign = true;
+  s->area_last = false;
   if ((rc = set_counter(c, s, st, CNT_N_ELEV, n))) return rc;
   if ((rc = set_counter(c, s, st, CNT_NUM_CLUSTER, num_cluster))) return rc;
   s->res = &c->results[0];
@@ -1009,6 +1060,7 @@ int lmot_detect_dev(lmot_ctx* ctx, const float* d_points, int n) {
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
+  if (c->own_cfg.masked() && c->timing) return LMOT_ERR_STATE;
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, true);
   LMOT_CUDA(c, cudaEventRecord(s->ev_fork, c->stream));
@@ -1020,7 +1072,7 @@ int lmot_frame_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp
   if (!ctx || n < 0 || (n > 0 && !d_points) || (reinterpret_cast<uintptr_t>(d_points) & 15u)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   const bool dsk = c->own_cfg.deskew.on != 0;
-  if (dsk && c->timing) return LMOT_ERR_STATE;
+  if ((dsk || c->own_cfg.masked()) && c->timing) return LMOT_ERR_STATE;
   if (dsk && c->own_cfg.deskew.time_field != 3) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
@@ -1041,6 +1093,7 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
+  if (c->own_cfg.masked() && c->timing) return LMOT_ERR_STATE;
   const bool dsk = c->own_cfg.deskew.on != 0;
   if (dsk) {                           // (validated before anything is submitted: upload_points checks the rest without deskew)
     if (c->timing) return LMOT_ERR_STATE;
@@ -1149,7 +1202,7 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   const bool dsk = with_tracker && q.deskew.on != 0;                // (lmot_batch_detect_dev has no stamp: never deskewed)
   if (dsk && c->timing) return LMOT_ERR_STATE;
   if (dsk && (host ? stride <= q.deskew.time_field : q.deskew.time_field != 3)) return LMOT_ERR_INVALID;
-  if (q.merges() && c->timing) return LMOT_ERR_STATE;
+  if ((q.merges() || q.masked()) && c->timing) return LMOT_ERR_STATE;
   if (host && c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;
   int rc = batch_ensure(c, n_frames);
   if (rc) return rc;
@@ -1175,7 +1228,9 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&d_fc, r->h_frame_counts, 0));
   const DetGroup grp{&q, with_tracker ? &c->own.th : nullptr, points, n, n_frames, ts, v, yaw, d_fc};
   DetUnits U;
-  if ((rc = detect_front(c, b, &grp, 1, stride, host, r->h_deskew, false, U))) return rc;
+  if ((rc = detect_front(c, b, &grp, 1, stride, host, r->h_deskew, r->h_area, false, U))) return rc;
+  c->n_area_dbg = q.masked() ? U.f0[1] : 0;
+  for (int i = 0; i < c->n_area_dbg; ++i) c->area_dbg[i] = U.u[i]->d_area_mask;
   const bool gf = with_tracker && c->prm.global_frame;
   if ((rc = boxes_concat_launch(c, U.u, U.f0[1], st, k->d_boxes, k->d_counters, U.fc[0], (with_tracker && !gf) ? k->d_det_sem : nullptr,
                                 U.rig_on[0] ? U.rig : nullptr))) return rc;
@@ -1491,7 +1546,7 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
       g[G++] = DetGroup{&c->seq_cfg[k], &c->seq[k].th, e[k].data, e[k].n, f0[k + 1] - f0[k], e[k].timestamp_us, e[k].v_gps, e[k].yaw_gps, fc};
     }
     DetUnits U;
-    if ((rc = detect_front(c, b, g, G, stride, host, t->h_deskew, !rigged && !gf, U))) return rc;
+    if ((rc = detect_front(c, b, g, G, stride, host, t->h_deskew, t->h_area, !rigged && !gf, U))) return rc;
     SeqMeas dm[kMaxBatch];
     for (int d = 0; d < G; ++d) {
       const Slot* s = U.u[U.f0[d]];
@@ -1948,6 +2003,80 @@ int lmot_seq_get_deskew(const lmot_ctx* ctx, int k, lmot_deskew* d) {
 int lmot_deskew_table(const lmot_deskew* d, double v, double omega, const lmot_sensor* mount, float out[LMOT_DESKEW_SLICES][12]) {
   if (!d || !out || !deskew_valid(*d) || !std::isfinite(v) || !std::isfinite(omega) || (mount && !sensors_valid(mount, 1))) return LMOT_ERR_INVALID;
   return deskew_table(*d, v, omega, mount, &out[0][0]);
+}
+
+// ---- detection areas (detect_area.cu).  Host state only, as the sensor tables; setting one allocates the pinned staging blocks of the
+// ring (once): `per` blocks at each of the n entries `blocks`, `stride` bytes apart
+static int area_set(Ctx* c, AreaBlock& dst, const lmot_area* a, AreaBlock** blocks, int n, size_t stride, int per) {
+  if (!area_valid(a)) return LMOT_ERR_INVALID;
+  if (a && a->n_rings > 0) {
+    cudaSetDevice(c->device);
+    for (int i = 0; i < n; ++i) {
+      AreaBlock** p = reinterpret_cast<AreaBlock**>(reinterpret_cast<char*>(blocks) + i * stride);
+      if (!*p) LMOT_CUDA(c, cudaHostAlloc((void**)p, (size_t)per * sizeof(AreaBlock), cudaHostAllocDefault));
+    }
+  }
+  area_copy(dst, a);
+  return LMOT_OK;
+}
+
+static int area_get(const AreaBlock& a, int* n_rings, int* ring_len, int cap_rings, int* n_vertices, double* xy, int cap_vertices,
+                    int* keep_outside) {
+  if (cap_rings < 0 || cap_vertices < 0 || (cap_rings > 0 && !ring_len) || (cap_vertices > 0 && !xy)) return LMOT_ERR_INVALID;
+  if (n_rings) *n_rings = a.n_rings;
+  if (n_vertices) *n_vertices = a.n_vertices;
+  if (keep_outside) *keep_outside = a.keep_outside;
+  const int nr = a.n_rings < cap_rings ? a.n_rings : cap_rings, nv = a.n_vertices < cap_vertices ? a.n_vertices : cap_vertices;
+  if (nr > 0) memcpy(ring_len, a.ring_len, (size_t)nr * sizeof(int));
+  if (nv > 0) memcpy(xy, a.xy, (size_t)nv * 2 * sizeof(double));
+  return LMOT_OK;
+}
+
+int lmot_set_detect_area(lmot_ctx* ctx, const lmot_area* area) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  return area_set(c, c->own_cfg.area, area, &c->results[0].h_area, c->n_results, sizeof(Result), 1);
+}
+
+int lmot_get_detect_area(const lmot_ctx* ctx, int* n_rings, int* ring_len, int cap_rings, int* n_vertices, double* xy, int cap_vertices,
+                         int* keep_outside) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  return area_get(ctx->c.own_cfg.area, n_rings, ring_len, cap_rings, n_vertices, xy, cap_vertices, keep_outside);
+}
+
+int lmot_seq_set_detect_area(lmot_ctx* ctx, int k, const lmot_area* area) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  return area_set(c, c->seq_cfg[k].area, area, &c->seq_ticks[0].h_area, c->seq_ring, sizeof(SeqTick), kMaxBatch);
+}
+
+int lmot_seq_get_detect_area(const lmot_ctx* ctx, int k, int* n_rings, int* ring_len, int cap_rings, int* n_vertices, double* xy,
+                             int cap_vertices, int* keep_outside) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  return area_get(ctx->c.seq_cfg[k].area, n_rings, ring_len, cap_rings, n_vertices, xy, cap_vertices, keep_outside);
+}
+
+int lmot_detect_area_mask(const lmot_area* area, const lmot_sensor* mount, float roi_m, uint32_t out[LMOT_NUM_GRID * 8]) {
+  if (!area || area->n_rings < 1 || !out || !area_valid(area) || !std::isfinite(roi_m) || !(roi_m > 0.f) ||
+      (mount && !sensors_valid(mount, 1))) return LMOT_ERR_INVALID;
+  AreaBlock* a = new (std::nothrow) AreaBlock;
+  if (!a) return LMOT_ERR_INVALID;
+  area_copy(*a, area);
+  area_mask_host(*a, mount ? mount->pose : nullptr, roi_m, out);
+  delete a;
+  return LMOT_OK;
+}
+
+int lmot_debug_area_masks(lmot_ctx* ctx, uint32_t* out, int cap_units, int* n_units) {
+  if (!ctx || cap_units < 0 || (cap_units > 0 && !out)) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  int rc = lmot_sync(ctx);
+  if (rc) return rc;
+  if (n_units) *n_units = c->n_area_dbg;
+  const int n = c->n_area_dbg < cap_units ? c->n_area_dbg : cap_units;
+  for (int i = 0; i < n; ++i)
+    LMOT_CUDA(c, cudaMemcpy(out + (size_t)i * LMOT_NUM_GRID * 8, c->area_dbg[i], LMOT_NUM_GRID * 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  return LMOT_OK;
 }
 
 // after the table was received from another rank (NCCL broadcast into lmot_tracker_table's pointer, count already in the device

@@ -25,6 +25,7 @@
 #include <random>
 #include <vector>
 #include "lmot_internal.cuh"
+#include "ccl_device.cuh"
 
 namespace lmot {
 
@@ -60,8 +61,10 @@ struct FitBatch { FitFrame f[kMaxBatch]; };
 
 __device__ __forceinline__ void seg_offsets_body(const FitFrame& F, int max_clusters);
 
-__global__ void __launch_bounds__(kTile)
-tile_hist_kernel(const __grid_constant__ FitBatch B, int max_clusters) {
+// kArea: a point whose cell is outside its unit's detection-area mask `area` gets cluster 0 -- dilation can label masked cells, and
+// those hold no point of the masked cloud E_area
+template <bool kArea>
+__device__ __forceinline__ void tile_hist_body(const FitBatch& B, int max_clusters, const unsigned* __restrict__ area) {
   extern __shared__ int s_hist[];
   fit_pdl_trigger();
   const FitFrame& F = B.f[blockIdx.y];
@@ -77,7 +80,7 @@ tile_hist_kernel(const __grid_constant__ FitBatch B, int max_clusters) {
   unsigned cid = 0;
   if (i < n) {
     const unsigned c = cart[i];
-    if (c != kNoCell) cid = (unsigned)__ldg(&label_grid[c]);
+    if (c != kNoCell && (!kArea || !area || area_kept(area, c))) cid = (unsigned)__ldg(&label_grid[c]);
     if (cid > (unsigned)K) cid = 0;                    // capacity overflow is reported by seg_offsets_kernel
     pcid[i] = (uint16_t)cid;
   }
@@ -94,6 +97,17 @@ tile_hist_kernel(const __grid_constant__ FitBatch B, int max_clusters) {
   if (threadIdx.x == 0) s_last = (atomicInc(F.hist_ctr, gridDim.x - 1u) == gridDim.x - 1u) ? 1 : 0;
   __syncthreads();
   if (s_last) { __threadfence(); seg_offsets_body(F, max_clusters); }
+}
+
+__global__ void __launch_bounds__(kTile)
+tile_hist_kernel(const __grid_constant__ FitBatch B, int max_clusters) { tile_hist_body<false>(B, max_clusters, nullptr); }
+
+// detection areas: frame blockIdx.y's unit mask A.m[blockIdx.y] (nullptr: an unmasked unit of the same launch)
+struct FitAreaMasks { const unsigned* m[kMaxBatch]; };
+
+__global__ void __launch_bounds__(kTile)
+tile_hist_area_kernel(const __grid_constant__ FitBatch B, int max_clusters, const __grid_constant__ FitAreaMasks A) {
+  tile_hist_body<true>(B, max_clusters, A.m[blockIdx.y]);
 }
 
 // ---------------------------------------------------------------------------------------------- B2
@@ -450,6 +464,7 @@ int boxfit_alloc_shared(Ctx* c) {
   const int sh = (c->prm.max_clusters + 1) * (int)sizeof(int);
   if (sh > 48 * 1024) {
     LMOT_CUDA(c, cudaFuncSetAttribute(tile_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh));
+    LMOT_CUDA(c, cudaFuncSetAttribute(tile_hist_area_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh));
     LMOT_CUDA(c, cudaFuncSetAttribute(scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh));
   }
   return LMOT_OK;
@@ -513,7 +528,7 @@ static BoxParams box_params_of(const lmot_detect_params& p) {
 }
 
 int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig,
-                        const lmot_detect_params* det) {
+                        const lmot_detect_params* det, const unsigned* const* area) {
   if (F < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   const int K1 = c->prm.max_clusters + 1;
   int tiles = 0;
@@ -523,7 +538,11 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
   for (int i = 0; i < F; ++i) { fit_frame_of(slots[i], B.f[i], post_sem); if (rig) B.f[i].sensor_height = rig[i].sensor_height; }
   for (int i = F; i < kMaxBatch; ++i) B.f[i] = B.f[0];
   Slot* s0 = slots[0];
-  if (tiles > 0) tile_hist_kernel<<<dim3(tiles, F), kTile, sh, st>>>(B, c->prm.max_clusters);     // + segment offsets by its last CTA per frame
+  bool masked = false;
+  FitAreaMasks A{};
+  for (int i = 0; area && i < F; ++i) { A.m[i] = area[i]; masked |= area[i] != nullptr; }
+  if (tiles > 0 && masked) tile_hist_area_kernel<<<dim3(tiles, F), kTile, sh, st>>>(B, c->prm.max_clusters, A);
+  else if (tiles > 0) tile_hist_kernel<<<dim3(tiles, F), kTile, sh, st>>>(B, c->prm.max_clusters);     // + segment offsets by its last CTA per frame
   else seg_offsets_kernel<<<F, 1024, 0, st>>>(B, c->prm.max_clusters);
   kernel_mark(c, s0, st);
   // scatter and box_fit as programmatic dependents of the kernel before them (timing mode records an event between the kernels,
@@ -722,10 +741,11 @@ int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const SeqLists& L, int 
   return LMOT_OK;
 }
 
-int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem) {
+int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem, const unsigned* area) {
   Slot* sl[1] = {s};
   const int nu[1] = {n_upper};
-  return boxfit_launch_batch(c, sl, 1, st, nu, post_sem);
+  const unsigned* am[1] = {area};
+  return boxfit_launch_batch(c, sl, 1, st, nu, post_sem, nullptr, nullptr, area ? am : nullptr);
 }
 
 }  // namespace lmot

@@ -60,6 +60,13 @@ __device__ __forceinline__ unsigned piece_starts(unsigned m) { return m & ~(m <<
 // index (inside its word) of the piece that contains set bit p of word m
 __device__ __forceinline__ int piece_of(unsigned m, int p) { return __popc(piece_starts(m) & ((2u << p) - 1u)) - 1; }
 
+// detection areas: whether cell c (x*250+y, or kNoCell) of a point has its bit set in the unit's cell mask
+__device__ __forceinline__ bool area_kept(const unsigned* __restrict__ area, unsigned c) {
+  if (c == kNoCell) return false;
+  const unsigned x = c / (unsigned)kNumGrid, y = c - x * (unsigned)kNumGrid;
+  return (__ldg(&area[x * kRowWords + (y >> 5)]) >> (y & 31u)) & 1u;
+}
+
 // One frame of a launch (blockIdx.x): bit planes in, label grid + cluster count out
 struct CclFrame {
   unsigned* once; unsigned* twice; unsigned* prev_occ;
@@ -101,7 +108,10 @@ __device__ __forceinline__ void ccl_flatten(volatile int* L, int P) {
   __syncthreads();
 }
 
-__device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char* ccl_smem) {
+// kArea: the unit's cell mask (detection areas, nullptr: every cell) is ANDed into the seeds as they load -- a masked cell holds no point
+// of the masked cloud, and seeds are "more than one point per cell", so masking whole cells is exact
+template <bool kArea = false>
+__device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char* ccl_smem, const unsigned* __restrict__ area = nullptr) {
   int* s_par = reinterpret_cast<int*>(ccl_smem);                       // [<= 32000] parent id, later -(cluster id) at roots
   unsigned* s_seed = reinterpret_cast<unsigned*>(s_par + kNodes);       // [2000]
   unsigned* s_occ = s_seed + kBitWords;                                 // [2000]
@@ -116,7 +126,8 @@ __device__ __forceinline__ void ccl_dense_body(const CclFrame& F, unsigned char*
   const bool own = tid < kBitWords / 2;
   // A: seed = cells with more than one point (component_clustering.cpp:136); the bit planes are re-armed for the next frame
   if (own) {
-    const uint2 tw = __ldcg(reinterpret_cast<const uint2*>(twice) + tid);
+    uint2 tw = __ldcg(reinterpret_cast<const uint2*>(twice) + tid);
+    if (kArea && area) { const uint2 am = __ldg(reinterpret_cast<const uint2*>(area) + tid); tw.x &= am.x; tw.y &= am.y; }
     const uint2 pv = __ldcg(reinterpret_cast<const uint2*>(prev_occ) + tid);
     s_seed[w0] = tw.x; s_seed[w0 + 1] = tw.y;
     s_prev[w0] = pv.x; s_prev[w0 + 1] = pv.y;

@@ -57,6 +57,15 @@ ccl_dense_kernel(const __grid_constant__ CclBatch B) {
   ccl_dense_body(B.f[blockIdx.x], ccl_smem);
 }
 
+// detection areas: frame blockIdx.x's seeds masked by its unit's cell mask (A.m[i], nullptr: an unmasked unit of the same launch)
+struct AreaMasks { const unsigned* m[kMaxBatch]; };
+
+__global__ void __launch_bounds__(kCclThreads, 1)
+ccl_area_kernel(const __grid_constant__ CclBatch B, const __grid_constant__ AreaMasks A) {
+  extern __shared__ __align__(16) unsigned char ccl_smem[];
+  ccl_dense_body<true>(B.f[blockIdx.x], ccl_smem, A.m[blockIdx.x]);
+}
+
 // ---- the cluster node's side outputs (src/cluster/main.cpp:62-99), SURVEY.md §8(f)3 ------------------------------
 //   makeClusteredCloud (component_clustering.cpp:308-335): every elevated point inside the ROI whose cell carries a label
 //       becomes the CENTRE of its cell at z = -1, in cloud order
@@ -67,10 +76,12 @@ ccl_dense_kernel(const __grid_constant__ CclBatch B) {
 // One CTA; two order-preserving compactions (ballot + carried offset per 1024-point tile).
 constexpr int kCostW = 50, kCostH = 50;
 
-__global__ void __launch_bounds__(1024)
-cluster_outputs_kernel(const float4* __restrict__ elev, const uint16_t* __restrict__ cart, const int* __restrict__ counters,
-                       const int* __restrict__ label_grid, float roi, int* __restrict__ first_idx, float4* __restrict__ clustered,
-                       float4* __restrict__ obstacles, int* __restrict__ cost_map, int* __restrict__ out_counts) {
+// kArea: the points of cells outside the detection area's mask `area` are not part of the cloud (E_area): they are skipped
+template <bool kArea>
+__device__ __forceinline__ void cluster_outputs_body(const float4* __restrict__ elev, const uint16_t* __restrict__ cart, const int* __restrict__ counters,
+                                                     const int* __restrict__ label_grid, float roi, int* __restrict__ first_idx,
+                                                     float4* __restrict__ clustered, float4* __restrict__ obstacles, int* __restrict__ cost_map,
+                                                     int* __restrict__ out_counts, const unsigned* __restrict__ area) {
   __shared__ int s_cost[kCostW * kCostH];
   __shared__ int s_warp[32], s_warp2[32];
   __shared__ int s_carry, s_carry2;
@@ -84,6 +95,7 @@ cluster_outputs_kernel(const float4* __restrict__ elev, const uint16_t* __restri
   const double res = 1.0, cx = (kCostW / 2.0) * res - 0.0, cy = (kCostH / 2.0) * res - 25.0;   // g_resolution, g_offset_x/y (:15-20)
   for (int i = tid; i < n; i += 1024) {
     const unsigned cc = cart[i];
+    if (kArea && !area_kept(area, cc)) continue;
     if (cc != kNoCell && label_grid[cc] != 0) atomicMin(&first_idx[cc], i);
     const float4 q = __ldg(&elev[i]);
     if (!((double)q.z > 0.1) && !(fabs((double)q.x) < 4.5 && fabs((double)q.y) < 2.0)) {
@@ -100,7 +112,7 @@ cluster_outputs_kernel(const float4* __restrict__ elev, const uint16_t* __restri
     unsigned cc = kNoCell;
     if (i < n) {
       cc = cart[i];
-      if (cc != kNoCell) { lab = label_grid[cc]; obs = (lab != 0 && first_idx[cc] == i) ? 1 : 0; }
+      if (cc != kNoCell && (!kArea || area_kept(area, cc))) { lab = label_grid[cc]; obs = (lab != 0 && first_idx[cc] == i) ? 1 : 0; }
     }
     const unsigned bl = __ballot_sync(0xFFFFFFFFu, lab != 0), bo = __ballot_sync(0xFFFFFFFFu, obs);
     if (lane == 0) { s_warp[warp] = __popc(bl); s_warp2[warp] = __popc(bo); }
@@ -124,6 +136,21 @@ cluster_outputs_kernel(const float4* __restrict__ elev, const uint16_t* __restri
   if (tid == 0) { out_counts[0] = s_carry; out_counts[1] = s_carry2; }
 }
 
+__global__ void __launch_bounds__(1024)
+cluster_outputs_kernel(const float4* __restrict__ elev, const uint16_t* __restrict__ cart, const int* __restrict__ counters,
+                       const int* __restrict__ label_grid, float roi, int* __restrict__ first_idx, float4* __restrict__ clustered,
+                       float4* __restrict__ obstacles, int* __restrict__ cost_map, int* __restrict__ out_counts) {
+  cluster_outputs_body<false>(elev, cart, counters, label_grid, roi, first_idx, clustered, obstacles, cost_map, out_counts, nullptr);
+}
+
+__global__ void __launch_bounds__(1024)
+cluster_outputs_area_kernel(const float4* __restrict__ elev, const uint16_t* __restrict__ cart, const int* __restrict__ counters,
+                            const int* __restrict__ label_grid, float roi, int* __restrict__ first_idx, float4* __restrict__ clustered,
+                            float4* __restrict__ obstacles, int* __restrict__ cost_map, int* __restrict__ out_counts,
+                            const unsigned* __restrict__ area) {
+  cluster_outputs_body<true>(elev, cart, counters, label_grid, roi, first_idx, clustered, obstacles, cost_map, out_counts, area);
+}
+
 __global__ void fill_i32_kernel(int* p, int n, int v) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
@@ -145,6 +172,7 @@ int cluster_alloc(Ctx* c, Slot* s) {
   LMOT_CUDA(c, cudaMemsetAsync(s->d_label_grid, 0, kCartCells * sizeof(int), s->stream));
   s->label_grid_foreign = false;
   LMOT_CUDA(c, cudaFuncSetAttribute(ccl_dense_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDenseSmem));
+  LMOT_CUDA(c, cudaFuncSetAttribute(ccl_area_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDenseSmem));
   return LMOT_OK;
 }
 
@@ -154,7 +182,7 @@ void cluster_free(Slot* s) {
 }
 
 // elevated cloud = s->d_elev with its length in d_counters[CNT_N_ELEV]; n_upper bounds that length on the host
-int cluster_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool counted) {
+int cluster_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool counted, const unsigned* area) {
   unsigned* once = s->d_cart_bits, *twice = once + kBitWords, *prev = twice + kBitWords;
   if (s->label_grid_foreign) {   // the caller uploaded its own label grid (lmot_box_fit): the sparse update needs a clean slate
     LMOT_CUDA(c, cudaMemsetAsync(s->d_label_grid, 0, kCartCells * sizeof(int), st));
@@ -166,11 +194,12 @@ int cluster_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool counted) 
     kernel_mark(c, s, st);
   }
   Slot* sl[1] = {s};
-  return ccl_launch_batch(c, sl, 1, st);
+  const unsigned* am[1] = {area};
+  return ccl_launch_batch(c, sl, 1, st, area ? am : nullptr);
 }
 
 // connected components of F frames in one launch, one CTA per frame (the bit planes were marked by the ground kernel)
-int ccl_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st) {
+int ccl_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const unsigned* const* area) {
   if (F < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   CclBatch B;
   for (int i = 0; i < F; ++i) {
@@ -179,7 +208,11 @@ int ccl_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st) {
     B.f[i].out = s->d_label_grid; B.f[i].counters = s->d_counters;
   }
   for (int i = F; i < kMaxBatch; ++i) B.f[i] = B.f[0];
-  ccl_dense_kernel<<<F, kCclThreads, kDenseSmem, st>>>(B);
+  bool masked = false;
+  AreaMasks A{};
+  for (int i = 0; area && i < F; ++i) { A.m[i] = area[i]; masked |= area[i] != nullptr; }
+  if (masked) ccl_area_kernel<<<F, kCclThreads, kDenseSmem, st>>>(B, A);
+  else ccl_dense_kernel<<<F, kCclThreads, kDenseSmem, st>>>(B);
   kernel_mark(c, slots[0], st);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
@@ -194,8 +227,13 @@ int cluster_outputs_launch(Ctx* c, Slot* s, cudaStream_t st) {
     LMOT_CUDA(c, cudaMalloc(&s->d_cost_map, (kCostW * kCostH + 2) * sizeof(int)));
     fill_i32_kernel<<<(kCartCells + 255) / 256, 256, 0, st>>>(s->d_first_idx, kCartCells, INT_MAX);
   }
-  cluster_outputs_kernel<<<1, 1024, 0, st>>>(s->d_elev, s->d_cart, s->d_counters, s->d_label_grid, c->prm.roi_m, s->d_first_idx,
-                                             s->d_clustered, s->d_obstacles, s->d_cost_map, s->d_cost_map + kCostW * kCostH);
+  if (s->area_last)
+    cluster_outputs_area_kernel<<<1, 1024, 0, st>>>(s->d_elev, s->d_cart, s->d_counters, s->d_label_grid, c->prm.roi_m, s->d_first_idx,
+                                                    s->d_clustered, s->d_obstacles, s->d_cost_map, s->d_cost_map + kCostW * kCostH,
+                                                    s->d_area_mask);
+  else
+    cluster_outputs_kernel<<<1, 1024, 0, st>>>(s->d_elev, s->d_cart, s->d_counters, s->d_label_grid, c->prm.roi_m, s->d_first_idx,
+                                               s->d_clustered, s->d_obstacles, s->d_cost_map, s->d_cost_map + kCostW * kCostH);
   LMOT_CUDA(c, cudaGetLastError());
   return LMOT_OK;
 }

@@ -103,6 +103,14 @@ struct TrackerHost {
   double fold[3] = {0, 0, -1.5707963267948966};
 };
 
+// A stream's detection area (lmot_set_detect_area / lmot_seq_set_detect_area) as it is staged: the host copy in StreamCfg, one block per
+// masked stream in the pinned source of a submission (Result::h_area, SeqTick::h_area) and on the device (Slot::d_area).  n_rings 0: off.
+struct AreaBlock {
+  int n_rings, keep_outside, n_vertices, pad;
+  int ring_len[LMOT_AREA_MAX_RINGS];
+  double xy[2 * LMOT_AREA_MAX_VERTICES];
+};
+
 constexpr int kMaxKernelEvents = 20;
 
 // Result block: where one frame's results land.  Pinned, device-mapped host memory written by the kernels themselves
@@ -137,6 +145,8 @@ struct Result {
   // deskew: pinned host source of the pose tables copied for this block's submission ([kMaxBatch][LMOT_DESKEW_SLICES * 12], allocated
   // by lmot_set_deskew).  Reusing a block means its previous submission has completed, so the copy from it has too.
   float* h_deskew = nullptr;
+  // detection area: pinned host source of the context's area staged for this block's submission (one block, lmot_set_detect_area)
+  AreaBlock* h_area = nullptr;
   // merging rig (lmot_set_rig_merge): the tick's sensors, 0 when it did not merge.  h_frame_counts rows 0..merge_rows-1 hold the
   // sensors' (n_elev, n_ground, 0, 0) from rig_merge_kernel, row merge_rows the merged cloud's row from the concatenation; collect
   // moves its num_cluster / n_boxes into row 0 (collect_result)
@@ -211,7 +221,12 @@ struct Slot {
   int* d_done = nullptr;               // last-CTA-done counter
   int* d_det_sem = nullptr;            // semaphore: +1 by box_fit_kernel's last CTA (frame submissions), -1 by spawn_output_kernel
 
-  struct Result* res = nullptr;        // result block of the frame currently (or last) processed on this slot
+  // ---- detection area (detect_area.cu; allocated on the first masked submission that uses the slot)
+  unsigned* d_area_mask = nullptr;     // [2000] cell mask of the unit this slot box-fits, in the bit-plane layout
+  AreaBlock* d_area = nullptr;         // vertex staging: one block on a frame slot, kMaxBatch on a bank pseudo-slot
+  bool area_last = false;              // the slot's most recent frame was masked (lmot_cluster_outputs)
+
+  struct Result* res = nullptr;       // result block of the frame currently (or last) processed on this slot
 };
 
 enum HostHdr { HDR_N_ELEV = 0, HDR_N_GROUND, HDR_NUM_CLUSTER, HDR_N_BOXES, HDR_N_TRACKS, HDR_N_VIS, HDR_ERROR, HDR_WARN, HDR_N_ACT, HDR_COUNT = 16 };
@@ -293,6 +308,7 @@ struct SeqTick {
   uint32_t stepped = 0;                // bit k: sequence k stepped in this tick
   bool in_flight = false;
   float* h_deskew = nullptr;           // deskew: pinned host source of the tick's pose tables, as Result::h_deskew (lmot_seq_set_deskew)
+  AreaBlock* h_area = nullptr;         // detection areas: [kMaxBatch] pinned blocks, as Result::h_area (lmot_seq_set_detect_area)
 };
 
 // lmot_default_deskew
@@ -317,7 +333,9 @@ struct StreamCfg {
   bool det_on = false;
   lmot_detect_params det = {};
   lmot_deskew deskew = deskew_defaults();   // sweep deskew (deskew.cu)
+  AreaBlock area = {};                      // detection area (detect_area.cu)
   bool merges() const { return rig_merge && n_sensors > 0; }
+  bool masked() const { return area.n_rings > 0; }
 };
 
 struct Ctx {
@@ -391,6 +409,10 @@ struct Ctx {
   size_t pred_stage_bytes = 0;
   int* h_pred_n = nullptr;             // pinned: the staged row count
 
+  // ---- lmot_debug_area_masks: the unit masks of the most recent own-stream submission (none: it was not masked)
+  const unsigned* area_dbg[kMaxBatch] = {};
+  int n_area_dbg = 0;
+
   // ---- timing
   bool timing = false;
   float stage_ms[4] = {0, 0, 0, 0};
@@ -457,18 +479,20 @@ bool ground_reads_input_once(const Ctx* c, int n);
 int ground_repack(Ctx* c, cudaStream_t st, const float* d_in, int n, int stride, float4* d_out);
 int cluster_alloc(Ctx* c, Slot* s);
 void cluster_free(Slot* s);
-int cluster_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool counted = false);
-int ccl_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st);
+// area (nullable): unit i's cell mask (detect_area.cu), nullptr for an unmasked unit; any mask -> the masking kernel variants
+int cluster_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool counted = false, const unsigned* area = nullptr);
+int ccl_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const unsigned* const* area = nullptr);
 int cluster_cells_only(Ctx* c, Slot* s, cudaStream_t st, int n_upper);
 int cluster_outputs_launch(Ctx* c, Slot* s, cudaStream_t st);      // makeClusteredCloud / setObsMsg / createCostMap  // d_cart for a cloud whose label grid comes from the caller
 int boxfit_alloc(Ctx* c, Slot* s);
 int boxfit_alloc_shared(Ctx* c);
 void boxfit_free(Slot* s);
-int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem = false);
+int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem = false, const unsigned* area = nullptr);
 // rig (nullable): sensor i's sensor_height for frame i (box fitting) / sensor i's pose for list i (concatenation)
 // det (nullable): frame i's own detection values, as ground_launch_batch's; rig is then unused
+// area (nullable): as ccl_launch_batch's
 int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig = nullptr,
-                        const lmot_detect_params* det = nullptr);
+                        const lmot_detect_params* det = nullptr, const unsigned* const* area = nullptr);
 int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int n_lists, int cap, float* d_boxes, int* d_counters,
                             const lmot_sensor* rig = nullptr);
 int boxes_concat_launch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, float* d_boxes, int* d_counters, int* d_frame_counts, int* det_sem,
@@ -513,5 +537,15 @@ void merge_unit_destroy(Slot* u);      // frees whatever is allocated (also a pa
 // (grid bound).  roi[u]: unit u's clustering ROI
 int rig_merge_launch(Ctx* c, cudaStream_t st, Slot* const* src, const lmot_sensor* pose, const int* n_upper, int n_units, const int* s0,
                      Slot* const* units, int* const* frame_counts, const float* roi);
+// detection areas (detect_area.cu).  area_valid: lmot_area's rules; area_copy: a valid area into its staging block (NULL: off)
+bool area_valid(const lmot_area* a);
+void area_copy(AreaBlock& dst, const lmot_area* a);
+// lmot_detect_area_mask of a staged area: pose = row-major 3x4 (nullptr: identity), out = uint32[2000]
+void area_mask_host(const AreaBlock& a, const float* pose, float roi, unsigned* out);
+// the unit buffers a masked submission needs on slot s (its mask, and `blocks` vertex staging blocks when blocks > 0), allocated once
+int area_ensure(Ctx* c, Slot* s, int blocks);
+// one launch over the masked units of a submission: unit i's mask from its stream's staged block a, its pose and roi
+struct AreaJob { const AreaBlock* a; unsigned* mask; float pose[12]; float roi; };
+int area_launch(Ctx* c, cudaStream_t st, const AreaJob* jobs, int n_jobs);
 
 }  // namespace lmot

@@ -93,6 +93,7 @@ bool merge_unit_ready(const Slot* u) {
 
 void merge_unit_destroy(Slot* u) {
   cudaFree(u->d_elev); cudaFree(u->d_counters);              // (cudaFree(nullptr) is a no-op: a partly created unit is fine)
+  cudaFree(u->d_area_mask);
   cluster_free(u); boxfit_free(u);
   *u = Slot{};
 }

@@ -729,6 +729,69 @@ int lmot_seq_get_deskew(const lmot_ctx* ctx, int k, lmot_deskew* d);
 /* the pose table of one frame: v, omega as above, mount NULL: identity */
 int lmot_deskew_table(const lmot_deskew* d, double v, double omega, const lmot_sensor* mount, float out[LMOT_DESKEW_SLICES][12]);
 
+/* ---- detection areas: cluster and box only the elevated points inside caller-given polygons -------------------------------------------
+ * The detector is geometric: every elevated cluster that passes the rule filter becomes a box, and every unmatched box spawns a track --
+ * poles, hedges, building corners, parked rows and the ego vehicle's own body included.  A detection area restricts clustering and box
+ * fitting to a region of interest (a drivable-area polygon from a map, moved into the vehicle frame each tick) or, with keep_outside,
+ * excludes zones from them, while ground removal still sees the whole frame.
+ *
+ * Definition.  An area is a set of closed polygon rings, vertices double (x, y) in metres in the VEHICLE frame (a stream without a sensor
+ * table: the sensor frame).  For every unit of a FRAMES step of a stream with an area (a table-less frame, an unmerged rig frame, or a
+ * merge unit):
+ *   1. ground removal runs exactly as without an area: n_elevated, n_ground and both clouds are unchanged;
+ *   2. the unit has a pose M = [R | t] (table-less frame and merge unit: identity; unmerged rig frame: sensor j's pose) and a clustering
+ *      extent roi (lmot_params.roi_m, or the sequence's lmot_detect_params.roi_m).  Its cell mask is lmot_detect_area_mask(area, pose, roi):
+ *      the 250 x 250 clustering grid in the bit-plane layout word x*8 + (y>>5), bit y&31 (bits above 250 in word 7 are 0).  All arithmetic
+ *      is double, evaluated left to right without contraction; the pose is widened from float and only its xy block is used:
+ *        vertex p in unit coordinates: dx = px - t0, dy = py - t1, u = r00*dx + r10*dy, w = r01*dx + r11*dy (identity: exactly (px, py));
+ *        cell centre cx(xI) = ((double)xI + 0.5) * roi / 250.0 - roi / 2.0, cy(yI) likewise;
+ *        PNPOLY with the ray along +y: an edge a -> b (rings closed implicitly) straddles row xI iff (a.u > cx) != (b.u > cx), and crosses it
+ *        at yc = a.w + (cx - a.u) * (b.w - a.w) / (b.u - a.u); cell (xI, yI) is inside iff an odd number of straddling edges, over all
+ *        rings, have cy(yI) < yc (even-odd: nested rings are holes, rectangles rasterise a raster);
+ *        mask bit = inside != keep_outside;
+ *   3. E_area = the points of the unit's elevated cloud whose clustering cell (componentClustering's float binning with the unit's roi)
+ *      has its mask bit set, in cloud order;
+ *   4. componentClustering(E_area) and boxFitting(E_area, grid, numCluster) with the unit's values; the tracker, global frame, retirement
+ *      and the rest run as usual on those boxes.
+ * That is the pipeline without an area with this filter between ground removal and clustering, bit for bit.
+ *
+ * Applies to lmot_frame / _submit / _dev and lmot_detect_dev (lmot_set_detect_area), lmot_batch* including lmot_batch_detect_dev (the
+ * context's area), and the FRAMES steps of lmot_seq* / lmot_seq_tick* (lmot_seq_set_detect_area).  Never to the stage entry points,
+ * lmot_batch_ground_ccl_dev, lmot_track_step*, LISTS steps and lmot_seq_track*.  lmot_cluster_outputs after a masked lmot_frame describes
+ * E_area (makeClusteredCloud, setObsMsg and createCostMap on E_area).
+ * Host state captured by value at submission, like the sensor tables: ticks in flight keep theirs, so a moving vehicle sets its polygons
+ * before each submission.  lmot_seq_open turns every sequence's area off; lmot_seq_tracker_reset / _load and LMOT_SEQ_RESTART keep it.
+ * The library copies the vertices.  NULL or n_rings = 0 turns the area off; a submission without an area runs exactly the launches it ran
+ * before areas existed.  A masked submission clusters in a launch of its own instead of the ground kernel's tail.
+ * Errors.  LMOT_ERR_INVALID, setting unchanged: n_rings outside [0, LMOT_AREA_MAX_RINGS], a ring with fewer than 3 vertices, more than
+ * LMOT_AREA_MAX_VERTICES vertices in all, a non-finite vertex, keep_outside not 0 or 1, null pointers with n_rings > 0, k out of range or
+ * no open set.  LMOT_ERR_STATE, nothing submitted: a masked submission in timing mode.
+ * Memory: on the first masked submission, 8 KB of mask per detection slot, batch slot or merge unit it uses, and 16.3 KB of vertex staging
+ * per stream, pinned per result-ring entry (sequence ticks: per ring tick and sequence) and on the device per slot or bank.  Freed with
+ * the context.
+ * lmot_detect_area_mask(area, mount, roi_m, out): the mask of step 2 on the host (no device needed), mount NULL: identity.
+ * lmot_get_detect_area / lmot_seq_get_detect_area: the counts into *n_rings / *n_vertices / *keep_outside (each nullable), and as many
+ * ring lengths and vertices as cap_rings / cap_vertices hold (ring_len / xy nullable when their capacity is 0).
+ * lmot_debug_area_masks(ctx, out, cap_units, n_units): the device masks of the context's most recent own-stream submission (lmot_frame*,
+ * lmot_detect_dev, lmot_batch*), one per unit in unit order, out = uint32[cap_units][LMOT_NUM_GRID * 8]; *n_units = 0 when it was not
+ * masked.  Waits for the device. */
+#define LMOT_AREA_MAX_RINGS 64
+#define LMOT_AREA_MAX_VERTICES 1024
+typedef struct lmot_area {
+  int n_rings;
+  const int* ring_len;         /* [n_rings] vertices of each ring, >= 3 */
+  const double* xy;            /* [sum(ring_len)][2] vertices, ring after ring, metres in the vehicle frame */
+  int keep_outside;            /* 0: keep the inside; 1: keep the outside (exclusion zones) */
+} lmot_area;
+int lmot_set_detect_area(lmot_ctx* ctx, const lmot_area* area);
+int lmot_get_detect_area(const lmot_ctx* ctx, int* n_rings, int* ring_len, int cap_rings, int* n_vertices, double* xy, int cap_vertices,
+                         int* keep_outside);
+int lmot_seq_set_detect_area(lmot_ctx* ctx, int k, const lmot_area* area);
+int lmot_seq_get_detect_area(const lmot_ctx* ctx, int k, int* n_rings, int* ring_len, int cap_rings, int* n_vertices, double* xy,
+                             int cap_vertices, int* keep_outside);
+int lmot_detect_area_mask(const lmot_area* area, const lmot_sensor* mount, float roi_m, uint32_t out[LMOT_NUM_GRID * 8]);
+int lmot_debug_area_masks(lmot_ctx* ctx, uint32_t* out, int cap_units, int* n_units);
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);
