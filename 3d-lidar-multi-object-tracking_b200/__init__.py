@@ -258,6 +258,54 @@ def detect_area_mask(rings, keep_outside=False, mount=None, roi_m=50.0) -> np.nd
     return out
 
 
+class Accumulate(C.Structure):
+    """lmot_accumulate: sweep accumulation of the context's frames (include/lmot.h)."""
+    _fields_ = [("sweeps", C.c_int), ("max_age_s", C.c_double)]
+
+
+MAX_SWEEPS = 8                          # LMOT_MAX_SWEEPS
+
+
+class AccumInfo(C.Structure):
+    """lmot_accum_info: what the most recently returned frame result accumulated, per unit."""
+    _fields_ = [("n_units", C.c_int), ("sweeps_used", C.c_int * 8), ("n_points", C.c_int * 8),
+                ("stamp_us", (C.c_double * (MAX_SWEEPS - 1)) * 8), ("pose", ((C.c_float * 12) * (MAX_SWEEPS - 1)) * 8)]
+
+
+def default_accumulate() -> dict:
+    lib = load_library()
+    a = Accumulate()
+    lib.lmot_default_accumulate(C.byref(a))
+    return {name: getattr(a, name) for name, _ in Accumulate._fields_}
+
+
+def _accumulate(fields: dict) -> Accumulate:
+    base = default_accumulate()
+    unknown = set(fields) - set(base)
+    if unknown:
+        raise KeyError(f"unknown accumulate fields {sorted(unknown)}")
+    base.update(fields)
+    return Accumulate(int(base["sweeps"]), float(base["max_age_s"]))
+
+
+def accumulate_pose(fold_s, fold_t, mount=None) -> np.ndarray:
+    """lmot_accumulate_pose: the (3, 4) float32 pose D moving a sweep recorded at fold_s = (x, y, yaw) (ego8[5..7] after that step) into
+    the frame of fold_t, for a unit mounted at `mount` ((3, 4) or (12,) [R | t]; None: identity)."""
+    lib = load_library()
+    fs = np.ascontiguousarray(fold_s, np.float64).reshape(3)
+    ft = np.ascontiguousarray(fold_t, np.float64).reshape(3)
+    m = None
+    if mount is not None:
+        m = Sensor()
+        lib.lmot_default_sensor(None, C.byref(m))
+        m.pose[:] = [float(x) for x in np.asarray(mount, np.float32).reshape(12)]
+    out = np.zeros(12, np.float32)
+    st = lib.lmot_accumulate_pose(fs.ctypes.data, ft.ctypes.data, C.cast(C.byref(m), C.c_void_p) if m is not None else None, out.ctypes.data)
+    if st != OK:
+        raise LmotError(st, lib.lmot_strerror(st).decode())
+    return out.reshape(3, 4)
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -315,6 +363,8 @@ ABI_SYMBOLS = [
     "lmot_default_deskew", "lmot_set_deskew", "lmot_get_deskew", "lmot_seq_set_deskew", "lmot_seq_get_deskew", "lmot_deskew_table",
     "lmot_set_detect_area", "lmot_get_detect_area", "lmot_seq_set_detect_area", "lmot_seq_get_detect_area", "lmot_detect_area_mask",
     "lmot_debug_area_masks",
+    "lmot_default_accumulate", "lmot_set_accumulate", "lmot_get_accumulate", "lmot_accumulate_info", "lmot_accumulate_pose",
+    "lmot_seq_set_accumulate", "lmot_seq_get_accumulate", "lmot_seq_accumulate_info",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
@@ -342,6 +392,7 @@ def load_library() -> C.CDLL:
         lib.lmot_last_error.argtypes = [C.c_void_p]
         lib.lmot_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(Params), C.c_int]
         lib.lmot_destroy.argtypes = [C.c_void_p]
+        lib.lmot_accumulate_pose.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = lib
     return _lib
 
@@ -920,6 +971,49 @@ class Lmot:
         fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
         self._chk(fn(self.h, out.ctypes.data, MAX_BATCH, C.byref(n)))
         return out[: n.value]
+
+    # ---- sweep accumulation (lmot_set_accumulate) ----------------------------------------------------------------------------------
+    def set_accumulate(self, **fields):
+        """The context's frames: accumulation settings with `fields` replaced (sweeps=K > 1 turns it on; no fields: the defaults, off).
+        Applies from the next submitted frame on; the history starts empty again."""
+        self._chk(self.lib.lmot_set_accumulate(self.h, C.byref(_accumulate(fields)) if fields else None))
+
+    def get_accumulate(self) -> dict:
+        a = Accumulate()
+        self._chk(self.lib.lmot_get_accumulate(self.h, C.byref(a)))
+        return {name: getattr(a, name) for name, _ in Accumulate._fields_}
+
+    def seq_set_accumulate(self, k: int, **fields):
+        """Sequence k's FRAMES steps, arguments as set_accumulate."""
+        self._chk(self.lib.lmot_seq_set_accumulate(self.h, int(k), C.byref(_accumulate(fields)) if fields else None))
+
+    def seq_get_accumulate(self, k: int) -> dict:
+        a = Accumulate()
+        self._chk(self.lib.lmot_seq_get_accumulate(self.h, int(k), C.byref(a)))
+        return {name: getattr(a, name) for name, _ in Accumulate._fields_}
+
+    @staticmethod
+    def _accum_info(a: AccumInfo) -> list:
+        out = []
+        for u in range(a.n_units):
+            k = a.sweeps_used[u]
+            out.append(dict(sweeps_used=k, n_points=a.n_points[u],
+                            stamp_us=np.array([a.stamp_us[u][j] for j in range(k)], np.float64),
+                            pose=np.array([list(a.pose[u][j]) for j in range(k)], np.float32).reshape(k, 3, 4)))
+        return out
+
+    def accumulate_info(self) -> list:
+        """lmot_accumulate_info: one dict per unit of the most recently returned own-stream result (empty: it did not accumulate):
+        sweeps_used, n_points (|E_acc|), stamp_us (sweeps_used,) and pose (sweeps_used, 3, 4) of the used sweeps, newest first."""
+        a = AccumInfo()
+        self._chk(self.lib.lmot_accumulate_info(self.h, C.byref(a)))
+        return self._accum_info(a)
+
+    def seq_accumulate_info(self, k: int) -> list:
+        """lmot_seq_accumulate_info: as accumulate_info, for sequence k's most recently returned step"""
+        a = AccumInfo()
+        self._chk(self.lib.lmot_seq_accumulate_info(self.h, int(k), C.byref(a)))
+        return self._accum_info(a)
 
     def seq_frame_counts(self, k: int) -> np.ndarray:
         """(n_frames, 4) int32: n_elevated, n_ground, num_cluster, n_boxes of each of sequence k's frames in the tick collected last"""

@@ -185,6 +185,7 @@ Result* acquire_result(Ctx* c, bool drop_oldest) {
   c->res_next = (c->res_next + 1) % c->n_results;
   c->last_res = r;
   r->merge_rows = 0;                             // only a merging batched tick sets it (batch_common): collect_result reads it
+  r->acc_units = 0;                              // only an accumulating step sets it (accumulate_step)
   return r;
 }
 
@@ -222,6 +223,19 @@ int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tra
   r->batch_frames = 0;
   // the slot's previous boxes / counters must have been consumed by the tracker
   LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_trk_done, 0));
+  // sweep accumulation: the frame's candidate sweeps from the stream's history into r and the launch's job (the ring on first use);
+  // fit_upper bounds |E_acc| for the launches behind accumulate_kernel
+  AccHist& h = c->own_cfg.acc;
+  const bool acc = with_tracker && h.on();
+  AccJob aj;
+  int fit_upper = n;
+  if (acc) {
+    lmot_sensor id;
+    lmot_default_sensor(&c->prm, &id);
+    Slot* us[1] = {s};
+    const float roi = c->prm.roi_m;
+    if ((rc = accumulate_step(c, h, ACC_FRAME, 1, us, &id, &roi, &n, c->own.th, ts, v, yaw, r, &aj, &fit_upper))) return rc;
+  }
   // detection area: the slot's cell mask first; clustering then runs as its own launch, masked, and box fitting skips masked points
   const bool masked = c->own_cfg.masked();
   if (masked && (rc = area_frame(c, s, r))) return rc;        // (allocates the slot's mask on first use)
@@ -229,14 +243,16 @@ int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tra
   s->area_last = masked;
   c->n_area_dbg = masked ? 1 : 0;
   c->area_dbg[0] = mask;
-  const bool fuse = c->fuse_ccl && !masked;
+  const bool fuse = c->fuse_ccl && !masked && !acc;
   if (c->timing) cudaEventRecord(r->ev[0], s->stream);
   if ((rc = ground_launch(c, s, s->stream, d_pts, n, true, false, fuse))) return rc;
   if (c->timing) cudaEventRecord(r->ev[1], s->stream);
-  if (!fuse && (rc = cluster_launch(c, s, s->stream, n, true, mask))) return rc;      // (fused: the ground kernel's last CTA did it)
+  AccHist* hp = &h;
+  if (acc && (rc = accumulate_launch(c, s->stream, s, &aj, 1, &hp, 1))) return rc;     // E_t into the ring, the earlier sweeps behind it
+  if (!fuse && (rc = cluster_launch(c, s, s->stream, fit_upper, true, mask))) return rc;      // (fused: the ground kernel's last CTA did it)
   if (c->timing) cudaEventRecord(r->ev[2], s->stream);
   const bool gf = with_tracker && c->prm.global_frame;
-  if ((rc = boxfit_launch(c, s, s->stream, n, with_tracker && !gf, mask))) return rc;      // with_tracker: posts the slot's detection semaphore
+  if ((rc = boxfit_launch(c, s, s->stream, fit_upper, with_tracker && !gf, mask))) return rc;      // with_tracker: posts the slot's detection semaphore
   if (gf && (rc = boxes_to_global_launch(c, s, s->stream, s->d_boxes, s->d_counters, ts, v, yaw, true))) return rc;   // ... or this one does
   if (c->timing) cudaEventRecord(r->ev[3], s->stream);
   LMOT_CUDA(c, cudaEventRecord(s->ev_det_done, s->stream));
@@ -345,6 +361,7 @@ struct DetGroup {
   int nf;
   double ts, v, yaw;
   int* fc;                             // device view of the stream's per-frame counts in its result block (nullptr: none are written)
+  Result* res = nullptr;               // the stream's result block (sweep accumulation: its candidates and count rows)
 };
 
 // what the front end box-fitted, by group: group g's units are u[f0[g] .. f0[g + 1]) (its frames, or its merge unit), unit i with pose
@@ -469,12 +486,31 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
     if ((rc = area_launch(c, st, aj, na))) return rc;
   }
   const unsigned* const* area = nblk > 0 ? amask : nullptr;
-  const bool fuse = c->fuse_ccl && !merging && nblk == 0;
+  // sweep accumulation: a group with a stamp whose stream accumulates -- its units' candidates and jobs (accumulate.cu), one launch for
+  // every accumulating unit behind the ground kernel and the rig merge; clustering then runs as its own launch
+  AccJob acj[kMaxBatch];
+  AccHist* ach[kMaxBatch];
+  int nacj = 0, nach = 0;
+  for (int d = 0; d < G; ++d) {
+    StreamCfg& q = *g[d].cfg;
+    if (!g[d].th || !q.acc.on()) continue;
+    const int u0 = U.f0[d], nu_d = U.f0[d + 1] - u0;
+    const int kind = q.merges() ? ACC_MERGE : q.n_sensors > 0 ? ACC_RIG : ACC_FRAME;
+    const float roi = (q.det_on ? q.det : base).roi_m;
+    float rois[kMaxBatch];
+    for (int i = 0; i < nu_d; ++i) rois[i] = roi;
+    if ((rc = accumulate_step(c, q.acc, kind, nu_d, U.u + u0, U.rig + u0, rois, unn + u0, *g[d].th, g[d].ts, g[d].v, g[d].yaw, g[d].res,
+                              acj + nacj, unn + u0))) return rc;
+    nacj += nu_d;
+    ach[nach++] = &q.acc;
+  }
+  const bool fuse = c->fuse_ccl && !merging && nblk == 0 && nacj == 0;
   Result* r = bk->res;
   if (c->timing) cudaEventRecord(r->ev[0], st);
   if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, fuse, false, rigged ? rig : nullptr, own_det ? det : nullptr))) return rc;
   if (c->timing) cudaEventRecord(r->ev[1], st);
   if (nm > 0 && (rc = rig_merge_launch(c, st, src, mpose, mn, nm, ms0, mu, mfc, mroi))) return rc;
+  if (nacj > 0 && (rc = accumulate_launch(c, st, bk, acj, nacj, ach, nach))) return rc;
   if (!fuse && (rc = ccl_launch_batch(c, U.u, nu, st, area))) return rc;
   if (c->timing) cudaEventRecord(r->ev[2], st);
   return boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr, area);
@@ -532,6 +568,31 @@ int collect_result(Ctx* c, Result* r, lmot_frame_out* out, Tracker* trk = nullpt
     int ne = 0;
     for (int j = 0; j < F; ++j) ne += fc[4 * j];
     r->h_hdr[HDR_N_ELEV] = ne;
+  }
+  if (r->acc_units > 0 && r->merge_rows == 0) {
+    // accumulating units: clustering counted E_acc, n_elevated is each frame's own (a merge unit's rows are the sensors' already)
+    if (r->batch_frames > 0) {
+      for (int u = 0; u < r->acc_units; ++u) {
+        r->h_hdr[HDR_N_ELEV] -= r->h_frame_counts[4 * u] - r->h_acc[4 * u + 2];
+        r->h_frame_counts[4 * u] = r->h_acc[4 * u + 2];
+      }
+    } else {
+      r->h_hdr[HDR_N_ELEV] = r->h_acc[2];
+    }
+  }
+  {                                                   // lmot_accumulate_info / lmot_seq_accumulate_info: what this result used
+    lmot_accum_info& ai = trk ? c->seq_acc_info[trk - c->seq] : c->acc_info;
+    memset(&ai, 0, sizeof(ai));
+    ai.n_units = r->acc_units;
+    for (int u = 0; u < r->acc_units; ++u) {
+      const int used = r->h_acc[4 * u + 1] < r->acc_cand ? r->h_acc[4 * u + 1] : r->acc_cand;
+      ai.sweeps_used[u] = used;
+      ai.n_points[u] = r->h_acc[4 * u];
+      for (int j = 0; j < used; ++j) {
+        ai.stamp_us[u][j] = r->acc_ts[j];
+        memcpy(ai.pose[u][j], r->acc_pose[u][j], sizeof(ai.pose[u][j]));
+      }
+    }
   }
   const int err = r->h_hdr[HDR_ERROR];
   const int warn = r->has_tracks ? r->h_hdr[HDR_WARN] : 0;
@@ -605,6 +666,7 @@ void result_destroy(Result* r) {
   if (r->h_ids) cudaFreeHost(r->h_ids);
   if (r->h_deskew) cudaFreeHost(r->h_deskew);
   if (r->h_area) cudaFreeHost(r->h_area);
+  if (r->h_acc) cudaFreeHost(r->h_acc);
   if (r->d_ids) cudaFree(r->d_ids);
   if (r->d_block) cudaFree(r->d_block);
   if (r->ev_tc) cudaEventDestroy(r->ev_tc);
@@ -628,7 +690,9 @@ void seq_destroy(Ctx* c) {
   for (int b = 0; b < kBatchBanks; ++b) { cudaFree(c->seq_stage[b]); c->seq_stage[b] = nullptr; }
   for (int k = 0; k < kMaxBatch; ++k) {
     for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&c->seq_cfg[k].merge_unit[b]);
+    accumulate_free(c->seq_cfg[k].acc);
     c->seq_cfg[k] = StreamCfg{};
+    c->seq_acc_info[k] = lmot_accum_info{};
     c->seq_fc_n[k] = 0;
   }
   for (int i = 0; i < c->seq_ring; ++i) {
@@ -834,6 +898,7 @@ void lmot_destroy(lmot_ctx* ctx) {
   batch_destroy(c);
   for (int i = 0; i < c->n_results; ++i) result_destroy(&c->results[i]);
   tracker_free(c->own);
+  accumulate_free(c->own_cfg.acc);
   seq_destroy(c);
   cudaFree(c->d_mt_raw);
   if (c->ev_pred) cudaEventDestroy(c->ev_pred);
@@ -1072,7 +1137,7 @@ int lmot_frame_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp
   if (!ctx || n < 0 || (n > 0 && !d_points) || (reinterpret_cast<uintptr_t>(d_points) & 15u)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   const bool dsk = c->own_cfg.deskew.on != 0;
-  if ((dsk || c->own_cfg.masked()) && c->timing) return LMOT_ERR_STATE;
+  if ((dsk || c->own_cfg.masked() || c->own_cfg.acc.on()) && c->timing) return LMOT_ERR_STATE;
   if (dsk && c->own_cfg.deskew.time_field != 3) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
@@ -1093,7 +1158,7 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
-  if (c->own_cfg.masked() && c->timing) return LMOT_ERR_STATE;
+  if ((c->own_cfg.masked() || c->own_cfg.acc.on()) && c->timing) return LMOT_ERR_STATE;
   const bool dsk = c->own_cfg.deskew.on != 0;
   if (dsk) {                           // (validated before anything is submitted: upload_points checks the rest without deskew)
     if (c->timing) return LMOT_ERR_STATE;
@@ -1203,6 +1268,7 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   if (dsk && c->timing) return LMOT_ERR_STATE;
   if (dsk && (host ? stride <= q.deskew.time_field : q.deskew.time_field != 3)) return LMOT_ERR_INVALID;
   if ((q.merges() || q.masked()) && c->timing) return LMOT_ERR_STATE;
+  if (with_tracker && q.acc.on() && c->timing) return LMOT_ERR_STATE;
   if (host && c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;
   int rc = batch_ensure(c, n_frames);
   if (rc) return rc;
@@ -1226,7 +1292,7 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   r->merge_rows = q.merges() ? n_frames : 0;
   int* d_fc = nullptr;                       // the per-frame counts go straight into the result's pinned, device-mapped block
   LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&d_fc, r->h_frame_counts, 0));
-  const DetGroup grp{&q, with_tracker ? &c->own.th : nullptr, points, n, n_frames, ts, v, yaw, d_fc};
+  const DetGroup grp{&q, with_tracker ? &c->own.th : nullptr, points, n, n_frames, ts, v, yaw, d_fc, r};
   DetUnits U;
   if ((rc = detect_front(c, b, &grp, 1, stride, host, r->h_deskew, r->h_area, false, U))) return rc;
   c->n_area_dbg = q.masked() ? U.f0[1] : 0;
@@ -1484,11 +1550,13 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
     ++p;
     stepped |= 1u << k;
     if (e[k].flags & LMOT_SEQ_RESTART) {
+      c->seq_cfg[k].acc.forget();
       tracker_restart_host(c->seq[k]);
       LMOT_CUDA(c, cudaMemsetAsync(c->seq[k].d_trk_counters, 0, CNT_COUNT * sizeof(int), c->trk_stream));
     }
     Result* r = &t->blocks[k];
     r->n_kev = 0; r->has_tracks = true;
+    r->acc_units = 0;                  // (an accumulating FRAMES step sets it in detect_front)
     // > 0: the concatenation / pack writes the block's per-frame counts; 0: one frame, counts from the header
     r->batch_frames = (e[k].kind == LMOT_SEQ_LISTS || rigged) ? f0[k + 1] - f0[k] : 0;
     r->merge_rows = merge[k] ? f0[k + 1] - f0[k] : 0;
@@ -1543,7 +1611,7 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
       int* fc = nullptr;
       if (rigged) LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc, t->blocks[k].h_frame_counts, 0));
       gk[G] = k;
-      g[G++] = DetGroup{&c->seq_cfg[k], &c->seq[k].th, e[k].data, e[k].n, f0[k + 1] - f0[k], e[k].timestamp_us, e[k].v_gps, e[k].yaw_gps, fc};
+      g[G++] = DetGroup{&c->seq_cfg[k], &c->seq[k].th, e[k].data, e[k].n, f0[k + 1] - f0[k], e[k].timestamp_us, e[k].v_gps, e[k].yaw_gps, fc, &t->blocks[k]};
     }
     DetUnits U;
     if ((rc = detect_front(c, b, g, G, stride, host, t->h_deskew, t->h_area, !rigged && !gf, U))) return rc;
@@ -1783,7 +1851,11 @@ static int sensors_get(const StreamCfg& q, lmot_sensor* s, int cap, int* n) {
   return LMOT_OK;
 }
 
-int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n) { return ctx ? sensors_set(ctx->c.own_cfg, s, n) : LMOT_ERR_INVALID; }
+int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  ctx->c.own_cfg.acc.forget();                    // sweep accumulation: the history starts empty again (set or not)
+  return sensors_set(ctx->c.own_cfg, s, n);
+}
 
 int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n) { return ctx ? sensors_get(ctx->c.own_cfg, s, cap, n) : LMOT_ERR_INVALID; }
 
@@ -1791,6 +1863,7 @@ int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n) { ret
 int lmot_seq_set_sensors(lmot_ctx* ctx, int k, const lmot_sensor* s, int n) {
   if (!ctx || k < 0 || k >= ctx->c.n_seq || !sensors_valid(s, n)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
+  c->seq_cfg[k].acc.forget();          // sweep accumulation: the history starts empty again (set or not)
   int frames = 0;
   for (int j = 0; j < c->n_seq; ++j) {
     const int nj = j == k ? n : c->seq_cfg[j].n_sensors;
@@ -1816,12 +1889,18 @@ static int rig_merge_get(const StreamCfg& q, int* on) {
   return LMOT_OK;
 }
 
-int lmot_set_rig_merge(lmot_ctx* ctx, int on) { return ctx ? rig_merge_set(ctx->c.own_cfg, on) : LMOT_ERR_INVALID; }
+int lmot_set_rig_merge(lmot_ctx* ctx, int on) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  ctx->c.own_cfg.acc.forget();
+  return rig_merge_set(ctx->c.own_cfg, on);
+}
 
 int lmot_get_rig_merge(const lmot_ctx* ctx, int* on) { return ctx ? rig_merge_get(ctx->c.own_cfg, on) : LMOT_ERR_INVALID; }
 
 int lmot_seq_set_rig_merge(lmot_ctx* ctx, int k, int on) {
-  return ctx && k >= 0 && k < ctx->c.n_seq ? rig_merge_set(ctx->c.seq_cfg[k], on) : LMOT_ERR_INVALID;
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  ctx->c.seq_cfg[k].acc.forget();
+  return rig_merge_set(ctx->c.seq_cfg[k], on);
 }
 
 int lmot_seq_get_rig_merge(const lmot_ctx* ctx, int k, int* on) {
@@ -2005,6 +2084,75 @@ int lmot_deskew_table(const lmot_deskew* d, double v, double omega, const lmot_s
   return deskew_table(*d, v, omega, mount, &out[0][0]);
 }
 
+// ---- sweep accumulation (accumulate.cu).  Host state, as deskew: turning it on pins each result block's count block (once)
+int lmot_default_accumulate(lmot_accumulate* a) {
+  if (!a) return LMOT_ERR_INVALID;
+  *a = accumulate_defaults();
+  return LMOT_OK;
+}
+
+// a (NULL: the defaults) validated into the stream's setting; turning it on pins the count rows of `n` result blocks `stride` bytes apart
+// (once).  The history starts empty again.
+static int accumulate_set(Ctx* c, AccHist& h, const lmot_accumulate* a, Result* blocks, int n, size_t stride) {
+  const lmot_accumulate v = a ? *a : accumulate_defaults();
+  if (!accumulate_valid(v)) return LMOT_ERR_INVALID;
+  if (v.sweeps > 1) {
+    cudaSetDevice(c->device);
+    for (int i = 0; i < n; ++i) {
+      Result* r = reinterpret_cast<Result*>(reinterpret_cast<char*>(blocks) + i * stride);
+      if (!r->h_acc) {
+        LMOT_CUDA(c, cudaHostAlloc((void**)&r->h_acc, 4 * kMaxBatch * sizeof(int), cudaHostAllocMapped));
+        memset(r->h_acc, 0, 4 * kMaxBatch * sizeof(int));
+      }
+    }
+  }
+  h.cfg = v;
+  h.forget();                          // (the next accumulate launch is ordered behind every earlier one: entry 0 is free)
+  return LMOT_OK;
+}
+
+int lmot_set_accumulate(lmot_ctx* ctx, const lmot_accumulate* a) {
+  if (!ctx) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  return accumulate_set(c, c->own_cfg.acc, a, &c->results[0], c->n_results, sizeof(Result));
+}
+
+int lmot_get_accumulate(const lmot_ctx* ctx, lmot_accumulate* a) {
+  if (!ctx || !a) return LMOT_ERR_INVALID;
+  *a = ctx->c.own_cfg.acc.cfg;
+  return LMOT_OK;
+}
+
+int lmot_seq_set_accumulate(lmot_ctx* ctx, int k, const lmot_accumulate* a) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  return accumulate_set(c, c->seq_cfg[k].acc, a, &c->seq_ticks[0].blocks[k], c->seq_ring, sizeof(SeqTick));
+}
+
+int lmot_seq_get_accumulate(const lmot_ctx* ctx, int k, lmot_accumulate* a) {
+  if (!ctx || !a || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  *a = ctx->c.seq_cfg[k].acc.cfg;
+  return LMOT_OK;
+}
+
+int lmot_accumulate_info(lmot_ctx* ctx, lmot_accum_info* out) {
+  if (!ctx || !out) return LMOT_ERR_INVALID;
+  *out = ctx->c.acc_info;
+  return LMOT_OK;
+}
+
+int lmot_seq_accumulate_info(lmot_ctx* ctx, int k, lmot_accum_info* out) {
+  if (!ctx || !out || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  *out = ctx->c.seq_acc_info[k];
+  return LMOT_OK;
+}
+
+int lmot_accumulate_pose(const double fold_s[3], const double fold_t[3], const lmot_sensor* mount, float out[12]) {
+  if (!fold_s || !fold_t || !out || (mount && !sensors_valid(mount, 1))) return LMOT_ERR_INVALID;
+  accumulate_pose(fold_s, fold_t, mount ? mount->pose : nullptr, out);
+  return LMOT_OK;
+}
+
 // ---- detection areas (detect_area.cu).  Host state only, as the sensor tables; setting one allocates the pinned staging blocks of the
 // ring (once): `per` blocks at each of the n entries `blocks`, `stride` bytes apart
 static int area_set(Ctx* c, AreaBlock& dst, const lmot_area* a, AreaBlock** blocks, int n, size_t stride, int per) {
@@ -2112,6 +2260,7 @@ static int tracker_reset(Ctx* c, Tracker& t) {
 
 int lmot_tracker_reset(lmot_ctx* ctx) {
   if (!ctx) return LMOT_ERR_INVALID;
+  ctx->c.own_cfg.acc.forget();                    // sweep accumulation: the history starts empty again
   return tracker_reset(&ctx->c, ctx->c.own);
 }
 
@@ -2234,6 +2383,7 @@ static int tracker_load(Ctx* c, Tracker& trk, const double* dumps, int n, int in
 int lmot_tracker_load(lmot_ctx* ctx, const double* dumps, int n, int init, double timestamp_us, double ego_velo,
                       double ego_yaw, double ego_pre_yaw, double ego_point_yaw) {
   if (!ctx) return LMOT_ERR_INVALID;
+  ctx->c.own_cfg.acc.forget();
   return tracker_load(&ctx->c, ctx->c.own, dumps, n, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw);
 }
 
@@ -2411,6 +2561,7 @@ int lmot_seq_predict_tracks_dev(lmot_ctx* ctx, const double* t_us, int n_t, cons
 int lmot_seq_tracker_reset(lmot_ctx* ctx, int k) {
   if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
+  c->seq_cfg[k].acc.forget();          // sweep accumulation: the history starts empty again
   const int rc = tracker_reset(c, c->seq[k]);
   seq_forget(c);
   return rc;
@@ -2431,6 +2582,7 @@ int lmot_seq_tracker_load(lmot_ctx* ctx, int k, const double* dumps, int n, int 
                           double ego_pre_yaw, double ego_point_yaw) {
   if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
+  c->seq_cfg[k].acc.forget();
   const int rc = tracker_load(c, c->seq[k], dumps, n, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw);
   if (rc == LMOT_OK) seq_forget(c);        // (as lmot_seq_tracker_reset: the drained ticks are dropped)
   return rc;
@@ -2448,12 +2600,14 @@ static int tracker_set_ego(Ctx* c, Tracker& t, const double ego8[8]) {
 
 int lmot_tracker_set_ego(lmot_ctx* ctx, const double ego8[8]) {
   if (!ctx || !ego8) return LMOT_ERR_INVALID;
+  ctx->c.own_cfg.acc.forget();
   return tracker_set_ego(&ctx->c, ctx->c.own, ego8);
 }
 
 int lmot_seq_tracker_set_ego(lmot_ctx* ctx, int k, const double ego8[8]) {
   if (!ctx || !ego8 || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
+  c->seq_cfg[k].acc.forget();
   const int rc = tracker_set_ego(c, c->seq[k], ego8);
   if (rc == LMOT_OK) seq_forget(c);
   return rc;

@@ -24,6 +24,7 @@ constexpr int kMaxBatch = 8;                         // frames (one per sensor s
 enum Counter {
   CNT_N_ELEV = 0, CNT_N_GROUND, CNT_NUM_CLUSTER, CNT_N_BOXES, CNT_N_CLUSTERED, CNT_ERROR, CNT_N_TRACKS, CNT_N_VIS,
   CNT_N_ACT,        // tracks the next frame has to visit (live, or dead with a stale isVisBB_ flag): length of d_act_list
+  CNT_ACC_DONE = 14,   // accumulate_kernel's finished blocks (accumulate.cu), 0 at rest
   CNT_COUNT = 16
 };
 
@@ -147,6 +148,15 @@ struct Result {
   float* h_deskew = nullptr;
   // detection area: pinned host source of the context's area staged for this block's submission (one block, lmot_set_detect_area)
   AreaBlock* h_area = nullptr;
+  // sweep accumulation (lmot_set_accumulate / lmot_seq_set_accumulate): h_acc = pinned, device-mapped [kMaxBatch][4] rows (n_points,
+  // sweeps_used, n_elevated) of the stream's units written by accumulate_kernel (allocated by the setter); acc_units: the units this
+  // block's step accumulated (0: none), with acc_cand candidate sweeps whose stamps and per-unit poses follow, newest first
+  // (accumulate_kernel used the first h_acc[4 u + 1] of them for unit u)
+  int* h_acc = nullptr;
+  int acc_units = 0;
+  int acc_cand = 0;
+  double acc_ts[LMOT_MAX_SWEEPS - 1] = {};
+  float acc_pose[kMaxBatch][LMOT_MAX_SWEEPS - 1][12] = {};
   // merging rig (lmot_set_rig_merge): the tick's sensors, 0 when it did not merge.  h_frame_counts rows 0..merge_rows-1 hold the
   // sensors' (n_elev, n_ground, 0, 0) from rig_merge_kernel, row merge_rows the merged cloud's row from the concatenation; collect
   // moves its num_cluster / n_boxes into row 0 (collect_result)
@@ -319,6 +329,29 @@ inline lmot_deskew deskew_defaults() {
   return d;
 }
 
+// lmot_default_accumulate
+inline lmot_accumulate accumulate_defaults() { lmot_accumulate a; memset(&a, 0, sizeof(a)); a.sweeps = 1; a.max_age_s = 0.5; return a; }
+
+// One stream's sweep accumulation (accumulate.cu): the setting, and the history of its last sweeps per detection unit.  Unit u's ring
+// entry e (of cap, allocated on the stream's first accumulating step for `units` units) holds E_s of the step that recorded it; the host
+// keeps that step's stamp, fold and per-unit frame sizes (bounds on |E_s|).  The n valid entries are the ones written last before entry
+// w, which the next step writes.  kind / units: the unit layout of the recorded steps (AccKind); a step with another layout starts empty.
+enum AccKind { ACC_FRAME = 0, ACC_RIG = 1, ACC_MERGE = 2 };
+struct AccHist {
+  lmot_accumulate cfg = accumulate_defaults();
+  float4* d_ring[kMaxBatch] = {};      // [cap][max_points] per unit
+  int* d_ring_n[kMaxBatch] = {};       // [cap] |E_s| per unit (written by accumulate_kernel)
+  int cap = 0, cap_units = 0;
+  int n = 0, w = 0, kind = -1, units = 0;
+  double ts[LMOT_MAX_SWEEPS] = {};
+  double fold[LMOT_MAX_SWEEPS][3] = {};
+  int n_upper[LMOT_MAX_SWEEPS][kMaxBatch] = {};
+  cudaEvent_t ev = nullptr;            // recorded after the stream's latest accumulate launch (the next one waits for it)
+  bool ev_live = false;
+  bool on() const { return cfg.sweeps > 1; }
+  void forget() { n = 0; w = 0; }
+};
+
 // One frame stream's detection-side settings: the context's own (lmot_set_sensors / _rig_merge / _deskew; batched ticks) and each
 // sequence's (lmot_seq_set_*).  Host state read at submission: ticks already submitted carry their own copy in their launch parameters.
 struct StreamCfg {
@@ -334,6 +367,7 @@ struct StreamCfg {
   lmot_detect_params det = {};
   lmot_deskew deskew = deskew_defaults();   // sweep deskew (deskew.cu)
   AreaBlock area = {};                      // detection area (detect_area.cu)
+  AccHist acc;                              // sweep accumulation and its history (accumulate.cu)
   bool merges() const { return rig_merge && n_sensors > 0; }
   bool masked() const { return area.n_rings > 0; }
 };
@@ -408,6 +442,10 @@ struct Ctx {
   unsigned char* d_pred_stage = nullptr;   // host forms: device staging of the outputs, grown to the largest request
   size_t pred_stage_bytes = 0;
   int* h_pred_n = nullptr;             // pinned: the staged row count
+
+  // ---- lmot_accumulate_info / lmot_seq_accumulate_info: what the most recently returned result of the own stream / sequence k used
+  lmot_accum_info acc_info = {};
+  lmot_accum_info seq_acc_info[kMaxBatch] = {};
 
   // ---- lmot_debug_area_masks: the unit masks of the most recent own-stream submission (none: it was not masked)
   const unsigned* area_dbg[kMaxBatch] = {};
@@ -547,5 +585,26 @@ int area_ensure(Ctx* c, Slot* s, int blocks);
 // one launch over the masked units of a submission: unit i's mask from its stream's staged block a, its pose and roi
 struct AreaJob { const AreaBlock* a; unsigned* mask; float pose[12]; float roi; };
 int area_launch(Ctx* c, cudaStream_t st, const AreaJob* jobs, int n_jobs);
+// sweep accumulation (accumulate.cu).  accumulate_pose: lmot_accumulate_pose (mount: row-major 3x4, nullptr: identity)
+void accumulate_pose(const double fold_s[3], const double fold_t[3], const float* mount, float out[12]);
+bool accumulate_valid(const lmot_accumulate& a);
+void accumulate_free(AccHist& h);
+// one accumulating unit of a launch: its cloud (E_t in front), cells, bit planes and counters, its ring, its row of the result block
+// (device view), its clustering ROI, and the step's candidates (ring entries and this unit's poses)
+struct AccJob {
+  float4* elev; uint16_t* cart; unsigned* bits; int* counters;
+  float4* ring; int* ring_n; int* info;
+  float roi; int w, n_sw;
+  int bound;                           // host: bounds |E_t| and every candidate's length (the launch's point blocks)
+  int entry[LMOT_MAX_SWEEPS - 1];
+  float m[LMOT_MAX_SWEEPS - 1][12];
+};
+// the host side of one stream's accumulating step: `units` units of layout `kind` (U[i], pose[i], roi[i], frame-size bound n_upper[i])
+// with the stream's fold th peeked at (ts, v, yaw).  Allocates the ring on first use, starts the history afresh on a new layout, picks
+// the candidates into r (units r's rows from 0) and the jobs, raises fit_upper[i] to bound |E_acc| of unit i, records the step.
+int accumulate_step(Ctx* c, AccHist& h, int kind, int units, Slot* const* U, const lmot_sensor* pose, const float* roi, const int* n_upper,
+                    const TrackerHost& th, double ts, double v, double yaw, Result* r, AccJob* jobs, int* fit_upper);
+// one launch over the jobs of a submission, behind each accumulating stream's previous launch (hists[0 .. nh)); records their events
+int accumulate_launch(Ctx* c, cudaStream_t st, Slot* mark, const AccJob* jobs, int n_jobs, AccHist* const* hists, int nh);
 
 }  // namespace lmot

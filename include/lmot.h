@@ -792,6 +792,83 @@ int lmot_seq_get_detect_area(const lmot_ctx* ctx, int k, int* n_rings, int* ring
 int lmot_detect_area_mask(const lmot_area* area, const lmot_sensor* mount, float roi_m, uint32_t out[LMOT_NUM_GRID * 8]);
 int lmot_debug_area_masks(lmot_ctx* ctx, uint32_t* out, int cap_units, int* n_units);
 
+/* ---- sweep accumulation: cluster and box a frame together with the stream's last sweeps, moved into the current frame ----------------
+ * The detector drops sparse objects where it counts points: componentClustering seeds only cells holding more than one point, and the
+ * rule filter drops clusters under min_cluster_points or t_pt_per_m3.  On 16- and 32-beam sensors a car at 20 m or a pedestrian at 15 m
+ * often stays under those counts.  Accumulation detects on the last K sweeps together, each moved by the ego motion between its stamp
+ * and the current one.  Static objects register; moving objects smear by their speed times max_age_s at most.
+ *
+ * Definition.  A stream (the context's own: lmot_set_accumulate; sequence k: lmot_seq_set_accumulate) with sweeps = K > 1 keeps a
+ * HISTORY per detection unit (a frame without a sensor table, an unmerged rig frame j, or a merge unit): the unit's cloud E_s (the
+ * elevated cloud after deskew, before any detection-area mask; a merge unit's: the merged vehicle-frame cloud) of each of the stream's
+ * last K-1 recorded steps, with that step's stamp ts_s and fold f_s = (x, y, yaw), the fold of the stream's track table after the
+ * step's getOriginPoints (ego8[5..7] of lmot_tracker_get_ego / lmot_seq_tracker_get_ego read after the step).  Step t of a unit:
+ *   1. ground removal, deskew and the rig merge are unchanged: n_elevated, n_ground and the clouds are what they are without it;
+ *   2. the pose of an earlier step s, in double with the host libm, left to right, without contraction:
+ *        c = cos(yaw_t - yaw_s), sn = sin(yaw_t - yaw_s), tx = x_t - (c*x_s - sn*y_s), ty = y_t - (sn*x_s + c*y_s),
+ *        A = [[c, -sn, 0, tx], [sn, c, 0, ty], [0, 0, 1, 0]] (= G_t G_s^-1, G the global -> sensor pose of lmot_params.global_frame);
+ *      D = M^-1 A M with M the unit pose as detection areas define it (a frame without a table and a merge unit: identity; unmerged
+ *      rig frame j: sensor j's pose), M^-1 = [R^T | -R^T t] with
+ *      -R^T t row r = -((R0r*t0 + R1r*t1) + R2r*t2), the pose widened from float.  Both products are 4x4 with the implicit last row
+ *      (0 0 0 1), entry (r, k) = ((X[r][0]*Y[0][k] + X[r][1]*Y[1][k]) + X[r][2]*Y[2][k]) + X[r][3]*Y[3][k]; first P = A M, then
+ *      D = M^-1 P; each entry of D's first three rows is rounded to float once.  lmot_accumulate_pose computes it;
+ *   3. E_acc = E_t | D_1 E_s1 | D_2 E_s2 | ...: earlier steps newest first, each in its own cloud order, each point moved by the rig
+ *      arithmetic of lmot_set_sensors (((d00*x + d01*y) + d02*z) + d03 per row, float, no contraction) with w = 1.  The steps used are
+ *      the longest newest-first prefix of the history whose every entry has 0 < (ts_t - ts_s) / 1e6 <= max_age_s and fits WHOLE,
+ *      together with E_t and every sweep before it, in max_points.  A sweep is never cut; leaving sweeps out is not an error;
+ *   4. the detection area, if any, filters E_acc with the unit's mask exactly as it filters a plain frame; then componentClustering(E_acc)
+ *      and boxFitting with the unit's values.  The tracker, global frame and retirement follow as usual on those boxes;
+ *   5. E_t (not E_acc) joins the history; the oldest entry beyond K-1 leaves.
+ * That is the pipeline without accumulation with this cloud between ground removal and clustering, bit for bit.
+ *
+ * Applies to lmot_frame / lmot_frame_submit / lmot_frame_dev, lmot_batch_submit / lmot_batch_dev / lmot_batch (every unit of the tick,
+ * merged or not) and the FRAMES steps of lmot_seq* / lmot_seq_tick*.  Never to entry points without a stamp, which never touch the
+ * history: the stage entry points, lmot_detect_dev, lmot_batch_detect_dev, lmot_batch_ground_ccl_dev, and lmot_shared_*.  LISTS steps,
+ * lmot_track_step* and lmot_seq_track* advance the fold without recording, so older sweeps still get the motion made during them; SKIP
+ * touches nothing.  lmot_cluster_outputs after an accumulating lmot_frame describes E_acc (intersected with the area).
+ * The history starts empty again on the next submitted step after lmot_tracker_reset, _load or _set_ego (or their lmot_seq_ forms),
+ * LMOT_SEQ_RESTART, lmot_seq_open, any call to lmot_set_accumulate, lmot_set_sensors or lmot_set_rig_merge (or their lmot_seq_ forms),
+ * and, on the context's own stream, after a step whose units differ in number or kind from the previous accumulating step's (for example
+ * an lmot_frame after a 2-sensor lmot_batch tick).  Deskew, detection-area and parameter changes keep it.  It holds coordinates: cells
+ * are computed at use with the step's roi.
+ * Submission.  The setting is host state captured by value at submission; frames in flight keep theirs.  Results depend neither on
+ * pipeline_depth nor on host versus device frames: the accumulate launch of frame t waits for frame t-1's on the device (an event across
+ * slot streams), so the ground kernels of consecutive frames still overlap and only this launch and the clustering behind it are
+ * serialised; one launch covers every accumulating unit of a submission.  An accumulating submission clusters in a launch of its own
+ * instead of the ground kernel's tail.  A submission without an accumulating stream runs exactly the launches, copies and memsets it ran
+ * before accumulation existed.
+ * Errors.  LMOT_ERR_INVALID, setting unchanged: sweeps outside [1, LMOT_MAX_SWEEPS], max_age_s not finite or <= 0, k out of range or
+ * no open set.  LMOT_ERR_STATE, nothing submitted: an accumulating submission in timing mode.
+ * Memory.  On a stream's first accumulating step, with one device synchronisation, all or nothing: per accumulating unit a ring of
+ * sweeps x max_points x 16 B plus one int per entry (64 MB per unit at K = 4 and the default max_points); a larger K or more units later
+ * reallocate it the same way.  The setters with sweeps > 1 pin 128 B per result-ring entry (sequences: per ring tick).  Freed with the
+ * context; a sequence's with the set (lmot_seq_open, lmot_destroy).
+ * lmot_accumulate_info / lmot_seq_accumulate_info: what the most recently RETURNED result of the own stream (lmot_frame*, lmot_batch*) /
+ * of sequence k used, per unit in unit order (n_units = 0 when that result did not accumulate): the earlier sweeps in E_acc, |E_acc|
+ * before the area mask, and each used sweep's stamp and pose D, newest first.  The counts travel in the result block: no extra
+ * synchronisation at collect.
+ * lmot_accumulate_pose(fold_s, fold_t, mount, out): step 2 on the host, no device needed; mount NULL: identity. */
+#define LMOT_MAX_SWEEPS 8
+typedef struct lmot_accumulate {
+  int sweeps;                  /* 1 = off (default) .. LMOT_MAX_SWEEPS: this step's cloud plus up to sweeps-1 earlier ones */
+  double max_age_s;            /* 0.5: an earlier sweep whose stamp is further back than this is not used */
+} lmot_accumulate;
+int lmot_default_accumulate(lmot_accumulate* a);
+int lmot_set_accumulate(lmot_ctx* ctx, const lmot_accumulate* a);     /* NULL: the defaults (off) */
+int lmot_get_accumulate(const lmot_ctx* ctx, lmot_accumulate* a);
+typedef struct lmot_accum_info {
+  int n_units;
+  int sweeps_used[LMOT_MAX_BATCH];                            /* earlier sweeps in E_acc */
+  int n_points[LMOT_MAX_BATCH];                               /* |E_acc| (before the area mask) */
+  double stamp_us[LMOT_MAX_BATCH][LMOT_MAX_SWEEPS - 1];       /* ts_s of each used sweep, newest first */
+  float pose[LMOT_MAX_BATCH][LMOT_MAX_SWEEPS - 1][12];        /* D of each used sweep, row-major 3x4 */
+} lmot_accum_info;
+int lmot_seq_set_accumulate(lmot_ctx* ctx, int k, const lmot_accumulate* a);
+int lmot_seq_get_accumulate(const lmot_ctx* ctx, int k, lmot_accumulate* a);
+int lmot_accumulate_info(lmot_ctx* ctx, lmot_accum_info* out);
+int lmot_seq_accumulate_info(lmot_ctx* ctx, int k, lmot_accum_info* out);
+int lmot_accumulate_pose(const double fold_s[3], const double fold_t[3], const lmot_sensor* mount, float out[12]);
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);
