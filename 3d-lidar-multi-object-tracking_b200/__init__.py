@@ -306,6 +306,40 @@ def accumulate_pose(fold_s, fold_t, mount=None) -> np.ndarray:
     return out.reshape(3, 4)
 
 
+class BoxSearch(C.Structure):
+    """lmot_box_search: each cluster's rectangle by a search over yaw with the closeness criterion (include/lmot.h)."""
+    _fields_ = [("on", C.c_int), ("n_angles", C.c_int)]
+
+
+BOX_SEARCH_MAX_ANGLES = 360             # LMOT_BOX_SEARCH_MAX_ANGLES
+
+
+def default_box_search() -> dict:
+    lib = load_library()
+    b = BoxSearch()
+    lib.lmot_default_box_search(C.byref(b))
+    return {name: getattr(b, name) for name, _ in BoxSearch._fields_}
+
+
+def _box_search(fields: dict) -> BoxSearch:
+    base = default_box_search()
+    unknown = set(fields) - set(base)
+    if unknown:
+        raise KeyError(f"unknown box search fields {sorted(unknown)}")
+    base.update(fields)
+    return BoxSearch(int(base["on"]), int(base["n_angles"]))
+
+
+def box_search_angles(n_angles: int) -> np.ndarray:
+    """lmot_box_search_angles: the (n_angles, 2) float32 table (cos, sin) of theta_a = (pi / 2) * a / n_angles; no device needed."""
+    lib = load_library()
+    out = np.zeros((max(int(n_angles), 1), 2), np.float32)
+    st = lib.lmot_box_search_angles(int(n_angles), out.ctypes.data_as(C.c_void_p))
+    if st != OK:
+        raise LmotError(st, lib.lmot_strerror(st).decode())
+    return out
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -365,6 +399,8 @@ ABI_SYMBOLS = [
     "lmot_debug_area_masks",
     "lmot_default_accumulate", "lmot_set_accumulate", "lmot_get_accumulate", "lmot_accumulate_info", "lmot_accumulate_pose",
     "lmot_seq_set_accumulate", "lmot_seq_get_accumulate", "lmot_seq_accumulate_info",
+    "lmot_default_box_search", "lmot_set_box_search", "lmot_get_box_search", "lmot_seq_set_box_search", "lmot_seq_get_box_search",
+    "lmot_box_search_angles",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
@@ -393,6 +429,7 @@ def load_library() -> C.CDLL:
         lib.lmot_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(Params), C.c_int]
         lib.lmot_destroy.argtypes = [C.c_void_p]
         lib.lmot_accumulate_pose.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.lmot_box_search_angles.argtypes = [C.c_int, C.c_void_p]
         _lib = lib
     return _lib
 
@@ -991,6 +1028,26 @@ class Lmot:
         a = Accumulate()
         self._chk(self.lib.lmot_seq_get_accumulate(self.h, int(k), C.byref(a)))
         return {name: getattr(a, name) for name, _ in Accumulate._fields_}
+
+    # ---- box search (lmot_set_box_search) -----------------------------------------------------------------------------------------
+    def set_box_search(self, **fields):
+        """The context's frames: box search settings with `fields` replaced (on=1 turns it on, n_angles=A; no fields: the defaults, off).
+        Applies from the next submission on; frames in flight keep theirs."""
+        self._chk(self.lib.lmot_set_box_search(self.h, C.byref(_box_search(fields)) if fields else None))
+
+    def get_box_search(self) -> dict:
+        b = BoxSearch()
+        self._chk(self.lib.lmot_get_box_search(self.h, C.byref(b)))
+        return {name: getattr(b, name) for name, _ in BoxSearch._fields_}
+
+    def seq_set_box_search(self, k: int, **fields):
+        """Sequence k's FRAMES steps, arguments as set_box_search."""
+        self._chk(self.lib.lmot_seq_set_box_search(self.h, int(k), C.byref(_box_search(fields)) if fields else None))
+
+    def seq_get_box_search(self, k: int) -> dict:
+        b = BoxSearch()
+        self._chk(self.lib.lmot_seq_get_box_search(self.h, int(k), C.byref(b)))
+        return {name: getattr(b, name) for name, _ in BoxSearch._fields_}
 
     @staticmethod
     def _accum_info(a: AccumInfo) -> list:

@@ -252,7 +252,7 @@ int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tra
   if (!fuse && (rc = cluster_launch(c, s, s->stream, fit_upper, true, mask))) return rc;      // (fused: the ground kernel's last CTA did it)
   if (c->timing) cudaEventRecord(r->ev[2], s->stream);
   const bool gf = with_tracker && c->prm.global_frame;
-  if ((rc = boxfit_launch(c, s, s->stream, fit_upper, with_tracker && !gf, mask))) return rc;      // with_tracker: posts the slot's detection semaphore
+  if ((rc = boxfit_launch(c, s, s->stream, fit_upper, with_tracker && !gf, mask, c->own_cfg.search_angles()))) return rc;   // with_tracker: posts the slot's detection semaphore
   if (gf && (rc = boxes_to_global_launch(c, s, s->stream, s->d_boxes, s->d_counters, ts, v, yaw, true))) return rc;   // ... or this one does
   if (c->timing) cudaEventRecord(r->ev[3], s->stream);
   LMOT_CUDA(c, cudaEventRecord(s->ev_det_done, s->stream));
@@ -505,6 +505,11 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
     ach[nach++] = &q.acc;
   }
   const bool fuse = c->fuse_ccl && !merging && nblk == 0 && nacj == 0;
+  // box search: each unit takes its stream's setting (into the launch parameters, as the detection values)
+  int usearch[kMaxBatch];
+  bool searching = false;
+  for (int d = 0; d < G; ++d)
+    for (int i = U.f0[d]; i < U.f0[d + 1]; ++i) { usearch[i] = g[d].cfg->search_angles(); searching |= usearch[i] > 0; }
   Result* r = bk->res;
   if (c->timing) cudaEventRecord(r->ev[0], st);
   if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, fuse, false, rigged ? rig : nullptr, own_det ? det : nullptr))) return rc;
@@ -513,7 +518,7 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
   if (nacj > 0 && (rc = accumulate_launch(c, st, bk, acj, nacj, ach, nach))) return rc;
   if (!fuse && (rc = ccl_launch_batch(c, U.u, nu, st, area))) return rc;
   if (c->timing) cudaEventRecord(r->ev[2], st);
-  return boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr, area);
+  return boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr, area, searching ? usearch : nullptr);
 }
 
 // the IDs of a result being returned (lmot_track_ids): copied now, the block is reused by later submissions
@@ -901,6 +906,7 @@ void lmot_destroy(lmot_ctx* ctx) {
   accumulate_free(c->own_cfg.acc);
   seq_destroy(c);
   cudaFree(c->d_mt_raw);
+  cudaFree(c->d_bs_tab);
   if (c->ev_pred) cudaEventDestroy(c->ev_pred);
   if (c->ev_pred_in) cudaEventDestroy(c->ev_pred_in);
   cudaFree(c->d_pred_stage);
@@ -1125,7 +1131,7 @@ int lmot_detect_dev(lmot_ctx* ctx, const float* d_points, int n) {
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
-  if (c->own_cfg.masked() && c->timing) return LMOT_ERR_STATE;
+  if ((c->own_cfg.masked() || c->own_cfg.search.on) && c->timing) return LMOT_ERR_STATE;
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, true);
   LMOT_CUDA(c, cudaEventRecord(s->ev_fork, c->stream));
@@ -1137,7 +1143,7 @@ int lmot_frame_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp
   if (!ctx || n < 0 || (n > 0 && !d_points) || (reinterpret_cast<uintptr_t>(d_points) & 15u)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   const bool dsk = c->own_cfg.deskew.on != 0;
-  if ((dsk || c->own_cfg.masked() || c->own_cfg.acc.on()) && c->timing) return LMOT_ERR_STATE;
+  if ((dsk || c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on) && c->timing) return LMOT_ERR_STATE;
   if (dsk && c->own_cfg.deskew.time_field != 3) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
@@ -1158,7 +1164,7 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
-  if ((c->own_cfg.masked() || c->own_cfg.acc.on()) && c->timing) return LMOT_ERR_STATE;
+  if ((c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on) && c->timing) return LMOT_ERR_STATE;
   const bool dsk = c->own_cfg.deskew.on != 0;
   if (dsk) {                           // (validated before anything is submitted: upload_points checks the rest without deskew)
     if (c->timing) return LMOT_ERR_STATE;
@@ -1267,7 +1273,7 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   const bool dsk = with_tracker && q.deskew.on != 0;                // (lmot_batch_detect_dev has no stamp: never deskewed)
   if (dsk && c->timing) return LMOT_ERR_STATE;
   if (dsk && (host ? stride <= q.deskew.time_field : q.deskew.time_field != 3)) return LMOT_ERR_INVALID;
-  if ((q.merges() || q.masked()) && c->timing) return LMOT_ERR_STATE;
+  if ((q.merges() || q.masked() || q.search.on) && c->timing) return LMOT_ERR_STATE;
   if (with_tracker && q.acc.on() && c->timing) return LMOT_ERR_STATE;
   if (host && c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;
   int rc = batch_ensure(c, n_frames);
@@ -2150,6 +2156,53 @@ int lmot_seq_accumulate_info(lmot_ctx* ctx, int k, lmot_accum_info* out) {
 int lmot_accumulate_pose(const double fold_s[3], const double fold_t[3], const lmot_sensor* mount, float out[12]) {
   if (!fold_s || !fold_t || !out || (mount && !sensors_valid(mount, 1))) return LMOT_ERR_INVALID;
   accumulate_pose(fold_s, fold_t, mount ? mount->pose : nullptr, out);
+  return LMOT_OK;
+}
+
+// ---- box search (box_search.cu).  Host state, as deskew: the launch parameters carry each unit's A; the first setter that turns it on
+// uploads the angle tables
+int lmot_default_box_search(lmot_box_search* b) {
+  if (!b) return LMOT_ERR_INVALID;
+  *b = box_search_defaults();
+  return LMOT_OK;
+}
+
+static int box_search_set(Ctx* c, lmot_box_search& dst, const lmot_box_search* b) {
+  const lmot_box_search v = b ? *b : box_search_defaults();
+  if (!box_search_valid(v)) return LMOT_ERR_INVALID;
+  if (v.on) {
+    cudaSetDevice(c->device);
+    const int rc = box_search_ensure(c);
+    if (rc) return rc;
+  }
+  dst = v;
+  return LMOT_OK;
+}
+
+int lmot_set_box_search(lmot_ctx* ctx, const lmot_box_search* b) {
+  return ctx ? box_search_set(&ctx->c, ctx->c.own_cfg.search, b) : LMOT_ERR_INVALID;
+}
+
+int lmot_get_box_search(const lmot_ctx* ctx, lmot_box_search* b) {
+  if (!ctx || !b) return LMOT_ERR_INVALID;
+  *b = ctx->c.own_cfg.search;
+  return LMOT_OK;
+}
+
+int lmot_seq_set_box_search(lmot_ctx* ctx, int k, const lmot_box_search* b) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  return box_search_set(&ctx->c, ctx->c.seq_cfg[k].search, b);
+}
+
+int lmot_seq_get_box_search(const lmot_ctx* ctx, int k, lmot_box_search* b) {
+  if (!ctx || !b || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  *b = ctx->c.seq_cfg[k].search;
+  return LMOT_OK;
+}
+
+int lmot_box_search_angles(int n_angles, float out[][2]) {
+  if (!out || n_angles < 1 || n_angles > LMOT_BOX_SEARCH_MAX_ANGLES) return LMOT_ERR_INVALID;
+  box_search_table(n_angles, out);
   return LMOT_OK;
 }
 

@@ -26,6 +26,7 @@
 #include <vector>
 #include "lmot_internal.cuh"
 #include "ccl_device.cuh"
+#include "boxfit_device.cuh"
 
 namespace lmot {
 
@@ -38,27 +39,7 @@ constexpr int kCols = 1800;        // pixel columns a cluster can span: offsetX-
 constexpr int kColShift = 899 - 450;
 constexpr int kHullCap = 2048;
 
-// Programmatic dependent launch inside a slot's detection stream: scatter behind tile_hist, box_fit behind scatter.  The dependent's
-// CTAs become resident once EVERY CTA of the kernel before it has started (they all trigger at their first instruction) and wait there
-// for it to finish -- its launch latency leaves the frame's critical path.  Deadlock-free next to the ground kernel's own barrier: a
-// waiting CTA only ever waits for a grid that is completely resident and waits for nobody.  (Not used in front of tile_hist: its CTAs
-// would hold SM slots for the duration of the ground kernel, slots the tracker chain needs.)
-__device__ __forceinline__ void fit_pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void fit_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
 // ---------------------------------------------------------------------------------------------- B1
-// One frame of a launch (blockIdx.y): every buffer the four kernels touch for it (the Slot's, see lmot_internal.cuh)
-struct FitFrame {
-  const uint16_t* cart; const int* label_grid; int* counters;
-  uint16_t* pcid; int* table; int* seg_start; int* seg_size;
-  const float4* elev; float4* sorted_pts;
-  float* cl_box; float* cl_marker; uint8_t* cl_ok;
-  float* boxes; float* markers; int* done; int* det_sem;
-  unsigned* hist_ctr;      // atomicInc counter of finished tile_hist CTAs (wraps at the grid size: needs no reset)
-  float sensor_height;     // box_fit_kernel<., true>: this frame's sensor's (lmot_set_sensors); unread otherwise
-};
-struct FitBatch { FitFrame f[kMaxBatch]; };
-
 __device__ __forceinline__ void seg_offsets_body(const FitFrame& F, int max_clusters);
 
 // kArea: a point whose cell is outside its unit's detection-area mask `area` gets cluster 0 -- dilation can label masked cells, and
@@ -257,13 +238,6 @@ scatter_kernel(const __grid_constant__ FitBatch B, int max_clusters) {
 }
 
 // ---------------------------------------------------------------------------------------------- B4
-struct BoxParams {
-  float roi, pic_scale, sensor_height;
-  int ram_points, l_slope_dist, l_num_points, min_points, rule_mode;
-  float t_height_min, t_height_max, t_width_min, t_width_max, t_len_min, t_len_max, t_area_max, t_ratio_min, t_ratio_max,
-      min_len_ratio, t_pt_per_m3;
-};
-
 __device__ __forceinline__ unsigned okey(float f) {   // order-preserving, -0 == +0
   if (f == 0.f) f = 0.f;
   const unsigned u = __float_as_uint(f);
@@ -291,31 +265,6 @@ struct AddD { __device__ double operator()(double a, double b) const { return a 
 struct MinI { __device__ int operator()(int a, int b) const { return a < b ? a : b; } };
 struct MaxI { __device__ int operator()(int a, int b) const { return a > b ? a : b; } };
 
-// ruleBasedFilter, box_fitting.cpp:97-158 (see lmot_rule_filter in lmot.h for the two modes)
-__device__ bool rule_filter(const float pc[4][2], float maxZ, int n, const BoxParams& P, float sensor_height) {
-  if (n < P.min_points) return false;
-  const float x1 = pc[0][0], y1 = pc[0][1], x2 = pc[1][0], y2 = pc[1][1], x3 = pc[2][0], y3 = pc[2][1];
-  const float dist1 = sqrtf((x1 - x2) * (x1 - x2) + (y1 - y2) * (y1 - y2));
-  const float dist2 = sqrtf((x3 - x2) * (x3 - x2) + (y3 - y2) * (y3 - y2));
-  float length, width;
-  if (dist1 > dist2) { length = dist1; width = dist2; } else { length = dist2; width = dist1; }
-  const float height = maxZ + sensor_height;
-  const float area = dist1 * dist2;
-  const float mass = area * height;
-  const float ratio = length / width;
-  if (height > P.t_height_min && height < P.t_height_max) {
-    if (P.rule_mode == LMOT_RULE_GCC13_O2_COMPAT) return true;
-    if (width > P.t_width_min && width < P.t_width_max)
-      if (length > P.t_len_min && length < P.t_len_max)
-        if (area < P.t_area_max)
-          if ((float)n > mass * P.t_pt_per_m3) {
-            if (length > P.min_len_ratio) { if (ratio > P.t_ratio_min && ratio < P.t_ratio_max) return true; }
-            else return true;
-          }
-    return false;   // INTENDED: the reference falls off the end here (undefined behaviour)
-  }
-  return false;
-}
 
 // kRig: sensor_height from the frame's FitFrame (a sensor rig, lmot_set_sensors) instead of P
 template <int NT, bool kRig>
@@ -326,9 +275,6 @@ box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxPa
 #include "box_fit_body.inc"
 }
 
-// sequence ticks with their own detection values (lmot_seq_set_detect_params): frame blockIdx.y's whole BoxParams -- ROI and picScale,
-// L-shape gates, ram_points, min_points, rule mode and window, the sensor's height folded in on the host
-struct BoxFrameParams { BoxParams p[kMaxBatch]; };
 static_assert(sizeof(FitBatch) + sizeof(BoxFrameParams) + 32 <= 4096, "box_fit_frame_kernel: parameter block");
 
 template <int NT>
@@ -502,33 +448,12 @@ static void rig_poses_of(const lmot_sensor* rig, int n, RigPoses& R) {
   for (int i = 0; i < n; ++i) memcpy(R.m[i], rig[i].pose, sizeof(R.m[i]));
 }
 
-static void fit_frame_of(const Slot* s, FitFrame& f, bool post_sem) {
-  f.sensor_height = 0.f;
-  f.cart = s->d_cart; f.label_grid = s->d_label_grid; f.counters = s->d_counters;
-  f.pcid = s->d_pcid; f.table = s->d_table; f.seg_start = s->d_seg_start; f.seg_size = s->d_seg_size;
-  f.elev = s->d_elev; f.sorted_pts = s->d_sorted_pts;
-  f.cl_box = s->d_cl_box; f.cl_marker = s->d_cl_marker; f.cl_ok = s->d_cl_ok;
-  f.boxes = s->d_boxes; f.markers = s->d_markers; f.done = s->d_done; f.det_sem = post_sem ? s->d_det_sem : nullptr;
-  f.hist_ctr = reinterpret_cast<unsigned*>(s->d_done + 1);
-}
 
 // inputs per frame: s->d_elev / CNT_N_ELEV, s->d_cart (from clustering), s->d_label_grid / CNT_NUM_CLUSTER.
 // F > 1: one frame per sensor stream; the four kernels run over the union of the frames' clusters (blockIdx.y = frame).
-// BoxParams of detection values d (the context's, or a frame's own)
-static BoxParams box_params_of(const lmot_detect_params& p) {
-  BoxParams P;
-  P.roi = p.roi_m;
-  { volatile float ps = 900 / p.roi_m; P.pic_scale = ps; }   // float picScale = 900/roiM (box_fitting.cpp:18)
-  P.sensor_height = p.sensor_height; P.ram_points = p.ram_points; P.l_slope_dist = p.l_slope_dist;
-  P.l_num_points = p.l_num_points; P.min_points = p.min_cluster_points; P.rule_mode = p.rule_filter;
-  P.t_height_min = p.t_height_min; P.t_height_max = p.t_height_max; P.t_width_min = p.t_width_min; P.t_width_max = p.t_width_max;
-  P.t_len_min = p.t_len_min; P.t_len_max = p.t_len_max; P.t_area_max = p.t_area_max; P.t_ratio_min = p.t_ratio_min;
-  P.t_ratio_max = p.t_ratio_max; P.min_len_ratio = p.min_len_ratio; P.t_pt_per_m3 = p.t_pt_per_m3;
-  return P;
-}
 
 int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig,
-                        const lmot_detect_params* det, const unsigned* const* area) {
+                        const lmot_detect_params* det, const unsigned* const* area, const int* search) {
   if (F < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   const int K1 = c->prm.max_clusters + 1;
   int tiles = 0;
@@ -560,15 +485,35 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
   const BoxParams P = box_params_of(detect_params_of(c->prm));
   // one CTA per cluster: a frame rarely holds more than a few hundred clusters, F frames share the grid
   const int gx = F == 1 ? c->fit_ctas : (c->fit_ctas / 2 > 8 ? c->fit_ctas / 2 : 8);
-  {
+  // box search (box_search.cu): the searching units leave this launch for box_search_launch behind it; the others keep their kernel and
+  // thread count, their frames (and own values) moved to the front of B in unit order
+  Slot* su[kMaxBatch];
+  lmot_detect_params sd[kMaxBatch];
+  int sa[kMaxBatch], fi[kMaxBatch], ns = 0, nf = F;
+  for (int i = 0; i < F; ++i) fi[i] = i;
+  if (search) {
+    const lmot_detect_params base = detect_params_of(c->prm);
+    nf = 0;
+    for (int i = 0; i < F; ++i) {
+      if (search[i] > 0) {
+        su[ns] = slots[i]; sa[ns] = search[i];
+        sd[ns] = det ? det[i] : base;
+        if (!det && rig) sd[ns].sensor_height = rig[i].sensor_height;
+        ++ns;
+      } else {
+        B.f[nf] = B.f[i]; fi[nf++] = i;
+      }
+    }
+  }
+  if (nf > 0) {
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(gx, F); cfg.blockDim = dim3(F == 1 ? kFitThreadsFrame : kFitThreadsBatch); cfg.dynamicSmemBytes = 0; cfg.stream = st; cfg.attrs = &pdl; cfg.numAttrs = 1;
+    cfg.gridDim = dim3(gx, nf); cfg.blockDim = dim3(F == 1 ? kFitThreadsFrame : kFitThreadsBatch); cfg.dynamicSmemBytes = 0; cfg.stream = st; cfg.attrs = &pdl; cfg.numAttrs = 1;
     const unsigned long long* mt = c->d_mt_raw;
     const int n_raw = c->n_mt_raw, max_boxes = c->prm.max_boxes;
     if (det) {
       BoxFrameParams FP;
       memset(&FP, 0, sizeof(FP));
-      for (int i = 0; i < F; ++i) FP.p[i] = box_params_of(det[i]);
+      for (int i = 0; i < nf; ++i) FP.p[i] = box_params_of(det[fi[i]]);
       if (F == 1) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_frame_kernel<kFitThreadsFrame>, B, FP, mt, n_raw, max_clusters, max_boxes));
       else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_frame_kernel<kFitThreadsBatch>, B, FP, mt, n_raw, max_clusters, max_boxes));
     } else if (rig) {
@@ -578,6 +523,10 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
       if (F == 1) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsFrame, false>, B, P, mt, n_raw, max_clusters, max_boxes));
       else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_kernel<kFitThreadsBatch, false>, B, P, mt, n_raw, max_clusters, max_boxes));
     }
+  }
+  if (ns > 0) {
+    int rc = box_search_launch(c, su, ns, sd, sa, st, post_sem, gx, !c->timing);
+    if (rc) return rc;
   }
   kernel_mark(c, s0, st);
   LMOT_CUDA(c, cudaGetLastError());
@@ -741,11 +690,11 @@ int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const SeqLists& L, int 
   return LMOT_OK;
 }
 
-int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem, const unsigned* area) {
+int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem, const unsigned* area, int search) {
   Slot* sl[1] = {s};
   const int nu[1] = {n_upper};
   const unsigned* am[1] = {area};
-  return boxfit_launch_batch(c, sl, 1, st, nu, post_sem, nullptr, nullptr, area ? am : nullptr);
+  return boxfit_launch_batch(c, sl, 1, st, nu, post_sem, nullptr, nullptr, area ? am : nullptr, search > 0 ? &search : nullptr);
 }
 
 }  // namespace lmot

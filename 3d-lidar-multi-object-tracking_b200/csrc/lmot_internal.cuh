@@ -329,6 +329,9 @@ inline lmot_deskew deskew_defaults() {
   return d;
 }
 
+// lmot_default_box_search
+inline lmot_box_search box_search_defaults() { lmot_box_search b; b.on = 0; b.n_angles = 90; return b; }
+
 // lmot_default_accumulate
 inline lmot_accumulate accumulate_defaults() { lmot_accumulate a; memset(&a, 0, sizeof(a)); a.sweeps = 1; a.max_age_s = 0.5; return a; }
 
@@ -368,8 +371,10 @@ struct StreamCfg {
   lmot_deskew deskew = deskew_defaults();   // sweep deskew (deskew.cu)
   AreaBlock area = {};                      // detection area (detect_area.cu)
   AccHist acc;                              // sweep accumulation and its history (accumulate.cu)
+  lmot_box_search search = box_search_defaults();   // box search (box_search.cu)
   bool merges() const { return rig_merge && n_sensors > 0; }
   bool masked() const { return area.n_rings > 0; }
+  int search_angles() const { return search.on ? search.n_angles : 0; }   // A of the stream's units, 0: boxFitting's fit
 };
 
 struct Ctx {
@@ -390,6 +395,7 @@ struct Ctx {
   unsigned spin_limit = 1u << 24;      // polls after which a device-side wait traps instead of hanging the GPU (LMOT_SPIN_LIMIT, 0 = wait for ever)
   int pts_per_cta = 768;               // target chunk of the fused ground kernel (LMOT_PTS_PER_CTA overrides, tuning only)
   unsigned long long* d_mt_raw = nullptr;  // raw mt19937_64(0) outputs (shared, read only)
+  float2* d_bs_tab = nullptr;          // box search: the angle tables of A = 1 .. LMOT_BOX_SEARCH_MAX_ANGLES, table A at A(A-1)/2 (read only)
 
   // ---- detection slots
   int n_slots = 1;
@@ -525,12 +531,23 @@ int cluster_outputs_launch(Ctx* c, Slot* s, cudaStream_t st);      // makeCluste
 int boxfit_alloc(Ctx* c, Slot* s);
 int boxfit_alloc_shared(Ctx* c);
 void boxfit_free(Slot* s);
-int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem = false, const unsigned* area = nullptr);
+// search: the frame's box search angle count A (0: boxFitting's fit)
+int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem = false, const unsigned* area = nullptr, int search = 0);
 // rig (nullable): sensor i's sensor_height for frame i (box fitting) / sensor i's pose for list i (concatenation)
 // det (nullable): frame i's own detection values, as ground_launch_batch's; rig is then unused
 // area (nullable): as ccl_launch_batch's
+// search (nullable): frame i's box search angle count A, 0: boxFitting's fit (box_search.cu fits the others)
 int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig = nullptr,
-                        const lmot_detect_params* det = nullptr, const unsigned* const* area = nullptr);
+                        const lmot_detect_params* det = nullptr, const unsigned* const* area = nullptr, const int* search = nullptr);
+// box search (box_search.cu): setting validation, the angle table of A (lmot_box_search_angles), and the device tables of every A
+// (Ctx::d_bs_tab, uploaded once by the first setter that turns the search on)
+bool box_search_valid(const lmot_box_search& b);
+void box_search_table(int A, float (*out)[2]);
+int box_search_ensure(Ctx* c);
+// box search over n units (their Slots' box-fitting buffers): unit i with detection values det[i] (its sensor's height folded in) and A[i]
+// angles, gx CTAs per unit, as a programmatic dependent of the kernel before it iff pdl
+int box_search_launch(Ctx* c, Slot* const* units, int n, const lmot_detect_params* det, const int* A, cudaStream_t st, bool post_sem, int gx,
+                      bool pdl);
 int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int n_lists, int cap, float* d_boxes, int* d_counters,
                             const lmot_sensor* rig = nullptr);
 int boxes_concat_launch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, float* d_boxes, int* d_counters, int* d_frame_counts, int* det_sem,

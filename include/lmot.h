@@ -869,6 +869,51 @@ int lmot_accumulate_info(lmot_ctx* ctx, lmot_accum_info* out);
 int lmot_seq_accumulate_info(lmot_ctx* ctx, int k, lmot_accum_info* out);
 int lmot_accumulate_pose(const double fold_s[3], const double fold_t[3], const lmot_sensor* mount, float out[12]);
 
+/* ---- box search: fit each cluster's rectangle by a search over yaw with the closeness criterion -------------------------------------
+ * boxFitting's fit (getBoundingBox: an L-shape from three points, or cv::minAreaRect on an 18 px/m image) depends on point order and on
+ * random draws, and its L-shape is a parallelogram.  A car seen from one corner, the common case, often gets a rotated box.  Box search
+ * fits the rectangle that best explains the points over A yaw angles in [0, pi/2) (Zhang et al., "Efficient L-Shape Fitting for Vehicle
+ * Detection Using Laser Scanners", IV 2017, closeness criterion).
+ *
+ * Definition.  A stream (the context's own: lmot_set_box_search; sequence k: lmot_seq_set_box_search) with on = 1 and n_angles = A
+ * replaces the fit of each cluster of each detection unit (a frame without a sensor table, an unmerged rig frame, or a merge unit; its
+ * cloud is what reaches box fitting: after deskew, the rig merge, accumulation and the detection area).  Clustering, the gather of each
+ * cluster's points, maxZ and the rule filter's first test (n >= min_cluster_points) are unchanged.  For a cluster of n points (x_i, y_i):
+ *   1. angles: theta_a = (M_PI / 2) * a / A in double, left to right, a = 0 .. A-1; c_a = (float)cos(theta_a), s_a = (float)sin(theta_a)
+ *      with the host libm, each rounded to float once.  lmot_box_search_angles returns the table;
+ *   2. projections, float, no contraction: u_i = (x_i*c_a) + (y_i*s_a), w_i = (y_i*c_a) - (x_i*s_a); their minima and maxima;
+ *   3. closeness, float: d1 = min(u_max - u_i, u_i - u_min), d2 = min(w_max - w_i, w_i - w_min), d = max(min(d1, d2), 0.01f); the
+ *      point's score q_i = (uint32)(65536.0f / d) (correctly rounded division, truncated), at most 6,553,600; S_a = sum of q_i in uint64.
+ *      Integer sums and min / max do not depend on order, so neither does the fit;
+ *   4. a* = argmax S_a, ties to the smallest a;
+ *   5. corners in (u, w): P0 = (u_min, w_min), P1 = (u_max, w_min), P2 = (u_max, w_max), P3 = (u_min, w_max), counter-clockwise; in the
+ *      unit frame x = (u*c) - (w*s), y = (u*s) + (w*c), float, no contraction;
+ *   6. ruleBasedFilter (lmot_rule_filter, both modes) on those corners with the unit's values, maxZ and n; an accepted cluster gives the
+ *      usual 8-corner box: bottom z = -(the unit's sensor_height), top z = maxZ.  Boxes are in cluster-id order.
+ * Everything behind box fitting runs as usual: concatenation, rig poses, global frame, tracker and retirement.
+ *
+ * Applies to lmot_frame / _submit / _dev, lmot_detect_dev, lmot_batch* including lmot_batch_detect_dev (every unit, merged or not) and
+ * the FRAMES steps of lmot_seq* / lmot_seq_tick*.  Never to the stage entry points (lmot_box_fit stays the reference's boxFitting),
+ * lmot_batch_ground_ccl_dev, LISTS steps, lmot_track_step*, lmot_seq_track* or lmot_shared_*.
+ * Submission.  The setting is host state captured by value at submission; frames and ticks in flight keep theirs.  lmot_seq_open turns
+ * it off for every sequence; lmot_seq_tracker_reset, _load and LMOT_SEQ_RESTART keep it.  A submission without a searching stream runs
+ * exactly the launches, copies and memsets it ran before box search existed.
+ * Errors.  LMOT_ERR_INVALID, setting unchanged: on not 0 / 1, n_angles outside [1, LMOT_BOX_SEARCH_MAX_ANGLES], k out of range or no
+ * open set.  LMOT_ERR_STATE, nothing submitted: a searching submission in timing mode.
+ * Memory.  The first setter that turns the search on uploads the angle tables of every A (520 KB of device memory, one synchronous copy),
+ * freed with the context. */
+#define LMOT_BOX_SEARCH_MAX_ANGLES 360
+typedef struct lmot_box_search {
+  int on;                      /* 0 (default): boxFitting's fit; 1: the search above */
+  int n_angles;                /* A, 90: angle step (pi/2) / A */
+} lmot_box_search;
+int lmot_default_box_search(lmot_box_search* b);
+int lmot_set_box_search(lmot_ctx* ctx, const lmot_box_search* b);          /* NULL: the defaults (off) */
+int lmot_get_box_search(const lmot_ctx* ctx, lmot_box_search* b);
+int lmot_seq_set_box_search(lmot_ctx* ctx, int k, const lmot_box_search* b);
+int lmot_seq_get_box_search(const lmot_ctx* ctx, int k, lmot_box_search* b);
+int lmot_box_search_angles(int n_angles, float out[][2]);                  /* step 1 on the host, no device needed: out[a] = (c_a, s_a) */
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);
