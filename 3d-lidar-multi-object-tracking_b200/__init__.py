@@ -340,6 +340,42 @@ def box_search_angles(n_angles: int) -> np.ndarray:
     return out
 
 
+class GroundLines(C.Structure):
+    """lmot_ground_lines: slope-following ground removal and box heights from the local ground (include/lmot.h)."""
+    _fields_ = [("on", C.c_int), ("max_slope", C.c_double), ("max_rmse", C.c_double), ("max_step", C.c_double)]
+
+
+def default_ground_lines() -> dict:
+    lib = load_library()
+    g = GroundLines()
+    lib.lmot_default_ground_lines(C.byref(g))
+    return {name: getattr(g, name) for name, _ in GroundLines._fields_}
+
+
+def _ground_lines(fields: dict) -> GroundLines:
+    base = default_ground_lines()
+    unknown = set(fields) - set(base)
+    if unknown:
+        raise KeyError(f"unknown ground lines fields {sorted(unknown)}")
+    base.update(fields)
+    return GroundLines(int(base["on"]), float(base["max_slope"]), float(base["max_rmse"]), float(base["max_step"]))
+
+
+def ground_lines_grid(minz, r_min: float, r_max: float, sensor_height: float, **fields) -> np.ndarray:
+    """lmot_ground_lines_grid: the (80, 120) float32 ground heights of the lines through a (80, 120) float32 min-z grid (1000: empty
+    cell); `fields` replace the default setting's values.  A frame's grid is reproduced with its float32 r_min / r_max / sensor_height
+    widened to double.  No device needed."""
+    lib = load_library()
+    mz = np.ascontiguousarray(np.asarray(minz, np.float32).reshape(80, 120))
+    out = np.zeros((80, 120), np.float32)
+    g = _ground_lines(fields)
+    st = lib.lmot_ground_lines_grid(C.byref(g), mz.ctypes.data_as(C.c_void_p), float(r_min), float(r_max), float(sensor_height),
+                                    out.ctypes.data_as(C.c_void_p))
+    if st != OK:
+        raise LmotError(st, lib.lmot_strerror(st).decode())
+    return out
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -401,6 +437,8 @@ ABI_SYMBOLS = [
     "lmot_seq_set_accumulate", "lmot_seq_get_accumulate", "lmot_seq_accumulate_info",
     "lmot_default_box_search", "lmot_set_box_search", "lmot_get_box_search", "lmot_seq_set_box_search", "lmot_seq_get_box_search",
     "lmot_box_search_angles",
+    "lmot_default_ground_lines", "lmot_set_ground_lines", "lmot_get_ground_lines", "lmot_seq_set_ground_lines", "lmot_seq_get_ground_lines",
+    "lmot_ground_lines_grid", "lmot_debug_ground_lines",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
@@ -430,6 +468,7 @@ def load_library() -> C.CDLL:
         lib.lmot_destroy.argtypes = [C.c_void_p]
         lib.lmot_accumulate_pose.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.lmot_box_search_angles.argtypes = [C.c_int, C.c_void_p]
+        lib.lmot_ground_lines_grid.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_void_p]
         _lib = lib
     return _lib
 
@@ -1048,6 +1087,35 @@ class Lmot:
         b = BoxSearch()
         self._chk(self.lib.lmot_seq_get_box_search(self.h, int(k), C.byref(b)))
         return {name: getattr(b, name) for name, _ in BoxSearch._fields_}
+
+    # ---- ground lines (lmot_set_ground_lines) ------------------------------------------------------------------------------------
+    def set_ground_lines(self, **fields):
+        """The context's frames: ground lines settings with `fields` replaced (on=1 turns them on; no fields: the defaults, off).
+        Applies from the next submission on; frames in flight keep theirs."""
+        self._chk(self.lib.lmot_set_ground_lines(self.h, C.byref(_ground_lines(fields)) if fields else None))
+
+    def get_ground_lines(self) -> dict:
+        g = GroundLines()
+        self._chk(self.lib.lmot_get_ground_lines(self.h, C.byref(g)))
+        return {name: getattr(g, name) for name, _ in GroundLines._fields_}
+
+    def seq_set_ground_lines(self, k: int, **fields):
+        """Sequence k's FRAMES steps, arguments as set_ground_lines."""
+        self._chk(self.lib.lmot_seq_set_ground_lines(self.h, int(k), C.byref(_ground_lines(fields)) if fields else None))
+
+    def seq_get_ground_lines(self, k: int) -> dict:
+        g = GroundLines()
+        self._chk(self.lib.lmot_seq_get_ground_lines(self.h, int(k), C.byref(g)))
+        return {name: getattr(g, name) for name, _ in GroundLines._fields_}
+
+    def debug_ground_lines(self) -> np.ndarray:
+        """lmot_debug_ground_lines: (n_frames, 80, 120) float32 ground grids of the most recent own-stream submission (0: lines off)"""
+        out = np.zeros((MAX_BATCH, 80, 120), np.float32)
+        n = C.c_int(0)
+        fn = self.lib.lmot_debug_ground_lines
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
+        self._chk(fn(self.h, out.ctypes.data, MAX_BATCH, C.byref(n)))
+        return out[: n.value]
 
     @staticmethod
     def _accum_info(a: AccumInfo) -> list:

@@ -16,6 +16,7 @@
 #include <vector>
 #include "lmot_internal.cuh"
 #include "exact_math.cuh"
+#include "ground_lines.cuh"
 
 using namespace lmot;
 
@@ -214,6 +215,12 @@ int submit_tracker(Ctx* c, Slot* s, Result* r, const float* d_boxes, const int* 
   return LMOT_OK;
 }
 
+// ground lines: the slot's ground grid, allocated on its first frame with lines on
+int lines_ensure(Ctx* c, Slot* s) {
+  if (!s->d_gz) LMOT_CUDA(c, cudaMalloc(&s->d_gz, kPolarCells * sizeof(float)));
+  return LMOT_OK;
+}
+
 // the asynchronous frame: detection on the slot stream, tracker on the tracker stream
 int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tracker, double ts, double v, double yaw) {
   int rc;
@@ -244,15 +251,26 @@ int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tra
   c->n_area_dbg = masked ? 1 : 0;
   c->area_dbg[0] = mask;
   const bool fuse = c->fuse_ccl && !masked && !acc;
+  // ground lines: the ground kernel's lines variant writes the slot's ground grid, box fitting measures each cluster from it
+  const lmot_ground_lines* gl = c->own_cfg.lines_on();
+  if (gl && (rc = lines_ensure(c, s))) return rc;
+  c->n_gz_dbg = gl ? 1 : 0;
+  c->gz_dbg[0] = s->d_gz;
   if (c->timing) cudaEventRecord(r->ev[0], s->stream);
-  if ((rc = ground_launch(c, s, s->stream, d_pts, n, true, false, fuse))) return rc;
+  if (gl) {
+    Slot* sl[1] = {s};
+    const float4* pp[1] = {d_pts};
+    const int nn[1] = {n};
+    const GroundLinesJob lj{gl, s->d_gz};
+    if ((rc = ground_launch_batch(c, sl, 1, pp, nn, s->stream, true, false, fuse, false, nullptr, nullptr, &lj))) return rc;
+  } else if ((rc = ground_launch(c, s, s->stream, d_pts, n, true, false, fuse))) return rc;
   if (c->timing) cudaEventRecord(r->ev[1], s->stream);
   AccHist* hp = &h;
   if (acc && (rc = accumulate_launch(c, s->stream, s, &aj, 1, &hp, 1))) return rc;     // E_t into the ring, the earlier sweeps behind it
   if (!fuse && (rc = cluster_launch(c, s, s->stream, fit_upper, true, mask))) return rc;      // (fused: the ground kernel's last CTA did it)
   if (c->timing) cudaEventRecord(r->ev[2], s->stream);
   const bool gf = with_tracker && c->prm.global_frame;
-  if ((rc = boxfit_launch(c, s, s->stream, fit_upper, with_tracker && !gf, mask, c->own_cfg.search_angles()))) return rc;   // with_tracker: posts the slot's detection semaphore
+  if ((rc = boxfit_launch(c, s, s->stream, fit_upper, with_tracker && !gf, mask, c->own_cfg.search_angles(), gl ? s->d_gz : nullptr))) return rc;   // with_tracker: posts the slot's detection semaphore
   if (gf && (rc = boxes_to_global_launch(c, s, s->stream, s->d_boxes, s->d_counters, ts, v, yaw, true))) return rc;   // ... or this one does
   if (c->timing) cudaEventRecord(r->ev[3], s->stream);
   LMOT_CUDA(c, cudaEventRecord(s->ev_det_done, s->stream));
@@ -505,6 +523,20 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
     ach[nach++] = &q.acc;
   }
   const bool fuse = c->fuse_ccl && !merging && nblk == 0 && nacj == 0;
+  // ground lines: a frame whose stream has them on gets its slot's ground grid; its unit (an unmerged frame) measures boxes from it
+  GroundLinesJob lj[kMaxBatch];
+  const float* ugz[kMaxBatch] = {};
+  bool lining = false;
+  for (int d = 0, i0 = 0; d < G; i0 += g[d].nf, ++d) {
+    const lmot_ground_lines* gl = g[d].cfg->lines_on();
+    for (int i = i0; i < i0 + g[d].nf; ++i) {
+      if (gl && (rc = lines_ensure(c, sl[i]))) return rc;
+      lj[i] = GroundLinesJob{gl, sl[i]->d_gz};
+    }
+    if (gl && !g[d].cfg->merges())
+      for (int i = U.f0[d]; i < U.f0[d + 1]; ++i) ugz[i] = U.u[i]->d_gz;
+    lining |= gl != nullptr;
+  }
   // box search: each unit takes its stream's setting (into the launch parameters, as the detection values)
   int usearch[kMaxBatch];
   bool searching = false;
@@ -512,13 +544,15 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
     for (int i = U.f0[d]; i < U.f0[d + 1]; ++i) { usearch[i] = g[d].cfg->search_angles(); searching |= usearch[i] > 0; }
   Result* r = bk->res;
   if (c->timing) cudaEventRecord(r->ev[0], st);
-  if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, fuse, false, rigged ? rig : nullptr, own_det ? det : nullptr))) return rc;
+  if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, fuse, false, rigged ? rig : nullptr, own_det ? det : nullptr,
+                                lining ? lj : nullptr))) return rc;
   if (c->timing) cudaEventRecord(r->ev[1], st);
   if (nm > 0 && (rc = rig_merge_launch(c, st, src, mpose, mn, nm, ms0, mu, mfc, mroi))) return rc;
   if (nacj > 0 && (rc = accumulate_launch(c, st, bk, acj, nacj, ach, nach))) return rc;
   if (!fuse && (rc = ccl_launch_batch(c, U.u, nu, st, area))) return rc;
   if (c->timing) cudaEventRecord(r->ev[2], st);
-  return boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr, area, searching ? usearch : nullptr);
+  return boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr, area, searching ? usearch : nullptr,
+                             lining ? ugz : nullptr);
 }
 
 // the IDs of a result being returned (lmot_track_ids): copied now, the block is reused by later submissions
@@ -775,7 +809,7 @@ int slot_create(Ctx* c, Slot* s, int index) {
 
 void slot_destroy(Slot* s) {
   ground_free(s); cluster_free(s); boxfit_free(s);
-  cudaFree(s->d_deskew); cudaFree(s->d_stage_wide); cudaFree(s->d_area_mask); cudaFree(s->d_area);
+  cudaFree(s->d_deskew); cudaFree(s->d_stage_wide); cudaFree(s->d_area_mask); cudaFree(s->d_area); cudaFree(s->d_gz);
   if (s->ev_fork) cudaEventDestroy(s->ev_fork);
   if (s->ev_det_done) cudaEventDestroy(s->ev_det_done);
   if (s->ev_trk_done) cudaEventDestroy(s->ev_trk_done);
@@ -1131,7 +1165,7 @@ int lmot_detect_dev(lmot_ctx* ctx, const float* d_points, int n) {
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
-  if ((c->own_cfg.masked() || c->own_cfg.search.on) && c->timing) return LMOT_ERR_STATE;
+  if ((c->own_cfg.masked() || c->own_cfg.search.on || c->own_cfg.lines.on) && c->timing) return LMOT_ERR_STATE;
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, true);
   LMOT_CUDA(c, cudaEventRecord(s->ev_fork, c->stream));
@@ -1143,7 +1177,7 @@ int lmot_frame_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp
   if (!ctx || n < 0 || (n > 0 && !d_points) || (reinterpret_cast<uintptr_t>(d_points) & 15u)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   const bool dsk = c->own_cfg.deskew.on != 0;
-  if ((dsk || c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on) && c->timing) return LMOT_ERR_STATE;
+  if ((dsk || c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on) && c->timing) return LMOT_ERR_STATE;
   if (dsk && c->own_cfg.deskew.time_field != 3) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
@@ -1164,7 +1198,7 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
-  if ((c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on) && c->timing) return LMOT_ERR_STATE;
+  if ((c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on) && c->timing) return LMOT_ERR_STATE;
   const bool dsk = c->own_cfg.deskew.on != 0;
   if (dsk) {                           // (validated before anything is submitted: upload_points checks the rest without deskew)
     if (c->timing) return LMOT_ERR_STATE;
@@ -1273,7 +1307,7 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   const bool dsk = with_tracker && q.deskew.on != 0;                // (lmot_batch_detect_dev has no stamp: never deskewed)
   if (dsk && c->timing) return LMOT_ERR_STATE;
   if (dsk && (host ? stride <= q.deskew.time_field : q.deskew.time_field != 3)) return LMOT_ERR_INVALID;
-  if ((q.merges() || q.masked() || q.search.on) && c->timing) return LMOT_ERR_STATE;
+  if ((q.merges() || q.masked() || q.search.on || q.lines.on) && c->timing) return LMOT_ERR_STATE;
   if (with_tracker && q.acc.on() && c->timing) return LMOT_ERR_STATE;
   if (host && c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;
   int rc = batch_ensure(c, n_frames);
@@ -1303,6 +1337,8 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   if ((rc = detect_front(c, b, &grp, 1, stride, host, r->h_deskew, r->h_area, false, U))) return rc;
   c->n_area_dbg = q.masked() ? U.f0[1] : 0;
   for (int i = 0; i < c->n_area_dbg; ++i) c->area_dbg[i] = U.u[i]->d_area_mask;
+  c->n_gz_dbg = q.lines.on ? n_frames : 0;
+  for (int i = 0; i < c->n_gz_dbg; ++i) c->gz_dbg[i] = c->bslots[b * c->batch_frames + i].d_gz;
   const bool gf = with_tracker && c->prm.global_frame;
   if ((rc = boxes_concat_launch(c, U.u, U.f0[1], st, k->d_boxes, k->d_counters, U.fc[0], (with_tracker && !gf) ? k->d_det_sem : nullptr,
                                 U.rig_on[0] ? U.rig : nullptr))) return rc;
@@ -2203,6 +2239,70 @@ int lmot_seq_get_box_search(const lmot_ctx* ctx, int k, lmot_box_search* b) {
 int lmot_box_search_angles(int n_angles, float out[][2]) {
   if (!out || n_angles < 1 || n_angles > LMOT_BOX_SEARCH_MAX_ANGLES) return LMOT_ERR_INVALID;
   box_search_table(n_angles, out);
+  return LMOT_OK;
+}
+
+// ---- ground lines (ground_lines.cuh).  Host state, as box search: the launch parameters carry each frame's values
+int lmot_default_ground_lines(lmot_ground_lines* g) {
+  if (!g) return LMOT_ERR_INVALID;
+  *g = ground_lines_defaults();
+  return LMOT_OK;
+}
+
+static bool ground_lines_valid(const lmot_ground_lines& g) {
+  return (g.on == 0 || g.on == 1) && std::isfinite(g.max_slope) && std::isfinite(g.max_rmse) && std::isfinite(g.max_step) &&
+         g.max_slope > 0 && g.max_rmse > 0 && g.max_step > 0;
+}
+
+static int ground_lines_set(lmot_ground_lines& dst, const lmot_ground_lines* g) {
+  const lmot_ground_lines v = g ? *g : ground_lines_defaults();
+  if (!ground_lines_valid(v)) return LMOT_ERR_INVALID;
+  dst = v;
+  return LMOT_OK;
+}
+
+int lmot_set_ground_lines(lmot_ctx* ctx, const lmot_ground_lines* g) {
+  return ctx ? ground_lines_set(ctx->c.own_cfg.lines, g) : LMOT_ERR_INVALID;
+}
+
+int lmot_get_ground_lines(const lmot_ctx* ctx, lmot_ground_lines* g) {
+  if (!ctx || !g) return LMOT_ERR_INVALID;
+  *g = ctx->c.own_cfg.lines;
+  return LMOT_OK;
+}
+
+int lmot_seq_set_ground_lines(lmot_ctx* ctx, int k, const lmot_ground_lines* g) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  return ground_lines_set(ctx->c.seq_cfg[k].lines, g);
+}
+
+int lmot_seq_get_ground_lines(const lmot_ctx* ctx, int k, lmot_ground_lines* g) {
+  if (!ctx || !g || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  *g = ctx->c.seq_cfg[k].lines;
+  return LMOT_OK;
+}
+
+int lmot_ground_lines_grid(const lmot_ground_lines* g, const float minz[LMOT_NUM_CHANNEL * LMOT_NUM_BIN], double r_min, double r_max,
+                           double sensor_height, float gz[LMOT_NUM_CHANNEL * LMOT_NUM_BIN]) {
+  if (!g || !minz || !gz || !ground_lines_valid(*g) || !std::isfinite(r_min) || !std::isfinite(r_max) || !std::isfinite(sensor_height) ||
+      !(r_max > r_min))
+    return LMOT_ERR_INVALID;
+  struct Src { const float* z; float operator()(int b) const { return z[b]; } };
+  struct Dst { float* o; void operator()(int b, float v) const { o[b] = v; } };
+  for (int ch = 0; ch < kNumChannel; ++ch)
+    ground_lines_channel(Src{minz + ch * kNumBin}, Dst{gz + ch * kNumBin}, r_min, r_max, sensor_height, g->max_slope, g->max_rmse, g->max_step);
+  return LMOT_OK;
+}
+
+int lmot_debug_ground_lines(lmot_ctx* ctx, float* gz, int cap_units, int* n_units) {
+  if (!ctx || cap_units < 0 || (cap_units > 0 && !gz)) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  int rc = lmot_sync(ctx);
+  if (rc) return rc;
+  if (n_units) *n_units = c->n_gz_dbg;
+  const int n = c->n_gz_dbg < cap_units ? c->n_gz_dbg : cap_units;
+  for (int i = 0; i < n; ++i)
+    LMOT_CUDA(c, cudaMemcpy(gz + (size_t)i * kPolarCells, c->gz_dbg[i], kPolarCells * sizeof(float), cudaMemcpyDeviceToHost));
   return LMOT_OK;
 }
 

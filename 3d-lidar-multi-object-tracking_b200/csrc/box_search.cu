@@ -38,9 +38,10 @@ __device__ __forceinline__ float2 search_pt(bool smem, const float2* s_xy, const
   return make_float2(q.x, q.y);
 }
 
-__global__ void __launch_bounds__(kSearchThreads)
-box_search_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxFrameParams PF, const __grid_constant__ SearchFrames S,
-                  int max_clusters, int max_boxes) {
+// kLines: each cluster's sensor_height from its unit's ground grid (ground lines, LF)
+template <bool kLines>
+__device__ __forceinline__ void box_search_body(const FitBatch& B, const BoxFrameParams& PF, const SearchFrames& S, const LinesFit* LF,
+                                                int max_clusters, int max_boxes) {
   fit_pdl_trigger();
   fit_pdl_wait();                          // the kernel before it (scatter_kernel, or box fitting of the launch's other units) is complete
   const FitFrame& F = B.f[blockIdx.y];
@@ -81,6 +82,8 @@ box_search_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ Bo
     __syncthreads();
     maxZ = s_maxz[0];
     for (int w = 1; w < kSearchWarps; ++w) maxZ = fmaxf(maxZ, s_maxz[w]);
+    float lsh = 0.f;                                                   // ground lines: the cluster's local ground
+    if (kLines) lsh = lines_sensor_height(seg, n, *LF, P.sensor_height, s_key);
 
     // ---- this warp's angles: extremes of u and w, then the closeness sums; best key (S_a << 9) | (511 - a) with its extremes
     unsigned long long best = 0ull;
@@ -145,12 +148,12 @@ box_search_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ Bo
       const float U[4] = {u0, u1, u1, u0}, W[4] = {w0, w0, w1, w1};
       float pc[4][2];
       for (int q = 0; q < 4; ++q) { pc[q][0] = U[q] * c - W[q] * s; pc[q][1] = U[q] * s + W[q] * c; }
-      const bool ok = rule_filter(pc, maxZ, n, P, P.sensor_height);
+      const bool ok = rule_filter(pc, maxZ, n, P, kLines ? lsh : P.sensor_height);
       cl_ok[k] = ok ? 1 : 0;
       if (ok) {
         float* b = cl_box + (size_t)k * 24;
         for (int h = 0; h < 2; ++h)
-          for (int q = 0; q < 4; ++q) { b[(h * 4 + q) * 3] = pc[q][0]; b[(h * 4 + q) * 3 + 1] = pc[q][1]; b[(h * 4 + q) * 3 + 2] = h == 0 ? -P.sensor_height : maxZ; }
+          for (int q = 0; q < 4; ++q) { b[(h * 4 + q) * 3] = pc[q][0]; b[(h * 4 + q) * 3 + 1] = pc[q][1]; b[(h * 4 + q) * 3 + 2] = h == 0 ? -(kLines ? lsh : P.sensor_height) : maxZ; }
       }
     }
     __syncthreads();                       // (s_xy, s_key and s_maxz are the next cluster's)
@@ -194,6 +197,20 @@ box_search_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ Bo
   }
 }
 
+__global__ void __launch_bounds__(kSearchThreads)
+box_search_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxFrameParams PF, const __grid_constant__ SearchFrames S,
+                  int max_clusters, int max_boxes) {
+  box_search_body<false>(B, PF, S, nullptr, max_clusters, max_boxes);
+}
+
+static_assert(sizeof(FitBatch) + sizeof(BoxFrameParams) + sizeof(SearchFrames) + sizeof(LinesFit) + 16 <= 4096,
+              "box_search_lines_kernel: parameter block");
+__global__ void __launch_bounds__(kSearchThreads)
+box_search_lines_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxFrameParams PF, const __grid_constant__ SearchFrames S,
+                        const __grid_constant__ LinesFit LG, int max_clusters, int max_boxes) {
+  box_search_body<true>(B, PF, S, &LG, max_clusters, max_boxes);
+}
+
 }  // namespace
 
 bool box_search_valid(const lmot_box_search& b) {
@@ -225,16 +242,19 @@ int box_search_ensure(Ctx* c) {
 }
 
 int box_search_launch(Ctx* c, Slot* const* units, int n, const lmot_detect_params* det, const int* A, cudaStream_t st, bool post_sem, int gx,
-                      bool pdl) {
+                      bool pdl, const float* const* lines) {
   if (n < 1 || n > kMaxBatch || !c->d_bs_tab) return LMOT_ERR_STATE;
   FitBatch B;
   BoxFrameParams FP;
   SearchFrames S;
+  LinesFit LG;
   memset(&FP, 0, sizeof(FP));
   memset(&S, 0, sizeof(S));
+  memset(&LG, 0, sizeof(LG));
   for (int i = 0; i < n; ++i) {
     fit_frame_of(units[i], B.f[i], post_sem);
     FP.p[i] = box_params_of(det[i]);
+    if (lines) lines_fit_of(det[i], lines[i], LG, i);
     S.tab[i] = c->d_bs_tab + (size_t)A[i] * (A[i] - 1) / 2;
     S.A[i] = A[i];
   }
@@ -244,7 +264,8 @@ int box_search_launch(Ctx* c, Slot* const* units, int n, const lmot_detect_param
   at.val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(gx, n); cfg.blockDim = dim3(kSearchThreads); cfg.dynamicSmemBytes = 0; cfg.stream = st; cfg.attrs = &at; cfg.numAttrs = 1;
-  LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_search_kernel, B, FP, S, c->prm.max_clusters, c->prm.max_boxes));
+  if (lines) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_search_lines_kernel, B, FP, S, LG, c->prm.max_clusters, c->prm.max_boxes));
+  else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_search_kernel, B, FP, S, c->prm.max_clusters, c->prm.max_boxes));
   return LMOT_OK;
 }
 

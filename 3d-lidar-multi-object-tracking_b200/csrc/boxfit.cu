@@ -271,7 +271,9 @@ template <int NT, bool kRig>
 __global__ void __launch_bounds__(NT, 1024 / NT)     // <= 64 registers: 1,024 threads of box fitting per SM
 box_fit_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxParams P,
                const unsigned long long* __restrict__ mt_raw, int n_raw, int max_clusters, int max_boxes) {
-  // box_fit_body.inc reads: B, P, NT, kRig, mt_raw, n_raw, max_clusters, max_boxes
+  constexpr bool kLines = false;
+  const LinesFit* LF = nullptr;
+  // box_fit_body.inc reads: B, P, NT, kRig, kLines, LF, mt_raw, n_raw, max_clusters, max_boxes
 #include "box_fit_body.inc"
 }
 
@@ -282,8 +284,26 @@ __global__ void __launch_bounds__(NT, 1024 / NT)
 box_fit_frame_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxFrameParams PF,
                      const unsigned long long* __restrict__ mt_raw, int n_raw, int max_clusters, int max_boxes) {
   constexpr bool kRig = false;                 // (the sensor's height is folded into the frame's entry)
+  constexpr bool kLines = false;
+  const LinesFit* LF = nullptr;
   const BoxParams& P = PF.p[blockIdx.y];
-  // box_fit_body.inc reads: B, P, NT, kRig, mt_raw, n_raw, max_clusters, max_boxes
+  // box_fit_body.inc reads: B, P, NT, kRig, kLines, LF, mt_raw, n_raw, max_clusters, max_boxes
+#include "box_fit_body.inc"
+}
+
+// ground lines (lmot_set_ground_lines): box_fit_frame_kernel with each cluster's sensor_height from its unit's ground grid (a unit without
+// one: its entry's, as box_fit_frame_kernel)
+static_assert(sizeof(FitBatch) + sizeof(BoxFrameParams) + sizeof(LinesFit) + 32 <= 4096, "box_fit_lines_kernel: parameter block");
+
+template <int NT>
+__global__ void __launch_bounds__(NT, 1024 / NT)
+box_fit_lines_kernel(const __grid_constant__ FitBatch B, const __grid_constant__ BoxFrameParams PF, const __grid_constant__ LinesFit LG,
+                     const unsigned long long* __restrict__ mt_raw, int n_raw, int max_clusters, int max_boxes) {
+  constexpr bool kRig = false;
+  constexpr bool kLines = true;
+  const LinesFit* LF = &LG;
+  const BoxParams& P = PF.p[blockIdx.y];
+  // box_fit_body.inc reads: B, P, NT, kRig, kLines, LF, mt_raw, n_raw, max_clusters, max_boxes
 #include "box_fit_body.inc"
 }
 
@@ -453,7 +473,7 @@ static void rig_poses_of(const lmot_sensor* rig, int n, RigPoses& R) {
 // F > 1: one frame per sensor stream; the four kernels run over the union of the frames' clusters (blockIdx.y = frame).
 
 int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig,
-                        const lmot_detect_params* det, const unsigned* const* area, const int* search) {
+                        const lmot_detect_params* det, const unsigned* const* area, const int* search, const float* const* lines) {
   if (F < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   const int K1 = c->prm.max_clusters + 1;
   int tiles = 0;
@@ -487,16 +507,18 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
   const int gx = F == 1 ? c->fit_ctas : (c->fit_ctas / 2 > 8 ? c->fit_ctas / 2 : 8);
   // box search (box_search.cu): the searching units leave this launch for box_search_launch behind it; the others keep their kernel and
   // thread count, their frames (and own values) moved to the front of B in unit order
+  // ground lines: every unit of the launch runs the per-unit variants, a unit with a grid measures its clusters from it
   Slot* su[kMaxBatch];
   lmot_detect_params sd[kMaxBatch];
   int sa[kMaxBatch], fi[kMaxBatch], ns = 0, nf = F;
+  const float* sg[kMaxBatch];
   for (int i = 0; i < F; ++i) fi[i] = i;
+  const lmot_detect_params base = detect_params_of(c->prm);
   if (search) {
-    const lmot_detect_params base = detect_params_of(c->prm);
     nf = 0;
     for (int i = 0; i < F; ++i) {
       if (search[i] > 0) {
-        su[ns] = slots[i]; sa[ns] = search[i];
+        su[ns] = slots[i]; sa[ns] = search[i]; sg[ns] = lines ? lines[i] : nullptr;
         sd[ns] = det ? det[i] : base;
         if (!det && rig) sd[ns].sensor_height = rig[i].sensor_height;
         ++ns;
@@ -510,7 +532,20 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
     cfg.gridDim = dim3(gx, nf); cfg.blockDim = dim3(F == 1 ? kFitThreadsFrame : kFitThreadsBatch); cfg.dynamicSmemBytes = 0; cfg.stream = st; cfg.attrs = &pdl; cfg.numAttrs = 1;
     const unsigned long long* mt = c->d_mt_raw;
     const int n_raw = c->n_mt_raw, max_boxes = c->prm.max_boxes;
-    if (det) {
+    if (lines) {
+      BoxFrameParams FP;
+      LinesFit LG;
+      memset(&FP, 0, sizeof(FP));
+      memset(&LG, 0, sizeof(LG));
+      for (int i = 0; i < nf; ++i) {
+        lmot_detect_params d = det ? det[fi[i]] : base;
+        if (!det && rig) d.sensor_height = rig[fi[i]].sensor_height;
+        FP.p[i] = box_params_of(d);
+        lines_fit_of(d, lines[fi[i]], LG, i);
+      }
+      if (F == 1) LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_lines_kernel<kFitThreadsFrame>, B, FP, LG, mt, n_raw, max_clusters, max_boxes));
+      else LMOT_CUDA(c, cudaLaunchKernelEx(&cfg, box_fit_lines_kernel<kFitThreadsBatch>, B, FP, LG, mt, n_raw, max_clusters, max_boxes));
+    } else if (det) {
       BoxFrameParams FP;
       memset(&FP, 0, sizeof(FP));
       for (int i = 0; i < nf; ++i) FP.p[i] = box_params_of(det[fi[i]]);
@@ -525,7 +560,7 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
     }
   }
   if (ns > 0) {
-    int rc = box_search_launch(c, su, ns, sd, sa, st, post_sem, gx, !c->timing);
+    int rc = box_search_launch(c, su, ns, sd, sa, st, post_sem, gx, !c->timing, lines ? sg : nullptr);
     if (rc) return rc;
   }
   kernel_mark(c, s0, st);
@@ -690,11 +725,12 @@ int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const SeqLists& L, int 
   return LMOT_OK;
 }
 
-int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem, const unsigned* area, int search) {
+int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem, const unsigned* area, int search, const float* lines) {
   Slot* sl[1] = {s};
   const int nu[1] = {n_upper};
   const unsigned* am[1] = {area};
-  return boxfit_launch_batch(c, sl, 1, st, nu, post_sem, nullptr, nullptr, area ? am : nullptr, search > 0 ? &search : nullptr);
+  return boxfit_launch_batch(c, sl, 1, st, nu, post_sem, nullptr, nullptr, area ? am : nullptr, search > 0 ? &search : nullptr,
+                             lines ? &lines : nullptr);
 }
 
 }  // namespace lmot

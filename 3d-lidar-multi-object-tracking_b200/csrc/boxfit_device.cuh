@@ -3,6 +3,7 @@
 // include it; everything here has internal linkage.
 #pragma once
 #include "lmot_internal.cuh"
+#include "polar_cell.cuh"
 
 namespace lmot {
 
@@ -62,6 +63,39 @@ __device__ bool rule_filter(const float pc[4][2], float maxZ, int n, const BoxPa
   return false;
 }
 
+// ground lines (lmot_set_ground_lines): unit blockIdx.y's ground grid (nullptr: flat, its BoxParams' sensor_height) and the range window of
+// its polar cells
+struct LinesFit { const float* gz[kMaxBatch]; float r_min[kMaxBatch], r_max[kMaxBatch], r_span[kMaxBatch]; };
+
+// the sensor_height a cluster's box takes with ground lines: -gz of the polar cell of its lowest point (min z, ties to the first in cloud
+// order), or the flat `sh` where that point is outside the window or the unit has no grid.  Every thread of the CTA calls it and gets the
+// value; s_buf: one word per warp
+__device__ __forceinline__ float lines_sensor_height(const float4* __restrict__ seg, int n, const LinesFit& L, float sh, unsigned long long* s_buf) {
+  const float* __restrict__ gz = L.gz[blockIdx.y];
+  if (!gz) return sh;
+  unsigned long long key = ~0ull;
+  for (int j = threadIdx.x; j < n; j += blockDim.x) {
+    float z = __ldg(&seg[j]).z;
+    if (z == 0.f) z = 0.f;                               // -0 == +0
+    const unsigned u = __float_as_uint(z);
+    const unsigned long long k = ((unsigned long long)((u & 0x80000000u) ? ~u : (u | 0x80000000u)) << 32) | (unsigned)j;
+    key = k < key ? k : key;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { const unsigned long long v = __shfl_xor_sync(0xFFFFFFFFu, key, o); key = v < key ? v : key; }
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) s_buf[threadIdx.x >> 5] = key;
+  __syncthreads();
+  for (int w = 1; w < (int)(blockDim.x >> 5); ++w) { const unsigned long long v = s_buf[w]; key = v < key ? v : key; }
+  key = s_buf[0] < key ? s_buf[0] : key;
+  __syncthreads();                                       // (s_buf is the caller's again)
+  const float4 q = __ldg(&seg[(unsigned)(key & 0xFFFFFFFFull)]);
+  GroundParams p;
+  p.r_min = L.r_min[blockIdx.y]; p.r_max = L.r_max[blockIdx.y]; p.r_span = L.r_span[blockIdx.y];
+  const uint16_t cell = polar_cell_exact(q.x, q.y, p);
+  return cell == kNoCell ? sh : -__ldg(&gz[cell]);
+}
+
 // sequence ticks with their own detection values (lmot_seq_set_detect_params): frame blockIdx.y's whole BoxParams -- ROI and picScale,
 // L-shape gates, ram_points, min_points, rule mode and window, the sensor's height folded in on the host
 struct BoxFrameParams { BoxParams p[kMaxBatch]; };
@@ -76,6 +110,13 @@ static inline void fit_frame_of(const Slot* s, FitFrame& f, bool post_sem) {
   f.cl_box = s->d_cl_box; f.cl_marker = s->d_cl_marker; f.cl_ok = s->d_cl_ok;
   f.boxes = s->d_boxes; f.markers = s->d_markers; f.done = s->d_done; f.det_sem = post_sem ? s->d_det_sem : nullptr;
   f.hist_ctr = reinterpret_cast<unsigned*>(s->d_done + 1);
+}
+
+// unit i's entry of a LinesFit: its ground grid gz (nullptr: flat) and the window of detection values d
+static inline void lines_fit_of(const lmot_detect_params& d, const float* gz, LinesFit& L, int i) {
+  L.gz[i] = gz;
+  L.r_min[i] = d.r_min; L.r_max[i] = d.r_max;
+  { volatile float span = d.r_max - d.r_min; L.r_span[i] = span; }      // as ground_params_of
 }
 
 // BoxParams of detection values d (the context's, or a frame's own)

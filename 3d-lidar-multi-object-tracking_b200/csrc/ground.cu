@@ -28,6 +28,8 @@
 #include "exact_math.cuh"
 #include "tma.cuh"
 #include "ccl_device.cuh"
+#include "ground_lines.cuh"
+#include "polar_cell.cuh"
 
 namespace lmot {
 
@@ -50,24 +52,6 @@ __device__ __forceinline__ unsigned fkey(float f) {
 }
 __device__ __forceinline__ float fkey_inv(unsigned k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
-// ground_removal.cpp:46-64 (range filter) + :67-76 (getCellIndexFromPoints) + :89 (index guard), evaluated exactly as the
-// reference does: IEEE sqrt and divisions, glibc's atan2f (fdlibm restatement, exact_math.cuh), the double add / divide.
-// kClone: ground_fused_frame_kernel calls its own copy -- one shared non-inlined function would be compiled for the most general of its
-// callers' arguments (a frame's entry of a parameter array) and change the code of the other kernels
-template <int kClone = 0>
-__device__ __noinline__ uint16_t polar_cell_exact(float x, float y, const GroundParams& p) {
-  const float d = fsqrt(fadd(fmul(x, x), fmul(y, y)));
-  if (d <= p.r_min || d >= p.r_max || d != d) return kNoCell;
-  const float binP = fdiv(fsub(d, p.r_min), p.r_span);
-  const float binF = floorf(fmul(binP, (float)kNumBin));
-  if (!(binF >= 0.f && binF < (float)kNumBin)) return kNoCell;
-  const float a = atan2f_fdlibm(y, x);
-  const double chD = __ddiv_rn(__dadd_rn((double)a, 3.14159265358979323846), 6.28318530717958647692);
-  const float chF = floorf(fmul((float)chD, (float)kNumChannel));
-  if (!(chF >= 0.f && chF < (float)kNumChannel)) return kNoCell;
-  return (uint16_t)((int)chF * kNumBin + (int)binF);
 }
 
 // The cell index must equal the exact evaluation above bit for bit, but ~170 instructions per point (two IEEE divisions,
@@ -368,6 +352,39 @@ struct GroundBatch {
   float mount[kMaxBatch][3];  // ground_fused_rig_kernel: t_hmin, t_hmax, h_sensor of each frame's sensor (phase 2); unread otherwise
 };
 
+// ground_fused_lines_kernel: frame i's ground lines (lmot_set_ground_lines) -- its ground grid (nullptr: the frame's stream has them off,
+// phase 2 is groundRemove's polar grid), its sensor_height and the setting's three values
+struct GroundLinesFrames {
+  float* gz[kMaxBatch];
+  double sensor_height[kMaxBatch], max_slope[kMaxBatch], max_rmse[kMaxBatch], max_step[kMaxBatch];
+};
+
+struct LinesSrc {
+  const float* z;
+  __device__ float operator()(int b) const { return z[b]; }
+};
+struct LinesLimDst {
+  float* gz; float* lim; double tol;
+  __device__ void operator()(int b, float g) const { gz[b] = g; lim[b] = label_limit(g, true, tol); }
+};
+
+// phase 2 of a frame with ground lines: the CTA's own channels' min z into shared memory (H, one coalesced pass: the walk then never
+// waits for L2), then warp t's first lane walks own channel own0 + t (ground_lines.cuh) and writes its ground heights and label limits.
+// One channel per warp: the walks branch differently, and lanes of one warp would run each other's branches in turn.  The halo channels
+// are not needed.
+__device__ __forceinline__ void lines_slice(const GroundParams& p, const GroundLinesFrames& L, int frame, const unsigned* __restrict__ keys,
+                                            int own0, int n_own, float* H, float* __restrict__ lim) {
+  const int tid = threadIdx.x;
+  for (int l = tid; l < n_own * kNumBin; l += kFusedThreads) H[l] = fkey_inv(__ldcg(&keys[own0 * kNumBin + l]));
+  __syncthreads();
+  const int t = tid >> 5;
+  if ((tid & 31) == 0 && t < n_own) {
+    const int off = (own0 + t) * kNumBin;
+    ground_lines_channel(LinesSrc{H + t * kNumBin}, LinesLimDst{L.gz[frame] + off, lim + off, p.tol}, (double)p.r_min, (double)p.r_max,
+                         L.sensor_height[frame], L.max_slope[frame], L.max_rmse[frame], L.max_step[frame]);
+  }
+}
+
 // the fast evaluation of polar_cell(): cell id, kNoCell (certainly outside the range window) or kPending (within the guard band
 // of a cell boundary, or not a number: the exact evaluation decides)
 __device__ __forceinline__ unsigned polar_cell_fast(float x, float y, const GroundParams& p) {
@@ -484,8 +501,8 @@ __device__ __forceinline__ void bin_pair(int t0, int T, int cnt, int res_tiles, 
 // memory.  With ring-major clouds a chunk spans most of the 80 channels, so every CTA redid most of the grid and the kernel
 // issued far more instructions.  The grid is evaluated ONCE, spread over the CTAs.)
 // kRig: phase 2 takes each frame's t_hmin / t_hmax / h_sensor from B.mount (a sensor rig, lmot_set_sensors) instead of p
-template <bool kRig, int kClone = 0>
-__device__ __forceinline__ void ground_fused_body(const GroundBatch& B, const GroundParams& p, float roi) {
+template <bool kRig, int kClone = 0, bool kLines = false>
+__device__ __forceinline__ void ground_fused_body(const GroundBatch& B, const GroundParams& p, float roi, const GroundLinesFrames* L = nullptr) {
   extern __shared__ __align__(128) unsigned char fsm[];
   const int Gf = B.ctas_per_frame;
   const int frame = blockIdx.x / Gf, cta = blockIdx.x - frame * Gf;
@@ -578,7 +595,8 @@ __device__ __forceinline__ void ground_fused_body(const GroundBatch& B, const Gr
     const int gc = Gf < kNumChannel ? Gf : kNumChannel;
     if (cta < gc) {
       const int own0 = cta * kNumChannel / gc, own1 = (cta + 1) * kNumChannel / gc;
-      if (kRig) polar_grid_slice(p, B.mount[frame][0], B.mount[frame][1], B.mount[frame][2], keys, own0, own1 - own0, s_H, s_G, (float*)nullptr,
+      if (kLines && L->gz[frame]) lines_slice(p, *L, frame, keys, own0, own1 - own0, s_H, F.lim);
+      else if (kRig) polar_grid_slice(p, B.mount[frame][0], B.mount[frame][1], B.mount[frame][2], keys, own0, own1 - own0, s_H, s_G, (float*)nullptr,
                                  (float*)nullptr, (float*)nullptr, (float*)nullptr, F.hg, F.lim);
       else polar_grid_slice(p, p.t_hmin, p.t_hmax, p.h_sensor, keys, own0, own1 - own0, s_H, s_G, (float*)nullptr, (float*)nullptr, (float*)nullptr,
                             (float*)nullptr, F.hg, F.lim);
@@ -763,6 +781,15 @@ ground_fused_frame_kernel(const __grid_constant__ GroundBatch B, const __grid_co
   ground_fused_body<false, 1>(B, P.p[frame], P.roi[frame]);
 }
 
+// ground lines (lmot_set_ground_lines): the per-frame kernel with phase 2 replaced by each frame's lines where its stream has them on
+static_assert(sizeof(GroundBatch) + sizeof(GroundFrameParams) + sizeof(GroundLinesFrames) <= 4096, "ground_fused_lines_kernel: parameter block");
+__global__ void __launch_bounds__(kFusedThreads, 1)
+ground_fused_lines_kernel(const __grid_constant__ GroundBatch B, const __grid_constant__ GroundFrameParams P,
+                          const __grid_constant__ GroundLinesFrames L) {
+  const int frame = blockIdx.x / B.ctas_per_frame;
+  ground_fused_body<false, 2, true>(B, P.p[frame], P.roi[frame], &L);
+}
+
 // inspection only (lmot_debug_polar_grid): all five 80x120 grids of the reference from the min-z keys of the last launch, ten
 // channels per CTA.  (The fused kernel evaluates, per CTA, only the channels that CTA's points need, and keeps them in shared memory.)
 __global__ void __launch_bounds__(kFusedThreads)
@@ -801,11 +828,13 @@ int ground_alloc(Ctx* c, Slot* s) {
     LMOT_CUDA(c, cudaFuncSetAttribute(ground_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFusedSmem));
     LMOT_CUDA(c, cudaFuncSetAttribute(ground_fused_rig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFusedSmem));
     LMOT_CUDA(c, cudaFuncSetAttribute(ground_fused_frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFusedSmem));
+    LMOT_CUDA(c, cudaFuncSetAttribute(ground_fused_lines_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFusedSmem));
     int sms = 0, per_sm = 0, coop = 0;
     LMOT_CUDA(c, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
     LMOT_CUDA(c, cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, c->device));
-    // the grid barrier needs every CTA co-resident: the limit is the smallest over the three variants a launch may pick
-    const void* variants[] = {(const void*)ground_fused_kernel, (const void*)ground_fused_rig_kernel, (const void*)ground_fused_frame_kernel};
+    // the grid barrier needs every CTA co-resident: the limit is the smallest over the four variants a launch may pick
+    const void* variants[] = {(const void*)ground_fused_kernel, (const void*)ground_fused_rig_kernel, (const void*)ground_fused_frame_kernel,
+                              (const void*)ground_fused_lines_kernel};
     per_sm = INT_MAX;
     for (const void* k : variants) {
       int v = 0;
@@ -878,7 +907,8 @@ bool ground_reads_input_once(const Ctx* c, int n) {
 // One launch for F frames (F = 1: the frame pipeline and the stage entry points; F > 1: one frame per sensor stream, api.cu
 // lmot_batch_*).  Frame i runs on slots[i]'s buffers; its CTAs are [i * G, (i + 1) * G) of the grid and synchronise among themselves.
 int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* pts, const int* n, cudaStream_t st, bool fuse_count,
-                        bool want_labels, bool fuse_ccl, bool chain, const lmot_sensor* rig, const lmot_detect_params* det) {
+                        bool want_labels, bool fuse_ccl, bool chain, const lmot_sensor* rig, const lmot_detect_params* det,
+                        const GroundLinesJob* lines) {
   if (fuse_ccl && !fuse_count) return LMOT_ERR_INVALID;
   if (F < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   int n_max = 0;
@@ -935,11 +965,26 @@ int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* 
   void* args3[] = {(void*)&B, (void*)&gp, (void*)&roi};
   GroundFrameParams FP;
   void* args2[] = {(void*)&B, (void*)&FP};
-  if (det) {
+  GroundLinesFrames L;
+  memset(&L, 0, sizeof(L));
+  void* argsl[] = {(void*)&B, (void*)&FP, (void*)&L};
+  if (det || lines) {
     memset(&FP, 0, sizeof(FP));
-    for (int i = 0; i < F; ++i) { FP.p[i] = ground_params_of(det[i], c->gp.tap); FP.roi[i] = det[i].roi_m; }
+    const lmot_detect_params base = detect_params_of(c->prm);
+    for (int i = 0; i < F; ++i) {
+      lmot_detect_params d = det ? det[i] : base;
+      if (!det && rig) { d.h_sensor = rig[i].h_sensor; d.t_hmin = rig[i].t_hmin; d.t_hmax = rig[i].t_hmax; d.sensor_height = rig[i].sensor_height; }
+      FP.p[i] = ground_params_of(d, c->gp.tap); FP.roi[i] = d.roi_m;
+      if (lines) {
+        const lmot_ground_lines* g = lines[i].cfg;
+        L.gz[i] = g ? lines[i].gz : nullptr;
+        L.sensor_height[i] = d.sensor_height;
+        if (g) { L.max_slope[i] = g->max_slope; L.max_rmse[i] = g->max_rmse; L.max_step[i] = g->max_step; }
+      }
+    }
   }
-  void** args = det ? args2 : args3;
+  if (lines) kern = (const void*)ground_fused_lines_kernel;
+  void** args = lines ? argsl : det ? args2 : args3;
   // every frame's chunk is laid out with the tile count of the longest one (the kernel derives its layout from its own chunk;
   // a shorter chunk just leaves the tail of the allocation unused)
   const int tiles = (chunk_max + kTilePts - 1) / kTilePts;

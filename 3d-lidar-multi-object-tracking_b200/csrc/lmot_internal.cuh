@@ -236,6 +236,8 @@ struct Slot {
   AreaBlock* d_area = nullptr;         // vertex staging: one block on a frame slot, kMaxBatch on a bank pseudo-slot
   bool area_last = false;              // the slot's most recent frame was masked (lmot_cluster_outputs)
 
+  float* d_gz = nullptr;               // [9600] ground heights of the slot's latest frame with ground lines (allocated on first use)
+
   struct Result* res = nullptr;       // result block of the frame currently (or last) processed on this slot
 };
 
@@ -332,6 +334,12 @@ inline lmot_deskew deskew_defaults() {
 // lmot_default_box_search
 inline lmot_box_search box_search_defaults() { lmot_box_search b; b.on = 0; b.n_angles = 90; return b; }
 
+// lmot_default_ground_lines
+inline lmot_ground_lines ground_lines_defaults() { lmot_ground_lines g; g.on = 0; g.max_slope = 0.3; g.max_rmse = 0.08; g.max_step = 0.3; return g; }
+
+// one frame of a launch with ground lines: its stream's setting (nullptr: off) and the grid of ground heights its lines go to
+struct GroundLinesJob { const lmot_ground_lines* cfg; float* gz; };
+
 // lmot_default_accumulate
 inline lmot_accumulate accumulate_defaults() { lmot_accumulate a; memset(&a, 0, sizeof(a)); a.sweeps = 1; a.max_age_s = 0.5; return a; }
 
@@ -372,9 +380,11 @@ struct StreamCfg {
   AreaBlock area = {};                      // detection area (detect_area.cu)
   AccHist acc;                              // sweep accumulation and its history (accumulate.cu)
   lmot_box_search search = box_search_defaults();   // box search (box_search.cu)
+  lmot_ground_lines lines = ground_lines_defaults(); // ground lines (ground_lines.cuh)
   bool merges() const { return rig_merge && n_sensors > 0; }
   bool masked() const { return area.n_rings > 0; }
   int search_angles() const { return search.on ? search.n_angles : 0; }   // A of the stream's units, 0: boxFitting's fit
+  const lmot_ground_lines* lines_on() const { return lines.on ? &lines : nullptr; }
 };
 
 struct Ctx {
@@ -456,6 +466,9 @@ struct Ctx {
   // ---- lmot_debug_area_masks: the unit masks of the most recent own-stream submission (none: it was not masked)
   const unsigned* area_dbg[kMaxBatch] = {};
   int n_area_dbg = 0;
+  // ---- lmot_debug_ground_lines: the ground grids of the most recent own-stream submission (none: its lines were off)
+  const float* gz_dbg[kMaxBatch] = {};
+  int n_gz_dbg = 0;
 
   // ---- timing
   bool timing = false;
@@ -514,8 +527,10 @@ int ground_launch(Ctx* c, Slot* s, cudaStream_t st, const float4* pts, int n, bo
 // rig (nullable): sensor i's h_sensor / t_hmin / t_hmax for frame i (lmot_set_sensors); nullptr: lmot_params' values for every frame
 // det (nullable): frame i's own detection values (sensor values already folded in; lmot_seq_set_detect_params) -> the per-frame kernel
 // variant; rig is then unused
+// lines (nullable): frame i's ground lines (cfg nullptr: off) and the grid its lines go to -> ground_fused_lines_kernel, every frame with
+// its own values (det, else lmot_params' with rig's folded in)
 int ground_launch_batch(Ctx* c, Slot* const* slots, int F, const float4* const* pts, const int* n, cudaStream_t st, bool fuse_count, bool want_labels, bool fuse_ccl = false, bool chain = false, const lmot_sensor* rig = nullptr,
-                        const lmot_detect_params* det = nullptr);
+                        const lmot_detect_params* det = nullptr, const GroundLinesJob* lines = nullptr);
 void ground_chain_forget(int device, bool device_idle);
 int ground_cells_debug(Ctx* c, Slot* s, cudaStream_t st);
 int ground_grids_debug(Ctx* c, Slot* s, cudaStream_t st);   // d_minz / d_height / d_smoothed / d_hdiff / d_hg_dbg from the last launch's keys
@@ -532,13 +547,18 @@ int boxfit_alloc(Ctx* c, Slot* s);
 int boxfit_alloc_shared(Ctx* c);
 void boxfit_free(Slot* s);
 // search: the frame's box search angle count A (0: boxFitting's fit)
-int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem = false, const unsigned* area = nullptr, int search = 0);
+// lines: the frame's ground grid (ground lines; nullptr: off)
+int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem = false, const unsigned* area = nullptr, int search = 0,
+                  const float* lines = nullptr);
 // rig (nullable): sensor i's sensor_height for frame i (box fitting) / sensor i's pose for list i (concatenation)
 // det (nullable): frame i's own detection values, as ground_launch_batch's; rig is then unused
 // area (nullable): as ccl_launch_batch's
 // search (nullable): frame i's box search angle count A, 0: boxFitting's fit (box_search.cu fits the others)
+// lines (nullable): unit i's ground grid, nullptr for a unit measured from the flat sensor_height; any -> every unit through the ground
+// lines variants (box_fit_lines_kernel, box_search_lines_kernel)
 int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig = nullptr,
-                        const lmot_detect_params* det = nullptr, const unsigned* const* area = nullptr, const int* search = nullptr);
+                        const lmot_detect_params* det = nullptr, const unsigned* const* area = nullptr, const int* search = nullptr,
+                        const float* const* lines = nullptr);
 // box search (box_search.cu): setting validation, the angle table of A (lmot_box_search_angles), and the device tables of every A
 // (Ctx::d_bs_tab, uploaded once by the first setter that turns the search on)
 bool box_search_valid(const lmot_box_search& b);
@@ -546,8 +566,9 @@ void box_search_table(int A, float (*out)[2]);
 int box_search_ensure(Ctx* c);
 // box search over n units (their Slots' box-fitting buffers): unit i with detection values det[i] (its sensor's height folded in) and A[i]
 // angles, gx CTAs per unit, as a programmatic dependent of the kernel before it iff pdl
+// lines (nullable): unit i's ground grid as boxfit_launch_batch's -> box_search_lines_kernel
 int box_search_launch(Ctx* c, Slot* const* units, int n, const lmot_detect_params* det, const int* A, cudaStream_t st, bool post_sem, int gx,
-                      bool pdl);
+                      bool pdl, const float* const* lines = nullptr);
 int boxes_pack_lists_launch(Ctx* c, cudaStream_t st, const float* d_lists, const int* d_counts, int n_lists, int cap, float* d_boxes, int* d_counters,
                             const lmot_sensor* rig = nullptr);
 int boxes_concat_launch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, float* d_boxes, int* d_counters, int* d_frame_counts, int* det_sem,

@@ -914,6 +914,64 @@ int lmot_seq_set_box_search(lmot_ctx* ctx, int k, const lmot_box_search* b);
 int lmot_seq_get_box_search(const lmot_ctx* ctx, int k, lmot_box_search* b);
 int lmot_box_search_angles(int n_angles, float out[][2]);                  /* step 1 on the host, no device needed: out[a] = (c_a, s_a) */
 
+/* ---- ground lines: slope-following ground removal and box heights from the local ground ---------------------------------------------
+ * groundRemove clamps each polar cell's min z into [t_hmin, t_hmax] and boxFitting measures a cluster's height from z = -sensor_height:
+ * both assume the ground is the sensor frame's plane z = -sensor_height.  On a grade, under pitch, or with a sensor that is not mounted
+ * level, objects uphill are too tall and objects downhill are labelled ground or too short.  Ground lines fit the ground of each of the
+ * 80 channels as a chain of straight lines over range, and measure each cluster's height from the line under its lowest point.
+ *
+ * Definition.  A stream (the context's own: lmot_set_ground_lines; sequence k: lmot_seq_set_ground_lines) with on = 1: each frame of a
+ * FRAMES step, with its unit values r_min, r_max, sensor_height and ground_tolerance (lmot_params', or the sequence's detection values; a
+ * rig frame takes its sensor's sensor_height):
+ *   1. phase 1 of ground removal is unchanged: the pre-filters, each point's polar cell (bit-exact) and minZ per cell (1000: empty);
+ *   2. lines per channel: bins b = 0 .. 119 in order; a bin with minZ < 1000 is the prototype (r_b, z_b), r_b = r_min + (b + 0.5) *
+ *      (r_max - r_min) / 120, z_b = (double)minZ.  Every operation is double, left to right, without contraction; the unit values are
+ *      the float parameters widened to double (lmot_ground_lines_grid reproduces a frame when passed (double)p.r_min etc.).  S = (n, Sr, Sz, Srr,
+ *      Srz, Szz) is the open point set; fit(S): den = n*Srr - Sr*Sr, m = (n*Srz - Sr*Sz) / den, c = (Sz - m*Sr) / n,
+ *      sse = Szz - 2*m*Srz - 2*c*Sz + m*m*Srr + 2*m*c*Sr + n*c*c.  Closing S appends the line (first bin of S, m, c) of fit(S) if n >= 2,
+ *      then empties S.  For each prototype:
+ *        extend: if n >= 2, fit S plus the point; if |m| <= max_slope and sse <= n' * max_rmse * max_rmse (n' = n + 1) the point joins S,
+ *          else S is closed and the point is a seed;
+ *        seed test: with a line of the channel, |z - (m_last*r + c_last)| <= max_step; without one, |z + sensor_height| <= max_slope*r +
+ *          max_step; with n == 1 also |z - z0| <= max_slope*(r - r0) ((r0, z0): S's point).  Pass: the point joins S.  Fail with n == 1:
+ *          S is emptied and the seed test repeats for the point.  Fail with n == 0: the point is dropped.
+ *      After bin 119, S is closed;
+ *   3. ground height of a cell: gz(ch, b) = (float)(m*r_b + c) of the channel's last line whose first bin is <= b; none: its first line;
+ *      a channel without lines: (float)(-sensor_height).  lmot_ground_lines_grid computes this grid on the host;
+ *   4. labels: an in-window point is ground iff (double)z < (double)gz + ground_tolerance, elevated otherwise.  The median and outlier
+ *      filters, t_hmin, t_hmax, h_sensor and t_hdiff are not read.  Both clouds keep the input order;
+ *   5. box heights: each cluster's lowest point (min z, ties to the first in cloud order) gives g = gz of its polar cell, or
+ *      -sensor_height when it lies outside the window.  The rule filter and the box's bottom corners use sensor_height := -g: the cluster
+ *      gets what boxFitting gives it with sensorHeight = -g.  This holds for boxFitting's fit and for box search.  A merge unit
+ *      (lmot_set_rig_merge) keeps the vehicle's flat sensor_height, because its cloud mixes sensor frames; its sensors' labels still
+ *      come from their lines.
+ * Applies to lmot_frame / _submit / _dev, lmot_detect_dev, lmot_batch* including lmot_batch_detect_dev, and the FRAMES steps of
+ * lmot_seq* / lmot_seq_tick*.  Never to the stage entry points (they stay the reference), lmot_batch_ground_ccl_dev, LISTS steps,
+ * lmot_track_step*, lmot_seq_track* or lmot_shared_*.
+ * Submission.  Host state captured by value at submission; frames and ticks in flight keep theirs.  lmot_seq_open turns it off for every
+ * sequence; lmot_seq_tracker_reset, _load and LMOT_SEQ_RESTART keep it.  A submission without a stream that has lines on runs exactly the
+ * launches, copies and memsets it ran before ground lines existed.
+ * Errors.  LMOT_ERR_INVALID, setting unchanged: on not 0 / 1, a value not finite, max_slope <= 0, max_rmse <= 0, max_step <= 0, k out of
+ * range or no open set.  LMOT_ERR_STATE, nothing submitted: a submission with lines on in timing mode.
+ * Memory.  Each detection slot that runs a frame with lines on allocates its 9,600-float ground grid once (38 KB).
+ * lmot_debug_ground_lines(ctx, gz, cap_units, n_units): the device grids of the context's most recent own-stream submission, frame by
+ * frame (9,600 floats each, cell ch * 120 + b); n_units = 0 when its lines were off.  Synchronises the device. */
+typedef struct lmot_ground_lines {
+  int on;                      /* 0 (default): groundRemove's polar grid and the flat sensor_height; 1: the lines above */
+  double max_slope;            /* 0.3: largest |dz/dr| of a line, and the seed window's slope */
+  double max_rmse;             /* 0.08 m: largest root-mean-square residual of a line */
+  double max_step;             /* 0.3 m: largest step from the previous line (or the flat ground) to a seed */
+} lmot_ground_lines;
+int lmot_default_ground_lines(lmot_ground_lines* g);
+int lmot_set_ground_lines(lmot_ctx* ctx, const lmot_ground_lines* g);     /* NULL: the defaults (off) */
+int lmot_get_ground_lines(const lmot_ctx* ctx, lmot_ground_lines* g);
+int lmot_seq_set_ground_lines(lmot_ctx* ctx, int k, const lmot_ground_lines* g);
+int lmot_seq_get_ground_lines(const lmot_ctx* ctx, int k, lmot_ground_lines* g);
+/* steps 2-3 on the host, no device needed (on is not read): minz[ch * 120 + b] -> gz[ch * 120 + b] */
+int lmot_ground_lines_grid(const lmot_ground_lines* g, const float minz[LMOT_NUM_CHANNEL * LMOT_NUM_BIN], double r_min, double r_max,
+                           double sensor_height, float gz[LMOT_NUM_CHANNEL * LMOT_NUM_BIN]);
+int lmot_debug_ground_lines(lmot_ctx* ctx, float* gz, int cap_units, int* n_units);
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);
