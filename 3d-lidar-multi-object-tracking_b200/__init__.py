@@ -376,6 +376,27 @@ def ground_lines_grid(minz, r_min: float, r_max: float, sensor_height: float, **
     return out
 
 
+class Layers(C.Structure):
+    """lmot_layers: layered clustering, connected components over (x, y, height slice) (include/lmot.h)."""
+    _fields_ = [("on", C.c_int), ("n_slices", C.c_int), ("slice_m", C.c_double), ("z_min", C.c_double), ("gap_slices", C.c_int)]
+
+
+def default_layers() -> dict:
+    lib = load_library()
+    l = Layers()
+    lib.lmot_default_layers(C.byref(l))
+    return {name: getattr(l, name) for name, _ in Layers._fields_}
+
+
+def _layers(fields: dict) -> Layers:
+    base = default_layers()
+    unknown = set(fields) - set(base)
+    if unknown:
+        raise KeyError(f"unknown layers fields {sorted(unknown)}")
+    base.update(fields)
+    return Layers(int(base["on"]), int(base["n_slices"]), float(base["slice_m"]), float(base["z_min"]), int(base["gap_slices"]))
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -439,6 +460,7 @@ ABI_SYMBOLS = [
     "lmot_box_search_angles",
     "lmot_default_ground_lines", "lmot_set_ground_lines", "lmot_get_ground_lines", "lmot_seq_set_ground_lines", "lmot_seq_get_ground_lines",
     "lmot_ground_lines_grid", "lmot_debug_ground_lines",
+    "lmot_default_layers", "lmot_set_layers", "lmot_get_layers", "lmot_seq_set_layers", "lmot_seq_get_layers", "lmot_debug_point_clusters",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
@@ -1116,6 +1138,45 @@ class Lmot:
         fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
         self._chk(fn(self.h, out.ctypes.data, MAX_BATCH, C.byref(n)))
         return out[: n.value]
+
+    # ---- layered clustering (lmot_set_layers) -----------------------------------------------------------------------------------
+    def set_layers(self, **fields):
+        """The context's frames: layered clustering settings with `fields` replaced (on=1 turns it on; no fields: the defaults, off).
+        Applies from the next submission on; frames in flight keep theirs."""
+        self._chk(self.lib.lmot_set_layers(self.h, C.byref(_layers(fields)) if fields else None))
+
+    def get_layers(self) -> dict:
+        l = Layers()
+        self._chk(self.lib.lmot_get_layers(self.h, C.byref(l)))
+        return {name: getattr(l, name) for name, _ in Layers._fields_}
+
+    def seq_set_layers(self, k: int, **fields):
+        """Sequence k's FRAMES steps, arguments as set_layers."""
+        self._chk(self.lib.lmot_seq_set_layers(self.h, int(k), C.byref(_layers(fields)) if fields else None))
+
+    def seq_get_layers(self, k: int) -> dict:
+        l = Layers()
+        self._chk(self.lib.lmot_seq_get_layers(self.h, int(k), C.byref(l)))
+        return {name: getattr(l, name) for name, _ in Layers._fields_}
+
+    def debug_point_clusters(self) -> list:
+        """lmot_debug_point_clusters: one int32 array of per-point cluster ids per unit of the most recent own-stream submission, in
+        each unit's cloud order ([]: it was not layered)"""
+        fn = self.lib.lmot_debug_point_clusters
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_void_p]
+        nu = C.c_int(0)
+        npt = np.zeros(MAX_BATCH, np.int32)
+        st = fn(self.h, None, 0, C.byref(nu), npt.ctypes.data)
+        if st not in (OK, ERR_CAPACITY):
+            self._chk(st)
+        tot = int(npt[: nu.value].sum())
+        ids = np.zeros(max(tot, 1), np.int32)
+        self._chk(fn(self.h, ids.ctypes.data, tot, C.byref(nu), npt.ctypes.data))
+        out, off = [], 0
+        for u in range(nu.value):
+            out.append(ids[off: off + npt[u]].copy())
+            off += int(npt[u])
+        return out
 
     @staticmethod
     def _accum_info(a: AccumInfo) -> list:

@@ -250,7 +250,17 @@ int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tra
   s->area_last = masked;
   c->n_area_dbg = masked ? 1 : 0;
   c->area_dbg[0] = mask;
-  const bool fuse = c->fuse_ccl && !masked && !acc;
+  // layered clustering: the slot's layer buffers; clustering then runs as its own launch, layered, and box fitting reads its run tables
+  const bool layered = c->own_cfg.layers.on != 0;
+  LayerTab ltab{};
+  if (layered) {
+    if ((rc = layers_ensure(c, s, s->stream))) return rc;
+    ltab = layer_tab_of(s);
+  }
+  s->layers_last = layered;
+  c->n_lay_dbg = layered ? 1 : 0;
+  c->lay_dbg[0] = s;
+  const bool fuse = c->fuse_ccl && !masked && !acc && !layered;
   // ground lines: the ground kernel's lines variant writes the slot's ground grid, box fitting measures each cluster from it
   const lmot_ground_lines* gl = c->own_cfg.lines_on();
   if (gl && (rc = lines_ensure(c, s))) return rc;
@@ -267,10 +277,16 @@ int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tra
   if (c->timing) cudaEventRecord(r->ev[1], s->stream);
   AccHist* hp = &h;
   if (acc && (rc = accumulate_launch(c, s->stream, s, &aj, 1, &hp, 1))) return rc;     // E_t into the ring, the earlier sweeps behind it
-  if (!fuse && (rc = cluster_launch(c, s, s->stream, fit_upper, true, mask))) return rc;      // (fused: the ground kernel's last CTA did it)
+  if (layered) {
+    const LayerUnit lu{s, mask, c->own_cfg.layers, c->prm.sensor_height, fit_upper};
+    if ((rc = layers_launch(c, s->stream, &lu, 1, s))) return rc;
+  } else if (!fuse && (rc = cluster_launch(c, s, s->stream, fit_upper, true, mask))) {     // (fused: the ground kernel's last CTA did it)
+    return rc;
+  }
   if (c->timing) cudaEventRecord(r->ev[2], s->stream);
   const bool gf = with_tracker && c->prm.global_frame;
-  if ((rc = boxfit_launch(c, s, s->stream, fit_upper, with_tracker && !gf, mask, c->own_cfg.search_angles(), gl ? s->d_gz : nullptr))) return rc;   // with_tracker: posts the slot's detection semaphore
+  if ((rc = boxfit_launch(c, s, s->stream, fit_upper, with_tracker && !gf, mask, c->own_cfg.search_angles(), gl ? s->d_gz : nullptr,
+                          layered ? &ltab : nullptr))) return rc;   // with_tracker: posts the slot's detection semaphore
   if (gf && (rc = boxes_to_global_launch(c, s, s->stream, s->d_boxes, s->d_counters, ts, v, yaw, true))) return rc;   // ... or this one does
   if (c->timing) cudaEventRecord(r->ev[3], s->stream);
   LMOT_CUDA(c, cudaEventRecord(s->ev_det_done, s->stream));
@@ -522,7 +538,26 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
     nacj += nu_d;
     ach[nach++] = &q.acc;
   }
-  const bool fuse = c->fuse_ccl && !merging && nblk == 0 && nacj == 0;
+  // layered clustering: the units of a stream with layers on cluster in layers_launch (sensor_height: the unit's box-fitting value), the
+  // others in ccl_launch_batch; box fitting reads the layered units' run tables
+  LayerUnit lu[kMaxBatch];
+  LayerTab ltab[kMaxBatch];
+  Slot* cu[kMaxBatch];
+  const unsigned* camask[kMaxBatch];
+  int nl = 0, ncu = 0;
+  bool layering = false;
+  for (int d = 0; d < G; ++d) layering |= g[d].cfg->layers.on != 0;
+  for (int d = 0; layering && d < G; ++d) {
+    const StreamCfg& q = *g[d].cfg;
+    for (int i = U.f0[d]; i < U.f0[d + 1]; ++i) {
+      ltab[i] = LayerTab{};
+      if (!q.layers.on) { cu[ncu] = U.u[i]; camask[ncu++] = amask[i]; continue; }
+      if ((rc = layers_ensure(c, U.u[i], st))) return rc;
+      lu[nl++] = LayerUnit{U.u[i], amask[i], q.layers, own_det ? udet[i].sensor_height : U.rig[i].sensor_height, unn[i]};
+      ltab[i] = layer_tab_of(U.u[i]);
+    }
+  }
+  const bool fuse = c->fuse_ccl && !merging && nblk == 0 && nacj == 0 && !layering;
   // ground lines: a frame whose stream has them on gets its slot's ground grid; its unit (an unmerged frame) measures boxes from it
   GroundLinesJob lj[kMaxBatch];
   const float* ugz[kMaxBatch] = {};
@@ -549,10 +584,15 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
   if (c->timing) cudaEventRecord(r->ev[1], st);
   if (nm > 0 && (rc = rig_merge_launch(c, st, src, mpose, mn, nm, ms0, mu, mfc, mroi))) return rc;
   if (nacj > 0 && (rc = accumulate_launch(c, st, bk, acj, nacj, ach, nach))) return rc;
-  if (!fuse && (rc = ccl_launch_batch(c, U.u, nu, st, area))) return rc;
+  if (!layering) {
+    if (!fuse && (rc = ccl_launch_batch(c, U.u, nu, st, area))) return rc;
+  } else {
+    if ((rc = layers_launch(c, st, lu, nl, bk))) return rc;
+    if (ncu > 0 && (rc = ccl_launch_batch(c, cu, ncu, st, area ? camask : nullptr))) return rc;
+  }
   if (c->timing) cudaEventRecord(r->ev[2], st);
   return boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr, area, searching ? usearch : nullptr,
-                             lining ? ugz : nullptr);
+                             lining ? ugz : nullptr, layering ? ltab : nullptr);
 }
 
 // the IDs of a result being returned (lmot_track_ids): copied now, the block is reused by later submissions
@@ -1043,6 +1083,8 @@ int lmot_component_cluster(lmot_ctx* ctx, const float* elevated, int n, int stri
   if ((rc = upload_points(c, s, st, elevated, n, stride, s->d_elev))) return rc;
   if ((rc = set_counter(c, s, st, CNT_N_ELEV, n))) return rc;
   s->area_last = false;
+  s->layers_last = false;
+  c->n_lay_dbg = 0;
   if ((rc = cluster_launch(c, s, st, n))) return rc;
   if ((rc = fetch_counters(c, s, st))) return rc;
   if (num_cluster) *num_cluster = s->h_counters[CNT_NUM_CLUSTER];
@@ -1062,6 +1104,7 @@ int lmot_cluster_outputs(lmot_ctx* ctx, float* clustered, int cap_clustered, int
   int rc = lmot_sync(ctx);
   if (rc) return rc;
   Slot* s = &c->slots[c->last_slot];
+  if (s->layers_last) return LMOT_ERR_STATE;           // the label grid does not name the layered clusters
   cudaStream_t st = c->stream;
   if ((rc = cluster_outputs_launch(c, s, st))) return rc;
   int cnt[2] = {0, 0};
@@ -1083,6 +1126,7 @@ int lmot_debug_label_grid(lmot_ctx* ctx, int32_t* grid, int* num_cluster) {
   int rc = lmot_sync(ctx);
   if (rc) return rc;
   Slot* s = &c->slots[c->last_slot];
+  if (s->layers_last) return LMOT_ERR_STATE;
   if ((rc = fetch_counters(c, s, c->stream))) return rc;
   if (num_cluster) *num_cluster = s->h_counters[CNT_NUM_CLUSTER];
   if (grid) {
@@ -1107,6 +1151,8 @@ int lmot_box_fit(lmot_ctx* ctx, const float* elevated, int n, int stride, const 
   LMOT_CUDA(c, cudaMemcpyAsync(s->d_label_grid, grid, kCartCells * sizeof(int), cudaMemcpyHostToDevice, st));
   s->label_grid_foreign = true;
   s->area_last = false;
+  s->layers_last = false;
+  c->n_lay_dbg = 0;
   if ((rc = set_counter(c, s, st, CNT_N_ELEV, n))) return rc;
   if ((rc = set_counter(c, s, st, CNT_NUM_CLUSTER, num_cluster))) return rc;
   s->res = &c->results[0];
@@ -1165,7 +1211,7 @@ int lmot_detect_dev(lmot_ctx* ctx, const float* d_points, int n) {
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
-  if ((c->own_cfg.masked() || c->own_cfg.search.on || c->own_cfg.lines.on) && c->timing) return LMOT_ERR_STATE;
+  if ((c->own_cfg.masked() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on) && c->timing) return LMOT_ERR_STATE;
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, true);
   LMOT_CUDA(c, cudaEventRecord(s->ev_fork, c->stream));
@@ -1177,7 +1223,8 @@ int lmot_frame_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp
   if (!ctx || n < 0 || (n > 0 && !d_points) || (reinterpret_cast<uintptr_t>(d_points) & 15u)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   const bool dsk = c->own_cfg.deskew.on != 0;
-  if ((dsk || c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on) && c->timing) return LMOT_ERR_STATE;
+  if ((dsk || c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on) && c->timing)
+    return LMOT_ERR_STATE;
   if (dsk && c->own_cfg.deskew.time_field != 3) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
@@ -1198,7 +1245,8 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
-  if ((c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on) && c->timing) return LMOT_ERR_STATE;
+  if ((c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on) && c->timing)
+    return LMOT_ERR_STATE;
   const bool dsk = c->own_cfg.deskew.on != 0;
   if (dsk) {                           // (validated before anything is submitted: upload_points checks the rest without deskew)
     if (c->timing) return LMOT_ERR_STATE;
@@ -1307,7 +1355,7 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   const bool dsk = with_tracker && q.deskew.on != 0;                // (lmot_batch_detect_dev has no stamp: never deskewed)
   if (dsk && c->timing) return LMOT_ERR_STATE;
   if (dsk && (host ? stride <= q.deskew.time_field : q.deskew.time_field != 3)) return LMOT_ERR_INVALID;
-  if ((q.merges() || q.masked() || q.search.on || q.lines.on) && c->timing) return LMOT_ERR_STATE;
+  if ((q.merges() || q.masked() || q.search.on || q.lines.on || q.layers.on) && c->timing) return LMOT_ERR_STATE;
   if (with_tracker && q.acc.on() && c->timing) return LMOT_ERR_STATE;
   if (host && c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;
   int rc = batch_ensure(c, n_frames);
@@ -1339,6 +1387,8 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   for (int i = 0; i < c->n_area_dbg; ++i) c->area_dbg[i] = U.u[i]->d_area_mask;
   c->n_gz_dbg = q.lines.on ? n_frames : 0;
   for (int i = 0; i < c->n_gz_dbg; ++i) c->gz_dbg[i] = c->bslots[b * c->batch_frames + i].d_gz;
+  c->n_lay_dbg = q.layers.on ? U.f0[1] : 0;
+  for (int i = 0; i < c->n_lay_dbg; ++i) c->lay_dbg[i] = U.u[i];
   const bool gf = with_tracker && c->prm.global_frame;
   if ((rc = boxes_concat_launch(c, U.u, U.f0[1], st, k->d_boxes, k->d_counters, U.fc[0], (with_tracker && !gf) ? k->d_det_sem : nullptr,
                                 U.rig_on[0] ? U.rig : nullptr))) return rc;
@@ -2303,6 +2353,57 @@ int lmot_debug_ground_lines(lmot_ctx* ctx, float* gz, int cap_units, int* n_unit
   const int n = c->n_gz_dbg < cap_units ? c->n_gz_dbg : cap_units;
   for (int i = 0; i < n; ++i)
     LMOT_CUDA(c, cudaMemcpy(gz + (size_t)i * kPolarCells, c->gz_dbg[i], kPolarCells * sizeof(float), cudaMemcpyDeviceToHost));
+  return LMOT_OK;
+}
+
+// ---- layered clustering (layers.cu).  Host state, as ground lines: the launch parameters carry each unit's values
+int lmot_default_layers(lmot_layers* l) {
+  if (!l) return LMOT_ERR_INVALID;
+  *l = layers_defaults();
+  return LMOT_OK;
+}
+
+static int layers_set(lmot_layers& dst, const lmot_layers* l) {
+  const lmot_layers v = l ? *l : layers_defaults();
+  if (!layers_valid(v)) return LMOT_ERR_INVALID;
+  dst = v;
+  return LMOT_OK;
+}
+
+int lmot_set_layers(lmot_ctx* ctx, const lmot_layers* l) { return ctx ? layers_set(ctx->c.own_cfg.layers, l) : LMOT_ERR_INVALID; }
+
+int lmot_get_layers(const lmot_ctx* ctx, lmot_layers* l) {
+  if (!ctx || !l) return LMOT_ERR_INVALID;
+  *l = ctx->c.own_cfg.layers;
+  return LMOT_OK;
+}
+
+int lmot_seq_set_layers(lmot_ctx* ctx, int k, const lmot_layers* l) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  return layers_set(ctx->c.seq_cfg[k].layers, l);
+}
+
+int lmot_seq_get_layers(const lmot_ctx* ctx, int k, lmot_layers* l) {
+  if (!ctx || !l || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  *l = ctx->c.seq_cfg[k].layers;
+  return LMOT_OK;
+}
+
+int lmot_debug_point_clusters(lmot_ctx* ctx, int32_t* ids, int cap, int* n_units, int n_points[LMOT_MAX_BATCH]) {
+  if (!ctx || cap < 0 || (cap > 0 && !ids)) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  int rc = lmot_sync(ctx);
+  if (rc) return rc;
+  int n[kMaxBatch], tot = 0;
+  for (int u = 0; u < c->n_lay_dbg; ++u) {
+    LMOT_CUDA(c, cudaMemcpy(&n[u], c->lay_dbg[u]->d_counters + CNT_N_ELEV, sizeof(int), cudaMemcpyDeviceToHost));
+    tot += n[u];
+    if (n_points) n_points[u] = n[u];
+  }
+  if (n_units) *n_units = c->n_lay_dbg;
+  if (tot > cap) return LMOT_ERR_CAPACITY;
+  for (int u = 0, off = 0; u < c->n_lay_dbg; off += n[u], ++u)
+    if ((rc = layers_point_ids(c, c->lay_dbg[u], n[u], ids + off))) return rc;
   return LMOT_OK;
 }
 

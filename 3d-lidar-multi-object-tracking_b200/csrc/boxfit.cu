@@ -44,8 +44,11 @@ __device__ __forceinline__ void seg_offsets_body(const FitFrame& F, int max_clus
 
 // kArea: a point whose cell is outside its unit's detection-area mask `area` gets cluster 0 -- dilation can label masked cells, and
 // those hold no point of the masked cloud E_area
-template <bool kArea>
-__device__ __forceinline__ void tile_hist_body(const FitBatch& B, int max_clusters, const unsigned* __restrict__ area) {
+// kLayers: a layered unit (lt->slice set) takes each point's cluster from its slice and its column's run table (layers.cu) instead of the
+// label grid; its slice byte already excludes points without a column or outside the detection area
+template <bool kArea, bool kLayers = false>
+__device__ __forceinline__ void tile_hist_body(const FitBatch& B, int max_clusters, const unsigned* __restrict__ area,
+                                               const LayerTab* lt = nullptr) {
   extern __shared__ int s_hist[];
   fit_pdl_trigger();
   const FitFrame& F = B.f[blockIdx.y];
@@ -61,7 +64,15 @@ __device__ __forceinline__ void tile_hist_body(const FitBatch& B, int max_cluste
   unsigned cid = 0;
   if (i < n) {
     const unsigned c = cart[i];
-    if (c != kNoCell && (!kArea || !area || area_kept(area, c))) cid = (unsigned)__ldg(&label_grid[c]);
+    if (kLayers && lt->slice) {
+      const unsigned sl = __ldg(&lt->slice[i]);
+      if (sl != 0xFFu) {
+        const unsigned d = __ldg(&lt->cols[c]);
+        if ((d >> sl) & 1u) cid = (unsigned)(-__ldg(&lt->lab[__ldg(&lt->base[c]) + __popc(piece_starts(d) & ((2u << sl) - 1u)) - 1]));
+      }
+    } else if (c != kNoCell && (!kArea || !area || area_kept(area, c))) {
+      cid = (unsigned)__ldg(&label_grid[c]);
+    }
     if (cid > (unsigned)K) cid = 0;                    // capacity overflow is reported by seg_offsets_kernel
     pcid[i] = (uint16_t)cid;
   }
@@ -89,6 +100,15 @@ struct FitAreaMasks { const unsigned* m[kMaxBatch]; };
 __global__ void __launch_bounds__(kTile)
 tile_hist_area_kernel(const __grid_constant__ FitBatch B, int max_clusters, const __grid_constant__ FitAreaMasks A) {
   tile_hist_body<true>(B, max_clusters, A.m[blockIdx.y]);
+}
+
+// layered clustering: unit blockIdx.y's run tables (slice nullptr: a unit of the same launch clustered on its label grid) and area mask
+struct FitLayers { LayerTab t[kMaxBatch]; };
+
+__global__ void __launch_bounds__(kTile)
+tile_hist_layers_kernel(const __grid_constant__ FitBatch B, int max_clusters, const __grid_constant__ FitAreaMasks A,
+                        const __grid_constant__ FitLayers L) {
+  tile_hist_body<true, true>(B, max_clusters, A.m[blockIdx.y], &L.t[blockIdx.y]);
 }
 
 // ---------------------------------------------------------------------------------------------- B2
@@ -431,6 +451,7 @@ int boxfit_alloc_shared(Ctx* c) {
   if (sh > 48 * 1024) {
     LMOT_CUDA(c, cudaFuncSetAttribute(tile_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh));
     LMOT_CUDA(c, cudaFuncSetAttribute(tile_hist_area_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh));
+    LMOT_CUDA(c, cudaFuncSetAttribute(tile_hist_layers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh));
     LMOT_CUDA(c, cudaFuncSetAttribute(scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh));
   }
   return LMOT_OK;
@@ -473,7 +494,8 @@ static void rig_poses_of(const lmot_sensor* rig, int n, RigPoses& R) {
 // F > 1: one frame per sensor stream; the four kernels run over the union of the frames' clusters (blockIdx.y = frame).
 
 int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig,
-                        const lmot_detect_params* det, const unsigned* const* area, const int* search, const float* const* lines) {
+                        const lmot_detect_params* det, const unsigned* const* area, const int* search, const float* const* lines,
+                        const LayerTab* layers) {
   if (F < 1 || F > kMaxBatch) return LMOT_ERR_INVALID;
   const int K1 = c->prm.max_clusters + 1;
   int tiles = 0;
@@ -486,7 +508,11 @@ int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, cons
   bool masked = false;
   FitAreaMasks A{};
   for (int i = 0; area && i < F; ++i) { A.m[i] = area[i]; masked |= area[i] != nullptr; }
-  if (tiles > 0 && masked) tile_hist_area_kernel<<<dim3(tiles, F), kTile, sh, st>>>(B, c->prm.max_clusters, A);
+  if (tiles > 0 && layers) {
+    FitLayers L{};
+    for (int i = 0; i < F; ++i) L.t[i] = layers[i];
+    tile_hist_layers_kernel<<<dim3(tiles, F), kTile, sh, st>>>(B, c->prm.max_clusters, A, L);
+  } else if (tiles > 0 && masked) tile_hist_area_kernel<<<dim3(tiles, F), kTile, sh, st>>>(B, c->prm.max_clusters, A);
   else if (tiles > 0) tile_hist_kernel<<<dim3(tiles, F), kTile, sh, st>>>(B, c->prm.max_clusters);     // + segment offsets by its last CTA per frame
   else seg_offsets_kernel<<<F, 1024, 0, st>>>(B, c->prm.max_clusters);
   kernel_mark(c, s0, st);
@@ -725,12 +751,13 @@ int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const SeqLists& L, int 
   return LMOT_OK;
 }
 
-int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem, const unsigned* area, int search, const float* lines) {
+int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem, const unsigned* area, int search, const float* lines,
+                  const LayerTab* layers) {
   Slot* sl[1] = {s};
   const int nu[1] = {n_upper};
   const unsigned* am[1] = {area};
   return boxfit_launch_batch(c, sl, 1, st, nu, post_sem, nullptr, nullptr, area ? am : nullptr, search > 0 ? &search : nullptr,
-                             lines ? &lines : nullptr);
+                             lines ? &lines : nullptr, layers);
 }
 
 }  // namespace lmot

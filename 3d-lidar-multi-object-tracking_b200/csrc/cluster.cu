@@ -179,6 +179,7 @@ int cluster_alloc(Ctx* c, Slot* s) {
 void cluster_free(Slot* s) {
   cudaFree(s->d_cart); cudaFree(s->d_cart_bits); cudaFree(s->d_label_grid);
   cudaFree(s->d_first_idx); cudaFree(s->d_clustered); cudaFree(s->d_obstacles); cudaFree(s->d_cost_map);
+  cudaFree(s->d_slice); cudaFree(s->d_colmask); cudaFree(s->d_layer_cols); cudaFree(s->d_layer_base); cudaFree(s->d_layer_lab);
 }
 
 // elevated cloud = s->d_elev with its length in d_counters[CNT_N_ELEV]; n_upper bounds that length on the host

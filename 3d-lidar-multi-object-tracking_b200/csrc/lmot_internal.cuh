@@ -238,6 +238,14 @@ struct Slot {
 
   float* d_gz = nullptr;               // [9600] ground heights of the slot's latest frame with ground lines (allocated on first use)
 
+  // ---- layered clustering (layers.cu; allocated on the first layered unit that uses the slot)
+  uint8_t* d_slice = nullptr;          // per point of E its height slice, 0xFF: no column (or outside the detection area)
+  unsigned* d_colmask = nullptr;       // [62500] slices seen per column (layer_mark_kernel), zero at rest
+  unsigned* d_layer_cols = nullptr;    // [62500] occupied slices per column (the runs are the nodes), 0 for an empty column
+  int* d_layer_base = nullptr;         // [62500 + 1] id of each occupied column's first run, then the number of runs
+  int* d_layer_lab = nullptr;          // [62500 * 16] -(cluster id) of every run
+  bool layers_last = false;            // the slot's most recent frame was layered (the label grid does not name its clusters)
+
   struct Result* res = nullptr;       // result block of the frame currently (or last) processed on this slot
 };
 
@@ -337,6 +345,9 @@ inline lmot_box_search box_search_defaults() { lmot_box_search b; b.on = 0; b.n_
 // lmot_default_ground_lines
 inline lmot_ground_lines ground_lines_defaults() { lmot_ground_lines g; g.on = 0; g.max_slope = 0.3; g.max_rmse = 0.08; g.max_step = 0.3; return g; }
 
+// lmot_default_layers
+inline lmot_layers layers_defaults() { lmot_layers l; memset(&l, 0, sizeof(l)); l.on = 0; l.n_slices = 32; l.slice_m = 0.2; l.z_min = -0.5; l.gap_slices = 2; return l; }
+
 // one frame of a launch with ground lines: its stream's setting (nullptr: off) and the grid of ground heights its lines go to
 struct GroundLinesJob { const lmot_ground_lines* cfg; float* gz; };
 
@@ -381,6 +392,7 @@ struct StreamCfg {
   AccHist acc;                              // sweep accumulation and its history (accumulate.cu)
   lmot_box_search search = box_search_defaults();   // box search (box_search.cu)
   lmot_ground_lines lines = ground_lines_defaults(); // ground lines (ground_lines.cuh)
+  lmot_layers layers = layers_defaults();            // layered clustering (layers.cu)
   bool merges() const { return rig_merge && n_sensors > 0; }
   bool masked() const { return area.n_rings > 0; }
   int search_angles() const { return search.on ? search.n_angles : 0; }   // A of the stream's units, 0: boxFitting's fit
@@ -469,6 +481,9 @@ struct Ctx {
   // ---- lmot_debug_ground_lines: the ground grids of the most recent own-stream submission (none: its lines were off)
   const float* gz_dbg[kMaxBatch] = {};
   int n_gz_dbg = 0;
+  // ---- lmot_debug_point_clusters: the units of the most recent own-stream submission (none: it was not layered)
+  const Slot* lay_dbg[kMaxBatch] = {};
+  int n_lay_dbg = 0;
 
   // ---- timing
   bool timing = false;
@@ -548,17 +563,20 @@ int boxfit_alloc_shared(Ctx* c);
 void boxfit_free(Slot* s);
 // search: the frame's box search angle count A (0: boxFitting's fit)
 // lines: the frame's ground grid (ground lines; nullptr: off)
+// layers: the frame's layered run tables (nullptr: its label grid)
+struct LayerTab;
 int boxfit_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool post_sem = false, const unsigned* area = nullptr, int search = 0,
-                  const float* lines = nullptr);
+                  const float* lines = nullptr, const LayerTab* layers = nullptr);
 // rig (nullable): sensor i's sensor_height for frame i (box fitting) / sensor i's pose for list i (concatenation)
 // det (nullable): frame i's own detection values, as ground_launch_batch's; rig is then unused
 // area (nullable): as ccl_launch_batch's
 // search (nullable): frame i's box search angle count A, 0: boxFitting's fit (box_search.cu fits the others)
 // lines (nullable): unit i's ground grid, nullptr for a unit measured from the flat sensor_height; any -> every unit through the ground
 // lines variants (box_fit_lines_kernel, box_search_lines_kernel)
+// layers (nullable): unit i's run tables (slice nullptr: a unit clustered on the label grid); any -> tile_hist_layers_kernel
 int boxfit_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const int* n_upper, bool post_sem, const lmot_sensor* rig = nullptr,
                         const lmot_detect_params* det = nullptr, const unsigned* const* area = nullptr, const int* search = nullptr,
-                        const float* const* lines = nullptr);
+                        const float* const* lines = nullptr, const LayerTab* layers = nullptr);
 // box search (box_search.cu): setting validation, the angle table of A (lmot_box_search_angles), and the device tables of every A
 // (Ctx::d_bs_tab, uploaded once by the first setter that turns the search on)
 bool box_search_valid(const lmot_box_search& b);
@@ -644,5 +662,18 @@ int accumulate_step(Ctx* c, AccHist& h, int kind, int units, Slot* const* U, con
                     const TrackerHost& th, double ts, double v, double yaw, Result* r, AccJob* jobs, int* fit_upper);
 // one launch over the jobs of a submission, behind each accumulating stream's previous launch (hists[0 .. nh)); records their events
 int accumulate_launch(Ctx* c, cudaStream_t st, Slot* mark, const AccJob* jobs, int n_jobs, AccHist* const* hists, int nh);
+// layered clustering (layers.cu).  What box fitting reads of a layered unit: each point's slice, and per column the occupied slices, the
+// id of its first run and the cluster of every run (as -(id))
+struct LayerTab { const uint8_t* slice; const unsigned* cols; const int* base; const int* lab; };
+bool layers_valid(const lmot_layers& l);
+int layers_ensure(Ctx* c, Slot* s, cudaStream_t st);   // the slot's layer buffers, allocated once (column masks zeroed on st)
+LayerTab layer_tab_of(const Slot* s);
+// one layered unit of a submission: its slot (cloud, cells, bit planes, counters, layer buffers), detection-area mask (nullable), setting,
+// box-fitting sensor_height and a bound on |E|
+struct LayerUnit { Slot* s; const unsigned* area; lmot_layers cfg; float sensor_height; int n_upper; };
+// layer_mark_kernel over every unit, then ccl_layer_kernel with one CTA per unit
+int layers_launch(Ctx* c, cudaStream_t st, const LayerUnit* u, int n, Slot* mark);
+// step 6 on the host from the unit's device tables (synchronous): ids[i] for the n points of its cloud
+int layers_point_ids(Ctx* c, const Slot* s, int n, int32_t* ids);
 
 }  // namespace lmot

@@ -972,6 +972,64 @@ int lmot_ground_lines_grid(const lmot_ground_lines* g, const float minz[LMOT_NUM
                            double sensor_height, float gz[LMOT_NUM_CHANNEL * LMOT_NUM_BIN]);
 int lmot_debug_ground_lines(lmot_ctx* ctx, float* gz, int cap_units, int* n_units);
 
+/* ---- layered clustering: connected components over height slices ----------------------------------------------------------------------
+ * componentClustering projects every elevated point onto the 250 x 250 grid and ignores z, so a car under a tree canopy, a pedestrian
+ * under a shelter roof or a car under a sign gantry become one cluster with the structure above them; boxFitting then measures it to the
+ * top of the canopy and the rule filter drops it.  Layered clustering labels connected components over (x, y, height slice) instead, so
+ * that a vertical gap separates objects.
+ *
+ * Definition.  A stream (the context's own: lmot_set_layers; sequence k: lmot_seq_set_layers) with on = 1: each detection unit of a
+ * FRAMES step (a frame without a sensor table, an unmerged rig frame, or a merge unit) with its cloud E (what reaches clustering: after
+ * deskew, the rig merge, accumulation and the detection area), its clustering extent roi and its box-fitting sensor_height (lmot_params',
+ * the sequence's own detection value, sensor j's for an unmerged rig frame, the vehicle's for a merge unit):
+ *   1. column: the column (xI, yI) of a point is componentClustering's float binning with roi; points outside it have none.  N(x, y) is
+ *      the number of points of E in the column;
+ *   2. slice: in double, left to right, without contraction, h = ((double)z + (double)sensor_height) - z_min; s = floor(h / slice_m)
+ *      clamped to [0, S - 1];
+ *   3. seed voxels V = {(x, y, s(p)) : p in E, N(x, y) > 1} (the reference's "more than one point" rule, per column);
+ *   4. occupied voxels O: every (x', y', s') inside the grid and inside [0, S) with |x' - x| <= 1, |y' - y| <= 1, |s' - s| <= g for some
+ *      (x, y, s) in V;
+ *   5. components: the connected parts of O under 26-adjacency (max(|dx|, |dy|, |ds|) = 1), numbered 1.. in the order of each
+ *      component's smallest (x, y, s), x outermost; num_cluster is their number;
+ *   6. cluster of a point: the id of the component holding (x, y, s(p)); 0 when that voxel is not in O or the point has no column;
+ *   7. boxes: box fitting runs as it does without layers on each cluster's points in cloud order -- boxFitting's fit, box search,
+ *      ground-line box heights, the rule filter in both modes, max_clusters and LMOT_ERR_CAPACITY -- and everything behind it
+ *      (concatenation, poses, global frame, tracker, retirement) is unchanged.
+ * With S = 1, step 5 is 8-connected labelling of the 3 x 3 dilation of the seed cells in raster order, i.e. componentClustering: S = 1
+ * reproduces the unlayered pipeline bit for bit.  For any S a unit's boxes equal boxFitting(E_c, grid_c, 1) per cluster c (E_c: c's
+ * points in cloud order, grid_c: their columns labelled 1), accepted boxes in id order.  Slices are measured from the flat
+ * z = -sensor_height also with ground lines on.  Components do not depend on where the slices start except through the clamping at both
+ * ends: two seeds closer than 2g + 2 slices join wherever slice 0 lies, unless clamping moves them together.
+ * Applies to lmot_frame / _submit / _dev, lmot_detect_dev, lmot_batch* including lmot_batch_detect_dev, and the FRAMES steps of
+ * lmot_seq* / lmot_seq_tick*.  Never to the stage entry points (lmot_component_cluster stays the reference), lmot_batch_ground_ccl_dev,
+ * LISTS steps, lmot_track_step*, lmot_seq_track* or lmot_shared_*.
+ * Submission.  Host state captured by value at submission; frames and ticks in flight keep theirs.  lmot_seq_open turns it off for every
+ * sequence; lmot_seq_tracker_reset, _load and LMOT_SEQ_RESTART keep it.  A submission without a layered stream runs exactly the launches,
+ * copies and memsets it ran before layered clustering existed.
+ * Errors.  LMOT_ERR_INVALID, setting unchanged: on not 0 / 1, n_slices outside [1, LMOT_MAX_SLICES], slice_m not finite or <= 0, z_min
+ * not finite, gap_slices outside [0, n_slices - 1], k out of range or no open set.  LMOT_ERR_STATE, nothing submitted: a layered
+ * submission in timing mode.  LMOT_ERR_STATE from lmot_cluster_outputs and lmot_debug_label_grid after a layered own-stream frame: the
+ * 2-D label grid does not name the layered clusters.
+ * Memory.  Each detection slot or merge unit that runs a layered unit allocates, once, its column masks, run tables and a node table for
+ * the worst case of 16 runs in each of the 62,500 columns: about 4.8 MB plus one byte per point of max_points.
+ * lmot_debug_point_clusters(ctx, ids, cap, n_units, n_points): step 6's id of every point of E of every unit of the context's most recent
+ * own-stream submission, unit after unit (n_points[u] points of unit u, in its cloud order); n_units = 0 when it was not layered.
+ * LMOT_ERR_CAPACITY (nothing written) when the ids do not fit in cap.  Synchronises the device. */
+#define LMOT_MAX_SLICES 32
+typedef struct lmot_layers {
+  int on;                      /* 0 (default): componentClustering's 2-D grid; 1: layered components (above) */
+  int n_slices;                /* S = 32, 1 .. LMOT_MAX_SLICES */
+  double slice_m;              /* 0.2: thickness of one slice, metres */
+  double z_min;                /* -0.5: bottom of slice 0, metres above the unit's flat ground z = -sensor_height */
+  int gap_slices;              /* g = 2, 0 .. S - 1: vertical reach of a seed (seeds with at most 2g empty slices between them join) */
+} lmot_layers;
+int lmot_default_layers(lmot_layers* l);
+int lmot_set_layers(lmot_ctx* ctx, const lmot_layers* l);                  /* NULL: the defaults (off) */
+int lmot_get_layers(const lmot_ctx* ctx, lmot_layers* l);
+int lmot_seq_set_layers(lmot_ctx* ctx, int k, const lmot_layers* l);
+int lmot_seq_get_layers(const lmot_ctx* ctx, int k, lmot_layers* l);
+int lmot_debug_point_clusters(lmot_ctx* ctx, int32_t* ids, int cap, int* n_units, int n_points[LMOT_MAX_BATCH]);
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);
