@@ -397,6 +397,43 @@ def _layers(fields: dict) -> Layers:
     return Layers(int(base["on"]), int(base["n_slices"]), float(base["slice_m"]), float(base["z_min"]), int(base["gap_slices"]))
 
 
+class Obstacles(C.Structure):
+    """lmot_obstacles: obstacle footprints of every cluster (include/lmot.h)."""
+    _fields_ = [("on", C.c_int), ("max_vertices", C.c_int)]
+
+
+OBSTACLE_MAX_HULL = 140                # LMOT_OBSTACLE_MAX_HULL
+OBSTACLE_DTYPE = np.dtype([("cluster", np.int32), ("n_points", np.int32), ("n_cells", np.int32), ("box", np.int32),
+                           ("vertex_offset", np.int32), ("vertex_count", np.int32), ("z_min", np.float32), ("z_max", np.float32)])
+
+
+class ObstaclesOut(C.Structure):
+    _fields_ = [("obstacles", C.c_void_p), ("cap_obstacles", C.c_int), ("vertices", C.c_void_p), ("cap_vertices", C.c_int),
+                ("n_units", C.c_int), ("n_obstacles", C.c_int), ("n_vertices", C.c_int)]
+
+
+def default_obstacles() -> dict:
+    lib = load_library()
+    o = Obstacles()
+    lib.lmot_default_obstacles(C.byref(o))
+    return {name: getattr(o, name) for name, _ in Obstacles._fields_}
+
+
+def _obstacles(fields: dict) -> Obstacles:
+    base = default_obstacles()
+    unknown = set(fields) - set(base)
+    if unknown:
+        raise KeyError(f"unknown obstacles fields {sorted(unknown)}")
+    base.update(fields)
+    return Obstacles(int(base["on"]), int(base["max_vertices"]))
+
+
+def obstacle_polygons(res: dict) -> list:
+    """The footprint of every obstacle of an obstacles_result as a float32 [count, 2] array (empty where the pool overflowed)."""
+    v = res["vertices"]
+    return [v[o: o + c] for o, c in zip(res["obstacles"]["vertex_offset"], res["obstacles"]["vertex_count"])]
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -461,6 +498,8 @@ ABI_SYMBOLS = [
     "lmot_default_ground_lines", "lmot_set_ground_lines", "lmot_get_ground_lines", "lmot_seq_set_ground_lines", "lmot_seq_get_ground_lines",
     "lmot_ground_lines_grid", "lmot_debug_ground_lines",
     "lmot_default_layers", "lmot_set_layers", "lmot_get_layers", "lmot_seq_set_layers", "lmot_seq_get_layers", "lmot_debug_point_clusters",
+    "lmot_default_obstacles", "lmot_set_obstacles", "lmot_get_obstacles", "lmot_seq_set_obstacles", "lmot_seq_get_obstacles",
+    "lmot_obstacles_result", "lmot_seq_obstacles_result",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
@@ -1158,6 +1197,54 @@ class Lmot:
         l = Layers()
         self._chk(self.lib.lmot_seq_get_layers(self.h, int(k), C.byref(l)))
         return {name: getattr(l, name) for name, _ in Layers._fields_}
+
+    # ---- obstacle footprints (lmot_set_obstacles) --------------------------------------------------------------------------------
+    def set_obstacles(self, **fields):
+        """The context's frames: obstacle footprint settings with `fields` replaced (on=1 turns them on; no fields: the defaults, off).
+        Applies from the next submission on; frames in flight keep theirs."""
+        self._chk(self.lib.lmot_set_obstacles(self.h, C.byref(_obstacles(fields)) if fields else None))
+
+    def get_obstacles(self) -> dict:
+        o = Obstacles()
+        self._chk(self.lib.lmot_get_obstacles(self.h, C.byref(o)))
+        return {name: getattr(o, name) for name, _ in Obstacles._fields_}
+
+    def seq_set_obstacles(self, k: int, **fields):
+        """Sequence k's FRAMES steps, arguments as set_obstacles."""
+        self._chk(self.lib.lmot_seq_set_obstacles(self.h, int(k), C.byref(_obstacles(fields)) if fields else None))
+
+    def seq_get_obstacles(self, k: int) -> dict:
+        o = Obstacles()
+        self._chk(self.lib.lmot_seq_get_obstacles(self.h, int(k), C.byref(o)))
+        return {name: getattr(o, name) for name, _ in Obstacles._fields_}
+
+    def _obstacles_result(self, call) -> dict:
+        probe = ObstaclesOut()
+        st = call(C.byref(probe))
+        if st not in (OK, ERR_CAPACITY):
+            self._chk(st)
+        rows = np.zeros(max(probe.n_obstacles, 1), OBSTACLE_DTYPE)
+        nv = probe.n_vertices
+        xy = np.zeros((max(nv, 1), 2), np.float32)
+        out = ObstaclesOut(rows.ctypes.data, probe.n_obstacles, xy.ctypes.data, nv, 0, 0, 0)
+        st = call(C.byref(out))
+        if st not in (OK, ERR_CAPACITY):
+            self._chk(st)
+        r = rows[: out.n_obstacles]
+        fit = r["vertex_count"] > 0
+        stored = int((r["vertex_offset"][fit] + r["vertex_count"][fit]).max()) if fit.any() else 0     # the pool's filled part
+        return {"status": st, "n_units": out.n_units, "obstacles": r.copy(), "n_vertices": out.n_vertices,
+                "vertices": xy[:stored].copy()}
+
+    def obstacles_result(self, unit: int = 0) -> dict:
+        """lmot_obstacles_result: unit `unit` of the own-stream result most recently returned.  dict: status (OK, or ERR_CAPACITY when
+        the vertex pool overflowed), n_units, obstacles (OBSTACLE_DTYPE rows in cluster order), n_vertices (needed in all) and
+        vertices (float32 [stored, 2]); obstacle_polygons() cuts them per obstacle."""
+        return self._obstacles_result(lambda o: self.lib.lmot_obstacles_result(self.h, int(unit), o))
+
+    def seq_obstacles_result(self, k: int, unit: int = 0) -> dict:
+        """lmot_seq_obstacles_result: sequence k's step of the tick most recently returned, as obstacles_result."""
+        return self._obstacles_result(lambda o: self.lib.lmot_seq_obstacles_result(self.h, int(k), int(unit), o))
 
     def debug_point_clusters(self) -> list:
         """lmot_debug_point_clusters: one int32 array of per-point cluster ids per unit of the most recent own-stream submission, in

@@ -187,6 +187,7 @@ Result* acquire_result(Ctx* c, bool drop_oldest) {
   c->last_res = r;
   r->merge_rows = 0;                             // only a merging batched tick sets it (batch_common): collect_result reads it
   r->acc_units = 0;                              // only an accumulating step sets it (accumulate_step)
+  r->obs_units = 0;                              // only a step with obstacles on sets it (obstacles_ensure)
   return r;
 }
 
@@ -288,6 +289,10 @@ int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tra
   if ((rc = boxfit_launch(c, s, s->stream, fit_upper, with_tracker && !gf, mask, c->own_cfg.search_angles(), gl ? s->d_gz : nullptr,
                           layered ? &ltab : nullptr))) return rc;   // with_tracker: posts the slot's detection semaphore
   if (gf && (rc = boxes_to_global_launch(c, s, s->stream, s->d_boxes, s->d_counters, ts, v, yaw, true))) return rc;   // ... or this one does
+  if (c->own_cfg.obs.on) {             // obstacle footprints of the frame's clusters into r's obstacle block, behind box fitting
+    const ObsUnit ou{s, c->prm.roi_m, c->own_cfg.obs.max_vertices, r, 0};
+    if ((rc = obstacles_ensure(c, &ou, 1, s->stream)) || (rc = obstacles_launch(c, s->stream, &ou, 1, s))) return rc;
+  }
   if (c->timing) cudaEventRecord(r->ev[3], s->stream);
   LMOT_CUDA(c, cudaEventRecord(s->ev_det_done, s->stream));
   if (with_tracker) {
@@ -591,8 +596,20 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
     if (ncu > 0 && (rc = ccl_launch_batch(c, cu, ncu, st, area ? camask : nullptr))) return rc;
   }
   if (c->timing) cudaEventRecord(r->ev[2], st);
-  return boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr, area, searching ? usearch : nullptr,
-                             lining ? ugz : nullptr, layering ? ltab : nullptr);
+  if ((rc = boxfit_launch_batch(c, U.u, nu, st, unn, post_sem, rig_fit ? U.rig : nullptr, own_det ? udet : nullptr, area, searching ? usearch : nullptr,
+                                lining ? ugz : nullptr, layering ? ltab : nullptr))) return rc;
+  // obstacle footprints: every unit of a stream with obstacles on, in one launch behind box fitting, into its group's result block (unit
+  // i - f0 of the group)
+  ObsUnit ou[kMaxBatch];
+  int no = 0;
+  for (int d = 0; d < G; ++d) {
+    const StreamCfg& q = *g[d].cfg;
+    if (!q.obs.on) continue;
+    const float roi = (q.det_on ? q.det : base).roi_m;
+    for (int i = U.f0[d]; i < U.f0[d + 1]; ++i) ou[no++] = ObsUnit{U.u[i], roi, q.obs.max_vertices, g[d].res, i - U.f0[d]};
+  }
+  if (no > 0 && ((rc = obstacles_ensure(c, ou, no, st)) || (rc = obstacles_launch(c, st, ou, no, bk)))) return rc;
+  return LMOT_OK;
 }
 
 // the IDs of a result being returned (lmot_track_ids): copied now, the block is reused by later submissions
@@ -673,6 +690,10 @@ int collect_result(Ctx* c, Result* r, lmot_frame_out* out, Tracker* trk = nullpt
       }
     }
   }
+  {                                                   // lmot_obstacles_result / lmot_seq_obstacles_result: this result's footprints
+    const int rc = obstacles_collect(c, r, trk ? c->seq_obs_last[trk - c->seq] : c->obs_last);
+    if (rc) return rc;
+  }
   const int err = r->h_hdr[HDR_ERROR];
   const int warn = r->has_tracks ? r->h_hdr[HDR_WARN] : 0;
   if (r->has_tracks) {
@@ -746,6 +767,7 @@ void result_destroy(Result* r) {
   if (r->h_deskew) cudaFreeHost(r->h_deskew);
   if (r->h_area) cudaFreeHost(r->h_area);
   if (r->h_acc) cudaFreeHost(r->h_acc);
+  obstacles_result_free(r);
   if (r->d_ids) cudaFree(r->d_ids);
   if (r->d_block) cudaFree(r->d_block);
   if (r->ev_tc) cudaEventDestroy(r->ev_tc);
@@ -772,6 +794,7 @@ void seq_destroy(Ctx* c) {
     accumulate_free(c->seq_cfg[k].acc);
     c->seq_cfg[k] = StreamCfg{};
     c->seq_acc_info[k] = lmot_accum_info{};
+    c->seq_obs_last[k].valid = false;
     c->seq_fc_n[k] = 0;
   }
   for (int i = 0; i < c->seq_ring; ++i) {
@@ -814,7 +837,7 @@ int seq_collect_tick(Ctx* c, SeqTick* t, lmot_seq_out* out) {
   if (out) out->n_seq = c->n_seq;
   c->seq_stepped = t->stepped;
   for (int k = 0; k < c->n_seq; ++k) {
-    if (!(t->stepped >> k & 1u)) { c->seq_fc_n[k] = 0; continue; }
+    if (!(t->stepped >> k & 1u)) { c->seq_fc_n[k] = 0; c->seq_obs_last[k].valid = false; continue; }
     Result* b = &t->blocks[k];
     const int r = collect_result(c, b, out ? &out->seq[k] : nullptr, &c->seq[k]);
     if (r < 0 ? (rc >= 0) : (rc == LMOT_OK)) rc = r;       // the first error, else the first warning
@@ -1211,7 +1234,8 @@ int lmot_detect_dev(lmot_ctx* ctx, const float* d_points, int n) {
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
-  if ((c->own_cfg.masked() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on) && c->timing) return LMOT_ERR_STATE;
+  if ((c->own_cfg.masked() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on || c->own_cfg.obs.on) && c->timing)
+    return LMOT_ERR_STATE;
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, true);
   LMOT_CUDA(c, cudaEventRecord(s->ev_fork, c->stream));
@@ -1223,7 +1247,8 @@ int lmot_frame_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp
   if (!ctx || n < 0 || (n > 0 && !d_points) || (reinterpret_cast<uintptr_t>(d_points) & 15u)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   const bool dsk = c->own_cfg.deskew.on != 0;
-  if ((dsk || c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on) && c->timing)
+  if ((dsk || c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on ||
+       c->own_cfg.obs.on) && c->timing)
     return LMOT_ERR_STATE;
   if (dsk && c->own_cfg.deskew.time_field != 3) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
   cudaSetDevice(c->device);
@@ -1245,7 +1270,8 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
-  if ((c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on) && c->timing)
+  if ((c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on ||
+       c->own_cfg.obs.on) && c->timing)
     return LMOT_ERR_STATE;
   const bool dsk = c->own_cfg.deskew.on != 0;
   if (dsk) {                           // (validated before anything is submitted: upload_points checks the rest without deskew)
@@ -1355,7 +1381,7 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   const bool dsk = with_tracker && q.deskew.on != 0;                // (lmot_batch_detect_dev has no stamp: never deskewed)
   if (dsk && c->timing) return LMOT_ERR_STATE;
   if (dsk && (host ? stride <= q.deskew.time_field : q.deskew.time_field != 3)) return LMOT_ERR_INVALID;
-  if ((q.merges() || q.masked() || q.search.on || q.lines.on || q.layers.on) && c->timing) return LMOT_ERR_STATE;
+  if ((q.merges() || q.masked() || q.search.on || q.lines.on || q.layers.on || q.obs.on) && c->timing) return LMOT_ERR_STATE;
   if (with_tracker && q.acc.on() && c->timing) return LMOT_ERR_STATE;
   if (host && c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;
   int rc = batch_ensure(c, n_frames);
@@ -1649,6 +1675,7 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
     Result* r = &t->blocks[k];
     r->n_kev = 0; r->has_tracks = true;
     r->acc_units = 0;                  // (an accumulating FRAMES step sets it in detect_front)
+    r->obs_units = 0;                  // (a FRAMES step with obstacles on sets it in detect_front)
     // > 0: the concatenation / pack writes the block's per-frame counts; 0: one frame, counts from the header
     r->batch_frames = (e[k].kind == LMOT_SEQ_LISTS || rigged) ? f0[k + 1] - f0[k] : 0;
     r->merge_rows = merge[k] ? f0[k + 1] - f0[k] : 0;
@@ -2405,6 +2432,71 @@ int lmot_debug_point_clusters(lmot_ctx* ctx, int32_t* ids, int cap, int* n_units
   for (int u = 0, off = 0; u < c->n_lay_dbg; off += n[u], ++u)
     if ((rc = layers_point_ids(c, c->lay_dbg[u], n[u], ids + off))) return rc;
   return LMOT_OK;
+}
+
+// ---- obstacle footprints (obstacles.cu).  Host state, as layered clustering: the launch parameters carry each unit's values; results are
+// read from the host copy collect_result took of the step most recently returned
+int lmot_default_obstacles(lmot_obstacles* o) {
+  if (!o) return LMOT_ERR_INVALID;
+  *o = obstacles_defaults();
+  return LMOT_OK;
+}
+
+static int obstacles_set(lmot_obstacles& dst, const lmot_obstacles* o) {
+  const lmot_obstacles v = o ? *o : obstacles_defaults();
+  if (!obstacles_valid(v)) return LMOT_ERR_INVALID;
+  dst = v;
+  return LMOT_OK;
+}
+
+int lmot_set_obstacles(lmot_ctx* ctx, const lmot_obstacles* o) { return ctx ? obstacles_set(ctx->c.own_cfg.obs, o) : LMOT_ERR_INVALID; }
+
+int lmot_get_obstacles(const lmot_ctx* ctx, lmot_obstacles* o) {
+  if (!ctx || !o) return LMOT_ERR_INVALID;
+  *o = ctx->c.own_cfg.obs;
+  return LMOT_OK;
+}
+
+int lmot_seq_set_obstacles(lmot_ctx* ctx, int k, const lmot_obstacles* o) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  return obstacles_set(ctx->c.seq_cfg[k].obs, o);
+}
+
+int lmot_seq_get_obstacles(const lmot_ctx* ctx, int k, lmot_obstacles* o) {
+  if (!ctx || !o || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  *o = ctx->c.seq_cfg[k].obs;
+  return LMOT_OK;
+}
+
+static int obstacles_out(const ObsLast& L, int unit, lmot_obstacles_out* out) {
+  if (!out || out->cap_obstacles < 0 || out->cap_vertices < 0) return LMOT_ERR_INVALID;
+  if (!L.valid) return LMOT_ERR_STATE;
+  if (unit < 0 || unit >= L.units) return LMOT_ERR_INVALID;
+  out->n_units = L.units;
+  out->n_obstacles = L.n_obs[unit];
+  out->n_vertices = L.n_vert[unit];
+  const int K = L.n_obs[unit], nv = (int)(L.xy[unit].size() / 2);
+  bool short_arr = false;
+  if (out->obstacles) {
+    const int m = K < out->cap_obstacles ? K : out->cap_obstacles;
+    if (m > 0) memcpy(out->obstacles, L.rows[unit].data(), (size_t)m * sizeof(lmot_obstacle));
+    short_arr |= K > out->cap_obstacles;
+  }
+  if (out->vertices) {
+    const int m = nv < out->cap_vertices ? nv : out->cap_vertices;
+    if (m > 0) memcpy(out->vertices, L.xy[unit].data(), (size_t)m * 2 * sizeof(float));
+    short_arr |= nv > out->cap_vertices;
+  }
+  return (short_arr || L.n_vert[unit] > L.max_vertices[unit]) ? LMOT_ERR_CAPACITY : LMOT_OK;
+}
+
+int lmot_obstacles_result(lmot_ctx* ctx, int unit, lmot_obstacles_out* out) {
+  return ctx ? obstacles_out(ctx->c.obs_last, unit, out) : LMOT_ERR_INVALID;
+}
+
+int lmot_seq_obstacles_result(lmot_ctx* ctx, int k, int unit, lmot_obstacles_out* out) {
+  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  return obstacles_out(ctx->c.seq_obs_last[k], unit, out);
 }
 
 // ---- detection areas (detect_area.cu).  Host state only, as the sensor tables; setting one allocates the pinned staging blocks of the

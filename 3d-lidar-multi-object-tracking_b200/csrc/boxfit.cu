@@ -482,6 +482,7 @@ void boxfit_free(Slot* s) {
   cudaFree(s->d_pcid); cudaFree(s->d_table); cudaFree(s->d_seg_start); cudaFree(s->d_seg_size); cudaFree(s->d_sorted_pts);
   cudaFree(s->d_cl_box); cudaFree(s->d_cl_marker); cudaFree(s->d_cl_ok); cudaFree(s->d_boxes); cudaFree(s->d_boxes_g); cudaFree(s->d_markers);
   cudaFree(s->d_done); cudaFree(s->d_det_sem);
+  cudaFree(s->d_obs_hull);                                      // obstacle footprints (obstacles.cu), allocated on first use
 }
 
 static void rig_poses_of(const lmot_sensor* rig, int n, RigPoses& R) {

@@ -161,6 +161,15 @@ struct Result {
   // sensors' (n_elev, n_ground, 0, 0) from rig_merge_kernel, row merge_rows the merged cloud's row from the concatenation; collect
   // moves its num_cluster / n_boxes into row 0 (collect_result)
   int merge_rows = 0;
+  // obstacle footprints (obstacles.cu): h_obs = pinned, device-mapped block of obs_cap_units units (ObsUnit layout, obs_cap_vertices
+  // vertex pairs each), allocated by the first step that needs it; obs_units: the units this block's step reported (0: obstacles off),
+  // ev_obs: recorded behind the obstacle kernel that wrote them
+  unsigned char* h_obs = nullptr;
+  int obs_cap_units = 0, obs_cap_vertices = 0;
+  int obs_units = 0;
+  int obs_max_vertices[kMaxBatch] = {};
+  cudaEvent_t ev_obs = nullptr;
+  bool obs_pending = false;            // an obstacle kernel was recorded into h_obs (the next writer or reallocation waits for ev_obs)
 };
 
 // Detection slot: every buffer the three detection stages (ground -> cluster -> box) touch for ONE frame, plus the
@@ -245,6 +254,9 @@ struct Slot {
   int* d_layer_base = nullptr;         // [62500 + 1] id of each occupied column's first run, then the number of runs
   int* d_layer_lab = nullptr;          // [62500 * 16] -(cluster id) of every run
   bool layers_last = false;            // the slot's most recent frame was layered (the label grid does not name its clusters)
+
+  // ---- obstacle footprints (obstacles.cu; allocated on the first obstacle unit that uses the slot)
+  unsigned char* d_obs_hull = nullptr; // [max_clusters + 1] hull size, then [max_clusters + 1][140] (u, v) corner bytes; + done counter
 
   struct Result* res = nullptr;       // result block of the frame currently (or last) processed on this slot
 };
@@ -345,6 +357,9 @@ inline lmot_box_search box_search_defaults() { lmot_box_search b; b.on = 0; b.n_
 // lmot_default_ground_lines
 inline lmot_ground_lines ground_lines_defaults() { lmot_ground_lines g; g.on = 0; g.max_slope = 0.3; g.max_rmse = 0.08; g.max_step = 0.3; return g; }
 
+// lmot_default_obstacles
+inline lmot_obstacles obstacles_defaults() { lmot_obstacles o; o.on = 0; o.max_vertices = 65536; return o; }
+
 // lmot_default_layers
 inline lmot_layers layers_defaults() { lmot_layers l; memset(&l, 0, sizeof(l)); l.on = 0; l.n_slices = 32; l.slice_m = 0.2; l.z_min = -0.5; l.gap_slices = 2; return l; }
 
@@ -393,10 +408,20 @@ struct StreamCfg {
   lmot_box_search search = box_search_defaults();   // box search (box_search.cu)
   lmot_ground_lines lines = ground_lines_defaults(); // ground lines (ground_lines.cuh)
   lmot_layers layers = layers_defaults();            // layered clustering (layers.cu)
+  lmot_obstacles obs = obstacles_defaults();         // obstacle footprints (obstacles.cu)
   bool merges() const { return rig_merge && n_sensors > 0; }
   bool masked() const { return area.n_rings > 0; }
   int search_angles() const { return search.on ? search.n_angles : 0; }   // A of the stream's units, 0: boxFitting's fit
   const lmot_ground_lines* lines_on() const { return lines.on ? &lines : nullptr; }
+};
+
+// the obstacle footprints of one returned step, copied out of its result block (the block is reused by later submissions)
+struct ObsLast {
+  bool valid = false;                  // false: no step returned yet, or it ran with obstacles off
+  int units = 0;
+  int n_obs[kMaxBatch] = {}, n_vert[kMaxBatch] = {}, max_vertices[kMaxBatch] = {};
+  std::vector<lmot_obstacle> rows[kMaxBatch];
+  std::vector<float> xy[kMaxBatch];
 };
 
 struct Ctx {
@@ -484,6 +509,10 @@ struct Ctx {
   // ---- lmot_debug_point_clusters: the units of the most recent own-stream submission (none: it was not layered)
   const Slot* lay_dbg[kMaxBatch] = {};
   int n_lay_dbg = 0;
+
+  // ---- lmot_obstacles_result / lmot_seq_obstacles_result: host copies of the most recently returned step's footprints
+  ObsLast obs_last;
+  ObsLast seq_obs_last[kMaxBatch];
 
   // ---- timing
   bool timing = false;
@@ -675,5 +704,16 @@ struct LayerUnit { Slot* s; const unsigned* area; lmot_layers cfg; float sensor_
 int layers_launch(Ctx* c, cudaStream_t st, const LayerUnit* u, int n, Slot* mark);
 // step 6 on the host from the unit's device tables (synchronous): ids[i] for the n points of its cloud
 int layers_point_ids(Ctx* c, const Slot* s, int n, int32_t* ids);
+// obstacle footprints (obstacles.cu).  One unit of a submission: its slot (box-fitting buffers), clustering ROI, vertex pool, and where its
+// footprints go: the result block r's unit `slot`
+struct ObsUnit { Slot* s; float roi; int max_vertices; Result* r; int slot; };
+bool obstacles_valid(const lmot_obstacles& o);
+// the units' hull scratch and their blocks' pinned obstacle blocks (allocated or grown once; st: the stream the launch will run on)
+int obstacles_ensure(Ctx* c, const ObsUnit* u, int n, cudaStream_t st);
+// one launch over the n units behind box fitting on st; records each block's ev_obs
+int obstacles_launch(Ctx* c, cudaStream_t st, const ObsUnit* u, int n, Slot* mark);
+// the block's footprints into `dst` (waits for ev_obs); r->obs_units == 0: dst becomes invalid
+int obstacles_collect(Ctx* c, Result* r, ObsLast& dst);
+void obstacles_result_free(Result* r);
 
 }  // namespace lmot

@@ -1030,6 +1030,86 @@ int lmot_seq_set_layers(lmot_ctx* ctx, int k, const lmot_layers* l);
 int lmot_seq_get_layers(const lmot_ctx* ctx, int k, lmot_layers* l);
 int lmot_debug_point_clusters(lmot_ctx* ctx, int32_t* ids, int cap, int* n_units, int n_points[LMOT_MAX_BATCH]);
 
+/* ---- obstacle footprints: every cluster of a step as a convex polygon with its height range ----------------------------------------
+ * Boxes and tracks only ever describe clusters the rule filter accepts (car- and pedestrian-shaped ones).  Trucks, buses, walls, hedges,
+ * barriers and clusters below min_cluster_points leave no trace in them.  With obstacles on, every cluster of a step is also reported as
+ * geometry, so that a planner sees whatever the filter drops.
+ *
+ * Definition.  A stream (the context's own: lmot_set_obstacles; sequence k: lmot_seq_set_obstacles) with on = 1: each detection unit of a
+ * FRAMES step (a frame without a sensor table, an unmerged rig frame, or a merge unit -- the units of layered clustering and accumulation),
+ * numbered from 0 in the step's frame order (a merging rig: its one merge unit):
+ *   clusters    the clusters box fitting received for the unit, with their ids 1..K and in id order (K = min(num_cluster, max_clusters)):
+ *               the 2-D label grid, the area-masked grid, layered point clusters, E_acc with accumulation, a merge unit's vehicle-frame
+ *               cloud.  One obstacle per cluster, including clusters below min_cluster_points and clusters the rule filter rejects;
+ *   cells       the clustering cells (u, v) of the unit's grid (u = floor(250 (x + roi/2) / roi) in componentClustering's float
+ *               arithmetic, the same for v from y) holding at least one of the cluster's points: the point footprint, not the dilated
+ *               label grid;
+ *   footprint   the convex hull of every corner (u or u + 1, v or v + 1) of those cells.  Corners are lattice points, so the hull is exact
+ *               in integer arithmetic.  Vertices counter-clockwise, starting at the corner with the smallest u, then the smallest v; no
+ *               three consecutive vertices collinear; a single cell gives 4.  Vertex (u, v) is reported in metres as
+ *               x = (float)((double)u * roi / 250.0 - roi / 2.0), y likewise from v, with the unit's own roi_m (a sequence's
+ *               lmot_detect_params, else lmot_params').  The frame is the unit's cloud's: the sensor frame, or the vehicle frame for a
+ *               merge unit.  (An unmerged rig frame's boxes are moved into the vehicle frame by its sensor's pose: apply the same pose.)
+ *   z_min/max   float min and max of z over the cluster's points in the unit frame;
+ *   box         the index, in the unit's own box list (lmot_frame_out.boxes; a batched or sequence unit's share of the concatenated list,
+ *               in the unit's order), of the box this cluster produced, or -1 (no box: rejected, or cut by max_boxes).  A consumer that
+ *               skips obstacles with box >= 0 never counts one object twice.
+ * Vertex count.  No convex lattice polygon in [0, 250]^2 has more than LMOT_OBSTACLE_MAX_HULL = 140 vertices.  Its edge vectors are
+ * multiples of distinct primitive vectors (a, b), and sum |a| = 2 width <= 500, sum |b| = 2 height <= 500, so sum (|a| + |b|) <= 1000.
+ * There are 4 primitive vectors with |a| + |b| = 1 and 4 phi(m) with |a| + |b| = m >= 2.  Taking them by increasing m, all of m <= 10 cost
+ * 868 for 128 vectors, and 132 buys at most 12 of the 40 with m = 11: at most 140 edges.  The bound is reached: all 128 vectors of
+ * m <= 10 (width and height 217) plus +-(1,10), +-(10,1), +-(2,9), +-(9,2), +-(3,8), +-(8,3) (33 more each way) close to a polygon of
+ * 140 vertices in [0, 250]^2.  No hull is ever truncated.
+ * Setting.  lmot_obstacles { on, max_vertices }: max_vertices is each unit's vertex pool, LMOT_OBSTACLE_MAX_HULL .. 1 << 24 (65,536).
+ * Vertex offsets run in cluster order; an obstacle whose vertices do not fit whole in the pool keeps its header, and gets the count 0.
+ * Retrieval then returns LMOT_ERR_CAPACITY with the needed total in n_vertices, as lmot_cluster_outputs does.
+ * Applies to lmot_frame / _submit / _dev, lmot_detect_dev, lmot_batch* and the FRAMES steps of lmot_seq* / lmot_seq_tick*.  Never to the
+ * stage entry points (they have lmot_cluster_outputs), lmot_batch_ground_ccl_dev, LISTS steps, lmot_track_step* or lmot_seq_track*.
+ * Submission.  Host state captured at submission; steps in flight keep theirs.  lmot_seq_open turns it off for every sequence;
+ * lmot_seq_tracker_reset, _load and LMOT_SEQ_RESTART keep it.  A submission without a stream that has obstacles on runs exactly the
+ * launches, copies and memsets it ran before obstacles existed.  One launch per submission covers every unit with obstacles on, behind
+ * box fitting on the detection stream; its kernel writes the footprints straight into the result's pinned, device-mapped obstacle block.
+ * Retrieval.  lmot_obstacles_result(ctx, unit, out) reads the result most recently returned for the own stream (lmot_frame,
+ * lmot_frame_collect / _fetch, lmot_batch / _collect / _fetch); lmot_seq_obstacles_result(ctx, k, unit, out) sequence k's step of the
+ * tick most recently returned.  They copy out->n_obstacles rows (cap_obstacles) and the pool's first n_vertices x/y pairs (cap_vertices
+ * pairs); out->n_units is the step's unit count.  NULL arrays ask for the counts only.
+ * Errors.  LMOT_ERR_INVALID, setting unchanged: on not 0 / 1, max_vertices out of range, k out of range or no open set; a unit outside
+ * the step's units.  LMOT_ERR_STATE: an obstacle submission in timing mode (nothing submitted); retrieval without a returned result, or for
+ * a result submitted with obstacles off (a LISTS step, a skipped sequence).  LMOT_ERR_CAPACITY: the pool overflowed (headers intact), or a
+ * caller array is too small (the counts are still returned).
+ * Memory.  Each detection slot or merge unit that runs an obstacle unit allocates, once, a hull scratch of (max_clusters + 1) x (4 + 2 x 140)
+ * bytes plus 16 bytes (1.2 MB at the default max_clusters).  Each result block that receives one allocates, once per unit count and pool
+ * size it needs, units x (32 B x max_clusters + 8 B x max_vertices + 16 B) of pinned host memory (0.64 MB per unit at the defaults);
+ * the host keeps one copy of the most recently returned step per stream. */
+#define LMOT_OBSTACLE_MAX_HULL 140
+typedef struct lmot_obstacles {
+  int on;                      /* 0 (default) / 1 */
+  int max_vertices;            /* 65536: each unit's vertex pool, LMOT_OBSTACLE_MAX_HULL .. 1 << 24 */
+} lmot_obstacles;
+typedef struct lmot_obstacle {
+  int cluster;                 /* cluster id, 1..K */
+  int n_points, n_cells;
+  int box;                     /* index in the unit's box list, or -1 */
+  int vertex_offset, vertex_count;   /* into the unit's vertex array (pairs); count 0 when the pool overflowed */
+  float z_min, z_max;
+} lmot_obstacle;
+typedef struct lmot_obstacles_out {
+  lmot_obstacle* obstacles;    /* nullable, [cap_obstacles] */
+  int cap_obstacles;
+  float* vertices;             /* nullable, [cap_vertices][2] x, y metres */
+  int cap_vertices;
+  int n_units;                 /* out: the step's detection units */
+  int n_obstacles;             /* out: K of the unit */
+  int n_vertices;              /* out: vertices the unit's hulls need in all (pool overflow: more than max_vertices) */
+} lmot_obstacles_out;
+int lmot_default_obstacles(lmot_obstacles* o);
+int lmot_set_obstacles(lmot_ctx* ctx, const lmot_obstacles* o);            /* NULL: the defaults (off) */
+int lmot_get_obstacles(const lmot_ctx* ctx, lmot_obstacles* o);
+int lmot_seq_set_obstacles(lmot_ctx* ctx, int k, const lmot_obstacles* o);
+int lmot_seq_get_obstacles(const lmot_ctx* ctx, int k, lmot_obstacles* o);
+int lmot_obstacles_result(lmot_ctx* ctx, int unit, lmot_obstacles_out* out);
+int lmot_seq_obstacles_result(lmot_ctx* ctx, int k, int unit, lmot_obstacles_out* out);
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);

@@ -22,5 +22,6 @@ timeout 600 python scripts/rig_merge_measure.py > measure_out/${T}_rig_merge.txt
 timeout 600 python scripts/box_search_measure.py > measure_out/${T}_box_search.txt 2>&1; tail -3 measure_out/${T}_box_search.txt
 timeout 600 python scripts/ground_lines_measure.py > measure_out/${T}_ground_lines.txt 2>&1; tail -3 measure_out/${T}_ground_lines.txt
 timeout 900 python scripts/layers_measure.py > measure_out/${T}_layers.txt 2>&1; tail -3 measure_out/${T}_layers.txt
+timeout 900 python scripts/obstacles_measure.py > measure_out/${T}_obstacles.txt 2>&1; tail -3 measure_out/${T}_obstacles.txt
 timeout 300 python scripts/diag_timeline.py ${T}_timeline > measure_out/${T}_timeline.txt 2>&1; tail -5 measure_out/${T}_timeline.txt
 ls -la measure_out/${T}*
