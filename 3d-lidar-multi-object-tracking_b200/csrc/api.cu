@@ -102,31 +102,6 @@ int deskew_stage_host(Ctx* c, Slot* s, cudaStream_t st, const float* points, int
   return LMOT_OK;
 }
 
-// a single-stream frame (lmot_frame*): its table from the context's own fold (no mount) into r's pinned block, copied to the slot's
-// table; the frame's records d_raw (stride floats each) deskewed into the slot's point buffer, all on the slot stream
-int deskew_frame(Ctx* c, Slot* s, Result* r, const float* d_raw, int n, int stride, double ts, double v, double yaw) {
-  if (n == 0) return LMOT_OK;
-  const lmot_deskew& d = c->own_cfg.deskew;
-  deskew_table(d, std::isfinite(v) ? v : 0.0, deskew_omega(c->own.th, ts, v, yaw), nullptr, r->h_deskew);
-  LMOT_CUDA(c, cudaMemcpyAsync(s->d_deskew, r->h_deskew, kDeskewTabBytes, cudaMemcpyHostToDevice, s->stream));
-  const DeskewJob j{d_raw, s->d_points, s->d_deskew, n, stride, d};
-  return deskew_launch(c, s->stream, &j, 1);
-}
-
-// a single-stream frame with the context's detection area: the area into r's pinned block, one copy to the slot's staging, the slot's
-// cell mask (identity pose, lmot_params.roi_m), all on the slot stream
-int area_frame(Ctx* c, Slot* s, Result* r) {
-  int rc;
-  if ((rc = area_ensure(c, s, 1))) return rc;
-  *r->h_area = c->own_cfg.area;
-  LMOT_CUDA(c, cudaMemcpyAsync(s->d_area, r->h_area, sizeof(AreaBlock), cudaMemcpyHostToDevice, s->stream));
-  AreaJob j{s->d_area, s->d_area_mask, {}, c->prm.roi_m};
-  lmot_sensor id;
-  lmot_default_sensor(&c->prm, &id);
-  memcpy(j.pose, id.pose, sizeof(j.pose));
-  return area_launch(c, s->stream, &j, 1);
-}
-
 int fetch_counters(Ctx* c, Slot* s, cudaStream_t st) {
   LMOT_CUDA(c, cudaMemcpyAsync(s->h_counters, s->d_counters, CNT_COUNT * sizeof(int), cudaMemcpyDeviceToHost, st));
   LMOT_CUDA(c, cudaStreamSynchronize(st));
@@ -222,93 +197,6 @@ int lines_ensure(Ctx* c, Slot* s) {
   return LMOT_OK;
 }
 
-// the asynchronous frame: detection on the slot stream, tracker on the tracker stream
-int submit(Ctx* c, Slot* s, Result* r, const float4* d_pts, int n, bool with_tracker, double ts, double v, double yaw) {
-  int rc;
-  struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
-  s->res = r;
-  r->n_kev = 0;
-  r->batch_frames = 0;
-  // the slot's previous boxes / counters must have been consumed by the tracker
-  LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_trk_done, 0));
-  // sweep accumulation: the frame's candidate sweeps from the stream's history into r and the launch's job (the ring on first use);
-  // fit_upper bounds |E_acc| for the launches behind accumulate_kernel
-  AccHist& h = c->own_cfg.acc;
-  const bool acc = with_tracker && h.on();
-  AccJob aj;
-  int fit_upper = n;
-  if (acc) {
-    lmot_sensor id;
-    lmot_default_sensor(&c->prm, &id);
-    Slot* us[1] = {s};
-    const float roi = c->prm.roi_m;
-    if ((rc = accumulate_step(c, h, ACC_FRAME, 1, us, &id, &roi, &n, c->own.th, ts, v, yaw, r, &aj, &fit_upper))) return rc;
-  }
-  // detection area: the slot's cell mask first; clustering then runs as its own launch, masked, and box fitting skips masked points
-  const bool masked = c->own_cfg.masked();
-  if (masked && (rc = area_frame(c, s, r))) return rc;        // (allocates the slot's mask on first use)
-  const unsigned* mask = masked ? s->d_area_mask : nullptr;
-  s->area_last = masked;
-  c->n_area_dbg = masked ? 1 : 0;
-  c->area_dbg[0] = mask;
-  // layered clustering: the slot's layer buffers; clustering then runs as its own launch, layered, and box fitting reads its run tables
-  const bool layered = c->own_cfg.layers.on != 0;
-  LayerTab ltab{};
-  if (layered) {
-    if ((rc = layers_ensure(c, s, s->stream))) return rc;
-    ltab = layer_tab_of(s);
-  }
-  s->layers_last = layered;
-  c->n_lay_dbg = layered ? 1 : 0;
-  c->lay_dbg[0] = s;
-  const bool fuse = c->fuse_ccl && !masked && !acc && !layered;
-  // ground lines: the ground kernel's lines variant writes the slot's ground grid, box fitting measures each cluster from it
-  const lmot_ground_lines* gl = c->own_cfg.lines_on();
-  if (gl && (rc = lines_ensure(c, s))) return rc;
-  c->n_gz_dbg = gl ? 1 : 0;
-  c->gz_dbg[0] = s->d_gz;
-  if (c->timing) cudaEventRecord(r->ev[0], s->stream);
-  if (gl) {
-    Slot* sl[1] = {s};
-    const float4* pp[1] = {d_pts};
-    const int nn[1] = {n};
-    const GroundLinesJob lj{gl, s->d_gz};
-    if ((rc = ground_launch_batch(c, sl, 1, pp, nn, s->stream, true, false, fuse, false, nullptr, nullptr, &lj))) return rc;
-  } else if ((rc = ground_launch(c, s, s->stream, d_pts, n, true, false, fuse))) return rc;
-  if (c->timing) cudaEventRecord(r->ev[1], s->stream);
-  AccHist* hp = &h;
-  if (acc && (rc = accumulate_launch(c, s->stream, s, &aj, 1, &hp, 1))) return rc;     // E_t into the ring, the earlier sweeps behind it
-  if (layered) {
-    const LayerUnit lu{s, mask, c->own_cfg.layers, c->prm.sensor_height, fit_upper};
-    if ((rc = layers_launch(c, s->stream, &lu, 1, s))) return rc;
-  } else if (!fuse && (rc = cluster_launch(c, s, s->stream, fit_upper, true, mask))) {     // (fused: the ground kernel's last CTA did it)
-    return rc;
-  }
-  if (c->timing) cudaEventRecord(r->ev[2], s->stream);
-  const bool gf = with_tracker && c->prm.global_frame;
-  if ((rc = boxfit_launch(c, s, s->stream, fit_upper, with_tracker && !gf, mask, c->own_cfg.search_angles(), gl ? s->d_gz : nullptr,
-                          layered ? &ltab : nullptr))) return rc;   // with_tracker: posts the slot's detection semaphore
-  if (gf && (rc = boxes_to_global_launch(c, s, s->stream, s->d_boxes, s->d_counters, ts, v, yaw, true))) return rc;   // ... or this one does
-  if (c->own_cfg.obs.on) {             // obstacle footprints of the frame's clusters into r's obstacle block, behind box fitting
-    const ObsUnit ou{s, c->prm.roi_m, c->own_cfg.obs.max_vertices, r, 0};
-    if ((rc = obstacles_ensure(c, &ou, 1, s->stream)) || (rc = obstacles_launch(c, s->stream, &ou, 1, s))) return rc;
-  }
-  if (c->timing) cudaEventRecord(r->ev[3], s->stream);
-  LMOT_CUDA(c, cudaEventRecord(s->ev_det_done, s->stream));
-  if (with_tracker) {
-    if ((rc = submit_tracker(c, s, r, s->d_boxes, s->d_counters, ts, v, yaw))) return rc;
-  } else {
-    // no spawn_output_kernel will snapshot the counters / boxes: copy them before the slot is reused
-    LMOT_CUDA(c, cudaMemcpyAsync(r->h_det, s->d_counters, CNT_COUNT * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-    if ((rc = boxes_publish(c, s, r, s->stream))) return rc;
-    LMOT_CUDA(c, cudaEventRecord(s->ev_trk_done, s->stream));
-    LMOT_CUDA(c, cudaEventRecord(r->ev_done, s->stream));
-  }
-  r->has_tracks = with_tracker;
-  if (!r->in_flight) { r->in_flight = true; ++c->n_in_flight; }
-  return LMOT_OK;
-}
-
 // ---- batched ticks: F sensor streams, one frame each, ONE track table (BASELINE.json configs[3]) -------------------------
 // Their own detection slots (allocated on first use, two banks of F so that the detection of tick t+1 overlaps the tracker of
 // tick t); a bank's kernels all run on its first slot's stream.  `bank` is a pseudo-slot: the concatenated box list, its
@@ -329,6 +217,7 @@ int bank_ensure(Ctx* c) {
     LMOT_CUDA(c, cudaMalloc(&k->d_det_sem, sizeof(int)));
     LMOT_CUDA(c, cudaMemset(k->d_det_sem, 0, sizeof(int)));
     LMOT_CUDA(c, cudaMalloc(&k->d_deskew, kMaxBatch * kDeskewTabBytes));
+    LMOT_CUDA(c, cudaMalloc(&k->d_area, kMaxBatch * sizeof(AreaBlock)));
     LMOT_CUDA(c, cudaEventCreateWithFlags(&k->ev_det_done, cudaEventDisableTiming));
     LMOT_CUDA(c, cudaEventCreateWithFlags(&k->ev_trk_done, cudaEventDisableTiming));
     LMOT_CUDA(c, cudaEventCreateWithFlags(&k->ev_fork, cudaEventDisableTiming));
@@ -389,9 +278,10 @@ int merge_ensure(Ctx* c, Slot* units, int index) {
   return rc;
 }
 
-// ---- the detection front end of batched and sequence ticks: frames -> box-fitted units ---------------------------------------------
-// A tick's frames come in groups, one per stream: a batched tick is one group (the context's own settings and fold), a sequence tick
-// has one per FRAMES sequence.  Frame j of a group is its sensor j's.
+// ---- the detection front end: frames -> box-fitted units ---------------------------------------------------------------------------
+// A submission's frames come in groups, one per stream: a single-stream frame (lmot_frame*, lmot_detect_dev) and a batched tick are one
+// group (the context's own settings and fold), a sequence tick has one per FRAMES sequence.  Frame j of a group of sensors is its sensor
+// j's; a single-stream frame ignores the stream's sensor table.
 struct DetGroup {
   StreamCfg* cfg;                      // the stream's settings and merge units
   const TrackerHost* th;               // the fold the frames' motion is taken from (nullptr: frames without a stamp, never deskewed)
@@ -401,6 +291,9 @@ struct DetGroup {
   double ts, v, yaw;
   int* fc;                             // device view of the stream's per-frame counts in its result block (nullptr: none are written)
   Result* res = nullptr;               // the stream's result block (sweep accumulation: its candidates and count rows)
+  bool sensors = false;                // the frames are the stream's sensors: its sensor table and merging apply
+  bool tab() const { return sensors && cfg->n_sensors > 0; }
+  bool merges() const { return sensors && cfg->merges(); }
 };
 
 // what the front end box-fitted, by group: group g's units are u[f0[g] .. f0[g + 1]) (its frames, or its merge unit), unit i with pose
@@ -413,35 +306,37 @@ struct DetUnits {
   int* fc[kMaxBatch];
 };
 
-// G groups of frames on bank b's detection slots, in group order, all on the first slot's stream, for the bank's result block
-// (bank[b].res): staging (host frames uploaded, device frames read in place), deskew (tables into the pinned block h_dsk, one copy, one
-// launch), ground removal, the merging groups' elevated clouds into their merge units, clustering, box fitting.  post_sem: every unit's
-// last box-fitting CTA posts the unit's semaphore (nothing concatenates its list).
-//   Ground removal gets the tick's pose table iff some group has a sensor table, box fitting iff some unit is an unmerged frame of such
-// a group (a frame without a table: lmot_default_sensor); both get per-frame detection values iff some group has its own (sensor values
-// folded in).  A merge unit is the vehicle's cloud: identity pose, the group's detection values without a sensor's, at most max_points
-// points.  Clustering runs in the ground kernel's tail (fuse_ccl) unless a group merges in between.
+// G groups of frames on the consecutive detection slots fr[0 ..], in group order, all on stream st, for the staging slot's result block
+// (stage->res).  The staging slot holds the deskew tables and area blocks the launches read and records the kernel events: a batch
+// bank's pseudo-slot (bank b: its merge units), or a single-stream frame's own slot.  Staging (host frames uploaded, device frames read
+// in place), deskew (tables into the pinned block h_dsk, one copy, one launch), ground removal, the merging groups' elevated clouds into
+// their merge units, clustering, box fitting.  post_sem: every unit's last box-fitting CTA posts the unit's semaphore (nothing
+// concatenates its list).
+//   Ground removal gets the submission's pose table iff some group has a sensor table, box fitting iff some unit is an unmerged frame of
+// such a group (a frame without a table: lmot_default_sensor); both get per-frame detection values iff some group has its own (sensor
+// values folded in).  A merge unit is the vehicle's cloud: identity pose, the group's detection values without a sensor's, at most
+// max_points points.  Clustering runs in the ground kernel's tail (fuse_ccl) unless a group masks, accumulates, layers or merges.  With
+// one frame and nothing but the plain path on, these are the launches of the frame pipeline (F == 1 variants).
 //   Detection areas: a group whose stream has one stages it into the pinned block h_area[i] (i-th masked group) -- one copy, one launch for
 // every masked unit's cell mask (unit pose: the merge unit's identity, else U.rig); clustering then runs as its own launch, and the
 // masked units cluster and box-fit through the masking kernel variants.
-int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host, float* h_dsk, AreaBlock* h_area, bool post_sem, DetUnits& U) {
+int detect_front(Ctx* c, Slot* stage, Slot* fr, cudaStream_t st, int b, const DetGroup* g, int G, int stride, bool host, float* h_dsk,
+                 AreaBlock* h_area, bool post_sem, DetUnits& U) {
   int rc;
-  Slot* bk = &c->bank[b];
   Slot* sl[kMaxBatch];
   const float4* pp[kMaxBatch];
   int nn[kMaxBatch], F = 0, nj = 0;
   lmot_sensor rig[kMaxBatch];
   DeskewJob dj[kMaxBatch];
   bool rigged = false, own_det = false, merging = false;
-  cudaStream_t st = c->bslots[b * c->batch_frames].stream;
-  c->bslots[b * c->batch_frames].res = bk->res;      // (kernel_mark)
+  fr[0].res = stage->res;              // (kernel_mark)
   for (int d = 0; d < G; ++d) {
     const StreamCfg& q = *g[d].cfg;
-    const bool tab = q.n_sensors > 0, dsk = g[d].th && q.deskew.on;
-    rigged |= tab; own_det |= q.det_on; merging |= q.merges();
+    const bool tab = g[d].tab(), dsk = q.deskews(g[d].th != nullptr);
+    rigged |= tab; own_det |= q.det_on; merging |= g[d].merges();
     const double om = dsk ? deskew_omega(*g[d].th, g[d].ts, g[d].v, g[d].yaw) : 0.0, vv = std::isfinite(g[d].v) ? g[d].v : 0.0;
     for (int j = 0; j < g[d].nf; ++j, ++F) {
-      Slot* s = sl[F] = &c->bslots[b * c->batch_frames + F];
+      Slot* s = sl[F] = &fr[F];
       nn[F] = g[d].n[j];
       if (tab) rig[F] = q.sensors[j];
       else lmot_default_sensor(&c->prm, &rig[F]);
@@ -450,7 +345,7 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
         const float* raw = g[d].data[j];
         if (host && (rc = deskew_stage_host(c, s, st, g[d].data[j], nn[F], stride, &raw))) return rc;
         deskew_table(q.deskew, vv, om, tab ? &q.sensors[j] : nullptr, h_dsk + (size_t)F * kDeskewTab);
-        dj[nj++] = DeskewJob{raw, s->d_points, bk->d_deskew + (size_t)F * kDeskewTab, nn[F], host ? stride : 4, q.deskew};
+        if (nn[F] > 0) dj[nj++] = DeskewJob{raw, s->d_points, stage->d_deskew + (size_t)F * kDeskewTab, nn[F], host ? stride : 4, q.deskew};
       } else if (host) {
         if ((rc = upload_points(c, s, st, g[d].data[j], nn[F], stride, s->d_points))) return rc;
       } else {
@@ -458,8 +353,8 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
       }
     }
   }
-  if (nj > 0) {                        // frame i's table at table i of the bank
-    LMOT_CUDA(c, cudaMemcpyAsync(bk->d_deskew, h_dsk, (size_t)F * kDeskewTabBytes, cudaMemcpyHostToDevice, st));
+  if (nj > 0) {                        // frame i's table at table i of the staging slot
+    LMOT_CUDA(c, cudaMemcpyAsync(stage->d_deskew, h_dsk, (size_t)F * kDeskewTabBytes, cudaMemcpyHostToDevice, st));
     if ((rc = deskew_launch(c, st, dj, nj))) return rc;
   }
   // per-frame detection values and the units (copied into the launch parameters: later setting changes leave this tick alone)
@@ -478,15 +373,15 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
     if (own_det)
       for (int i = i0; i < i0 + g[d].nf; ++i) {
         det[i] = vd;
-        if (q.n_sensors > 0) {
+        if (g[d].tab()) {
           const lmot_sensor& s = rig[i];
           det[i].h_sensor = s.h_sensor; det[i].t_hmin = s.t_hmin; det[i].t_hmax = s.t_hmax; det[i].sensor_height = s.sensor_height;
         }
       }
     U.f0[d] = nu;
-    U.rig_on[d] = q.n_sensors > 0 && !q.merges();
+    U.rig_on[d] = g[d].tab() && !g[d].merges();
     U.fc[d] = g[d].fc;
-    if (q.merges()) {
+    if (g[d].merges()) {
       long long tot = 0;
       for (int i = i0; i < i0 + g[d].nf; ++i) { src[nsrc] = sl[i]; mpose[nsrc] = rig[i]; mn[nsrc] = nn[i]; ++nsrc; tot += nn[i]; }
       mu[nm] = &q.merge_unit[b]; mfc[nm] = g[d].fc; mroi[nm] = vd.roi_m;
@@ -509,19 +404,19 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
   for (int d = 0; d < G; ++d) {
     const StreamCfg& q = *g[d].cfg;
     if (!q.masked()) continue;
-    if ((rc = area_ensure(c, bk, kMaxBatch))) return rc;
+    if ((rc = area_ensure(c, stage, G))) return rc;        // (a bank's kMaxBatch blocks come with it: bank_ensure)
     h_area[nblk] = q.area;
     const float roi = (q.det_on ? q.det : base).roi_m;
     for (int i = U.f0[d]; i < U.f0[d + 1]; ++i) {
       if ((rc = area_ensure(c, U.u[i], 0))) return rc;
-      aj[na] = AreaJob{bk->d_area + nblk, U.u[i]->d_area_mask, {}, roi};
+      aj[na] = AreaJob{stage->d_area + nblk, U.u[i]->d_area_mask, {}, roi};
       memcpy(aj[na++].pose, U.rig[i].pose, sizeof(aj[0].pose));
       amask[i] = U.u[i]->d_area_mask;
     }
     ++nblk;
   }
   if (nblk > 0) {
-    LMOT_CUDA(c, cudaMemcpyAsync(bk->d_area, h_area, (size_t)nblk * sizeof(AreaBlock), cudaMemcpyHostToDevice, st));
+    LMOT_CUDA(c, cudaMemcpyAsync(stage->d_area, h_area, (size_t)nblk * sizeof(AreaBlock), cudaMemcpyHostToDevice, st));
     if ((rc = area_launch(c, st, aj, na))) return rc;
   }
   const unsigned* const* area = nblk > 0 ? amask : nullptr;
@@ -534,7 +429,7 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
     StreamCfg& q = *g[d].cfg;
     if (!g[d].th || !q.acc.on()) continue;
     const int u0 = U.f0[d], nu_d = U.f0[d + 1] - u0;
-    const int kind = q.merges() ? ACC_MERGE : q.n_sensors > 0 ? ACC_RIG : ACC_FRAME;
+    const int kind = g[d].merges() ? ACC_MERGE : g[d].tab() ? ACC_RIG : ACC_FRAME;
     const float roi = (q.det_on ? q.det : base).roi_m;
     float rois[kMaxBatch];
     for (int i = 0; i < nu_d; ++i) rois[i] = roi;
@@ -573,7 +468,7 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
       if (gl && (rc = lines_ensure(c, sl[i]))) return rc;
       lj[i] = GroundLinesJob{gl, sl[i]->d_gz};
     }
-    if (gl && !g[d].cfg->merges())
+    if (gl && !g[d].merges())
       for (int i = U.f0[d]; i < U.f0[d + 1]; ++i) ugz[i] = U.u[i]->d_gz;
     lining |= gl != nullptr;
   }
@@ -582,17 +477,17 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
   bool searching = false;
   for (int d = 0; d < G; ++d)
     for (int i = U.f0[d]; i < U.f0[d + 1]; ++i) { usearch[i] = g[d].cfg->search_angles(); searching |= usearch[i] > 0; }
-  Result* r = bk->res;
+  Result* r = stage->res;
   if (c->timing) cudaEventRecord(r->ev[0], st);
   if ((rc = ground_launch_batch(c, sl, F, pp, nn, st, true, false, fuse, false, rigged ? rig : nullptr, own_det ? det : nullptr,
                                 lining ? lj : nullptr))) return rc;
   if (c->timing) cudaEventRecord(r->ev[1], st);
   if (nm > 0 && (rc = rig_merge_launch(c, st, src, mpose, mn, nm, ms0, mu, mfc, mroi))) return rc;
-  if (nacj > 0 && (rc = accumulate_launch(c, st, bk, acj, nacj, ach, nach))) return rc;
+  if (nacj > 0 && (rc = accumulate_launch(c, st, stage, acj, nacj, ach, nach))) return rc;
   if (!layering) {
     if (!fuse && (rc = ccl_launch_batch(c, U.u, nu, st, area))) return rc;
   } else {
-    if ((rc = layers_launch(c, st, lu, nl, bk))) return rc;
+    if ((rc = layers_launch(c, st, lu, nl, stage))) return rc;
     if (ncu > 0 && (rc = ccl_launch_batch(c, cu, ncu, st, area ? camask : nullptr))) return rc;
   }
   if (c->timing) cudaEventRecord(r->ev[2], st);
@@ -608,7 +503,57 @@ int detect_front(Ctx* c, int b, const DetGroup* g, int G, int stride, bool host,
     const float roi = (q.det_on ? q.det : base).roi_m;
     for (int i = U.f0[d]; i < U.f0[d + 1]; ++i) ou[no++] = ObsUnit{U.u[i], roi, q.obs.max_vertices, g[d].res, i - U.f0[d]};
   }
-  if (no > 0 && ((rc = obstacles_ensure(c, ou, no, st)) || (rc = obstacles_launch(c, st, ou, no, bk)))) return rc;
+  if (no > 0 && ((rc = obstacles_ensure(c, ou, no, st)) || (rc = obstacles_launch(c, st, ou, no, stage)))) return rc;
+  return LMOT_OK;
+}
+
+// what the debug getters read of the most recent own-stream submission: its units' cell masks and layer tables, its frames' ground grids
+// (none where the setting was off), and the units' area_last / layers_last (lmot_cluster_outputs, lmot_debug_label_grid)
+void own_debug_note(Ctx* c, Slot* fr, int nf, const DetUnits& U) {
+  const StreamCfg& q = c->own_cfg;
+  const int nu = U.f0[1];
+  c->n_area_dbg = q.masked() ? nu : 0;
+  c->n_lay_dbg = q.layers.on ? nu : 0;
+  c->n_gz_dbg = q.lines.on ? nf : 0;
+  for (int i = 0; i < nu; ++i) {
+    c->area_dbg[i] = U.u[i]->d_area_mask;
+    c->lay_dbg[i] = U.u[i];
+    U.u[i]->area_last = q.masked();
+    U.u[i]->layers_last = q.layers.on != 0;
+  }
+  for (int i = 0; i < nf; ++i) c->gz_dbg[i] = fr[i].d_gz;
+}
+
+// the asynchronous single-stream frame: the detection front end on the frame's slot (its staging slot and only frame, on its stream),
+// then the tracker on the tracker stream.  points: n host records of `stride` floats (host), or a device float4 frame
+int submit(Ctx* c, Slot* s, Result* r, const float* points, int n, int stride, bool host, bool with_tracker, double ts, double v, double yaw) {
+  int rc;
+  struct Tail { Ctx* c; double t0; ~Tail() { c->host_ns[0] += now_ns() - t0; } } tail{c, now_ns()};
+  s->res = r;
+  r->n_kev = 0;
+  r->batch_frames = 0;
+  // the slot's previous boxes / counters must have been consumed by the tracker
+  LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_trk_done, 0));
+  const bool gf = with_tracker && c->prm.global_frame;
+  const DetGroup g{&c->own_cfg, with_tracker ? &c->own.th : nullptr, &points, &n, 1, ts, v, yaw, nullptr, r, false};
+  DetUnits U;
+  // with_tracker: the slot's last box-fitting CTA posts its detection semaphore (global_frame: boxes_to_global_kernel does)
+  if ((rc = detect_front(c, s, s, s->stream, 0, &g, 1, stride, host, r->h_deskew, r->h_area, with_tracker && !gf, U))) return rc;
+  own_debug_note(c, s, 1, U);
+  if (gf && (rc = boxes_to_global_launch(c, s, s->stream, s->d_boxes, s->d_counters, ts, v, yaw, true))) return rc;
+  if (c->timing) cudaEventRecord(r->ev[3], s->stream);
+  LMOT_CUDA(c, cudaEventRecord(s->ev_det_done, s->stream));
+  if (with_tracker) {
+    if ((rc = submit_tracker(c, s, r, s->d_boxes, s->d_counters, ts, v, yaw))) return rc;
+  } else {
+    // no spawn_output_kernel will snapshot the counters / boxes: copy them before the slot is reused
+    LMOT_CUDA(c, cudaMemcpyAsync(r->h_det, s->d_counters, CNT_COUNT * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+    if ((rc = boxes_publish(c, s, r, s->stream))) return rc;
+    LMOT_CUDA(c, cudaEventRecord(s->ev_trk_done, s->stream));
+    LMOT_CUDA(c, cudaEventRecord(r->ev_done, s->stream));
+  }
+  r->has_tracks = with_tracker;
+  if (!r->in_flight) { r->in_flight = true; ++c->n_in_flight; }
   return LMOT_OK;
 }
 
@@ -1234,49 +1179,36 @@ int lmot_detect_dev(lmot_ctx* ctx, const float* d_points, int n) {
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
-  if ((c->own_cfg.masked() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on || c->own_cfg.obs.on) && c->timing)
-    return LMOT_ERR_STATE;
+  if (c->own_cfg.beyond_plain(false, false) && c->timing) return LMOT_ERR_STATE;
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, true);
   LMOT_CUDA(c, cudaEventRecord(s->ev_fork, c->stream));
   LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_fork, 0));
-  return submit(c, s, r, reinterpret_cast<const float4*>(d_points), n, false, 0, 0, 0);
+  return submit(c, s, r, d_points, n, 4, false, false, 0, 0, 0);
 }
 
 int lmot_frame_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp_us, double v_gps, double yaw_gps) {
   if (!ctx || n < 0 || (n > 0 && !d_points) || (reinterpret_cast<uintptr_t>(d_points) & 15u)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  const bool dsk = c->own_cfg.deskew.on != 0;
-  if ((dsk || c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on ||
-       c->own_cfg.obs.on) && c->timing)
-    return LMOT_ERR_STATE;
-  if (dsk && c->own_cfg.deskew.time_field != 3) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
+  if (c->own_cfg.beyond_plain(true, false) && c->timing) return LMOT_ERR_STATE;
+  if (!c->own_cfg.deskew_fits(true, 4)) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, true);
   LMOT_CUDA(c, cudaEventRecord(s->ev_fork, c->stream));          // the caller's stream produced d_points
   LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_fork, 0));
-  if (dsk) {                           // one extra pass: the caller's frame, deskewed, into the slot's own point buffer
-    LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_trk_done, 0));
-    int rc = deskew_frame(c, s, r, d_points, n, 4, timestamp_us, v_gps, yaw_gps);
-    if (rc) return rc;
-    return submit(c, s, r, s->d_points, n, true, timestamp_us, v_gps, yaw_gps);
-  }
-  return submit(c, s, r, reinterpret_cast<const float4*>(d_points), n, true, timestamp_us, v_gps, yaw_gps);
+  return submit(c, s, r, d_points, n, 4, false, true, timestamp_us, v_gps, yaw_gps);
 }
 
 int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, double timestamp_us, double v_gps, double yaw_gps) {
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
-  if ((c->own_cfg.masked() || c->own_cfg.acc.on() || c->own_cfg.search.on || c->own_cfg.lines.on || c->own_cfg.layers.on ||
-       c->own_cfg.obs.on) && c->timing)
-    return LMOT_ERR_STATE;
-  const bool dsk = c->own_cfg.deskew.on != 0;
+  if (c->own_cfg.beyond_plain(true, false) && c->timing) return LMOT_ERR_STATE;
+  const bool dsk = c->own_cfg.deskews(true);
   if (dsk) {                           // (validated before anything is submitted: upload_points checks the rest without deskew)
-    if (c->timing) return LMOT_ERR_STATE;
-    if (n < 0 || (n > 0 && !points) || stride <= c->own_cfg.deskew.time_field) return LMOT_ERR_INVALID;
+    if (n < 0 || (n > 0 && !points) || !c->own_cfg.deskew_fits(true, stride)) return LMOT_ERR_INVALID;
     if (n > c->max_points) return LMOT_ERR_CAPACITY;
   }
   if (c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;    // result ring full: collect first
@@ -1295,19 +1227,10 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   if (!dsk && c->zero_copy && stride == 4 && n > 0 && n <= c->max_points && (reinterpret_cast<uintptr_t>(points) & 15u) == 0 && ground_reads_input_once(c, n)) {
     cudaPointerAttributes pa;
     if (cudaPointerGetAttributes(&pa, points) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer)
-      return submit(c, s, r, reinterpret_cast<const float4*>(pa.devicePointer), n, true, timestamp_us, v_gps, yaw_gps);
+      return submit(c, s, r, static_cast<const float*>(pa.devicePointer), n, 4, false, true, timestamp_us, v_gps, yaw_gps);
     cudaGetLastError();      // (pageable memory: not an error, take the copy path)
   }
-  LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_trk_done, 0));
-  int rc;
-  if (dsk) {                           // the raw records to the device, then deskewed into the slot's point buffer (in place of repack_kernel)
-    const float* raw = nullptr;
-    if ((rc = deskew_stage_host(c, s, s->stream, points, n, stride, &raw))) return rc;
-    if ((rc = deskew_frame(c, s, r, raw, n, stride, timestamp_us, v_gps, yaw_gps))) return rc;
-  } else if ((rc = upload_points(c, s, s->stream, points, n, stride, s->d_points))) {
-    return rc;
-  }
-  return submit(c, s, r, s->d_points, n, true, timestamp_us, v_gps, yaw_gps);
+  return submit(c, s, r, points, n, stride, true, true, timestamp_us, v_gps, yaw_gps);
 }
 
 int lmot_frame_collect(lmot_ctx* ctx, lmot_frame_out* out) {
@@ -1378,11 +1301,9 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
     if (n[i] > c->max_points) return LMOT_ERR_CAPACITY;
     if (!host && n[i] > 0 && (reinterpret_cast<uintptr_t>(points[i]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies need 16-byte alignment
   }
-  const bool dsk = with_tracker && q.deskew.on != 0;                // (lmot_batch_detect_dev has no stamp: never deskewed)
-  if (dsk && c->timing) return LMOT_ERR_STATE;
-  if (dsk && (host ? stride <= q.deskew.time_field : q.deskew.time_field != 3)) return LMOT_ERR_INVALID;
-  if ((q.merges() || q.masked() || q.search.on || q.lines.on || q.layers.on || q.obs.on) && c->timing) return LMOT_ERR_STATE;
-  if (with_tracker && q.acc.on() && c->timing) return LMOT_ERR_STATE;
+  // (lmot_batch_detect_dev has no stamp: never deskewed, never accumulated)
+  if (q.beyond_plain(with_tracker, true) && c->timing) return LMOT_ERR_STATE;
+  if (!q.deskew_fits(with_tracker, stride)) return LMOT_ERR_INVALID;
   if (host && c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;
   int rc = batch_ensure(c, n_frames);
   if (rc) return rc;
@@ -1406,15 +1327,11 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   r->merge_rows = q.merges() ? n_frames : 0;
   int* d_fc = nullptr;                       // the per-frame counts go straight into the result's pinned, device-mapped block
   LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&d_fc, r->h_frame_counts, 0));
-  const DetGroup grp{&q, with_tracker ? &c->own.th : nullptr, points, n, n_frames, ts, v, yaw, d_fc, r};
+  const DetGroup grp{&q, with_tracker ? &c->own.th : nullptr, points, n, n_frames, ts, v, yaw, d_fc, r, true};
   DetUnits U;
-  if ((rc = detect_front(c, b, &grp, 1, stride, host, r->h_deskew, r->h_area, false, U))) return rc;
-  c->n_area_dbg = q.masked() ? U.f0[1] : 0;
-  for (int i = 0; i < c->n_area_dbg; ++i) c->area_dbg[i] = U.u[i]->d_area_mask;
-  c->n_gz_dbg = q.lines.on ? n_frames : 0;
-  for (int i = 0; i < c->n_gz_dbg; ++i) c->gz_dbg[i] = c->bslots[b * c->batch_frames + i].d_gz;
-  c->n_lay_dbg = q.layers.on ? U.f0[1] : 0;
-  for (int i = 0; i < c->n_lay_dbg; ++i) c->lay_dbg[i] = U.u[i];
+  Slot* fr = &c->bslots[b * c->batch_frames];
+  if ((rc = detect_front(c, k, fr, st, b, &grp, 1, stride, host, r->h_deskew, r->h_area, false, U))) return rc;
+  own_debug_note(c, fr, n_frames, U);
   const bool gf = with_tracker && c->prm.global_frame;
   if ((rc = boxes_concat_launch(c, U.u, U.f0[1], st, k->d_boxes, k->d_counters, U.fc[0], (with_tracker && !gf) ? k->d_det_sem : nullptr,
                                 U.rig_on[0] ? U.rig : nullptr))) return rc;
@@ -1618,8 +1535,7 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
       if (q.n[j] < 0 || (q.n[j] > 0 && !q.data[j])) return LMOT_ERR_INVALID;
       if (!host && q.kind == LMOT_SEQ_FRAMES && q.n[j] > 0 && (reinterpret_cast<uintptr_t>(q.data[j]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies
     }
-    const lmot_deskew& dk = c->seq_cfg[k].deskew;
-    if (q.kind == LMOT_SEQ_FRAMES && dk.on && (host ? stride <= dk.time_field : dk.time_field != 3)) return LMOT_ERR_INVALID;
+    if (q.kind == LMOT_SEQ_FRAMES && !c->seq_cfg[k].deskew_fits(true, host ? stride : 4)) return LMOT_ERR_INVALID;
     ++S;
     if (q.kind == LMOT_SEQ_FRAMES) { F += nk; rigged |= rig_on[k]; merge[k] = c->seq_cfg[k].merges(); }
     else FL += nk;
@@ -1730,10 +1646,11 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
       int* fc = nullptr;
       if (rigged) LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc, t->blocks[k].h_frame_counts, 0));
       gk[G] = k;
-      g[G++] = DetGroup{&c->seq_cfg[k], &c->seq[k].th, e[k].data, e[k].n, f0[k + 1] - f0[k], e[k].timestamp_us, e[k].v_gps, e[k].yaw_gps, fc, &t->blocks[k]};
+      g[G++] = DetGroup{&c->seq_cfg[k], &c->seq[k].th, e[k].data, e[k].n, f0[k + 1] - f0[k], e[k].timestamp_us, e[k].v_gps, e[k].yaw_gps, fc, &t->blocks[k], true};
     }
     DetUnits U;
-    if ((rc = detect_front(c, b, g, G, stride, host, t->h_deskew, t->h_area, !rigged && !gf, U))) return rc;
+    if ((rc = detect_front(c, bk, &c->bslots[b * c->batch_frames], st, b, g, G, stride, host, t->h_deskew, t->h_area, !rigged && !gf, U)))
+      return rc;
     SeqMeas dm[kMaxBatch];
     for (int d = 0; d < G; ++d) {
       const Slot* s = U.u[U.f0[d]];

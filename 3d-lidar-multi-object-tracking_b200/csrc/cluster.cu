@@ -184,12 +184,7 @@ void cluster_free(Slot* s) {
 
 // elevated cloud = s->d_elev with its length in d_counters[CNT_N_ELEV]; n_upper bounds that length on the host
 int cluster_launch(Ctx* c, Slot* s, cudaStream_t st, int n_upper, bool counted, const unsigned* area) {
-  unsigned* once = s->d_cart_bits, *twice = once + kBitWords, *prev = twice + kBitWords;
-  if (s->label_grid_foreign) {   // the caller uploaded its own label grid (lmot_box_fit): the sparse update needs a clean slate
-    LMOT_CUDA(c, cudaMemsetAsync(s->d_label_grid, 0, kCartCells * sizeof(int), st));
-    LMOT_CUDA(c, cudaMemsetAsync(prev, 0, kBitWords * sizeof(unsigned), st));
-    s->label_grid_foreign = false;
-  }
+  unsigned* once = s->d_cart_bits, *twice = once + kBitWords;
   if (n_upper > 0 && !counted) {   // `counted`: ground_fused_kernel already marked the elevated points (fused frame path)
     cart_mark_kernel<<<(n_upper + 255) / 256, 256, 0, st>>>(s->d_elev, s->d_counters, c->prm.roi_m, s->d_cart, once, twice);
     kernel_mark(c, s, st);
@@ -205,6 +200,11 @@ int ccl_launch_batch(Ctx* c, Slot* const* slots, int F, cudaStream_t st, const u
   CclBatch B;
   for (int i = 0; i < F; ++i) {
     Slot* s = slots[i];
+    if (s->label_grid_foreign) {   // the caller uploaded its own label grid (lmot_box_fit): the sparse update needs a clean slate
+      LMOT_CUDA(c, cudaMemsetAsync(s->d_label_grid, 0, kCartCells * sizeof(int), st));
+      LMOT_CUDA(c, cudaMemsetAsync(s->d_cart_bits + 2 * kBitWords, 0, kBitWords * sizeof(unsigned), st));
+      s->label_grid_foreign = false;
+    }
     B.f[i].once = s->d_cart_bits; B.f[i].twice = s->d_cart_bits + kBitWords; B.f[i].prev_occ = s->d_cart_bits + 2 * kBitWords;
     B.f[i].out = s->d_label_grid; B.f[i].counters = s->d_counters;
   }

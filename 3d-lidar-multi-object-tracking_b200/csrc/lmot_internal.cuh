@@ -413,6 +413,14 @@ struct StreamCfg {
   bool masked() const { return area.n_rings > 0; }
   int search_angles() const { return search.on ? search.n_angles : 0; }   // A of the stream's units, 0: boxFitting's fit
   const lmot_ground_lines* lines_on() const { return lines.on ? &lines : nullptr; }
+  // a submission of the stream runs more than the plain detection path (timing mode times only that path).  stamped: it has a stamp
+  // (deskew and accumulation apply); sensors: its frames are the stream's sensors (merging applies)
+  bool beyond_plain(bool stamped, bool sensors) const {
+    return masked() || search.on || lines.on || layers.on || obs.on || deskews(stamped) || (stamped && acc.on()) || (sensors && merges());
+  }
+  bool deskews(bool stamped) const { return stamped && deskew.on; }
+  // records of `stride` floats hold the time field where the submission deskews them (device frames: stride 4)
+  bool deskew_fits(bool stamped, int stride) const { return !deskews(stamped) || stride > deskew.time_field; }
 };
 
 // the obstacle footprints of one returned step, copied out of its result block (the block is reused by later submissions)
