@@ -860,12 +860,15 @@ class Lmot:
         return dict(poses=np.array([list(e.pose) for e in s], np.float32).reshape(-1, 3, 4),
                     **{k: np.array([getattr(e, k) for e in s], np.float32) for k in ("h_sensor", "t_hmin", "t_hmax", "sensor_height")})
 
-    def get_sensors(self):
-        """-> dict(poses (n, 3, 4) f32, h_sensor, t_hmin, t_hmax, sensor_height: (n,) f32 each)"""
+    def _get_sensors(self, fn, *k):
         arr = (Sensor * MAX_BATCH)()
         n = C.c_int(0)
-        self._chk(self.lib.lmot_get_sensors(self.h, arr, MAX_BATCH, C.byref(n)))
+        self._chk(fn(self.h, *k, arr, MAX_BATCH, C.byref(n)))
         return self._sensor_dict(arr[: n.value])
+
+    def get_sensors(self):
+        """-> dict(poses (n, 3, 4) f32, h_sensor, t_hmin, t_hmax, sensor_height: (n,) f32 each)"""
+        return self._get_sensors(self.lib.lmot_get_sensors)
 
     # ---- merging rigs (lmot_set_rig_merge): the sensors' elevated clouds clustered and boxed as one vehicle-frame cloud ----------
     def set_rig_merge(self, on):
@@ -874,19 +877,20 @@ class Lmot:
         sensor_height is then the vehicle frame origin's height above the ground.  Applies from the next submitted tick on."""
         self._chk(self.lib.lmot_set_rig_merge(self.h, int(on)))
 
-    def get_rig_merge(self) -> bool:
+    def _get_switch(self, fn, *k) -> bool:
         v = C.c_int(0)
-        self._chk(self.lib.lmot_get_rig_merge(self.h, C.byref(v)))
+        self._chk(fn(self.h, *k, C.byref(v)))
         return bool(v.value)
+
+    def get_rig_merge(self) -> bool:
+        return self._get_switch(self.lib.lmot_get_rig_merge)
 
     def seq_set_rig_merge(self, k: int, on):
         """Sequence k's FRAMES steps, as set_rig_merge (with sequence k's sensor table and detection values)."""
         self._chk(self.lib.lmot_seq_set_rig_merge(self.h, int(k), int(on)))
 
     def seq_get_rig_merge(self, k: int) -> bool:
-        v = C.c_int(0)
-        self._chk(self.lib.lmot_seq_get_rig_merge(self.h, int(k), C.byref(v)))
-        return bool(v.value)
+        return self._get_switch(self.lib.lmot_seq_get_rig_merge, int(k))
 
     # ---- independent sequences: one frame of each sequence per tick, one track table per sequence (lmot_seq_*) ---------------
     def seq_open(self, n_seq: int, ring: int = 8):
@@ -926,10 +930,7 @@ class Lmot:
 
     def seq_get_sensors(self, k: int):
         """-> dict as get_sensors, for sequence k"""
-        arr = (Sensor * MAX_BATCH)()
-        n = C.c_int(0)
-        self._chk(self.lib.lmot_seq_get_sensors(self.h, int(k), arr, MAX_BATCH, C.byref(n)))
-        return self._sensor_dict(arr[: n.value])
+        return self._get_sensors(self.lib.lmot_seq_get_sensors, int(k))
 
     # ---- tracker parameters (lmot_set_tracker_params / lmot_seq_set_tracker_params) --------------------------------------------
     def set_tracker_params(self, **fields):
@@ -937,19 +938,21 @@ class Lmot:
         Array fields take sequences (std_a (3,), trans (3, 3), ...).  Applies from the next submitted step on."""
         self._chk(self.lib.lmot_set_tracker_params(self.h, C.byref(_tracker_params(fields)) if fields else None))
 
+    def _get_record(self, fn, cls, *k, as_dict=None) -> dict:
+        """a stream's setting record (cls) read by fn, as a dict of field -> value (as_dict: the conversion, default getattr per field)"""
+        r = cls()
+        self._chk(fn(self.h, *k, C.byref(r)))
+        return as_dict(r) if as_dict else {name: getattr(r, name) for name, _ in cls._fields_}
+
     def get_tracker_params(self) -> dict:
-        p = TrackerParams()
-        self._chk(self.lib.lmot_get_tracker_params(self.h, C.byref(p)))
-        return _tracker_params_dict(p)
+        return self._get_record(self.lib.lmot_get_tracker_params, TrackerParams, as_dict=_tracker_params_dict)
 
     def seq_set_tracker_params(self, k: int, **fields):
         """Sequence k's parameters, arguments as set_tracker_params."""
         self._chk(self.lib.lmot_seq_set_tracker_params(self.h, int(k), C.byref(_tracker_params(fields)) if fields else None))
 
     def seq_get_tracker_params(self, k: int) -> dict:
-        p = TrackerParams()
-        self._chk(self.lib.lmot_seq_get_tracker_params(self.h, int(k), C.byref(p)))
-        return _tracker_params_dict(p)
+        return self._get_record(self.lib.lmot_seq_get_tracker_params, TrackerParams, int(k), as_dict=_tracker_params_dict)
 
     # ---- track retirement and track IDs (lmot_set_track_retirement / lmot_track_ids) -------------------------------------------
     def set_track_retirement(self, on: bool):
@@ -957,17 +960,13 @@ class Lmot:
         self._chk(self.lib.lmot_set_track_retirement(self.h, 1 if on else 0))
 
     def get_track_retirement(self) -> bool:
-        v = C.c_int(0)
-        self._chk(self.lib.lmot_get_track_retirement(self.h, C.byref(v)))
-        return bool(v.value)
+        return self._get_switch(self.lib.lmot_get_track_retirement)
 
     def seq_set_track_retirement(self, k: int, on: bool):
         self._chk(self.lib.lmot_seq_set_track_retirement(self.h, int(k), 1 if on else 0))
 
     def seq_get_track_retirement(self, k: int) -> bool:
-        v = C.c_int(0)
-        self._chk(self.lib.lmot_seq_get_track_retirement(self.h, int(k), C.byref(v)))
-        return bool(v.value)
+        return self._get_switch(self.lib.lmot_seq_get_track_retirement, int(k))
 
     def _ids(self, fn, *k) -> np.ndarray:
         n = C.c_int(0)
@@ -1041,9 +1040,7 @@ class Lmot:
         self._chk(self.lib.lmot_seq_set_detect_params(self.h, int(k), arg))
 
     def seq_get_detect_params(self, k: int) -> dict:
-        d = DetectParams()
-        self._chk(self.lib.lmot_seq_get_detect_params(self.h, int(k), C.byref(d)))
-        return {name: getattr(d, name) for name, _ in DetectParams._fields_}
+        return self._get_record(self.lib.lmot_seq_get_detect_params, DetectParams, int(k))
 
     # ---- sweep deskew (lmot_set_deskew / lmot_seq_set_deskew) --------------------------------------------------------------------
     def set_deskew(self, **fields):
@@ -1052,34 +1049,29 @@ class Lmot:
         self._chk(self.lib.lmot_set_deskew(self.h, C.byref(_deskew(fields)) if fields else None))
 
     def get_deskew(self) -> dict:
-        d = Deskew()
-        self._chk(self.lib.lmot_get_deskew(self.h, C.byref(d)))
-        return {name: getattr(d, name) for name, _ in Deskew._fields_}
+        return self._get_record(self.lib.lmot_get_deskew, Deskew)
 
     def seq_set_deskew(self, k: int, **fields):
         """Sequence k's FRAMES steps, arguments as set_deskew."""
         self._chk(self.lib.lmot_seq_set_deskew(self.h, int(k), C.byref(_deskew(fields)) if fields else None))
 
     def seq_get_deskew(self, k: int) -> dict:
-        d = Deskew()
-        self._chk(self.lib.lmot_seq_get_deskew(self.h, int(k), C.byref(d)))
-        return {name: getattr(d, name) for name, _ in Deskew._fields_}
+        return self._get_record(self.lib.lmot_seq_get_deskew, Deskew, int(k))
 
     # ---- detection areas (lmot_set_detect_area / lmot_seq_set_detect_area) ----------------------------------------------------------
+    def _set_area(self, fn, rings, keep_outside, *k):
+        a, keep = _area(rings, keep_outside)
+        fn.argtypes = [C.c_void_p] + [C.c_int] * len(k) + [C.c_void_p]
+        self._chk(fn(self.h, *k, C.cast(C.byref(a), C.c_void_p) if a is not None else None))
+
     def set_detect_area(self, rings, keep_outside=False):
         """The context's frames and batched ticks: cluster and box only the elevated points in cells inside `rings` (a sequence of (m, 2)
         vertex arrays in the vehicle frame; None or empty: off), or outside them with keep_outside.  Applies from the next submission."""
-        a, keep = _area(rings, keep_outside)
-        fn = self.lib.lmot_set_detect_area
-        fn.argtypes = [C.c_void_p, C.c_void_p]
-        self._chk(fn(self.h, C.cast(C.byref(a), C.c_void_p) if a is not None else None))
+        self._set_area(self.lib.lmot_set_detect_area, rings, keep_outside)
 
     def seq_set_detect_area(self, k: int, rings, keep_outside=False):
         """Sequence k's FRAMES steps, arguments as set_detect_area."""
-        a, keep = _area(rings, keep_outside)
-        fn = self.lib.lmot_seq_set_detect_area
-        fn.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-        self._chk(fn(self.h, int(k), C.cast(C.byref(a), C.c_void_p) if a is not None else None))
+        self._set_area(self.lib.lmot_seq_set_detect_area, rings, keep_outside, int(k))
 
     def _get_area(self, fn, *k):
         lens = np.zeros(AREA_MAX_RINGS, np.int32)
@@ -1116,18 +1108,14 @@ class Lmot:
         self._chk(self.lib.lmot_set_accumulate(self.h, C.byref(_accumulate(fields)) if fields else None))
 
     def get_accumulate(self) -> dict:
-        a = Accumulate()
-        self._chk(self.lib.lmot_get_accumulate(self.h, C.byref(a)))
-        return {name: getattr(a, name) for name, _ in Accumulate._fields_}
+        return self._get_record(self.lib.lmot_get_accumulate, Accumulate)
 
     def seq_set_accumulate(self, k: int, **fields):
         """Sequence k's FRAMES steps, arguments as set_accumulate."""
         self._chk(self.lib.lmot_seq_set_accumulate(self.h, int(k), C.byref(_accumulate(fields)) if fields else None))
 
     def seq_get_accumulate(self, k: int) -> dict:
-        a = Accumulate()
-        self._chk(self.lib.lmot_seq_get_accumulate(self.h, int(k), C.byref(a)))
-        return {name: getattr(a, name) for name, _ in Accumulate._fields_}
+        return self._get_record(self.lib.lmot_seq_get_accumulate, Accumulate, int(k))
 
     # ---- box search (lmot_set_box_search) -----------------------------------------------------------------------------------------
     def set_box_search(self, **fields):
@@ -1136,18 +1124,14 @@ class Lmot:
         self._chk(self.lib.lmot_set_box_search(self.h, C.byref(_box_search(fields)) if fields else None))
 
     def get_box_search(self) -> dict:
-        b = BoxSearch()
-        self._chk(self.lib.lmot_get_box_search(self.h, C.byref(b)))
-        return {name: getattr(b, name) for name, _ in BoxSearch._fields_}
+        return self._get_record(self.lib.lmot_get_box_search, BoxSearch)
 
     def seq_set_box_search(self, k: int, **fields):
         """Sequence k's FRAMES steps, arguments as set_box_search."""
         self._chk(self.lib.lmot_seq_set_box_search(self.h, int(k), C.byref(_box_search(fields)) if fields else None))
 
     def seq_get_box_search(self, k: int) -> dict:
-        b = BoxSearch()
-        self._chk(self.lib.lmot_seq_get_box_search(self.h, int(k), C.byref(b)))
-        return {name: getattr(b, name) for name, _ in BoxSearch._fields_}
+        return self._get_record(self.lib.lmot_seq_get_box_search, BoxSearch, int(k))
 
     # ---- ground lines (lmot_set_ground_lines) ------------------------------------------------------------------------------------
     def set_ground_lines(self, **fields):
@@ -1156,18 +1140,14 @@ class Lmot:
         self._chk(self.lib.lmot_set_ground_lines(self.h, C.byref(_ground_lines(fields)) if fields else None))
 
     def get_ground_lines(self) -> dict:
-        g = GroundLines()
-        self._chk(self.lib.lmot_get_ground_lines(self.h, C.byref(g)))
-        return {name: getattr(g, name) for name, _ in GroundLines._fields_}
+        return self._get_record(self.lib.lmot_get_ground_lines, GroundLines)
 
     def seq_set_ground_lines(self, k: int, **fields):
         """Sequence k's FRAMES steps, arguments as set_ground_lines."""
         self._chk(self.lib.lmot_seq_set_ground_lines(self.h, int(k), C.byref(_ground_lines(fields)) if fields else None))
 
     def seq_get_ground_lines(self, k: int) -> dict:
-        g = GroundLines()
-        self._chk(self.lib.lmot_seq_get_ground_lines(self.h, int(k), C.byref(g)))
-        return {name: getattr(g, name) for name, _ in GroundLines._fields_}
+        return self._get_record(self.lib.lmot_seq_get_ground_lines, GroundLines, int(k))
 
     def debug_ground_lines(self) -> np.ndarray:
         """lmot_debug_ground_lines: (n_frames, 80, 120) float32 ground grids of the most recent own-stream submission (0: lines off)"""
@@ -1185,18 +1165,14 @@ class Lmot:
         self._chk(self.lib.lmot_set_layers(self.h, C.byref(_layers(fields)) if fields else None))
 
     def get_layers(self) -> dict:
-        l = Layers()
-        self._chk(self.lib.lmot_get_layers(self.h, C.byref(l)))
-        return {name: getattr(l, name) for name, _ in Layers._fields_}
+        return self._get_record(self.lib.lmot_get_layers, Layers)
 
     def seq_set_layers(self, k: int, **fields):
         """Sequence k's FRAMES steps, arguments as set_layers."""
         self._chk(self.lib.lmot_seq_set_layers(self.h, int(k), C.byref(_layers(fields)) if fields else None))
 
     def seq_get_layers(self, k: int) -> dict:
-        l = Layers()
-        self._chk(self.lib.lmot_seq_get_layers(self.h, int(k), C.byref(l)))
-        return {name: getattr(l, name) for name, _ in Layers._fields_}
+        return self._get_record(self.lib.lmot_seq_get_layers, Layers, int(k))
 
     # ---- obstacle footprints (lmot_set_obstacles) --------------------------------------------------------------------------------
     def set_obstacles(self, **fields):
@@ -1205,18 +1181,14 @@ class Lmot:
         self._chk(self.lib.lmot_set_obstacles(self.h, C.byref(_obstacles(fields)) if fields else None))
 
     def get_obstacles(self) -> dict:
-        o = Obstacles()
-        self._chk(self.lib.lmot_get_obstacles(self.h, C.byref(o)))
-        return {name: getattr(o, name) for name, _ in Obstacles._fields_}
+        return self._get_record(self.lib.lmot_get_obstacles, Obstacles)
 
     def seq_set_obstacles(self, k: int, **fields):
         """Sequence k's FRAMES steps, arguments as set_obstacles."""
         self._chk(self.lib.lmot_seq_set_obstacles(self.h, int(k), C.byref(_obstacles(fields)) if fields else None))
 
     def seq_get_obstacles(self, k: int) -> dict:
-        o = Obstacles()
-        self._chk(self.lib.lmot_seq_get_obstacles(self.h, int(k), C.byref(o)))
-        return {name: getattr(o, name) for name, _ in Obstacles._fields_}
+        return self._get_record(self.lib.lmot_seq_get_obstacles, Obstacles, int(k))
 
     def _obstacles_result(self, call) -> dict:
         probe = ObstaclesOut()
@@ -1265,8 +1237,9 @@ class Lmot:
             off += int(npt[u])
         return out
 
-    @staticmethod
-    def _accum_info(a: AccumInfo) -> list:
+    def _accum_info(self, fn, *k) -> list:
+        a = AccumInfo()
+        self._chk(fn(self.h, *k, C.byref(a)))
         out = []
         for u in range(a.n_units):
             k = a.sweeps_used[u]
@@ -1278,15 +1251,11 @@ class Lmot:
     def accumulate_info(self) -> list:
         """lmot_accumulate_info: one dict per unit of the most recently returned own-stream result (empty: it did not accumulate):
         sweeps_used, n_points (|E_acc|), stamp_us (sweeps_used,) and pose (sweeps_used, 3, 4) of the used sweeps, newest first."""
-        a = AccumInfo()
-        self._chk(self.lib.lmot_accumulate_info(self.h, C.byref(a)))
-        return self._accum_info(a)
+        return self._accum_info(self.lib.lmot_accumulate_info)
 
     def seq_accumulate_info(self, k: int) -> list:
         """lmot_seq_accumulate_info: as accumulate_info, for sequence k's most recently returned step"""
-        a = AccumInfo()
-        self._chk(self.lib.lmot_seq_accumulate_info(self.h, int(k), C.byref(a)))
-        return self._accum_info(a)
+        return self._accum_info(self.lib.lmot_seq_accumulate_info, int(k))
 
     def seq_frame_counts(self, k: int) -> np.ndarray:
         """(n_frames, 4) int32: n_elevated, n_ground, num_cluster, n_boxes of each of sequence k's frames in the tick collected last"""
@@ -1460,33 +1429,45 @@ class Lmot:
 
     def seq_tracker_load(self, k: int, dumps, init, timestamp_us, ego_velo=0.0, ego_yaw=0.0, ego_pre_yaw=0.0, ego_point_yaw=-np.pi / 2):
         """tracker_load for sequence k"""
-        d = np.ascontiguousarray(dumps, np.float64).reshape(-1, TRACK_DUMP_DOUBLES)
-        n = d.shape[0]
-        if n == 0:
-            d = np.zeros((1, TRACK_DUMP_DOUBLES), np.float64)
-        self._chk(self.lib.lmot_seq_tracker_load(self.h, int(k), d.ctypes.data_as(C.POINTER(C.c_double)), n, int(init), C.c_double(timestamp_us),
-                                                 C.c_double(ego_velo), C.c_double(ego_yaw), C.c_double(ego_pre_yaw), C.c_double(ego_point_yaw)))
+        self._tracker_load(self.lib.lmot_seq_tracker_load, (int(k),), dumps, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw)
 
     def seq_tracker_set_ego(self, k: int, ego8):
         """tracker_set_ego for sequence k"""
-        e = np.ascontiguousarray(ego8, np.float64)
-        assert e.shape == (8,)
-        self._chk(self.lib.lmot_seq_tracker_set_ego(self.h, int(k), e.ctypes.data_as(C.POINTER(C.c_double))))
+        self._tracker_set_ego(self.lib.lmot_seq_tracker_set_ego, ego8, int(k))
 
     def seq_tracker_reset(self, k: int):
         self._chk(self.lib.lmot_seq_tracker_reset(self.h, int(k)))
 
     def seq_tracker_dump(self, k: int) -> np.ndarray:
-        n = C.c_int(0)
-        self._chk(self.lib.lmot_seq_tracker_dump(self.h, int(k), None, 0, C.byref(n)))
-        out = np.zeros((max(n.value, 1), TRACK_DUMP_DOUBLES), np.float64)
-        self._chk(self.lib.lmot_seq_tracker_dump(self.h, int(k), out.ctypes.data_as(C.POINTER(C.c_double)), max(n.value, 1), C.byref(n)))
-        return out[: n.value]
+        return self._tracker_dump(self.lib.lmot_seq_tracker_dump, int(k))
 
     def seq_tracker_get_ego(self, k: int) -> np.ndarray:
+        return self._tracker_get_ego(self.lib.lmot_seq_tracker_get_ego, int(k))
+
+    def _tracker_dump(self, fn, *k) -> np.ndarray:
+        n = C.c_int(0)
+        self._chk(fn(self.h, *k, None, 0, C.byref(n)))
+        out = np.zeros((max(n.value, 1), TRACK_DUMP_DOUBLES), np.float64)
+        self._chk(fn(self.h, *k, out.ctypes.data_as(C.POINTER(C.c_double)), max(n.value, 1), C.byref(n)))
+        return out[: n.value]
+
+    def _tracker_load(self, fn, k, dumps, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw):
+        d = np.ascontiguousarray(dumps, np.float64).reshape(-1, TRACK_DUMP_DOUBLES)
+        n = d.shape[0]
+        if n == 0:
+            d = np.zeros((1, TRACK_DUMP_DOUBLES), np.float64)
+        self._chk(fn(self.h, *k, d.ctypes.data_as(C.POINTER(C.c_double)), n, int(init), C.c_double(timestamp_us), C.c_double(ego_velo),
+                     C.c_double(ego_yaw), C.c_double(ego_pre_yaw), C.c_double(ego_point_yaw)))
+
+    def _tracker_get_ego(self, fn, *k) -> np.ndarray:
         e = np.zeros(8, np.float64)
-        self._chk(self.lib.lmot_seq_tracker_get_ego(self.h, int(k), e.ctypes.data_as(C.POINTER(C.c_double))))
+        self._chk(fn(self.h, *k, e.ctypes.data_as(C.POINTER(C.c_double))))
         return e
+
+    def _tracker_set_ego(self, fn, ego8, *k):
+        e = np.ascontiguousarray(ego8, np.float64)
+        assert e.shape == (8,)
+        self._chk(fn(self.h, *k, e.ctypes.data_as(C.POINTER(C.c_double))))
 
     def tracker_reset(self):
         self._chk(self.lib.lmot_tracker_reset(self.h))
@@ -1497,19 +1478,10 @@ class Lmot:
         return n.value
 
     def tracker_dump(self) -> np.ndarray:
-        t = self.tracker_num_tracks()
-        out = np.zeros((max(t, 1), TRACK_DUMP_DOUBLES), np.float64)
-        n = C.c_int(0)
-        self._chk(self.lib.lmot_tracker_dump(self.h, out.ctypes.data_as(C.POINTER(C.c_double)), max(t, 1), C.byref(n)))
-        return out[: n.value]
+        return self._tracker_dump(self.lib.lmot_tracker_dump)
 
     def tracker_load(self, dumps, init, timestamp_us, ego_velo=0.0, ego_yaw=0.0, ego_pre_yaw=0.0, ego_point_yaw=-np.pi / 2):
-        d = np.ascontiguousarray(dumps, np.float64).reshape(-1, TRACK_DUMP_DOUBLES)
-        n = d.shape[0]
-        if n == 0:
-            d = np.zeros((1, TRACK_DUMP_DOUBLES), np.float64)
-        self._chk(self.lib.lmot_tracker_load(self.h, d.ctypes.data_as(C.POINTER(C.c_double)), n, int(init), C.c_double(timestamp_us),
-                                             C.c_double(ego_velo), C.c_double(ego_yaw), C.c_double(ego_pre_yaw), C.c_double(ego_point_yaw)))
+        self._tracker_load(self.lib.lmot_tracker_load, (), dumps, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw)
 
     def origin_points(self, timestamp_us, v_gps=0.0, yaw_gps=0.0) -> np.ndarray:
         """getOriginPoints for this frame WITHOUT advancing the tracker: (x, y, yaw, x, y, yaw + pi/2)."""
@@ -1518,14 +1490,10 @@ class Lmot:
         return o
 
     def tracker_get_ego(self) -> np.ndarray:
-        e = np.zeros(8, np.float64)
-        self._chk(self.lib.lmot_tracker_get_ego(self.h, e.ctypes.data_as(C.POINTER(C.c_double))))
-        return e
+        return self._tracker_get_ego(self.lib.lmot_tracker_get_ego)
 
     def tracker_set_ego(self, ego8):
-        e = np.ascontiguousarray(ego8, np.float64)
-        assert e.shape == (8,)
-        self._chk(self.lib.lmot_tracker_set_ego(self.h, e.ctypes.data_as(C.POINTER(C.c_double))))
+        self._tracker_set_ego(self.lib.lmot_tracker_set_ego, ego8)
 
     def tracker_table(self):
         """-> (device pointer, bytes per track, capacity) of the track table (for NCCL broadcast, see shared_tracker.py)"""

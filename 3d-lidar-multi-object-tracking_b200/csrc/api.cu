@@ -249,7 +249,6 @@ int batch_ensure(Ctx* c, int F) {
 
 void batch_destroy(Ctx* c) {
   for (int i = 0; i < c->n_bslots; ++i) slot_destroy(&c->bslots[i]);
-  for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&c->own_cfg.merge_unit[b]);
   for (int b = 0; b < kBatchBanks; ++b) {
     Slot* k = &c->bank[b];
     cudaFree(k->d_boxes); cudaFree(k->d_boxes_g); cudaFree(k->d_counters); cudaFree(k->d_det_sem); cudaFree(k->d_deskew); cudaFree(k->d_area);
@@ -510,7 +509,7 @@ int detect_front(Ctx* c, Slot* stage, Slot* fr, cudaStream_t st, int b, const De
 // what the debug getters read of the most recent own-stream submission: its units' cell masks and layer tables, its frames' ground grids
 // (none where the setting was off), and the units' area_last / layers_last (lmot_cluster_outputs, lmot_debug_label_grid)
 void own_debug_note(Ctx* c, Slot* fr, int nf, const DetUnits& U) {
-  const StreamCfg& q = c->own_cfg;
+  const StreamCfg& q = c->own.cfg;
   const int nu = U.f0[1];
   c->n_area_dbg = q.masked() ? nu : 0;
   c->n_lay_dbg = q.layers.on ? nu : 0;
@@ -535,7 +534,7 @@ int submit(Ctx* c, Slot* s, Result* r, const float* points, int n, int stride, b
   // the slot's previous boxes / counters must have been consumed by the tracker
   LMOT_CUDA(c, cudaStreamWaitEvent(s->stream, s->ev_trk_done, 0));
   const bool gf = with_tracker && c->prm.global_frame;
-  const DetGroup g{&c->own_cfg, with_tracker ? &c->own.th : nullptr, &points, &n, 1, ts, v, yaw, nullptr, r, false};
+  const DetGroup g{&c->own.cfg, with_tracker ? &c->own.trk.th : nullptr, &points, &n, 1, ts, v, yaw, nullptr, r, false};
   DetUnits U;
   // with_tracker: the slot's last box-fitting CTA posts its detection semaphore (global_frame: boxes_to_global_kernel does)
   if ((rc = detect_front(c, s, s, s->stream, 0, &g, 1, stride, host, r->h_deskew, r->h_area, with_tracker && !gf, U))) return rc;
@@ -583,8 +582,8 @@ int copy_track_outputs(const Result* s, lmot_track_out* out) {
   return (wants && T > out->cap) ? LMOT_ERR_CAPACITY : LMOT_OK;      // a zero-initialised lmot_track_out asks for the counts only
 }
 
-// results of a finished frame from its pinned host block; `trk`: the tracker whose step the block holds (nullptr: the context's own)
-int collect_result(Ctx* c, Result* r, lmot_frame_out* out, Tracker* trk = nullptr) {
+// results of a finished frame from its pinned host block; `s`: the stream whose step the block holds
+int collect_result(Ctx* c, Result* r, lmot_frame_out* out, Stream& s) {
   const double t0 = now_ns();
   LMOT_CUDA(c, cudaEventSynchronize(r->ev_done));
   const double t1 = now_ns();
@@ -622,7 +621,7 @@ int collect_result(Ctx* c, Result* r, lmot_frame_out* out, Tracker* trk = nullpt
     }
   }
   {                                                   // lmot_accumulate_info / lmot_seq_accumulate_info: what this result used
-    lmot_accum_info& ai = trk ? c->seq_acc_info[trk - c->seq] : c->acc_info;
+    lmot_accum_info& ai = s.acc_info;
     memset(&ai, 0, sizeof(ai));
     ai.n_units = r->acc_units;
     for (int u = 0; u < r->acc_units; ++u) {
@@ -636,15 +635,14 @@ int collect_result(Ctx* c, Result* r, lmot_frame_out* out, Tracker* trk = nullpt
     }
   }
   {                                                   // lmot_obstacles_result / lmot_seq_obstacles_result: this result's footprints
-    const int rc = obstacles_collect(c, r, trk ? c->seq_obs_last[trk - c->seq] : c->obs_last);
+    const int rc = obstacles_collect(c, r, s.obs_last);
     if (rc) return rc;
   }
   const int err = r->h_hdr[HDR_ERROR];
   const int warn = r->has_tracks ? r->h_hdr[HDR_WARN] : 0;
   if (r->has_tracks) {
-    Tracker& t = trk ? *trk : c->own;
-    t.last_n_act = r->h_hdr[HDR_N_ACT];
-    note_ids(t, r);
+    s.trk.last_n_act = r->h_hdr[HDR_N_ACT];
+    note_ids(s.trk, r);
   }
   if (out) {
     out->n_elevated = r->h_hdr[HDR_N_ELEV]; out->n_ground = r->h_hdr[HDR_N_GROUND];
@@ -721,12 +719,21 @@ void result_destroy(Result* r) {
   for (int i = 0; i < kMaxKernelEvents; ++i) if (r->kev[i]) cudaEventDestroy(r->kev[i]);
 }
 
+// what a stream holds on the device and in pinned memory (track table, merge units, accumulation history), then its record back to the
+// defaults
+void stream_free(Stream& s) {
+  tracker_free(s.trk);
+  for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&s.cfg.merge_unit[b]);
+  accumulate_free(s.cfg.acc);
+  s = Stream{};
+}
+
 // ---- independent sequences (lmot_seq_*): S frame streams, one or more frames each per tick, S track tables ---------------------------
 // Detection runs on the batch banks (batch_ensure).  Without sensor tables the box lists are NOT concatenated: a FRAMES sequence's tracker
 // reads its detection slot's own list and counters (seq_tick_common's map).  With a table among the tick's FRAMES sequences,
 // concat_boxes_seq_kernel concatenates each of their frames into that sequence's list on the bank (seq_meas) and the tracker reads those.
 void seq_destroy(Ctx* c) {
-  for (int k = 0; k < c->n_seq; ++k) tracker_free(c->seq[k]);
+  for (int k = 0; k < kMaxBatch; ++k) stream_free(c->seq[k]);
   for (int b = 0; b < kBatchBanks; ++b)
     for (int k = 0; k < kMaxBatch; ++k) {
       SeqMeas& m = c->seq_meas[b][k];
@@ -734,14 +741,6 @@ void seq_destroy(Ctx* c) {
       m = SeqMeas{};
     }
   for (int b = 0; b < kBatchBanks; ++b) { cudaFree(c->seq_stage[b]); c->seq_stage[b] = nullptr; }
-  for (int k = 0; k < kMaxBatch; ++k) {
-    for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&c->seq_cfg[k].merge_unit[b]);
-    accumulate_free(c->seq_cfg[k].acc);
-    c->seq_cfg[k] = StreamCfg{};
-    c->seq_acc_info[k] = lmot_accum_info{};
-    c->seq_obs_last[k].valid = false;
-    c->seq_fc_n[k] = 0;
-  }
   for (int i = 0; i < c->seq_ring; ++i) {
     for (int k = 0; k < c->n_seq; ++k) result_destroy(&c->seq_ticks[i].blocks[k]);
     if (c->seq_ticks[i].h_deskew) cudaFreeHost(c->seq_ticks[i].h_deskew);
@@ -757,6 +756,35 @@ void seq_forget(Ctx* c) {
   for (int i = 0; i < c->seq_ring; ++i) c->seq_ticks[i].in_flight = false;
   c->seq_in_flight = 0;
   c->seq_oldest = c->seq_next;
+}
+
+// The stream an entry point addresses: the context's own (k == kOwnStream, the lmot_X forms) or sequence k (the lmot_seq_X forms,
+// 0 <= k < n_seq); nullptr for any other k and for a null context.  kOwnStream lies outside int: no k a caller passes names the own stream.
+constexpr long long kOwnStream = -(1LL << 32);
+
+Stream* stream_at(lmot_ctx* ctx, long long k) {
+  if (!ctx) return nullptr;
+  Ctx* c = &ctx->c;
+  if (k == kOwnStream) return &c->own;
+  return k >= 0 && k < c->n_seq ? &c->seq[k] : nullptr;
+}
+
+const Stream* stream_at(const lmot_ctx* ctx, long long k) { return stream_at(const_cast<lmot_ctx*>(ctx), k); }
+
+// The pinned host blocks stream k's submissions stage from, at entry i of its ring (the setters that turn a feature on allocate them):
+// deskew tables and detection-area blocks (area_blocks of them) of the own stream's result block i / of sequence tick i, and the
+// accumulation count rows of the stream's result block there
+struct RingPins { float** deskew; AreaBlock** area; int area_blocks; int** acc; };
+
+int ring_size(const Ctx* c, long long k) { return k == kOwnStream ? c->n_results : c->seq_ring; }
+
+RingPins ring_pins(Ctx* c, long long k, int i) {
+  if (k == kOwnStream) {
+    Result& r = c->results[i];
+    return RingPins{&r.h_deskew, &r.h_area, 1, &r.h_acc};
+  }
+  SeqTick& t = c->seq_ticks[i];
+  return RingPins{&t.h_deskew, &t.h_area, kMaxBatch, &t.blocks[k].h_acc};
 }
 
 // next tick of the sequence ring; `drop_oldest` as acquire_result
@@ -782,17 +810,18 @@ int seq_collect_tick(Ctx* c, SeqTick* t, lmot_seq_out* out) {
   if (out) out->n_seq = c->n_seq;
   c->seq_stepped = t->stepped;
   for (int k = 0; k < c->n_seq; ++k) {
-    if (!(t->stepped >> k & 1u)) { c->seq_fc_n[k] = 0; c->seq_obs_last[k].valid = false; continue; }
+    Stream& q = c->seq[k];
+    if (!(t->stepped >> k & 1u)) { q.fc_n = 0; q.obs_last.valid = false; continue; }
     Result* b = &t->blocks[k];
-    const int r = collect_result(c, b, out ? &out->seq[k] : nullptr, &c->seq[k]);
+    const int r = collect_result(c, b, out ? &out->seq[k] : nullptr, q);
     if (r < 0 ? (rc >= 0) : (rc == LMOT_OK)) rc = r;       // the first error, else the first warning
     // per-frame counts (lmot_seq_frame_counts): the concatenation / pack wrote them into the block; else the one frame's
     if (b->batch_frames > 0) {
-      c->seq_fc_n[k] = b->batch_frames;
-      memcpy(c->seq_fc[k], b->h_frame_counts, (size_t)b->batch_frames * 4 * sizeof(int));
+      q.fc_n = b->batch_frames;
+      memcpy(q.fc, b->h_frame_counts, (size_t)b->batch_frames * 4 * sizeof(int));
     } else {
-      c->seq_fc_n[k] = 1;
-      for (int j = 0; j < 4; ++j) c->seq_fc[k][0][j] = b->h_hdr[HDR_N_ELEV + j];
+      q.fc_n = 1;
+      for (int j = 0; j < 4; ++j) q.fc[0][j] = b->h_hdr[HDR_N_ELEV + j];
     }
   }
   return rc;
@@ -928,7 +957,7 @@ int lmot_create(lmot_ctx** out, const lmot_params* params, int device) {
   for (int i = 0; i < c->n_results && rc == LMOT_OK; ++i) rc = result_create(c, &c->results[i]);
   for (int i = 0; i < c->n_slots && rc == LMOT_OK; ++i) rc = slot_create(c, &c->slots[i], i);
   c->last_res = &c->results[0];
-  if (rc == LMOT_OK) rc = tracker_alloc(c, c->own);
+  if (rc == LMOT_OK) rc = tracker_alloc(c, c->own.trk);
   if (rc == LMOT_OK) rc = (cudaDeviceSynchronize() == cudaSuccess) ? LMOT_OK : LMOT_ERR_CUDA;
   if (rc != LMOT_OK) { lmot_destroy(h); return rc; }
   *out = h;
@@ -944,8 +973,7 @@ void lmot_destroy(lmot_ctx* ctx) {
   for (int i = 0; i < c->n_slots; ++i) slot_destroy(&c->slots[i]);
   batch_destroy(c);
   for (int i = 0; i < c->n_results; ++i) result_destroy(&c->results[i]);
-  tracker_free(c->own);
-  accumulate_free(c->own_cfg.acc);
+  stream_free(c->own);
   seq_destroy(c);
   cudaFree(c->d_mt_raw);
   cudaFree(c->d_bs_tab);
@@ -1167,8 +1195,8 @@ int lmot_track_step(lmot_ctx* ctx, const float* boxes, int m, double timestamp_u
     for (int i = 0; i < s->res->n_kev; ++i) cudaEventElapsedTime(&c->kernel_ms[i], i == 0 ? s->res->ev[3] : s->res->kev[i - 1], s->res->kev[i]);
   }
   const int err = s->res->h_hdr[HDR_ERROR];
-  c->own.last_n_act = s->res->h_hdr[HDR_N_ACT];
-  note_ids(c->own, s->res);
+  c->own.trk.last_n_act = s->res->h_hdr[HDR_N_ACT];
+  note_ids(c->own.trk, s->res);
   rc = copy_track_outputs(s->res, out);
   return err ? err : (rc ? rc : s->res->h_hdr[HDR_WARN]);
 }
@@ -1179,7 +1207,7 @@ int lmot_detect_dev(lmot_ctx* ctx, const float* d_points, int n) {
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
-  if (c->own_cfg.beyond_plain(false, false) && c->timing) return LMOT_ERR_STATE;
+  if (c->own.cfg.beyond_plain(false, false) && c->timing) return LMOT_ERR_STATE;
   Slot* s = acquire_slot(c);
   Result* r = acquire_result(c, true);
   LMOT_CUDA(c, cudaEventRecord(s->ev_fork, c->stream));
@@ -1190,8 +1218,8 @@ int lmot_detect_dev(lmot_ctx* ctx, const float* d_points, int n) {
 int lmot_frame_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp_us, double v_gps, double yaw_gps) {
   if (!ctx || n < 0 || (n > 0 && !d_points) || (reinterpret_cast<uintptr_t>(d_points) & 15u)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  if (c->own_cfg.beyond_plain(true, false) && c->timing) return LMOT_ERR_STATE;
-  if (!c->own_cfg.deskew_fits(true, 4)) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
+  if (c->own.cfg.beyond_plain(true, false) && c->timing) return LMOT_ERR_STATE;
+  if (!c->own.cfg.deskew_fits(true, 4)) return LMOT_ERR_INVALID;     // device frames are float4: the time is the 4th float
   cudaSetDevice(c->device);
   if (n > c->max_points) return LMOT_ERR_CAPACITY;
   Slot* s = acquire_slot(c);
@@ -1205,10 +1233,10 @@ int lmot_frame_submit(lmot_ctx* ctx, const float* points, int n, int stride, dou
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
-  if (c->own_cfg.beyond_plain(true, false) && c->timing) return LMOT_ERR_STATE;
-  const bool dsk = c->own_cfg.deskews(true);
+  if (c->own.cfg.beyond_plain(true, false) && c->timing) return LMOT_ERR_STATE;
+  const bool dsk = c->own.cfg.deskews(true);
   if (dsk) {                           // (validated before anything is submitted: upload_points checks the rest without deskew)
-    if (n < 0 || (n > 0 && !points) || !c->own_cfg.deskew_fits(true, stride)) return LMOT_ERR_INVALID;
+    if (n < 0 || (n > 0 && !points) || !c->own.cfg.deskew_fits(true, stride)) return LMOT_ERR_INVALID;
     if (n > c->max_points) return LMOT_ERR_CAPACITY;
   }
   if (c->n_in_flight >= c->n_results) return LMOT_ERR_STATE;    // result ring full: collect first
@@ -1241,7 +1269,7 @@ int lmot_frame_collect(lmot_ctx* ctx, lmot_frame_out* out) {
   int guard = 0;
   while (!r->in_flight && guard++ < c->n_results) { c->res_oldest = (c->res_oldest + 1) % c->n_results; r = &c->results[c->res_oldest]; }
   if (!r->in_flight) return LMOT_ERR_STATE;
-  const int rc = collect_result(c, r, out);
+  const int rc = collect_result(c, r, out, c->own);
   r->in_flight = false;
   --c->n_in_flight;
   c->res_oldest = (c->res_oldest + 1) % c->n_results;
@@ -1269,7 +1297,7 @@ int lmot_frame_fetch(lmot_ctx* ctx, lmot_frame_out* out) {
   if (!ctx) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   Result* r = c->last_res;
-  const int rc = collect_result(c, r, out);
+  const int rc = collect_result(c, r, out, c->own);
   for (int i = 0; i < c->n_results; ++i) c->results[i].in_flight = false;
   c->n_in_flight = 0;
   c->res_oldest = c->res_next;
@@ -1293,7 +1321,7 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
                         double ts, double v, double yaw) {
   if (!ctx || !points || !n || n_frames < 1 || n_frames > kMaxBatch) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  StreamCfg& q = c->own_cfg;
+  StreamCfg& q = c->own.cfg;
   if (q.n_sensors > 0 && n_frames > q.n_sensors) return LMOT_ERR_INVALID;     // a frame without a sensor pose
   cudaSetDevice(c->device);
   for (int i = 0; i < n_frames; ++i) {
@@ -1327,7 +1355,7 @@ static int batch_common(lmot_ctx* ctx, const float* const* points, const int* n,
   r->merge_rows = q.merges() ? n_frames : 0;
   int* d_fc = nullptr;                       // the per-frame counts go straight into the result's pinned, device-mapped block
   LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&d_fc, r->h_frame_counts, 0));
-  const DetGroup grp{&q, with_tracker ? &c->own.th : nullptr, points, n, n_frames, ts, v, yaw, d_fc, r, true};
+  const DetGroup grp{&q, with_tracker ? &c->own.trk.th : nullptr, points, n, n_frames, ts, v, yaw, d_fc, r, true};
   DetUnits U;
   Slot* fr = &c->bslots[b * c->batch_frames];
   if ((rc = detect_front(c, k, fr, st, b, &grp, 1, stride, host, r->h_deskew, r->h_area, false, U))) return rc;
@@ -1369,7 +1397,8 @@ int lmot_batch_detect_dev(lmot_ctx* ctx, const float* const* d_points, const int
 int lmot_batch_ground_ccl_dev(lmot_ctx* ctx, const float* const* d_points, const int* n, int n_frames) {
   if (!ctx || !d_points || !n || n_frames < 1 || n_frames > kMaxBatch) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  if (c->own_cfg.n_sensors > 0 && n_frames > c->own_cfg.n_sensors) return LMOT_ERR_INVALID;
+  const StreamCfg& q = c->own.cfg;
+  if (q.n_sensors > 0 && n_frames > q.n_sensors) return LMOT_ERR_INVALID;
   cudaSetDevice(c->device);
   int rc = batch_ensure(c, n_frames);
   if (rc) return rc;
@@ -1382,7 +1411,7 @@ int lmot_batch_ground_ccl_dev(lmot_ctx* ctx, const float* const* d_points, const
   }
   sl[0]->res = &c->results[0];
   c->results[0].n_kev = 0;
-  if ((rc = ground_launch_batch(c, sl, n_frames, pp, n, c->stream, true, false, c->fuse_ccl, c->fuse_ccl, c->own_cfg.n_sensors > 0 ? c->own_cfg.sensors : nullptr))) return rc;
+  if ((rc = ground_launch_batch(c, sl, n_frames, pp, n, c->stream, true, false, c->fuse_ccl, c->fuse_ccl, q.n_sensors > 0 ? q.sensors : nullptr))) return rc;
   return c->fuse_ccl ? LMOT_OK : ccl_launch_batch(c, sl, n_frames, c->stream);
 }
 
@@ -1410,7 +1439,7 @@ int lmot_batch_collect(lmot_ctx* ctx, lmot_batch_out* out) {
   if (!r->in_flight) return LMOT_ERR_STATE;
   lmot_frame_out fo{};
   if (out) { fo.boxes = out->boxes; fo.max_boxes = out->max_boxes; fo.tracks = out->tracks; }
-  const int rc = collect_result(c, r, out ? &fo : nullptr);
+  const int rc = collect_result(c, r, out ? &fo : nullptr, c->own);
   r->in_flight = false;
   --c->n_in_flight;
   c->res_oldest = (c->res_oldest + 1) % c->n_results;
@@ -1423,7 +1452,7 @@ int lmot_batch_fetch(lmot_ctx* ctx, lmot_batch_out* out) {
   Result* r = c->last_res;
   lmot_frame_out fo{};
   if (out) { fo.boxes = out->boxes; fo.max_boxes = out->max_boxes; fo.tracks = out->tracks; }
-  const int rc = collect_result(c, r, out ? &fo : nullptr);
+  const int rc = collect_result(c, r, out ? &fo : nullptr, c->own);
   for (int i = 0; i < c->n_results; ++i) c->results[i].in_flight = false;
   c->n_in_flight = 0;
   c->res_oldest = c->res_next;
@@ -1464,7 +1493,7 @@ int lmot_seq_open(lmot_ctx* ctx, int n_seq, int ring) {
   if (!c->seq_ticks) return LMOT_ERR_INVALID;
   c->seq_ring = ring;
   c->n_seq = n_seq;                    // (set before the allocations: seq_destroy frees whatever was allocated on failure)
-  for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = tracker_alloc(c, c->seq[k]);
+  for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = tracker_alloc(c, c->seq[k].trk);
   for (int b = 0; b < kBatchBanks && rc == LMOT_OK; ++b)         // (nothing is in flight: drained above)
     for (int k = 0; k < n_seq && rc == LMOT_OK; ++k) rc = seq_meas_alloc(c, c->seq_meas[b][k]);
   for (int b = 0; b < kBatchBanks && rc == LMOT_OK; ++b)
@@ -1492,9 +1521,9 @@ static bool seq_layout(const Ctx* c, int* f0, bool* rig_on) {
   bool rigged = false;
   f0[0] = 0;
   for (int k = 0; k < c->n_seq; ++k) {
-    rig_on[k] = c->seq_cfg[k].n_sensors > 0;
+    rig_on[k] = c->seq[k].cfg.n_sensors > 0;
     rigged |= rig_on[k];
-    f0[k + 1] = f0[k] + (rig_on[k] ? c->seq_cfg[k].n_sensors : 1);
+    f0[k + 1] = f0[k] + (rig_on[k] ? c->seq[k].cfg.n_sensors : 1);
   }
   return rigged;
 }
@@ -1535,9 +1564,9 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
       if (q.n[j] < 0 || (q.n[j] > 0 && !q.data[j])) return LMOT_ERR_INVALID;
       if (!host && q.kind == LMOT_SEQ_FRAMES && q.n[j] > 0 && (reinterpret_cast<uintptr_t>(q.data[j]) & 15u)) return LMOT_ERR_INVALID;   // bulk copies
     }
-    if (q.kind == LMOT_SEQ_FRAMES && !c->seq_cfg[k].deskew_fits(true, host ? stride : 4)) return LMOT_ERR_INVALID;
+    if (q.kind == LMOT_SEQ_FRAMES && !c->seq[k].cfg.deskew_fits(true, host ? stride : 4)) return LMOT_ERR_INVALID;
     ++S;
-    if (q.kind == LMOT_SEQ_FRAMES) { F += nk; rigged |= rig_on[k]; merge[k] = c->seq_cfg[k].merges(); }
+    if (q.kind == LMOT_SEQ_FRAMES) { F += nk; rigged |= rig_on[k]; merge[k] = c->seq[k].cfg.merges(); }
     else FL += nk;
   }
   if (S == 0 || (host && F > 0 && stride < 3)) return LMOT_ERR_INVALID;
@@ -1557,7 +1586,7 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
     LMOT_CUDA(c, cudaDeviceSynchronize());
   }
   for (int k = 0; k < n_seq; ++k)
-    if (merge[k] && (rc = merge_ensure(c, c->seq_cfg[k].merge_unit, 4000 + 16 * k))) return rc;
+    if (merge[k] && (rc = merge_ensure(c, c->seq[k].cfg.merge_unit, 4000 + 16 * k))) return rc;
   // the tick's ring slot and bank; the front end runs on the bank's first detection slot's stream (on the bank's own stream when no
   // sequence sends frames), after the bank's previous tick has been consumed by the tracker
   SeqTick* t = seq_acquire(c, !host);
@@ -1584,9 +1613,9 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
     ++p;
     stepped |= 1u << k;
     if (e[k].flags & LMOT_SEQ_RESTART) {
-      c->seq_cfg[k].acc.forget();
-      tracker_restart_host(c->seq[k]);
-      LMOT_CUDA(c, cudaMemsetAsync(c->seq[k].d_trk_counters, 0, CNT_COUNT * sizeof(int), c->trk_stream));
+      c->seq[k].cfg.acc.forget();
+      tracker_restart_host(c->seq[k].trk);
+      LMOT_CUDA(c, cudaMemsetAsync(c->seq[k].trk.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->trk_stream));
     }
     Result* r = &t->blocks[k];
     r->n_kev = 0; r->has_tracks = true;
@@ -1624,7 +1653,7 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
         } else {
           L.lists[i] = e[k].data[j]; L.counts[i] = e[k].d_counts + j; L.cap[i] = e[k].cap_per_list;
         }
-        if (rig_on[k]) rig[i] = c->seq_cfg[k].sensors[j];
+        if (rig_on[k]) rig[i] = c->seq[k].cfg.sensors[j];
         else lmot_default_sensor(&c->prm, &rig[i]);
       }
       lrig[nl] = rig_on[k];
@@ -1646,7 +1675,7 @@ static int seq_tick_common(lmot_ctx* ctx, const lmot_seq_entry* e, int n_seq, in
       int* fc = nullptr;
       if (rigged) LMOT_CUDA(c, cudaHostGetDevicePointer((void**)&fc, t->blocks[k].h_frame_counts, 0));
       gk[G] = k;
-      g[G++] = DetGroup{&c->seq_cfg[k], &c->seq[k].th, e[k].data, e[k].n, f0[k + 1] - f0[k], e[k].timestamp_us, e[k].v_gps, e[k].yaw_gps, fc, &t->blocks[k], true};
+      g[G++] = DetGroup{&c->seq[k].cfg, &c->seq[k].trk.th, e[k].data, e[k].n, f0[k + 1] - f0[k], e[k].timestamp_us, e[k].v_gps, e[k].yaw_gps, fc, &t->blocks[k], true};
     }
     DetUnits U;
     if ((rc = detect_front(c, bk, &c->bslots[b * c->batch_frames], st, b, g, G, stride, host, t->h_deskew, t->h_area, !rigged && !gf, U)))
@@ -1810,7 +1839,7 @@ int lmot_detect_boxes_dev(lmot_ctx* ctx, const float** d_boxes, const int** d_n_
 
 int lmot_tracker_counters_dev(lmot_ctx* ctx, int** d_n_tracks) {
   if (!ctx || !d_n_tracks) return LMOT_ERR_INVALID;
-  *d_n_tracks = ctx->c.own.d_trk_counters + CNT_N_TRACKS;
+  *d_n_tracks = ctx->c.own.trk.d_trk_counters + CNT_N_TRACKS;
   return LMOT_OK;
 }
 
@@ -1821,7 +1850,8 @@ int lmot_track_step_lists_dev(lmot_ctx* ctx, const float* d_lists, const int* d_
                               double v_gps, double yaw_gps) {
   if (!ctx || !d_lists || !d_counts || n_lists < 1 || n_lists > kMaxBatch || cap_per_list < 1) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  if (c->own_cfg.n_sensors > 0 && n_lists > c->own_cfg.n_sensors) return LMOT_ERR_INVALID;     // a list without a sensor pose
+  const StreamCfg& q = c->own.cfg;
+  if (q.n_sensors > 0 && n_lists > q.n_sensors) return LMOT_ERR_INVALID;     // a list without a sensor pose
   cudaSetDevice(c->device);
   int rc = batch_ensure(c, 1);              // the bank's box buffer + counters are the tracker's input
   if (rc) return rc;
@@ -1830,7 +1860,7 @@ int lmot_track_step_lists_dev(lmot_ctx* ctx, const float* d_lists, const int* d_
   k->res = r;
   r->n_kev = 0; r->batch_frames = 0;
   cudaStream_t st = c->stream;
-  if ((rc = boxes_pack_lists_launch(c, st, d_lists, d_counts, n_lists, cap_per_list, k->d_boxes, k->d_counters, c->own_cfg.n_sensors > 0 ? c->own_cfg.sensors : nullptr)))
+  if ((rc = boxes_pack_lists_launch(c, st, d_lists, d_counts, n_lists, cap_per_list, k->d_boxes, k->d_counters, q.n_sensors > 0 ? q.sensors : nullptr)))
     return rc;
   if (c->prm.global_frame && (rc = boxes_to_global_launch(c, k, st, k->d_boxes, k->d_counters, timestamp_us, v_gps, yaw_gps, false))) return rc;
   if ((rc = tracker_launch(c, k, st, k->d_boxes, k->d_counters, timestamp_us, v_gps, yaw_gps))) return rc;
@@ -1873,82 +1903,70 @@ static bool sensors_valid(const lmot_sensor* s, int n) {
 }
 
 // a stream's sensor table, host state only: ticks already submitted carry their own copy in their launch parameters
-static int sensors_set(StreamCfg& q, const lmot_sensor* s, int n) {
+static int sensors_set(Stream& q, const lmot_sensor* s, int n) {
   if (!sensors_valid(s, n)) return LMOT_ERR_INVALID;
-  for (int k = 0; k < n; ++k) q.sensors[k] = s[k];
-  q.n_sensors = n;
+  for (int k = 0; k < n; ++k) q.cfg.sensors[k] = s[k];
+  q.cfg.n_sensors = n;
   return LMOT_OK;
 }
 
-static int sensors_get(const StreamCfg& q, lmot_sensor* s, int cap, int* n) {
-  if (cap < 0 || (cap > 0 && !s)) return LMOT_ERR_INVALID;
-  if (n) *n = q.n_sensors;
-  for (int k = 0; k < q.n_sensors && k < cap; ++k) s[k] = q.sensors[k];
+static int sensors_get(const Stream* q, lmot_sensor* s, int cap, int* n) {
+  if (!q || cap < 0 || (cap > 0 && !s)) return LMOT_ERR_INVALID;
+  if (n) *n = q->cfg.n_sensors;
+  for (int k = 0; k < q->cfg.n_sensors && k < cap; ++k) s[k] = q->cfg.sensors[k];
   return LMOT_OK;
 }
 
 int lmot_set_sensors(lmot_ctx* ctx, const lmot_sensor* s, int n) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  ctx->c.own_cfg.acc.forget();                    // sweep accumulation: the history starts empty again (set or not)
-  return sensors_set(ctx->c.own_cfg, s, n);
+  Stream* q = stream_at(ctx, kOwnStream);
+  if (!q) return LMOT_ERR_INVALID;
+  q->cfg.acc.forget();                 // sweep accumulation: the history starts empty again (set or not)
+  return sensors_set(*q, s, n);
 }
 
-int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n) { return ctx ? sensors_get(ctx->c.own_cfg, s, cap, n) : LMOT_ERR_INVALID; }
+int lmot_get_sensors(const lmot_ctx* ctx, lmot_sensor* s, int cap, int* n) { return sensors_get(stream_at(ctx, kOwnStream), s, cap, n); }
 
 // sequence k's table: its frames of later ticks, in table order.  A tick's frames (one per sequence without a table) stay within kMaxBatch
 int lmot_seq_set_sensors(lmot_ctx* ctx, int k, const lmot_sensor* s, int n) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq || !sensors_valid(s, n)) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  c->seq_cfg[k].acc.forget();          // sweep accumulation: the history starts empty again (set or not)
+  Stream* q = stream_at(ctx, k);
+  if (!q || !sensors_valid(s, n)) return LMOT_ERR_INVALID;
+  q->cfg.acc.forget();                 // sweep accumulation: the history starts empty again (set or not)
   int frames = 0;
-  for (int j = 0; j < c->n_seq; ++j) {
-    const int nj = j == k ? n : c->seq_cfg[j].n_sensors;
+  for (int j = 0; j < ctx->c.n_seq; ++j) {
+    const int nj = j == k ? n : ctx->c.seq[j].cfg.n_sensors;
     frames += nj > 0 ? nj : 1;
   }
-  return frames > kMaxBatch ? LMOT_ERR_INVALID : sensors_set(c->seq_cfg[k], s, n);
+  return frames > kMaxBatch ? LMOT_ERR_INVALID : sensors_set(*q, s, n);
 }
 
-int lmot_seq_get_sensors(const lmot_ctx* ctx, int k, lmot_sensor* s, int cap, int* n) {
-  return ctx && k >= 0 && k < ctx->c.n_seq ? sensors_get(ctx->c.seq_cfg[k], s, cap, n) : LMOT_ERR_INVALID;
-}
+int lmot_seq_get_sensors(const lmot_ctx* ctx, int k, lmot_sensor* s, int cap, int* n) { return sensors_get(stream_at(ctx, k), s, cap, n); }
 
-// ---- merging rigs (rig_merge.cu)
-static int rig_merge_set(StreamCfg& q, int on) {
+// ---- merging rigs (rig_merge.cu).  The history is forgotten also when `on` is refused
+static int rig_merge_set(Stream* q, int on) {
+  if (!q) return LMOT_ERR_INVALID;
+  q->cfg.acc.forget();
   if (on != 0 && on != 1) return LMOT_ERR_INVALID;
-  q.rig_merge = on != 0;
+  q->cfg.rig_merge = on != 0;
   return LMOT_OK;
 }
 
-static int rig_merge_get(const StreamCfg& q, int* on) {
-  if (!on) return LMOT_ERR_INVALID;
-  *on = q.rig_merge ? 1 : 0;
+static int rig_merge_get(const Stream* q, int* on) {
+  if (!q || !on) return LMOT_ERR_INVALID;
+  *on = q->cfg.rig_merge ? 1 : 0;
   return LMOT_OK;
 }
 
-int lmot_set_rig_merge(lmot_ctx* ctx, int on) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  ctx->c.own_cfg.acc.forget();
-  return rig_merge_set(ctx->c.own_cfg, on);
-}
-
-int lmot_get_rig_merge(const lmot_ctx* ctx, int* on) { return ctx ? rig_merge_get(ctx->c.own_cfg, on) : LMOT_ERR_INVALID; }
-
-int lmot_seq_set_rig_merge(lmot_ctx* ctx, int k, int on) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  ctx->c.seq_cfg[k].acc.forget();
-  return rig_merge_set(ctx->c.seq_cfg[k], on);
-}
-
-int lmot_seq_get_rig_merge(const lmot_ctx* ctx, int k, int* on) {
-  return ctx && k >= 0 && k < ctx->c.n_seq ? rig_merge_get(ctx->c.seq_cfg[k], on) : LMOT_ERR_INVALID;
-}
+int lmot_set_rig_merge(lmot_ctx* ctx, int on) { return rig_merge_set(stream_at(ctx, kOwnStream), on); }
+int lmot_get_rig_merge(const lmot_ctx* ctx, int* on) { return rig_merge_get(stream_at(ctx, kOwnStream), on); }
+int lmot_seq_set_rig_merge(lmot_ctx* ctx, int k, int on) { return rig_merge_set(stream_at(ctx, k), on); }
+int lmot_seq_get_rig_merge(const lmot_ctx* ctx, int k, int* on) { return rig_merge_get(stream_at(ctx, k), on); }
 
 int lmot_seq_frame_counts(lmot_ctx* ctx, int k, int counts[LMOT_MAX_BATCH][4], int* n_frames) {
-  if (!ctx || !counts || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  const Ctx* c = &ctx->c;
-  if (n_frames) *n_frames = c->seq_fc_n[k];
-  for (int j = 0; j < c->seq_fc_n[k]; ++j)
-    for (int i = 0; i < 4; ++i) counts[j][i] = c->seq_fc[k][j][i];
+  const Stream* q = stream_at(ctx, k);
+  if (!q || !counts) return LMOT_ERR_INVALID;
+  if (n_frames) *n_frames = q->fc_n;
+  for (int j = 0; j < q->fc_n; ++j)
+    for (int i = 0; i < 4; ++i) counts[j][i] = q->fc[j][i];
   return LMOT_OK;
 }
 
@@ -1980,9 +1998,10 @@ static bool tracker_params_valid(const lmot_tracker_params& p) {
 }
 
 // host state only, as the sensor tables: submitted steps carry their own copy in their launch parameters
-static int tracker_params_set(Tracker& t, const lmot_tracker_params* p) {
+static int tracker_params_set(Stream* s, const lmot_tracker_params* p) {
+  if (!s || (p && !tracker_params_valid(*p))) return LMOT_ERR_INVALID;
   const lmot_tracker_params d = tracker_params_defaults();
-  if (p && !tracker_params_valid(*p)) return LMOT_ERR_INVALID;
+  Tracker& t = s->trk;
   t.prm = p ? *p : d;
   // field by field (a caller's struct may carry anything in its padding)
   const lmot_tracker_params& q = t.prm;
@@ -1996,27 +2015,16 @@ static int tracker_params_set(Tracker& t, const lmot_tracker_params* p) {
   return LMOT_OK;
 }
 
-int lmot_set_tracker_params(lmot_ctx* ctx, const lmot_tracker_params* p) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  return tracker_params_set(ctx->c.own, p);
-}
-
-int lmot_get_tracker_params(const lmot_ctx* ctx, lmot_tracker_params* p) {
-  if (!ctx || !p) return LMOT_ERR_INVALID;
-  *p = ctx->c.own.prm;
+static int tracker_params_get(const Stream* s, lmot_tracker_params* p) {
+  if (!s || !p) return LMOT_ERR_INVALID;
+  *p = s->trk.prm;
   return LMOT_OK;
 }
 
-int lmot_seq_set_tracker_params(lmot_ctx* ctx, int k, const lmot_tracker_params* p) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  return tracker_params_set(ctx->c.seq[k], p);
-}
-
-int lmot_seq_get_tracker_params(const lmot_ctx* ctx, int k, lmot_tracker_params* p) {
-  if (!ctx || !p || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *p = ctx->c.seq[k].prm;
-  return LMOT_OK;
-}
+int lmot_set_tracker_params(lmot_ctx* ctx, const lmot_tracker_params* p) { return tracker_params_set(stream_at(ctx, kOwnStream), p); }
+int lmot_get_tracker_params(const lmot_ctx* ctx, lmot_tracker_params* p) { return tracker_params_get(stream_at(ctx, kOwnStream), p); }
+int lmot_seq_set_tracker_params(lmot_ctx* ctx, int k, const lmot_tracker_params* p) { return tracker_params_set(stream_at(ctx, k), p); }
+int lmot_seq_get_tracker_params(const lmot_ctx* ctx, int k, lmot_tracker_params* p) { return tracker_params_get(stream_at(ctx, k), p); }
 
 // ---------------------------------------------------------------------------------------------- detection parameters of a sequence
 int lmot_default_detect_params(const lmot_params* p, lmot_detect_params* out) {
@@ -2046,18 +2054,17 @@ static bool detect_params_valid(const lmot_detect_params& d) {
 
 // host state only, as the sensor tables: submitted ticks carry their own copy in their launch parameters
 int lmot_seq_set_detect_params(lmot_ctx* ctx, int k, const lmot_detect_params* p) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  if (p && !detect_params_valid(*p)) return LMOT_ERR_INVALID;
-  StreamCfg& q = ctx->c.seq_cfg[k];
-  q.det_on = p != nullptr;
-  if (p) q.det = *p;
+  Stream* s = stream_at(ctx, k);
+  if (!s || (p && !detect_params_valid(*p))) return LMOT_ERR_INVALID;
+  s->cfg.det_on = p != nullptr;
+  if (p) s->cfg.det = *p;
   return LMOT_OK;
 }
 
 int lmot_seq_get_detect_params(const lmot_ctx* ctx, int k, lmot_detect_params* p) {
-  if (!ctx || !p || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  const Ctx* c = &ctx->c;
-  *p = c->seq_cfg[k].det_on ? c->seq_cfg[k].det : detect_params_of(c->prm);
+  const Stream* s = stream_at(ctx, k);
+  if (!s || !p) return LMOT_ERR_INVALID;
+  *p = s->cfg.det_on ? s->cfg.det : detect_params_of(ctx->c.prm);
   return LMOT_OK;
 }
 
@@ -2074,46 +2081,35 @@ static bool deskew_valid(const lmot_deskew& d) {
   return d.t_min < d.t_max && d.t_max - d.t_min <= 1.0 && d.time_field >= 3;
 }
 
-// d (NULL: the defaults) validated; turning deskew on allocates the pinned table blocks `n` blocks of the ring need (once)
-static int deskew_set(Ctx* c, lmot_deskew& dst, const lmot_deskew* d, float** blocks, int n, size_t stride) {
+// d (NULL: the defaults) validated; turning deskew on allocates the pinned table blocks of the stream's ring (once).  Host state only, as
+// the sensor tables: submitted frames carry their own tables and launch parameters
+static int deskew_set(lmot_ctx* ctx, long long k, const lmot_deskew* d) {
+  Stream* s = stream_at(ctx, k);
   lmot_deskew v = d ? *d : deskew_defaults();
-  if (!deskew_valid(v)) return LMOT_ERR_INVALID;
+  if (!s || !deskew_valid(v)) return LMOT_ERR_INVALID;
   v.on = v.on ? 1 : 0;
   if (v.on) {
+    Ctx* c = &ctx->c;
     cudaSetDevice(c->device);
-    for (int i = 0; i < n; ++i) {
-      float** p = reinterpret_cast<float**>(reinterpret_cast<char*>(blocks) + i * stride);
+    for (int i = 0; i < ring_size(c, k); ++i) {
+      float** p = ring_pins(c, k, i).deskew;
       if (!*p) LMOT_CUDA(c, cudaHostAlloc((void**)p, kMaxBatch * kDeskewTabBytes, cudaHostAllocDefault));
     }
   }
-  dst = v;
+  s->cfg.deskew = v;
   return LMOT_OK;
 }
 
-// host state only, as the sensor tables: submitted frames carry their own tables and launch parameters
-int lmot_set_deskew(lmot_ctx* ctx, const lmot_deskew* d) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  return deskew_set(c, c->own_cfg.deskew, d, &c->results[0].h_deskew, c->n_results, sizeof(Result));
-}
-
-int lmot_get_deskew(const lmot_ctx* ctx, lmot_deskew* d) {
-  if (!ctx || !d) return LMOT_ERR_INVALID;
-  *d = ctx->c.own_cfg.deskew;
+static int deskew_get(const Stream* s, lmot_deskew* d) {
+  if (!s || !d) return LMOT_ERR_INVALID;
+  *d = s->cfg.deskew;
   return LMOT_OK;
 }
 
-int lmot_seq_set_deskew(lmot_ctx* ctx, int k, const lmot_deskew* d) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  return deskew_set(c, c->seq_cfg[k].deskew, d, &c->seq_ticks[0].h_deskew, c->seq_ring, sizeof(SeqTick));
-}
-
-int lmot_seq_get_deskew(const lmot_ctx* ctx, int k, lmot_deskew* d) {
-  if (!ctx || !d || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *d = ctx->c.seq_cfg[k].deskew;
-  return LMOT_OK;
-}
+int lmot_set_deskew(lmot_ctx* ctx, const lmot_deskew* d) { return deskew_set(ctx, kOwnStream, d); }
+int lmot_get_deskew(const lmot_ctx* ctx, lmot_deskew* d) { return deskew_get(stream_at(ctx, kOwnStream), d); }
+int lmot_seq_set_deskew(lmot_ctx* ctx, int k, const lmot_deskew* d) { return deskew_set(ctx, k, d); }
+int lmot_seq_get_deskew(const lmot_ctx* ctx, int k, lmot_deskew* d) { return deskew_get(stream_at(ctx, k), d); }
 
 int lmot_deskew_table(const lmot_deskew* d, double v, double omega, const lmot_sensor* mount, float out[LMOT_DESKEW_SLICES][12]) {
   if (!d || !out || !deskew_valid(*d) || !std::isfinite(v) || !std::isfinite(omega) || (mount && !sensors_valid(mount, 1))) return LMOT_ERR_INVALID;
@@ -2127,61 +2123,46 @@ int lmot_default_accumulate(lmot_accumulate* a) {
   return LMOT_OK;
 }
 
-// a (NULL: the defaults) validated into the stream's setting; turning it on pins the count rows of `n` result blocks `stride` bytes apart
-// (once).  The history starts empty again.
-static int accumulate_set(Ctx* c, AccHist& h, const lmot_accumulate* a, Result* blocks, int n, size_t stride) {
+// a (NULL: the defaults) validated into the stream's setting; turning it on pins the count rows of the stream's result blocks (once).  The
+// history starts empty again.
+static int accumulate_set(lmot_ctx* ctx, long long k, const lmot_accumulate* a) {
+  Stream* s = stream_at(ctx, k);
   const lmot_accumulate v = a ? *a : accumulate_defaults();
-  if (!accumulate_valid(v)) return LMOT_ERR_INVALID;
+  if (!s || !accumulate_valid(v)) return LMOT_ERR_INVALID;
   if (v.sweeps > 1) {
+    Ctx* c = &ctx->c;
     cudaSetDevice(c->device);
-    for (int i = 0; i < n; ++i) {
-      Result* r = reinterpret_cast<Result*>(reinterpret_cast<char*>(blocks) + i * stride);
-      if (!r->h_acc) {
-        LMOT_CUDA(c, cudaHostAlloc((void**)&r->h_acc, 4 * kMaxBatch * sizeof(int), cudaHostAllocMapped));
-        memset(r->h_acc, 0, 4 * kMaxBatch * sizeof(int));
+    for (int i = 0; i < ring_size(c, k); ++i) {
+      int** p = ring_pins(c, k, i).acc;
+      if (!*p) {
+        LMOT_CUDA(c, cudaHostAlloc((void**)p, 4 * kMaxBatch * sizeof(int), cudaHostAllocMapped));
+        memset(*p, 0, 4 * kMaxBatch * sizeof(int));
       }
     }
   }
-  h.cfg = v;
-  h.forget();                          // (the next accumulate launch is ordered behind every earlier one: entry 0 is free)
+  s->cfg.acc.cfg = v;
+  s->cfg.acc.forget();                 // (the next accumulate launch is ordered behind every earlier one: entry 0 is free)
   return LMOT_OK;
 }
 
-int lmot_set_accumulate(lmot_ctx* ctx, const lmot_accumulate* a) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  return accumulate_set(c, c->own_cfg.acc, a, &c->results[0], c->n_results, sizeof(Result));
-}
-
-int lmot_get_accumulate(const lmot_ctx* ctx, lmot_accumulate* a) {
-  if (!ctx || !a) return LMOT_ERR_INVALID;
-  *a = ctx->c.own_cfg.acc.cfg;
+static int accumulate_get(const Stream* s, lmot_accumulate* a) {
+  if (!s || !a) return LMOT_ERR_INVALID;
+  *a = s->cfg.acc.cfg;
   return LMOT_OK;
 }
 
-int lmot_seq_set_accumulate(lmot_ctx* ctx, int k, const lmot_accumulate* a) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  return accumulate_set(c, c->seq_cfg[k].acc, a, &c->seq_ticks[0].blocks[k], c->seq_ring, sizeof(SeqTick));
-}
-
-int lmot_seq_get_accumulate(const lmot_ctx* ctx, int k, lmot_accumulate* a) {
-  if (!ctx || !a || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *a = ctx->c.seq_cfg[k].acc.cfg;
+static int accumulate_info(const Stream* s, lmot_accum_info* out) {
+  if (!s || !out) return LMOT_ERR_INVALID;
+  *out = s->acc_info;
   return LMOT_OK;
 }
 
-int lmot_accumulate_info(lmot_ctx* ctx, lmot_accum_info* out) {
-  if (!ctx || !out) return LMOT_ERR_INVALID;
-  *out = ctx->c.acc_info;
-  return LMOT_OK;
-}
-
-int lmot_seq_accumulate_info(lmot_ctx* ctx, int k, lmot_accum_info* out) {
-  if (!ctx || !out || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *out = ctx->c.seq_acc_info[k];
-  return LMOT_OK;
-}
+int lmot_set_accumulate(lmot_ctx* ctx, const lmot_accumulate* a) { return accumulate_set(ctx, kOwnStream, a); }
+int lmot_get_accumulate(const lmot_ctx* ctx, lmot_accumulate* a) { return accumulate_get(stream_at(ctx, kOwnStream), a); }
+int lmot_seq_set_accumulate(lmot_ctx* ctx, int k, const lmot_accumulate* a) { return accumulate_set(ctx, k, a); }
+int lmot_seq_get_accumulate(const lmot_ctx* ctx, int k, lmot_accumulate* a) { return accumulate_get(stream_at(ctx, k), a); }
+int lmot_accumulate_info(lmot_ctx* ctx, lmot_accum_info* out) { return accumulate_info(stream_at(ctx, kOwnStream), out); }
+int lmot_seq_accumulate_info(lmot_ctx* ctx, int k, lmot_accum_info* out) { return accumulate_info(stream_at(ctx, k), out); }
 
 int lmot_accumulate_pose(const double fold_s[3], const double fold_t[3], const lmot_sensor* mount, float out[12]) {
   if (!fold_s || !fold_t || !out || (mount && !sensors_valid(mount, 1))) return LMOT_ERR_INVALID;
@@ -2197,38 +2178,29 @@ int lmot_default_box_search(lmot_box_search* b) {
   return LMOT_OK;
 }
 
-static int box_search_set(Ctx* c, lmot_box_search& dst, const lmot_box_search* b) {
+static int box_search_set(lmot_ctx* ctx, long long k, const lmot_box_search* b) {
+  Stream* s = stream_at(ctx, k);
   const lmot_box_search v = b ? *b : box_search_defaults();
-  if (!box_search_valid(v)) return LMOT_ERR_INVALID;
+  if (!s || !box_search_valid(v)) return LMOT_ERR_INVALID;
   if (v.on) {
-    cudaSetDevice(c->device);
-    const int rc = box_search_ensure(c);
+    cudaSetDevice(ctx->c.device);
+    const int rc = box_search_ensure(&ctx->c);
     if (rc) return rc;
   }
-  dst = v;
+  s->cfg.search = v;
   return LMOT_OK;
 }
 
-int lmot_set_box_search(lmot_ctx* ctx, const lmot_box_search* b) {
-  return ctx ? box_search_set(&ctx->c, ctx->c.own_cfg.search, b) : LMOT_ERR_INVALID;
-}
-
-int lmot_get_box_search(const lmot_ctx* ctx, lmot_box_search* b) {
-  if (!ctx || !b) return LMOT_ERR_INVALID;
-  *b = ctx->c.own_cfg.search;
+static int box_search_get(const Stream* s, lmot_box_search* b) {
+  if (!s || !b) return LMOT_ERR_INVALID;
+  *b = s->cfg.search;
   return LMOT_OK;
 }
 
-int lmot_seq_set_box_search(lmot_ctx* ctx, int k, const lmot_box_search* b) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  return box_search_set(&ctx->c, ctx->c.seq_cfg[k].search, b);
-}
-
-int lmot_seq_get_box_search(const lmot_ctx* ctx, int k, lmot_box_search* b) {
-  if (!ctx || !b || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *b = ctx->c.seq_cfg[k].search;
-  return LMOT_OK;
-}
+int lmot_set_box_search(lmot_ctx* ctx, const lmot_box_search* b) { return box_search_set(ctx, kOwnStream, b); }
+int lmot_get_box_search(const lmot_ctx* ctx, lmot_box_search* b) { return box_search_get(stream_at(ctx, kOwnStream), b); }
+int lmot_seq_set_box_search(lmot_ctx* ctx, int k, const lmot_box_search* b) { return box_search_set(ctx, k, b); }
+int lmot_seq_get_box_search(const lmot_ctx* ctx, int k, lmot_box_search* b) { return box_search_get(stream_at(ctx, k), b); }
 
 int lmot_box_search_angles(int n_angles, float out[][2]) {
   if (!out || n_angles < 1 || n_angles > LMOT_BOX_SEARCH_MAX_ANGLES) return LMOT_ERR_INVALID;
@@ -2248,33 +2220,23 @@ static bool ground_lines_valid(const lmot_ground_lines& g) {
          g.max_slope > 0 && g.max_rmse > 0 && g.max_step > 0;
 }
 
-static int ground_lines_set(lmot_ground_lines& dst, const lmot_ground_lines* g) {
+static int ground_lines_set(Stream* s, const lmot_ground_lines* g) {
   const lmot_ground_lines v = g ? *g : ground_lines_defaults();
-  if (!ground_lines_valid(v)) return LMOT_ERR_INVALID;
-  dst = v;
+  if (!s || !ground_lines_valid(v)) return LMOT_ERR_INVALID;
+  s->cfg.lines = v;
   return LMOT_OK;
 }
 
-int lmot_set_ground_lines(lmot_ctx* ctx, const lmot_ground_lines* g) {
-  return ctx ? ground_lines_set(ctx->c.own_cfg.lines, g) : LMOT_ERR_INVALID;
-}
-
-int lmot_get_ground_lines(const lmot_ctx* ctx, lmot_ground_lines* g) {
-  if (!ctx || !g) return LMOT_ERR_INVALID;
-  *g = ctx->c.own_cfg.lines;
+static int ground_lines_get(const Stream* s, lmot_ground_lines* g) {
+  if (!s || !g) return LMOT_ERR_INVALID;
+  *g = s->cfg.lines;
   return LMOT_OK;
 }
 
-int lmot_seq_set_ground_lines(lmot_ctx* ctx, int k, const lmot_ground_lines* g) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  return ground_lines_set(ctx->c.seq_cfg[k].lines, g);
-}
-
-int lmot_seq_get_ground_lines(const lmot_ctx* ctx, int k, lmot_ground_lines* g) {
-  if (!ctx || !g || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *g = ctx->c.seq_cfg[k].lines;
-  return LMOT_OK;
-}
+int lmot_set_ground_lines(lmot_ctx* ctx, const lmot_ground_lines* g) { return ground_lines_set(stream_at(ctx, kOwnStream), g); }
+int lmot_get_ground_lines(const lmot_ctx* ctx, lmot_ground_lines* g) { return ground_lines_get(stream_at(ctx, kOwnStream), g); }
+int lmot_seq_set_ground_lines(lmot_ctx* ctx, int k, const lmot_ground_lines* g) { return ground_lines_set(stream_at(ctx, k), g); }
+int lmot_seq_get_ground_lines(const lmot_ctx* ctx, int k, lmot_ground_lines* g) { return ground_lines_get(stream_at(ctx, k), g); }
 
 int lmot_ground_lines_grid(const lmot_ground_lines* g, const float minz[LMOT_NUM_CHANNEL * LMOT_NUM_BIN], double r_min, double r_max,
                            double sensor_height, float gz[LMOT_NUM_CHANNEL * LMOT_NUM_BIN]) {
@@ -2307,31 +2269,23 @@ int lmot_default_layers(lmot_layers* l) {
   return LMOT_OK;
 }
 
-static int layers_set(lmot_layers& dst, const lmot_layers* l) {
+static int layers_set(Stream* s, const lmot_layers* l) {
   const lmot_layers v = l ? *l : layers_defaults();
-  if (!layers_valid(v)) return LMOT_ERR_INVALID;
-  dst = v;
+  if (!s || !layers_valid(v)) return LMOT_ERR_INVALID;
+  s->cfg.layers = v;
   return LMOT_OK;
 }
 
-int lmot_set_layers(lmot_ctx* ctx, const lmot_layers* l) { return ctx ? layers_set(ctx->c.own_cfg.layers, l) : LMOT_ERR_INVALID; }
-
-int lmot_get_layers(const lmot_ctx* ctx, lmot_layers* l) {
-  if (!ctx || !l) return LMOT_ERR_INVALID;
-  *l = ctx->c.own_cfg.layers;
+static int layers_get(const Stream* s, lmot_layers* l) {
+  if (!s || !l) return LMOT_ERR_INVALID;
+  *l = s->cfg.layers;
   return LMOT_OK;
 }
 
-int lmot_seq_set_layers(lmot_ctx* ctx, int k, const lmot_layers* l) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  return layers_set(ctx->c.seq_cfg[k].layers, l);
-}
-
-int lmot_seq_get_layers(const lmot_ctx* ctx, int k, lmot_layers* l) {
-  if (!ctx || !l || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *l = ctx->c.seq_cfg[k].layers;
-  return LMOT_OK;
-}
+int lmot_set_layers(lmot_ctx* ctx, const lmot_layers* l) { return layers_set(stream_at(ctx, kOwnStream), l); }
+int lmot_get_layers(const lmot_ctx* ctx, lmot_layers* l) { return layers_get(stream_at(ctx, kOwnStream), l); }
+int lmot_seq_set_layers(lmot_ctx* ctx, int k, const lmot_layers* l) { return layers_set(stream_at(ctx, k), l); }
+int lmot_seq_get_layers(const lmot_ctx* ctx, int k, lmot_layers* l) { return layers_get(stream_at(ctx, k), l); }
 
 int lmot_debug_point_clusters(lmot_ctx* ctx, int32_t* ids, int cap, int* n_units, int n_points[LMOT_MAX_BATCH]) {
   if (!ctx || cap < 0 || (cap > 0 && !ids)) return LMOT_ERR_INVALID;
@@ -2359,34 +2313,22 @@ int lmot_default_obstacles(lmot_obstacles* o) {
   return LMOT_OK;
 }
 
-static int obstacles_set(lmot_obstacles& dst, const lmot_obstacles* o) {
+static int obstacles_set(Stream* s, const lmot_obstacles* o) {
   const lmot_obstacles v = o ? *o : obstacles_defaults();
-  if (!obstacles_valid(v)) return LMOT_ERR_INVALID;
-  dst = v;
+  if (!s || !obstacles_valid(v)) return LMOT_ERR_INVALID;
+  s->cfg.obs = v;
   return LMOT_OK;
 }
 
-int lmot_set_obstacles(lmot_ctx* ctx, const lmot_obstacles* o) { return ctx ? obstacles_set(ctx->c.own_cfg.obs, o) : LMOT_ERR_INVALID; }
-
-int lmot_get_obstacles(const lmot_ctx* ctx, lmot_obstacles* o) {
-  if (!ctx || !o) return LMOT_ERR_INVALID;
-  *o = ctx->c.own_cfg.obs;
+static int obstacles_get(const Stream* s, lmot_obstacles* o) {
+  if (!s || !o) return LMOT_ERR_INVALID;
+  *o = s->cfg.obs;
   return LMOT_OK;
 }
 
-int lmot_seq_set_obstacles(lmot_ctx* ctx, int k, const lmot_obstacles* o) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  return obstacles_set(ctx->c.seq_cfg[k].obs, o);
-}
-
-int lmot_seq_get_obstacles(const lmot_ctx* ctx, int k, lmot_obstacles* o) {
-  if (!ctx || !o || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *o = ctx->c.seq_cfg[k].obs;
-  return LMOT_OK;
-}
-
-static int obstacles_out(const ObsLast& L, int unit, lmot_obstacles_out* out) {
-  if (!out || out->cap_obstacles < 0 || out->cap_vertices < 0) return LMOT_ERR_INVALID;
+static int obstacles_result(const Stream* s, int unit, lmot_obstacles_out* out) {
+  if (!s || !out || out->cap_obstacles < 0 || out->cap_vertices < 0) return LMOT_ERR_INVALID;
+  const ObsLast& L = s->obs_last;
   if (!L.valid) return LMOT_ERR_STATE;
   if (unit < 0 || unit >= L.units) return LMOT_ERR_INVALID;
   out->n_units = L.units;
@@ -2407,33 +2349,34 @@ static int obstacles_out(const ObsLast& L, int unit, lmot_obstacles_out* out) {
   return (short_arr || L.n_vert[unit] > L.max_vertices[unit]) ? LMOT_ERR_CAPACITY : LMOT_OK;
 }
 
-int lmot_obstacles_result(lmot_ctx* ctx, int unit, lmot_obstacles_out* out) {
-  return ctx ? obstacles_out(ctx->c.obs_last, unit, out) : LMOT_ERR_INVALID;
-}
-
-int lmot_seq_obstacles_result(lmot_ctx* ctx, int k, int unit, lmot_obstacles_out* out) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  return obstacles_out(ctx->c.seq_obs_last[k], unit, out);
-}
+int lmot_set_obstacles(lmot_ctx* ctx, const lmot_obstacles* o) { return obstacles_set(stream_at(ctx, kOwnStream), o); }
+int lmot_get_obstacles(const lmot_ctx* ctx, lmot_obstacles* o) { return obstacles_get(stream_at(ctx, kOwnStream), o); }
+int lmot_seq_set_obstacles(lmot_ctx* ctx, int k, const lmot_obstacles* o) { return obstacles_set(stream_at(ctx, k), o); }
+int lmot_seq_get_obstacles(const lmot_ctx* ctx, int k, lmot_obstacles* o) { return obstacles_get(stream_at(ctx, k), o); }
+int lmot_obstacles_result(lmot_ctx* ctx, int unit, lmot_obstacles_out* out) { return obstacles_result(stream_at(ctx, kOwnStream), unit, out); }
+int lmot_seq_obstacles_result(lmot_ctx* ctx, int k, int unit, lmot_obstacles_out* out) { return obstacles_result(stream_at(ctx, k), unit, out); }
 
 // ---- detection areas (detect_area.cu).  Host state only, as the sensor tables; setting one allocates the pinned staging blocks of the
-// ring (once): `per` blocks at each of the n entries `blocks`, `stride` bytes apart
-static int area_set(Ctx* c, AreaBlock& dst, const lmot_area* a, AreaBlock** blocks, int n, size_t stride, int per) {
-  if (!area_valid(a)) return LMOT_ERR_INVALID;
+// stream's ring (once)
+static int area_set(lmot_ctx* ctx, long long k, const lmot_area* a) {
+  Stream* s = stream_at(ctx, k);
+  if (!s || !area_valid(a)) return LMOT_ERR_INVALID;
   if (a && a->n_rings > 0) {
+    Ctx* c = &ctx->c;
     cudaSetDevice(c->device);
-    for (int i = 0; i < n; ++i) {
-      AreaBlock** p = reinterpret_cast<AreaBlock**>(reinterpret_cast<char*>(blocks) + i * stride);
-      if (!*p) LMOT_CUDA(c, cudaHostAlloc((void**)p, (size_t)per * sizeof(AreaBlock), cudaHostAllocDefault));
+    for (int i = 0; i < ring_size(c, k); ++i) {
+      const RingPins p = ring_pins(c, k, i);
+      if (!*p.area) LMOT_CUDA(c, cudaHostAlloc((void**)p.area, (size_t)p.area_blocks * sizeof(AreaBlock), cudaHostAllocDefault));
     }
   }
-  area_copy(dst, a);
+  area_copy(s->cfg.area, a);
   return LMOT_OK;
 }
 
-static int area_get(const AreaBlock& a, int* n_rings, int* ring_len, int cap_rings, int* n_vertices, double* xy, int cap_vertices,
+static int area_get(const Stream* s, int* n_rings, int* ring_len, int cap_rings, int* n_vertices, double* xy, int cap_vertices,
                     int* keep_outside) {
-  if (cap_rings < 0 || cap_vertices < 0 || (cap_rings > 0 && !ring_len) || (cap_vertices > 0 && !xy)) return LMOT_ERR_INVALID;
+  if (!s || cap_rings < 0 || cap_vertices < 0 || (cap_rings > 0 && !ring_len) || (cap_vertices > 0 && !xy)) return LMOT_ERR_INVALID;
+  const AreaBlock& a = s->cfg.area;
   if (n_rings) *n_rings = a.n_rings;
   if (n_vertices) *n_vertices = a.n_vertices;
   if (keep_outside) *keep_outside = a.keep_outside;
@@ -2443,28 +2386,18 @@ static int area_get(const AreaBlock& a, int* n_rings, int* ring_len, int cap_rin
   return LMOT_OK;
 }
 
-int lmot_set_detect_area(lmot_ctx* ctx, const lmot_area* area) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  return area_set(c, c->own_cfg.area, area, &c->results[0].h_area, c->n_results, sizeof(Result), 1);
-}
+int lmot_set_detect_area(lmot_ctx* ctx, const lmot_area* area) { return area_set(ctx, kOwnStream, area); }
 
 int lmot_get_detect_area(const lmot_ctx* ctx, int* n_rings, int* ring_len, int cap_rings, int* n_vertices, double* xy, int cap_vertices,
                          int* keep_outside) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  return area_get(ctx->c.own_cfg.area, n_rings, ring_len, cap_rings, n_vertices, xy, cap_vertices, keep_outside);
+  return area_get(stream_at(ctx, kOwnStream), n_rings, ring_len, cap_rings, n_vertices, xy, cap_vertices, keep_outside);
 }
 
-int lmot_seq_set_detect_area(lmot_ctx* ctx, int k, const lmot_area* area) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  return area_set(c, c->seq_cfg[k].area, area, &c->seq_ticks[0].h_area, c->seq_ring, sizeof(SeqTick), kMaxBatch);
-}
+int lmot_seq_set_detect_area(lmot_ctx* ctx, int k, const lmot_area* area) { return area_set(ctx, k, area); }
 
 int lmot_seq_get_detect_area(const lmot_ctx* ctx, int k, int* n_rings, int* ring_len, int cap_rings, int* n_vertices, double* xy,
                              int cap_vertices, int* keep_outside) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  return area_get(ctx->c.seq_cfg[k].area, n_rings, ring_len, cap_rings, n_vertices, xy, cap_vertices, keep_outside);
+  return area_get(stream_at(ctx, k), n_rings, ring_len, cap_rings, n_vertices, xy, cap_vertices, keep_outside);
 }
 
 int lmot_detect_area_mask(const lmot_area* area, const lmot_sensor* mount, float roi_m, uint32_t out[LMOT_NUM_GRID * 8]) {
@@ -2494,17 +2427,17 @@ int lmot_debug_area_masks(lmot_ctx* ctx, uint32_t* out, int cap_units, int* n_un
 // counter lmot_tracker_counters_dev points at): rebuild the side arrays before the next step.  n = the count, as the host knows it.
 int lmot_tracker_table_received(lmot_ctx* ctx, int n) {
   if (!ctx || n < 0 || n > ctx->c.prm.max_tracks) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  c->own.h_trk_counters[CNT_N_TRACKS] = n;
-  c->own.act_valid = false;
-  c->own.ids_identity = true;
-  c->own.last_trk_res = nullptr;
+  Tracker& t = ctx->c.own.trk;
+  t.h_trk_counters[CNT_N_TRACKS] = n;
+  t.act_valid = false;
+  t.ids_identity = true;
+  t.last_trk_res = nullptr;
   return LMOT_OK;
 }
 
 int lmot_origin_points(lmot_ctx* ctx, double timestamp_us, double v_gps, double yaw_gps, double out6[6]) {
   if (!ctx || !out6) return LMOT_ERR_INVALID;
-  TrackerHost h = ctx->c.own.th;                       // peek: fold on a copy
+  TrackerHost h = ctx->c.own.trk.th;                   // peek: fold on a copy
   origin_points_fold(h, timestamp_us, v_gps, yaw_gps);
   out6[0] = h.egoPoint[0]; out6[1] = h.egoPoint[1]; out6[2] = h.egoPoint[2];
   out6[3] = h.egoPoint[0]; out6[4] = h.egoPoint[1]; out6[5] = h.egoPoint[2] + M_PI / 2;
@@ -2512,19 +2445,27 @@ int lmot_origin_points(lmot_ctx* ctx, double timestamp_us, double v_gps, double 
 }
 
 // ---------------------------------------------------------------------------------------------- tracker state
-static int tracker_reset(Ctx* c, Tracker& t) {
+// The sequence forms of reset, load and set_ego also drop the uncollected sequence ticks: reset whatever its outcome, load and set_ego
+// on success.  The own-stream forms never touch the sequence ring.
+static int tracker_reset(lmot_ctx* ctx, long long k) {
+  Stream* s = stream_at(ctx, k);
+  if (!s) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  s->cfg.acc.forget();                 // sweep accumulation: the history starts empty again
   int rc = drain(c);
   if (rc) return rc;
-  tracker_restart_host(t);
-  LMOT_CUDA(c, cudaMemsetAsync(t.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
+  tracker_restart_host(s->trk);
+  LMOT_CUDA(c, cudaMemsetAsync(s->trk.d_trk_counters, 0, CNT_COUNT * sizeof(int), c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
   return LMOT_OK;
 }
 
-int lmot_tracker_reset(lmot_ctx* ctx) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  ctx->c.own_cfg.acc.forget();                    // sweep accumulation: the history starts empty again
-  return tracker_reset(&ctx->c, ctx->c.own);
+int lmot_tracker_reset(lmot_ctx* ctx) { return tracker_reset(ctx, kOwnStream); }
+
+int lmot_seq_tracker_reset(lmot_ctx* ctx, int k) {
+  const int rc = tracker_reset(ctx, k);
+  if (rc != LMOT_ERR_INVALID) seq_forget(&ctx->c);
+  return rc;
 }
 
 static int fetch_trk_counters(Ctx* c, Tracker& t) {
@@ -2537,15 +2478,16 @@ static int fetch_trk_counters(Ctx* c, Tracker& t) {
 
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n) {
   if (!ctx || !n) return LMOT_ERR_INVALID;
-  int rc = fetch_trk_counters(&ctx->c, ctx->c.own);
+  Tracker& t = ctx->c.own.trk;
+  int rc = fetch_trk_counters(&ctx->c, t);
   if (rc) return rc;
-  *n = ctx->c.own.h_trk_counters[CNT_N_TRACKS];
+  *n = t.h_trk_counters[CNT_N_TRACKS];
   return LMOT_OK;
 }
 
 int lmot_tracker_table(lmot_ctx* ctx, void** dev_ptr, int* bytes_per_track, int* capacity) {
   if (!ctx) return LMOT_ERR_INVALID;
-  if (dev_ptr) *dev_ptr = ctx->c.own.d_tracks;
+  if (dev_ptr) *dev_ptr = ctx->c.own.trk.d_tracks;
   if (bytes_per_track) *bytes_per_track = (int)sizeof(TrackState);
   if (capacity) *capacity = ctx->c.prm.max_tracks;
   return LMOT_OK;
@@ -2554,12 +2496,13 @@ int lmot_tracker_table(lmot_ctx* ctx, void** dev_ptr, int* bytes_per_track, int*
 int lmot_tracker_set_num_tracks(lmot_ctx* ctx, int n) {
   if (!ctx || n < 0 || n > ctx->c.prm.max_tracks) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
+  Tracker& t = c->own.trk;
   int rc = drain(c);
   if (rc) return rc;
-  c->own.h_trk_counters[CNT_N_TRACKS] = n;
-  c->own.act_valid = false;
-  c->own.ids_identity = true;
-  LMOT_CUDA(c, cudaMemcpyAsync(c->own.d_trk_counters + CNT_N_TRACKS, c->own.h_trk_counters + CNT_N_TRACKS, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  t.h_trk_counters[CNT_N_TRACKS] = n;
+  t.act_valid = false;
+  t.ids_identity = true;
+  LMOT_CUDA(c, cudaMemcpyAsync(t.d_trk_counters + CNT_N_TRACKS, t.h_trk_counters + CNT_N_TRACKS, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   LMOT_CUDA(c, cudaStreamSynchronize(c->stream));
   return LMOT_OK;
 }
@@ -2569,7 +2512,11 @@ enum { D_TRACKNUM = 0, D_LIFETIME = 1, D_STATIC = 2, D_VIS = 3, D_X = 4, D_P = 2
        D_K = 145, D_BESTYAW = 175, D_BBYAW = 176, D_BBAREA = 177, D_DISTINIT = 178, D_XMERGEYAW = 179, D_INITMEAS = 180,
        D_VELON = 182, D_VELO = 183, D_BBN = 186, D_BB = 187, D_BESTBBN = 211, D_BESTBB = 212, D_TOTAL = LMOT_TRACK_DUMP_DOUBLES };
 
-static int tracker_dump(Ctx* c, Tracker& trk, double* dumps, int cap, int* n_out) {
+static int tracker_dump(lmot_ctx* ctx, long long k, double* dumps, int cap, int* n_out) {
+  Stream* s = stream_at(ctx, k);
+  if (!s || cap < 0) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  Tracker& trk = s->trk;
   int rc = fetch_trk_counters(c, trk);
   if (rc) return rc;
   const int T = trk.h_trk_counters[CNT_N_TRACKS];
@@ -2591,20 +2538,25 @@ static int tracker_dump(Ctx* c, Tracker& trk, double* dumps, int cap, int* n_out
     }
     d[D_BESTYAW] = t.bestYaw; d[D_DISTINIT] = t.distFromInit; d[D_XMERGEYAW] = t.x_merge_yaw;
     d[D_INITMEAS] = t.initMeas[0]; d[D_INITMEAS + 1] = t.initMeas[1];
-    d[D_VELON] = t.nVelo; for (int k = 0; k < t.nVelo && k < 3; ++k) d[D_VELO + k] = t.velo[k];
+    d[D_VELON] = t.nVelo; for (int j = 0; j < t.nVelo && j < 3; ++j) d[D_VELO + j] = t.velo[j];
     d[D_BBN] = t.nBBox; for (int p = 0; p < t.nBBox && p < 8; ++p) for (int q = 0; q < 3; ++q) d[D_BB + 3 * p + q] = t.BBox[p][q];
     d[D_BESTBBN] = t.nBest; for (int p = 0; p < t.nBest && p < 8; ++p) for (int q = 0; q < 3; ++q) d[D_BESTBB + 3 * p + q] = t.bestBBox[p][q];
   }
   return T > cap ? LMOT_ERR_CAPACITY : LMOT_OK;
 }
 
-int lmot_tracker_dump(lmot_ctx* ctx, double* dumps, int cap, int* n_out) {
-  if (!ctx || cap < 0) return LMOT_ERR_INVALID;
-  return tracker_dump(&ctx->c, ctx->c.own, dumps, cap, n_out);
-}
+int lmot_tracker_dump(lmot_ctx* ctx, double* dumps, int cap, int* n_out) { return tracker_dump(ctx, kOwnStream, dumps, cap, n_out); }
 
-static int tracker_load(Ctx* c, Tracker& trk, const double* dumps, int n, int init, double timestamp_us, double ego_velo, double ego_yaw,
-                        double ego_pre_yaw, double ego_point_yaw) {
+int lmot_seq_tracker_dump(lmot_ctx* ctx, int k, double* dumps, int cap, int* n_out) { return tracker_dump(ctx, k, dumps, cap, n_out); }
+
+// the history is forgotten before the arguments are validated
+static int tracker_load(lmot_ctx* ctx, long long k, const double* dumps, int n, int init, double timestamp_us, double ego_velo,
+                        double ego_yaw, double ego_pre_yaw, double ego_point_yaw) {
+  Stream* s = stream_at(ctx, k);
+  if (!s) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  Tracker& trk = s->trk;
+  s->cfg.acc.forget();
   if (n < 0 || (n > 0 && !dumps)) return LMOT_ERR_INVALID;
   if (n > c->prm.max_tracks) return LMOT_ERR_CAPACITY;
   int rc = drain(c);
@@ -2622,7 +2574,7 @@ static int tracker_load(Ctx* c, Tracker& trk, const double* dumps, int n, int in
     }
     t.bestYaw = d[D_BESTYAW]; t.distFromInit = d[D_DISTINIT]; t.x_merge_yaw = d[D_XMERGEYAW];
     t.initMeas[0] = d[D_INITMEAS]; t.initMeas[1] = d[D_INITMEAS + 1];
-    t.nVelo = (int)d[D_VELON]; for (int k = 0; k < t.nVelo && k < 3; ++k) t.velo[k] = d[D_VELO + k];
+    t.nVelo = (int)d[D_VELON]; for (int j = 0; j < t.nVelo && j < 3; ++j) t.velo[j] = d[D_VELO + j];
     t.nBBox = (int)d[D_BBN]; for (int p = 0; p < t.nBBox && p < 8; ++p) for (int q = 0; q < 3; ++q) t.BBox[p][q] = (float)d[D_BB + 3 * p + q];
     t.nBest = (int)d[D_BESTBBN]; for (int p = 0; p < t.nBest && p < 8; ++p) for (int q = 0; q < 3; ++q) t.bestBBox[p][q] = (float)d[D_BESTBB + 3 * p + q];
   }
@@ -2645,66 +2597,80 @@ static int tracker_load(Ctx* c, Tracker& trk, const double* dumps, int n, int in
 
 int lmot_tracker_load(lmot_ctx* ctx, const double* dumps, int n, int init, double timestamp_us, double ego_velo,
                       double ego_yaw, double ego_pre_yaw, double ego_point_yaw) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  ctx->c.own_cfg.acc.forget();
-  return tracker_load(&ctx->c, ctx->c.own, dumps, n, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw);
+  return tracker_load(ctx, kOwnStream, dumps, n, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw);
+}
+
+int lmot_seq_tracker_load(lmot_ctx* ctx, int k, const double* dumps, int n, int init, double timestamp_us, double ego_velo, double ego_yaw,
+                          double ego_pre_yaw, double ego_point_yaw) {
+  const int rc = tracker_load(ctx, k, dumps, n, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw);
+  if (rc == LMOT_OK) seq_forget(&ctx->c);
+  return rc;
 }
 
 // the frame-level scalars of getOriginPoints / immUkfJpdaf (imm_ukf_jpda.cpp:19-24,56-58) incl. the accumulated dead-reckoning pose
-static void get_ego(const TrackerHost& h, double ego8[8]) {
+static int tracker_get_ego(const Stream* s, double ego8[8]) {
+  if (!s || !ego8) return LMOT_ERR_INVALID;
+  const TrackerHost& h = s->trk.th;
   ego8[0] = h.init ? 1.0 : 0.0; ego8[1] = h.timestamp; ego8[2] = h.egoVelo; ego8[3] = h.egoYaw; ego8[4] = h.egoPreYaw;
   ego8[5] = h.fold[0]; ego8[6] = h.fold[1]; ego8[7] = h.fold[2];
+  return LMOT_OK;
 }
 
-int lmot_tracker_get_ego(lmot_ctx* ctx, double ego8[8]) {
-  if (!ctx || !ego8) return LMOT_ERR_INVALID;
-  get_ego(ctx->c.own.th, ego8);
+int lmot_tracker_get_ego(lmot_ctx* ctx, double ego8[8]) { return tracker_get_ego(stream_at(ctx, kOwnStream), ego8); }
+
+int lmot_seq_tracker_get_ego(lmot_ctx* ctx, int k, double ego8[8]) { return tracker_get_ego(stream_at(ctx, k), ego8); }
+
+static int tracker_set_ego(lmot_ctx* ctx, long long k, const double ego8[8]) {
+  Stream* s = stream_at(ctx, k);
+  if (!s || !ego8) return LMOT_ERR_INVALID;
+  s->cfg.acc.forget();
+  int rc = drain(&ctx->c);
+  if (rc) return rc;
+  TrackerHost& h = s->trk.th;
+  h.init = ego8[0] != 0.0; h.timestamp = ego8[1]; h.egoVelo = ego8[2]; h.egoYaw = ego8[3]; h.egoPreYaw = ego8[4];
+  h.fold[0] = ego8[5]; h.fold[1] = ego8[6]; h.fold[2] = ego8[7];
+  h.egoPoint[0] = h.fold[0]; h.egoPoint[1] = h.fold[1]; h.egoPoint[2] = h.fold[2];
   return LMOT_OK;
+}
+
+int lmot_tracker_set_ego(lmot_ctx* ctx, const double ego8[8]) { return tracker_set_ego(ctx, kOwnStream, ego8); }
+
+int lmot_seq_tracker_set_ego(lmot_ctx* ctx, int k, const double ego8[8]) {
+  const int rc = tracker_set_ego(ctx, k, ego8);
+  if (rc == LMOT_OK) seq_forget(&ctx->c);
+  return rc;
 }
 
 // ---- track retirement and track IDs
-int lmot_set_track_retirement(lmot_ctx* ctx, int on) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  ctx->c.own.retire = on != 0;
+static int track_retirement_set(Stream* s, int on) {
+  if (!s) return LMOT_ERR_INVALID;
+  s->trk.retire = on != 0;
   return LMOT_OK;
 }
 
-int lmot_get_track_retirement(const lmot_ctx* ctx, int* on) {
-  if (!ctx || !on) return LMOT_ERR_INVALID;
-  *on = ctx->c.own.retire ? 1 : 0;
+static int track_retirement_get(const Stream* s, int* on) {
+  if (!s || !on) return LMOT_ERR_INVALID;
+  *on = s->trk.retire ? 1 : 0;
   return LMOT_OK;
 }
 
-int lmot_seq_set_track_retirement(lmot_ctx* ctx, int k, int on) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  ctx->c.seq[k].retire = on != 0;
-  return LMOT_OK;
-}
+int lmot_set_track_retirement(lmot_ctx* ctx, int on) { return track_retirement_set(stream_at(ctx, kOwnStream), on); }
+int lmot_get_track_retirement(const lmot_ctx* ctx, int* on) { return track_retirement_get(stream_at(ctx, kOwnStream), on); }
+int lmot_seq_set_track_retirement(lmot_ctx* ctx, int k, int on) { return track_retirement_set(stream_at(ctx, k), on); }
+int lmot_seq_get_track_retirement(const lmot_ctx* ctx, int k, int* on) { return track_retirement_get(stream_at(ctx, k), on); }
 
-int lmot_seq_get_track_retirement(const lmot_ctx* ctx, int k, int* on) {
-  if (!ctx || !on || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  *on = ctx->c.seq[k].retire ? 1 : 0;
-  return LMOT_OK;
-}
-
-static int track_ids(const Tracker& t, long long* ids, int cap, int* n) {
-  if (!n || cap < 0 || (cap > 0 && !ids)) return LMOT_ERR_INVALID;
+static int track_ids(const Stream* s, int64_t* ids, int cap, int* n) {
+  if (!s || !n || cap < 0 || (cap > 0 && !ids)) return LMOT_ERR_INVALID;
+  const Tracker& t = s->trk;
   if (t.ids_n < 0) return LMOT_ERR_STATE;
   *n = t.ids_n;
   const int m = t.ids_n < cap ? t.ids_n : cap;
-  for (int i = 0; i < m; ++i) ids[i] = t.ids_rows ? (long long)i : t.ids_last[i];
+  for (int i = 0; i < m; ++i) ids[i] = t.ids_rows ? (int64_t)i : (int64_t)t.ids_last[i];
   return LMOT_OK;
 }
 
-int lmot_track_ids(lmot_ctx* ctx, int64_t* ids, int cap, int* n) {
-  if (!ctx) return LMOT_ERR_INVALID;
-  return track_ids(ctx->c.own, reinterpret_cast<long long*>(ids), cap, n);
-}
-
-int lmot_seq_track_ids(lmot_ctx* ctx, int k, int64_t* ids, int cap, int* n) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  return track_ids(ctx->c.seq[k], reinterpret_cast<long long*>(ids), cap, n);
-}
+int lmot_track_ids(lmot_ctx* ctx, int64_t* ids, int cap, int* n) { return track_ids(stream_at(ctx, kOwnStream), ids, cap, n); }
+int lmot_seq_track_ids(lmot_ctx* ctx, int k, int64_t* ids, int cap, int* n) { return track_ids(stream_at(ctx, k), ids, cap, n); }
 
 // ---- track prediction (lmot_predict_tracks*; tracker.cu predict_launch)
 static bool pred_out_valid(const lmot_pred_out& o) {
@@ -2783,27 +2749,30 @@ static int predict_host(Ctx* c, Tracker& t, const double* t_us, int n_t, lmot_pr
 }
 
 int lmot_predict_tracks(lmot_ctx* ctx, const double* t_us, int n_t, lmot_pred_out* out) {
-  if (!ctx) return LMOT_ERR_INVALID;
+  Stream* s = stream_at(ctx, kOwnStream);
+  if (!s) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   cudaSetDevice(c->device);
-  return predict_host(c, c->own, t_us, n_t, out, pred_stream_of(c, c->own));
+  return predict_host(c, s->trk, t_us, n_t, out, pred_stream_of(c, s->trk));
 }
 
 int lmot_predict_tracks_dev(lmot_ctx* ctx, const double* t_us, int n_t, const lmot_pred_out* d_out, int* d_n_rows) {
   if (!ctx || !d_out || !pred_out_valid(*d_out)) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
-  if (int rc = pred_times_valid(c->own, t_us, n_t)) return rc;
+  Tracker* tabs[1] = {&c->own.trk};
+  if (int rc = pred_times_valid(*tabs[0], t_us, n_t)) return rc;
   cudaSetDevice(c->device);
-  Tracker* tabs[1] = {&c->own};
-  return predict_dev(c, tabs, 1, t_us, n_t, d_out, &d_n_rows, pred_stream_of(c, c->own));
+  return predict_dev(c, tabs, 1, t_us, n_t, d_out, &d_n_rows, pred_stream_of(c, *tabs[0]));
 }
 
+// a sequence's table on the tracker stream (behind the sequence ticks); refused in timing mode before the outputs are looked at
 int lmot_seq_predict_tracks(lmot_ctx* ctx, int k, const double* t_us, int n_t, lmot_pred_out* out) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
+  Stream* s = stream_at(ctx, k);
+  if (!s) return LMOT_ERR_INVALID;
   Ctx* c = &ctx->c;
   if (c->timing) return LMOT_ERR_STATE;
   cudaSetDevice(c->device);
-  return predict_host(c, c->seq[k], t_us, n_t, out, c->trk_stream);
+  return predict_host(c, s->trk, t_us, n_t, out, c->trk_stream);
 }
 
 int lmot_seq_predict_tracks_dev(lmot_ctx* ctx, const double* t_us, int n_t, const lmot_pred_out* d_outs, int* d_n_rows) {
@@ -2812,68 +2781,12 @@ int lmot_seq_predict_tracks_dev(lmot_ctx* ctx, const double* t_us, int n_t, cons
   const int S = c->n_seq;
   for (int k = 0; k < S; ++k) if (!pred_out_valid(d_outs[k])) return LMOT_ERR_INVALID;
   if (c->timing) return LMOT_ERR_STATE;
-  for (int k = 0; k < S; ++k) if (int rc = pred_times_valid(c->seq[k], t_us + (size_t)k * n_t, n_t)) return rc;
+  for (int k = 0; k < S; ++k) if (int rc = pred_times_valid(c->seq[k].trk, t_us + (size_t)k * n_t, n_t)) return rc;
   cudaSetDevice(c->device);
   Tracker* tabs[kMaxBatch];
   int* dn[kMaxBatch];
-  for (int k = 0; k < S; ++k) { tabs[k] = &c->seq[k]; dn[k] = d_n_rows ? d_n_rows + k : nullptr; }
+  for (int k = 0; k < S; ++k) { tabs[k] = &c->seq[k].trk; dn[k] = d_n_rows ? d_n_rows + k : nullptr; }
   return predict_dev(c, tabs, S, t_us, n_t, d_outs, dn, c->trk_stream);
-}
-
-// ---- per-sequence state (lmot_seq_*)
-int lmot_seq_tracker_reset(lmot_ctx* ctx, int k) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  c->seq_cfg[k].acc.forget();          // sweep accumulation: the history starts empty again
-  const int rc = tracker_reset(c, c->seq[k]);
-  seq_forget(c);
-  return rc;
-}
-
-int lmot_seq_tracker_dump(lmot_ctx* ctx, int k, double* dumps, int cap, int* n_out) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq || cap < 0) return LMOT_ERR_INVALID;
-  return tracker_dump(&ctx->c, ctx->c.seq[k], dumps, cap, n_out);
-}
-
-int lmot_seq_tracker_get_ego(lmot_ctx* ctx, int k, double ego8[8]) {
-  if (!ctx || !ego8 || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  get_ego(ctx->c.seq[k].th, ego8);
-  return LMOT_OK;
-}
-
-int lmot_seq_tracker_load(lmot_ctx* ctx, int k, const double* dumps, int n, int init, double timestamp_us, double ego_velo, double ego_yaw,
-                          double ego_pre_yaw, double ego_point_yaw) {
-  if (!ctx || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  c->seq_cfg[k].acc.forget();
-  const int rc = tracker_load(c, c->seq[k], dumps, n, init, timestamp_us, ego_velo, ego_yaw, ego_pre_yaw, ego_point_yaw);
-  if (rc == LMOT_OK) seq_forget(c);        // (as lmot_seq_tracker_reset: the drained ticks are dropped)
-  return rc;
-}
-
-static int tracker_set_ego(Ctx* c, Tracker& t, const double ego8[8]) {
-  int rc = drain(c);
-  if (rc) return rc;
-  TrackerHost& h = t.th;
-  h.init = ego8[0] != 0.0; h.timestamp = ego8[1]; h.egoVelo = ego8[2]; h.egoYaw = ego8[3]; h.egoPreYaw = ego8[4];
-  h.fold[0] = ego8[5]; h.fold[1] = ego8[6]; h.fold[2] = ego8[7];
-  h.egoPoint[0] = h.fold[0]; h.egoPoint[1] = h.fold[1]; h.egoPoint[2] = h.fold[2];
-  return LMOT_OK;
-}
-
-int lmot_tracker_set_ego(lmot_ctx* ctx, const double ego8[8]) {
-  if (!ctx || !ego8) return LMOT_ERR_INVALID;
-  ctx->c.own_cfg.acc.forget();
-  return tracker_set_ego(&ctx->c, ctx->c.own, ego8);
-}
-
-int lmot_seq_tracker_set_ego(lmot_ctx* ctx, int k, const double ego8[8]) {
-  if (!ctx || !ego8 || k < 0 || k >= ctx->c.n_seq) return LMOT_ERR_INVALID;
-  Ctx* c = &ctx->c;
-  c->seq_cfg[k].acc.forget();
-  const int rc = tracker_set_ego(c, c->seq[k], ego8);
-  if (rc == LMOT_OK) seq_forget(c);
-  return rc;
 }
 
 // ---------------------------------------------------------------------------------------------- inspection

@@ -432,6 +432,17 @@ struct ObsLast {
   std::vector<float> xy[kMaxBatch];
 };
 
+// One frame stream: the context's own (lmot_frame*, lmot_batch*, lmot_track_step*, lmot_tracker_*) or a sequence of lmot_seq_*.  Its
+// settings, its track table, and what collect_result copied out of its most recently returned step.  Released by api.cu stream_free.
+struct Stream {
+  StreamCfg cfg;
+  Tracker trk;
+  lmot_accum_info acc_info = {};       // lmot_accumulate_info / lmot_seq_accumulate_info: what the step used
+  ObsLast obs_last;                    // lmot_obstacles_result / lmot_seq_obstacles_result: its footprints
+  int fc_n = 0;                        // lmot_seq_frame_counts: the frames of the sequence's step ...
+  int fc[kMaxBatch][4] = {};           // ... and their n_elev, n_ground, num_cluster, n_boxes (host copies: the ring slot is reused)
+};
+
 struct Ctx {
   lmot_params prm;
   int device = 0;
@@ -462,9 +473,6 @@ struct Ctx {
   int n_bslots = 0, batch_frames = 0, next_bank = 0;
   Slot bank[kBatchBanks];              // pseudo-slots: concatenated boxes + counters + semaphore + events of a bank, and the stream its
                                        // tracking-only sequence ticks (lmot_seq_track*) run on
-  // the context's own stream: sensor k = frame k of a batched tick / list k of lmot_track_step_lists_dev; deskew of lmot_frame* and of
-  // batched ticks.  The sequences' records never apply to it, nor it to sequence ticks
-  StreamCfg own_cfg;
 
   // ---- result ring
   int n_results = 1;
@@ -472,28 +480,28 @@ struct Ctx {
   int res_next = 0, res_oldest = 0, n_in_flight = 0;
   Result* last_res = nullptr;
 
+  // ---- the context's own stream: sensor k = frame k of a batched tick / list k of lmot_track_step_lists_dev; its settings apply to
+  // lmot_frame* and batched ticks.  The sequences' records never apply to it, nor it to sequence ticks
+  Stream own;
+
   // ---- tracker
-  Tracker own;                         // the context's own track table (lmot_frame*, lmot_batch*, lmot_track_step*, lmot_tracker_*)
   cudaStream_t trk_stream = nullptr;
   cudaStream_t pub_stream = nullptr;   // device -> host publication of finished frames
   int trk_ctas = 0, gate_words = 0;
   bool tc_wide = false;
   int tc_force = -1;           // LMOT_TC_WIDE: -1 by count, 0 / 1 pinned
-  // ---- independent sequences (lmot_seq_*): one Tracker each, a ring of ticks of n_seq result blocks; detection on the batch banks
+  // ---- independent sequences (lmot_seq_*): one Stream each (its frames of a tick are its sensors in table order; no table: one frame),
+  // a ring of ticks of n_seq result blocks; detection on the batch banks
   int n_seq = 0;
-  Tracker seq[kMaxBatch];
+  Stream seq[kMaxBatch];
   SeqTick* seq_ticks = nullptr;        // [seq_ring]
   int seq_ring = 0, seq_next = 0, seq_oldest = 0, seq_in_flight = 0;
   SeqTick* seq_last = nullptr;         // most recent submission (lmot_seq_fetch)
   uint32_t seq_stepped = 0;            // lmot_seq_stepped: the stepped mask of the tick most recently returned
   bool seq_wide = false;               // spawn_output_kernel's variant of the sequence ticks (largest last_n_act of the stepped tables)
-  // each sequence's stream: its frames of a tick are its sensors in table order (no table: one frame)
-  StreamCfg seq_cfg[kMaxBatch];
   SeqMeas seq_meas[kBatchBanks][kMaxBatch];    // per-sequence measurement lists of each batch bank, allocated by lmot_seq_open
   // staging of lmot_seq_track_submit's host lists, per bank: kMaxBatch lists of max_boxes boxes, then kMaxBatch counts (lmot_seq_open)
   float* seq_stage[kBatchBanks] = {};
-  int seq_fc_n[kMaxBatch] = {};                // lmot_seq_frame_counts: frames of sequence k in the tick collected last
-  int seq_fc[kMaxBatch][kMaxBatch][4] = {};    // ... and their n_elev, n_ground, num_cluster, n_boxes (host copies: the ring slot is reused)
 
   // ---- track prediction (lmot_predict_tracks*, tracker.cu predict_launch)
   bool pred_pending = false;           // a prediction was queued since the last tracker step: the next step's first kernel waits for it
@@ -504,10 +512,6 @@ struct Ctx {
   size_t pred_stage_bytes = 0;
   int* h_pred_n = nullptr;             // pinned: the staged row count
 
-  // ---- lmot_accumulate_info / lmot_seq_accumulate_info: what the most recently returned result of the own stream / sequence k used
-  lmot_accum_info acc_info = {};
-  lmot_accum_info seq_acc_info[kMaxBatch] = {};
-
   // ---- lmot_debug_area_masks: the unit masks of the most recent own-stream submission (none: it was not masked)
   const unsigned* area_dbg[kMaxBatch] = {};
   int n_area_dbg = 0;
@@ -517,10 +521,6 @@ struct Ctx {
   // ---- lmot_debug_point_clusters: the units of the most recent own-stream submission (none: it was not layered)
   const Slot* lay_dbg[kMaxBatch] = {};
   int n_lay_dbg = 0;
-
-  // ---- lmot_obstacles_result / lmot_seq_obstacles_result: host copies of the most recently returned step's footprints
-  ObsLast obs_last;
-  ObsLast seq_obs_last[kMaxBatch];
 
   // ---- timing
   bool timing = false;
@@ -644,7 +644,7 @@ int boxes_concat_seq_launch(Ctx* c, Slot* const* slots, int S, const int* f0, co
 int boxes_pack_lists_seq_launch(Ctx* c, cudaStream_t st, const SeqLists& L, int S, const int* f0, const bool* rig_on, const lmot_sensor* rig,
                                 const SeqMeas* m, int* const* frame_counts, bool post_sem);
 // sequence ticks over the S stepped sequences: chain position k is sequence seq[k]; measurement list m[k] and ego values ts / v / yaw[k]
-// are indexed by position -> track table c->seq[seq[k]] -> tick->blocks[seq[k]] (tracker.cu)
+// are indexed by position -> track table c->seq[seq[k]].trk -> tick->blocks[seq[k]] (tracker.cu)
 int seq_global_launch(Ctx* c, const int* seq, const SeqMeas* m, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw);
 int seq_tracker_launch(Ctx* c, const int* seq, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw);
 // track prediction of S tables (1..kMaxBatch) at n_t times each (t_us[k * n_t + j]) into outs[k] (device arrays), row counts into

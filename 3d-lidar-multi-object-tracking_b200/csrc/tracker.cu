@@ -2109,7 +2109,7 @@ void global_frame_xf(const double ego[3], Xf2* fwd, Xf2* back) {
 // post_sem: post the slot's detection semaphore afterwards (frame pipeline)
 int boxes_to_global_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, const int* det_counters, double timestamp, double v_gps,
                            double yaw_gps, bool post_sem) {
-  TrackerHost peek = c->own.th;
+  TrackerHost peek = c->own.trk.th;
   origin_points_fold(peek, timestamp, v_gps, yaw_gps);
   Xf2 fwd, back;
   global_frame_xf(peek.egoPoint, &fwd, &back);
@@ -2265,7 +2265,7 @@ int chain_launch(Ctx* c, Chain& ch, cudaStream_t st, bool own, ChainGate gate, b
 
 int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, const int* det_counters, double timestamp, double v_gps,
                    double yaw_gps, bool gate, bool* gated) {
-  const bool compat_first = !c->own.th.init && c->prm.oracle_compat_first_frame;   // the reference's first-frame quirk: TC alone
+  const bool compat_first = !c->own.trk.th.init && c->prm.oracle_compat_first_frame;   // the reference's first-frame quirk: TC alone
   // `gate` (frame submissions): the detection stages of this frame post sl->d_det_sem.  Either the gate kernel waits for it on
   // the device (see tracker_gate_kernel), or -- timing mode, the reference's first-frame quirk -- the stream waits for the event.
   const bool use_gate = gate && !c->timing && !compat_first;
@@ -2273,7 +2273,7 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
   if (gated) *gated = use_gate;
   Chain ch(c);
   const SeqMeas m{const_cast<float*>(d_boxes), sl->d_boxes_g, const_cast<int*>(det_counters), gate ? sl->d_det_sem : nullptr};
-  if (int rc = chain_prepare(c, c->own, m, sl->res, st, timestamp, v_gps, yaw_gps, ch)) return rc;
+  if (int rc = chain_prepare(c, c->own.trk, m, sl->res, st, timestamp, v_gps, yaw_gps, ch)) return rc;
   return chain_launch(c, ch, st, true, use_gate ? ChainGate::one : ChainGate::none, !c->timing, sl, !compat_first);
 }
 
@@ -2281,7 +2281,7 @@ int tracker_launch(Ctx* c, Slot* sl, cudaStream_t st, const float* d_boxes, cons
 int tracker_publish(Ctx* c, Result* r, cudaStream_t st) {
   OutPtrs d{r->d_targets, r->d_vandyaw, r->d_manage, r->d_static, r->d_vis, r->d_visbb, r->d_hdr, r->d_boxes};
   OutPtrs h{r->h_targets, r->h_vandyaw, r->h_manage, r->h_static, r->h_vis, r->h_visbb, r->h_hdr, r->h_boxes};
-  publish_kernel<<<1, kPubThreads, 0, st>>>(d, h, c->own.d_tc_seq, c->own.tc_launched, c->spin_limit, r->back);
+  publish_kernel<<<1, kPubThreads, 0, st>>>(d, h, c->own.trk.d_tc_seq, c->own.trk.tc_launched, c->spin_limit, r->back);
   if (r->ids) {
     PubIdsParams p{};
     p.s[0] = PubIds{r->d_hdr, r->d_ids, r->h_ids};
@@ -2298,7 +2298,7 @@ int boxes_publish(Ctx* c, Slot* s, Result* r, cudaStream_t st) {
 }
 
 // ---------------------------------------------------------------------------------------------- sequence ticks (lmot_seq_*)
-// Sequence k of a tick: measurement list m[k] (box list, counters, semaphore), track table c->seq[k], result block tick->blocks[k].
+// Sequence k of a tick: measurement list m[k] (box list, counters, semaphore), track table c->seq[k].trk, result block tick->blocks[k].
 // Every launch below covers all S sequences; per-sequence arguments travel in __grid_constant__ parameter blocks.
 
 // global_frame: position k's sensor- (or vehicle-) frame boxes -> m[k].d_boxes_g with THIS tick's ego pose of sequence seq[k] (peeked:
@@ -2306,7 +2306,7 @@ int boxes_publish(Ctx* c, Slot* s, Result* r, cudaStream_t st) {
 int seq_global_launch(Ctx* c, const int* seq, const SeqMeas* m, int S, cudaStream_t st, const double* ts, const double* v, const double* yaw) {
   GlobalSeqParams p{};
   for (int k = 0; k < S; ++k) {
-    TrackerHost peek = c->seq[seq[k]].th;
+    TrackerHost peek = c->seq[seq[k]].trk.th;
     origin_points_fold(peek, ts[k], v[k], yaw[k]);
     Xf2 back;
     global_frame_xf(peek.egoPoint, &p.s[k].fwd, &back);
@@ -2322,7 +2322,7 @@ int seq_global_launch(Ctx* c, const int* seq, const SeqMeas* m, int S, cudaStrea
 int seq_tracker_launch(Ctx* c, const int* seq, const SeqMeas* m, SeqTick* tick, int S, const double* ts, const double* v, const double* yaw) {
   Chain ch(c);
   for (int k = 0; k < S; ++k)
-    if (int rc = chain_prepare(c, c->seq[seq[k]], m[k], &tick->blocks[seq[k]], c->trk_stream, ts[k], v[k], yaw[k], ch)) return rc;
+    if (int rc = chain_prepare(c, c->seq[seq[k]].trk, m[k], &tick->blocks[seq[k]], c->trk_stream, ts[k], v[k], yaw[k], ch)) return rc;
   if (int rc = chain_launch(c, ch, c->trk_stream, false, ChainGate::seq, true, nullptr, true)) return rc;
   publish_seq_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(ch.pub);
   if (ch.ids_on) publish_ids_kernel<<<S, kPubThreads, 0, c->pub_stream>>>(ch.ids);
