@@ -1,6 +1,8 @@
 // TEST INFRASTRUCTURE ONLY -- C ABI of the plain-C++ restatement, same signatures as oracle/ref_harness.cpp
-// (prefix port_ instead of ref_) so tests can swap one oracle for the other.
+// (prefix port_ instead of ref_) so tests can swap one oracle for the other.  Inputs are double (the reference's values, exact in
+// any wider type); what the reference computes in double -- the dump row, vandyaw, the prediction -- is returned as port::real.
 #include <cstring>
+#include <limits>
 #include "port.h"
 
 using namespace port;
@@ -16,6 +18,7 @@ static int g_rule_mode = 0;
 extern "C" {
 
 void port_set_rule_mode(int mode) { g_rule_mode = mode; }
+int port_real_digits() { return std::numeric_limits<real>::digits; }   // mantissa bits of port::real: 53, or 64 for long double
 
 void port_cell_index(const float* xy, int n, int stride, int* ch, int* bin) {
   for (int i = 0; i < n; ++i) cell_index(xy[(size_t)i * stride], xy[(size_t)i * stride + 1], ch[i], bin[i]);
@@ -56,7 +59,7 @@ void port_tracker_reset() { g_T = Tracker(); }
 int port_tracker_num_tracks() { return (int)g_T.targets.size(); }
 
 void port_tracker_step(const float* boxes, int m, double timestamp, double v_gps, double yaw_gps, int cap, float* targets,
-                       double* vandyaw, int* track_manage, uint8_t* is_static, uint8_t* is_vis, float* vis_bb, int* n_vis,
+                       real* vandyaw, int* track_manage, uint8_t* is_static, uint8_t* is_vis, float* vis_bb, int* n_vis,
                        int* n_tracks_out) {
   get_origin_points(g_T, timestamp, v_gps, yaw_gps);
   StepOut o;
@@ -73,14 +76,14 @@ void port_tracker_step(const float* boxes, int m, double timestamp, double v_gps
   for (size_t k = 0; k < o.vis_bb.size() && k < (size_t)cap * 24; ++k) vis_bb[k] = o.vis_bb[k];
 }
 
-void port_tracker_dump(int i, double* d) {
-  memset(d, 0, sizeof(double) * D_TOTAL);
+void port_tracker_dump(int i, real* d) {
+  for (int k = 0; k < D_TOTAL; ++k) d[k] = 0;
   const Track& t = g_T.targets[i];
   d[D_TRACKNUM] = g_T.trackNum[i]; d[D_LIFETIME] = t.lifetime; d[D_STATIC] = t.isStatic; d[D_VIS] = t.isVisBB;
-  for (int m = 0; m < 4; ++m) { memcpy(d + D_X + 5 * m, t.x[m], 5 * sizeof(double)); memcpy(d + D_P + 25 * m, t.P[m], 25 * sizeof(double)); }
+  for (int m = 0; m < 4; ++m) { memcpy(d + D_X + 5 * m, t.x[m], 5 * sizeof(real)); memcpy(d + D_P + 25 * m, t.P[m], 25 * sizeof(real)); }
   for (int m = 0; m < 3; ++m) {
     d[D_MODE + m] = t.modeProb[m]; d[D_ZPRED + 2 * m] = t.zPred[m][0]; d[D_ZPRED + 2 * m + 1] = t.zPred[m][1];
-    memcpy(d + D_S + 4 * m, t.S[m], 4 * sizeof(double)); memcpy(d + D_K + 10 * m, t.K[m], 10 * sizeof(double));
+    memcpy(d + D_S + 4 * m, t.S[m], 4 * sizeof(real)); memcpy(d + D_K + 10 * m, t.K[m], 10 * sizeof(real));
   }
   d[D_BESTYAW] = t.bestYaw; d[D_BBYAW] = t.bb_yaw; d[D_BBAREA] = t.bb_area; d[D_DISTINIT] = t.distFromInit; d[D_XMERGEYAW] = t.x_merge_yaw;
   d[D_INITMEAS] = t.initMeas[0]; d[D_INITMEAS + 1] = t.initMeas[1];
@@ -96,10 +99,14 @@ void port_tracker_load(int n_tracks, const double* dumps, int init, double times
     const double* d = dumps + (size_t)i * D_TOTAL;
     Track t; memset(&t, 0, sizeof(t));
     t.lifetime = (int)d[D_LIFETIME]; t.isStatic = d[D_STATIC] != 0; t.isVisBB = d[D_VIS] != 0;
-    for (int m = 0; m < 4; ++m) { memcpy(t.x[m], d + D_X + 5 * m, 5 * sizeof(double)); memcpy(t.P[m], d + D_P + 25 * m, 25 * sizeof(double)); }
+    for (int m = 0; m < 4; ++m) {
+      for (int e = 0; e < 5; ++e) t.x[m][e] = d[D_X + 5 * m + e];
+      for (int e = 0; e < 25; ++e) t.P[m][e] = d[D_P + 25 * m + e];
+    }
     for (int m = 0; m < 3; ++m) {
       t.modeProb[m] = d[D_MODE + m]; t.zPred[m][0] = d[D_ZPRED + 2 * m]; t.zPred[m][1] = d[D_ZPRED + 2 * m + 1];
-      memcpy(t.S[m], d + D_S + 4 * m, 4 * sizeof(double)); memcpy(t.K[m], d + D_K + 10 * m, 10 * sizeof(double));
+      for (int e = 0; e < 4; ++e) t.S[m][e] = d[D_S + 4 * m + e];
+      for (int e = 0; e < 10; ++e) t.K[m][e] = d[D_K + 10 * m + e];
     }
     t.bestYaw = d[D_BESTYAW]; t.bb_yaw = d[D_BBYAW]; t.bb_area = d[D_BBAREA]; t.distFromInit = d[D_DISTINIT]; t.x_merge_yaw = d[D_XMERGEYAW];
     t.initMeas[0] = d[D_INITMEAS]; t.initMeas[1] = d[D_INITMEAS + 1];
@@ -111,6 +118,28 @@ void port_tracker_load(int n_tracks, const double* dumps, int init, double times
   g_T.init = init != 0; g_T.timestamp = timestamp; g_T.egoVelo = ego_velo; g_T.egoYaw = ego_yaw; g_T.egoPreYaw = ego_pre_yaw;
   g_T.egoPoint[0] = 0; g_T.egoPoint[1] = 0; g_T.egoPoint[2] = ego_point_yaw;
   g_T.fold[0] = 0; g_T.fold[1] = 0; g_T.fold[2] = -1.5707963267948966;
+}
+
+// ref_tracker_predict's signature and semantics (oracle/ref_predict.cpp), on the port's table
+int port_tracker_predict(const double* t_us, int n_t, int cap, int* track_manage, unsigned char* flags, real* x, real* P, real* mode_prob,
+                         real* gate_z, real* gate_S) {
+  const int n = (int)g_T.targets.size();
+  const int m = n < cap ? n : cap;
+  const real nan = std::numeric_limits<real>::quiet_NaN();
+  for (int i = 0; i < m; ++i) {
+    track_manage[i] = g_T.trackNum[i];
+    for (int j = 0; j < n_t; ++j) {
+      const size_t row = (size_t)j * cap + i;
+      for (int e = 0; e < 5; ++e) x[row * 5 + e] = nan;
+      for (int e = 0; e < 25; ++e) P[row * 25 + e] = nan;
+      for (int e = 0; e < 3; ++e) mode_prob[row * 3 + e] = nan;
+      for (int e = 0; e < 2; ++e) gate_z[row * 2 + e] = nan;
+      for (int e = 0; e < 4; ++e) gate_S[row * 4 + e] = nan;
+      flags[row] = (unsigned char)predict_track(g_T, i, t_us[j], x + row * 5, P + row * 25, mode_prob + row * 3, gate_z + row * 2,
+                                                gate_S + row * 4);
+    }
+  }
+  return n;
 }
 
 }  // extern "C"

@@ -3,6 +3,8 @@
   RefOracle("o2" | "intended")  -> oracle/_ref/libref_*.so : the reference's own sources compiled unmodified
                                    (see oracle/Makefile, oracle/ref_harness.cpp)
   PortOracle()                  -> oracle/liboracle_port.so : the plain-C++ restatement (oracle/port/)
+  PortOracleHP()                -> oracle/liboracle_port_hp.so : the same restatement evaluated in x87 long double (64-bit
+                                   mantissa); tracker dumps, vandyaw and predictions come back as np.longdouble
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import this.
 The product library (liblmot.so) never does.
@@ -40,9 +42,11 @@ def _as_pts(points: np.ndarray):
 class _OracleBase:
     """Shared marshalling; `prefix` selects ref_* (reference sources) or port_* (restatement) symbols."""
 
-    def __init__(self, path: str, prefix: str):
+    def __init__(self, path: str, prefix: str, real=np.float64):
         self.lib = C.CDLL(path)
         self.prefix = prefix
+        self.real = real            # the type of every tracker value the reference computes in double
+        _rp = np.ctypeslib.ndpointer(real, flags="C_CONTIGUOUS")
         L, p = self.lib, prefix
         self._cell = getattr(L, p + "cell_index"); self._cell.argtypes = [_f32p, C.c_int, C.c_int, _i32p, _i32p]
         self._gr = getattr(L, p + "ground_remove"); self._gr.argtypes = [_f32p, C.c_int, C.c_int, _f32p, C.POINTER(C.c_int), _f32p, C.POINTER(C.c_int)]
@@ -55,9 +59,9 @@ class _OracleBase:
         self._tr = getattr(L, p + "tracker_reset"); self._tr.argtypes = []
         self._tn = getattr(L, p + "tracker_num_tracks"); self._tn.restype = C.c_int
         self._ts = getattr(L, p + "tracker_step")
-        self._ts.argtypes = [_f32p, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, _f32p, _f64p, _i32p, _u8p, _u8p, _f32p,
+        self._ts.argtypes = [_f32p, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, _f32p, _rp, _i32p, _u8p, _u8p, _f32p,
                              C.POINTER(C.c_int), C.POINTER(C.c_int)]
-        self._td = getattr(L, p + "tracker_dump"); self._td.argtypes = [C.c_int, _f64p]
+        self._td = getattr(L, p + "tracker_dump"); self._td.argtypes = [C.c_int, _rp]
         self._tl = getattr(L, p + "tracker_load")
         self._tl.argtypes = [C.c_int, _f64p, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double]
 
@@ -122,7 +126,7 @@ class _OracleBase:
         m = b.shape[0]
         if m == 0:
             b = np.zeros((1, 8, 3), np.float32)
-        tg = np.zeros((cap, 3), np.float32); vy = np.zeros((cap, 2), np.float64); tm = np.zeros(cap, np.int32)
+        tg = np.zeros((cap, 3), np.float32); vy = np.zeros((cap, 2), self.real); tm = np.zeros(cap, np.int32)
         st = np.zeros(cap, np.uint8); vis = np.zeros(cap, np.uint8); vbb = np.zeros((cap, 8, 3), np.float32)
         nv = C.c_int(0); nt = C.c_int(0)
         self._ts(b, m, float(timestamp_us), float(v_gps), float(yaw_gps), cap, tg, vy, tm, st, vis, vbb, C.byref(nv), C.byref(nt))
@@ -132,8 +136,8 @@ class _OracleBase:
 
     def tracker_dump(self) -> np.ndarray:
         t = self.tracker_num_tracks()
-        out = np.zeros((t, TRACK_DUMP_DOUBLES), np.float64)
-        row = np.zeros(TRACK_DUMP_DOUBLES, np.float64)
+        out = np.zeros((t, TRACK_DUMP_DOUBLES), self.real)
+        row = np.zeros(TRACK_DUMP_DOUBLES, self.real)
         for i in range(t):
             self._td(i, row)
             out[i] = row
@@ -169,18 +173,56 @@ class RefOracle(_OracleBase):
 
 
 class PortOracle(_OracleBase):
+    LIB, REAL, DIGITS = "liboracle_port.so", np.float64, 53
+
     def __init__(self, mode: str = "intended"):
-        super().__init__(os.path.join(HERE, "liboracle_port.so"), "port_")
+        super().__init__(os.path.join(HERE, self.LIB), "port_", self.REAL)
+        digits = self.lib.port_real_digits()
+        if digits != self.DIGITS:
+            raise RuntimeError(f"{self.LIB}: port::real has {digits} mantissa bits, expected {self.DIGITS}")
         self.mode = mode
         self.lib.port_set_rule_mode(0 if mode == "intended" else 1)
+        self._tp = self.lib.port_tracker_predict
+        self._tp.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 7
+        self._tp.restype = C.c_int
 
     def box_fitting(self, elevated, grid, num_cluster, max_boxes: int = 4096):
         self.lib.port_set_rule_mode(0 if self.mode == "intended" else 1)   # the mode is process-global in the port
         return super().box_fitting(elevated, grid, num_cluster, max_boxes)
 
+    def tracker_predict(self, t_us, cap: int | None = None) -> dict:
+        """ref_tracker_predict (oracle/ref_predict.py's predict) on the port's table, values in self.real"""
+        t = np.ascontiguousarray(np.atleast_1d(np.asarray(t_us, np.float64)))
+        n_t = int(t.shape[0])
+        if cap is None:
+            cap = self.tracker_num_tracks()
+        z = lambda *shape: np.zeros(shape, self.real)
+        r = {"track_manage": np.zeros(cap, np.int32), "flags": np.zeros((n_t, cap), np.uint8), "x": z(n_t, cap, 5),
+             "P": z(n_t, cap, 5, 5), "mode_prob": z(n_t, cap, 3), "gate_z": z(n_t, cap, 2), "gate_S": z(n_t, cap, 4)}
+        n = self._tp(t.ctypes.data, n_t, cap, *(r[k].ctypes.data for k in ("track_manage", "flags", "x", "P", "mode_prob", "gate_z", "gate_S")))
+        m = min(n, cap)
+        return {k: (a[:m] if k == "track_manage" else a[:, :m]) for k, a in r.items()}
+
+
+class PortOracleHP(PortOracle):
+    """The restatement in extended precision: the same operations, order and double-rounded constants as PortOracle, with x87
+    long double (64-bit mantissa) for every value the reference computes in double.  Its rounding error (~5e-20 per operation) is
+    far below the reference's, so the difference of any double evaluation from it is that evaluation's own error."""
+    LIB, REAL, DIGITS = "liboracle_port_hp.so", np.longdouble, 64
+
+    def __init__(self, mode: str = "intended"):
+        if np.finfo(np.longdouble).nmant != 63:
+            raise RuntimeError(f"np.longdouble has {np.finfo(np.longdouble).nmant} mantissa bits, not x87's 63 (+1 implicit): "
+                               "the extended-precision oracle cannot be marshalled on this platform")
+        super().__init__(mode)
+
 
 def have_port() -> bool:
     return os.path.exists(os.path.join(HERE, "liboracle_port.so"))
+
+
+def have_port_hp() -> bool:
+    return os.path.exists(os.path.join(HERE, "liboracle_port_hp.so"))
 
 
 def labels_from_clouds(points, elevated, ground) -> np.ndarray:
