@@ -434,6 +434,38 @@ def obstacle_polygons(res: dict) -> list:
     return [v[o: o + c] for o, c in zip(res["obstacles"]["vertex_offset"], res["obstacles"]["vertex_count"])]
 
 
+class EgoMatch(C.Structure):
+    """lmot_ego_match: scan-matched ego motion settings (include/lmot.h)."""
+    _fields_ = [("grid", C.c_int), ("cell_m", C.c_double), ("z_min", C.c_double), ("z_max", C.c_double), ("r_min", C.c_double),
+                ("r_max", C.c_double), ("sub_m", C.c_double), ("max_points", C.c_int), ("yaw_step", C.c_double), ("yaw_half", C.c_int),
+                ("shift_half", C.c_int), ("refine", C.c_int), ("min_points", C.c_int), ("min_score_frac", C.c_double), ("sensor", C.c_int)]
+
+
+class EgoOut(C.Structure):
+    _fields_ = [("ok", C.c_int), ("n_used", C.c_int), ("n_ref", C.c_int), ("score", C.c_int), ("score_max", C.c_int),
+                ("dx", C.c_double), ("dy", C.c_double), ("dtheta", C.c_double), ("v", C.c_double), ("yaw", C.c_double)]
+
+
+def default_ego_match() -> dict:
+    lib = load_library()
+    m = EgoMatch()
+    lib.lmot_default_ego_match(C.byref(m))
+    return {name: getattr(m, name) for name, _ in EgoMatch._fields_}
+
+
+def _ego_match(fields: dict) -> EgoMatch:
+    base = default_ego_match()
+    unknown = set(fields) - set(base)
+    if unknown:
+        raise KeyError(f"unknown ego match fields {sorted(unknown)}")
+    base.update(fields)
+    return EgoMatch(*[t(base[name]) for name, t in ((n, int if c is C.c_int else float) for n, c in EgoMatch._fields_)])
+
+
+def _ego_dict(o: EgoOut) -> dict:
+    return {name: getattr(o, name) for name, _ in EgoOut._fields_}
+
+
 class FrameOut(C.Structure):
     _fields_ = [
         ("n_elevated", C.c_int), ("n_ground", C.c_int), ("num_cluster", C.c_int), ("n_boxes", C.c_int),
@@ -500,6 +532,8 @@ ABI_SYMBOLS = [
     "lmot_default_layers", "lmot_set_layers", "lmot_get_layers", "lmot_seq_set_layers", "lmot_seq_get_layers", "lmot_debug_point_clusters",
     "lmot_default_obstacles", "lmot_set_obstacles", "lmot_get_obstacles", "lmot_seq_set_obstacles", "lmot_seq_get_obstacles",
     "lmot_obstacles_result", "lmot_seq_obstacles_result",
+    "lmot_default_ego_match", "lmot_set_ego_match", "lmot_get_ego_match", "lmot_seq_set_ego_match", "lmot_seq_get_ego_match",
+    "lmot_ego_reset", "lmot_seq_ego_reset", "lmot_ego_estimate", "lmot_ego_estimate_dev", "lmot_seq_ego_estimate", "lmot_seq_ego_estimate_dev",
     "lmot_default_tracker_params", "lmot_set_tracker_params", "lmot_get_tracker_params", "lmot_seq_set_tracker_params",
     "lmot_seq_get_tracker_params", "lmot_default_detect_params", "lmot_seq_set_detect_params", "lmot_seq_get_detect_params",
     "lmot_set_track_retirement", "lmot_get_track_retirement", "lmot_seq_set_track_retirement", "lmot_seq_get_track_retirement",
@@ -530,6 +564,10 @@ def load_library() -> C.CDLL:
         lib.lmot_accumulate_pose.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.lmot_box_search_angles.argtypes = [C.c_int, C.c_void_p]
         lib.lmot_ground_lines_grid.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_void_p]
+        lib.lmot_ego_estimate.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_void_p]
+        lib.lmot_ego_estimate_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_void_p]
+        lib.lmot_seq_ego_estimate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        lib.lmot_seq_ego_estimate_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         _lib = lib
     return _lib
 
@@ -538,6 +576,9 @@ def default_params() -> Params:
     p = Params()
     load_library().lmot_default_params(C.byref(p))
     return p
+
+
+_EMPTY = np.zeros(4, np.float32)        # the data pointer of an empty host frame (never read)
 
 
 def _fp(a):
@@ -1132,6 +1173,71 @@ class Lmot:
 
     def seq_get_box_search(self, k: int) -> dict:
         return self._get_record(self.lib.lmot_seq_get_box_search, BoxSearch, int(k))
+
+    # ---- scan-matched ego motion (lmot_ego_estimate) -----------------------------------------------------------------------------
+    def set_ego_match(self, **fields):
+        """The context's own stream: scan matcher settings with `fields` replaced (no fields: the defaults).  Resets the matcher."""
+        self._ego_set(None, fields)
+
+    def get_ego_match(self) -> dict:
+        return self._get_record(self.lib.lmot_get_ego_match, EgoMatch)
+
+    def seq_set_ego_match(self, k: int, **fields):
+        """Sequence k's matcher, arguments as set_ego_match."""
+        self._ego_set(int(k), fields)
+
+    def seq_get_ego_match(self, k: int) -> dict:
+        return self._get_record(self.lib.lmot_seq_get_ego_match, EgoMatch, int(k))
+
+    def _ego_set(self, k, fields):
+        m = C.byref(_ego_match(fields)) if fields else None
+        self._chk(self.lib.lmot_set_ego_match(self.h, m) if k is None else self.lib.lmot_seq_set_ego_match(self.h, k, m))
+
+    def ego_reset(self):
+        """The next ego_estimate is the stream's first: no reference, yaw back to 0."""
+        self._chk(self.lib.lmot_ego_reset(self.h))
+
+    def seq_ego_reset(self, k: int):
+        self._chk(self.lib.lmot_seq_ego_reset(self.h, int(k)))
+
+    def ego_estimate(self, points, timestamp_us) -> dict:
+        """Synchronous: one host frame through the matcher -> dict of lmot_ego_out (pass its v / yaw as v_gps / yaw_gps)."""
+        p, n, s = _pts(points)
+        o = EgoOut()
+        self._chk(self.lib.lmot_ego_estimate(self.h, p.ctypes.data if n else None, n, s, float(timestamp_us), C.byref(o)))
+        return _ego_dict(o)
+
+    def ego_estimate_dev(self, d_ptr: int, n: int, timestamp_us) -> dict:
+        """Synchronous: a device XYZI frame (stride 4), ordered after the context's stream."""
+        o = EgoOut()
+        self._chk(self.lib.lmot_ego_estimate_dev(self.h, C.c_void_p(d_ptr or None), int(n), float(timestamp_us), C.byref(o)))
+        return _ego_dict(o)
+
+    def seq_ego_estimate(self, frames, timestamps) -> list:
+        """One host frame per sequence (None: skipped, its state untouched) -> [dict or None]; frames share one stride."""
+        arrs = [None if f is None else _pts(f) for f in frames]
+        strides = {a[2] for a in arrs if a is not None}
+        if len(strides) > 1:
+            raise ValueError("every frame of one call has the same stride")
+        ptrs = [None if a is None else (a[0].ctypes.data if a[1] else _EMPTY.ctypes.data) for a in arrs]
+        return self._seq_ego(ptrs, [0 if a is None else a[1] for a in arrs], strides.pop() if strides else 4, timestamps, True)
+
+    def seq_ego_estimate_dev(self, d_ptrs, ns, timestamps) -> list:
+        """One device frame (stride 4) per sequence (0 / None: skipped), ordered after the context's stream."""
+        return self._seq_ego([p or None for p in d_ptrs], list(ns), 4, timestamps, False)
+
+    def _seq_ego(self, ptrs, ns, stride, timestamps, host):
+        S = len(ptrs)
+        P = (C.c_void_p * S)(*ptrs)
+        N = (C.c_int * S)(*[int(v) for v in ns])
+        T = (C.c_double * S)(*[float(t) for t in timestamps])
+        O = (EgoOut * S)()
+        if host:
+            st = self.lib.lmot_seq_ego_estimate(self.h, P, N, S, stride, T, O)
+        else:
+            st = self.lib.lmot_seq_ego_estimate_dev(self.h, P, N, S, T, O)
+        self._chk(st)
+        return [None if ptrs[k] is None else _ego_dict(O[k]) for k in range(S)]
 
     # ---- ground lines (lmot_set_ground_lines) ------------------------------------------------------------------------------------
     def set_ground_lines(self, **fields):

@@ -723,6 +723,7 @@ void result_destroy(Result* r) {
 // defaults
 void stream_free(Stream& s) {
   tracker_free(s.trk);
+  ego_free(s.ego);
   for (int b = 0; b < kBatchBanks; ++b) merge_unit_destroy(&s.cfg.merge_unit[b]);
   accumulate_free(s.cfg.acc);
   s = Stream{};
@@ -975,6 +976,7 @@ void lmot_destroy(lmot_ctx* ctx) {
   for (int i = 0; i < c->n_results; ++i) result_destroy(&c->results[i]);
   stream_free(c->own);
   seq_destroy(c);
+  ego_ctx_free(c);
   cudaFree(c->d_mt_raw);
   cudaFree(c->d_bs_tab);
   if (c->ev_pred) cudaEventDestroy(c->ev_pred);
@@ -2201,6 +2203,86 @@ int lmot_set_box_search(lmot_ctx* ctx, const lmot_box_search* b) { return box_se
 int lmot_get_box_search(const lmot_ctx* ctx, lmot_box_search* b) { return box_search_get(stream_at(ctx, kOwnStream), b); }
 int lmot_seq_set_box_search(lmot_ctx* ctx, int k, const lmot_box_search* b) { return box_search_set(ctx, k, b); }
 int lmot_seq_get_box_search(const lmot_ctx* ctx, int k, lmot_box_search* b) { return box_search_get(stream_at(ctx, k), b); }
+
+// ---- scan-matched ego motion (ego_match.cu).  Synchronous calls on the context's matcher stream; the frame pipeline never reads it
+int lmot_default_ego_match(lmot_ego_match* m) {
+  if (!m) return LMOT_ERR_INVALID;
+  *m = ego_match_defaults();
+  return LMOT_OK;
+}
+
+static int ego_match_set(Stream* s, const lmot_ego_match* m) {
+  const lmot_ego_match v = m ? *m : ego_match_defaults();
+  if (!s || !ego_match_valid(v)) return LMOT_ERR_INVALID;
+  s->ego.cfg = v;
+  s->ego.reset();
+  return LMOT_OK;
+}
+
+static int ego_match_get(const Stream* s, lmot_ego_match* m) {
+  if (!s || !m) return LMOT_ERR_INVALID;
+  *m = s->ego.cfg;
+  return LMOT_OK;
+}
+
+static int ego_reset(Stream* s) {
+  if (!s) return LMOT_ERR_INVALID;
+  s->ego.reset();
+  return LMOT_OK;
+}
+
+int lmot_set_ego_match(lmot_ctx* ctx, const lmot_ego_match* m) { return ego_match_set(stream_at(ctx, kOwnStream), m); }
+int lmot_get_ego_match(const lmot_ctx* ctx, lmot_ego_match* m) { return ego_match_get(stream_at(ctx, kOwnStream), m); }
+int lmot_seq_set_ego_match(lmot_ctx* ctx, int k, const lmot_ego_match* m) { return ego_match_set(stream_at(ctx, k), m); }
+int lmot_seq_get_ego_match(const lmot_ctx* ctx, int k, lmot_ego_match* m) { return ego_match_get(stream_at(ctx, k), m); }
+int lmot_ego_reset(lmot_ctx* ctx) { return ego_reset(stream_at(ctx, kOwnStream)); }
+int lmot_seq_ego_reset(lmot_ctx* ctx, int k) { return ego_reset(stream_at(ctx, k)); }
+
+// the own stream (k0 = kOwnStream, one frame) or every sequence whose frame is non-NULL: validate all, then one run over them
+static int ego_estimate_common(lmot_ctx* ctx, long long k0, int n_seq, const float* const* pts, const int* n, int stride, const double* ts,
+                               bool host, lmot_ego_out* out) {
+  if (!ctx || !pts || !n || !ts || !out || stride < 3) return LMOT_ERR_INVALID;
+  Ctx* c = &ctx->c;
+  if (k0 != kOwnStream && (c->n_seq == 0 || n_seq != c->n_seq)) return LMOT_ERR_INVALID;
+  if (c->timing) return LMOT_ERR_STATE;
+  EgoMatch* q[kMaxBatch];
+  const float* p[kMaxBatch];
+  int nn[kMaxBatch];
+  double tt[kMaxBatch];
+  const lmot_sensor* pose[kMaxBatch];
+  lmot_ego_out* o[kMaxBatch];
+  int S = 0;
+  for (int i = 0; i < n_seq; ++i) {
+    if (!pts[i]) continue;
+    Stream* s = stream_at(ctx, k0 == kOwnStream ? k0 : i);
+    const int j = s->ego.cfg.sensor;
+    if (n[i] < 0 || (j >= 0 && j >= s->cfg.n_sensors)) return LMOT_ERR_INVALID;
+    if (!host && ((uintptr_t)pts[i] & 15)) return LMOT_ERR_INVALID;
+    q[S] = &s->ego; p[S] = pts[i]; nn[S] = n[i]; tt[S] = ts[i]; pose[S] = j >= 0 ? &s->cfg.sensors[j] : nullptr; o[S] = &out[i];
+    ++S;
+  }
+  cudaSetDevice(c->device);
+  return ego_estimate_run(c, q, p, nn, stride, tt, pose, S, host, o);
+}
+
+alignas(16) static const float kNoPoints[4] = {};   // an empty frame may come without data: never read
+
+int lmot_ego_estimate(lmot_ctx* ctx, const float* points, int n, int stride_floats, double timestamp_us, lmot_ego_out* out) {
+  if (!points && n == 0) points = kNoPoints;
+  return ego_estimate_common(ctx, kOwnStream, 1, &points, &n, stride_floats, &timestamp_us, true, out);
+}
+int lmot_ego_estimate_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp_us, lmot_ego_out* out) {
+  if (!d_points && n == 0) d_points = kNoPoints;
+  return ego_estimate_common(ctx, kOwnStream, 1, &d_points, &n, 4, &timestamp_us, false, out);
+}
+int lmot_seq_ego_estimate(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride_floats, const double* timestamp_us,
+                          lmot_ego_out* out) {
+  return ego_estimate_common(ctx, 0, n_seq, points, n, stride_floats, timestamp_us, true, out);
+}
+int lmot_seq_ego_estimate_dev(lmot_ctx* ctx, const float* const* d_points, const int* n, int n_seq, const double* timestamp_us,
+                              lmot_ego_out* out) {
+  return ego_estimate_common(ctx, 0, n_seq, d_points, n, 4, timestamp_us, false, out);
+}
 
 int lmot_box_search_angles(int n_angles, float out[][2]) {
   if (!out || n_angles < 1 || n_angles > LMOT_BOX_SEARCH_MAX_ANGLES) return LMOT_ERR_INVALID;

@@ -432,9 +432,38 @@ struct ObsLast {
   std::vector<float> xy[kMaxBatch];
 };
 
+// lmot_default_ego_match
+inline lmot_ego_match ego_match_defaults() {
+  lmot_ego_match m;
+  memset(&m, 0, sizeof(m));
+  m.grid = 768; m.cell_m = 0.1; m.z_min = -1.5; m.z_max = 0.5; m.r_min = 3.0; m.r_max = 38.0; m.sub_m = 0.4; m.max_points = 4096;
+  m.yaw_step = 0.005; m.yaw_half = 30; m.shift_half = 30; m.refine = 5; m.min_points = 200; m.min_score_frac = 0.3; m.sensor = -1;
+  return m;
+}
+
+// One stream's scan matcher (ego_match.cu): its setting, its state between calls and its device buffers (allocated on its first call,
+// grown when a later setting needs more).  Fields d_field[ref] is the reference, d_field[ref ^ 1] the next call's field.
+struct EgoMatch {
+  lmot_ego_match cfg = ego_match_defaults();
+  bool has_ref = false;
+  double ts = 0, dt = 0;               // stamp of the reference; dt of the stored delta
+  double delta[3] = {0, 0, 0};         // dx, dy, dth
+  bool delta_ok = false;
+  double yaw = 0;                      // Y
+  int n_ref = 0;                       // occupied cells of the reference
+  int ref = 0;
+  unsigned char* d_field[2] = {nullptr, nullptr};
+  unsigned* d_occ = nullptr;
+  int* d_sub = nullptr;
+  float2* d_samp = nullptr;
+  size_t cap_field = 0, cap_sub = 0, cap_samp = 0;   // bytes of a field / entries of d_sub / entries of d_samp
+  void reset() { has_ref = false; ts = 0; dt = 0; delta[0] = delta[1] = delta[2] = 0; delta_ok = false; yaw = 0; n_ref = 0; }
+};
+
 // One frame stream: the context's own (lmot_frame*, lmot_batch*, lmot_track_step*, lmot_tracker_*) or a sequence of lmot_seq_*.  Its
 // settings, its track table, and what collect_result copied out of its most recently returned step.  Released by api.cu stream_free.
 struct Stream {
+  EgoMatch ego;                        // scan-matched ego motion (ego_match.cu): never read by the frame pipeline
   StreamCfg cfg;
   Tracker trk;
   lmot_accum_info acc_info = {};       // lmot_accumulate_info / lmot_seq_accumulate_info: what the step used
@@ -521,6 +550,17 @@ struct Ctx {
   // ---- lmot_debug_point_clusters: the units of the most recent own-stream submission (none: it was not layered)
   const Slot* lay_dbg[kMaxBatch] = {};
   int n_lay_dbg = 0;
+
+  // ---- scan-matched ego motion (ego_match.cu): the matcher stream and what every call stages, created / grown on first use
+  cudaStream_t ego_stream = nullptr;
+  cudaEvent_t ev_ego_in = nullptr;     // _dev forms: the caller stream's work so far
+  float* d_ego_stage = nullptr;        // host frames
+  size_t ego_stage_bytes = 0;
+  float2* h_ego_tab = nullptr;         // pinned angle tables of a call, and their device copy
+  float2* d_ego_tab = nullptr;
+  size_t ego_tab_cap = 0;              // entries
+  void* h_ego_res = nullptr;           // pinned per-stream results of a call, and their device rows
+  void* d_ego_res = nullptr;
 
   // ---- timing
   bool timing = false;
@@ -722,6 +762,14 @@ int obstacles_ensure(Ctx* c, const ObsUnit* u, int n, cudaStream_t st);
 int obstacles_launch(Ctx* c, cudaStream_t st, const ObsUnit* u, int n, Slot* mark);
 // the block's footprints into `dst` (waits for ev_obs); r->obs_units == 0: dst becomes invalid
 int obstacles_collect(Ctx* c, Result* r, ObsLast& dst);
+// scan-matched ego motion (ego_match.cu): setting validation, and one synchronous call over S streams q[i] with frame pts[i] of n[i]
+// points of `stride` floats (host frames when host, else device frames ordered after the caller stream), stamp ts[i], poses[i] (nullable:
+// the frame as given) -> out[i]
+bool ego_match_valid(const lmot_ego_match& m);
+int ego_estimate_run(Ctx* c, EgoMatch* const* q, const float* const* pts, const int* n, int stride, const double* ts,
+                     const lmot_sensor* const* poses, int S, bool host, lmot_ego_out* const* out);
+void ego_free(EgoMatch& e);
+void ego_ctx_free(Ctx* c);
 void obstacles_result_free(Result* r);
 
 }  // namespace lmot

@@ -1110,6 +1110,95 @@ int lmot_seq_get_obstacles(const lmot_ctx* ctx, int k, lmot_obstacles* o);
 int lmot_obstacles_result(lmot_ctx* ctx, int unit, lmot_obstacles_out* out);
 int lmot_seq_obstacles_result(lmot_ctx* ctx, int k, int unit, lmot_obstacles_out* out);
 
+/* ---- scan-matched ego motion: a stream's speed and yaw from consecutive sweeps, for rigs without GPS ---------------------------------
+ * Every motion-aware part of the library (getOriginPoints' fold, global_frame, deskew, accumulation, the static flag) reads the ego motion
+ * a caller passes as v_gps / yaw_gps.  A LiDAR-only rig has none.  The estimator matches each sweep against the previous one and returns
+ * (v, yaw) in exactly the form lmot_frame* / lmot_seq* take: call it on a frame, then pass its v and yaw with that frame.  It is a separate,
+ * synchronous call: the frame pipeline, the fold and the tracker are not touched by it.
+ *
+ * Definition.  A stream (the context's own: lmot_set_ego_match; sequence k: lmot_seq_set_ego_match) has the settings below and a matcher
+ * state: the previous stamp, the previous frame's likelihood field L, the previous delta (dx, dy, dth), its dt and ok flag, and an
+ * accumulated yaw Y.  H = (float)(grid * (double)cell_m * 0.5); float values below are the settings rounded to float once.  One call on
+ * frame P with stamp ts:
+ *   1. band: point p (moved first, with sensor = j, by sensor j's pose of the stream's table with the rig arithmetic of lmot_set_sensors:
+ *      x' = ((r00*x + r01*y) + r02*z) + t0, likewise y', z', float without contraction) is used iff x, y, z are finite, z_min <= z <=
+ *      z_max and r_min*r_min <= x*x + y*y <= r_max*r_max, in float without contraction.  Its cell is ((int)floorf((x + H) / cell_m),
+ *      (int)floorf((y + H) / cell_m)); it is in the window iff both lie in [0, grid);
+ *   2. field: O = the cells holding a window point; L[c] = 3 - min(3, Chebyshev distance from c to O), 0..3.  L becomes the stream's
+ *      reference at the end of the call;
+ *   3. sample: window points only; sub-cell (min((int)floorf((x + H) / sub_m), NS - 1), likewise y), NS = ceil(grid * cell_m / sub_m) + 1
+ *      in double.  The lowest-index point of each occupied sub-cell, sub-cells in raster order (y outer); if more than max_points remain,
+ *      every k-th of them from the first, k = ceil(count / max_points).  n_used points (x, y) remain;
+ *   4. match, iff the stream has a reference, dt = (ts - ts_prev) / 1e6 is finite and > 0, and n_used >= min_points:
+ *      prior: the previous delta times dt / dt_prev (double) if it was ok, else 0.  j0 = llround(prior_th / yaw_step), k0 =
+ *      llround(prior_xy / cell_m) per axis (a quotient of 2^20 or more in magnitude: 0).  Coarse level: j in j0 +- yaw_half, kx, ky in k0 +- shift_half; cs = (float)cos(j * yaw_step),
+ *      sn = (float)sin(j * yaw_step) in double with the host libm; xr = cs*x - sn*y, yr = sn*x + cs*y in float without contraction, base
+ *      cell (bx, by) = floorf((xr + H) / cell_m), floorf((yr + H) / cell_m); score(j, kx, ky) = sum over the points of L_prev[bx + kx,
+ *      by + ky], a cell outside the grid scoring 0.  Fine level (refine = R > 1) around the coarse winner (j1, k1): angles
+ *      (double)(R*j1 + u) * yaw_step / R, translations t = (float)((double)(R*k1 + a) * cell_m / R) per axis, u, a in [-R, R]; cell =
+ *      floorf(((xr + t) + H) / cell_m).  Both levels: the best score wins, ties to the first hypothesis in ascending (j, kx, ky) order
+ *      ((u, ax, ay) for the fine one).  (dx, dy, dth) is the winner's lattice value in double: the pose of this frame's origin in the
+ *      previous frame.  ok = (double)best >= min_score_frac * 3 * n_used.  Scores are integers: any reduction order gives the same result;
+ *   5. outputs: ok: v = (dx*cos(dth) + dy*sin(dth)) / dt (getOriginPoints' own model: the displacement along the new heading), Y += dth.
+ *      Not ok with dt valid (no match, or a weak one): the prior is reported as the delta, v and Y from it (constant velocity).  No valid
+ *      dt (first call, after a reset, dt <= 0 or not finite): v = 0, dth = 0, ok = 0.  yaw = Y.  In every case the reference, the stamp
+ *      and the delta (with its dt and ok) are then replaced.
+ * The matched yaw starts at 0: the fold only reads its differences.
+ * Settings.  Setting them (also to the same values) resets the stream's matcher state; so do lmot_ego_reset / lmot_seq_ego_reset and
+ * lmot_seq_open (every sequence back to the defaults).  LMOT_ERR_INVALID, setting and state unchanged: a value not finite; grid outside
+ * [32, 1024] or not a multiple of 32; cell_m outside [0.01, 10]; a window grid * cell_m above 400 m; z_min >= z_max; r_min < 0; r_min >=
+ * r_max; r_max > 1000; sub_m <= 0 or NS > 1024; max_points outside [1, 8192]; yaw_step outside (0, 0.1]; yaw_half outside [0, 180];
+ * shift_half outside [0, 127]; refine outside [1, 15]; min_points < 1; min_score_frac outside [0, 1]; sensor outside [-1, LMOT_MAX_BATCH);
+ * k out of range or no open set.  No device is needed for the validation.
+ * Estimation.  lmot_ego_estimate: a HOST frame of n points, stride floats each (>= 3).  lmot_ego_estimate_dev: a DEVICE frame (stride 4),
+ * ordered after the caller stream.  lmot_seq_ego_estimate / _dev: one frame per sequence (n_seq entries = the open set's), every sequence
+ * whose pointer is non-NULL stepped in one launch per kernel; a NULL entry leaves its sequence's state and out[k] untouched.  The calls run
+ * on a matcher stream of the context and wait for their own work only: they never wait for, reorder or change frames and ticks in flight.
+ * LMOT_ERR_INVALID: null arguments, n < 0, stride < 3, n_seq not the set's, sensor = j without a j-th sensor in the stream's table
+ * (nothing is stepped).  LMOT_ERR_STATE: timing mode (lmot_enable_timing) is on.
+ * Memory.  A stream's first call allocates two fields of grid^2 bytes, an occupancy bitmap of grid^2 / 8 bytes, NS^2 ints of sub-cells and
+ * max_points x 8 bytes of samples (1.4 MB at the defaults); a later call whose settings need more reallocates them.  Per context: the
+ * host-frame staging grows to the largest frame (sum of frames for the sequence form) seen, and the angle tables to (2 yaw_half + 1) +
+ * (2 yaw_half refine + 2 refine + 1) float pairs per stream (3 KB at the defaults).  Freed with the context; a sequence's with the set. */
+typedef struct lmot_ego_match {
+  int grid;                    /* 768 cells per side, 32 .. 1024, a multiple of 32 */
+  double cell_m;               /* 0.1 */
+  double z_min, z_max;         /* -1.5, 0.5: the height band, stream frame (vehicle frame with sensor >= 0) */
+  double r_min, r_max;         /* 3, 38: the range band */
+  double sub_m;                /* 0.4: sampling sub-cell */
+  int max_points;              /* 4096 */
+  double yaw_step;             /* 0.005 rad */
+  int yaw_half;                /* 30: coarse angles j0 +- yaw_half */
+  int shift_half;              /* 30: coarse shifts k0 +- shift_half cells (+-3 m at the default cell) */
+  int refine;                  /* 5: fine level at 1/refine of the coarse lattice; 1: none */
+  int min_points;              /* 200: fewer sampled points: no match */
+  double min_score_frac;       /* 0.3: ok iff best >= min_score_frac * 3 * n_used */
+  int sensor;                  /* -1: the frame as given; j: sensor j's frame of the stream's table, moved into the vehicle frame */
+} lmot_ego_match;
+typedef struct lmot_ego_out {
+  int ok;                      /* the match passed min_score_frac */
+  int n_used;                  /* sampled points */
+  int n_ref;                   /* occupied cells of the reference the match used (0: no match ran) */
+  int score;                   /* the best score (0: no match ran) */
+  int score_max;               /* 3 * n_used */
+  double dx, dy, dtheta;       /* this frame's origin in the previous frame (m, m, rad) */
+  double v;                    /* m/s: pass as v_gps */
+  double yaw;                  /* rad, Y: pass as yaw_gps */
+} lmot_ego_out;
+int lmot_default_ego_match(lmot_ego_match* m);
+int lmot_set_ego_match(lmot_ctx* ctx, const lmot_ego_match* m);            /* NULL: the defaults */
+int lmot_get_ego_match(const lmot_ctx* ctx, lmot_ego_match* m);
+int lmot_seq_set_ego_match(lmot_ctx* ctx, int k, const lmot_ego_match* m);
+int lmot_seq_get_ego_match(const lmot_ctx* ctx, int k, lmot_ego_match* m);
+int lmot_ego_reset(lmot_ctx* ctx);
+int lmot_seq_ego_reset(lmot_ctx* ctx, int k);
+int lmot_ego_estimate(lmot_ctx* ctx, const float* points, int n, int stride_floats, double timestamp_us, lmot_ego_out* out);
+int lmot_ego_estimate_dev(lmot_ctx* ctx, const float* d_points, int n, double timestamp_us, lmot_ego_out* out);
+int lmot_seq_ego_estimate(lmot_ctx* ctx, const float* const* points, const int* n, int n_seq, int stride_floats, const double* timestamp_us,
+                          lmot_ego_out* out);
+int lmot_seq_ego_estimate_dev(lmot_ctx* ctx, const float* const* d_points, const int* n, int n_seq, const double* timestamp_us,
+                              lmot_ego_out* out);
+
 /* ---- tracker state (checkpoint / teacher-forced parity tests) ------------------------------------------ */
 int lmot_tracker_reset(lmot_ctx* ctx);
 int lmot_tracker_num_tracks(lmot_ctx* ctx, int* n);

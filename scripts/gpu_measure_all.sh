@@ -23,5 +23,6 @@ timeout 600 python scripts/box_search_measure.py > measure_out/${T}_box_search.t
 timeout 600 python scripts/ground_lines_measure.py > measure_out/${T}_ground_lines.txt 2>&1; tail -3 measure_out/${T}_ground_lines.txt
 timeout 900 python scripts/layers_measure.py > measure_out/${T}_layers.txt 2>&1; tail -3 measure_out/${T}_layers.txt
 timeout 900 python scripts/obstacles_measure.py > measure_out/${T}_obstacles.txt 2>&1; tail -3 measure_out/${T}_obstacles.txt
+timeout 600 python scripts/ego_match_measure.py --out measure_out/${T}_ego_match.json > measure_out/${T}_ego_match.txt 2>&1; tail -3 measure_out/${T}_ego_match.txt
 timeout 300 python scripts/diag_timeline.py ${T}_timeline > measure_out/${T}_timeline.txt 2>&1; tail -5 measure_out/${T}_timeline.txt
 ls -la measure_out/${T}*
